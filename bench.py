@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — AR frames/s of the Sopro hot path on N B200s (one process per GPU).
+"""bench.py — AR frames/s of the Sopro hot path on N H100s (one process per GPU).
 
 Workload (BASELINE.json configs[2]; x N GPUs it is configs[3]): per GPU a batch of 64 independent 400-frame
 utterances (401 AR steps: reference model.py:242), 52 text tokens each, one shared prepared reference voice (3 s = 38
@@ -8,7 +8,7 @@ length is pinned, SURVEY.md §8d).  A bench "step" is one full pass of the hot p
 
   value   device-resident: text-K/V build + ONE persistent AR kernel launch (64 x 401 frames), inputs already in HBM
   e2e     the same metric through the PUBLIC API: SoproTTS.synthesize_batch(64 texts) = tokenise -> batched CUDA prefill ->
-          noise tapes drawn on the host and uploaded -> persistent AR kernel -> CUDA NAR refiner -> tcgen05 Mimi decode
+          noise tapes drawn on the host and uploaded -> persistent AR kernel -> CUDA NAR refiner -> tensor-core Mimi decode
           -> waveforms copied to pinned host memory.  Host->device: text ids + noise tapes; device->host: the waveforms.
 
 Data parallel, no data-path collective ("weak" scaling); NCCL is used once, to broadcast the weights from rank 0.
@@ -16,6 +16,7 @@ Data parallel, no data-path collective ("weak" scaling); NCCL is used once, to b
   python bench.py --gpus 1 --steps 5 --warmup 3
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
   python bench.py --impl reference ...      # the reference's own CPU path (baseline/_ref when present, else the oracle port)
+  python bench.py ... --dump-outputs DIR     # also write what the last timed step computed, as DIR/<name>.npy
 """
 from __future__ import annotations
 
@@ -51,7 +52,7 @@ def _peaks():
             j = json.load(f)
         return float(j["hbm_gbs"]), float(j.get("bf16_tflops_sustained", 1456.6)), float(j.get("bf16_tflops", 1710.5)), \
             "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1400.0, 1590.0, "fallback (B200_PROFILING.md 6.65 TB/s, 1.59 PFLOP/s burst / ~1.4 sustained)"
+    return 3350.0, 989.0, 989.0, "data sheet (H100 SXM: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16; not measured)"
 
 
 def _inputs(cfg, rank, B, steps, L):
@@ -376,15 +377,30 @@ def extras(tts, ref, cfg, dev, peaks):
             "precision": tts.codec.engine.precision, "alg_bytes_per_frame": MIMI_ALG_BYTES_PER_FRAME,
             "alg_gb_per_s": 10000 * MIMI_ALG_BYTES_PER_FRAME / t / 1e9, "alg_frac_of_hbm": 10000 * MIMI_ALG_BYTES_PER_FRAME / t / 1e9 / hbm,
             "peak_source": src, "traffic": None,
-            "note": "whole decode (about 85 launches), 431.2 MFLOP of contractions per frame (SURVEY.md §8a11); peak = sustained cuBLAS bf16; "
-                    "per-kernel tensor-pipe and DRAM figures: profiles/"}
-    tp = os.path.join(ROOT, "profiles", "mimi_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            tj = json.load(f)
-        mimi["traffic"] = tj.get("dram_bytes_per_frame")
-        mimi["ncu_capture"] = tj.get("ncu")
+            "note": "whole decode (about 85 launches), 431.2 MFLOP of contractions per frame (SURVEY.md §8a11); peak: see peak_source; "
+                    "DRAM traffic not measured"}
     return out, mimi
+
+
+DUMP_WAV_SAMPLES = 1 << 22  # 16 MB of float32
+
+
+def dump_outputs(out_dir, prefix, toks, n_tok, wav_host, e2e_frames):
+    """What the two timed legs returned in their last step, for comparing two builds output for output:
+    the resident leg's sampled token ids [B, 401] and counts, and a fixed seeded sample of the API leg's waveforms
+    (the whole batch is ~200 MB) with the flat indices it was taken at."""
+    os.makedirs(out_dir, exist_ok=True)
+    flat = wav_host.reshape(-1).numpy()
+    idx = np.sort(np.random.default_rng(0).integers(0, flat.size, size=min(DUMP_WAV_SAMPLES, flat.size)))
+    arrays = {
+        "ar_tokens": np.asarray(toks, dtype=np.float64),
+        "ar_n_tokens": np.asarray(n_tok, dtype=np.float64),
+        "e2e_wav_sample": flat[idx].astype(np.float32),
+        "e2e_wav_sample_index": idx.astype(np.float64),
+        "e2e_frames_per_step": np.array([e2e_frames], dtype=np.float64),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{prefix}{name}.npy"), a)
 
 
 def main():
@@ -396,6 +412,8 @@ def main():
     ap.add_argument("--batch", type=int, default=BATCH_PER_GPU, help="utterances per GPU")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip batch-1 / TTFA / RTF / Mimi side measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step of each leg computed as DIR/<name>.npy")
     args = ap.parse_args()
     torch.set_grad_enabled(False)
     # Libraries (NCCL's version banner, ...) write to fd 1; the contract is ONE JSON line on stdout.
@@ -453,9 +471,9 @@ def main():
         emit(line)
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference for the CPU baseline)")
+        raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference for the CPU baseline)")
     import torch.distributed as dist
 
     torch.cuda.set_device(local_rank)
@@ -542,6 +560,8 @@ def main():
         e2e_ms += a.elapsed_time(b)
     clocks.stop_flag = True
     clocks.join(timeout=2)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, f"rank{rank}_" if world > 1 else "", toks, n_tok, wav_host, e2e_frames // max(args.steps, 1))
     t = torch.tensor([t_total_ms, e2e_ms, t_kernel_ms], dtype=torch.float64, device=dev)
     fr = torch.tensor([float(frames_per_pass), float(e2e_frames)], dtype=torch.float64, device=dev)
     if world > 1:
@@ -560,14 +580,7 @@ def main():
     w_step = eng.step_weight_bytes
     alg_bytes_launch = (w_step + B * S_UTT_BYTES) * STEPS_AR
     achieved = alg_bytes_launch / (t_kernel_ms / 1e3) / 1e9
-    traffic = None
-    ncu_note = None
-    tp = os.path.join(ROOT, "profiles", "ar_kernel_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            tj = json.load(f)
-        traffic = tj.get("dram_bytes_per_launch")
-        ncu_note = tj.get("ncu")
+    traffic = None  # DRAM bytes per launch: not measured
     W = max(world, 1)
     # launches of OUR kernels inside the timed regions, per rank: resident leg = kv_build + persistent AR per step; API leg per
     # step = prefill 24 + kv_build 1 + AR 6 (the launch resumes once per noise-tape block) + NAR on the tensor cores (1 + 4
@@ -588,9 +601,7 @@ def main():
                      "traffic": traffic, "kernel": "ar_persistent_kernel<bf16>", "ms_per_launch": t_kernel_ms,
                      "alg_bytes_per_launch": alg_bytes_launch, "peak_source": peak_src,
                      "note": "algorithmic bytes = (W_step + B*3280) per AR step x 401 steps (SURVEY.md §8d); W_step is L2-resident "
-                             "after the first step, so DRAM traffic is far below this",
-                     # last committed ncu --set full capture of this kernel (not measured in this run)
-                     "ncu_capture": ncu_note},
+                             "after the first step, so DRAM traffic is far below this"},
         "clocks": clocks.summary(),
         "extra": {"us_per_ar_step": t_kernel_ms / STEPS_AR * 1e3, "frames_per_pass_per_gpu": frames_per_pass,
                   "synthesize_batch_ms": e2e_ms / args.steps, "rtf_batch": (e2e_ms / 1e3) / (e2e_frames_all / W * 0.08),

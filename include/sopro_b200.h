@@ -1,5 +1,5 @@
 /*
- * sopro_b200 — C-ABI of the B200-native Sopro hot path.
+ * sopro_b200 — C-ABI of the H100-native Sopro hot path.
  *
  * The reference (samuel-vitorino/sopro) is pure Python/PyTorch and has no FFI;
  * every entry point below names the reference interface it replaces
@@ -9,7 +9,7 @@
  * void* (NULL = legacy default stream).  Every function returns 0 on success
  * or a negative sopro_status; sopro_last_error() gives the message for the
  * calling thread.  There is no CPU fallback: creating an engine on a device
- * that is not sm_100 fails.
+ * that is not sm_90 fails.
  */
 #ifndef SOPRO_B200_H_
 #define SOPRO_B200_H_
@@ -27,7 +27,7 @@ enum sopro_status {
   SOPRO_OK = 0,
   SOPRO_ERR_INVALID = -1,     /* bad argument / unsupported geometry */
   SOPRO_ERR_CUDA = -2,        /* a CUDA runtime call failed */
-  SOPRO_ERR_UNSUPPORTED = -3, /* device is not sm_100, or feature not built */
+  SOPRO_ERR_UNSUPPORTED = -3, /* device is not sm_90, or feature not built */
   SOPRO_ERR_STATE = -4        /* call out of order */
 };
 
@@ -121,8 +121,8 @@ int sopro_ar_session_destroy(sopro_ar_session_t* s);
 /* Launch geometry override (0 = automatic): utterances per CTA team. */
 int sopro_ar_session_set_team(sopro_ar_session_t* s, int utts_per_team);
 
-/* Arithmetic unit of the step's contractions: 0 or -1 = packed fp32 FMA (FFMA2) tiles -- the default and the faster one at
- * the 22..86 weight rows a CTA owns per stage; 1 = tensor cores (tcgen05, every fp32 activation split into three exact bf16
+/* Arithmetic unit of the step's contractions: 0 or -1 = fp32 FMA tiles -- the default and the faster one at
+ * the 22..86 weight rows a CTA owns per stage; 1 = tensor cores (wgmma, every fp32 activation split into three exact bf16
  * terms against bf16 weights, fp32 accumulation) or fail when the launch cannot use them (needs bf16 weight storage,
  * d_model % 64 == 0, teams of 5..8 utterances).  -1 also honours the environment variable SOPRO_AR_TC=1.  Both produce the
  * reference's token ids (tests/test_ar_gpu.py). */
@@ -275,8 +275,8 @@ int sopro_mimi_decode(sopro_mimi_t* m, const int32_t* codes, int B, int T, float
 int sopro_mimi_decode_host(sopro_mimi_t* m, const int32_t* codes_host, int B, int T, float* wav_host, void* stream);
 
 /* Arithmetic of the dense blocks (transformer linears, SEANet Conv1d / ConvTranspose1d).
- *   SOPRO_MIMI_BF16_TC (default): bf16 operands on the tcgen05 tensor cores, fp32 accumulation in tensor
- *     memory, fp32 residual streams / LayerNorm / softmax; within 2e-2 * max|wav| of the fp32 reference.
+ *   SOPRO_MIMI_BF16_TC (default): bf16 operands on the tensor cores (wgmma), fp32 accumulation,
+ *     fp32 residual streams / LayerNorm / softmax; within 2e-2 * max|wav| of the fp32 reference.
  *   SOPRO_MIMI_FP32: every contraction in fp32 on the FMA pipe; within 1e-4 of the reference
  *     (what transformers computes on CPU, modeling_mimi.py). */
 #define SOPRO_MIMI_FP32 0
@@ -413,7 +413,7 @@ int sopro_nar_refine(sopro_nar_t* n, const float* cond, int64_t cond_batch_strid
 /* test hook (teacher forcing): when non-NULL, every stage conditions on the previous codebooks of forced_codes
  * [B, Tmax, Q] i32 (device) instead of on its own argmax results, so one near-tie flip cannot cascade. */
 int sopro_nar_set_forced(sopro_nar_t* n, const int32_t* forced_codes);
-/* Arithmetic unit of the refiner's contractions: -1 = automatic (tensor cores -- tcgen05, every fp32 operand split into
+/* Arithmetic unit of the refiner's contractions: -1 = automatic (tensor cores -- wgmma, every fp32 operand split into
  * three exact bf16 terms, the six products that reach fp32's last bit, fp32 accumulation -- whenever more than 16 rows are
  * refined; the fp32 FMA skinny kernel below that), 0 = fp32 FMA kernels only (also: environment SOPRO_NAR_TC=0), 1 = as -1
  * but fails if the geometry has no tensor-core images. */

@@ -1,4 +1,4 @@
-"""sopro_b200 — B200-native engine for the Sopro TTS hot path behind the reference's API.
+"""sopro_b200 — H100-native engine for the Sopro TTS hot path behind the reference's API.
 
     from sopro_b200 import SoproTTS          # drop-in for `from sopro import SoproTTS`
 

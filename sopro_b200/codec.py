@@ -193,7 +193,7 @@ class MimiEngine:
         self.set_precision(precision)
 
     def set_precision(self, precision: str) -> None:
-        """"bf16_tc": dense blocks on the tcgen05 tensor cores (bf16 operands, fp32 accumulate); "fp32": exact mode."""
+        """"bf16_tc": dense blocks on the tensor cores (wgmma) (bf16 operands, fp32 accumulate); "fp32": exact mode."""
         if precision not in self.PRECISIONS:
             raise ValueError(f"precision must be one of {sorted(self.PRECISIONS)}")
         _lib.check(self.lib.sopro_mimi_set_precision(self._h, self.PRECISIONS[precision]))

@@ -1,4 +1,4 @@
-"""Model configuration for the B200 Sopro engine.
+"""Model configuration for the H100 Sopro engine.
 
 Field names, defaults and meaning mirror the reference's ``SoproTTSConfig``
 (reference: src/sopro/config.py:7-43) so that a ``cfg`` JSON blob read out of a

@@ -48,7 +48,7 @@ uint16_t f32_to_bf16_rne(float f) {
 
 struct Arena {
   std::vector<unsigned char> host;
-  // Tensor-core operand IMAGE of W[N][K] (bf16): what tcgen05.mma reads from shared memory after a plain 1-D bulk copy.
+  // Tensor-core operand IMAGE of W[N][K] (bf16): what wgmma reads from shared memory after a plain 1-D bulk copy.
   //   [K / D slices][G groups of 8 rows][D / 64 chunks][8 rows x 128 B], 16-byte unit j of row r stored at unit j ^ r
   //   (128-byte swizzle, K-major).  glu: group g = channels 4g..4g+3, rows 0..3 their value rows, 4..7 their gate rows.
   size_t add_packed(const float* src, int N, int K, int D, bool glu, int* groups_out) {
@@ -172,7 +172,7 @@ struct sopro_ar_session {
 extern "C" {
 
 const char* sopro_last_error(void) { return g_err.c_str(); }
-const char* sopro_version(void) { return "sopro_b200 0.1 (sm_100a)"; }
+const char* sopro_version(void) { return "sopro_b200 0.1 (sm_90a)"; }
 
 int sopro_engine_create(const sopro_ar_config_t* cfg, const sopro_ar_weights_t* w, int device,
                         sopro_engine_t** out) {
@@ -186,8 +186,8 @@ int sopro_engine_create(const sopro_ar_config_t* cfg, const sopro_ar_weights_t* 
   if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range [0,%d)", device, ndev);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(SOPRO_ERR_UNSUPPORTED, "device %d is sm_%d%d; this build targets sm_100a only", device, prop.major,
+  if (prop.major != 9)
+    return fail(SOPRO_ERR_UNSUPPORTED, "device %d is sm_%d%d; this build targets sm_90a only", device, prop.major,
                 prop.minor);
   const int D = cfg->d_model, NL = cfg->n_layers, Kc = cfg->kernel, H = cfg->n_heads, V = cfg->vocab;
   if (D <= 0 || D % 4 != 0) return fail(SOPRO_ERR_INVALID, "d_model must be a positive multiple of 4 (got %d)", D);
@@ -628,7 +628,7 @@ struct StageW {
   int N, K, parts;    // parts = 2 for the GLU (value rows + gate rows of the same channels)
   const float* epi;   // GLU: packed [D][KcE] epilogue rows; else the bias vector [N] (or null)
   bool by_head;       // fused q + attention stage: rank r gets ALL rows of head r % H (ranks >= H * (P / H): none)
-  const unsigned char* packed;  // tensor-core operand image of the matrix (null: row-major FFMA2 tiles)
+  const unsigned char* packed;  // tensor-core operand image of the matrix (null: row-major FMA tiles)
 };
 
 // the fused q-projection + attention stage needs at least one CTA per head
@@ -873,10 +873,9 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   p.t_begin = t_begin;
   p.t_end = t_end;
   // ---- tensor cores for the contractions?  Needs bf16 weight storage, an engine with operand images, teams of 5..8
-  // utterances (one 8-utterance B operand) and the fused q + attention stage (Wq stays on the FFMA2 path).  OPT-IN
-  // (sopro_ar_session_set_contraction(1) or SOPRO_AR_TC=1): exact, but measured slower than the FFMA2 tiles at the
-  // 22..86 weight rows a CTA owns per stage -- a 64 x 32 x 16 instruction costs ~89 cycles whatever its useful part
-  // (profiles/r02d_tc_summary.md), 231 vs 161 us per step at 64 utterances.
+  // utterances (one 8-utterance B operand) and the fused q + attention stage (Wq stays on the FMA path).  OPT-IN
+  // (sopro_ar_session_set_contraction(1) or SOPRO_AR_TC=1): exact, but not the default -- a CTA owns only 22..86 weight
+  // rows per stage, so most of every 64-row instruction is idle work and the operand-building stage-in is extra.
   static const int tc_env = getenv("SOPRO_AR_TC") ? atoi(getenv("SOPRO_AR_TC")) : -1;
   const bool tc_want = s->tc_mode == 1 || (s->tc_mode == -1 && tc_env == 1);
   bool tc = tc_want && e->tc_ok && Bt >= 5 && Bt <= 8 && use_qatt(e, P);
@@ -897,7 +896,8 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
     const size_t glu_need = ksc * 4096 + (size_t)2 * Bt * e->D * 4 + (size_t)64 * 8 * e->KcP * 4;
     PH = P / e->H;
     const size_t need_att = need_att_base + (size_t)((Bt + PH - 1) / PH) * (e->D + e->Dh) * 4;
-    act_bytes = align_up(std::max(std::max(bt_full, glu_need), std::max(need_att, need_smp)), 1024);
+    // + the accumulator scratch at the end of the region
+    act_bytes = align_up(std::max(std::max(bt_full, glu_need), std::max(need_att, need_smp)), 1024) + kTcDBytes;
     if (act_bytes + table_bytes + 3 * 8192 > kSmemCap) {
       tc = false;
     } else {
@@ -922,7 +922,7 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
     full = align_up(full, 128);
     // The fused q + attention stage (one exchange and one GEMV stage fewer per attention layer) streams a whole head's
     // Wq rows through every serving CTA: taken when that head tile fits at most two ring buffers (batched launches); a
-    // batch-1 launch, whose 148 CTAs hold slivers of every matrix, keeps the q stage spread over all CTAs.
+    // batch-1 launch, whose CTAs (one per SM) hold slivers of every matrix, keeps the q stage spread over all CTAs.
     for (;;) {
       size_t need_att = need_att_base;
       PH = qatt ? P / e->H : 1;

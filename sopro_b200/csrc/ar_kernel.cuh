@@ -1,4 +1,4 @@
-// Persistent autoregressive codec-token kernel for sm_100a.
+// Persistent autoregressive codec-token kernel for sm_90a.
 //
 // One launch runs up to n_steps frames for a batch of independent utterances:
 // the body of SoproTTSModel.ar_stream's loop (reference model.py:265-305) —
@@ -16,7 +16,7 @@
 // of its use (the weights do not depend on other CTAs), so a stage never waits
 // on a weight load; the [utterances x K] activations are broadcast through L2.
 // Stages are separated by a team-scoped barrier (one counter per team,
-// release/acquire at gpu scope).  All arithmetic is fp32 (FFMA2 packed pairs,
+// release/acquire at gpu scope).  All arithmetic is fp32 (FMA on element pairs,
 // warp-shuffle reductions); bf16 is a weight STORAGE format only.
 //
 // The step is written as a small INTERPRETER over a host-built stage program
@@ -27,6 +27,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace sopro {
 
@@ -42,6 +44,9 @@ constexpr int kTimingSlots = 224;  // [0,160) stage stamps, [160,192) sampler ph
 constexpr int kMaxStages = 6 * kMaxLayers + 2;
 constexpr int kMaxTilesPerStep = 128;
 constexpr int kMaxWBuf = 8;
+
+// fma of an element pair, one rounding per element
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 enum StageKind { K_GLU = 0, K_FFN1 = 1, K_FFN2 = 2, K_Q = 3, K_O = 4, K_HEAD = 5, K_ATT = 6, K_SAMPLE = 7, K_QATT = 8 };
 
@@ -93,7 +98,7 @@ struct TileDesc {
   int off2;                 // float index of the tile's first row inside part 2
   int row0;                 // first output feature of the tile
   int nrows;
-  int ngrp;                 // tensor-core tiles: 8-row groups in part 0 (0 = row-major tile of the FFMA2 path)
+  int ngrp;                 // tensor-core tiles: 8-row groups in part 0 (0 = row-major tile of the FMA path)
   int kc0;                  // tensor-core tiles: first 64-wide K chunk of the B operand this tile contracts with
   int flags;                // tensor-core tiles: bit 0 = first K slice of its rows (accumulator reset), bit 1 = last (epilogue)
 };
@@ -141,10 +146,10 @@ struct ArParams {
   const int* n_tiles;     // [P] tiles per step of each rank
   const unsigned char* stage_tiles;  // [P][kMaxStages] tiles of each stage
   int nbuf, wbuf_bytes, act_bytes;
-  // dynamic shared-memory map (bytes from the 1024-byte aligned base): FFMA2 path [act | ring | table]; tensor-core
+  // dynamic shared-memory map (bytes from the 1024-byte aligned base): FMA path [act | ring | table]; tensor-core
   // path [ring | B operand + staging | table]
   int act_off, ring_off, table_off;
-  int tc;   // 1: the GEMV stages contract on tcgen05 (bf16 weights, teams of <= 8 utterances)
+  int tc;   // 1: the GEMV stages contract on the tensor cores (wgmma; bf16 weights, teams of <= 8 utterances)
   int ksc;  // tensor-core path: 64-wide K chunks per K slice (= D / 64); a [.. x F] matrix is F / D slices
   long long* timing;  // debug: [grid][kTimingSlots] clock64 stamps of step `timing_step` (null = off)
   int timing_step;
@@ -273,7 +278,7 @@ __device__ __forceinline__ void team_barrier(unsigned* counter, unsigned P, unsi
 }
 
 // ---------------------------------------------------------------------------
-// TMA 1-D bulk copy + mbarrier + cp.async helpers (sm_90+/sm_100a PTX)
+// TMA 1-D bulk copy + mbarrier + cp.async helpers (sm_90 PTX)
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
@@ -333,55 +338,26 @@ __device__ __forceinline__ float4 ldsw4<__nv_bfloat16>(unsigned a) {
 }
 
 // ---------------------------------------------------------------------------
-// tcgen05 contraction of the batched launches (bf16 weight storage, teams of <= 8 utterances).
-//   D[64 rows x 32] (+)= A[64 x 16] . B[32 x 16]^T per instruction, fp32 accumulation in tensor memory.
+// Tensor-core (wgmma) contraction of the batched launches (bf16 weight storage, teams of <= 8 utterances).
+//   D[64 rows x 32] (+)= A[64 x 16] . B[32 x 16]^T per instruction, fp32 accumulation in the registers of warpgroup 0.
 //   A = this CTA's weight rows: the host stores them as the shared-memory IMAGE the tensor core reads (K-major,
 //       128-byte swizzle, 8-row groups of [K chunks][8 x 128 B]; group stride = SBO), so the 1-D TMA bulk copy of the
 //       weight ring delivers a ready operand.  A tile has <= 8 groups; the instruction always reads 64 rows, the rows
-//       past the tile are whatever follows in shared memory and only reach accumulator lanes nobody reads.
-//       (M = 64: accumulator row m lives in tensor-memory lane 32 * (m / 16) + m % 16, cute's "half subpartitions" atom.)
+//       past the tile are whatever follows in shared memory and only reach accumulator rows nobody reads.
 //   B = the team's activations, each fp32 value split into THREE bf16 terms x = hi + mid + lo (exact: 3 x 8 mantissa
 //       bits): B row 4u + s holds term s of utterance u (row 4u + 3 is zero).  bf16 x bf16 products are exact in fp32,
-//       so D column 4u+0..2 summed = sum_k w[k] * x[k] with fp32 accumulation -- the same arithmetic as the FFMA2 path
+//       so D column 4u+0..2 summed = sum_k w[k] * x[k] with fp32 accumulation -- the same arithmetic as the FMA path
 //       up to the order of the fp32 additions.
+//   The finished accumulator goes through a [64][kTcDPitch] fp32 scratch in shared memory (behind the activation
+//   region) to the epilogue threads, one (row, two utterances) per thread.
 // ---------------------------------------------------------------------------
 constexpr int kTcCols = 32;            // B rows = accumulator columns of one instruction
-constexpr int kTcAcc = 4;              // independent accumulator tiles: consecutive instructions of a tile's K loop go to
-                                       // different tiles (summed in the epilogue), so none waits for its predecessor's result
 constexpr int kTcBChunk = 32 * 128;    // bytes of one 64-wide K chunk of the B operand
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(unsigned tmem_d, unsigned long long da, unsigned long long db, unsigned idesc,
-                                            unsigned accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 8 consecutive fp32 columns -> 8 registers of this thread's lane
-__device__ __forceinline__ void tc_ld8(unsigned taddr, unsigned (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups `sbo` bytes apart (bit layout:
-// cute/arch/mma_sm100_desc.hpp; the same constructor the Mimi kernels use, mimi_tc.cuh)
-__device__ __forceinline__ unsigned long long tc_desc(unsigned addr, unsigned sbo) {
-  return (unsigned long long)((addr & 0x3FFFFu) >> 4) | ((unsigned long long)(sbo >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor kind::f16: D fp32, A / B bf16, both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-__host__ __device__ constexpr unsigned tc_idesc(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(N >> 3) << 17) | ((unsigned)(M >> 4) << 24);
-}
+constexpr int kTcDPitch = kTcCols + 1;  // accumulator scratch row pitch (floats)
+constexpr int kTcDBytes = 9 * 1024;     // accumulator scratch, 1024-byte multiple
+static_assert(64 * kTcDPitch * 4 <= kTcDBytes, "accumulator scratch");
+// shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups `sbo` bytes apart
+__device__ __forceinline__ unsigned long long tc_desc(unsigned addr, unsigned sbo) { return wg::desc_sw128(addr, sbo); }
 __device__ __forceinline__ void sts128(unsigned a, unsigned x, unsigned y, unsigned z, unsigned w) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
 }
@@ -577,7 +553,7 @@ struct WeightRing {
 
 // ---------------------------------------------------------------------------
 // warp GEMV tile, 2 rows x TU utterances: out[r][u] = sum_k W[row_r][k] * act[u][k]
-// lanes split K (4 consecutive k per lane per 128-k chunk), FFMA2 accumulation, butterfly
+// lanes split K (4 consecutive k per lane per 128-k chunk), fp32 FMA accumulation on element pairs, butterfly
 // reduction (every lane ends with all totals).  Weights AND activations in shared memory.
 // ---------------------------------------------------------------------------
 // After the K loop the 2*TU partial sums of every lane are combined with a TRANSPOSED reduction:
@@ -631,8 +607,8 @@ __device__ __forceinline__ float warp_rows_s(const unsigned (&w)[R], unsigned ac
       const float4 x = lds128(act + ((unsigned)u * (unsigned)K + (unsigned)k) * 4u);
 #pragma unroll
       for (int r = 0; r < R; ++r) {
-        acc[r][u] = __ffma2_rn(make_float2(wv[r].x, wv[r].y), make_float2(x.x, x.y), acc[r][u]);
-        acc[r][u] = __ffma2_rn(make_float2(wv[r].z, wv[r].w), make_float2(x.z, x.w), acc[r][u]);
+        acc[r][u] = ffma2(make_float2(wv[r].x, wv[r].y), make_float2(x.x, x.y), acc[r][u]);
+        acc[r][u] = ffma2(make_float2(wv[r].z, wv[r].w), make_float2(x.z, x.w), acc[r][u]);
       }
     }
   }
@@ -658,10 +634,10 @@ __device__ __forceinline__ void warp_rows_g(const WT* w0, const WT* w1, const fl
 #pragma unroll
     for (int u = 0; u < TU; ++u) {
       const float4 x = *reinterpret_cast<const float4*>(act + (size_t)u * K + k);
-      acc[0][u] = __ffma2_rn(make_float2(wa.x, wa.y), make_float2(x.x, x.y), acc[0][u]);
-      acc[0][u] = __ffma2_rn(make_float2(wa.z, wa.w), make_float2(x.z, x.w), acc[0][u]);
-      acc[1][u] = __ffma2_rn(make_float2(wb.x, wb.y), make_float2(x.x, x.y), acc[1][u]);
-      acc[1][u] = __ffma2_rn(make_float2(wb.z, wb.w), make_float2(x.z, x.w), acc[1][u]);
+      acc[0][u] = ffma2(make_float2(wa.x, wa.y), make_float2(x.x, x.y), acc[0][u]);
+      acc[0][u] = ffma2(make_float2(wa.z, wa.w), make_float2(x.z, x.w), acc[0][u]);
+      acc[1][u] = ffma2(make_float2(wb.x, wb.y), make_float2(x.x, x.y), acc[1][u]);
+      acc[1][u] = ffma2(make_float2(wb.z, wb.w), make_float2(x.z, x.w), acc[1][u]);
     }
   }
 #pragma unroll
@@ -1522,11 +1498,9 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
   __shared__ unsigned char stage_tiles[kMaxStages];
   __shared__ int conv_phase[kMaxLayers], conv_slot[kMaxLayers];
   __shared__ int s_tok[kMaxUttPerTeam], s_done[kMaxUttPerTeam];
-  __shared__ __align__(8) unsigned long long accbar;  // tensor-core path: "accumulator ready" mbarrier
-  __shared__ unsigned tmem_slot;
   __shared__ float tc_part[TC ? 8 * 32 : 1];  // tensor-core stage-in: per-row partial sums of squares
   constexpr int EL = LL ? 2 : 1;  // floats per activation element in the exchange buffers
-  // the tcgen05 instantiations (TC: bf16 weights, TU == 8) carry no FFMA2 tile loop and vice versa
+  // the tensor-core instantiations (TC: bf16 weights, TU == 8) carry no FMA tile loop and vice versa
   static_assert(!TC || (TU == 8 && sizeof(WT) == 2), "tensor-core path: bf16 weights, 8-utterance B operand");
   // dynamic shared memory, 1024-byte aligned (the swizzled tensor-core operands need it): p.act_off / ring_off / table_off
   unsigned char* const smem_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -1552,7 +1526,7 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
   const unsigned gact_s = smem_u32(gact);
   float* xraw = gact + (size_t)tc.nb * D;  // second [nb][D] buffer (GLU stage only)
   const unsigned scratch_s = gact_s + (unsigned)(2 * tc.nb * D) * 4u;  // GLU stage: dwconv tap rows
-  unsigned acc_phase = 0;
+  float* const tcd = reinterpret_cast<float*>(smem_base + p.act_off + p.act_bytes - kTcDBytes);  // tensor-core path only
   const int n_ut = (tc.nb + TU - 1) / TU;
   // ---- weight ring: [act region][nbuf x wbuf][tile table]
   WeightRing ring;
@@ -1564,18 +1538,9 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
     for (int i = threadIdx.x; i < p.n_stage; i += kThreads) stage_tiles[i] = p.stage_tiles[(size_t)tc.rank * kMaxStages + i];
     if (threadIdx.x == 0) {
       for (int i = 0; i < p.nbuf; ++i) mbar_init(&wbars[i], 1);
-      mbar_init(&accbar, TC ? kTcAcc : 1);  // one commit per issuing thread
       asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (TC && warp == 0) {  // 32 tensor-memory columns for the whole launch
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                   "r"((unsigned)(kTcCols * kTcAcc))
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (TC) tc_fence_before();
     __syncthreads();
-    if (TC) tc_fence_after();
     ring.bars = wbars;
     ring.base = smem_u32(smem_base + p.ring_off);
     ring.wbuf = (unsigned)p.wbuf_bytes;
@@ -1720,11 +1685,10 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
         const int dil = L.dil;
         const int phase = conv_phase[li], slot_now = conv_slot[li];
         if constexpr (TC) {
-          // ================= tensor-core tiles: thread = (accumulator row, two utterances)
-          // M = 64: accumulator row m sits in tensor-memory lane 32 * (m / 16) + m % 16 -> lanes 0..15 of every warp work
-          const int q = warp & 3, jc = warp >> 2;  // tensor-memory lane quarter; columns 8jc..8jc+7 = utterances 2jc, 2jc+1
+          // ================= tensor-core tiles: epilogue thread = (accumulator row, two utterances)
+          const int q = warp & 3, jc = warp >> 2;  // rows 16q..16q+15 (lanes 0..15); columns 8jc..8jc+7 = utterances 2jc, 2jc+1
           const int rt = lane < 16 ? 16 * q + lane : 64;  // row of the tile (64 = none)
-          const unsigned tmem = tmem_slot;
+          float dacc[kTcCols / 2];  // warpgroup 0: the accumulator, carried across the tiles of one output row block
           long long* tdbg = (ts.buf && (si == 1 || si == 7)) ? ts.buf + (si == 1 ? 192 : 208) : nullptr;  // tile phase stamps
           int tdn = 0;
 #define TCMARK() do { if (tdbg && tdn < 16) tdbg[tdn++] = clock64(); } while (0)
@@ -1761,41 +1725,42 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
               }
               cp_async_commit();
             }
-            // ---- the contraction: one thread issues (K slices of the tile) x (D / 64) x 4 instructions [64 x 32 x 16]
-            if (lane == 0 && warp < kTcAcc) {  // one issuing thread per accumulator tile (K slice `warp` of every chunk)
-              tc_fence_after();
-              constexpr unsigned idesc = tc_idesc(64, kTcCols);
+            // ---- the contraction: warpgroup 0 issues (K slices of the tile) x (D / 64) x 4 instructions [64 x 32 x 16]
+            if (warp < 4) {
               const bool first = (td->flags & 1) != 0;
               const int nsl = td->bytes1 ? 2 : 1;  // part 1 = the same rows' next K slice
+              wg::fence();
 #pragma unroll 1
               for (int sl = 0; sl < nsl; ++sl) {
                 const unsigned long long da = tc_desc(wb + (unsigned)sl * td->bytes0, (unsigned)p.ksc * 1024u);
                 const unsigned long long db = tc_desc(act_s + (unsigned)(td->kc0 + sl * p.ksc) * (unsigned)kTcBChunk, 1024u);
 #pragma unroll 1
                 for (int c = 0; c < p.ksc; ++c) {
-                  const int k = warp;  // K slice k of every chunk accumulates in tile k (kTcAcc == 4)
-                  tc_mma_bf16(tmem + (unsigned)(k * kTcCols), da + (unsigned long long)(c * 64 + k * 2),
-                              db + (unsigned long long)(c * (kTcBChunk >> 4) + k * 2), idesc, (first && sl == 0 && c == 0) ? 0u : 1u);
+#pragma unroll
+                  for (int k = 0; k < 4; ++k)
+                    wg::mma_ss<kTcCols>(dacc, da + (unsigned long long)(c * 64 + k * 2), db + (unsigned long long)(c * (kTcBChunk >> 4) + k * 2),
+                                        (first && sl == 0 && c == 0 && k == 0) ? 0u : 1u);
                 }
               }
-              tc_commit(&accbar);  // arrives when every instruction above has completed (also frees the weight buffer)
+              wg::commit();
               TCMARK();  // instructions issued
+              wg::wait<0>();  // also: the weight buffer may be released
+              wg::fence_regs(dacc);
+              if (last) {
+#pragma unroll
+                for (int i = 0; i < kTcCols / 2; ++i)
+                  tcd[(16 * warp + (lane >> 2) + 8 * ((i >> 1) & 1)) * kTcDPitch + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)] = dacc[i];
+              }
             }
-            mbar_wait(&accbar, acc_phase);
-            acc_phase ^= 1u;
             TCMARK();  // accumulator complete
             if (last) {
-              tc_fence_after();
+              __syncthreads();
               float vv[2] = {0.f, 0.f};
-#pragma unroll
-              for (int a = 0; a < kTcAcc; ++a) {  // the accumulator tiles in a fixed order
-                unsigned d8[8];
-                tc_ld8(tmem + ((unsigned)(32 * q) << 16) + (unsigned)(a * kTcCols + 8 * jc), d8);
-                // x = hi + mid + lo: add the small terms first
-                vv[0] += (__uint_as_float(d8[2]) + __uint_as_float(d8[1])) + __uint_as_float(d8[0]);
-                vv[1] += (__uint_as_float(d8[6]) + __uint_as_float(d8[5])) + __uint_as_float(d8[4]);
+              if (rt < 64) {  // x = hi + mid + lo: add the small terms first
+                const float* dr = tcd + rt * kTcDPitch + 8 * jc;
+                vv[0] = (dr[2] + dr[1]) + dr[0];
+                vv[1] = (dr[6] + dr[5]) + dr[4];
               }
-              tc_fence_before();
               cp_async_wait0();
               TCMARK();  // accumulator in registers
 #pragma unroll
@@ -1987,14 +1952,6 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
     }
   }
   ring.drain();  // early team exit: prefetched tiles must land before the CTA exits
-  if (TC) {
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-      tc_fence_after();
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"((unsigned)(kTcCols * kTcAcc)) : "memory");
-    }
-  }
 }
 
 // ---------------------------------------------------------------------------

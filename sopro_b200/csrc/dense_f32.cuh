@@ -1,7 +1,7 @@
 // fp32 building blocks of the parallel-in-time stages around the AR kernel: the NAR refiner
 // (reference nn/nar.py:13-116, model.py:307-347) and the prefill (model.py:172-216, nn/text.py:16-44,
 // nn/speaker.py:64-85, nn/ref.py:16-160).  Their results are integer ids (NAR argmax) or inputs of the
-// id-exact AR kernel (cond_ar, txt_seq), so every contraction is fp32 on the FMA pipe (FFMA2 pairs, fp32
+// id-exact AR kernel (cond_ar, txt_seq), so every contraction is fp32 on the FMA pipe (element pairs, fp32
 // accumulate) -- no tensor cores, no reduced precision.
 //
 //   dense_tile_kernel    C[M][N] = epi(prologue(A)[M][K] . W[N][K]^T): 128x128x16 tiles, 8x8 outputs per thread
@@ -15,6 +15,9 @@
 #include <stdint.h>
 
 namespace dense {
+
+// fma of an element pair, one rounding per element
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 enum { EPI_BIAS = 0, EPI_GELU = 1, EPI_RES = 2, EPI_GLU = 3, EPI_ARGMAX = 4, EPI_RES_GATE = 5 };
 
@@ -212,7 +215,7 @@ __global__ void __launch_bounds__(kTileThreads, 2) dense_tile_kernel(const Dense
       for (int i = 0; i < TM; ++i) {
         const float2 aa = make_float2(a[i], a[i]);
 #pragma unroll
-        for (int j = 0; j < TP; ++j) acc[i][j] = __ffma2_rn(aa, b[j], acc[i][j]);
+        for (int j = 0; j < TP; ++j) acc[i][j] = ffma2(aa, b[j], acc[i][j]);
       }
     }
     if (kt + 1 < nk) store(buf ^ 1, ra, rb);

@@ -1,4 +1,4 @@
-// Mimi codec DECODE path on sm_100a: codes [B, Q, T] -> wav [B, T*1920].
+// Mimi codec DECODE path on sm_90a: codes [B, Q, T] -> wav [B, T*1920].
 //
 // Replaces transformers.MimiModel.decode as called by the reference (codec/mimi.py:65-72):
 // RVQ lookup-sum + 1x1 projections, depthwise 2x ConvTranspose upsample, 8-layer causal
@@ -11,10 +11,10 @@
 // activations [T, C]: Linear, causal Conv1d (K = taps x Cin gathered from shifted rows) and causal
 // ConvTranspose1d (stride s, kernel 2s == a 2-tap conv producing s*Cout columns, which IS the
 // channel-last upsampled tensor), with ELU fused on the operand load and bias / GELU / LayerScale
-// residual fused in the epilogue.  This first version runs the contractions in fp32 on the FFMA2
+// residual fused in the epilogue.  This first version runs the contractions in fp32 on the FMA
 // pipe (parity 1e-4 against the fp32 oracle).  SOPRO_MIMI_BF16_TC mode (mimi_tc.cuh) runs every
-// contraction whose channel count allows it on the tcgen05 tensor cores with bf16 operands, fp32
-// accumulation in tensor memory and the same fused epilogues; the fp32 kernels stay for the exact mode
+// contraction whose channel count allows it on the tensor cores (wgmma) with bf16 operands, fp32
+// accumulation in registers and the same fused epilogues; the fp32 kernels stay for the exact mode
 // and for the few narrow layers (Cin < 64).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -537,7 +537,7 @@ int sopro_mimi_create(const sopro_mimi_config_t* cfg, const sopro_mimi_weights_t
   if (device < 0 || device >= ndev) return mfail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
   MCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return mfail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return mfail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int C = cfg->hidden, Dc = cfg->codebook_dim, Q = cfg->n_q, V = cfg->vocab, NL = cfg->n_layers, FF = cfg->ffn;
   if (C % 64 || Dc % 4 || C != 2 * Dc || NL < 1 || cfg->n_ratios < 1 || cfg->n_ratios > 8 || cfg->n_heads < 1 || C % cfg->n_heads ||
       (C / cfg->n_heads) % 4 || FF % 16)
@@ -1642,7 +1642,7 @@ int sopro_mimi_encoder_create(const sopro_mimi_config_t* cfg, const sopro_mimi_e
   if (device < 0 || device >= ndev) return mfail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
   MCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return mfail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return mfail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int C = cfg->hidden, Dc = cfg->codebook_dim, Q = cfg->n_q, V = cfg->vocab, NL = cfg->n_layers, FF = cfg->ffn, F0 = cfg->num_filters;
   if (C % 64 || Dc != 256 || C != 2 * Dc || NL < 1 || NL > SOPRO_MIMI_MAX_LAYERS || cfg->n_ratios < 1 || cfg->n_ratios > SOPRO_MIMI_MAX_RATIOS ||
       cfg->n_heads < 1 || C % cfg->n_heads || (C / cfg->n_heads) % 4 || FF % 16 || F0 % 16 || cfg->compress != 2 || Q < 1 || cfg->n_sem < 1 ||

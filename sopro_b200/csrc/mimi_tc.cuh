@@ -1,22 +1,21 @@
-// tcgen05 / TMEM / TMA implicit GEMM for the Mimi decoder's dense blocks (sm_100a only).
+// wgmma / TMA implicit GEMM for the Mimi decoder's dense blocks (sm_90a).
 //
 //   C[b][m][n] = epi( sum_{j<taps} sum_{ci<Cin} X[b][m + j*dil - pad][ci] * W[n][j*Cin + ci] + bias[n % bias_mod] )
 //
 // X is a channel-last bf16 activation [B][Min][Cin] (already passed through ELU by its producer when
 // the layer wants ELU(x)), W is a bf16 weight matrix [N][K] (K = taps*Cin, K-major), accumulation is
-// fp32 in tensor memory.  This covers Linear, the causal Conv1d and the causal ConvTranspose1d of
+// fp32 in registers.  This covers Linear, the causal Conv1d and the causal ConvTranspose1d of
 // transformers' modeling_mimi.py (:331-351, :402-409) exactly as mimi_engine.cu's fp32 path does.
 //
 // One CTA computes one 128 x BN tile:
-//   warp 0    TMA producer: per 64-wide K chunk one 3-D box of X (rows shifted by the tap; rows outside
-//             [0, Min) are zero-filled by the TMA unit == the causal left pad) and one 2-D box of W,
-//             both landing 128B-swizzled in a ring of shared-memory stages, completion on mbarriers
-//   warp 1    allocates BN tensor-memory columns, one lane issues tcgen05.mma (M=128, N=BN, K=16) four
-//             times per chunk; tcgen05.commit releases the stage / signals the accumulator
-//   warps 2-5 epilogue: tcgen05.ld 32 lanes x 32 columns, bias / GELU / LayerScale-residual / skip,
-//             writes fp32 and/or bf16 (optionally ELU'd: the next layer's operand)
-// Two CTAs are resident per SM (<= 100 KB of stages each), so one tile's epilogue overlaps the other's
-// main loop.
+//   warp 8      TMA producer: per K chunk one 3-D box of X (rows shifted by the tap; rows outside
+//               [0, Min) are zero-filled by the TMA unit == the causal left pad) and one 2-D box of W,
+//               both landing swizzled in a ring of shared-memory stages, completion on mbarriers
+//   warps 0-7   two consumer warpgroups, 64 tile rows each: wgmma (M=64, N=BN, K=16) from shared-memory
+//               descriptors, one chunk in flight while the previous one's stage goes back to the producer;
+//               then the accumulators go through the idle stage memory so that the epilogue (bias / GELU /
+//               LayerScale-residual / skip, fp32 and/or bf16 out, optionally ELU'd: the next layer's operand)
+//               reads and writes whole rows with 16-byte accesses
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -25,6 +24,8 @@
 #include <cmath>
 #include <cstdint>
 #include <cstdlib>
+
+#include "wgmma.cuh"
 
 namespace tc {
 
@@ -51,6 +52,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
       "{\n"
@@ -74,97 +78,42 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm,
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> one row slice per thread
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 bf16 (128 B) stacked
-// densely: 8-row groups are 1024 B apart (SBO), one swizzle atom along K (LBO unused).
-// Bit layout: cute/arch/mma_sm100_desc.hpp (SmemDescriptor): addr>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type [61,64) with SWIZZLE_128B = 2.
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t addr) {
-  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// same for rows of 32 bf16 (64 B), 64-byte swizzle: 8-row groups 512 B apart, layout_type SWIZZLE_64B = 4
-__device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t addr) {
-  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(512u >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
-template <int BK>
-__device__ __forceinline__ uint64_t smem_desc_k(uint32_t addr) {
-  return BK == 64 ? smem_desc_sw128(addr) : smem_desc_sw64(addr);
-}
-// instruction descriptor, kind::f16: D fp32 (bits [4,6) = 1), A/B bf16 ([7,10) = [10,13) = 1), both
-// K-major (bits 15, 16 = 0), N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t instr_desc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// 256-bit global accesses (one full 32-byte sector per thread per instruction)
-__device__ __forceinline__ void stg256(void* p, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-               "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void ldg256(const void* p, float (&v)[8]) {
-  asm volatile("ld.global.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
-}
+// barrier of the 128 threads of one warpgroup (ids 1, 2: 0 is __syncthreads')
+__device__ __forceinline__ void wg_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
 
 __device__ __forceinline__ float elu1(float x) { return x > 0.f ? x : expm1f(x); }
 // ELU whose result is rounded to bf16 right away: exp(x) - 1 with the fast exponential is exact to well below
 // half a bf16 ulp (absolute error ~1e-7 against a result of magnitude >= |x|/2)
 __device__ __forceinline__ float elu_fast(float x) { return x > 0.f ? x : __expf(x) - 1.0f; }
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
 
-constexpr int kBM = 128, kBK = 64, kThreads = 192;
-constexpr int kGemmThreads = 320;  // TMA warp, MMA warp, 8 epilogue warps (2 per tensor-memory lane quarter)
+constexpr int kBM = 128, kBK = 64;
+constexpr int kGemmThreads = 288;  // two consumer warpgroups (64 tile rows each) + one TMA producer warp
+constexpr int kProducerWarp = 8;
 template <int BN, int BK>
 struct TileCfg {
   static constexpr int kMaxStages = BN >= 128 ? 3 : 4;
   static constexpr int kABytes = kBM * BK * 2;  // 16 KB at BK = 64
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int smem(int stages) { return stages * kStageBytes + 1024; }  // + alignment slack
-  static constexpr int kTmemCols = BN < 32 ? 32 : BN;
+  static constexpr int kEpiPitch = BN + 8;                    // floats per row of the epilogue tile (conflict-free fragment stores)
+  static constexpr int kEpiBytes = kBM * kEpiPitch * 4;       // the 128 x BN fp32 tile, over the stages once they are idle
+  static constexpr int smem(int stages) { return (stages * kStageBytes > kEpiBytes ? stages * kStageBytes : kEpiBytes) + 1024; }
 };
 
 template <int BN, int BK>
-__global__ void __launch_bounds__(kGemmThreads, 3) igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                const __grid_constant__ CUtensorMap tmW, const TcOp op) {
+__global__ void __launch_bounds__(kGemmThreads, BN >= 128 ? 1 : 2) igemm_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                                   const __grid_constant__ CUtensorMap tmW, const TcOp op) {
   using Cfg = TileCfg<BN, BK>;
   constexpr int SM = Cfg::kMaxStages;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bars[2 * SM + 1];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bars[2 * SM];
   const uint32_t tiles = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[SM]), accbar = smem_u32(&bars[2 * SM]);
+  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[SM]);
   const int S = op.stages;  // min(kMaxStages, K chunks): short-K layers take less shared memory -> more CTAs per SM
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * kBM, n0 = blockIdx.y * BN, b = blockIdx.z;
@@ -173,23 +122,13 @@ __global__ void __launch_bounds__(kGemmThreads, 3) igemm_tc_kernel(const __grid_
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(accbar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                 "r"((uint32_t)Cfg::kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       for (int kc = 0; kc < nk; ++kc) {
         const int s = kc % S;
@@ -203,119 +142,81 @@ __global__ void __launch_bounds__(kGemmThreads, 3) igemm_tc_kernel(const __grid_
         tma_load_2d(sa + Cfg::kABytes, &tmW, full0 + 8 * s, k0, n0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = instr_desc_bf16(kBM, BN);
-      for (int kc = 0; kc < nk; ++kc) {
-        const int s = kc % S;
-        const uint32_t ph = (uint32_t)(kc / S) & 1u;
-        mbar_wait(full0 + 8 * s, ph);
-        tc_fence_after();
-        const uint32_t sa = tiles + s * Cfg::kStageBytes;
-        const uint64_t da = smem_desc_k<BK>(sa), db = smem_desc_k<BK>(sa + Cfg::kABytes);
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)  // +32 B per K=16 slice inside the swizzle atom
-          tc_mma_bf16(tmem, da + 2 * k, db + 2 * k, idesc, (kc | k) != 0);
-        tc_commit(empty0 + 8 * s);
-      }
-      tc_commit(accbar);
-    }
-  } else {
-    mbar_wait(accbar, 0);
-    tc_fence_after();
-    const int q = warp & 3;  // tensor-memory lane quarter this warp may read
-    const int m = m0 + 32 * q + lane;
-    const bool row_ok = m < op.M;
-    const size_t row = (size_t)b * (size_t)op.c_bs + (size_t)m * op.N;
-    // the two warps of a quarter split the columns (a 32-column tile is done by the first alone)
-    constexpr int kColsPerWarp = BN >= 64 ? BN / 2 : BN;
-    const int cbeg = BN >= 64 ? ((warp - 2) >> 2) * kColsPerWarp : ((warp - 2) >> 2) * BN;
-#pragma unroll 1
-    for (int c0 = cbeg; c0 < cbeg + kColsPerWarp && c0 < BN; c0 += 32) {
-      uint32_t r[32];
-      tc_ld32(tmem + ((uint32_t)(32 * q) << 16) + (uint32_t)c0, r);
-      if (!row_ok) continue;
-      const int n = n0 + c0;
-      float v[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-      if (op.bias) {
-        const int nb = n % op.bias_mod;  // bias_mod is a multiple of 32 whenever N > bias_mod
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          const float4 bv = __ldg(reinterpret_cast<const float4*>(op.bias + nb + i));
-          v[i] += bv.x;
-          v[i + 1] += bv.y;
-          v[i + 2] += bv.z;
-          v[i + 3] += bv.w;
-        }
-      }
-      if (op.epi == EPI_GELU) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-      } else if (op.epi == EPI_RES_SCALE || op.epi == EPI_RES) {
-        const float* rp = op.R + row + n;
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          float rv[8];
-          ldg256(rp + i, rv);
-          if (op.epi == EPI_RES_SCALE) {
-            const float4 s0 = __ldg(reinterpret_cast<const float4*>(op.scale + n + i));
-            const float4 s1 = __ldg(reinterpret_cast<const float4*>(op.scale + n + i + 4));
-            const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-#pragma unroll
-            for (int e = 0; e < 8; ++e) v[i + e] = fmaf(sv[e], v[i + e], rv[e]);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) v[i + e] += rv[e];
-          }
-        }
-      }
-      if (op.out_f32) {
-        float* o = op.out_f32 + row + n;
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint32_t w8[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) w8[e] = __float_as_uint(v[i + e]);
-          stg256(o + i, w8);
-        }
-      }
-      if (op.out_bf16) {
-        __nv_bfloat16* o = op.out_bf16 + row + n;
-#pragma unroll
-        for (int i = 0; i < 32; i += 16) {
-          uint32_t pk[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float a = v[i + 2 * e], c = v[i + 2 * e + 1];
-            if (op.out_elu) {
-              a = elu_fast(a);
-              c = elu_fast(c);
-            }
-            const __nv_bfloat162 h = __floats2bfloat162_rn(a, c);
-            pk[e] = *reinterpret_cast<const uint32_t*>(&h);
-          }
-          stg256(o + i, pk);
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)Cfg::kTmemCols) : "memory");
+  const int g = warp >> 2;  // consumer warpgroup: tile rows 64g .. 64g + 63
+  float d[BN / 2];
+#pragma unroll 1
+  for (int kc = 0; kc < nk; ++kc) {
+    const int s = kc % S;
+    mbar_wait(full0 + 8 * s, (uint32_t)(kc / S) & 1u);
+    const uint32_t sa = tiles + s * Cfg::kStageBytes;
+    const uint64_t da = wg::desc_k<BK>(sa + (uint32_t)g * (64u * BK * 2u)), db = wg::desc_k<BK>(sa + Cfg::kABytes);
+    wg::fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)  // +32 B per K=16 slice inside the swizzle atom
+      wg::mma_ss<BN>(d, da + 2 * k, db + 2 * k, (kc | k) != 0);
+    wg::commit();
+    wg::wait<1>();  // chunk kc - 1 has completed: its stage goes back to the producer
+    if (kc > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty0 + 8 * ((kc - 1) % S));
+  }
+  wg::wait<0>();
+  wg::fence_regs(d);
+  // ---- epilogue: both warpgroups are done with every stage -> the fp32 tile goes to shared memory, then each warp
+  // handles whole rows (4 consecutive columns per thread)
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  float* et = reinterpret_cast<float*>(smem_raw + (tiles - smem_u32(smem_raw)));
+  {
+    const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(et + (r0 + 8 * h) * Cfg::kEpiPitch + 8 * j + 2 * (lane & 3)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  constexpr int TPR = BN / 4, RPP = 256 / TPR;  // threads per row, rows per pass
+  const int t = threadIdx.x, c = 4 * (t % TPR), n = n0 + c;
+#pragma unroll 1
+  for (int r = t / TPR; r < kBM; r += RPP) {
+    const int m = m0 + r;
+    if (m >= op.M) break;
+    const size_t row = (size_t)b * (size_t)op.c_bs + (size_t)m * op.N;
+    float4 v = *reinterpret_cast<const float4*>(et + r * Cfg::kEpiPitch + c);
+    if (op.bias) {
+      const float4 bv = __ldg(reinterpret_cast<const float4*>(op.bias + n % op.bias_mod));  // bias_mod is a multiple of 4
+      v.x += bv.x;
+      v.y += bv.y;
+      v.z += bv.z;
+      v.w += bv.w;
+    }
+    if (op.epi == EPI_GELU) {
+      v = make_float4(gelu_erf(v.x), gelu_erf(v.y), gelu_erf(v.z), gelu_erf(v.w));
+    } else if (op.epi == EPI_RES_SCALE || op.epi == EPI_RES) {
+      const float4 rv = *reinterpret_cast<const float4*>(op.R + row + n);  // may alias out_f32 (in-place residual)
+      if (op.epi == EPI_RES_SCALE) {
+        const float4 sv = __ldg(reinterpret_cast<const float4*>(op.scale + n));
+        v = make_float4(fmaf(sv.x, v.x, rv.x), fmaf(sv.y, v.y, rv.y), fmaf(sv.z, v.z, rv.z), fmaf(sv.w, v.w, rv.w));
+      } else {
+        v = make_float4(v.x + rv.x, v.y + rv.y, v.z + rv.z, v.w + rv.w);
+      }
+    }
+    if (op.out_f32) *reinterpret_cast<float4*>(op.out_f32 + row + n) = v;
+    if (op.out_bf16) {
+      if (op.out_elu) v = make_float4(elu_fast(v.x), elu_fast(v.y), elu_fast(v.z), elu_fast(v.w));
+      *reinterpret_cast<uint2*>(op.out_bf16 + row + n) = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+    }
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 // Fused ResnetBlock (MimiResnetBlock, modeling_mimi.py:437-451): out = z + conv1x1(ELU(conv3(ELU(z)))).
-//   GEMM 1: h[128 x HID] = conv k=3 of the bf16 ELU(z) rows (3-D TMA boxes per tap), accumulators in tensor
-//           memory columns [0, HID)
-//   epilogue A: + bias, ELU, round to bf16, written swizzled into shared memory as the next A operand
-//   GEMM 2: [128 x 2*HID] = h . W2^T (W2 loaded once per CTA) into columns [HID, 3*HID)
-//   epilogue B: + bias + z (fp32 skip, read once), then fp32 and/or bf16(ELU) out
+//   GEMM 1: h[128 x HID] = conv k=3 of the bf16 ELU(z) rows (3-D TMA boxes per tap), accumulators in registers
+//   epilogue A: + bias, ELU, round to bf16, written swizzled into shared memory as the next A operand (each
+//           warpgroup writes the 64 rows its own GEMM 2 reads)
+//   GEMM 2: [128 x 2*HID] = h . W2^T (W2 loaded once per CTA), in column blocks of <= 128
+//   epilogue B: through the idle stage memory (whole rows, 16-byte accesses): + bias + z (fp32 skip, read once),
+//           then fp32 and/or bf16(ELU) out
 // The hidden activation never touches HBM and one launch replaces two.  HID in {32, 64, 128}.
 // ---------------------------------------------------------------------------------------------
 struct ResOp {
@@ -333,32 +234,33 @@ struct ResCfg {
   static constexpr int kCout = 2 * HID;
   static constexpr int kBKH = HID < 64 ? HID : 64;       // K chunk of the second GEMM
   static constexpr int kNK2 = HID / kBKH;
+  static constexpr int kN2 = kCout < 128 ? kCout : 128;  // column block of the second GEMM
   static constexpr int kMaxStages = 3;
   static constexpr int kABytes = kBM * kBK * 2;           // 16 KB
   static constexpr int kBBytes = HID * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kHBytes = kBM * HID * 2;           // hidden activation as the A operand of GEMM 2
   static constexpr int kW2Bytes = kCout * HID * 2;
-  static constexpr int kTmemCols = 3 * HID <= 128 ? 128 : (3 * HID <= 256 ? 256 : 512);
-  static constexpr int smem(int stages) { return stages * kStageBytes + kHBytes + kW2Bytes + 1024; }
+  static constexpr int kEpiPitch = kN2 + 8;                  // floats per row of the epilogue tile
+  static constexpr int kEpiBytes = kBM * kEpiPitch * 4;
+  // the stage ring, which also holds the epilogue tile of GEMM 2 once GEMM 1 is done
+  static constexpr int ring(int stages) { return stages * kStageBytes > kEpiBytes ? stages * kStageBytes : kEpiBytes; }
+  static constexpr int smem(int stages) { return ring(stages) + kHBytes + kW2Bytes + 1024; }
 };
 
 template <int HID>
-__global__ void __launch_bounds__(kGemmThreads, HID <= 32 ? 3 : (HID <= 64 ? 2 : 1)) resblock_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                                     const __grid_constant__ CUtensorMap tmW1,
-                                                                                     const __grid_constant__ CUtensorMap tmW2,
-                                                                                     const ResOp op) {
+__global__ void __launch_bounds__(kGemmThreads, HID <= 64 ? 2 : 1) resblock_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                                      const __grid_constant__ CUtensorMap tmW1,
+                                                                                      const __grid_constant__ CUtensorMap tmW2,
+                                                                                      const ResOp op) {
   using Cfg = ResCfg<HID>;
-  constexpr int SM = Cfg::kMaxStages, COUT = Cfg::kCout, BKH = Cfg::kBKH;
+  constexpr int SM = Cfg::kMaxStages, COUT = Cfg::kCout, BKH = Cfg::kBKH, N2 = Cfg::kN2;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bars[2 * SM + 4];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bars[2 * SM + 1];
   const int S = op.stages;
   const uint32_t tiles = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sH = tiles + S * Cfg::kStageBytes, sW2 = sH + Cfg::kHBytes;
-  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[SM]);
-  const uint32_t w2_full = smem_u32(&bars[2 * SM]), acc1 = smem_u32(&bars[2 * SM + 1]), h_ready = smem_u32(&bars[2 * SM + 2]),
-                 acc2 = smem_u32(&bars[2 * SM + 3]);
+  const uint32_t sH = tiles + Cfg::ring(S), sW2 = sH + Cfg::kHBytes;
+  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[SM]), w2_full = smem_u32(&bars[2 * SM]);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * kBM, b = blockIdx.y;
   const int nk = op.taps * COUT / kBK;  // K chunks of GEMM 1 (COUT is a multiple of 64)
@@ -366,26 +268,14 @@ __global__ void __launch_bounds__(kGemmThreads, HID <= 32 ? 3 : (HID <= 64 ? 2 :
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, 2);
     }
     mbar_init(w2_full, 1);
-    mbar_init(acc1, 1);
-    mbar_init(h_ready, kGemmThreads - 64);
-    mbar_init(acc2, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                 "r"((uint32_t)Cfg::kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       mbar_expect_tx(w2_full, Cfg::kW2Bytes);
       for (int c = 0; c < Cfg::kNK2; ++c) tma_load_2d(sW2 + c * (COUT * BKH * 2), &tmW2, w2_full, c * BKH, 0);
@@ -401,134 +291,99 @@ __global__ void __launch_bounds__(kGemmThreads, HID <= 32 ? 3 : (HID <= 64 ? 2 :
         tma_load_2d(sa + Cfg::kABytes, &tmW1, full0 + 8 * s, k0, 0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int kc = 0; kc < nk; ++kc) {
-        const int s = kc % S;
-        const uint32_t ph = (uint32_t)(kc / S) & 1u;
-        mbar_wait(full0 + 8 * s, ph);
-        tc_fence_after();
-        const uint32_t sa = tiles + s * Cfg::kStageBytes;
-        const uint64_t da = smem_desc_sw128(sa), db = smem_desc_sw128(sa + Cfg::kABytes);
-#pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) tc_mma_bf16(tmem, da + 2 * k, db + 2 * k, instr_desc_bf16(kBM, HID), (kc | k) != 0);
-        tc_commit(empty0 + 8 * s);
-      }
-      tc_commit(acc1);
-      mbar_wait(w2_full, 0);
-      mbar_wait(h_ready, 0);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < Cfg::kNK2; ++c) {
-        const uint64_t dh = smem_desc_k<BKH>(sH + c * (kBM * BKH * 2)), dw = smem_desc_k<BKH>(sW2 + c * (COUT * BKH * 2));
-#pragma unroll
-        for (int k = 0; k < BKH / 16; ++k) tc_mma_bf16(tmem + HID, dh + 2 * k, dw + 2 * k, instr_desc_bf16(kBM, COUT), (c | k) != 0);
-      }
-      tc_commit(acc2);
-    }
-  } else {
-    const int q = warp & 3, half = (warp - 2) >> 2;
-    const int r = 32 * q + lane;  // tile row == tensor-memory lane
-    const int m = m0 + r;
-    const bool row_ok = m < op.M;
-    const uint32_t trow = tmem + ((uint32_t)(32 * q) << 16);
-    // ---- epilogue A: hidden activation -> shared memory (bf16, swizzled K-major rows of BKH elements)
-    mbar_wait(acc1, 0);
-    tc_fence_after();
-    constexpr int kColsA = HID >= 64 ? HID / 2 : HID;
-    const int abeg = HID >= 64 ? half * kColsA : half * HID;
+    return;
+  }
+  const int g = warp >> 2;
+  const int r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);  // tile rows r0 and r0 + 8
+  // ---- GEMM 1
+  {
+    float d[HID / 2];
 #pragma unroll 1
-    for (int c0 = abeg; c0 < abeg + kColsA && c0 < HID; c0 += 32) {
-      uint32_t v[32];
-      tc_ld32(trow + (uint32_t)c0, v);
-      uint32_t pk[16];
+    for (int kc = 0; kc < nk; ++kc) {
+      const int s = kc % S;
+      mbar_wait(full0 + 8 * s, (uint32_t)(kc / S) & 1u);
+      const uint32_t sa = tiles + s * Cfg::kStageBytes;
+      const uint64_t da = wg::desc_sw128(sa + (uint32_t)g * (64u * kBK * 2u)), db = wg::desc_sw128(sa + Cfg::kABytes);
+      wg::fence();
 #pragma unroll
-      for (int e = 0; e < 32; e += 4) {
-        const float4 bv = __ldg(reinterpret_cast<const float4*>(op.bias1 + c0 + e));
-        const __nv_bfloat162 h0 = __floats2bfloat162_rn(elu_fast(__uint_as_float(v[e]) + bv.x), elu_fast(__uint_as_float(v[e + 1]) + bv.y));
-        const __nv_bfloat162 h1 = __floats2bfloat162_rn(elu_fast(__uint_as_float(v[e + 2]) + bv.z), elu_fast(__uint_as_float(v[e + 3]) + bv.w));
-        pk[e >> 1] = *reinterpret_cast<const uint32_t*>(&h0);
-        pk[(e >> 1) + 1] = *reinterpret_cast<const uint32_t*>(&h1);
-      }
-      // 32 columns = 4 sixteen-byte chunks of row r inside K chunk c0 / BKH; chunk index XOR row bits (swizzle)
-      const uint32_t blk = sH + (uint32_t)(c0 / BKH) * (kBM * BKH * 2) + (uint32_t)r * (BKH * 2);
-      const int ch0 = (c0 % BKH) >> 3;
+      for (int k = 0; k < kBK / 16; ++k) wg::mma_ss<HID>(d, da + 2 * k, db + 2 * k, (kc | k) != 0);
+      wg::commit();
+      wg::wait<1>();
+      if (kc > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty0 + 8 * ((kc - 1) % S));
+    }
+    wg::wait<0>();
+    wg::fence_regs(d);
+    // ---- epilogue A: hidden activation -> shared memory (bf16, swizzled K-major rows of BKH elements)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + 8 * h;
       const int sw = BKH == 64 ? (r & 7) : ((r >> 1) & 3);
 #pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const uint32_t a = blk + (uint32_t)(((ch0 + cc) ^ sw) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(pk[4 * cc]), "r"(pk[4 * cc + 1]), "r"(pk[4 * cc + 2]),
-                     "r"(pk[4 * cc + 3])
-                     : "memory");
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(h_ready) : "memory");
-    // ---- epilogue B: + bias + skip, outputs
-    mbar_wait(acc2, 0);
-    tc_fence_after();
-    const size_t row = ((size_t)b * (size_t)op.M + (size_t)(row_ok ? m : 0)) * COUT;
-    constexpr int kColsB = COUT / 2;
-#pragma unroll 1
-    for (int c0 = half * kColsB; c0 < (half + 1) * kColsB; c0 += 32) {
-      uint32_t rr[32];
-      tc_ld32(trow + (uint32_t)(HID + c0), rr);
-      if (!row_ok) continue;
-      float v[32];
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        float zv[8];
-        ldg256(op.Z + row + c0 + i, zv);
-        const float4 b0 = __ldg(reinterpret_cast<const float4*>(op.bias2 + c0 + i));
-        const float4 b1 = __ldg(reinterpret_cast<const float4*>(op.bias2 + c0 + i + 4));
-        const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-        for (int e = 0; e < 8; ++e) v[i + e] = zv[e] + (__uint_as_float(rr[i + e]) + bb[e]);
-      }
-      if (op.out_f32) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-          uint32_t w8[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) w8[e] = __float_as_uint(v[i + e]);
-          stg256(op.out_f32 + row + c0 + i, w8);
-        }
-      }
-      if (op.out_bf16) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 16) {
-          uint32_t pk[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float a = v[i + 2 * e], c = v[i + 2 * e + 1];
-            if (op.out_elu) {
-              a = elu_fast(a);
-              c = elu_fast(c);
-            }
-            const __nv_bfloat162 hh = __floats2bfloat162_rn(a, c);
-            pk[e] = *reinterpret_cast<const uint32_t*>(&hh);
-          }
-          stg256(op.out_bf16 + row + c0 + i, pk);
-        }
+      for (int j = 0; j < HID / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(op.bias1 + c));
+        const uint32_t v = pack_bf16(elu_fast(d[4 * j + 2 * h] + bv.x), elu_fast(d[4 * j + 2 * h + 1] + bv.y));
+        const int cb = (c % BKH) * 2;  // byte offset inside the row of K chunk c / BKH
+        const uint32_t a = sH + (uint32_t)(c / BKH) * (kBM * BKH * 2) + (uint32_t)r * (BKH * 2) + (uint32_t)((((cb >> 4) ^ sw) << 4) | (cb & 15));
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)Cfg::kTmemCols) : "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> wgmma operand reads
+  wg_sync(g);
+  asm volatile("bar.sync 3, 256;" ::: "memory");  // both warpgroups are past GEMM 1: the stage ring is idle
+  mbar_wait(w2_full, 0);
+  float* et = reinterpret_cast<float*>(smem_raw + (tiles - smem_u32(smem_raw)));
+  constexpr int TPR = N2 / 4, RPP = 128 / TPR;  // threads per row, rows per pass (each warpgroup: its own 64 rows)
+  const int tg = threadIdx.x & 127, cl = 4 * (tg % TPR);
+  // ---- GEMM 2 and epilogue B, per column block
+#pragma unroll 1
+  for (int nb = 0; nb < COUT / N2; ++nb) {
+    float d[N2 / 2];
+    wg::fence();
+#pragma unroll
+    for (int c = 0; c < Cfg::kNK2; ++c) {
+      const uint64_t dh = wg::desc_k<BKH>(sH + c * (kBM * BKH * 2) + (uint32_t)g * (64u * BKH * 2u));
+      const uint64_t dw = wg::desc_k<BKH>(sW2 + c * (COUT * BKH * 2) + nb * (N2 * BKH * 2));
+#pragma unroll
+      for (int k = 0; k < BKH / 16; ++k) wg::mma_ss<N2>(d, dh + 2 * k, dw + 2 * k, (c | k) != 0);
+    }
+    wg::commit();
+    wg::wait<0>();
+    wg::fence_regs(d);
+#pragma unroll
+    for (int j = 0; j < N2 / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(et + (r0 + 8 * h) * Cfg::kEpiPitch + 8 * j + 2 * (lane & 3)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+    wg_sync(g);
+    const int c = nb * N2 + cl;
+#pragma unroll 1
+    for (int r = 64 * g + tg / TPR; r < 64 * g + 64; r += RPP) {
+      const int m = m0 + r;
+      if (m >= op.M) break;
+      const size_t row = ((size_t)b * (size_t)op.M + (size_t)m) * COUT;
+      const float4 a = *reinterpret_cast<const float4*>(et + r * Cfg::kEpiPitch + cl);
+      const float4 zv = *reinterpret_cast<const float4*>(op.Z + row + c);
+      const float4 bv = __ldg(reinterpret_cast<const float4*>(op.bias2 + c));
+      float4 v = make_float4(zv.x + (a.x + bv.x), zv.y + (a.y + bv.y), zv.z + (a.z + bv.z), zv.w + (a.w + bv.w));
+      if (op.out_f32) *reinterpret_cast<float4*>(op.out_f32 + row + c) = v;
+      if (op.out_bf16) {
+        if (op.out_elu) v = make_float4(elu_fast(v.x), elu_fast(v.y), elu_fast(v.z), elu_fast(v.w));
+        *reinterpret_cast<uint2*>(op.out_bf16 + row + c) = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+      }
+    }
+    wg_sync(g);  // the tile is read before the next column block overwrites it
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 // Causal sliding-window attention on the tensor cores (MimiAttention.forward, modeling_mimi.py:681-738,
-// head_dim 64, window <= 257).  One CTA = 128 queries of one (batch, head):
-//   S = Q K^T over the 384 keys [q0-256, q0+128) -> 384 fp32 columns of tensor memory (3 x M128 N128 K64)
-//   softmax with thread == query row (no shuffles): two passes over tensor memory, P rounded to bf16 and
-//   written 128B-swizzled into shared memory as the next A operand (over the dead Q/K tiles)
-//   O = P V with V^T [d][key] tiles as the K-major B operand -> 64 more columns; scaled by 1/sum on the way out
+// head_dim 64, window <= 257).  One CTA = 128 queries of one (batch, head), one warpgroup per 64 queries,
+// over the 384 keys [q0-256, q0+128) in three blocks of 128 (blocks outside a warpgroup's band are skipped):
+//   pass 1: S = Q K^T per block (M64 N128 K64, fp32 in registers) -> the exact row maximum over the valid keys
+//   pass 2: S again; P = exp(S - max) rounded to bf16 stays in registers as the A operand of O += P V, with
+//           V^T [d][key] tiles as the K-major B operand; the row sums add the rounded P; O / sum on the way out
 // Inputs are the rotated bf16 q / k [B][T2][C] and v transposed [B][C][T2p] written by rope_pack_kernel.
 // ---------------------------------------------------------------------------------------------
 struct AttnOp {
@@ -538,154 +393,127 @@ struct AttnOp {
 };
 
 constexpr int kAttnKeys = 384, kAttnDh = 64;
-constexpr int kAttnSmem = 65536 + 49152 + 32768 + 1024;
+constexpr int kAttnThreads = 256;
+constexpr int kAttnSmem = 16384 + 49152 + 49152 + 1024;  // Q, K (3 x 128 keys), V^T (6 x 64 keys), alignment slack
 
-static __global__ void __launch_bounds__(kThreads) attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                                                           const __grid_constant__ CUtensorMap tmVt, const AttnOp op) {
+// S block kt of warpgroup g: 64 queries x 128 keys
+__device__ __forceinline__ void attn_scores(float (&s)[64], uint32_t sQ, uint32_t sK, int g, int kt) {
+  const uint64_t dq = wg::desc_sw128(sQ + (uint32_t)g * 8192u), dk = wg::desc_sw128(sK + (uint32_t)kt * 16384u);
+  wg::fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wg::mma_ss<128>(s, dq + 2 * k, dk + 2 * k, k != 0);
+  wg::commit();
+  wg::wait<0>();
+  wg::fence_regs(s);
+}
+
+static __global__ void __launch_bounds__(kAttnThreads) attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                                                                      const __grid_constant__ CUtensorMap tmVt, const AttnOp op) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bars[5];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bars[2];
   const uint32_t tiles = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = tiles, sK = tiles + 16384, sV = tiles + 65536;
-  const uint32_t qk_full = smem_u32(&bars[0]), v_full = smem_u32(&bars[1]), s_full = smem_u32(&bars[2]),
-                 p_full = smem_u32(&bars[3]), o_full = smem_u32(&bars[4]);
+  const uint32_t qk_full = smem_u32(&bars[0]), v_full = smem_u32(&bars[1]);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
   const int kbase = q0 + 128 - kAttnKeys;
-  auto p_block = [&](int kb) -> uint32_t { return kb < 4 ? tiles + kb * 16384 : tiles + 65536 + 49152 + (kb - 4) * 16384; };
 
   if (threadIdx.x == 0) {
     mbar_init(qk_full, 1);
     mbar_init(v_full, 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_expect_tx(qk_full, 65536);
+    tma_load_3d(sQ, &tmQ, qk_full, h * kAttnDh, q0, b);
+    for (int kt = 0; kt < 3; ++kt) tma_load_3d(sK + kt * 16384, &tmK, qk_full, h * kAttnDh, kbase + kt * 128, b);
+    mbar_expect_tx(v_full, 49152);
+    for (int kb = 0; kb < 6; ++kb) tma_load_3d(sV + kb * 8192, &tmVt, v_full, kbase + kb * 64, h * kAttnDh, b);
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(qk_full, 65536);
-      tma_load_3d(sQ, &tmQ, qk_full, h * kAttnDh, q0, b);
-      for (int kt = 0; kt < 3; ++kt) tma_load_3d(sK + kt * 16384, &tmK, qk_full, h * kAttnDh, kbase + kt * 128, b);
-      mbar_expect_tx(v_full, 49152);
-      for (int kb = 0; kb < 6; ++kb) tma_load_3d(sV + kb * 8192, &tmVt, v_full, kbase + kb * 64, h * kAttnDh, b);
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      mbar_wait(qk_full, 0);
-      tc_fence_after();
-      const uint64_t dq = smem_desc_sw128(sQ);
-      for (int kt = 0; kt < 3; ++kt) {
-        const uint64_t dk = smem_desc_sw128(sK + kt * 16384);
+  const int g = warp >> 2;
+  // this thread's query rows i[0], i[1] = i[0] + 8 and their valid key columns [clo, chi] (relative to kbase)
+  int clo[2], chi[2];
+  bool row_ok[2];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc_mma_bf16(tmem + kt * 128, dq + 2 * k, dk + 2 * k, instr_desc_bf16(128, 128), k != 0);
-      }
-      tc_commit(s_full);
-      mbar_wait(p_full, 0);
-      mbar_wait(v_full, 0);
-      tc_fence_after();
-      for (int kb = 0; kb < 6; ++kb) {
-        const uint64_t dp = smem_desc_sw128(p_block(kb)), dv = smem_desc_sw128(sV + kb * 8192);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc_mma_bf16(tmem + kAttnKeys, dp + 2 * k, dv + 2 * k, instr_desc_bf16(128, 64), (kb | k) != 0);
-      }
-      tc_commit(o_full);
-    }
-  } else {
-    const int q = warp & 3;
-    const int r = 32 * q + lane;   // row of the tile == tensor-memory lane
-    const int i = q0 + r;          // query position
-    const bool row_ok = i < op.T2;
-    // valid key columns of this row / of the whole warp (slices outside the warp's band are skipped uniformly)
-    const int clo = row_ok ? max(0, i - op.window + 1) - kbase : 1, chi = row_ok ? i - kbase : 0;
-    const int i_first = q0 + 32 * q, i_last = min(i_first + 31, op.T2 - 1);
-    const int wlo = max(0, i_first - op.window + 1) - kbase, whi = i_last - kbase;  // whi < wlo when the warp has no rows
-    const uint32_t trow = tmem + ((uint32_t)(32 * q) << 16);
-    mbar_wait(s_full, 0);
-    tc_fence_after();
-    float mx = -INFINITY;
+  for (int e = 0; e < 2; ++e) {
+    const int i = q0 + 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * e;
+    row_ok[e] = i < op.T2;
+    clo[e] = row_ok[e] ? max(0, i - op.window + 1) - kbase : 1;
+    chi[e] = row_ok[e] ? i - kbase : 0;
+  }
+  // key blocks that hold a valid key of some row of the warpgroup (uniform over the warpgroup)
+  const int i_first = q0 + 64 * g, i_last = min(i_first + 63, op.T2 - 1);
+  const int wlo = max(0, i_first - op.window + 1) - kbase, whi = i_last - kbase;  // whi < wlo when the warpgroup has no rows
+  auto live = [&](int kt) { return !(128 * kt + 127 < wlo || 128 * kt > whi); };
+  auto valid = [&](int e, int col) { return col >= clo[e] && col <= chi[e]; };
+
+  mbar_wait(qk_full, 0);
+  float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll 1
-    for (int c0 = 0; c0 < kAttnKeys; c0 += 32) {
-      if (c0 + 31 < wlo || c0 > whi) continue;
-      uint32_t v[32];
-      tc_ld32(trow + c0, v);
+  for (int kt = 0; kt < 3; ++kt) {
+    if (!live(kt)) continue;
+    float s[64];
+    attn_scores(s, sQ, sK, g, kt);
 #pragma unroll
-      for (int e = 0; e < 32; ++e)
-        if (c0 + e >= clo && c0 + e <= chi) mx = fmaxf(mx, __uint_as_float(v[e]));
-    }
-    float sum = 0.f;
-    const float mxs = mx * op.scale_log2e;
-#pragma unroll 1
-    for (int c0 = 0; c0 < kAttnKeys; c0 += 32) {
-      const bool live = !(c0 + 31 < wlo || c0 > whi);
-      uint32_t pk[16];
-      if (live) {
-        uint32_t v[32];
-        tc_ld32(trow + c0, v);
-#pragma unroll
-        for (int e = 0; e < 32; e += 2) {
-          float p0 = 0.f, p1 = 0.f;
-          if (c0 + e >= clo && c0 + e <= chi) p0 = exp2f(fmaf(__uint_as_float(v[e]), op.scale_log2e, -mxs));
-          if (c0 + e + 1 >= clo && c0 + e + 1 <= chi) p1 = exp2f(fmaf(__uint_as_float(v[e + 1]), op.scale_log2e, -mxs));
-          const __nv_bfloat162 hh = __floats2bfloat162_rn(p0, p1);
-          sum += __low2float(hh) + __high2float(hh);
-          pk[e >> 1] = *reinterpret_cast<const uint32_t*>(&hh);
-        }
-      } else {
-#pragma unroll
-        for (int e = 0; e < 16; ++e) pk[e] = 0u;
-      }
-      // 32 keys = 4 sixteen-byte chunks of row r in P block c0/64, chunk index XOR (r & 7)
-      const uint32_t rowaddr = p_block(c0 >> 6) + r * 128;
-      const int ch0 = (c0 & 63) >> 3;
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const uint32_t a = rowaddr + (uint32_t)(((ch0 + cc) ^ (r & 7)) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(pk[4 * cc]), "r"(pk[4 * cc + 1]), "r"(pk[4 * cc + 2]),
-                     "r"(pk[4 * cc + 3])
-                     : "memory");
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(p_full) : "memory");
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    const float inv = row_ok ? 1.0f / sum : 0.f;
-    __nv_bfloat16* orow = op.out + ((size_t)b * op.T2 + (row_ok ? i : 0)) * op.C + h * kAttnDh;
-#pragma unroll 1
-    for (int c0 = 0; c0 < kAttnDh; c0 += 32) {
-      uint32_t v[32];
-      tc_ld32(trow + kAttnKeys + c0, v);
-      if (!row_ok) continue;
-#pragma unroll
-      for (int e = 0; e < 32; e += 8) {
-        uint32_t w4[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const __nv_bfloat162 hh = __floats2bfloat162_rn(__uint_as_float(v[e + 2 * u]) * inv, __uint_as_float(v[e + 2 * u + 1]) * inv);
-          w4[u] = *reinterpret_cast<const uint32_t*>(&hh);
-        }
-        *reinterpret_cast<uint4*>(orow + c0 + e) = make_uint4(w4[0], w4[1], w4[2], w4[3]);
-      }
+    for (int i = 0; i < 64; ++i) {
+      const int e = (i >> 1) & 1, col = 128 * kt + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      if (valid(e, col)) mx[e] = fmaxf(mx[e], s[i]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {  // the four lanes of a row hold its columns
+    mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 1));
+    mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 2));
+  }
+  const float mxs[2] = {mx[0] * op.scale_log2e, mx[1] * op.scale_log2e};
+  mbar_wait(v_full, 0);
+  float o[32];
+  float sum[2] = {0.f, 0.f};
+  uint32_t acc = 0;
+#pragma unroll 1
+  for (int kt = 0; kt < 3; ++kt) {
+    if (!live(kt)) continue;
+    float s[64];
+    attn_scores(s, sQ, sK, g, kt);
+    uint32_t p[32];
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int e = (i >> 1) & 1, col = 128 * kt + 8 * (i >> 2) + 2 * (lane & 3);
+      const float p0 = valid(e, col) ? exp2f(fmaf(s[i], op.scale_log2e, -mxs[e])) : 0.f;
+      const float p1 = valid(e, col + 1) ? exp2f(fmaf(s[i + 1], op.scale_log2e, -mxs[e])) : 0.f;
+      const __nv_bfloat162 hh = __floats2bfloat162_rn(p0, p1);
+      sum[e] += __low2float(hh) + __high2float(hh);
+      p[i >> 1] = *reinterpret_cast<const uint32_t*>(&hh);
+    }
+    // the accumulator layout of columns 16j .. 16j + 15 is the register A-operand layout of a K = 16 slice
+    wg::fence();
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t a[4] = {p[4 * j], p[4 * j + 1], p[4 * j + 2], p[4 * j + 3]};
+      wg::mma_rs<64>(o, a, wg::desc_sw128(sV + (uint32_t)(2 * kt + (j >> 2)) * 8192u) + 2 * (j & 3), acc | (uint32_t)j);
+    }
+    wg::commit();
+    wg::wait<0>();
+    wg::fence_regs(o);
+    acc = 1;
+  }
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 1);
+    sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 2);
+  }
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    if (!row_ok[e]) continue;
+    const int i = q0 + 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * e;
+    const float inv = 1.0f / sum[e];
+    __nv_bfloat16* orow = op.out + ((size_t)b * op.T2 + i) * op.C + h * kAttnDh;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<uint32_t*>(orow + 8 * j + 2 * (lane & 3)) = pack_bf16(o[4 * j + 2 * e] * inv, o[4 * j + 2 * e + 1] * inv);
   }
 }
+
 
 // ---------------------------------------------------------------------------------------------
 // host side: tensor maps through the driver entry point (no link-time dependency on libcuda)
@@ -768,7 +596,7 @@ inline cudaError_t launch_attn(const void* q, const void* k, const void* vt, __n
     return cudaErrorInvalidValue;
   AttnOp op{out, T2, C, window, 1.4426950408889634f / sqrtf((float)kAttnDh)};
   dim3 grid((unsigned)((T2 + 127) / 128), (unsigned)H, (unsigned)B);
-  attn_tc_kernel<<<grid, kThreads, kAttnSmem, st>>>(tmQ, tmK, tmV, op);
+  attn_tc_kernel<<<grid, kAttnThreads, kAttnSmem, st>>>(tmQ, tmK, tmV, op);
   return cudaGetLastError();
 }
 

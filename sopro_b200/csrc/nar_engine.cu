@@ -15,7 +15,7 @@
 
 #include "../../include/sopro_b200.h"
 #include "dense_f32.cuh"
-#include "mimi_tc.cuh"  // tc::launch: the tcgen05 / TMEM / TMA implicit-GEMM kernel, reused for the exact split products
+#include "mimi_tc.cuh"  // tc::launch: the wgmma / TMA implicit-GEMM kernel, reused for the exact split products
 
 namespace mimi {
 void set_error(const char* msg);  // ar_engine.cu: the string behind sopro_last_error()
@@ -130,7 +130,7 @@ int argmax_parts(int M, int N, int groups) {
 // of three bf16 terms (h + m + l: 3 x 8 mantissa bits), a product of two bf16 numbers is exact in fp32, so
 //   x . w = sum over the six term pairs whose magnitude reaches fp32's last bit (mm, lh, hl, mh, hm, hh; the pairs ml, lm,
 //   ll are below 2^-26 of the product)
-// accumulated in fp32 in tensor memory: the same quantity the fp32 FMA kernels compute, up to the order of the fp32
+// accumulated in fp32 by the tensor cores: the same quantity the fp32 FMA kernels compute, up to the order of the fp32
 // additions.  One GEMM launch does all six: the weights are stored as W6 [N][6K] (K blocks = the w term of each pair,
 // built once on the host), the activations as A3 [M][3K] = [h | m | l] written by split3_rows_kernel (fused with the
 // RMSNorm of the rows), and the GEMM kernel's "tap" j (mimi_tc.cuh: K block j of W against A columns tap_col[j] + ...)
@@ -439,7 +439,7 @@ int sopro_nar_create(const sopro_nar_config_t* cfg, const sopro_nar_weights_t* w
   if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
   PCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int D = cfg->d_model, NL = cfg->n_layers, k = cfg->kernel, Q = cfg->n_codebooks, V = cfg->codebook_size, Hn = cfg->head_dim,
             AH = cfg->adapter_hidden, NS = cfg->n_stages;
   if (D < 32 || D > 512 || D % 16 || Hn % 16 || NL < 1 || NL > SOPRO_MAX_SSM_LAYERS || k < 1 || k > 64 || Q < 2 || Q > SOPRO_NAR_MAX_CODEBOOKS ||
@@ -945,7 +945,7 @@ int sopro_prefill_create(const sopro_prefill_config_t* cfg, const sopro_prefill_
   if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
   PCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int D = cfg->d_model, NL = cfg->n_layers_text, k = cfg->text_kernel, SV = cfg->sv_dim, RL = cfg->ref_layers, H = cfg->ref_heads;
   if (D < 32 || D > 512 || D % 16 || NL < 0 || NL > SOPRO_MAX_SSM_LAYERS || k < 1 || k > 64 || SV < 16 || SV % 16 || RL < 0 ||
       RL > SOPRO_PREFILL_MAX_REF_LAYERS || H < 1 || D % H || (D / H) % 4 || cfg->text_vocab < 1 || cfg->max_text_len < 1 || cfg->max_frames_pos < 1)
@@ -1231,7 +1231,7 @@ int sopro_refprep_create(const sopro_refprep_config_t* cfg, const sopro_refprep_
   if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
   PCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int D = cfg->d_model, d = cfg->sv_embed_dim, SV = cfg->sv_dim, Q = cfg->n_codebooks, V = cfg->codebook_size, NL = cfg->ref_enc_layers,
             RL = cfg->ref_layers, H = cfg->ref_heads;
   if (D < 32 || D > 512 || D % 16 || d < 16 || d % 16 || SV < 16 || SV % 16 || Q < 1 || Q > 64 || V < 1 || NL < 0 || NL > SOPRO_MAX_SSM_LAYERS ||

@@ -142,7 +142,7 @@ class ArSession:
         _lib.check(self.lib.sopro_ar_session_set_team(self._h, int(utts_per_team)))
 
     def set_contraction(self, mode: int) -> None:
-        """-1 / 0: packed-fp32 FMA tiles (default; -1 honours SOPRO_AR_TC=1); 1: tensor cores (tcgen05, exact three-way
+        """-1 / 0: packed-fp32 FMA tiles (default; -1 honours SOPRO_AR_TC=1); 1: tensor cores (wgmma, exact three-way
         bf16 split of the activations against bf16 weights) -- exact but slower at this kernel's tile sizes."""
         _lib.check(self.lib.sopro_ar_session_set_contraction(self._h, int(mode)))
 

@@ -1,4 +1,4 @@
-"""Public API: ``SoproTTS`` with the reference's signatures (reference model.py:404-583) over the B200 engine.
+"""Public API: ``SoproTTS`` with the reference's signatures (reference model.py:404-583) over the H100 engine.
 
 ``SoproTTS.model`` is a ``SoproModel``: it stands where the reference's ``SoproTTSModel`` stands
 (model.py:53-401) and keeps its method names, but ``ar_stream`` drives the persistent CUDA kernel and the
@@ -193,7 +193,7 @@ class SoproModel:
     def __init__(self, cfg: SoproTTSConfig, state_dict: Dict[str, torch.Tensor], device, weight_dtype: str = "fp32"):
         dev = torch.device(device)
         if dev.type != "cuda":
-            raise RuntimeError("sopro_b200 runs on CUDA devices only (sm_100a); there is no CPU fallback")
+            raise RuntimeError("sopro_b200 runs on CUDA devices only (sm_90a); there is no CPU fallback")
         self.cfg = cfg
         state_dict = _complete_state_dict(cfg, state_dict)
         self.device = torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())

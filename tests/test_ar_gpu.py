@@ -109,7 +109,7 @@ def test_teacher_forced_logits_and_blocks(name):
 @pytest.mark.parametrize("mode", [1, 0])
 def test_batched_bf16_reference_case_on_both_contraction_units(mode):
     """The reference fixture default_bf16 replicated over a team of 8 utterances, through the tensor-core contraction
-    (mode 1: tcgen05, every fp32 activation split into three exact bf16 terms) and through the packed-fp32 FMA path
+    (mode 1: tensor cores, every fp32 activation split into three exact bf16 terms) and through the packed-fp32 FMA path
     (mode 0) of the same launch geometry: teacher-forced logits and per-block residuals within the fixture tolerances
     (3e-5 / 2e-5 of the peak, fp32 accumulation-order noise), and every sampled token is the reference's."""
     spec, cfg, sd, inp, g, eng, steps, tape = _case("default_bf16")

@@ -1,4 +1,4 @@
-"""bench.py's CPU arm (`--impl reference`) prints ONE JSON line with the contract's keys; the B200 arm refuses to run without a
+"""bench.py's CPU arm (`--impl reference`) prints ONE JSON line with the contract's keys; the GPU arm refuses to run without a
 device instead of falling back."""
 import json
 import os

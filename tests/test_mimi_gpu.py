@@ -35,7 +35,7 @@ def test_decode_matches_oracle(B, T):
 
 @pytest.mark.parametrize("B,T", [(1, 1), (2, 9), (1, 37), (3, 16), (1, 150), (2, 203)])
 def test_decode_tensor_core_mode(B, T):
-    """Default mode: bf16 operands on the tcgen05 tensor cores, fp32 accumulation.  Stated tolerance: max error
+    """Default mode: bf16 operands on the tensor cores, fp32 accumulation.  Stated tolerance: max error
     2e-2 of the waveform's peak and relative RMS error 1e-2 against the fp32 oracle."""
     eng, sd = _engine("bf16_tc")
     codes = torch.randint(0, 2048, (B, 32, T), generator=torch.Generator().manual_seed(100 + T))
@@ -119,7 +119,7 @@ TC_GEMM_CASES = [
 
 @pytest.mark.parametrize("case", TC_GEMM_CASES, ids=lambda c: "x".join(map(str, c)))
 def test_tc_gemm_matches_torch(case):
-    """The tcgen05 implicit GEMM alone against torch fp32 on the same bf16-rounded operands (differences are
+    """The tensor-core implicit GEMM alone against torch fp32 on the same bf16-rounded operands (differences are
     accumulation order only): 1e-3 of the output scale for fp32 results, one bf16 ulp (2^-8 relative) for bf16."""
     import ctypes as C
 
@@ -173,7 +173,7 @@ def test_host_buffer_path_and_stream_decoder(precision):
     assert got.shape == (1, 20 * 1920) and state.frames_seen == 20
     if precision == "fp32":  # the persistent-state stream decoder computes every sample in the one-shot decode's order
         np.testing.assert_array_equal(got[0], full[0, 0])
-    else:  # tensor-core mode: same tcgen05 tiles, the attention core runs in fp32 over the K/V ring (tolerance 1e-2 of peak)
+    else:  # tensor-core mode: same tensor-core tiles, the attention core runs in fp32 over the K/V ring (tolerance 1e-2 of peak)
         np.testing.assert_allclose(got[0], full[0, 0], rtol=0, atol=1e-2 * float(np.abs(full).max()))
 
 
@@ -208,7 +208,7 @@ def test_stream_decode_step_equals_the_full_decode(mode):
     the default 6, 16, a 40-frame chunk that is split internally, ...) over 310 frames -- 620 transformer positions,
     far past the 250-position window and past the ring's wrap-around -- concatenate to the one-shot decode.  fp32
     mode: bit for bit (every output element is computed in the same order).  Tensor-core mode: the dense blocks are the
-    same tcgen05 tiles, only the attention core runs in fp32 on the ring; the stated tolerance is 1e-2 of the peak vs the
+    same tensor-core tiles, only the attention core runs in fp32 on the ring; the stated tolerance is 1e-2 of the peak vs the
     one-shot tensor-core decode and the mode's 2e-2 vs the fp32 oracle."""
     eng, sd = _engine(mode)
     T = 310

@@ -130,7 +130,7 @@ def test_nar_strided_conditioning_rows():
 
 
 def test_tensor_core_path_equals_the_fp32_path():
-    """Above 16 rows the contractions run on tcgen05 with every fp32 operand split into three exact bf16 terms (six
+    """Above 16 rows the contractions run on the tensor cores with every fp32 operand split into three exact bf16 terms (six
     products, fp32 accumulation: the fp32 result up to summation order).  Same ids as the fp32 FMA kernels and as the CPU
     oracle on 4 x 300 frames; a differing id must be an oracle near-tie (the _check rule)."""
     eng = _engine()

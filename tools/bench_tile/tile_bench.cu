@@ -1,5 +1,5 @@
 // Micro-benchmark of the AR kernel's warp GEMV tiles in isolation (one CTA per SM, 512 threads, operands in shared
-// memory, clock64 around the task loop).  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tile_bench tile_bench.cu
+// memory, clock64 around the task loop).  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tile_bench tile_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -54,7 +54,7 @@ __device__ __forceinline__ float warp_rows_p(const unsigned (&w)[R], unsigned ac
 #pragma unroll
     for (int u = 0; u < TU; ++u)
 #pragma unroll
-      for (int r = 0; r < R; ++r) acc[r][u] = __ffma2_rn(wc[r], xc[u], acc[r][u]);
+      for (int r = 0; r < R; ++r) acc[r][u] = ffma2(wc[r], xc[u], acc[r][u]);
   }
   float v[R * TU];
 #pragma unroll
@@ -85,10 +85,10 @@ __device__ __forceinline__ float warp_rows_rp(unsigned wt, unsigned xt, int K, i
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       const float2 xx = make_float2(xs[u], xs[u]);
-      acc[0][u] = __ffma2_rn(w0, xx, acc[0][u]);
-      acc[1][u] = __ffma2_rn(w1, xx, acc[1][u]);
-      acc[2][u] = __ffma2_rn(w2, xx, acc[2][u]);
-      acc[3][u] = __ffma2_rn(w3, xx, acc[3][u]);
+      acc[0][u] = ffma2(w0, xx, acc[0][u]);
+      acc[1][u] = ffma2(w1, xx, acc[1][u]);
+      acc[2][u] = ffma2(w2, xx, acc[2][u]);
+      acc[3][u] = ffma2(w3, xx, acc[3][u]);
     }
   }
   float v[64];
@@ -161,8 +161,8 @@ __global__ void __launch_bounds__(512, 1) bench(int K, int n_tasks, int rows, fl
         for (int k = lane * 4; k < K; k += 128) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) {
-            acc[i] = __ffma2_rn(a, b, acc[i]);
-            acc[i] = __ffma2_rn(b, a, acc[i]);
+            acc[i] = ffma2(a, b, acc[i]);
+            acc[i] = ffma2(b, a, acc[i]);
           }
         }
         float s = 0.f;
@@ -196,18 +196,21 @@ __global__ void __launch_bounds__(512, 1) bench(int K, int n_tasks, int rows, fl
 
 template <int MODE>
 static void run(const char* name, int K, int n_tasks, int rows, int macs_per_task) {
+  int dev = 0, n_sm = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   float* out;
   long long* cyc;
-  cudaMalloc(&out, 148 * 512 * 4);
-  cudaMalloc(&cyc, 148 * 8);
+  cudaMalloc(&out, (size_t)n_sm * 512 * 4);
+  cudaMalloc(&cyc, (size_t)n_sm * 8);
   const int reps = 20;
   const size_t smem = (size_t)8 * K * 4 + (size_t)rows * K * 2 + 1024;
   cudaFuncSetAttribute(bench<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  bench<MODE><<<148, 512, smem>>>(K, n_tasks, rows, out, cyc, reps);
+  bench<MODE><<<n_sm, 512, smem>>>(K, n_tasks, rows, out, cyc, reps);
   cudaError_t e = cudaDeviceSynchronize();
   if (e != cudaSuccess) { printf("%s: %s\n", name, cudaGetErrorString(e)); return; }
-  std::vector<long long> h(148);
-  cudaMemcpy(h.data(), cyc, 148 * 8, cudaMemcpyDeviceToHost);
+  std::vector<long long> h(n_sm);
+  cudaMemcpy(h.data(), cyc, (size_t)n_sm * 8, cudaMemcpyDeviceToHost);
   long long best = h[0];
   for (auto v : h) best = v < best ? v : best;
   const double per = (double)best / reps;

@@ -1,4 +1,4 @@
-"""First-contact check of the tensor-core contraction path: the same bf16 batch through the FMA path and the tcgen05
+"""First-contact check of the tensor-core contraction path: the same bf16 batch through the FMA path and the tensor-core
 path, teacher-forced, per-block residual and logit differences per step."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,5 +1,5 @@
 import os, sys, time
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from tests.cases import AR_CASES, ar_case_inputs, _unit
 from sopro_b200.engine import ArEngine, Sampling

@@ -1,13 +1,13 @@
 """Per-kernel SASS opcode counts of the built library (cuobjdump -sass): the mnemonics that prove which hardware paths a
-kernel uses (UTCHMMA = tcgen05.mma, LDTM/STTM = tensor-memory access, UTMALDG/UTMASTG = TMA tensor copies, UBLKCP = 1-D TMA
-bulk copy, SYNCS = mbarrier, FFMA2 = packed fp32 FMA, LDGSTS = cp.async).  Usage: python tools/sass_opcodes.py > profiles/rXX_sass_opcodes.md"""
+kernel uses (HGMMA = wgmma, UTMALDG/UTMASTG = TMA tensor copies, UBLKCP = 1-D TMA bulk copy, SYNCS = mbarrier,
+LDGSTS = cp.async).  Usage: python tools/sass_opcodes.py > sass_opcodes.md"""
 import collections, os, re, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 so = os.path.join(ROOT, "sopro_b200", "lib", "libsopro_b200.so")
 out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
 demangle = lambda n: subprocess.run(["c++filt", n], capture_output=True, text=True).stdout.strip()
-WATCH = ["UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "SYNCS", "FFMA2", "FFMA", "LDGSTS", "LDS", "STS",
+WATCH = ["HGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "FFMA", "LDGSTS", "LDS", "STS",
          "SHFL", "HMMA", "BAR", "ATOMS", "RED", "MUFU"]
 cur, counts, size = None, collections.OrderedDict(), {}
 for line in out.splitlines():
@@ -21,7 +21,7 @@ for line in out.splitlines():
     if m and cur:
         counts[cur][m.group(1).split(".")[0]] += 1
         size[cur] += 1
-print("# SASS opcode counts per kernel (sm_100a, `cuobjdump -sass sopro_b200/lib/libsopro_b200.so`)\n")
+print("# SASS opcode counts per kernel (sm_90a, `cuobjdump -sass sopro_b200/lib/libsopro_b200.so`)\n")
 print("| kernel | instr | " + " | ".join(WATCH) + " |")
 print("|---|---|" + "---|" * len(WATCH))
 for k, c in counts.items():

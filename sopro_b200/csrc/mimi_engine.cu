@@ -13,9 +13,13 @@
 // channel-last upsampled tensor), with ELU fused on the operand load and bias / GELU / LayerScale
 // residual fused in the epilogue.  This first version runs the contractions in fp32 on the FMA
 // pipe (parity 1e-4 against the fp32 oracle).  SOPRO_MIMI_BF16_TC mode (mimi_tc.cuh) runs every
-// contraction whose channel count allows it on the tensor cores (wgmma) with bf16 operands, fp32
+// contraction after the RVQ projection on the tensor cores (wgmma) with bf16 operands, fp32
 // accumulation in registers and the same fused epilogues; the fp32 kernels stay for the exact mode
-// and for the few narrow layers (Cin < 64).
+// and for the small RVQ projection.
+//
+// The one-shot decode, the streaming step and the encoder's transformer share one host-side layer
+// sequence (run_layers, seanet_f32 / seanet_tc); they differ only in data: the batch, the rows of left
+// context in front of each conv operand and a stream's K/V rings.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
@@ -26,6 +30,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/sopro_b200.h"
@@ -526,6 +531,35 @@ struct sopro_mimi {
   cudaStream_t cap_stream = nullptr;
 };
 
+namespace {
+// one transformer layer's weights: fp32 into A (q, k and v concatenated into one [3C][C] matrix) and, when Hh is given,
+// bf16 copies of its four GEMM matrices into Hh
+sopro_mimi::Layer pack_layer(const sopro_mimi_layer_weights_t& L, int C, int FF, DevArena& A, Bf16Arena* Hh) {
+  sopro_mimi::Layer d{};
+  d.ln1w = A.add(L.ln1_w, C);
+  d.ln1b = A.add(L.ln1_b, C);
+  std::vector<float> qkv((size_t)3 * C * C);
+  memcpy(qkv.data(), L.q_w, (size_t)C * C * 4);
+  memcpy(qkv.data() + (size_t)C * C, L.k_w, (size_t)C * C * 4);
+  memcpy(qkv.data() + (size_t)2 * C * C, L.v_w, (size_t)C * C * 4);
+  d.qkv = A.add(qkv.data(), qkv.size());
+  d.wo = A.add(L.o_w, (size_t)C * C);
+  d.ls1 = A.add(L.ls1, C);
+  d.ln2w = A.add(L.ln2_w, C);
+  d.ln2b = A.add(L.ln2_b, C);
+  d.fc1 = A.add(L.fc1_w, (size_t)FF * C);
+  d.fc2 = A.add(L.fc2_w, (size_t)C * FF);
+  d.ls2 = A.add(L.ls2, C);
+  if (Hh) {
+    d.qkv_h = Hh->add(qkv.data(), qkv.size());
+    d.wo_h = Hh->add(L.o_w, (size_t)C * C);
+    d.fc1_h = Hh->add(L.fc1_w, (size_t)FF * C);
+    d.fc2_h = Hh->add(L.fc2_w, (size_t)C * FF);
+  }
+  return d;
+}
+}  // namespace
+
 extern "C" {
 
 int sopro_mimi_create(const sopro_mimi_config_t* cfg, const sopro_mimi_weights_t* w, int device, sopro_mimi_t** out) {
@@ -559,29 +593,7 @@ int sopro_mimi_create(const sopro_mimi_config_t* cfg, const sopro_mimi_weights_t
     m->rvq_w = A.add(cat.data(), cat.size());
   }
   m->up_w = A.add(w->upsample_w, (size_t)C * 4);
-  for (int l = 0; l < NL; ++l) {
-    const sopro_mimi_layer_weights_t& L = w->layer[l];
-    sopro_mimi::Layer d;
-    d.ln1w = A.add(L.ln1_w, C);
-    d.ln1b = A.add(L.ln1_b, C);
-    std::vector<float> qkv((size_t)3 * C * C);
-    memcpy(qkv.data(), L.q_w, (size_t)C * C * 4);
-    memcpy(qkv.data() + (size_t)C * C, L.k_w, (size_t)C * C * 4);
-    memcpy(qkv.data() + (size_t)2 * C * C, L.v_w, (size_t)C * C * 4);
-    d.qkv = A.add(qkv.data(), qkv.size());
-    d.qkv_h = Hh.add(qkv.data(), qkv.size());
-    d.wo = A.add(L.o_w, (size_t)C * C);
-    d.wo_h = Hh.add(L.o_w, (size_t)C * C);
-    d.fc1_h = Hh.add(L.fc1_w, (size_t)FF * C);
-    d.fc2_h = Hh.add(L.fc2_w, (size_t)C * FF);
-    d.ls1 = A.add(L.ls1, C);
-    d.ln2w = A.add(L.ln2_w, C);
-    d.ln2b = A.add(L.ln2_b, C);
-    d.fc1 = A.add(L.fc1_w, (size_t)FF * C);
-    d.fc2 = A.add(L.fc2_w, (size_t)C * FF);
-    d.ls2 = A.add(L.ls2, C);
-    m->layers.push_back(d);
-  }
+  for (int l = 0; l < NL; ++l) m->layers.push_back(pack_layer(w->layer[l], C, FF, A, &Hh));
   // conv weights [Cout][Cin][k] -> [Cout][(tap, ci)]
   auto repack_conv = [&](const float* src, int cout, int cin, int k, size_t* half_off) {
     std::vector<float> r((size_t)cout * k * cin);
@@ -669,19 +681,6 @@ int64_t sopro_mimi_samples_per_frame(const sopro_mimi_t* m) {
   return s;
 }
 
-static int launch_gemm(const GemmOp& op, int B, cudaStream_t st) {
-  if (op.K % 16 || op.Cin % 4) return mfail(SOPRO_ERR_INVALID, "igemm: K=%d Cin=%d not aligned", op.K, op.Cin);
-  if (op.N % 64 == 0 || op.N > 32) {
-    dim3 grid((op.M + 63) / 64, (op.N + 63) / 64, B);
-    igemm_kernel<64><<<grid, 256, 0, st>>>(op);
-  } else {
-    dim3 grid((op.M + 63) / 64, (op.N + 31) / 32, B);
-    igemm_kernel<32><<<grid, 256, 0, st>>>(op);
-  }
-  MCK(cudaGetLastError());
-  return SOPRO_OK;
-}
-
 int sopro_mimi_set_precision(sopro_mimi_t* m, int precision) {
   if (!m) return mfail(SOPRO_ERR_INVALID, "null argument");
   if (precision != SOPRO_MIMI_FP32 && precision != SOPRO_MIMI_BF16_TC) return mfail(SOPRO_ERR_INVALID, "unknown precision %d", precision);
@@ -699,30 +698,34 @@ void drop_replays(sopro_mimi* m) {
   m->replays.clear();
 }
 
-// Allocations and table uploads a decode of [B, T] needs; never called inside a stream capture.
-// RoPE table [cos rows 0..T2) | sin rows 0..T2)] covering at least T2 positions
-int ensure_rope(sopro_mimi* m, int T2, cudaStream_t st) {
-  const sopro_mimi_config_t& c = m->cfg;
+// RoPE table [cos rows 0..n) | sin rows 0..n)] of n positions, replacing *tab (n rows recorded in *tab_n); uploads and
+// synchronises, so never inside a stream capture
+int make_rope(const sopro_mimi_config_t& c, int n, float** tab, int* tab_n, cudaStream_t st) {
   const int Dh = c.hidden / c.n_heads;
-  if (m->rope_T2 < T2) {
-    drop_replays(m);
-    cudaFree(m->rope);
-    m->rope = nullptr;
-    m->rope_T2 = 0;
-    std::vector<float> tab((size_t)2 * T2 * (Dh / 2));
-    for (int t = 0; t < T2; ++t)
-      for (int d = 0; d < Dh / 2; ++d) {
-        const float inv = 1.0f / powf(c.rope_theta, (float)(2 * d) / (float)Dh);
-        const float f = (float)t * inv;
-        tab[(size_t)t * (Dh / 2) + d] = cosf(f);
-        tab[(size_t)(T2 + t) * (Dh / 2) + d] = sinf(f);
-      }
-    MCK(cudaMalloc(&m->rope, tab.size() * 4));
-    MCK(cudaMemcpyAsync(m->rope, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
-    MCK(cudaStreamSynchronize(st));
-    m->rope_T2 = T2;
-  }
+  cudaFree(*tab);
+  *tab = nullptr;
+  *tab_n = 0;
+  std::vector<float> h((size_t)2 * n * (Dh / 2));
+  for (int t = 0; t < n; ++t)
+    for (int d = 0; d < Dh / 2; ++d) {
+      const float inv = 1.0f / powf(c.rope_theta, (float)(2 * d) / (float)Dh);
+      const float f = (float)t * inv;
+      h[(size_t)t * (Dh / 2) + d] = cosf(f);
+      h[(size_t)(n + t) * (Dh / 2) + d] = sinf(f);
+    }
+  MCK(cudaMalloc(tab, h.size() * 4));
+  MCK(cudaMemcpyAsync(*tab, h.data(), h.size() * 4, cudaMemcpyHostToDevice, st));
+  MCK(cudaStreamSynchronize(st));
+  *tab_n = n;
   return SOPRO_OK;
+}
+
+// Allocations and table uploads a decode of [B, T] needs; never called inside a stream capture.
+// RoPE table covering at least T2 positions
+int ensure_rope(sopro_mimi* m, int T2, cudaStream_t st) {
+  if (m->rope_T2 >= T2) return SOPRO_OK;
+  drop_replays(m);
+  return make_rope(m->cfg, T2, &m->rope, &m->rope_T2, st);
 }
 
 int mimi_prepare(sopro_mimi* m, int B, int T, cudaStream_t st) {
@@ -752,7 +755,338 @@ int mimi_prepare(sopro_mimi* m, int B, int T, cudaStream_t st) {
   return SOPRO_OK;
 }
 
-int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, cudaStream_t st);
+// Tensor-core mode runs every contraction after the RVQ projection on the wgmma tiles; a geometry they cannot take
+// (none of Mimi's layers) is refused before the first launch.  The fp32 mode takes any geometry.
+int check_tc_geometry(const sopro_mimi* m) {
+  const sopro_mimi_config_t& c = m->cfg;
+  const int C = c.hidden, FF = c.ffn;
+  bool ok = tc::supported(3 * C, C, C) && tc::supported(C, C, C) && tc::supported(FF, C, C) && tc::supported(C, FF, FF) &&
+            tc::supported(c.num_filters << c.n_ratios, c.kernel * C, C) && c.num_filters % 8 == 0 && c.last_kernel <= 8;
+  for (const sopro_mimi::Stage& S : m->stages) {
+    const int hid = S.cout / c.compress;
+    ok = ok && tc::supported(S.ratio * S.cout, 2 * S.cin, S.cin) && tc::supported(hid, c.res_kernel * S.cout, S.cout) &&
+         tc::supported(S.cout, hid, hid);
+  }
+  return ok ? (int)SOPRO_OK : mfail(SOPRO_ERR_UNSUPPORTED, "tensor-core mode: unsupported Mimi geometry (use SOPRO_MIMI_FP32)");
+}
+
+// ---- the layer sequence shared by the one-shot decode, the streaming step and the encoder.  These routines only
+//      enqueue kernels (no allocation, upload or synchronisation): the one-shot decode runs them under graph capture.
+
+int launch_gemm(const GemmOp& op, int B, cudaStream_t st) {
+  if (op.K % 16 || op.Cin % 4) return mfail(SOPRO_ERR_INVALID, "igemm: K=%d Cin=%d not aligned", op.K, op.Cin);
+  if (op.N % 64 == 0 || op.N > 32) {
+    dim3 grid((op.M + 63) / 64, (op.N + 63) / 64, B);
+    igemm_kernel<64><<<grid, 256, 0, st>>>(op);
+  } else {
+    dim3 grid((op.M + 63) / 64, (op.N + 31) / 32, B);
+    igemm_kernel<32><<<grid, 256, 0, st>>>(op);
+  }
+  MCK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+// A channel-last GEMM operand: B items of [ctx + M] rows each.  The first ctx rows of an item are left context (the
+// rows a stream carried over from its previous chunk); with ctx = 0 the causal zero padding stands in for them.
+struct Operand {
+  const void* p;  // first context row of item 0
+  long long M;
+  int ctx, B;
+};
+
+// fp32 implicit GEMM (a causal conv of `taps` taps; a Linear with taps = 1) over an operand of cin channels:
+// pad = taps - 1 - ctx zero rows, Min = M + ctx readable rows.  elu: ELU on the operand load.
+int gemm_f32(const Operand& a, int cin, int taps, const float* W, const float* bias, int N, int bias_mod, int epi, const float* R,
+             const float* scale, float* out, int elu, cudaStream_t st) {
+  GemmOp g{};
+  g.A = static_cast<const float*>(a.p); g.W = W; g.C = out; g.R = R; g.bias = bias; g.scale = scale;
+  g.M = (int)a.M; g.N = N; g.K = taps * cin; g.Min = (int)(a.M + a.ctx); g.Cin = cin; g.taps = taps; g.dil = 1; g.pad = taps - 1 - a.ctx;
+  g.ldc = N; g.bias_mod = bias_mod; g.epi = epi; g.a_elu = elu;
+  g.a_bs = (a.M + a.ctx) * cin; g.c_bs = a.M * N; g.r_bs = a.M * N;
+  return launch_gemm(g, a.B, st);
+}
+
+// tensor-core implicit GEMM over a bf16 operand (ELU already applied by its producer where the layer wants it), same
+// operand geometry; fp32 and / or bf16 output, the bf16 copy through ELU when out_elu
+int gemm_tc(const Operand& a, int cin, int taps, const __nv_bfloat16* W, const float* bias, int N, int bias_mod, int epi, const float* R,
+            const float* scale, float* of, __nv_bfloat16* oh, int out_elu, cudaStream_t st) {
+  tc::TcOp o{};
+  o.bias = bias; o.R = R; o.scale = scale; o.out_f32 = of; o.out_bf16 = oh;
+  o.c_bs = a.M * N; o.M = (int)a.M; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = 1; o.pad = taps - 1 - a.ctx;
+  o.bias_mod = bias_mod; o.epi = epi; o.out_elu = out_elu;
+  cudaError_t e = tc::launch(a.p, a.M + a.ctx, W, o, a.B, st);
+  if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core GEMM (N=%d K=%d): %s", N, o.K, cudaGetErrorString(e));
+  return SOPRO_OK;
+}
+static_assert((int)EPI_NONE == tc::EPI_NONE && (int)EPI_GELU == tc::EPI_GELU && (int)EPI_RES_SCALE == tc::EPI_RES_SCALE &&
+                  (int)EPI_RES == tc::EPI_RES,
+              "both GEMMs take the same epilogue codes");
+
+// Scratch of the transformer layers.  ln, att and hid are fp32 in fp32 mode and bf16 in tensor-core mode; k and vt
+// take the tensor-core attention's keys and transposed values (written by rope_pack_kernel with the queries in ln).
+struct LayerBufs {
+  void *ln, *att, *hid;  // LayerNorm output [rows][C], attention output [rows][C], MLP hidden [rows][FF]
+  float* qkv;            // [rows][3C]
+  __nv_bfloat16 *k, *vt;  // [rows][C], [B][C][T2 rounded up to 8]
+};
+
+// A stream's K/V rings: layer l holds the rotated key / the value of position p in row p % R of k / v + l*R*C;
+// row 0 of the chunk is position pos0
+struct KVRing {
+  float *k, *v;
+  int R, pos0;
+};
+
+// Transformer layers (MimiTransformerLayer: x += LS1 * attn(LN1(x)); x += LS2 * MLP(LN2(x))) in place on the residual
+// stream x [B][T2][C].  Attention: given a ring, the chunk's keys and values are appended to it and the queries attend
+// over it; without one, tensor-core mode runs rope_pack_kernel + the tensor-core attention when its tiles take the
+// geometry; otherwise the plain RoPE and attention kernels run.
+int run_layers(const sopro_mimi_config_t& c, const std::vector<sopro_mimi::Layer>& layers, bool tcm, const float* Wd,
+               const __nv_bfloat16* Wh, const float* rope, int rope_T2, float* x, int B, int T2, const LayerBufs& b,
+               const KVRing* ring, cudaStream_t st) {
+  const int C = c.hidden, H = c.n_heads, Dh = C / H, FF = c.ffn;
+  const long long rows = (long long)B * T2;
+  const unsigned ln_grid = (unsigned)((rows + 7) / 8);
+  const size_t asm_bytes = (size_t)8 * (Dh + c.window) * 4, pack_bytes = (size_t)32 * (C + 2) * 2;
+  const bool tc_attn = tcm && !ring && tc::attn_supported(C, H, c.window) && pack_bytes <= 48 * 1024;
+  const long long T2p = (T2 + 7) / 8 * 8;  // v^T row pitch: tensor-map strides are multiples of 16 bytes
+  const int pos0 = ring ? ring->pos0 : 0, R = ring ? ring->R : 1;
+  // the layers over the LayerNorm output `ln`, the attention output `att` and the MLP hidden `hid`: bf16 in tensor-core
+  // mode, fp32 otherwise
+  auto run = [&](auto* ln, auto* att, auto* hid) -> int {
+    using T = std::remove_pointer_t<decltype(ln)>;
+    constexpr bool tc_mode = std::is_same<T, __nv_bfloat16>::value;
+    // one Linear over the rows; with `scale` its result, times the LayerScale, is added to x.  Output: fp32 `of`, or
+    // `oh` (the MLP hidden)
+    auto lin = [&](const T* A, int K, size_t w, size_t w_h, int N, int epi, const float* scale, float* of, T* oh) -> int {
+      const Operand a{A, T2, 0, B};
+      const float* res = scale ? x : nullptr;
+      if constexpr (tc_mode) return gemm_tc(a, K, 1, Wh + w_h, nullptr, N, N, epi, res, scale, of, oh, 0, st);
+      else return gemm_f32(a, K, 1, Wd + w, nullptr, N, N, epi, res, scale, of ? of : oh, 0, st);
+    };
+    int rc;
+    for (size_t li = 0; li < layers.size(); ++li) {
+      const sopro_mimi::Layer& L = layers[li];
+      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln1w, Wd + L.ln1b, ln, rows, C, c.norm_eps);
+      if ((rc = lin(ln, C, L.qkv, L.qkv_h, 3 * C, EPI_NONE, nullptr, b.qkv, nullptr))) return rc;
+      if (tc_attn) {
+        if constexpr (tc_mode) {  // q goes to ln (dead until the next LayerNorm)
+          rope_pack_kernel<tc::kAttnDh><<<dim3((T2 + 31) / 32, B), 256, pack_bytes, st>>>(b.qkv, rope, ln, b.k, b.vt, T2, T2p, rope_T2, C, H);
+          MCK(cudaGetLastError());
+          cudaError_t ae = tc::launch_attn(ln, b.k, b.vt, att, B, T2, T2p, C, H, c.window, st);
+          if (ae != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core attention: %s", cudaGetErrorString(ae));
+        }
+      } else {
+        float* kr = ring ? ring->k + li * (size_t)R * C : nullptr;
+        float* vr = ring ? ring->v + li * (size_t)R * C : nullptr;
+        rope_kernel<<<dim3(T2, B), 256, 0, st>>>(b.qkv, rope, T2, rope_T2, C, H, pos0, kr, vr, R);
+        attn_kernel<<<dim3((T2 + 7) / 8, H, B), 256, asm_bytes, st>>>(b.qkv, att, T2, C, H, c.window, pos0, kr, vr, R);
+        MCK(cudaGetLastError());
+      }
+      if ((rc = lin(att, C, L.wo, L.wo_h, C, EPI_RES_SCALE, Wd + L.ls1, x, nullptr))) return rc;
+      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln2w, Wd + L.ln2b, ln, rows, C, c.norm_eps);
+      if ((rc = lin(ln, C, L.fc1, L.fc1_h, FF, EPI_GELU, nullptr, nullptr, hid))) return rc;
+      if ((rc = lin(hid, FF, L.fc2, L.fc2_h, C, EPI_RES_SCALE, Wd + L.ls2, x, nullptr))) return rc;
+    }
+    return SOPRO_OK;
+  };
+  using bf16 = __nv_bfloat16;
+  if (tcm) return run(static_cast<bf16*>(b.ln), static_cast<bf16*>(b.att), static_cast<bf16*>(b.hid));
+  return run(static_cast<float*>(b.ln), static_cast<float*>(b.att), static_cast<float*>(b.hid));
+}
+
+}  // namespace
+
+// Context rows a stream moves to the front of its conv operand buffers after a step (the parameter of
+// tail_shift_kernel, so outside the anonymous namespace)
+struct TailShift {
+  void* base[16];
+  int row_bytes[16], ctx[16], rows[16];  // rows = new rows written behind the ctx rows this step
+  int n;
+};
+
+namespace {
+
+// A SEANet activation buffer: `ctx` rows of left context in front of the rows a pass writes
+struct Buf {
+  void* p;
+  int ctx;
+  template <typename T>
+  T* rows(int cols) const { return static_cast<T*>(p) + (size_t)ctx * cols; }  // the first row a pass writes
+  Operand operand(long long M, int B) const { return {p, M, ctx, B}; }
+};
+
+// Buffers of one SEANet decoder pass.  fp32 mode: every buffer is fp32 and `h` holds the raw ResnetBlock hidden.
+// Tensor-core mode: `in`, `a0`, `z`, `o` hold bf16 activations with their consumer's ELU applied, `zf` the fp32 skip
+// (the ConvTranspose output) and `h` the bf16 ELU'd hidden of a block that does not take the fused kernel.
+struct SeanetBufs {
+  Buf in;  // conv0 operand [ctx + T2][C]: the residual stream itself (fp32) or its bf16 copy (tensor-core mode)
+  Buf a0;  // conv0 output
+  struct Stage {
+    Buf z, h, o;  // ConvTranspose output, ResnetBlock hidden, block output
+    float* zf;
+  } stage[SOPRO_MIMI_MAX_RATIOS];
+};
+
+// records that `rows` new rows were written behind b's context rows (no-op without a record)
+void carry(TailShift* ts, const Buf& b, int row_bytes, long long rows) {
+  if (!ts) return;
+  ts->base[ts->n] = b.p;
+  ts->row_bytes[ts->n] = row_bytes;
+  ts->ctx[ts->n] = b.ctx;
+  ts->rows[ts->n] = (int)rows;
+  ++ts->n;
+}
+
+// SEANet decoder in fp32: conv0, per stage ELU -> ConvTranspose (stride r, kernel 2r: a 2-tap GEMM with r*Cout columns)
+// and the ResnetBlock z + conv1(ELU(conv3(ELU(z)))), then ELU -> final conv into wav [B][T2 * prod(ratios)].  The
+// tail shift of every buffer that holds a conv operand is recorded in *ts when ts is given.
+int seanet_f32(const sopro_mimi* m, const SeanetBufs& b, int B, long long T2, TailShift* ts, float* wav, cudaStream_t st) {
+  const sopro_mimi_config_t& c = m->cfg;
+  const float* Wd = m->dev;
+  long long Tn = T2;
+  int ch = c.num_filters << c.n_ratios, rc;
+  if ((rc = gemm_f32(b.in.operand(Tn, B), c.hidden, c.kernel, Wd + m->c0w, Wd + m->c0b, ch, ch, EPI_NONE, nullptr, nullptr,
+                     b.a0.rows<float>(ch), 0, st)))
+    return rc;
+  carry(ts, b.in, c.hidden * 4, Tn);
+  carry(ts, b.a0, ch * 4, Tn);
+  Buf cur = b.a0;
+  for (size_t si = 0; si < m->stages.size(); ++si) {
+    const sopro_mimi::Stage& S = m->stages[si];
+    const SeanetBufs::Stage& sb = b.stage[si];
+    const int hid = S.cout / c.compress;
+    if ((rc = gemm_f32(cur.operand(Tn, B), S.cin, 2, Wd + S.tw, Wd + S.tb, S.ratio * S.cout, S.cout, EPI_NONE, nullptr, nullptr,
+                       sb.z.rows<float>(S.cout), 1, st)))
+      return rc;
+    Tn *= S.ratio;
+    if ((rc = gemm_f32(sb.z.operand(Tn, B), S.cout, c.res_kernel, Wd + S.r1w, Wd + S.r1b, hid, hid, EPI_NONE, nullptr, nullptr,
+                       sb.h.rows<float>(hid), 1, st)))
+      return rc;
+    if ((rc = gemm_f32(sb.h.operand(Tn, B), hid, 1, Wd + S.r2w, Wd + S.r2b, S.cout, S.cout, EPI_RES, sb.z.rows<float>(S.cout), nullptr,
+                       sb.o.rows<float>(S.cout), 1, st)))
+      return rc;
+    carry(ts, sb.z, S.cout * 4, Tn);
+    carry(ts, sb.o, S.cout * 4, Tn);
+    cur = sb.o;
+    ch = S.cout;
+  }
+  final_conv_kernel<<<dim3((unsigned)((Tn + 255) / 256), B), 256, 0, st>>>(cur.rows<float>(ch), Wd + m->lw, Wd + m->lb, wav, Tn, ch,
+                                                                            c.last_kernel, -cur.ctx);
+  MCK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+// SEANet decoder in tensor-core mode (check_tc_geometry passed), from the fp32 residual stream x [B][T2][C].
+// Activations that feed a contraction travel as bf16 with the consumer's ELU already applied; the ResnetBlock skip
+// stays fp32.  A ResnetBlock runs in one launch when the fused kernel takes its geometry, else conv by conv.
+int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, long long T2, TailShift* ts, float* wav, cudaStream_t st) {
+  const sopro_mimi_config_t& c = m->cfg;
+  const int C = c.hidden;
+  const float* Wd = m->dev;
+  const __nv_bfloat16* Wh = m->dev_h;
+  long long Tn = T2;
+  int ch = c.num_filters << c.n_ratios, rc;
+  const long long n4 = (long long)B * T2 * C / 4;
+  cast_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(x, b.in.rows<__nv_bfloat16>(C), n4);
+  MCK(cudaGetLastError());
+  if ((rc = gemm_tc(b.in.operand(Tn, B), C, c.kernel, Wh + m->c0w_h, Wd + m->c0b, ch, ch, tc::EPI_NONE, nullptr, nullptr, nullptr,
+                    b.a0.rows<__nv_bfloat16>(ch), 1, st)))
+    return rc;
+  carry(ts, b.in, C * 2, Tn);
+  carry(ts, b.a0, ch * 2, Tn);
+  Buf cur = b.a0;
+  for (size_t si = 0; si < m->stages.size(); ++si) {
+    const sopro_mimi::Stage& S = m->stages[si];
+    const SeanetBufs::Stage& sb = b.stage[si];
+    const int hid = S.cout / c.compress;
+    // ELU -> ConvTranspose: fp32 skip zf, bf16 ELU(z) for the ResnetBlock
+    if ((rc = gemm_tc(cur.operand(Tn, B), S.cin, 2, Wh + S.tw_h, Wd + S.tb, S.ratio * S.cout, S.cout, tc::EPI_NONE, nullptr, nullptr,
+                      sb.zf, sb.z.rows<__nv_bfloat16>(S.cout), 1, st)))
+      return rc;
+    Tn *= S.ratio;
+    if (tc::resblock_supported(hid, S.cout) && (S.cout * c.res_kernel) % 64 == 0) {
+      tc::ResOp ro{};
+      ro.bias1 = Wd + S.r1b;
+      ro.bias2 = Wd + S.r2b;
+      ro.Z = sb.zf;
+      ro.out_bf16 = sb.o.rows<__nv_bfloat16>(S.cout);
+      ro.M = (int)Tn;
+      ro.Min = (int)Tn + sb.z.ctx;
+      ro.taps = c.res_kernel;
+      ro.pad = c.res_kernel - 1 - sb.z.ctx;
+      ro.out_elu = 1;
+      cudaError_t fe = tc::launch_resblock(sb.z.p, Wh + S.r1w_h, Wh + S.r2w_h, hid, ro, B, st);
+      if (fe != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "fused ResnetBlock (stage %zu): %s", si, cudaGetErrorString(fe));
+    } else {  // conv k=3 -> ELU(h) bf16, then the 1x1 conv + fp32 skip
+      if ((rc = gemm_tc(sb.z.operand(Tn, B), S.cout, c.res_kernel, Wh + S.r1w_h, Wd + S.r1b, hid, hid, tc::EPI_NONE, nullptr, nullptr,
+                        nullptr, sb.h.rows<__nv_bfloat16>(hid), 1, st)))
+        return rc;
+      if ((rc = gemm_tc(sb.h.operand(Tn, B), hid, 1, Wh + S.r2w_h, Wd + S.r2b, S.cout, S.cout, tc::EPI_RES, sb.zf, nullptr, nullptr,
+                        sb.o.rows<__nv_bfloat16>(S.cout), 1, st)))
+        return rc;
+    }
+    carry(ts, sb.z, S.cout * 2, Tn);
+    carry(ts, sb.o, S.cout * 2, Tn);
+    cur = sb.o;
+    ch = S.cout;
+  }
+  const int per = 256 - (c.last_kernel - 1);
+  final_conv_h_kernel<<<dim3((unsigned)((Tn + per - 1) / per), B), 256, (size_t)(c.last_kernel * 256 + c.last_kernel * ch) * 4, st>>>(
+      cur.rows<__nv_bfloat16>(ch), Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, -cur.ctx);
+  MCK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+// One-shot decode of codes [B][Q][T] into the workspace mimi_prepare sized: RVQ, projection, upsample, transformer,
+// SEANet.  Enqueues only (it runs under graph capture).
+int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, cudaStream_t st) {
+  const sopro_mimi_config_t& c = m->cfg;
+  const int C = c.hidden, T2 = 2 * T, FF = c.ffn;
+  const float* Wd = m->dev;
+  const bool use_tc = m->precision == SOPRO_MIMI_BF16_TC;
+  // ---- workspace (mimi_prepare): three fp32 ping-pong buffers sized for the widest SEANet activation + transformer
+  //      scratch, the residual stream and its normalised copy, three bf16 buffers for the tensor-core operands
+  long long up = 2;
+  for (int i = 0; i < c.n_ratios; ++i) up *= c.ratios[i];
+  const size_t big = (size_t)B * T * up * c.num_filters;                     // [T*1920][64]
+  const size_t tr = (size_t)B * T2 * (size_t)std::max(3 * C, FF);            // QKV / MLP hidden
+  const size_t bufsz = (std::max(std::max(big, tr), (size_t)B * T2 * (c.num_filters << c.n_ratios)) + 63) / 64 * 64;
+  const size_t xsz = ((size_t)B * T2 * C + 63) / 64 * 64;
+  float* b0 = m->ws;
+  float* b1 = b0 + bufsz;
+  float* b2 = b1 + bufsz;
+  float* x = b2 + bufsz;    // residual stream [B][T2][C]
+  float* ln = x + xsz;      // normalised copy (fp32 mode)
+  __nv_bfloat16* h0 = reinterpret_cast<__nv_bfloat16*>(ln + xsz);
+  __nv_bfloat16* h1 = h0 + bufsz;
+  __nv_bfloat16* h2 = h1 + bufsz;
+  // ---- RVQ + projection + upsample (small; fp32 in both modes)
+  rvq_gather_kernel<<<dim3(T, B), 256, 0, st>>>(codes, Wd + m->embed, b0, c.n_q, T, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
+  MCK(cudaGetLastError());
+  int rc;
+  if ((rc = gemm_f32({b0, T, 0, B}, C, 1, Wd + m->rvq_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, b1, 0, st))) return rc;
+  upsample_kernel<<<dim3(T2, B), 256, 0, st>>>(b1, Wd + m->up_w, x, T, C, nullptr);
+  MCK(cudaGetLastError());
+  // ---- transformer: b1 (idle until the SEANet) takes the attention output; tensor-core mode: the LayerNorm copy and
+  //      q in h0, k in h1, v^T and the MLP hidden in h2
+  LayerBufs lb{};
+  lb.ln = use_tc ? (void*)h0 : ln;
+  lb.qkv = b0;
+  lb.att = b1;
+  lb.hid = use_tc ? (void*)h2 : b0;
+  lb.k = h1;
+  lb.vt = h2;
+  if ((rc = run_layers(c, m->layers, use_tc, Wd, m->dev_h, m->rope, m->rope_T2, x, B, T2, lb, nullptr, st))) return rc;
+  // ---- SEANet decoder over ping-pong buffers, no context rows.  fp32: x -> b0, per stage b0 -> b1 -> b2 -> b0.
+  //      Tensor-core: bf16 copy of x in h2 -> h0, per stage h0 -> h1 (+ fp32 skip b1) -> [h2] -> h0
+  SeanetBufs sb{};
+  sb.in = {use_tc ? (void*)h2 : x, 0};
+  sb.a0 = {use_tc ? (void*)h0 : b0, 0};
+  for (int i = 0; i < c.n_ratios; ++i)
+    sb.stage[i] = use_tc ? SeanetBufs::Stage{{h1, 0}, {h2, 0}, {h0, 0}, b1} : SeanetBufs::Stage{{b1, 0}, {b2, 0}, {b0, 0}, nullptr};
+  return use_tc ? seanet_tc(m, x, sb, B, T2, nullptr, wav, st) : seanet_f32(m, sb, B, T2, nullptr, wav, st);
+}
 }  // namespace
 
 extern "C" {
@@ -761,10 +1095,12 @@ int sopro_mimi_decode(sopro_mimi_t* m, const int32_t* codes, int B, int T, float
   if (!m || !codes || !wav) return mfail(SOPRO_ERR_INVALID, "null argument");
   if (B < 1 || T < 1) return mfail(SOPRO_ERR_INVALID, "B and T must be >= 1");
   if (B > 65535) return mfail(SOPRO_ERR_INVALID, "B must be <= 65535");
+  if ((long long)T * sopro_mimi_samples_per_frame(m) > 0x7fffffffLL) return mfail(SOPRO_ERR_INVALID, "sequence too long for one launch");
+  int rc;
+  if (m->precision == SOPRO_MIMI_BF16_TC && (rc = check_tc_geometry(m))) return rc;
   MCK(cudaSetDevice(m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = mimi_prepare(m, B, T, st);
-  if (rc) return rc;
+  if ((rc = mimi_prepare(m, B, T, st))) return rc;
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   MCK(cudaStreamIsCapturing(st, &cap));
   if (!m->graphs || (long long)B * T > kGraphFrames || cap != cudaStreamCaptureStatusNone) return mimi_enqueue(m, codes, B, T, wav, st);
@@ -802,223 +1138,6 @@ int sopro_mimi_decode(sopro_mimi_t* m, const int32_t* codes, int B, int T, float
 
 }  // extern "C"
 
-namespace {
-int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, cudaStream_t st) {
-  const sopro_mimi_config_t& c = m->cfg;
-  const int C = c.hidden, T2 = 2 * T, H = c.n_heads, Dh = C / H, FF = c.ffn;
-  const float* Wd = m->dev;
-  const __nv_bfloat16* Wh = m->dev_h;
-  const bool use_tc = m->precision == SOPRO_MIMI_BF16_TC;
-  // ---- workspace (mimi_prepare): three fp32 ping-pong buffers sized for the widest SEANet activation + transformer
-  //      scratch, the residual stream and its normalised copy, three bf16 buffers for the tensor-core operands
-  long long up = 2;
-  for (int i = 0; i < c.n_ratios; ++i) up *= c.ratios[i];
-  const size_t big = (size_t)B * T * up * c.num_filters;                     // [T*1920][64]
-  const size_t tr = (size_t)B * T2 * (size_t)std::max(3 * C, FF);            // QKV / MLP hidden
-  const size_t bufsz = (std::max(std::max(big, tr), (size_t)B * T2 * (c.num_filters << c.n_ratios)) + 63) / 64 * 64;
-  const size_t xsz = ((size_t)B * T2 * C + 63) / 64 * 64;
-  float* b0 = m->ws;
-  float* b1 = b0 + bufsz;
-  float* b2 = b1 + bufsz;
-  float* x = b2 + bufsz;    // residual stream [B][T2][C]
-  float* ln = x + xsz;      // normalised copy (fp32 mode)
-  __nv_bfloat16* h0 = reinterpret_cast<__nv_bfloat16*>(ln + xsz);
-  __nv_bfloat16* h1 = h0 + bufsz;
-  __nv_bfloat16* h2 = h1 + bufsz;
-  // ---- RVQ + projection + upsample (small; fp32 in both modes)
-  rvq_gather_kernel<<<dim3(T, B), 256, 0, st>>>(codes, Wd + m->embed, b0, c.n_q, T, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
-  MCK(cudaGetLastError());
-  GemmOp g{};
-  auto lin = [&](const float* A, int M, int K, const float* W, int N, float* Cc, int epi, const float* R, const float* scale) {
-    g = GemmOp{};
-    g.A = A; g.W = W; g.C = Cc; g.R = R; g.scale = scale; g.bias = nullptr;
-    g.M = M; g.N = N; g.K = K; g.Min = M; g.Cin = K; g.taps = 1; g.dil = 1; g.pad = 0; g.ldc = N; g.bias_mod = N; g.epi = epi;
-    g.a_bs = (long long)M * K; g.c_bs = (long long)M * N; g.r_bs = (long long)M * N;
-    return launch_gemm(g, B, st);
-  };
-  auto conv = [&](const float* A, long long Tin, int cin, int taps, int pad, const float* W, const float* bias, int N, int bias_mod,
-                  float* Cc, int elu, int epi, const float* R) {
-    g = GemmOp{};
-    g.A = A; g.W = W; g.C = Cc; g.R = R; g.bias = bias; g.scale = nullptr;
-    g.M = (int)Tin; g.N = N; g.K = taps * cin; g.Min = (int)Tin; g.Cin = cin; g.taps = taps; g.dil = 1; g.pad = pad; g.ldc = N;
-    g.bias_mod = bias_mod; g.epi = epi; g.a_elu = elu;
-    g.a_bs = Tin * cin; g.c_bs = Tin * N; g.r_bs = Tin * N;
-    return launch_gemm(g, B, st);
-  };
-  // tensor-core implicit GEMM: X bf16 [B][rows][cin] (ELU already applied by its producer where the layer wants it)
-  auto tcg = [&](const __nv_bfloat16* X, long long rows, int cin, int taps, int pad, const __nv_bfloat16* W, const float* bias,
-                 int N, int bias_mod, int epi, const float* R, const float* scale, float* of, __nv_bfloat16* oh, int out_elu) {
-    tc::TcOp o{};
-    o.bias = bias; o.R = R; o.scale = scale; o.out_f32 = of; o.out_bf16 = oh;
-    o.c_bs = rows * N; o.M = (int)rows; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = 1; o.pad = pad;
-    o.bias_mod = bias_mod; o.epi = epi; o.out_elu = out_elu;
-    cudaError_t e = tc::launch(X, rows, W, o, B, st);
-    if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core GEMM (N=%d K=%d): %s", N, o.K, cudaGetErrorString(e));
-    return (int)SOPRO_OK;
-  };
-  int rc;
-  if ((rc = lin(b0, T, C, Wd + m->rvq_w, C, b1, EPI_NONE, nullptr, nullptr))) return rc;
-  upsample_kernel<<<dim3(T2, B), 256, 0, st>>>(b1, Wd + m->up_w, x, T, C, nullptr);
-  MCK(cudaGetLastError());
-  // ---- transformer
-  const long long rows = (long long)B * T2;
-  const unsigned ln_grid = (unsigned)((rows + 7) / 8);
-  const size_t asm_bytes = (size_t)8 * (Dh + c.window) * 4;
-  const bool tc_tr = use_tc && tc::supported(3 * C, C, C) && tc::supported(C, C, C) && tc::supported(FF, C, C) && tc::supported(C, FF, FF);
-  const bool tc_attn = tc_tr && tc::attn_supported(C, H, c.window) && (size_t)32 * (C + 2) * 2 <= 48 * 1024;
-  const long long T2p = (T2 + 7) / 8 * 8;  // v^T row pitch: tensor-map strides are multiples of 16 bytes
-  for (const sopro_mimi::Layer& L : m->layers) {
-    if (tc_tr) {
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln1w, Wd + L.ln1b, h0, rows, C, c.norm_eps);
-      if ((rc = tcg(h0, T2, C, 1, 0, Wh + L.qkv_h, nullptr, 3 * C, 3 * C, tc::EPI_NONE, nullptr, nullptr, b0, nullptr, 0))) return rc;
-      __nv_bfloat16* att = reinterpret_cast<__nv_bfloat16*>(b1);  // b1 is idle during the transformer
-      if (tc_attn) {
-        // q -> h0 (the LayerNorm copy is dead), k -> h1, v^T -> h2
-        rope_pack_kernel<tc::kAttnDh><<<dim3((T2 + 31) / 32, B), 256, (size_t)32 * (C + 2) * 2, st>>>(b0, m->rope, h0, h1, h2, T2, T2p, m->rope_T2, C, H);
-        MCK(cudaGetLastError());
-        cudaError_t ae = tc::launch_attn(h0, h1, h2, att, B, T2, T2p, C, H, c.window, st);
-        if (ae != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core attention: %s", cudaGetErrorString(ae));
-      } else {
-        rope_kernel<<<dim3(T2, B), 256, 0, st>>>(b0, m->rope, T2, m->rope_T2, C, H, 0, nullptr, nullptr, 1);
-        attn_kernel<<<dim3((T2 + 7) / 8, H, B), 256, asm_bytes, st>>>(b0, att, T2, C, H, c.window, 0, nullptr, nullptr, 1);
-        MCK(cudaGetLastError());
-      }
-      if ((rc = tcg(att, T2, C, 1, 0, Wh + L.wo_h, nullptr, C, C, tc::EPI_RES_SCALE, x, Wd + L.ls1, x, nullptr, 0))) return rc;
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln2w, Wd + L.ln2b, h0, rows, C, c.norm_eps);
-      if ((rc = tcg(h0, T2, C, 1, 0, Wh + L.fc1_h, nullptr, FF, FF, tc::EPI_GELU, nullptr, nullptr, nullptr, h2, 0))) return rc;
-      if ((rc = tcg(h2, T2, FF, 1, 0, Wh + L.fc2_h, nullptr, C, C, tc::EPI_RES_SCALE, x, Wd + L.ls2, x, nullptr, 0))) return rc;
-    } else {
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln1w, Wd + L.ln1b, ln, rows, C, c.norm_eps);
-      if ((rc = lin(ln, T2, C, Wd + L.qkv, 3 * C, b0, EPI_NONE, nullptr, nullptr))) return rc;
-      rope_kernel<<<dim3(T2, B), 256, 0, st>>>(b0, m->rope, T2, m->rope_T2, C, H, 0, nullptr, nullptr, 1);
-      attn_kernel<<<dim3((T2 + 7) / 8, H, B), 256, asm_bytes, st>>>(b0, b1, T2, C, H, c.window, 0, nullptr, nullptr, 1);
-      MCK(cudaGetLastError());
-      if ((rc = lin(b1, T2, C, Wd + L.wo, C, x, EPI_RES_SCALE, x, Wd + L.ls1))) return rc;
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln2w, Wd + L.ln2b, ln, rows, C, c.norm_eps);
-      if ((rc = lin(ln, T2, C, Wd + L.fc1, FF, b0, EPI_GELU, nullptr, nullptr))) return rc;
-      if ((rc = lin(b0, T2, FF, Wd + L.fc2, C, x, EPI_RES_SCALE, x, Wd + L.ls2))) return rc;
-    }
-  }
-  // ---- SEANet decoder
-  long long Tn = T2;
-  int ch = c.num_filters << c.n_ratios;
-  if (!use_tc) {
-    if ((rc = conv(x, Tn, C, c.kernel, c.kernel - 1, Wd + m->c0w, Wd + m->c0b, ch, ch, b0, 0, EPI_NONE, nullptr))) return rc;
-    float* cur = b0;
-    float* o1 = b1;
-    float* o2 = b2;
-    for (const sopro_mimi::Stage& S : m->stages) {
-      if (Tn * S.ratio > 0x7fffffffLL) return mfail(SOPRO_ERR_INVALID, "sequence too long for one launch");
-      // ELU -> ConvTranspose(stride r, kernel 2r) as a 2-tap implicit GEMM with r*Cout columns
-      if ((rc = conv(cur, Tn, S.cin, 2, 1, Wd + S.tw, Wd + S.tb, S.ratio * S.cout, S.cout, o1, 1, EPI_NONE, nullptr))) return rc;
-      Tn *= S.ratio;
-      // ResnetBlock: o1 + conv1(ELU(conv3(ELU(o1))))
-      const int hid = S.cout / c.compress;
-      if ((rc = conv(o1, Tn, S.cout, c.res_kernel, c.res_kernel - 1, Wd + S.r1w, Wd + S.r1b, hid, hid, o2, 1, EPI_NONE, nullptr))) return rc;
-      if ((rc = conv(o2, Tn, hid, 1, 0, Wd + S.r2w, Wd + S.r2b, S.cout, S.cout, cur, 1, EPI_RES, o1))) return rc;
-      ch = S.cout;
-    }
-    final_conv_kernel<<<dim3((unsigned)((Tn + 255) / 256), B), 256, 0, st>>>(cur, Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, 0);
-    MCK(cudaGetLastError());
-    return SOPRO_OK;
-  }
-  // tensor-core mode.  Activations that feed a contraction travel as bf16 with the consumer's ELU already
-  // applied; only the ConvTranspose output (the ResnetBlock skip) and whatever a fp32 kernel reads are fp32.
-  //   curh: bf16 operand of the next ConvTranspose;  z (b1): fp32 skip;  b0: fp32 block output when needed
-  __nv_bfloat16* curh = h0;
-  __nv_bfloat16* ha = h1;
-  __nv_bfloat16* hb = h2;
-  float* cur32 = nullptr;  // set when the running activation lives in fp32 (b0) instead of curh
-  if (tc::supported(ch, c.kernel * C, C)) {
-    const long long n4 = (long long)B * T2 * C / 4;
-    cast_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(x, hb, n4);
-    MCK(cudaGetLastError());
-    if ((rc = tcg(hb, Tn, C, c.kernel, c.kernel - 1, Wh + m->c0w_h, Wd + m->c0b, ch, ch, tc::EPI_NONE, nullptr, nullptr, nullptr, curh, 1)))
-      return rc;
-  } else {
-    if ((rc = conv(x, Tn, C, c.kernel, c.kernel - 1, Wd + m->c0w, Wd + m->c0b, ch, ch, b0, 0, EPI_NONE, nullptr))) return rc;
-    cur32 = b0;
-  }
-  const bool final_h = c.num_filters % 8 == 0 && c.last_kernel <= 8;  // final conv reads the bf16 ELU'd activation
-  for (size_t si = 0; si < m->stages.size(); ++si) {
-    const sopro_mimi::Stage& S = m->stages[si];
-    if (Tn * S.ratio > 0x7fffffffLL) return mfail(SOPRO_ERR_INVALID, "sequence too long for one launch");
-    const int hid = S.cout / c.compress, NT = S.ratio * S.cout;
-    const bool last = si + 1 == m->stages.size();
-    const bool t_ok = !cur32 && tc::supported(NT, 2 * S.cin, S.cin);
-    const bool r1_ok = tc::supported(hid, c.res_kernel * S.cout, S.cout);
-    const bool r2_ok = tc::supported(S.cout, hid, hid);
-    // the consumer of this stage's output: the next ConvTranspose on tensor cores wants bf16 ELU(x); the
-    // final conv and the fp32 kernels read fp32
-    bool next_tc = final_h;  // after the last stage: the bf16 final conv
-    if (!last) {
-      const sopro_mimi::Stage& Nx = m->stages[si + 1];
-      next_tc = tc::supported(Nx.ratio * Nx.cout, 2 * Nx.cin, Nx.cin);
-    }
-    // ConvTranspose -> z fp32 (b1) [+ bf16 ELU(z) in ha when res1 runs on tensor cores]
-    if (t_ok) {
-      if ((rc = tcg(curh, Tn, S.cin, 2, 1, Wh + S.tw_h, Wd + S.tb, NT, S.cout, tc::EPI_NONE, nullptr, nullptr, b1, r1_ok ? ha : nullptr, 1)))
-        return rc;
-    } else {
-      if (!cur32) return mfail(SOPRO_ERR_INVALID, "internal: stage %zu has no fp32 input", si);
-      if ((rc = conv(cur32, Tn, S.cin, 2, 1, Wd + S.tw, Wd + S.tb, NT, S.cout, b1, 1, EPI_NONE, nullptr))) return rc;
-    }
-    Tn *= S.ratio;
-    const bool ha_valid = t_ok && r1_ok;
-    // ResnetBlock in one launch when the geometry allows (hidden activation stays on chip), else conv by conv
-    static const bool fuse_res = !(getenv("SOPRO_MIMI_FUSE_RES") && atoi(getenv("SOPRO_MIMI_FUSE_RES")) == 0);
-    if (fuse_res && ha_valid && r2_ok && tc::resblock_supported(hid, S.cout) && (S.cout * c.res_kernel) % 64 == 0) {
-      tc::ResOp ro{};
-      ro.bias1 = Wd + S.r1b;
-      ro.bias2 = Wd + S.r2b;
-      ro.Z = b1;
-      ro.out_f32 = next_tc ? nullptr : b0;
-      ro.out_bf16 = next_tc ? curh : nullptr;
-      ro.M = (int)Tn;
-      ro.taps = c.res_kernel;
-      ro.pad = c.res_kernel - 1;
-      ro.out_elu = 1;
-      cudaError_t fe = tc::launch_resblock(ha, Wh + S.r1w_h, Wh + S.r2w_h, hid, ro, B, st);
-      if (fe != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "fused ResnetBlock (stage %zu): %s", si, cudaGetErrorString(fe));
-      cur32 = next_tc ? nullptr : b0;
-      ch = S.cout;
-      continue;
-    }
-    // res conv k=3 -> ELU(h) bf16 (hb) for a tensor-core res2, else raw h fp32 (b2)
-    if (ha_valid) {
-      if ((rc = tcg(ha, Tn, S.cout, c.res_kernel, c.res_kernel - 1, Wh + S.r1w_h, Wd + S.r1b, hid, hid, tc::EPI_NONE, nullptr, nullptr,
-                    r2_ok ? nullptr : b2, r2_ok ? hb : nullptr, 1)))
-        return rc;
-    } else {
-      if ((rc = conv(b1, Tn, S.cout, c.res_kernel, c.res_kernel - 1, Wd + S.r1w, Wd + S.r1b, hid, hid, b2, 1, EPI_NONE, nullptr))) return rc;
-    }
-    // res conv k=1 + skip
-    if (ha_valid && r2_ok) {
-      if ((rc = tcg(hb, Tn, hid, 1, 0, Wh + S.r2w_h, Wd + S.r2b, S.cout, S.cout, tc::EPI_RES, b1, nullptr, next_tc ? nullptr : b0,
-                    next_tc ? curh : nullptr, 1)))
-        return rc;
-      cur32 = next_tc ? nullptr : b0;
-    } else {
-      if ((rc = conv(b2, Tn, hid, 1, 0, Wd + S.r2w, Wd + S.r2b, S.cout, S.cout, b0, 1, EPI_RES, b1))) return rc;
-      cur32 = b0;
-      if (next_tc && !last) {  // fp32 block output feeding a tensor-core ConvTranspose: not reachable with Mimi's geometry
-        return mfail(SOPRO_ERR_UNSUPPORTED, "unsupported channel geometry for tensor-core mode (stage %zu)", si);
-      }
-    }
-    ch = S.cout;
-  }
-  if (cur32) {
-    final_conv_kernel<<<dim3((unsigned)((Tn + 255) / 256), B), 256, 0, st>>>(cur32, Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, 0);
-  } else {
-    const int per = 256 - (c.last_kernel - 1);
-    final_conv_h_kernel<<<dim3((unsigned)((Tn + per - 1) / per), B), 256, (size_t)(c.last_kernel * 256 + c.last_kernel * ch) * 4, st>>>(
-        curh, Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, 0);
-  }
-  MCK(cudaGetLastError());
-  return SOPRO_OK;
-}
-}  // namespace
-
 
 // ---------------------------------------------------------------------------------------------
 // Streaming decode with persistent state (reference codec/mimi.py:83-181 MimiStreamDecoder; transformers
@@ -1033,12 +1152,6 @@ int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, 
 // computes each output element in the same order as the full decode: in fp32 mode the chunks are bit-identical to the
 // full decode's prefix.  Work per chunk is O(chunk), not O(prefix).
 // ---------------------------------------------------------------------------------------------
-struct TailShift {
-  void* base[16];
-  int row_bytes[16], ctx[16], rows[16];  // rows = new rows written behind the ctx rows this step
-  int n;
-};
-
 // one block per buffer: rows [rows, rows + ctx) -> [0, ctx) (through shared memory: the ranges may overlap)
 __global__ void __launch_bounds__(256) tail_shift_kernel(const TailShift ts) {
   extern __shared__ uint4 tsm[];
@@ -1061,13 +1174,12 @@ struct sopro_mimi_stream {
   float* up_prev = nullptr;
   float *kring = nullptr, *vring = nullptr;  // [n_layers][R][C]
   // ---- chunk buffers
-  float *S = nullptr, *E = nullptr, *XC = nullptr, *LN = nullptr, *QKV = nullptr, *ATT = nullptr, *HID = nullptr;
-  __nv_bfloat16 *LNh = nullptr, *ATTh = nullptr, *HIDh = nullptr, *XCh = nullptr;
-  void* A0 = nullptr;               // conv0 output  [1 + T2][16F]    (fp32 raw | bf16 ELU'd)
-  void* Z[SOPRO_MIMI_MAX_RATIOS]{};    // ConvTranspose output [2 + Tn][cout] (fp32 raw | bf16 ELU'd)
-  float* Zf[SOPRO_MIMI_MAX_RATIOS]{};  // tensor-core mode: fp32 skip [Tn][cout]
-  float* Hs[SOPRO_MIMI_MAX_RATIOS]{};  // fp32 mode: res hidden [Tn][cout/2]
-  void* O[SOPRO_MIMI_MAX_RATIOS]{};    // block output [ctx + Tn][cout], ctx = 1 (next ConvTranspose) or taps-1 (final conv)
+  float *S = nullptr, *E = nullptr, *XC = nullptr;  // XC: [conv0 context | residual stream of the chunk]
+  LayerBufs tr{};  // transformer scratch (ln, att, hid: bf16 views in tensor-core mode)
+  // SEANet buffers, each conv operand [taps-1 context rows | Tn rows] (fp32 raw | bf16 ELU'd): in [2 + T2][C],
+  // a0 [1 + T2][16F], z [2 + Tn][cout], o [ctx + Tn][cout] with ctx = 1 (next ConvTranspose) or taps-1 (final conv);
+  // h [Tn][cout/2] and zf [Tn][cout] (tensor-core mode) have no context
+  SeanetBufs sea{};
   int* codes_dev = nullptr;
   float* wav_dev = nullptr;
 };
@@ -1097,15 +1209,15 @@ void stream_layout(sopro_mimi_stream* s, unsigned char* base) {
   // conv operand buffers: the context rows at their fronts are state too, so they come next
   const int k0 = c.kernel - 1;
   s->XC = (float*)at(P.take((k0 + T2) * C * 4));
-  s->XCh = tcm ? (__nv_bfloat16*)at(P.take((k0 + T2) * C * 2)) : nullptr;
+  s->sea.in = {tcm ? at(P.take((k0 + T2) * C * 2)) : (void*)s->XC, k0};
   size_t ch = (size_t)c.num_filters << c.n_ratios, Tn = T2;
-  s->A0 = at(P.take((1 + Tn) * ch * es));
+  s->sea.a0 = {at(P.take((1 + Tn) * ch * es)), 1};
   for (int i = 0; i < c.n_ratios; ++i) {
     const size_t cout = ch / 2;
     Tn *= c.ratios[i];
-    const size_t ctx_o = i + 1 == c.n_ratios ? (size_t)(c.last_kernel - 1) : 1;
-    s->Z[i] = at(P.take((c.res_kernel - 1 + Tn) * cout * es));
-    s->O[i] = at(P.take((ctx_o + Tn) * cout * es));
+    const int ctx_o = i + 1 == c.n_ratios ? c.last_kernel - 1 : 1;
+    s->sea.stage[i].z = {at(P.take((c.res_kernel - 1 + Tn) * cout * es)), c.res_kernel - 1};
+    s->sea.stage[i].o = {at(P.take((ctx_o + Tn) * cout * es)), ctx_o};
     ch = cout;
   }
   s->state_bytes = P.off;  // everything up to here is zeroed by reset (a superset of the state proper)
@@ -1114,190 +1226,42 @@ void stream_layout(sopro_mimi_stream* s, unsigned char* base) {
   for (int i = 0; i < c.n_ratios; ++i) {
     const size_t cout = ch / 2;
     Tn *= c.ratios[i];
-    s->Zf[i] = tcm ? (float*)at(P.take(Tn * cout * 4)) : nullptr;
-    s->Hs[i] = (float*)at(P.take(Tn * (cout / c.compress) * 4));  // fp32 mode: fp32; tensor-core mode: bf16 view (unfused blocks)
+    s->sea.stage[i].zf = tcm ? (float*)at(P.take(Tn * cout * 4)) : nullptr;
+    s->sea.stage[i].h = {at(P.take(Tn * (cout / c.compress) * 4)), 0};  // fp32 mode: fp32; tensor-core mode: bf16 (unfused blocks)
     ch = cout;
   }
   s->S = (float*)at(P.take(n * C * 4));
   s->E = (float*)at(P.take(n * C * 4));
-  s->LN = (float*)at(P.take(T2 * C * 4));
-  s->QKV = (float*)at(P.take(T2 * 3 * C * 4));
-  s->ATT = (float*)at(P.take(T2 * C * 4));
-  s->HID = (float*)at(P.take(T2 * FF * 4));
-  s->LNh = (__nv_bfloat16*)s->LN;
-  s->ATTh = (__nv_bfloat16*)s->ATT;
-  s->HIDh = (__nv_bfloat16*)s->HID;
+  s->tr.ln = at(P.take(T2 * C * 4));
+  s->tr.qkv = (float*)at(P.take(T2 * 3 * C * 4));
+  s->tr.att = at(P.take(T2 * C * 4));
+  s->tr.hid = at(P.take(T2 * FF * 4));
   s->slab_bytes = P.off;
 }
 
 int stream_step(sopro_mimi_stream* s, const int32_t* codes, int n, int code_stride, float* wav, cudaStream_t st) {
   sopro_mimi* m = s->m;
   const sopro_mimi_config_t& c = m->cfg;
-  const int C = c.hidden, T2 = 2 * n, H = c.n_heads, Dh = C / H, FF = c.ffn;
+  const int C = c.hidden, T2 = 2 * n;
   const float* Wd = m->dev;
-  const __nv_bfloat16* Wh = m->dev_h;
   const bool tcm = s->precision == SOPRO_MIMI_BF16_TC;
   const int pos0 = (int)(2 * s->frames);
   int rc = ensure_rope(m, std::max(4096, 2 * (pos0 + T2)), st);
   if (rc) return rc;
-  GemmOp g{};
-  auto lin = [&](const float* A, int M, int K, const float* W, int N, float* Cc, int epi, const float* R, const float* scale) {
-    g = GemmOp{};
-    g.A = A; g.W = W; g.C = Cc; g.R = R; g.scale = scale; g.bias = nullptr;
-    g.M = M; g.N = N; g.K = K; g.Min = M; g.Cin = K; g.taps = 1; g.dil = 1; g.pad = 0; g.ldc = N; g.bias_mod = N; g.epi = epi;
-    return launch_gemm(g, 1, st);
-  };
-  // "valid" conv over [ctx rows | M rows]: A points at the first context row, Min = M + taps - 1, pad = 0
-  auto conv = [&](const float* A, long long M, int cin, int taps, const float* W, const float* bias, int N, int bias_mod, float* Cc,
-                  int elu, int epi, const float* R) {
-    g = GemmOp{};
-    g.A = A; g.W = W; g.C = Cc; g.R = R; g.bias = bias; g.scale = nullptr;
-    g.M = (int)M; g.N = N; g.K = taps * cin; g.Min = (int)M + taps - 1; g.Cin = cin; g.taps = taps; g.dil = 1; g.pad = 0; g.ldc = N;
-    g.bias_mod = bias_mod; g.epi = epi; g.a_elu = elu;
-    return launch_gemm(g, 1, st);
-  };
-  auto tcg = [&](const __nv_bfloat16* X, long long M, int cin, int taps, const __nv_bfloat16* W, const float* bias, int N, int bias_mod,
-                 int epi, const float* R, const float* scale, float* of, __nv_bfloat16* oh, int out_elu) {
-    tc::TcOp o{};
-    o.bias = bias; o.R = R; o.scale = scale; o.out_f32 = of; o.out_bf16 = oh;
-    o.c_bs = M * N; o.M = (int)M; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = 1; o.pad = 0;
-    o.bias_mod = bias_mod; o.epi = epi; o.out_elu = out_elu;
-    cudaError_t e = tc::launch(X, M + taps - 1, W, o, 1, st);
-    if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core GEMM (stream, N=%d K=%d): %s", N, o.K, cudaGetErrorString(e));
-    return (int)SOPRO_OK;
-  };
   // ---- RVQ + projection + upsample
   rvq_gather_kernel<<<dim3(n, 1), 256, 0, st>>>(codes, Wd + m->embed, s->S, c.n_q, code_stride, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
   MCK(cudaGetLastError());
-  if ((rc = lin(s->S, n, C, Wd + m->rvq_w, C, s->E, EPI_NONE, nullptr, nullptr))) return rc;
-  const int k0 = c.kernel - 1;
-  float* x = s->XC + (size_t)k0 * C;  // residual stream: the rows behind conv0's context rows
+  if ((rc = gemm_f32({s->S, n, 0, 1}, C, 1, Wd + m->rvq_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, s->E, 0, st))) return rc;
+  float* x = s->XC + (size_t)(c.kernel - 1) * C;  // residual stream: the rows behind conv0's context rows
   upsample_kernel<<<dim3(T2, 1), 256, 0, st>>>(s->E, Wd + m->up_w, x, n, C, s->up_prev);
   MCK(cudaGetLastError());
   MCK(cudaMemcpyAsync(s->up_prev, s->E + (size_t)(n - 1) * C, (size_t)C * 4, cudaMemcpyDeviceToDevice, st));
   // ---- transformer: K/V of the new positions go to the rings, queries attend over the ring
-  const unsigned ln_grid = (unsigned)((T2 + 7) / 8);
-  const size_t asm_bytes = (size_t)8 * (Dh + c.window) * 4;
-  for (size_t li = 0; li < m->layers.size(); ++li) {
-    const sopro_mimi::Layer& L = m->layers[li];
-    float* kr = s->kring + li * (size_t)s->R * C;
-    float* vr = s->vring + li * (size_t)s->R * C;
-    if (tcm) {
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln1w, Wd + L.ln1b, s->LNh, (long long)T2, C, c.norm_eps);
-      if ((rc = tcg(s->LNh, T2, C, 1, Wh + L.qkv_h, nullptr, 3 * C, 3 * C, tc::EPI_NONE, nullptr, nullptr, s->QKV, nullptr, 0))) return rc;
-      rope_kernel<<<dim3(T2, 1), 256, 0, st>>>(s->QKV, m->rope, T2, m->rope_T2, C, H, pos0, kr, vr, s->R);
-      attn_kernel<<<dim3((T2 + 7) / 8, H, 1), 256, asm_bytes, st>>>(s->QKV, s->ATTh, T2, C, H, c.window, pos0, kr, vr, s->R);
-      MCK(cudaGetLastError());
-      if ((rc = tcg(s->ATTh, T2, C, 1, Wh + L.wo_h, nullptr, C, C, tc::EPI_RES_SCALE, x, Wd + L.ls1, x, nullptr, 0))) return rc;
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln2w, Wd + L.ln2b, s->LNh, (long long)T2, C, c.norm_eps);
-      if ((rc = tcg(s->LNh, T2, C, 1, Wh + L.fc1_h, nullptr, FF, FF, tc::EPI_GELU, nullptr, nullptr, nullptr, s->HIDh, 0))) return rc;
-      if ((rc = tcg(s->HIDh, T2, FF, 1, Wh + L.fc2_h, nullptr, C, C, tc::EPI_RES_SCALE, x, Wd + L.ls2, x, nullptr, 0))) return rc;
-    } else {
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln1w, Wd + L.ln1b, s->LN, (long long)T2, C, c.norm_eps);
-      if ((rc = lin(s->LN, T2, C, Wd + L.qkv, 3 * C, s->QKV, EPI_NONE, nullptr, nullptr))) return rc;
-      rope_kernel<<<dim3(T2, 1), 256, 0, st>>>(s->QKV, m->rope, T2, m->rope_T2, C, H, pos0, kr, vr, s->R);
-      attn_kernel<<<dim3((T2 + 7) / 8, H, 1), 256, asm_bytes, st>>>(s->QKV, s->ATT, T2, C, H, c.window, pos0, kr, vr, s->R);
-      MCK(cudaGetLastError());
-      if ((rc = lin(s->ATT, T2, C, Wd + L.wo, C, x, EPI_RES_SCALE, x, Wd + L.ls1))) return rc;
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln2w, Wd + L.ln2b, s->LN, (long long)T2, C, c.norm_eps);
-      if ((rc = lin(s->LN, T2, C, Wd + L.fc1, FF, s->HID, EPI_GELU, nullptr, nullptr))) return rc;
-      if ((rc = lin(s->HID, T2, FF, Wd + L.fc2, C, x, EPI_RES_SCALE, x, Wd + L.ls2))) return rc;
-    }
-  }
-  // ---- SEANet decoder over [context | chunk] buffers
+  const KVRing ring{s->kring, s->vring, s->R, pos0};
+  if ((rc = run_layers(c, m->layers, tcm, Wd, m->dev_h, m->rope, m->rope_T2, x, 1, T2, s->tr, &ring, st))) return rc;
+  // ---- SEANet decoder over [context | chunk] buffers, then every buffer's last context rows move to its front
   TailShift ts{};
-  auto carry = [&](void* base, int row_bytes, int ctx, long long rows) {
-    ts.base[ts.n] = base;
-    ts.row_bytes[ts.n] = row_bytes;
-    ts.ctx[ts.n] = ctx;
-    ts.rows[ts.n] = (int)rows;
-    ++ts.n;
-  };
-  long long Tn = T2;
-  int ch = c.num_filters << c.n_ratios;
-  const int kr3 = c.res_kernel - 1;
-  if (!tcm) {
-    float* a0 = reinterpret_cast<float*>(s->A0);
-    if ((rc = conv(s->XC, Tn, C, c.kernel, Wd + m->c0w, Wd + m->c0b, ch, ch, a0 + (size_t)ch, 0, EPI_NONE, nullptr))) return rc;
-    carry(s->XC, C * 4, k0, Tn);
-    carry(a0, ch * 4, 1, Tn);
-    const float* cur = a0;  // [1 ctx row | Tn rows]
-    for (size_t si = 0; si < m->stages.size(); ++si) {
-      const sopro_mimi::Stage& S = m->stages[si];
-      const bool last = si + 1 == m->stages.size();
-      const int hid = S.cout / c.compress, ctx_o = last ? c.last_kernel - 1 : 1;
-      float* z = reinterpret_cast<float*>(s->Z[si]);
-      float* o = reinterpret_cast<float*>(s->O[si]);
-      if ((rc = conv(cur, Tn, S.cin, 2, Wd + S.tw, Wd + S.tb, S.ratio * S.cout, S.cout, z + (size_t)kr3 * S.cout, 1, EPI_NONE, nullptr))) return rc;
-      Tn *= S.ratio;
-      if ((rc = conv(z, Tn, S.cout, c.res_kernel, Wd + S.r1w, Wd + S.r1b, hid, hid, s->Hs[si], 1, EPI_NONE, nullptr))) return rc;
-      if ((rc = conv(s->Hs[si], Tn, hid, 1, Wd + S.r2w, Wd + S.r2b, S.cout, S.cout, o + (size_t)ctx_o * S.cout, 1, EPI_RES,
-                     z + (size_t)kr3 * S.cout)))
-        return rc;
-      carry(z, S.cout * 4, kr3, Tn);
-      carry(o, S.cout * 4, ctx_o, Tn);
-      cur = o;
-      ch = S.cout;
-    }
-    const int lk = c.last_kernel - 1;
-    final_conv_kernel<<<dim3((unsigned)((Tn + 255) / 256), 1), 256, 0, st>>>(cur + (size_t)lk * ch, Wd + m->lw, Wd + m->lb, wav, Tn, ch,
-                                                                              c.last_kernel, -lk);
-    MCK(cudaGetLastError());
-  } else {
-    if (!tc::supported(ch, c.kernel * C, C) || c.num_filters % 8 || c.last_kernel > 8)
-      return mfail(SOPRO_ERR_UNSUPPORTED, "streaming tensor-core mode: unsupported conv0 / final conv geometry (use SOPRO_MIMI_FP32)");
-    const long long n4 = (long long)T2 * C / 4;
-    cast_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(x, s->XCh + (size_t)k0 * C, n4);
-    MCK(cudaGetLastError());
-    __nv_bfloat16* a0 = reinterpret_cast<__nv_bfloat16*>(s->A0);
-    if ((rc = tcg(s->XCh, Tn, C, c.kernel, Wh + m->c0w_h, Wd + m->c0b, ch, ch, tc::EPI_NONE, nullptr, nullptr, nullptr, a0 + (size_t)ch, 1)))
-      return rc;
-    carry(s->XCh, C * 2, k0, Tn);
-    carry(a0, ch * 2, 1, Tn);
-    const __nv_bfloat16* cur = a0;
-    for (size_t si = 0; si < m->stages.size(); ++si) {
-      const sopro_mimi::Stage& S = m->stages[si];
-      const bool last = si + 1 == m->stages.size();
-      const int hid = S.cout / c.compress, NT = S.ratio * S.cout, ctx_o = last ? c.last_kernel - 1 : 1;
-      if (!tc::supported(NT, 2 * S.cin, S.cin) || !tc::supported(hid, c.res_kernel * S.cout, S.cout) || !tc::supported(S.cout, hid, hid))
-        return mfail(SOPRO_ERR_UNSUPPORTED, "streaming tensor-core mode: unsupported geometry at stage %zu (use SOPRO_MIMI_FP32)", si);
-      const bool fused = tc::resblock_supported(hid, S.cout) && (S.cout * c.res_kernel) % 64 == 0;
-      __nv_bfloat16* zh = reinterpret_cast<__nv_bfloat16*>(s->Z[si]);
-      __nv_bfloat16* oh = reinterpret_cast<__nv_bfloat16*>(s->O[si]);
-      if ((rc = tcg(cur, Tn, S.cin, 2, Wh + S.tw_h, Wd + S.tb, NT, S.cout, tc::EPI_NONE, nullptr, nullptr, s->Zf[si], zh + (size_t)kr3 * S.cout, 1)))
-        return rc;
-      Tn *= S.ratio;
-      if (fused) {
-        tc::ResOp ro{};
-        ro.bias1 = Wd + S.r1b;
-        ro.bias2 = Wd + S.r2b;
-        ro.Z = s->Zf[si];
-        ro.out_f32 = nullptr;
-        ro.out_bf16 = oh + (size_t)ctx_o * S.cout;
-        ro.M = (int)Tn;
-        ro.Min = (int)Tn + kr3;
-        ro.taps = c.res_kernel;
-        ro.pad = 0;
-        ro.out_elu = 1;
-        cudaError_t fe = tc::launch_resblock(zh, Wh + S.r1w_h, Wh + S.r2w_h, hid, ro, 1, st);
-        if (fe != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "fused ResnetBlock (stream, stage %zu): %s", si, cudaGetErrorString(fe));
-      } else {  // conv k=3 -> ELU(h) bf16, then the 1x1 conv + fp32 skip (same two launches as the one-shot decode)
-        __nv_bfloat16* hh = reinterpret_cast<__nv_bfloat16*>(s->Hs[si]);
-        if ((rc = tcg(zh, Tn, S.cout, c.res_kernel, Wh + S.r1w_h, Wd + S.r1b, hid, hid, tc::EPI_NONE, nullptr, nullptr, nullptr, hh, 1))) return rc;
-        if ((rc = tcg(hh, Tn, hid, 1, Wh + S.r2w_h, Wd + S.r2b, S.cout, S.cout, tc::EPI_RES, s->Zf[si], nullptr, nullptr,
-                      oh + (size_t)ctx_o * S.cout, 1)))
-          return rc;
-      }
-      carry(zh, S.cout * 2, kr3, Tn);
-      carry(oh, S.cout * 2, ctx_o, Tn);
-      cur = oh;
-      ch = S.cout;
-    }
-    const int lk = c.last_kernel - 1, per = 256 - lk;
-    final_conv_h_kernel<<<dim3((unsigned)((Tn + per - 1) / per), 1), 256, (size_t)(c.last_kernel * 256 + c.last_kernel * ch) * 4, st>>>(
-        cur + (size_t)lk * ch, Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, -lk);
-    MCK(cudaGetLastError());
-  }
+  if ((rc = tcm ? seanet_tc(m, x, s->sea, 1, T2, &ts, wav, st) : seanet_f32(m, s->sea, 1, T2, &ts, wav, st))) return rc;
   tail_shift_kernel<<<ts.n, 256, 16384, st>>>(ts);
   MCK(cudaGetLastError());
   s->frames += n;
@@ -1324,8 +1288,9 @@ int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_s
   }
   cudaError_t e = cudaMalloc(&s->slab, s->slab_bytes);
   if (e != cudaSuccess) {
+    const size_t mb = s->slab_bytes >> 20;
     delete s;
-    return mfail(SOPRO_ERR_CUDA, "stream state %zu MB: %s", s->slab_bytes >> 20, cudaGetErrorString(e));
+    return mfail(SOPRO_ERR_CUDA, "stream state %zu MB: %s", mb, cudaGetErrorString(e));
   }
   stream_layout(s, s->slab);
   e = cudaMemset(s->slab, 0, s->state_bytes);
@@ -1375,6 +1340,10 @@ int sopro_mimi_decode_step(sopro_mimi_stream_t* s, const int32_t* codes, int n, 
   if (s->precision != s->m->precision)
     return mfail(SOPRO_ERR_STATE, "the decoder's precision changed since this stream started: call sopro_mimi_stream_reset");
   if (2 * (s->frames + n) > 0x3fffffffLL) return mfail(SOPRO_ERR_INVALID, "stream too long");
+  if (s->precision == SOPRO_MIMI_BF16_TC) {
+    const int rc = check_tc_geometry(s->m);
+    if (rc) return rc;
+  }
   MCK(cudaSetDevice(s->m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int64_t hop = sopro_mimi_samples_per_frame(s->m);
@@ -1681,25 +1650,7 @@ int sopro_mimi_encoder_create(const sopro_mimi_config_t* cfg, const sopro_mimi_e
   }
   e->lw = repack_conv(w->last_w, C, ch, cfg->last_kernel);
   e->lb = A.add(w->last_b, C);
-  for (int l = 0; l < NL; ++l) {
-    const sopro_mimi_layer_weights_t& L = w->layer[l];
-    sopro_mimi::Layer d{};
-    d.ln1w = A.add(L.ln1_w, C);
-    d.ln1b = A.add(L.ln1_b, C);
-    std::vector<float> qkv((size_t)3 * C * C);
-    memcpy(qkv.data(), L.q_w, (size_t)C * C * 4);
-    memcpy(qkv.data() + (size_t)C * C, L.k_w, (size_t)C * C * 4);
-    memcpy(qkv.data() + (size_t)2 * C * C, L.v_w, (size_t)C * C * 4);
-    d.qkv = A.add(qkv.data(), qkv.size());
-    d.wo = A.add(L.o_w, (size_t)C * C);
-    d.ls1 = A.add(L.ls1, C);
-    d.ln2w = A.add(L.ln2_w, C);
-    d.ln2b = A.add(L.ln2_b, C);
-    d.fc1 = A.add(L.fc1_w, (size_t)FF * C);
-    d.fc2 = A.add(L.fc2_w, (size_t)C * FF);
-    d.ls2 = A.add(L.ls2, C);
-    e->layers.push_back(d);
-  }
+  for (int l = 0; l < NL; ++l) e->layers.push_back(pack_layer(w->layer[l], C, FF, A, nullptr));
   e->down_w = repack_conv(w->downsample_w, C, C, 4);
   {  // [2*Dc][C]: semantic input_proj rows, then acoustic
     std::vector<float> cat((size_t)2 * Dc * C);
@@ -1744,27 +1695,11 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
   MCK(cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
   const sopro_mimi_config_t& c = e->cfg;
-  const int C = c.hidden, H = c.n_heads, Dh = C / H, FF = c.ffn, Dc = c.codebook_dim;
+  const int C = c.hidden, Dc = c.codebook_dim;
   const EncPlan P = enc_plan(c, n_samples);
   const int T2 = (int)P.len[c.n_ratios], T = (int)P.T;
-  if (e->rope_T2 < T2) {  // RoPE table [cos rows | sin rows], as the decoder's
-    cudaFree(e->rope);
-    e->rope = nullptr;
-    e->rope_T2 = 0;
-    const int cap = std::max(T2, 256);
-    std::vector<float> tab((size_t)2 * cap * (Dh / 2));
-    for (int t = 0; t < cap; ++t)
-      for (int d = 0; d < Dh / 2; ++d) {
-        const float inv = 1.0f / powf(c.rope_theta, (float)(2 * d) / (float)Dh);
-        const float f = (float)t * inv;
-        tab[(size_t)t * (Dh / 2) + d] = cosf(f);
-        tab[(size_t)(cap + t) * (Dh / 2) + d] = sinf(f);
-      }
-    MCK(cudaMalloc(&e->rope, tab.size() * 4));
-    MCK(cudaMemcpyAsync(e->rope, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
-    MCK(cudaStreamSynchronize(st));
-    e->rope_T2 = cap;
-  }
+  int rc;
+  if (e->rope_T2 < T2 && (rc = make_rope(c, std::max(T2, 256), &e->rope, &e->rope_T2, st))) return rc;
   if (e->ws_bytes < P.need) {
     cudaFree(e->ws);
     e->ws = nullptr;
@@ -1779,18 +1714,6 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
   float* x = b2 + P.buf;
   float* ln = x + P.xsz;
   const float* Wd = e->dev;
-  GemmOp g{};
-  // conv over rows [Tin][cin] (row stride cin), `taps` taps, left pad `pad` rows, M output rows
-  auto conv = [&](const float* A, long long Tin, long long M, int cin, int taps, int pad, const float* W, const float* bias, int N,
-                  float* Cc, int elu, int epi, const float* R, const float* scale) {
-    g = GemmOp{};
-    g.A = A; g.W = W; g.C = Cc; g.R = R; g.bias = bias; g.scale = scale;
-    g.M = (int)M; g.N = N; g.K = taps * cin; g.Min = (int)Tin; g.Cin = cin; g.taps = taps; g.dil = 1; g.pad = pad; g.ldc = N;
-    g.bias_mod = N; g.epi = epi; g.a_elu = elu;
-    g.a_bs = Tin * cin; g.c_bs = M * N; g.r_bs = M * N;
-    return launch_gemm(g, 1, st);
-  };
-  int rc;
   // ---- SEANet encoder
   float* cur = b0;   // stage input [len][ch]
   float* hid = b1;   // resblock hidden [len][ch/2]
@@ -1806,35 +1729,25 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
     const long long Ls = P.len[s], Lp = P.padded[s];
     const int r = S.ratio;
     // ResnetBlock (:412-451): x + conv1(ELU(conv3(ELU(x))))
-    if ((rc = conv(cur, Ls, Ls, ch, c.res_kernel, c.res_kernel - 1, Wd + S.r1w, Wd + S.r1b, ch / 2, hid, 1, EPI_NONE, nullptr, nullptr))) return rc;
-    if ((rc = conv(hid, Ls, Ls, ch / 2, 1, 0, Wd + S.r2w, Wd + S.r2b, ch, cur, 1, EPI_RES, cur, nullptr))) return rc;
+    if ((rc = gemm_f32({cur, Ls, 0, 1}, ch, c.res_kernel, Wd + S.r1w, Wd + S.r1b, ch / 2, ch / 2, EPI_NONE, nullptr, nullptr, hid, 1, st)))
+      return rc;
+    if ((rc = gemm_f32({hid, Ls, 0, 1}, ch / 2, 1, Wd + S.r2w, Wd + S.r2b, ch, ch, EPI_RES, cur, nullptr, cur, 1, st))) return rc;
     // ELU + conv kernel 2r stride r: zero rows up to a multiple of r, then 2 taps over [Lp/r][r*ch]
     if (Lp > Ls) MCK(cudaMemsetAsync(cur + (size_t)Ls * ch, 0, (size_t)(Lp - Ls) * ch * 4, st));
-    if ((rc = conv(cur, Lp / r, Lp / r, r * ch, 2, 1, Wd + S.dw, Wd + S.db, 2 * ch, nxt, 1, EPI_NONE, nullptr, nullptr))) return rc;
+    if ((rc = gemm_f32({cur, Lp / r, 0, 1}, r * ch, 2, Wd + S.dw, Wd + S.db, 2 * ch, 2 * ch, EPI_NONE, nullptr, nullptr, nxt, 1, st)))
+      return rc;
     std::swap(cur, nxt);
     ch *= 2;
   }
   // ELU + conv k3 -> residual stream x [T2][C]
-  if ((rc = conv(cur, T2, T2, ch, c.last_kernel, c.last_kernel - 1, Wd + e->lw, Wd + e->lb, C, x, 1, EPI_NONE, nullptr, nullptr))) return rc;
+  if ((rc = gemm_f32({cur, T2, 0, 1}, ch, c.last_kernel, Wd + e->lw, Wd + e->lb, C, C, EPI_NONE, nullptr, nullptr, x, 1, st))) return rc;
   // ---- encoder transformer (MimiTransformerLayer.forward :966-993), fp32 path of the decoder
-  {
-    const unsigned ln_grid = (unsigned)((T2 + 7) / 8);
-    const size_t asm_bytes = (size_t)8 * (Dh + c.window) * 4;
-    auto lin = [&](const float* A, int K, const float* W, int N, float* Cc, int epi, const float* R, const float* scale) {
-      return conv(A, T2, T2, K, 1, 0, W, nullptr, N, Cc, 0, epi, R, scale);
-    };
-    for (const sopro_mimi::Layer& L : e->layers) {
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln1w, Wd + L.ln1b, ln, (long long)T2, C, c.norm_eps);
-      if ((rc = lin(ln, C, Wd + L.qkv, 3 * C, b0, EPI_NONE, nullptr, nullptr))) return rc;
-      rope_kernel<<<dim3(T2, 1), 256, 0, st>>>(b0, e->rope, T2, e->rope_T2, C, H, 0, nullptr, nullptr, 1);
-      attn_kernel<<<dim3((T2 + 7) / 8, H, 1), 256, asm_bytes, st>>>(b0, b1, T2, C, H, c.window, 0, nullptr, nullptr, 1);
-      MCK(cudaGetLastError());
-      if ((rc = lin(b1, C, Wd + L.wo, C, x, EPI_RES_SCALE, x, Wd + L.ls1))) return rc;
-      layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln2w, Wd + L.ln2b, ln, (long long)T2, C, c.norm_eps);
-      if ((rc = lin(ln, C, Wd + L.fc1, FF, b0, EPI_GELU, nullptr, nullptr))) return rc;
-      if ((rc = lin(b0, FF, Wd + L.fc2, C, x, EPI_RES_SCALE, x, Wd + L.ls2))) return rc;
-    }
-  }
+  LayerBufs lb{};
+  lb.ln = ln;
+  lb.qkv = b0;
+  lb.att = b1;
+  lb.hid = b0;
+  if ((rc = run_layers(c, e->layers, false, Wd, nullptr, e->rope, e->rope_T2, x, 1, T2, lb, nullptr, st))) return rc;
   // ---- 25 -> 12.5 Hz: kernel 4, stride 2, no bias, replicate padding (2 rows left, 0 or 1 right)
   {
     const int rows = 2 * T + 2;
@@ -1842,9 +1755,10 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
     replicate_pad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(x, b0, T2, C, 2, rows);
     MCK(cudaGetLastError());
     float* lat = latent ? latent : b1;
-    if ((rc = conv(b0, rows / 2, T, 2 * C, 2, 0, Wd + e->down_w, nullptr, C, lat, 0, EPI_NONE, nullptr, nullptr))) return rc;
+    // 2 taps over the T + 1 row pairs [rows/2][2C]: the first pair (the left padding) is the context of output row 0
+    if ((rc = gemm_f32({b0, T, 1, 1}, 2 * C, 2, Wd + e->down_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, lat, 0, st))) return rc;
     // ---- quantizer: both input projections in one GEMM, then the residual search
-    if ((rc = conv(lat, T, T, C, 1, 0, Wd + e->inproj, nullptr, 2 * Dc, b2, 0, EPI_NONE, nullptr, nullptr))) return rc;
+    if ((rc = gemm_f32({lat, T, 0, 1}, C, 1, Wd + e->inproj, nullptr, 2 * Dc, 2 * Dc, EPI_NONE, nullptr, nullptr, b2, 0, st))) return rc;
     rvq_encode_kernel<8><<<T, 256, 0, st>>>(b2, Wd + e->embed, codes, T, c.n_q, c.n_sem, c.vocab);
     MCK(cudaGetLastError());
   }

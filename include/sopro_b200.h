@@ -538,6 +538,26 @@ int sopro_debug_tc_gemm(const void* X, int B, int64_t rows, int cin, int taps, i
                         const float* bias, int bias_mod, int epi, const float* R, const float* scale, float* out_f32,
                         void* out_bf16, int out_elu, void* stream);
 
+/* test hooks: single tensor-core-mode kernels of the Mimi decoder (no reference counterpart).  Device pointers, no
+ * allocation; a shape the kernel does not take returns SOPRO_ERR_INVALID and launches nothing.
+ *
+ * sliding-window attention: q, k bf16 [B][T2][C] (rotated), vt bf16 [B][C][T2p] (v transposed, T2p >= T2 and a multiple
+ * of 8), out bf16 [B][T2][C]; C = 64*H, 1 <= window <= 257; query i attends to keys (i - window, i]. */
+int sopro_debug_tc_attn(const void* q, const void* k, const void* vt, void* out, int B, int T2, int64_t T2p, int C, int H, int window,
+                        void* stream);
+/* fused ResnetBlock: out = Z + W2 . bf16(ELU(conv_taps(X; W1) + bias1)) + bias2.  X bf16 [B][ctx + M][2*hid] (its first
+ * ctx rows are left context, 0 <= ctx <= taps-1; the causal zero pad supplies the other taps-1-ctx rows), W1 bf16
+ * [hid][taps*2*hid], W2 bf16 [2*hid][hid], bias1 [hid], bias2 [2*hid], Z fp32 [B][M][2*hid]; out_f32 / out_bf16
+ * [B][M][2*hid], either may be null, out_elu applies ELU to the bf16 copy only.  hid in {32, 64, 128}, 2*hid*taps a
+ * multiple of 64. */
+int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2, const float* Z,
+                            float* out_f32, void* out_bf16, int B, int M, int ctx, int hid, int taps, int out_elu, void* stream);
+/* attention operands from fp32 QKV rows [B][T2][3C]: rotated q -> qh, rotated k -> kh (bf16 [B][T2][C]), v -> vt (bf16
+ * [B][C][T2p], T2p = T2 rounded up to 8, pad columns zero).  table: RoPE table of tab_T2 >= T2 positions,
+ * [cos rows 0..tab_T2) | sin rows 0..tab_T2)] of 32 floats each; C = 64*H. */
+int sopro_debug_rope_pack(const float* qkv, const float* table, int tab_T2, void* qh, void* kh, void* vt, int B, int T2, int C, int H,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -210,7 +210,14 @@ def _bf(x: Tensor) -> Tensor:
     return x.to(torch.bfloat16).to(torch.float32)
 
 
-def transformer_bf16_operands(sd: SD, x: Tensor, n_layers: int = 8, n_heads: int = 8, window: int = 250, eps: float = 1e-5) -> Tensor:
+def transformer_bf16_operands(sd: SD, x: Tensor, n_layers: int = 8, n_heads: int = 8, window: int = 250, eps: float = 1e-5,
+                              attention: str = "tc") -> Tensor:
+    """attention="tc": the one-shot decode's tensor-core attention (rope_pack_kernel + attn_tc_kernel): q / k / v rounded
+    to bf16, probabilities rounded to bf16 before they are summed.  attention="fp32": the tensor-core stream's attention
+    (rope_kernel + attn_kernel over the K/V ring): RoPE and softmax in fp32 on the fp32 q / k / v, unrounded
+    probabilities.  Both round the attention output to bf16 (the operand of o_proj)."""
+    if attention not in ("tc", "fp32"):
+        raise ValueError(f"attention must be 'tc' or 'fp32', got {attention!r}")
     B, T, C = x.shape
     Dh = C // n_heads
     i = torch.arange(T)
@@ -221,11 +228,15 @@ def transformer_bf16_operands(sd: SD, x: Tensor, n_layers: int = 8, n_heads: int
         sp = lambda t: t.view(B, T, n_heads, Dh).transpose(1, 2)  # noqa: E731
         q, k, v = (sp(F.linear(h, _bf(sd[p + f"self_attn.{n}_proj.weight"]))) for n in ("q", "k", "v"))
         q, k = rope(q, k)
-        q, k, v = _bf(q), _bf(k), _bf(v)
-        s = torch.matmul(q, k.transpose(2, 3)) * (1.0 / math.sqrt(Dh))
-        s = s.masked_fill(~allowed, float("-inf"))
-        pr = _bf(torch.exp(s - s.amax(dim=-1, keepdim=True)))  # probabilities are rounded BEFORE they are summed
-        a = torch.matmul(pr, v) / pr.sum(dim=-1, keepdim=True)
+        if attention == "tc":
+            q, k, v = _bf(q), _bf(k), _bf(v)
+            s = torch.matmul(q, k.transpose(2, 3)) * (1.0 / math.sqrt(Dh))
+            s = s.masked_fill(~allowed, float("-inf"))
+            pr = _bf(torch.exp(s - s.amax(dim=-1, keepdim=True)))  # probabilities are rounded BEFORE they are summed
+            a = torch.matmul(pr, v) / pr.sum(dim=-1, keepdim=True)
+        else:
+            s = torch.matmul(q, k.transpose(2, 3)) * (1.0 / math.sqrt(Dh))
+            a = torch.matmul(F.softmax(s.masked_fill(~allowed, float("-inf")), dim=-1), v)
         a = _bf(a).transpose(1, 2).contiguous().view(B, T, C)
         x = x + sd[p + "self_attn_layer_scale.scale"] * F.linear(a, _bf(sd[p + "self_attn.o_proj.weight"]))
         h = _bf(F.layer_norm(x, (C,), sd[p + "post_attention_layernorm.weight"], sd[p + "post_attention_layernorm.bias"], eps))
@@ -247,7 +258,8 @@ def seanet_decoder_bf16_operands(sd: SD, x: Tensor) -> Tensor:
     return conv1d_causal(a, sd[f"decoder.layers.{li + 1}.conv.weight"], sd[f"decoder.layers.{li + 1}.conv.bias"])
 
 
-def mimi_decode_bf16_operands(sd: SD, codes_bqt: Tensor) -> Tensor:
+def mimi_decode_bf16_operands(sd: SD, codes_bqt: Tensor, attention: str = "tc") -> Tensor:
+    """attention="tc" models the one-shot tensor-core decode, "fp32" the tensor-core stream (transformer_bf16_operands)."""
     x = upsample(sd, rvq_decode(sd, codes_bqt))  # fp32 in both modes of the product
-    x = transformer_bf16_operands(sd, x)
+    x = transformer_bf16_operands(sd, x, attention=attention)
     return seanet_decoder_bf16_operands(sd, x).transpose(1, 2)

@@ -1414,6 +1414,54 @@ int sopro_debug_tc_gemm(const void* X, int B, int64_t rows, int cin, int taps, i
   return SOPRO_OK;
 }
 
+int sopro_debug_tc_attn(const void* q, const void* k, const void* vt, void* out, int B, int T2, int64_t T2p, int C, int H, int window,
+                        void* stream) {
+  if (!q || !k || !vt || !out) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535 || T2 < 1 || T2p < T2 || T2p % 8 != 0 || !tc::attn_supported(C, H, window))
+    return mfail(SOPRO_ERR_INVALID, "tc attention: unsupported shape (B=%d T2=%d T2p=%lld C=%d H=%d window=%d)", B, T2, (long long)T2p,
+                 C, H, window);
+  cudaError_t e = tc::launch_attn(q, k, vt, static_cast<__nv_bfloat16*>(out), B, T2, T2p, C, H, window,
+                                  reinterpret_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core attention launch: %s", cudaGetErrorString(e));
+  return SOPRO_OK;
+}
+
+int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2, const float* Z,
+                            float* out_f32, void* out_bf16, int B, int M, int ctx, int hid, int taps, int out_elu, void* stream) {
+  if (!X || !W1 || !W2 || !bias1 || !bias2 || !Z || (!out_f32 && !out_bf16)) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535 || M < 1 || taps < 1 || ctx < 0 || ctx > taps - 1 || (long long)M + ctx > 0x7fffffffLL ||
+      !tc::resblock_supported(hid, 2 * hid) || (2 * hid * taps) % 64 != 0)
+    return mfail(SOPRO_ERR_INVALID, "fused ResnetBlock: unsupported shape (B=%d M=%d ctx=%d hid=%d taps=%d)", B, M, ctx, hid, taps);
+  // the operand geometry of seanet_tc: ctx context rows in front of the M rows, the causal zero pad covers the rest
+  tc::ResOp ro{};
+  ro.bias1 = bias1;
+  ro.bias2 = bias2;
+  ro.Z = Z;
+  ro.out_f32 = out_f32;
+  ro.out_bf16 = static_cast<__nv_bfloat16*>(out_bf16);
+  ro.M = M;
+  ro.Min = M + ctx;
+  ro.taps = taps;
+  ro.pad = taps - 1 - ctx;
+  ro.out_elu = out_elu;
+  cudaError_t e = tc::launch_resblock(X, W1, W2, hid, ro, B, reinterpret_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "fused ResnetBlock launch: %s", cudaGetErrorString(e));
+  return SOPRO_OK;
+}
+
+int sopro_debug_rope_pack(const float* qkv, const float* table, int tab_T2, void* qh, void* kh, void* vt, int B, int T2, int C, int H,
+                          void* stream) {
+  if (!qkv || !table || !qh || !kh || !vt) return mfail(SOPRO_ERR_INVALID, "null argument");
+  const size_t pack_bytes = (size_t)32 * (C + 2) * 2;
+  if (B < 1 || B > 65535 || T2 < 1 || tab_T2 < T2 || H < 1 || C != H * tc::kAttnDh || pack_bytes > 48 * 1024)
+    return mfail(SOPRO_ERR_INVALID, "rope pack: unsupported shape (B=%d T2=%d tab_T2=%d C=%d H=%d)", B, T2, tab_T2, C, H);
+  const long long T2p = (T2 + 7) / 8 * 8;  // as run_layers pitches v^T
+  rope_pack_kernel<tc::kAttnDh><<<dim3((T2 + 31) / 32, B), 256, pack_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(
+      qkv, table, static_cast<__nv_bfloat16*>(qh), static_cast<__nv_bfloat16*>(kh), static_cast<__nv_bfloat16*>(vt), T2, T2p, tab_T2, C, H);
+  MCK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
 int sopro_mimi_decode_host(sopro_mimi_t* m, const int32_t* codes_host, int B, int T, float* wav_host, void* stream) {
   if (!m || !codes_host || !wav_host) return mfail(SOPRO_ERR_INVALID, "null argument");
   MCK(cudaSetDevice(m->device));

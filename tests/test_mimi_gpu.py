@@ -9,6 +9,24 @@ pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 _ENG = {}
 
+# Tensor-core mode against oracle.mimi_decode_bf16_operands, the model of the mode's own bf16 rounding: max distance as
+# a fraction of the model waveform's peak, RMS distance as a fraction of its RMS.  attention="tc" models the one-shot
+# decode, attention="fp32" the stream.  Measured on an H100 80GB HBM3 at a 700 W power limit: one-shot max 4.2e-3 ..
+# 5.5e-3, rms 5.0e-3 .. 5.2e-3 (six shapes below, and frames [0, 300) of the 10k-frame decode); stream max 5.1e-3, rms
+# 5.0e-3.  That is as far as the fp32 oracle, not the "accumulation order only" distance one might expect: every SEANet
+# stage re-rounds its activations to bf16, so any difference in fp32 summation order (GPU vs CPU) decorrelates the
+# roundings by the waveform.  The model itself moves as far when only its accumulation goes from fp32 to fp64
+# (DESIGN.md section 7).  So these bounds are ~2-3x the worst measurement and no waveform-level bound can see a window
+# one key off (8e-4 of the peak); tests/test_mimi_tc_kernels_gpu.py checks the kernels where that bug lives.
+TC_MODEL_MAX, TC_MODEL_RMS = 1.5e-2, 1e-2
+STREAM_MODEL_MAX, STREAM_MODEL_RMS = 1.5e-2, 1e-2
+
+
+def _model_distance(got, model):
+    """(max |got - model| / peak(model), rms(got - model) / rms(model))"""
+    d = got.cpu().reshape(model.shape) - model
+    return float(d.abs().max()) / float(model.abs().max()), float(d.pow(2).mean().sqrt()) / float(model.pow(2).mean().sqrt())
+
 
 def _engine(precision="fp32"):
     from sopro_b200.codec import MimiEngine
@@ -36,7 +54,11 @@ def test_decode_matches_oracle(B, T):
 @pytest.mark.parametrize("B,T", [(1, 1), (2, 9), (1, 37), (3, 16), (1, 150), (2, 203)])
 def test_decode_tensor_core_mode(B, T):
     """Default mode: bf16 operands on the tensor cores, fp32 accumulation.  Stated tolerance: max error
-    2e-2 of the waveform's peak and relative RMS error 1e-2 against the fp32 oracle."""
+    2e-2 of the waveform's peak and relative RMS error 1e-2 against the fp32 oracle.  Against the model of this mode's
+    rounding (oracle.mimi_decode_bf16_operands): max 1.5e-2 of the peak and relative RMS 1e-2 (TC_MODEL_MAX /
+    TC_MODEL_RMS; measured on an H100 at 700 W: max <= 5.5e-3, rms <= 5.2e-3 over these six shapes).  The model is no
+    closer than the fp32 oracle at the waveform: the SEANet's bf16 re-rounding turns the GPU's other fp32 summation
+    order into a distance as large as the rounding itself (see TC_MODEL_MAX)."""
     eng, sd = _engine("bf16_tc")
     codes = torch.randint(0, 2048, (B, 32, T), generator=torch.Generator().manual_seed(100 + T))
     want = M.mimi_decode(sd, codes)
@@ -44,22 +66,21 @@ def test_decode_tensor_core_mode(B, T):
     assert got.shape == want.shape and bool(torch.isfinite(got).all())
     peak = float(want.abs().max())
     err = got - want
+    emu = M.mimi_decode_bf16_operands(sd, codes)
+    dmax, drms = _model_distance(got, emu)
+    print(f"tensor-core mode B={B} T={T}: max err vs fp32 oracle {float(err.abs().max()) / peak:.2e} of peak; "
+          f"vs bf16-operand model max {dmax:.2e} of peak, rms {drms:.2e} of rms")
     assert float(err.abs().max()) <= 2e-2 * peak, (float(err.abs().max()), peak)
     assert float(err.pow(2).mean().sqrt()) <= 1e-2 * float(want.pow(2).mean().sqrt())
-    # against the bf16-operand model of this mode (oracle/mimi_oracle.py) the distance should be far smaller (accumulation
-    # order + rare bf16 rounding flips); reported here, to be tightened into the bound once it has GPU history
-    emu = M.mimi_decode_bf16_operands(sd, codes)
-    d = float((got - emu).abs().max())
-    print(f"tensor-core mode B={B} T={T}: max err vs fp32 oracle {float(err.abs().max()) / peak:.2e} of peak, "
-          f"vs bf16-operand model {d / peak:.2e} of peak")
-    assert d <= 2.6e-2 * peak
+    assert dmax <= TC_MODEL_MAX and drms <= TC_MODEL_RMS, (dmax, drms)
 
 
 def test_full_size_decode_properties():
     """BASELINE.json's standalone configuration (10k frames) through size-independent properties: the decoder is
     causal, so the first 300 frames of the 10k-frame waveform equal a 300-frame decode bit for bit (same kernels, other
     grid sizes); the tensor-core result stays within the stated tolerance of the fp32 mode at full size; a batch of 25
-    x 400 frames equals the same utterances decoded one by one."""
+    x 400 frames equals the same utterances decoded one by one.  Frames [0, 300) are also held to the bounds against the
+    model of the mode's rounding (TC_MODEL_MAX / TC_MODEL_RMS)."""
     eng, _ = _engine("bf16_tc")
     codes = torch.randint(0, 2048, (1, 32, 10000), generator=torch.Generator().manual_seed(5))
     big = eng.decode(codes)
@@ -83,6 +104,9 @@ def test_full_size_decode_properties():
         print(f"10k-frame decode vs oracle, frames [{lo},{hi}): tensor-core {e_tc / peak:.2e} of peak, fp32 {e_32 / peak:.2e} of peak")
         assert e_tc <= 2e-2 * peak, (lo, hi, e_tc, peak)
         assert e_32 <= 2e-4 * max(1.0, peak), (lo, hi, e_32, peak)
+    dmax, drms = _model_distance(big[..., : 300 * 1920], M.mimi_decode_bf16_operands(_ENG["sd"], codes[:, :, :300]))
+    print(f"10k-frame decode vs bf16-operand model, frames [0,300): max {dmax:.2e} of peak, rms {drms:.2e} of rms")
+    assert dmax <= TC_MODEL_MAX and drms <= TC_MODEL_RMS, (dmax, drms)
     batch = codes.view(1, 32, 25, 400).permute(2, 1, 0, 3).reshape(25, 32, 400).contiguous()
     wb = eng.decode(batch)
     for i in (0, 11, 24):
@@ -208,8 +232,12 @@ def test_stream_decode_step_equals_the_full_decode(mode):
     the default 6, 16, a 40-frame chunk that is split internally, ...) over 310 frames -- 620 transformer positions,
     far past the 250-position window and past the ring's wrap-around -- concatenate to the one-shot decode.  fp32
     mode: bit for bit (every output element is computed in the same order).  Tensor-core mode: the dense blocks are the
-    same tensor-core tiles, only the attention core runs in fp32 on the ring; the stated tolerance is 1e-2 of the peak vs the
-    one-shot tensor-core decode and the mode's 2e-2 vs the fp32 oracle."""
+    same tensor-core tiles, only the attention core runs in fp32 on the ring.  Every kernel of the tensor-core stream is
+    row-local with a fixed summation order, so one-frame chunks give the ragged schedule's output bit for bit; against
+    the model of the stream's rounding (oracle.mimi_decode_bf16_operands(attention="fp32")) the first 150 frames are
+    held to max 1.5e-2 of the peak and relative RMS 1e-2 (STREAM_MODEL_MAX / STREAM_MODEL_RMS; measured on an H100 at
+    700 W: max 5.1e-3, rms 5.0e-3), and to the mode's 2e-2 vs the fp32 oracle.  The distance to the one-shot
+    tensor-core decode (the two attention roundings differ; measured 5.3e-3) is reported and held to 1e-2 of the peak."""
     eng, sd = _engine(mode)
     T = 310
     codes = torch.randint(0, 2048, (1, 32, T), generator=torch.Generator().manual_seed(77))
@@ -231,9 +259,15 @@ def test_stream_decode_step_equals_the_full_decode(mode):
     if mode == "fp32":
         assert torch.equal(got, full)
     else:
-        assert err <= 1e-2 * peak, (err, peak)
+        ones = eng.stream(16)
+        one_by_one = torch.cat([ones.step(codes[0, :, t:t + 1]) for t in range(T)], dim=1)
+        assert torch.equal(one_by_one, got), f"chunk schedules differ at {int((one_by_one != got).sum())} samples"
+        dmax, drms = _model_distance(got[:, : 150 * 1920], M.mimi_decode_bf16_operands(sd, codes[:, :, :150], attention="fp32"))
+        print(f"stream [{mode}] vs its bf16-operand model (fp32 attention), frames [0,150): max {dmax:.2e} of peak, rms {drms:.2e} of rms")
+        assert dmax <= STREAM_MODEL_MAX and drms <= STREAM_MODEL_RMS, (dmax, drms)
         want = M.mimi_decode(sd, codes[:, :, :150]).reshape(1, -1)
         assert float((got[:, : 150 * 1920].cpu() - want).abs().max()) <= 2e-2 * float(want.abs().max())
+        assert err <= 1e-2 * peak, (err, peak)
     # reset -> the same stream object decodes a new utterance from frame 0; host-buffer entry point
     st.reset()
     assert st.frames == 0

@@ -74,6 +74,38 @@ def test_bf16_operand_model_stays_near_the_fp32_restatement():
     assert abs(err1 - 8.16e-4) <= 1e-4  # the error the tensor-core mode shows on these codes on an H100 (smoke())
 
 
+def test_bf16_operand_model_attention_switch():
+    """transformer_bf16_operands(attention=...): "tc" (the default) models the one-shot decode's tensor-core attention and
+    reproduces the model as it was before the switch existed: tests/golden/mimi_bf16_model_transformer.npz holds its
+    output on 12 positions with a 5-position window (so the mask matters), written by that earlier version.  The bound
+    1e-5 of the scale only absorbs another CPU's matmul order; the two attention models sit ~4e-4 apart on this input.
+    "fp32" models the tensor-core stream (unrounded q / k / v / probabilities) and must differ from "tc"."""
+    import os
+
+    import numpy as np
+
+    sd = M.synth_mimi_state_dict()
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "mimi_bf16_model_transformer.npz"))
+    x, old = torch.from_numpy(g["x"]), torch.from_numpy(g["y"])
+    dflt = M.transformer_bf16_operands(sd, x, window=5)
+    tc = M.transformer_bf16_operands(sd, x, window=5, attention="tc")
+    f32 = M.transformer_bf16_operands(sd, x, window=5, attention="fp32")
+    assert torch.equal(dflt, tc)
+    scale = float(old.abs().max())
+    d_old = float((tc - old).abs().max())
+    print(f"attention='tc' vs the fixture: {d_old / scale:.1e} of scale (bit-equal: {torch.equal(tc, old)})")
+    assert d_old <= 1e-5 * scale
+    assert float((f32 - tc).abs().max()) >= 1e-4 * scale
+    # the "fp32" model is causal: a prefix of the positions gives the prefix of the output
+    assert torch.equal(M.transformer_bf16_operands(sd, x[:, :7], window=5, attention="fp32"), f32[:, :7])
+    # the decode-level switch passes through; an unknown name is refused
+    codes = torch.randint(0, 2048, (1, 32, 3), generator=torch.Generator().manual_seed(2))
+    assert torch.equal(M.mimi_decode_bf16_operands(sd, codes), M.mimi_decode_bf16_operands(sd, codes, attention="tc"))
+    assert not torch.equal(M.mimi_decode_bf16_operands(sd, codes, attention="fp32"), M.mimi_decode_bf16_operands(sd, codes))
+    with pytest.raises(ValueError):
+        M.transformer_bf16_operands(sd, x, attention="bf16")
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # ENCODE path
 # ---------------------------------------------------------------------------------------------------------------

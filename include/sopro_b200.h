@@ -558,6 +558,49 @@ int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const
 int sopro_debug_rope_pack(const float* qkv, const float* table, int tab_T2, void* qh, void* kh, void* vt, int B, int T2, int C, int H,
                           void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Output resampling (no reference counterpart: the reference always returns 24 kHz): band-limited resampling of a
+ * waveform from sr_in to sr_out with torchaudio.functional.resample's default filter (sinc_interp_hann,
+ * lowpass_filter_width 6, rolloff 0.99).  With g = gcd(sr_in, sr_out), o = sr_in / g, n = sr_out / g,
+ * base = 0.99 * min(o, n), width = ceil(6 o / base): output j = q n + p is sum_i k[p][i] * x[q o - width + i] over the
+ * phase's nonzero taps (x = 0 outside [0, N)), ceil(n N / o) outputs.  Supported: integer rates in [4000, 192000], unequal,
+ * whose reduced o and n are both <= 4096; anything else is SOPRO_ERR_INVALID before any allocation or launch.
+ * fp32 accumulation, one FMA chain per output in increasing input index, shared by the one-shot and the stream paths. */
+typedef struct sopro_resampler sopro_resampler_t;
+typedef struct sopro_resampler_stream sopro_resampler_stream_t;
+/* host-only: the filter.  geometry [4] HOST out = (o, n, width, S), S = the longest nonzero span; when non-NULL,
+ * first [n], span [n] (i32) and taps [n][S] (f32, zero past each span) receive phase p's nonzero taps
+ * k[p][first[p] .. first[p] + span[p]) (evaluated in double, rounded to fp32 once). */
+int sopro_resampler_filter(int32_t sr_in, int32_t sr_out, int32_t* geometry, int32_t* first, int32_t* span, float* taps);
+/* host-only: ceil(n * n_in / o), the outputs of n_in input samples; < 0 for a refused rate pair or n_in < 0 */
+int64_t sopro_resampled_length(int32_t sr_in, int32_t sr_out, int64_t n_in);
+int sopro_resampler_create(int32_t sr_in, int32_t sr_out, int device, sopro_resampler_t** out);
+/* (destroy a resampler's streams first) */
+int sopro_resampler_destroy(sopro_resampler_t* r);
+/* one-shot, ragged batch: row b of x [B][x_stride] f32 (device) has lens_host[b] samples (HOST i64; NULL = x_stride each);
+ * samples at or past lens[b] are not read.  Row b's ceil(n lens[b] / o) outputs go to y + b * y_stride (device; y_stride
+ * >= the longest row's outputs when B > 1); the rest of the row is not written.  Row b equals that row resampled alone. */
+int sopro_resample(sopro_resampler_t* r, const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, float* y,
+                   int64_t y_stride, void* stream);
+/* Streaming: one utterance pushed in chunks of at most max_chunk samples.  After N input samples the pushes have emitted
+ * n * max(0, floor((N - width) / o)) outputs -- every block whose whole window [q o - width, q o + width + o) has arrived --
+ * and finish emits the rest up to ceil(n N / o).  The concatenated outputs equal sopro_resample of the concatenated input
+ * bit for bit, under any chunk schedule.  The state carries fewer than 2 width + o input samples on the device; output
+ * counts are host arithmetic (no call synchronises).  Calls on one stream state must be ordered (one CUDA stream). */
+int sopro_resampler_stream_create(sopro_resampler_t* r, int64_t max_chunk, sopro_resampler_stream_t** out);
+int sopro_resampler_stream_destroy(sopro_resampler_stream_t* s);
+/* back to sample 0 (host-only; also clears the finished state) */
+int sopro_resampler_stream_reset(sopro_resampler_stream_t* s);
+/* outputs the next call writes: a push of n_more samples (final == 0), or a push of n_more samples followed by finish
+ * (final != 0); < 0 on bad arguments or after finish */
+int64_t sopro_resampler_stream_ready(const sopro_resampler_stream_t* s, int64_t n_more, int final);
+/* x [n] f32 (device) -> y (device) receives stream_ready(s, n, 0) outputs.  n > max_chunk: SOPRO_ERR_INVALID, nothing
+ * launched, state unchanged.  After finish: SOPRO_ERR_STATE until a reset. */
+int sopro_resampler_push(sopro_resampler_stream_t* s, const float* x, int64_t n, float* y, void* stream);
+/* the remaining stream_ready(s, 0, 1) outputs (the input's end is zero padded) -> y (device); SOPRO_ERR_STATE when
+ * called twice without a reset */
+int sopro_resampler_finish(sopro_resampler_stream_t* s, float* y, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

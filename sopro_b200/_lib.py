@@ -204,6 +204,17 @@ SYMBOLS = {
     "sopro_debug_tc_attn": (_I, [_VP, _VP, _VP, _VP, _I, _I, C.c_int64, _I, _I, _I, _VP]),
     "sopro_debug_tc_resblock": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "sopro_debug_rope_pack": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
+    "sopro_resampler_filter": (_I, [C.c_int32, C.c_int32, _I32P, _I32P, _I32P, _VP]),
+    "sopro_resampled_length": (C.c_int64, [C.c_int32, C.c_int32, C.c_int64]),
+    "sopro_resampler_create": (_I, [C.c_int32, C.c_int32, _I, C.POINTER(_VP)]),
+    "sopro_resampler_destroy": (_I, [_VP]),
+    "sopro_resample": (_I, [_VP, _VP, C.c_int32, C.c_int64, _VP, _VP, C.c_int64, _VP]),
+    "sopro_resampler_stream_create": (_I, [_VP, C.c_int64, C.POINTER(_VP)]),
+    "sopro_resampler_stream_destroy": (_I, [_VP]),
+    "sopro_resampler_stream_reset": (_I, [_VP]),
+    "sopro_resampler_stream_ready": (C.c_int64, [_VP, C.c_int64, _I]),
+    "sopro_resampler_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP]),
+    "sopro_resampler_finish": (_I, [_VP, _VP, _VP]),
 }
 
 _lib = None

@@ -25,6 +25,7 @@ from .engine import ArEngine, ArSession, Sampling
 from .nar import NarEngine
 from .prefill_cuda import PrefillEngine, RefPrepEngine
 from .prefill import PreparedReference
+from .resample import Resampler, check_rates
 from .weights import load_safetensors, read_safetensors_cfg
 
 
@@ -510,6 +511,7 @@ class SoproTTS:
         self.tokenizer = tokenizer
         self.codec = codec
         self.device = torch.device(device)
+        self._resamplers: Dict[int, Resampler] = {}  # output rate -> its resampler (tap table on the device)
 
     # ---- construction
     @classmethod
@@ -579,7 +581,10 @@ class SoproTTS:
                    ref_tokens_tq: Optional[torch.Tensor] = None, max_frames: int = 400, top_p: float = 0.9,
                    temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                    ref_seconds: Optional[float] = None, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-                   generator: Optional[torch.Generator] = None) -> torch.Tensor:
+                   generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None) -> torch.Tensor:
+        """-> [1, 1, N] f32 on the device.  `sample_rate` (extension): the output rate in Hz (None = 24 kHz, the codec's
+        own); another rate resamples the decoded waveform on the GPU (sopro_b200/resample.py)."""
+        rs = self._resampler(sample_rate)  # a refused rate raises before any work
         text_ids = self.encode_text(text)
         if ref is None:
             ref = self.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
@@ -587,14 +592,18 @@ class SoproTTS:
             text_ids, ref=ref, max_frames=max_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
             style_strength=float(style_strength if style_strength is not None else self.cfg.style_strength),
             min_gen_frames=min_gen_frames, seed=seed, generator=generator)
-        return self.codec.decode_full(tokens_tq)
+        wav = self.codec.decode_full(tokens_tq)
+        return wav if rs is None else rs(wav)
 
     @torch.inference_mode()
     def synthesize_batch(self, texts: Sequence[str], *, ref: PreparedReference, max_frames: int = 400, top_p: float = 0.9,
                          temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
-                         min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None) -> List[torch.Tensor]:
+                         min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
+                         sample_rate: Optional[int] = None) -> List[torch.Tensor]:
         """NEW: B texts with one shared prepared reference -> B waveforms [1, 1, N_i].  One batched prefill, one
-        persistent AR launch, one ragged NAR pass, padded Mimi decodes; utterance i equals synthesize(texts[i], seed=seeds[i])."""
+        persistent AR launch, one ragged NAR pass, padded Mimi decodes (each resampled in one ragged launch when
+        `sample_rate` is given); utterance i equals synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate)."""
+        rs = self._resampler(sample_rate)
         st = float(style_strength if style_strength is not None else self.cfg.style_strength)
         model = self.model
         ids = [self.encode_text(t) for t in texts]
@@ -628,16 +637,34 @@ class SoproTTS:
             keep = torch.arange(frames, device=self.device)[None, :] < torch.tensor([Ts[i] for i in chunk], device=self.device)[:, None]
             batch = (batch * keep[:, None, :]).contiguous()  # padding frames decode code 0; their samples are cut below
             wav = self.codec.engine.decode(batch)
+            if rs is not None:  # the padding past Ts[i] * hop holds decoded filler: lens keeps the resampler from reading it
+                lens = [Ts[i] * hop for i in chunk]
+                wav = rs(wav.view(len(chunk), -1), lens=lens).unsqueeze(1)
+                for j, i in enumerate(chunk):
+                    out[i] = wav[j: j + 1, :, : rs.length(lens[j])].clone()
+                continue
             for j, i in enumerate(chunk):
                 out[i] = wav[j: j + 1, :, : Ts[i] * hop].clone()
         return out
 
-    def stream(self, text: str, **kwargs) -> Iterator[torch.Tensor]:
+    def stream(self, text: str, *, sample_rate: Optional[int] = None, **kwargs) -> Iterator[torch.Tensor]:
         from .streaming import stream as _stream
 
-        return _stream(self, text, **kwargs)
+        return _stream(self, text, sample_rate=sample_rate, **kwargs)
 
-    def save_wav(self, path: str, wav_1xT: torch.Tensor) -> None:
+    def save_wav(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
+        """`sample_rate`: the rate the waveform is at (the one passed to synthesize / stream)."""
         from .audio import save_audio
 
-        save_audio(path, wav_1xT, sr=TARGET_SR)
+        save_audio(path, wav_1xT, sr=int(sample_rate))
+
+    def _resampler(self, sample_rate: Optional[int]) -> Optional[Resampler]:
+        """None for the codec's own 24 kHz (no launch); otherwise this rate's cached resampler.  A refused rate raises
+        ValueError here, before a caller has consumed any random draws."""
+        if sample_rate is None or (not isinstance(sample_rate, bool) and sample_rate == TARGET_SR):
+            return None
+        sr = check_rates(TARGET_SR, sample_rate)[1]
+        rs = self._resamplers.get(sr)
+        if rs is None:
+            rs = self._resamplers[sr] = Resampler(TARGET_SR, sr, self.device)
+        return rs

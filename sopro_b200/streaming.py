@@ -48,8 +48,12 @@ class SoproTTSStreamer:
                anti_loop: bool = True, style_strength: Optional[float] = None, ref_seconds: Optional[float] = None,
                chunk_frames: Optional[int] = None, nar_context_frames: Optional[int] = None,
                min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-               generator: Optional[torch.Generator] = None) -> Iterator[torch.Tensor]:
+               generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None) -> Iterator[torch.Tensor]:
+        """`sample_rate` (extension): chunks at this rate (None = 24 kHz).  Each chunk's audio goes through a resampler
+        stream right after its Mimi step, so the chunks concatenate to the one-shot resample of the 24 kHz stream bit for
+        bit; the last chunk also carries the resampler's tail."""
         tts, model = self.tts, self.tts.model
+        rs = tts._resampler(sample_rate)  # a refused rate raises before the prefill
         text_ids = tts.encode_text(text)
         if ref is None:
             ref = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
@@ -62,22 +66,31 @@ class SoproTTSStreamer:
         hist: List[int] = []
         emitted = 0
         state = self.mimi_stream.new_state()
+        # resampler state: its tail carries at most the filter window; pushes are bounded by one chunk's samples
+        max_push = self.mimi_stream.max_chunk_frames * tts.codec.engine.hop
+        rstate = rs.checkout_stream(max_push) if rs is not None else None
         on_gpu = tts.device.type == "cuda"
         main = torch.cuda.current_stream(tts.device) if on_gpu else None
         side = torch.cuda.Stream(tts.device) if on_gpu else None
 
-        def refine_and_emit(end: int) -> Optional[torch.Tensor]:
+        def refine_and_emit(end: int, last: bool) -> Optional[torch.Tensor]:
             """NAR over the new frames + `ctx` frames of left context, Mimi stream step on the new frames' codes
-            (reference streaming.py:81-104); enqueued on the side stream."""
+            (reference streaming.py:81-104), then the resampler push (and, on the last chunk, its finish); enqueued on
+            the side stream."""
             nonlocal emitted, state
-            if end <= emitted:
-                return None
-            lo = max(0, emitted - ctx)
-            toks = torch.as_tensor(hist[lo:end], device=tts.device, dtype=torch.long).unsqueeze(0)
-            win = model.nar_refine(prep["cond_ar"][:, lo:end, :], toks).squeeze(0)
-            wav, state = self.mimi_stream.decode_step(win[emitted - lo:, :], state, _trusted=True)  # our own NAR's codes
-            emitted = end
-            return wav if wav.numel() > 0 else None
+            wav = None
+            if end > emitted:
+                lo = max(0, emitted - ctx)
+                toks = torch.as_tensor(hist[lo:end], device=tts.device, dtype=torch.long).unsqueeze(0)
+                win = model.nar_refine(prep["cond_ar"][:, lo:end, :], toks).squeeze(0)
+                wav, state = self.mimi_stream.decode_step(win[emitted - lo:, :], state, _trusted=True)  # our own NAR's codes
+                emitted = end
+            if rstate is not None and (wav is not None or last):
+                parts = [rstate.push(wav[:, i: i + max_push]) for i in range(0, wav.shape[1], max_push)] if wav is not None else []
+                if last:
+                    parts.append(rstate.finish())
+                wav = torch.cat(parts).unsqueeze(0) if len(parts) > 1 else parts[0].unsqueeze(0)
+            return wav if wav is not None and wav.numel() > 0 else None
 
         progress = {"consumed": 0}
         chunks = model.ar_chunks(prep, max_frames=max_frames, chunk_frames=cf, top_p=top_p, temperature=temperature,
@@ -97,7 +110,7 @@ class SoproTTSStreamer:
                 if on_gpu:
                     side.wait_stream(main)
                     with torch.cuda.stream(side):
-                        wav = refine_and_emit(end)
+                        wav = refine_and_emit(end, last)
                     if not last:
                         main.wait_stream(side)  # AR(k+1) behind chunk k's NAR + Mimi, never in front of them
                         prefetch()
@@ -105,7 +118,7 @@ class SoproTTSStreamer:
                     if wav is not None:
                         wav.record_stream(main)
                 else:
-                    wav = refine_and_emit(end)
+                    wav = refine_and_emit(end, last)
                 if wav is not None:
                     yield wav
                 if last:
@@ -113,11 +126,15 @@ class SoproTTSStreamer:
         finally:
             chunks.close()
             self.mimi_stream.release(state)
+            if rstate is not None:
+                rs.release_stream(rstate)
 
 
 @torch.inference_mode()
 def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
-           ref: Optional[PreparedReference] = None, chunk_frames: int = 6, **kwargs) -> Iterator[torch.Tensor]:
+           ref: Optional[PreparedReference] = None, chunk_frames: int = 6, sample_rate: Optional[int] = None,
+           **kwargs) -> Iterator[torch.Tensor]:
+    tts._resampler(sample_rate)  # a refused rate raises at the call, not at the first chunk
     streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
     return streamer.stream(text, ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref=ref,
-                           chunk_frames=chunk_frames, **kwargs)
+                           chunk_frames=chunk_frames, sample_rate=sample_rate, **kwargs)

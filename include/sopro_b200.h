@@ -601,6 +601,53 @@ int sopro_resampler_push(sopro_resampler_stream_t* s, const float* x, int64_t n,
  * called twice without a reset */
 int sopro_resampler_finish(sopro_resampler_stream_t* s, float* y, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Speaking rate (no reference counterpart: the reference has no rate control): pitch-preserving time-scale
+ * modification of a 24 kHz waveform by WSOLA.  Frame N = 480, synthesis hop Hs = 240, search tolerance D = 160,
+ * periodic Hann window w[n] = sin^2(pi n / N).  The speed is quantised to S = round(speed * 65536) (half to even),
+ * S in [16384, 262144] (speed 0.25 .. 4.0).  For L input samples (x = 0 outside [0, L)):
+ *   M = ceil(L * 65536 / S) outputs, K = ceil(M / Hs) + 1 frames (0 when M = 0), a_k = floor((k Hs S + 32768) / 65536);
+ *   d_0 = 0; for k >= 1, with p_{k-1} = a_{k-1} + d_{k-1}: d_k = argmax over d in [-D, D] of
+ *   sum_n x[p_{k-1} + n] x[a_k + d - N/2 + n] (ties: smallest |d|, then the negative one);
+ *   y[m] = sum_k w[m - k Hs + N/2] x[p_k + m - k Hs] over the two frames covering m, in increasing k, for m in [0, M).
+ * fp32 arithmetic; one device function computes a frame for both the one-shot and the stream paths. */
+typedef struct sopro_stretch_stream sopro_stretch_stream_t;
+/* host-only: validates and quantises a speed; SOPRO_ERR_INVALID for NaN, +-inf or anything outside [0.25, 4.0] */
+int sopro_stretch_speed(double speed, int32_t* S);
+/* host-only: M = ceil(n_in * 65536 / S); < 0 for a refused S or n_in < 0 */
+int64_t sopro_stretched_length(int32_t S, int64_t n_in);
+/* host-only: returns K, the frames of n_in input samples, and (when a is non-NULL) writes their nominal analysis
+ * positions a[0 .. K) (i64); < 0 for a refused S or n_in < 0 */
+int64_t sopro_stretch_positions(int32_t S, int64_t n_in, int64_t* a);
+/* host-only: the N = 480 window taps, sin^2(pi n / N) evaluated in double and rounded to fp32 once -> w [480] */
+int sopro_stretch_window(float* w);
+/* one-shot, ragged batch, one CTA per row: row b of x [B][x_stride] f32 (device) has lens_host[b] samples (HOST i64;
+ * NULL = x_stride each); samples at or past lens[b] are not read.  Row b's M_b outputs go to y + b * y_stride (device;
+ * y_stride >= the longest row's outputs when B > 1); the rest of the row is not written.  offsets (nullable, device
+ * i32 [B][K_max], K_max = the longest row's frame count) receives every d_k: a test hook. */
+int sopro_stretch(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t S, float* y, int64_t y_stride,
+                  int32_t* offsets, void* stream);
+/* Streaming: one utterance pushed in chunks of at most max_chunk samples.  Frame k is ready once
+ * max(a_k + D + N/2, a_{k-1} + D + Hs + N/2) input samples have arrived (a_0 + D + N/2 for frame 0); with frames
+ * [0, k_done) done, the pushes have emitted the outputs below max(0, k_done - 1) * Hs, and finish emits the rest up to
+ * M.  The concatenated outputs equal sopro_stretch of the concatenated input bit for bit, under any chunk schedule.
+ * The state on the device: the last p, the Hs pending overlap-add samples, and fewer than 2048 carried input samples;
+ * output counts are host arithmetic (no call synchronises).  Calls on one state must be ordered (one CUDA stream). */
+int sopro_stretch_stream_create(int64_t max_chunk, int device, sopro_stretch_stream_t** out);
+int sopro_stretch_stream_destroy(sopro_stretch_stream_t* s);
+/* back to sample 0 at speed S (host-only; also clears the finished state).  A new state takes no push until its first
+ * reset; one state serves every speed. */
+int sopro_stretch_stream_reset(sopro_stretch_stream_t* s, int32_t S);
+/* outputs the next call writes: a push of n_more samples (final == 0), or a push of n_more samples followed by finish
+ * (final != 0); < 0 on bad arguments, before the first reset or after finish */
+int64_t sopro_stretch_stream_ready(const sopro_stretch_stream_t* s, int64_t n_more, int final);
+/* x [n] f32 (device) -> y (device) receives stream_ready(s, n, 0) outputs.  n > max_chunk: SOPRO_ERR_INVALID, nothing
+ * launched, state unchanged.  After finish: SOPRO_ERR_STATE until a reset. */
+int sopro_stretch_push(sopro_stretch_stream_t* s, const float* x, int64_t n, float* y, void* stream);
+/* the remaining stream_ready(s, 0, 1) outputs (the input's end is zero padded) -> y (device); SOPRO_ERR_STATE when
+ * called twice without a reset */
+int sopro_stretch_finish(sopro_stretch_stream_t* s, float* y, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

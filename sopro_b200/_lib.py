@@ -215,6 +215,17 @@ SYMBOLS = {
     "sopro_resampler_stream_ready": (C.c_int64, [_VP, C.c_int64, _I]),
     "sopro_resampler_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP]),
     "sopro_resampler_finish": (_I, [_VP, _VP, _VP]),
+    "sopro_stretch_speed": (_I, [C.c_double, _I32P]),
+    "sopro_stretched_length": (C.c_int64, [C.c_int32, C.c_int64]),
+    "sopro_stretch_positions": (C.c_int64, [C.c_int32, C.c_int64, _VP]),
+    "sopro_stretch_window": (_I, [_VP]),
+    "sopro_stretch": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, _VP, C.c_int64, _VP, _VP]),
+    "sopro_stretch_stream_create": (_I, [C.c_int64, _I, C.POINTER(_VP)]),
+    "sopro_stretch_stream_destroy": (_I, [_VP]),
+    "sopro_stretch_stream_reset": (_I, [_VP, C.c_int32]),
+    "sopro_stretch_stream_ready": (C.c_int64, [_VP, C.c_int64, _I]),
+    "sopro_stretch_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP]),
+    "sopro_stretch_finish": (_I, [_VP, _VP, _VP]),
 }
 
 _lib = None

@@ -26,6 +26,7 @@ from .nar import NarEngine
 from .prefill_cuda import PrefillEngine, RefPrepEngine
 from .prefill import PreparedReference
 from .resample import Resampler, check_rates
+from .stretch import StretchPool, check_speed, stretch, stretched_length
 from .weights import load_safetensors, read_safetensors_cfg
 
 
@@ -512,6 +513,7 @@ class SoproTTS:
         self.codec = codec
         self.device = torch.device(device)
         self._resamplers: Dict[int, Resampler] = {}  # output rate -> its resampler (tap table on the device)
+        self._stretch_pool = StretchPool(self.device)  # idle time-stretch stream states, shared by every speed
 
     # ---- construction
     @classmethod
@@ -581,10 +583,14 @@ class SoproTTS:
                    ref_tokens_tq: Optional[torch.Tensor] = None, max_frames: int = 400, top_p: float = 0.9,
                    temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                    ref_seconds: Optional[float] = None, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-                   generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None) -> torch.Tensor:
+                   generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
+                   speed: Optional[float] = None) -> torch.Tensor:
         """-> [1, 1, N] f32 on the device.  `sample_rate` (extension): the output rate in Hz (None = 24 kHz, the codec's
-        own); another rate resamples the decoded waveform on the GPU (sopro_b200/resample.py)."""
+        own); another rate resamples the decoded waveform on the GPU (sopro_b200/resample.py).  `speed` (extension): the
+        speaking rate in [0.25, 4.0] (None = the model's own); the 24 kHz waveform is time-stretched on the GPU with its
+        pitch kept (sopro_b200/stretch.py), then resampled when `sample_rate` is set."""
         rs = self._resampler(sample_rate)  # a refused rate raises before any work
+        stretch_on = check_speed(speed) is not None  # so does a refused speed
         text_ids = self.encode_text(text)
         if ref is None:
             ref = self.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
@@ -593,17 +599,21 @@ class SoproTTS:
             style_strength=float(style_strength if style_strength is not None else self.cfg.style_strength),
             min_gen_frames=min_gen_frames, seed=seed, generator=generator)
         wav = self.codec.decode_full(tokens_tq)
+        if stretch_on:
+            wav = stretch(wav, speed)
         return wav if rs is None else rs(wav)
 
     @torch.inference_mode()
     def synthesize_batch(self, texts: Sequence[str], *, ref: PreparedReference, max_frames: int = 400, top_p: float = 0.9,
                          temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                          min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
-                         sample_rate: Optional[int] = None) -> List[torch.Tensor]:
+                         sample_rate: Optional[int] = None, speed: Optional[float] = None) -> List[torch.Tensor]:
         """NEW: B texts with one shared prepared reference -> B waveforms [1, 1, N_i].  One batched prefill, one
-        persistent AR launch, one ragged NAR pass, padded Mimi decodes (each resampled in one ragged launch when
-        `sample_rate` is given); utterance i equals synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate)."""
+        persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, in one
+        ragged launch when `speed` / `sample_rate` is given); utterance i equals synthesize(texts[i], seed=seeds[i],
+        sample_rate=sample_rate, speed=speed)."""
         rs = self._resampler(sample_rate)
+        stretch_on = check_speed(speed) is not None
         st = float(style_strength if style_strength is not None else self.cfg.style_strength)
         model = self.model
         ids = [self.encode_text(t) for t in texts]
@@ -637,20 +647,23 @@ class SoproTTS:
             keep = torch.arange(frames, device=self.device)[None, :] < torch.tensor([Ts[i] for i in chunk], device=self.device)[:, None]
             batch = (batch * keep[:, None, :]).contiguous()  # padding frames decode code 0; their samples are cut below
             wav = self.codec.engine.decode(batch)
-            if rs is not None:  # the padding past Ts[i] * hop holds decoded filler: lens keeps the resampler from reading it
-                lens = [Ts[i] * hop for i in chunk]
+            # the padding past Ts[i] * hop holds decoded filler: lens keeps the time-stretch and the resampler from reading it
+            lens = [Ts[i] * hop for i in chunk]
+            if stretch_on:
+                wav = stretch(wav.view(len(chunk), -1), speed, lens=lens).unsqueeze(1)
+                lens = [stretched_length(speed, n) for n in lens]
+            if rs is not None:
                 wav = rs(wav.view(len(chunk), -1), lens=lens).unsqueeze(1)
-                for j, i in enumerate(chunk):
-                    out[i] = wav[j: j + 1, :, : rs.length(lens[j])].clone()
-                continue
+                lens = [rs.length(n) for n in lens]
             for j, i in enumerate(chunk):
-                out[i] = wav[j: j + 1, :, : Ts[i] * hop].clone()
+                out[i] = wav[j: j + 1, :, : lens[j]].clone()
         return out
 
-    def stream(self, text: str, *, sample_rate: Optional[int] = None, **kwargs) -> Iterator[torch.Tensor]:
+    def stream(self, text: str, *, sample_rate: Optional[int] = None, speed: Optional[float] = None,
+               **kwargs) -> Iterator[torch.Tensor]:
         from .streaming import stream as _stream
 
-        return _stream(self, text, sample_rate=sample_rate, **kwargs)
+        return _stream(self, text, sample_rate=sample_rate, speed=speed, **kwargs)
 
     def save_wav(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
         """`sample_rate`: the rate the waveform is at (the one passed to synthesize / stream)."""

@@ -11,6 +11,7 @@ import torch
 
 from .codec import MimiDecodeState, MimiStreamDecoder
 from .prefill import PreparedReference
+from .stretch import check_speed
 
 
 @dataclass
@@ -48,12 +49,15 @@ class SoproTTSStreamer:
                anti_loop: bool = True, style_strength: Optional[float] = None, ref_seconds: Optional[float] = None,
                chunk_frames: Optional[int] = None, nar_context_frames: Optional[int] = None,
                min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-               generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None) -> Iterator[torch.Tensor]:
-        """`sample_rate` (extension): chunks at this rate (None = 24 kHz).  Each chunk's audio goes through a resampler
-        stream right after its Mimi step, so the chunks concatenate to the one-shot resample of the 24 kHz stream bit for
-        bit; the last chunk also carries the resampler's tail."""
+               generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
+               speed: Optional[float] = None) -> Iterator[torch.Tensor]:
+        """`sample_rate` (extension): chunks at this rate (None = 24 kHz).  `speed` (extension): the speaking rate in
+        [0.25, 4.0] (None = the model's own).  Each chunk's audio goes through a time-stretch stream, then a resampler
+        stream, right after its Mimi step, so the chunks concatenate to the one-shot stretch and resample of the 24 kHz
+        stream bit for bit; the last chunk also carries both tails."""
         tts, model = self.tts, self.tts.model
         rs = tts._resampler(sample_rate)  # a refused rate raises before the prefill
+        stretch_on = check_speed(speed) is not None  # so does a refused speed
         text_ids = tts.encode_text(text)
         if ref is None:
             ref = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
@@ -66,8 +70,10 @@ class SoproTTSStreamer:
         hist: List[int] = []
         emitted = 0
         state = self.mimi_stream.new_state()
-        # resampler state: its tail carries at most the filter window; pushes are bounded by one chunk's samples
+        # stretch / resampler states: their tails carry at most one frame's window / the filter window; pushes are
+        # bounded by one chunk's samples (a stretch push can yield up to 4x that, so the resampler pushes are split)
         max_push = self.mimi_stream.max_chunk_frames * tts.codec.engine.hop
+        sstate = tts._stretch_pool.checkout(max_push, speed) if stretch_on else None
         rstate = rs.checkout_stream(max_push) if rs is not None else None
         on_gpu = tts.device.type == "cuda"
         main = torch.cuda.current_stream(tts.device) if on_gpu else None
@@ -75,8 +81,8 @@ class SoproTTSStreamer:
 
         def refine_and_emit(end: int, last: bool) -> Optional[torch.Tensor]:
             """NAR over the new frames + `ctx` frames of left context, Mimi stream step on the new frames' codes
-            (reference streaming.py:81-104), then the resampler push (and, on the last chunk, its finish); enqueued on
-            the side stream."""
+            (reference streaming.py:81-104), then the stretch and resampler pushes (and, on the last chunk, their
+            finishes); enqueued on the side stream."""
             nonlocal emitted, state
             wav = None
             if end > emitted:
@@ -85,6 +91,11 @@ class SoproTTSStreamer:
                 win = model.nar_refine(prep["cond_ar"][:, lo:end, :], toks).squeeze(0)
                 wav, state = self.mimi_stream.decode_step(win[emitted - lo:, :], state, _trusted=True)  # our own NAR's codes
                 emitted = end
+            if sstate is not None and (wav is not None or last):
+                parts = [sstate.push(wav[:, i: i + max_push]) for i in range(0, wav.shape[1], max_push)] if wav is not None else []
+                if last:
+                    parts.append(sstate.finish())
+                wav = torch.cat(parts).unsqueeze(0) if len(parts) > 1 else parts[0].unsqueeze(0)
             if rstate is not None and (wav is not None or last):
                 parts = [rstate.push(wav[:, i: i + max_push]) for i in range(0, wav.shape[1], max_push)] if wav is not None else []
                 if last:
@@ -126,6 +137,8 @@ class SoproTTSStreamer:
         finally:
             chunks.close()
             self.mimi_stream.release(state)
+            if sstate is not None:
+                tts._stretch_pool.release(sstate)
             if rstate is not None:
                 rs.release_stream(rstate)
 
@@ -133,8 +146,9 @@ class SoproTTSStreamer:
 @torch.inference_mode()
 def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
            ref: Optional[PreparedReference] = None, chunk_frames: int = 6, sample_rate: Optional[int] = None,
-           **kwargs) -> Iterator[torch.Tensor]:
-    tts._resampler(sample_rate)  # a refused rate raises at the call, not at the first chunk
+           speed: Optional[float] = None, **kwargs) -> Iterator[torch.Tensor]:
+    tts._resampler(sample_rate)  # a refused rate or speed raises at the call, not at the first chunk
+    check_speed(speed)
     streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
     return streamer.stream(text, ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref=ref,
-                           chunk_frames=chunk_frames, sample_rate=sample_rate, **kwargs)
+                           chunk_frames=chunk_frames, sample_rate=sample_rate, speed=speed, **kwargs)

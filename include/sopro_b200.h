@@ -648,6 +648,44 @@ int sopro_stretch_push(sopro_stretch_stream_t* s, const float* x, int64_t n, flo
  * called twice without a reset */
 int sopro_stretch_finish(sopro_stretch_stream_t* s, float* y, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Loudness normalisation (no reference counterpart: the reference's output level follows its reference recording):
+ * ITU-R BS.1770-4 integrated loudness of mono rows x[0, n) at a rate sr, an integer in [4000, 192000], and a gain to
+ * a target T.
+ *   K-weighting: two biquads in cascade, zero initial state, x = 0 before sample 0; libebur128's coefficients from the
+ *   analog prototype, evaluated on the host in double (K = tan(pi f0 / sr), a0 = 1 + K/Q + K^2):
+ *     shelf: f0 = 1681.974450955533, G = 3.999843853973347 dB, Q = 0.7071752369554196, Vh = 10^(G/20),
+ *            Vb = Vh^0.4996667741545416; b = [Vh + Vb K/Q + K^2, 2 (K^2 - Vh), Vh - Vb K/Q + K^2] / a0,
+ *            a = [1, 2 (K^2 - 1) / a0, (1 - K/Q + K^2) / a0];
+ *     high-pass: f0 = 38.13547087602444, Q = 0.5003270373238773; b = [1, -2, 1], a as above with its own K and a0.
+ *   Blocks: sub-block s = floor((sr + 5) / 10) samples; block j = sub-blocks j .. j + 3 for j in [0, J),
+ *   J = max(0, floor(n / s) - 3); z_j = sum y^2 over the block / (4 s); l_j = -0.691 + 10 log10 z_j; a trailing partial
+ *   sub-block belongs to no block.
+ *   Gating: absolute, l_j > -70; Gamma_r = -0.691 + 10 log10(mean z over those blocks) - 10; L = -0.691 +
+ *   10 log10(mean z over the blocks with l_j > -70 and l_j > Gamma_r), compared as energies (thresholds converted once
+ *   in double); L = -inf when no block passes (silence, or n < 4 s).
+ *   Gain: g = fp32(min(10^((T - L) / 20), 10^(-1/20) / max|x|)), rounded once, toward zero, so that the fixed -1 dBFS
+ *   sample-peak ceiling holds in fp32: max|y| <= fp32(10^(-1/20)); g = 1 when L = -inf; y = g * x, one fp32 multiply.
+ * The filter, the y^2 sums, the block energies and the gating run in fp64 on the device; every sum has a fixed order,
+ * so a row's L, g and y depend only on its own samples.  No call synchronises with the host or allocates. */
+/* host-only: the K-weighting coefficients at sr -> c[10] = shelf b0, b1, b2, a1, a2, then high-pass b0, b1, b2, a1, a2
+ * (a0 = 1); SOPRO_ERR_INVALID for a rate outside [4000, 192000] */
+int sopro_loudness_filter(int32_t sr, double* c);
+/* host-only: SOPRO_OK for a target in [-60, 0] LUFS, SOPRO_ERR_INVALID otherwise (NaN and +-inf included) */
+int sopro_loudness_target(double T);
+/* host-only: the workspace bytes for B rows of at most max_len samples at sr; < 0 for bad arguments */
+int64_t sopro_loudness_workspace(int32_t B, int64_t max_len, int32_t sr);
+/* ragged batch: row b of x [B][x_stride] f32 (device) has lens_host[b] samples (HOST i64; NULL = x_stride each);
+ * samples at or past lens[b] are not read.  ws: device, at least loudness_workspace(B, max lens, sr) bytes.
+ * L of row b -> lufs_dev[b] (device f64; -inf when no block passes the gates). */
+int sopro_loudness_measure(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, void* ws,
+                           double* lufs_dev, void* stream);
+/* as the measure, then y + b * y_stride (device; y_stride >= the longest row when B > 1) receives g_b * x over
+ * [0, lens[b]); the rest of the row is not written.  y may alias x (y_stride = x_stride).  lufs_dev (nullable) receives
+ * L, gain_dev (nullable, device f32 [B]) receives g: a test hook.  A refused T is SOPRO_ERR_INVALID before any launch. */
+int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, double T,
+                             float* y, int64_t y_stride, void* ws, double* lufs_dev, float* gain_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

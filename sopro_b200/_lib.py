@@ -226,6 +226,12 @@ SYMBOLS = {
     "sopro_stretch_stream_ready": (C.c_int64, [_VP, C.c_int64, _I]),
     "sopro_stretch_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP]),
     "sopro_stretch_finish": (_I, [_VP, _VP, _VP]),
+    "sopro_loudness_filter": (_I, [C.c_int32, _VP]),
+    "sopro_loudness_target": (_I, [C.c_double]),
+    "sopro_loudness_workspace": (C.c_int64, [C.c_int32, C.c_int64, C.c_int32]),
+    "sopro_loudness_measure": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, _VP, _VP, _VP]),
+    "sopro_loudness_normalize": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, C.c_double, _VP, C.c_int64, _VP, _VP,
+                                      _VP, _VP]),
 }
 
 _lib = None

@@ -25,6 +25,7 @@ from .engine import ArEngine, ArSession, Sampling
 from .nar import NarEngine
 from .prefill_cuda import PrefillEngine, RefPrepEngine
 from .prefill import PreparedReference
+from .loudness import check_loudness, normalize_loudness
 from .resample import Resampler, check_rates
 from .stretch import StretchPool, check_speed, stretch, stretched_length
 from .weights import load_safetensors, read_safetensors_cfg
@@ -584,13 +585,16 @@ class SoproTTS:
                    temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                    ref_seconds: Optional[float] = None, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
                    generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
-                   speed: Optional[float] = None) -> torch.Tensor:
+                   speed: Optional[float] = None, loudness: Optional[float] = None) -> torch.Tensor:
         """-> [1, 1, N] f32 on the device.  `sample_rate` (extension): the output rate in Hz (None = 24 kHz, the codec's
         own); another rate resamples the decoded waveform on the GPU (sopro_b200/resample.py).  `speed` (extension): the
         speaking rate in [0.25, 4.0] (None = the model's own); the 24 kHz waveform is time-stretched on the GPU with its
-        pitch kept (sopro_b200/stretch.py), then resampled when `sample_rate` is set."""
+        pitch kept (sopro_b200/stretch.py), then resampled when `sample_rate` is set.  `loudness` (extension): a target
+        integrated loudness in LUFS, [-60, 0] (None = the level the model produced); the final waveform is measured per
+        ITU-R BS.1770-4 and scaled on the GPU under a -1 dBFS sample-peak ceiling (sopro_b200/loudness.py)."""
         rs = self._resampler(sample_rate)  # a refused rate raises before any work
         stretch_on = check_speed(speed) is not None  # so does a refused speed
+        target = check_loudness(loudness)  # and a refused loudness target
         text_ids = self.encode_text(text)
         if ref is None:
             ref = self.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
@@ -601,19 +605,25 @@ class SoproTTS:
         wav = self.codec.decode_full(tokens_tq)
         if stretch_on:
             wav = stretch(wav, speed)
-        return wav if rs is None else rs(wav)
+        if rs is not None:
+            wav = rs(wav)
+        if target is not None:
+            wav = normalize_loudness(wav, TARGET_SR if rs is None else rs.sr_out, target)
+        return wav
 
     @torch.inference_mode()
     def synthesize_batch(self, texts: Sequence[str], *, ref: PreparedReference, max_frames: int = 400, top_p: float = 0.9,
                          temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                          min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
-                         sample_rate: Optional[int] = None, speed: Optional[float] = None) -> List[torch.Tensor]:
+                         sample_rate: Optional[int] = None, speed: Optional[float] = None,
+                         loudness: Optional[float] = None) -> List[torch.Tensor]:
         """NEW: B texts with one shared prepared reference -> B waveforms [1, 1, N_i].  One batched prefill, one
-        persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, in one
-        ragged launch when `speed` / `sample_rate` is given); utterance i equals synthesize(texts[i], seed=seeds[i],
-        sample_rate=sample_rate, speed=speed)."""
+        persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, then
+        loudness-normalised, in one ragged launch when `speed` / `sample_rate` / `loudness` is given); utterance i equals
+        synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness)."""
         rs = self._resampler(sample_rate)
         stretch_on = check_speed(speed) is not None
+        target = check_loudness(loudness)
         st = float(style_strength if style_strength is not None else self.cfg.style_strength)
         model = self.model
         ids = [self.encode_text(t) for t in texts]
@@ -655,6 +665,9 @@ class SoproTTS:
             if rs is not None:
                 wav = rs(wav.view(len(chunk), -1), lens=lens).unsqueeze(1)
                 lens = [rs.length(n) for n in lens]
+            if target is not None:
+                wav = normalize_loudness(wav.view(len(chunk), -1), TARGET_SR if rs is None else rs.sr_out, target,
+                                         lens=lens).unsqueeze(1)
             for j, i in enumerate(chunk):
                 out[i] = wav[j: j + 1, :, : lens[j]].clone()
         return out

@@ -421,6 +421,33 @@ int sopro_nar_set_contraction(sopro_nar_t* n, int mode);
 /* One utterance's streaming windows (B == 1, <= 256 frames, no lens / forced codes) are replayed from CUDA graphs captured
  * over internal static buffers (a window is 113..217 launches): identical results, launch overhead removed.  Default on. */
 int sopro_nar_set_graphs(sopro_nar_t* n, int enabled);
+/* test hook: when non-NULL, every stage's pre-head activation z (nar.pre's output, before the head id embedding) is
+ * copied to z + s*B*Tmax*head_dim, layout [n_stages][B][Tmax][head_dim] f32 (device).  Bypasses the graph replay. */
+int sopro_nar_set_trace(sopro_nar_t* n, float* z);
+
+/* test hooks: the refiner's and the prefill's kernels one launch at a time, with the engine's own launchers.  Device
+ * pointers, no allocation; a shape the kernel does not take returns SOPRO_ERR_INVALID and launches nothing.
+ *
+ * One fp32 contraction (dense_f32.cuh DenseOp): C[m][n] = epi(prologue(A)[m] . W[n] + bias[n]) with the RMSNorm prologue
+ * (norm_w) and/or a_add; epi 0 bias, 1 bias+GELU, 2 R + acc, 3 GLU (C [M][ldc >= N/2]), 4 argmax, 5 R + gate*acc.
+ * kernel: 0 = the engine's choice, 16 = the skinny kernel (M <= 16, K <= 2048), 32 / 64 / 128 = that tile edge (not 32 for
+ * GLU).  groups > 1 (argmax only): group z uses W + z*zW, bias + z*zBias, a_add + z*zAdd.  Argmax: ids [M][groups] i32
+ * gets the first maximum of each row and group, through a workspace ws of >= 8*groups*M*ceil(N/8) bytes. */
+int sopro_debug_dense(const float* A, const float* W, const float* bias, const float* norm_w, const float* a_add, const float* R,
+                      float* C, float gate, int M, int N, int K, int ldc, int epi, int groups, int64_t zW, int64_t zBias,
+                      int64_t zAdd, int kernel, int32_t* ids, void* ws, int64_t ws_bytes, void* stream);
+/* The tensor-core contraction of the refiner: X [M][K] fp32 (optionally RMS-normalised by norm_w) is split into
+ * A3 [M][3K] bf16 = [h | m | l], then C [M][N] = epi(six products of A3 and W6 + bias); W6 [N][6K] as
+ * sopro_debug_pack_w6 builds it; epi 0 none, 1 GELU, 3 R + acc (R may alias C). */
+int sopro_debug_tc6(const float* X, const float* norm_w, const uint16_t* W6, const float* bias, const float* R, float* C, void* A3,
+                    int64_t M, int N, int K, int epi, void* stream);
+/* depthwise conv + residual of an SSMLiteBlock: out[b][t] = x[b][t] + bias + sum_j h[b][t + j*dil - left] * w[:, j] for
+ * t < lens[b] (rows outside [0, lens[b]) count as zero and are not read; output rows >= lens[b] are not written);
+ * rows [B][Tmax][D], lens NULL = Tmax. */
+int sopro_debug_dwconv_res(const float* h, const float* x, const float* w, const float* bias, float* out, const int32_t* lens, int B,
+                           int Tmax, int D, int k, int dil, int left, void* stream);
+/* first maximum of each head's V logits: logits [rows][heads][V] -> codes[r*Q + head] */
+int sopro_debug_argmax_heads(const float* logits, int64_t rows, int heads, int V, int32_t* codes, int Q, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Prefill: SoproTTSModel.prepare_conditioning (reference model.py:172-216) for B texts that share one prepared

@@ -11,7 +11,7 @@ mismatch can be classified as a near-tie or a bug.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -21,9 +21,9 @@ SD = Dict[str, Tensor]
 
 
 def rms_norm(x: Tensor, w: Tensor, eps: float = 1e-6) -> Tensor:
-    x32 = x.float()
+    x32 = x if x.dtype == torch.float64 else x.float()  # float64 mode keeps float64
     y = x32 * torch.rsqrt(x32.pow(2).mean(dim=-1, keepdim=True) + eps)
-    return (y * w.float()).to(x.dtype)
+    return (y * w.to(x32.dtype)).to(x.dtype)
 
 
 def dwconv_same(x_btd: Tensor, w: Tensor, b: Tensor, dilation: int) -> Tensor:
@@ -41,10 +41,16 @@ def ssm_block(sd: SD, p: str, x: Tensor, dilation: int) -> Tensor:
     return x + F.linear(F.gelu(f), sd[p + "ff.3.weight"], sd[p + "ff.3.bias"])
 
 
-def nar_refine(sd: SD, cfg, cond_seq: Tensor, rvq1_bt: Tensor, forced: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+def nar_refine(sd: SD, cfg, cond_seq: Tensor, rvq1_bt: Tensor, forced: Optional[Tensor] = None,
+               dtype: torch.dtype = torch.float32, z_out: Optional[List[Tensor]] = None) -> Tuple[Tensor, Tensor]:
     """-> (codes [B, T, Q] int64, margin [B, T, Q] f32).  margin[..., q] = (top1 - top2) / max|logit| of the head
     that decided codebook q (inf for q = 0).  `forced` [B, T, Q]: the previous codebooks every stage conditions on are
-    taken from it instead of from this run's own argmax."""
+    taken from it instead of from this run's own argmax.  dtype=torch.float64 runs the whole refiner on the state dict
+    and the conditioning cast to float64 (the reference the kernels' rounding is measured against).  z_out: a list that
+    receives each stage's pre-head activation z [B, T, Hn]."""
+    if dtype != torch.float32:
+        sd = {k: (v.to(dtype) if v.is_floating_point() else v) for k, v in sd.items() if k.startswith(("nar", "cb_embed."))}
+        cond_seq = cond_seq.to(dtype)
     B, T, D = cond_seq.shape
     Q, V = int(cfg.num_codebooks), int(cfg.codebook_size)
     out = torch.zeros((B, T, Q), dtype=torch.long)
@@ -59,7 +65,7 @@ def nar_refine(sd: SD, cfg, cond_seq: Tensor, rvq1_bt: Tensor, forced: Optional[
         cbt = torch.tensor(cbs, dtype=torch.long)
         toks = src[:, :, : idxs[0]] if forced is not None else out[:, :, : idxs[0]]
         e = emb[cbt.view(1, 1, -1) * V + toks]
-        w = F.softmax(sd["nar_prev_cb_weights"].float().index_select(0, cbt), dim=0)
+        w = F.softmax(sd["nar_prev_cb_weights"].to(dtype).index_select(0, cbt), dim=0)
         prev_sum = (e * w.view(1, 1, -1, 1)).sum(dim=2)
         mix = torch.softmax(sd[f"nar.mix.{name}"], dim=0)
         x = mix[0] * cond_seq + mix[1] * prev_sum
@@ -70,6 +76,8 @@ def nar_refine(sd: SD, cfg, cond_seq: Tensor, rvq1_bt: Tensor, forced: Optional[
         for i, d in enumerate(dils):
             x = ssm_block(sd, f"nar.blocks.{i}.", x, int(d))
         z = F.linear(rms_norm(x, sd["nar.norm.weight"]), sd["nar.pre.weight"], sd["nar.pre.bias"])
+        if z_out is not None:
+            z_out.append(z)
         for j, cb in enumerate(idxs):
             hb = sd[f"nar.head_id_emb.{name}.weight"][j].view(1, 1, -1)
             lg = F.linear(z + hb, sd[f"nar.heads.{name}.{j}.weight"], sd[f"nar.heads.{name}.{j}.bias"])

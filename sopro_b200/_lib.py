@@ -192,6 +192,12 @@ SYMBOLS = {
     "sopro_nar_set_forced": (_I, [_VP, _VP]),
     "sopro_nar_set_contraction": (_I, [_VP, _I]),
     "sopro_nar_set_graphs": (_I, [_VP, _I]),
+    "sopro_nar_set_trace": (_I, [_VP, _VP]),
+    "sopro_debug_dense": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float, _I, _I, _I, _I, _I, _I, C.c_int64, C.c_int64,
+                               C.c_int64, _I, _VP, _VP, C.c_int64, _VP]),
+    "sopro_debug_tc6": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_int64, _I, _I, _I, _VP]),
+    "sopro_debug_dwconv_res": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
+    "sopro_debug_argmax_heads": (_I, [_VP, C.c_int64, _I, _I, _VP, _I, _VP]),
     "sopro_nar_refine": (_I, [_VP, _VP, C.c_int64, _VP, _VP, _I, _I, _VP, _VP]),
     "sopro_prefill_create": (_I, [_VP, _VP, _I, C.POINTER(_VP)]),
     "sopro_prefill_destroy": (_I, [_VP]),

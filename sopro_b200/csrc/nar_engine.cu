@@ -84,10 +84,13 @@ int tile_edge(int M, int N, int groups, int epi) {
 }
 
 // C = epi(prologue(A) . W^T): picks the skinny kernel for M <= 16 rows, a tile kernel otherwise.
-// groups > 1 (argmax heads): blockIdx.z = group.
-int launch_dense(dense::DenseOp op, int groups, cudaStream_t st) {
+// groups > 1 (argmax heads): blockIdx.z = group.  edge (tests): 0 = that choice, 16 = the skinny kernel, 32 / 64 / 128 = that
+// tile edge.  parts_out: the argmax partial slots per row the launch writes.
+int launch_dense(dense::DenseOp op, int groups, cudaStream_t st, int edge = 0, int* parts_out = nullptr) {
   if (op.K % 16 || op.M < 1 || op.N < 1) return fail(SOPRO_ERR_INVALID, "dense: bad shape M=%d N=%d K=%d", op.M, op.N, op.K);
-  if (op.M <= dense::kSkinnyRows) {
+  if (edge == 0) edge = op.M <= dense::kSkinnyRows ? 16 : tile_edge(op.M, op.N, groups, op.epi);
+  if (edge == 16) {
+    if (op.M > dense::kSkinnyRows) return fail(SOPRO_ERR_INVALID, "dense: M=%d too many rows for the skinny kernel", op.M);
     const int ncol = op.epi == dense::EPI_GLU ? op.N / 2 : op.N;
     // about two waves of CTAs over the GPU, at least one column per warp
     int cols = std::max(8, (ncol * groups + 295) / 296);
@@ -95,17 +98,20 @@ int launch_dense(dense::DenseOp op, int groups, cudaStream_t st) {
     const int parts = (ncol + cols - 1) / cols;
     if (op.epi == dense::EPI_ARGMAX) op.parts = parts;
     const size_t smem = (size_t)dense::kSkinnyRows * op.K * 4;
-    static bool attr = false;
-    if (!attr) {
-      PCK(cudaFuncSetAttribute(dense::dense_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 2048 * 4));
-      attr = true;
-    }
     if (smem > (size_t)16 * 2048 * 4) return fail(SOPRO_ERR_INVALID, "dense: K=%d too large for the skinny kernel", op.K);
+    // a function attribute belongs to the current device's context: set once per device
+    static unsigned long long attr_done = 0;
+    if (tc::attr_needed(attr_done))
+      PCK(cudaFuncSetAttribute(dense::dense_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 2048 * 4));
+    if (parts_out) *parts_out = parts;
     dense::dense_skinny_kernel<<<dim3(parts, 1, groups), dense::kSkinnyThreads, smem, st>>>(op, cols);
   } else {
-    const int e = tile_edge(op.M, op.N, groups, op.epi);
+    const int e = edge;
+    if ((e != 32 && e != 64 && e != 128) || (e == 32 && op.epi == dense::EPI_GLU))
+      return fail(SOPRO_ERR_INVALID, "dense: no %d-wide tile for epilogue %d", e, op.epi);
     const dim3 grid((op.M + e - 1) / e, (op.N + e - 1) / e, groups);
     if (op.epi == dense::EPI_ARGMAX) op.parts = (int)grid.y;
+    if (parts_out) *parts_out = (int)grid.y;
     if (e == 128) dense::dense_tile_kernel<128, 128><<<grid, dense::kTileThreads, 0, st>>>(op);
     else if (e == 64) dense::dense_tile_kernel<64, 64><<<grid, dense::kTileThreads, 0, st>>>(op);
     else dense::dense_tile_kernel<32, 32><<<grid, dense::kTileThreads, 0, st>>>(op);
@@ -404,6 +410,7 @@ struct sopro_nar {
   float* ws = nullptr;
   size_t ws_bytes = 0;
   const int32_t* forced = nullptr;  // test hook: the previous codebooks every stage conditions on
+  float* trace_z = nullptr;         // test hook: every stage's pre-head activation z, [n_stages][B][Tmax][Hn]
   int tc_mode = -1;                 // -1 automatic (tensor cores above the skinny kernel's row count), 0 fp32 FMA kernels only
   // launch-bound streaming windows (one utterance, <= kNarGraphRows frames: 113..217 launches each) are replayed from
   // CUDA graphs captured over static buffers; every graph dies when the workspace is reallocated
@@ -594,6 +601,69 @@ int sopro_debug_pack_w6(const float* W, int N, int K, uint16_t* out) {
   return SOPRO_OK;
 }
 
+int sopro_debug_dense(const float* A, const float* W, const float* bias, const float* norm_w, const float* a_add, const float* R, float* C,
+                      float gate, int M, int N, int K, int ldc, int epi, int groups, int64_t zW, int64_t zBias, int64_t zAdd, int kernel,
+                      int32_t* ids, void* ws, int64_t ws_bytes, void* stream) {
+  if (!A || !W) return fail(SOPRO_ERR_INVALID, "null argument");
+  const bool glu = epi == dense::EPI_GLU, amax = epi == dense::EPI_ARGMAX;
+  if (epi < dense::EPI_BIAS || epi > dense::EPI_RES_GATE || groups < 1 || groups > 65535 || M < 1 || M > 0x3fffffff || N < 1 || K < 16 ||
+      K % 16 || zW < 0 || zBias < 0 || zAdd < 0 || (glu && (N % 2 || !bias)) ||
+      ((epi == dense::EPI_RES || epi == dense::EPI_RES_GATE) && !R) || (!amax && (!C || ldc < (glu ? N / 2 : N))))
+    return fail(SOPRO_ERR_INVALID, "debug dense: bad arguments (M=%d N=%d K=%d epi=%d groups=%d ldc=%d)", M, N, K, epi, groups, ldc);
+  if ((kernel != 0 && kernel != 16 && kernel != 32 && kernel != 64 && kernel != 128) || (kernel == 16 && M > dense::kSkinnyRows) ||
+      (kernel == 32 && glu) || (kernel == 16 && K > 2048))
+    return fail(SOPRO_ERR_INVALID, "debug dense: kernel %d does not take M=%d K=%d epi=%d", kernel, M, K, epi);
+  const long long slots = (long long)groups * M * ((N + 7) / 8);  // >= groups * M * parts of any kernel choice
+  if (amax && (!ids || !ws || ws_bytes < 8 * slots)) return fail(SOPRO_ERR_INVALID, "debug dense: argmax needs ids and %lld workspace bytes", 8 * slots);
+  if (!amax && groups > 1) return fail(SOPRO_ERR_INVALID, "debug dense: grouped launches are argmax only");
+  dense::DenseOp op{};
+  op.A = A; op.W = W; op.bias = bias; op.norm_w = norm_w; op.a_add = a_add; op.R = R; op.C = C; op.gate = gate;
+  op.M = M; op.N = N; op.K = K; op.ldc = ldc; op.epi = epi; op.zW = (size_t)zW; op.zBias = (size_t)zBias; op.zAdd = (size_t)zAdd;
+  if (amax) {
+    op.amax_val = static_cast<float*>(ws);
+    op.amax_idx = reinterpret_cast<int*>(static_cast<float*>(ws) + slots);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int parts = 0;
+  int rc = launch_dense(op, groups, st, kernel, &parts);
+  if (rc || !amax) return rc;
+  dense::argmax_finish_kernel<<<dim3((unsigned)((M + 127) / 128), groups), 128, 0, st>>>(op.amax_val, op.amax_idx, M, parts, ids, groups);
+  PCK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+int sopro_debug_tc6(const float* X, const float* norm_w, const uint16_t* W6, const float* bias, const float* R, float* C, void* A3, int64_t M,
+                    int N, int K, int epi, void* stream) {
+  if (!X || !W6 || !C || !A3 || (epi == tc::EPI_RES && !R)) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (M < 1 || M > 0x3fffffffLL || K < 4 || K % 4 || N < 1 || (epi != tc::EPI_NONE && epi != tc::EPI_GELU && epi != tc::EPI_RES) ||
+      !tc::supported(N, kPairs * K, K))
+    return fail(SOPRO_ERR_INVALID, "debug tc6: unsupported shape M=%lld N=%d K=%d epi=%d", (long long)M, N, K, epi);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  __nv_bfloat16* a3 = static_cast<__nv_bfloat16*>(A3);
+  split3_rows_kernel<<<(unsigned)((M + 7) / 8), 256, 0, st>>>(X, norm_w, a3, M, K);
+  PCK(cudaGetLastError());
+  return launch_tc6(a3, W6, bias, R, C, M, N, K, epi, st);
+}
+
+int sopro_debug_dwconv_res(const float* h, const float* x, const float* w, const float* bias, float* out, const int32_t* lens, int B, int Tmax,
+                           int D, int k, int dil, int left, void* stream) {
+  if (!h || !x || !w || !bias || !out) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535 || Tmax < 1 || D < 1 || k < 1 || k > 64 || dil < 1 || left < 0 || left > (k - 1) * dil)
+    return fail(SOPRO_ERR_INVALID, "debug dwconv: bad shape B=%d Tmax=%d D=%d k=%d dil=%d left=%d", B, Tmax, D, k, dil, left);
+  dense::dwconv_res_kernel<<<dim3(Tmax, B), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(h, x, w, bias, out, lens, Tmax, D, k, dil, left);
+  PCK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+int sopro_debug_argmax_heads(const float* logits, int64_t rows, int heads, int V, int32_t* codes, int Q, void* stream) {
+  if (!logits || !codes) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (rows < 1 || rows > 0x3fffffffLL || heads < 1 || V < 4 || V % 4 || Q < heads)
+    return fail(SOPRO_ERR_INVALID, "debug argmax heads: bad shape rows=%lld heads=%d V=%d Q=%d", (long long)rows, heads, V, Q);
+  argmax_heads_kernel<<<(unsigned)((rows * heads + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(logits, rows, heads, V, codes, Q);
+  PCK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
 int sopro_nar_set_contraction(sopro_nar_t* n, int mode) {
   if (!n || mode < -1 || mode > 1) return fail(SOPRO_ERR_INVALID, "bad argument");
   if (mode == 1 && !n->tc_ok) return fail(SOPRO_ERR_INVALID, "this NAR geometry has no tensor-core images");
@@ -604,6 +674,12 @@ int sopro_nar_set_contraction(sopro_nar_t* n, int mode) {
 int sopro_nar_set_forced(sopro_nar_t* n, const int32_t* forced_codes) {
   if (!n) return fail(SOPRO_ERR_INVALID, "null argument");
   n->forced = forced_codes;
+  return SOPRO_OK;
+}
+
+int sopro_nar_set_trace(sopro_nar_t* n, float* z) {
+  if (!n) return fail(SOPRO_ERR_INVALID, "null argument");
+  n->trace_z = z;
   return SOPRO_OK;
 }
 
@@ -661,6 +737,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
   const float* W = n->dev;
   set_first_codebook_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(rvq1, codes, M, Q);
   PCK(cudaGetLastError());
+  float* trace = n->trace_z;
   for (const auto& S : n->stages) {
     EmbedMix em{};
     em.cond = cond; em.cond_bs = cond_batch_stride; em.codes = n->forced ? n->forced : codes; em.emb = W + n->emb; em.w_prev = W + S.w_prev;
@@ -675,6 +752,10 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
       const unsigned rb = (unsigned)((M + 7) / 8);
       split3_rows_kernel<<<rb, 256, 0, st>>>(x, W + n->norm_w, a3, M, D);
       if ((rc = launch_tc6(a3, n->tcw + n->tc_pre, W + n->pre_b, nullptr, z, M, Hn, D, tc::EPI_NONE, st))) return rc;
+      if (trace) {
+        PCK(cudaMemcpyAsync(trace, z, (size_t)M * Hn * 4, cudaMemcpyDeviceToDevice, st));
+        trace += (size_t)M * Hn;
+      }
       split3_rows_kernel<<<rb, 256, 0, st>>>(z, nullptr, a3, M, Hn);
       for (long long m0 = 0; m0 < M; m0 += mc) {
         const long long rows = std::min<long long>(mc, M - m0);
@@ -691,6 +772,10 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
     g.A = x; g.W = W + n->pre_w; g.bias = W + n->pre_b; g.norm_w = W + n->norm_w; g.C = z; g.M = (int)M; g.N = Hn; g.K = D; g.ldc = Hn;
     g.epi = dense::EPI_BIAS;
     if ((rc = launch_dense(g, 1, st))) return rc;
+    if (trace) {
+      PCK(cudaMemcpyAsync(trace, z, (size_t)M * Hn * 4, cudaMemcpyDeviceToDevice, st));
+      trace += (size_t)M * Hn;
+    }
     g = dense::DenseOp{};
     g.A = z; g.W = W + S.head_w; g.bias = W + S.head_b; g.a_add = W + S.head_id; g.M = (int)M; g.N = V; g.K = Hn; g.epi = dense::EPI_ARGMAX;
     g.amax_val = amax_v; g.amax_idx = amax_i; g.zW = (size_t)V * Hn; g.zBias = V; g.zAdd = Hn;
@@ -718,7 +803,7 @@ int sopro_nar_refine(sopro_nar_t* n, const float* cond, int64_t cond_batch_strid
   PCK(cudaSetDevice(n->device));
   PCK(cudaStreamIsCapturing(st, &cap));
   // one utterance's streaming window: replay the whole pass (113..217 launches) from a graph over static buffers
-  if (!n->graphs || B != 1 || Tmax < 1 || Tmax > kNarGraphRows || lens || n->forced || cap != cudaStreamCaptureStatusNone)
+  if (!n->graphs || B != 1 || Tmax < 1 || Tmax > kNarGraphRows || lens || n->forced || n->trace_z || cap != cudaStreamCaptureStatusNone)
     return nar_refine_impl(n, cond, cond_batch_stride, rvq1, lens, B, Tmax, codes, stream);
   const sopro_nar_config_t& c = n->cfg;
   const int D = c.d_model, Q = c.n_codebooks;
@@ -1056,11 +1141,8 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
   // ---- reference cross-attention stack
   const size_t rsmem = (size_t)8 * (2 * D + ((Tr + 3) & ~3)) * 4;
   if (c.ref_layers > 0 && rsmem > 48 * 1024) {
-    static bool attr = false;
-    if (!attr) {
-      PCK(cudaFuncSetAttribute(ref_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      attr = true;
-    }
+    static unsigned long long attr_done = 0;  // per device, like every function attribute
+    if (tc::attr_needed(attr_done)) PCK(cudaFuncSetAttribute(ref_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
   for (int i = 0; i < c.ref_layers; ++i) {
     g = dense::DenseOp{};

@@ -104,6 +104,13 @@ class NarEngine:
         self._forced = None if forced_btq is None else forced_btq.to(device=self.device, dtype=torch.int32).contiguous()
         _lib.check(self.lib.sopro_nar_set_forced(self._h, self._forced.data_ptr() if self._forced is not None else None))
 
+    def set_trace(self, z: Optional[torch.Tensor]) -> None:
+        """Test hook: every stage's pre-head activation z goes to z [n_stages, B, T, head_dim] f32 on the engine's device."""
+        if z is not None and (z.device != self.device or z.dtype != torch.float32 or not z.is_contiguous()):
+            raise ValueError("trace buffer must be a contiguous float32 tensor on the engine's device")
+        self._trace = z
+        _lib.check(self.lib.sopro_nar_set_trace(self._h, z.data_ptr() if z is not None else None))
+
     def close(self) -> None:
         if getattr(self, "_h", None):
             self.lib.sopro_nar_destroy(self._h)

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import dense_probes as P
 from oracle import nar_oracle as N
 from tests.cases import _unit, e2e_inputs
 
@@ -170,3 +171,146 @@ def test_streaming_windows_replay_from_graphs_identically(T):
     replay_a = eng.refine(full[:, :T], rv[:, :T]).cpu()     # replay
     replay_b = eng.refine(full[:, 9:T + 9], rv[:, 9:T + 9]).cpu()
     assert torch.equal(first, plain_a) and torch.equal(replay_a, plain_a) and torch.equal(replay_b, plain_b)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# continuous values: each stage's pre-head activation z against the float64 oracle
+# ---------------------------------------------------------------------------------------------------------------
+def _stages(cfg):
+    return [(n, idx) for n, idx in cfg.stage_indices().items() if len(idx) > 0]
+
+
+def _traced(eng, cond, rvq1, lens, forced):
+    """teacher-forced run with the z trace on -> (ids [B, T, Q], z [n_stages, B, T, Hn]) on the host"""
+    B, T, _ = cond.shape
+    z = torch.full((len(_stages(eng.cfg)), B, T, int(eng.cfg.nar_head_dim)), float("nan"), device=eng.device)
+    eng.set_forced(forced)
+    eng.set_trace(z)
+    try:
+        ids = eng.refine(cond, rvq1, lens).cpu()
+    finally:
+        eng.set_trace(None)
+        eng.set_forced(None)
+    return ids, z.cpu()
+
+
+def _oracle_z(sd, cfg, cond, rvq1, forced, dtype):
+    zs = []
+    N.nar_refine(sd, cfg, cond, rvq1, forced=forced, dtype=dtype, z_out=zs)
+    return [z[0] for z in zs]
+
+
+def _z_errors(sd, cfg, cond, rvq1, lens, got_z, forced, utts):
+    """per stage: (GPU max-rel, GPU rms-rel, fp32 oracle max-rel, fp32 oracle rms-rel), over the valid rows of `utts`"""
+    per = [([], [], []) for _ in range(got_z.shape[0])]
+    for b in utts:
+        n = int(lens[b]) if lens is not None else cond.shape[1]
+        args = (cond[b:b + 1, :n], rvq1[b:b + 1, :n], forced[b:b + 1, :n])
+        z64 = _oracle_z(sd, cfg, *args, torch.float64)
+        z32 = _oracle_z(sd, cfg, *args, torch.float32)
+        for s in range(got_z.shape[0]):
+            per[s][0].append(got_z[s, b, :n])
+            per[s][1].append(z32[s])
+            per[s][2].append(z64[s])
+    out = []
+    for g, f, r in per:
+        g, f, r = torch.cat(g), torch.cat(f), torch.cat(r)
+        out.append(P.rel_errors(g, r) + P.rel_errors(f, r))
+    return out
+
+
+def _assert_kappa(errs, label):
+    for s, (eg, rg, ef, rf) in enumerate(errs):
+        print(f"{label} stage {s}: GPU max {eg:.2e} rms {rg:.2e} | fp32 oracle max {ef:.2e} rms {rf:.2e} | ratio max {eg / ef:.2f} "
+              f"rms {rg / rf:.2f}")
+    for s, (eg, rg, ef, rf) in enumerate(errs):
+        assert eg <= P.KAPPA * ef and rg <= P.KAPPA * rf, (label, s, eg / ef, rg / rf)
+
+
+@pytest.mark.parametrize("mode", [0, -1])
+@pytest.mark.parametrize("B,T", [(1, 6), (1, 16), (1, 17), (3, 129), (1, 401)])
+def test_nar_stage_activations_against_float64(B, T, mode):
+    """Teacher-forced on the oracle's codes, every stage's z (nar.pre's output) against the float64 oracle: the GPU's
+    relative error, max and RMS, is at most KAPPA (oracle/dense_probes.py) times the fp32 CPU oracle's on the same input.
+    mode 0 = fp32 FMA kernels, -1 = the default (tensor cores above 16 rows)."""
+    eng = _engine()
+    cfg, sd, _ = e2e_inputs()
+    cond = _cond(B, T, int(cfg.d_model), 9400 + 3 * T)
+    rvq1 = torch.randint(0, 2048, (B, T), generator=torch.Generator().manual_seed(T + 5))
+    lens = torch.tensor([T, T // 2 + 1, 1][:B]) if B > 1 else None
+    forced = torch.zeros((B, T, int(cfg.num_codebooks)), dtype=torch.long)
+    for b in range(B):
+        n = T if lens is None else int(lens[b])
+        forced[b, :n] = N.nar_refine(sd, cfg, cond[b:b + 1, :n], rvq1[b:b + 1, :n])[0][0]
+    eng.set_contraction(mode)
+    try:
+        _ids, z = _traced(eng, cond, rvq1, lens, forced)
+    finally:
+        eng.set_contraction(-1)
+    _assert_kappa(_z_errors(sd, cfg, cond, rvq1, lens, z, forced, range(B)), f"B={B} T={T} mode={mode}")
+
+
+def test_batch64_crosses_every_head_chunk():
+    """synthesize_batch's geometry: 64 utterances x 401 frames = 25,664 rows on the default tensor-core path, where the head
+    logits run in chunks of mc rows (nar_engine.cu: 256 MB of logits per chunk; 2048 rows for V = 2048 and 16 heads).  The
+    utterances holding rows mc j - 1 and mc j of every chunk boundary, plus the first and the last, are checked: ids against
+    the oracle (the _check near-tie rule, teacher-forced) and every stage's z against float64."""
+    eng = _engine()
+    cfg, sd, _ = e2e_inputs()
+    B, T, D, V, Q = 64, 401, int(cfg.d_model), int(cfg.codebook_size), int(cfg.num_codebooks)
+    M = B * T
+    heads = max(len(idx) for _n, idx in _stages(cfg))
+    mc = ((256 << 20) // (heads * V * 4)) // 128 * 128
+    mc = max(128, min(mc, (M + 127) // 128 * 128))
+    bounds = list(range(mc, M, mc))
+    assert len(bounds) >= 12, (mc, len(bounds))  # 13 chunks at the default geometry
+    rows = [r for m0 in bounds for r in (m0 - 1, m0)]
+    sel = sorted({r // T for r in rows} | {0, B - 1})
+    lens = torch.full((B,), T)
+    short = [b for b in range(1, B - 1) if b not in sel][:5]
+    for b, n in zip(short, (1, 17, 200, 399, 128)):
+        lens[b] = n
+    assert all(r % T < int(lens[r // T]) for r in rows), "every boundary row is a valid frame"
+    cond = torch.stack([_unit(T * D, 12000 + b).view(T, D) for b in range(B)])
+    rvq1 = torch.randint(0, V, (B, T), generator=torch.Generator().manual_seed(64))
+    got = eng.refine(cond, rvq1, lens).cpu()
+    want = got.clone()
+    margin = torch.full(got.shape, float("inf"))
+    for b in sel:
+        n = int(lens[b])
+        w, m = N.nar_refine(sd, cfg, cond[b:b + 1, :n], rvq1[b:b + 1, :n])
+        want[b, :n], margin[b, :n] = w[0], m[0]
+    tf, z = _traced(eng, cond, rvq1, lens, want)
+    for b in range(B):
+        got[b, int(lens[b]):] = 0
+        tf[b, int(lens[b]):] = 0
+        want[b, int(lens[b]):] = 0
+    sel_t = torch.tensor(sel)
+    n_diff = int((got[sel_t] != want[sel_t]).sum())
+    bad = [(b, t, q) for b, t, q in (tf != want).nonzero().tolist() if b in sel]
+    ties = [((b, t, q), float(margin[b, t, q])) for b, t, q in bad]
+    print(f"batch 64 x 401: {len(bounds) + 1} head chunks of {mc} rows, {len(sel)} utterances checked, {n_diff} ids differ, "
+          f"teacher-forced near-ties {ties}")
+    assert all(m < 1e-5 for _i, m in ties), f"NAR ids differ away from a tie: {ties}"
+    assert len(ties) <= max(2, len(sel) * T * Q // 20000), ties
+    _assert_kappa(_z_errors(sd, cfg, cond, rvq1, lens, z, want, sel), "B=64 T=401")
+
+
+def test_nar_engines_on_two_devices_in_one_process():
+    """Function attributes (the skinny kernel's 96 KB of shared memory for FFN2, K = 1536) belong to each device's context: a
+    second engine on another device must run the skinny path as the first does."""
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two CUDA devices")
+    from sopro_b200.nar import NarEngine
+
+    eng0 = _engine()
+    cfg, sd, _ = e2e_inputs()
+    cond = _cond(1, 9, int(cfg.d_model), 9555)
+    rvq1 = torch.randint(0, 2048, (1, 9), generator=torch.Generator().manual_seed(9))
+    a = eng0.refine(cond, rvq1).cpu()
+    eng1 = NarEngine(cfg, sd, 1)
+    try:
+        b = eng1.refine(cond, rvq1).cpu()
+    finally:
+        eng1.close()
+    assert torch.equal(a, b)

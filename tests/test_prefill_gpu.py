@@ -1,6 +1,7 @@
 """GPU parity of the CUDA prefill (sopro_prefill_run through the C-ABI) against (a) rows the unmodified reference
 wrote (tests/golden/e2e_prefill.npz) and (b) the torch-CPU restatement sopro_b200/prefill.py, which is bit-equal to the
 reference on CPU (tests/test_host_cpu.py).  cond_ar / txt_seq are inputs of the id-exact AR kernel: tolerance 2e-5."""
+import dataclasses
 import os
 
 import numpy as np
@@ -114,9 +115,9 @@ def test_refprep_matches_reference_fixture_rows():
     assert abs(float(sv.norm()) - 1.0) < 1e-5 and caches[0]["key_padding_mask"] is None
 
 
-@pytest.mark.parametrize("Tr,seed", [(1, 3), (5, 4), (38, 5), (150, 6)])
+@pytest.mark.parametrize("Tr,seed", [(1, 3), (5, 4), (38, 5), (150, 6), (769, 7), (1500, 8), (4096, 9)])
 def test_refprep_equals_the_cpu_restatement(Tr, seed):
-    """Every output tensor against sopro_b200/prefill.py on the CPU, short and long voices."""
+    """Every output tensor against sopro_b200/prefill.py on the CPU, short and long voices (up to the 4096-frame limit)."""
     from sopro_b200 import prefill as P
 
     rp = _refprep()
@@ -130,6 +131,34 @@ def test_refprep_equals_the_cpu_restatement(Tr, seed):
         for n in ("k", "v"):
             assert got[n].shape == ref[n].shape
             assert float((got[n].cpu() - ref[n]).abs().max()) <= 2e-5 * max(1.0, float(ref[n].abs().max()))
+
+
+@pytest.mark.parametrize("Tr", [769, 1500, 4096])
+def test_prefill_with_a_long_reference_equals_the_cpu_restatement(Tr):
+    """Above 768 reference frames the cross-attention kernel needs more than 48 KB of shared memory per CTA (its opt-in
+    branch); up to the 4096-frame limit it must still equal the CPU restatement.  4097 frames are refused."""
+    from sopro_b200 import _lib
+    from sopro_b200 import prefill as P
+
+    eng, _, (tpos, fpos) = _setup()
+    rp = _refprep()
+    cfg, sd, inp = e2e_inputs()
+    tok = torch.randint(0, 2048, (Tr, 32), generator=torch.Generator().manual_seed(Tr))
+    ref = P.prepare_reference(sd, cfg, tok, torch.device("cpu"))
+    texts = [inp["text_ids"], inp["text_ids"][:9]]
+    F = 40
+    txt, lens, pool, cond = eng.run(texts, ref, n_frames=F + 1, style_strength=1.0)
+    for i, ids in enumerate(texts):
+        want = P.prepare_conditioning(sd, cfg, ids, ref, max_frames=F, device="cpu", style_strength=1.0, text_pos=tpos, frame_pos=fpos)
+        err = float((cond[i].cpu() - want["cond_ar"][0]).abs().max())
+        assert err <= 2e-5, (Tr, i, err)
+    long_tok = torch.zeros((4097, 32), dtype=torch.long)
+    with pytest.raises(_lib.SoproError):
+        rp.run(long_tok)
+    kv = [{"k": c["k"].new_zeros((1, c["k"].shape[1], 4097, c["k"].shape[3])), "v": c["v"].new_zeros((1, c["v"].shape[1], 4097, c["v"].shape[3])),
+           "key_padding_mask": None} for c in ref.ref_kv_caches]
+    with pytest.raises(_lib.SoproError):
+        eng.run(texts, dataclasses.replace(ref, ref_kv_caches=kv), n_frames=F + 1, style_strength=1.0)
 
 
 def test_refprep_rejects_codes_outside_the_codebook():

@@ -713,6 +713,32 @@ int sopro_loudness_measure(const float* x, int32_t B, int64_t x_stride, const in
 int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, double T,
                              float* y, int64_t y_stride, void* ws, double* lufs_dev, float* gain_dev, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Long-form synthesis (no reference counterpart: the reference speaks one utterance of at most max_frames): the speech
+ * extent of each segment's decoded 24 kHz row, and the join of those extents into one waveform.
+ *   Extents: the energy trim of the reference's trim_silence_energy at 24 kHz.  For a row of n samples, frames of 600
+ *   samples every 240, K = floor((n - 600) / 240) + 1; e_k = sum x^2 / 600 and dB_k = 10 log10(e_k + 1e-10), in fp64;
+ *   thr = max(max_k dB_k - 40, -40); frame k is voiced when dB_k > thr; start = max(0, first * 240 - 720),
+ *   end = min(n, last * 240 + 600 + 720).  The extent is (0, n) when n < 2400, no frame is voiced, or end - start < 12000.
+ *   Each frame's sum has a fixed order, so a row gets the same extent alone or in any ragged batch.
+ *   Join: for each non-empty extent in order, x[start, end) with its first and last F = min(240, floor(span / 2)) samples
+ *   faded: y = x * f[i] for the i-th sample from the span's start and from its end, one fp32 multiply, with
+ *   f[i] = 0.5 - 0.5 cos(pi (i + 0.5) / F) evaluated in double on the host and rounded to fp32 once; P zero samples
+ *   between consecutive spans, none before the first or after the last.  The output has sum(spans) + (spans - 1) P
+ *   samples. */
+/* host-only: the fade's F taps -> f [F]; SOPRO_ERR_INVALID for F outside [0, 240] */
+int sopro_longform_fade(int32_t F, float* f);
+/* ragged batch, one launch per 128 rows: row b of x [B][x_stride] f32 (device) has lens_host[b] samples (HOST i64;
+ * NULL = x_stride each); samples at or past lens[b] are not read.  (start, end) of row b -> ext [B][2] (device i64).
+ * No call synchronises or allocates. */
+int sopro_longform_extents(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int64_t* ext, void* stream);
+/* src: HOST array of n_seg device pointers, segment i's row of lens_host[i] samples (HOST i64), read in place;
+ * ext_host: HOST i64 [n_seg][2], each 0 <= start <= end <= lens[i] (an empty extent is skipped, its src may be NULL);
+ * pause: P in [0, 48000] samples.  y (device f32) receives the joined waveform; y_len must equal its length.  Bad
+ * geometry is SOPRO_ERR_INVALID before any launch.  No call synchronises or allocates. */
+int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host, int64_t pause,
+                        float* y, int64_t y_len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -238,6 +238,9 @@ SYMBOLS = {
     "sopro_loudness_measure": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, _VP, _VP, _VP]),
     "sopro_loudness_normalize": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, C.c_double, _VP, C.c_int64, _VP, _VP,
                                       _VP, _VP]),
+    "sopro_longform_fade": (_I, [C.c_int32, _VP]),
+    "sopro_longform_extents": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP]),
+    "sopro_longform_join": (_I, [_VP, C.c_int32, _VP, _VP, C.c_int64, _VP, C.c_int64, _VP]),
 }
 
 _lib = None

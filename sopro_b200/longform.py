@@ -1,0 +1,232 @@
+"""Long-form synthesis (no reference counterpart: the reference speaks one utterance of at most max_frames, about 32 s).
+
+``split_text`` cuts a text into segments the model can speak; ``SoproTTS.synthesize_long`` generates them side by side
+through the batch path and joins them on the GPU.  The two GPU stages are public too, so a caller with their own
+``synthesize_batch`` outputs can join them the same way: ``speech_extents`` finds each decoded row's speech (the energy
+trim of sopro_b200.audio.trim_silence_energy at 24 kHz, one launch for a ragged batch) and ``join_segments`` joins the
+extents with a fixed pause and raised-cosine edges.  The kernels are sopro_b200/csrc/longform.cu, the contract is in
+include/sopro_b200.h."""
+from __future__ import annotations
+
+import ctypes as C
+import math
+import numbers
+import re
+from typing import List, Optional, Sequence, Union
+
+import numpy as np
+import torch
+
+from . import _lib
+
+SAMPLE_RATE = 24000       # the codec's rate: both stages work on the decoded rows
+FADE = 240                # the longest fade, 10 ms
+MAX_PAUSE_MS = 2000.0
+MIN_TOKENS = 4
+SEGMENT_GROUP = 64        # segments per synthesize_batch pass of synthesize_long
+
+_PARAGRAPH = re.compile(r"\n\s*\n")
+_TERMINATOR = re.compile("[.!?…]+[\"'”’)\\]]*")   # a maximal run of . ! ? ..., then closing quotes / brackets
+_CLAUSE = re.compile("[,;:—–](?= )")                   # a clause mark followed by whitespace
+
+
+def _check(rc: int) -> None:
+    """SOPRO_ERR_INVALID (bad geometry) is a ValueError; anything else a SoproError."""
+    if rc == -1:
+        msg = _lib.load().sopro_last_error()
+        raise ValueError(msg.decode() if msg else "invalid argument")
+    _lib.check(rc)
+
+
+# ---- text segmentation (host)
+
+def _sentences(par: str) -> List[str]:
+    """A normalised paragraph (single spaces, stripped) -> its sentences.  A boundary follows a terminator run and its
+    closing quotes or brackets when a space or the paragraph's end follows, unless the next character is lowercase."""
+    out, a = [], 0
+    for m in _TERMINATOR.finditer(par):
+        e = m.end()
+        if e < len(par) and (par[e] != " " or par[e + 1].islower()):
+            continue
+        out.append(par[a:e])
+        a = e + 1
+    if a < len(par):
+        out.append(par[a:])
+    return out
+
+
+def _cut(sentence: str, fits) -> List[str]:
+    """An over-long sentence -> pieces: at the last clause mark whose left piece fits, else at the last space whose left
+    piece fits, repeated on the rest; a space-free run that does not fit on its own is a piece of its own.  Candidates
+    are tried left to right up to the first that does not fit (with token counts that grow with the text, as for a
+    tokenizer that splits on whitespace first, that is the last one that fits)."""
+    pieces, rest = [], sentence
+    while not fits(rest):
+        cut = None
+        for marks, keep in ((_CLAUSE, 1), (re.compile(" "), 0)):
+            for m in marks.finditer(rest):
+                if not fits(rest[: m.start() + keep]):
+                    break
+                cut = m.start() + keep
+            if cut is not None:
+                break
+        if cut is None:  # the first word alone is over the budget
+            sp = rest.find(" ")
+            if sp < 0:
+                break
+            cut = sp
+        pieces.append(rest[:cut])
+        rest = rest[cut + 1:]  # (every cut is at a space of the normalised text)
+    pieces.append(rest)
+    return pieces
+
+
+def split_text(text: str, tokenizer, max_tokens: int = 64) -> List[str]:
+    """A text -> the segments ``synthesize_long`` speaks, in order.  Pure and deterministic:
+
+    1. Paragraphs: the text splits on blank lines (``\\n\\s*\\n``); inside a paragraph whitespace runs collapse to one
+       space and the ends are stripped; empty paragraphs are dropped.  No segment spans two paragraphs.
+    2. Sentences: a boundary follows a maximal run of ``.``, ``!``, ``?`` or ``…`` plus any closing quotes or brackets
+       (``"'”’)]``) when whitespace or the paragraph's end follows, except when the next non-space character is a
+       lowercase letter ("e.g. this", "approx. five").  There is no abbreviation list, so "Dr. Smith" splits.
+    3. Packing: consecutive sentences of a paragraph merge greedily while the merged segment's token count,
+       ``len(tokenizer.encode(segment))`` (BOS and EOS included), stays <= max_tokens.
+    4. A sentence over the budget is cut at the last clause mark (``,`` ``;`` ``:`` ``—`` ``–`` followed by whitespace)
+       whose left piece fits, failing that at the last whitespace whose left piece fits, and again on the rest; its
+       pieces are segments of their own.  A whitespace-free run over the budget is a segment of its own (its audio is
+       bounded by max_frames, as in ``synthesize``).
+
+    For each paragraph, ``" ".join(its segments)`` is the normalised paragraph; every segment is non-empty and fits the
+    budget, except a whitespace-free run that does not fit alone."""
+    budget = int(max_tokens)
+
+    def fits(s: str) -> bool:
+        return len(tokenizer.encode(s)) <= budget
+
+    out: List[str] = []
+    for raw in _PARAGRAPH.split(text):
+        par = " ".join(raw.split())
+        if not par:
+            continue
+        cur: Optional[str] = None
+        for s in _sentences(par):
+            if not fits(s):
+                if cur is not None:
+                    out.append(cur)
+                    cur = None
+                out.extend(_cut(s, fits))
+            elif cur is None:
+                cur = s
+            elif fits(cur + " " + s):
+                cur = cur + " " + s
+            else:
+                out.append(cur)
+                cur = s
+        if cur is not None:
+            out.append(cur)
+    return out
+
+
+def check_pause(pause_ms) -> float:
+    """The pause between segments in ms as a float; ValueError for anything but a real number in [0, 2000].  Host only."""
+    if isinstance(pause_ms, (bool, np.bool_)) or not isinstance(pause_ms, numbers.Real) or \
+            not (0.0 <= float(pause_ms) <= MAX_PAUSE_MS):
+        raise ValueError(f"pause_ms must be a real number in [0, {MAX_PAUSE_MS:g}], got {pause_ms!r}")
+    return float(pause_ms)
+
+
+def check_max_tokens(max_tokens, limit: int) -> int:
+    """The segment budget as an int; ValueError for anything but an integer in [4, limit] (limit: the prefill's
+    max_text_len).  Host only."""
+    if isinstance(max_tokens, (bool, np.bool_)) or not isinstance(max_tokens, numbers.Integral) or \
+            not (MIN_TOKENS <= int(max_tokens) <= int(limit)):
+        raise ValueError(f"max_tokens must be an integer in [{MIN_TOKENS}, {int(limit)}], got {max_tokens!r}")
+    return int(max_tokens)
+
+
+def pause_samples(pause_ms) -> int:
+    """P = round(pause_ms * 24), the pause in samples at 24 kHz (half to even)."""
+    return int(round(check_pause(pause_ms) * 24))
+
+
+def fade_length(span: int) -> int:
+    """F = min(240, floor(span / 2))."""
+    return min(FADE, int(span) // 2)
+
+
+def fade_window(F: int) -> np.ndarray:
+    """The F fp32 fade taps the join uses: 0.5 - 0.5 cos(pi (i + 0.5) / F) in double, rounded once.  Host only."""
+    f = np.zeros(int(F), dtype=np.float32)
+    _check(_lib.load().sopro_longform_fade(int(F), f.ctypes.data if F else None))
+    return f
+
+
+def joined_length(extents, pause: int) -> int:
+    """sum(spans) + (spans - 1) * P over the non-empty extents (host int64 [n, 2]); 0 when every extent is empty."""
+    spans = [int(e) - int(s) for s, e in np.asarray(extents, dtype=np.int64).reshape(-1, 2) if int(e) > int(s)]
+    return sum(spans) + max(0, len(spans) - 1) * int(pause)
+
+
+def _stream_ptr(device: torch.device) -> int:
+    return int(torch.cuda.current_stream(device).cuda_stream)
+
+
+def speech_extents(wav: torch.Tensor, lens: Optional[Sequence[int]] = None) -> torch.Tensor:
+    """wav [..., L] 24 kHz on a CUDA device (rows = the leading dims flattened) -> int64 [rows, 2] (start, end) of each
+    row's speech, on the device (nothing synchronises).  `lens`: valid samples per row (a ragged batch); samples past
+    lens[b] are not read."""
+    if wav.device.type != "cuda":
+        raise _lib.SoproError("speech extents need CUDA tensors; there is no CPU path")
+    L = int(wav.shape[-1])
+    B = math.prod(tuple(wav.shape[:-1]))
+    x = wav.detach().to(dtype=torch.float32).reshape(B, L).contiguous()
+    ext = torch.empty((B, 2), dtype=torch.int64, device=x.device)
+    if B == 0:
+        return ext
+    lp = None
+    if lens is not None:
+        if len(lens) != B:
+            raise ValueError(f"lens has {len(lens)} entries for {B} rows")
+        lp = (C.c_int64 * B)(*[int(v) for v in lens])
+    with torch.cuda.device(x.device):
+        _check(_lib.load().sopro_longform_extents(x.data_ptr(), B, L, lp, ext.data_ptr(), _stream_ptr(x.device)))
+    return ext
+
+
+def _rows(rows_or_chunks) -> List[torch.Tensor]:
+    """A tensor [..., L] (its rows) or a sequence of tensors (each one's rows, in order) -> 1-D fp32 CUDA rows."""
+    parts = [rows_or_chunks] if isinstance(rows_or_chunks, torch.Tensor) else list(rows_or_chunks)
+    out = []
+    for t in parts:
+        if t.device.type != "cuda":
+            raise _lib.SoproError("the join needs CUDA tensors; there is no CPU path")
+        t = t.detach().to(dtype=torch.float32)
+        t = t.reshape(1, -1) if t.dim() <= 1 or math.prod(tuple(t.shape[:-1])) == 1 else t.reshape(-1, t.shape[-1])
+        if t.numel() and t.stride(-1) != 1:
+            t = t.contiguous()
+        out.extend(t[i] for i in range(t.shape[0]))
+    return out
+
+
+def join_segments(rows_or_chunks: Union[torch.Tensor, Sequence[torch.Tensor]], extents, pause_ms) -> torch.Tensor:
+    """Segment rows and their extents -> one waveform [1, 1, N] f32 on the rows' device: each non-empty extent in order,
+    its first and last F = min(240, span // 2) samples faded by a raised cosine, round(pause_ms * 24) zeros between
+    consecutive spans.  `rows_or_chunks`: a tensor whose rows are the segments (padded decode chunks [rows, 1, L]), or a
+    sequence of them and of single rows; each row is read in place.  `extents`: int64 [segments, 2]; on the device, it
+    is copied to the host here, the one synchronisation."""
+    P = pause_samples(pause_ms)
+    rows = _rows(rows_or_chunks)
+    ext = (extents.detach().to("cpu") if isinstance(extents, torch.Tensor) else torch.as_tensor(extents)).to(torch.int64)
+    ext = np.ascontiguousarray(ext.numpy().reshape(-1, 2))
+    n = len(rows)
+    if n == 0 or ext.shape[0] != n:
+        raise ValueError(f"{ext.shape[0]} extents for {n} segment rows")
+    dev = rows[0].device
+    N = joined_length(ext, P)
+    y = torch.empty((1, 1, N), dtype=torch.float32, device=dev)
+    src = (C.c_void_p * n)(*[r.data_ptr() if r.numel() else None for r in rows])
+    lens = (C.c_int64 * n)(*[int(r.numel()) for r in rows])
+    with torch.cuda.device(dev):
+        _check(_lib.load().sopro_longform_join(src, n, lens, ext.ctypes.data, P, y.data_ptr() if N else None, N,
+                                               _stream_ptr(dev)))
+    return y

@@ -18,6 +18,7 @@ from typing import Dict, Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
+from . import longform as LF
 from . import prefill as P
 from .codec import MimiCodec
 from .config import TARGET_SR, SoproTTSConfig
@@ -624,41 +625,11 @@ class SoproTTS:
         rs = self._resampler(sample_rate)
         stretch_on = check_speed(speed) is not None
         target = check_loudness(loudness)
-        st = float(style_strength if style_strength is not None else self.cfg.style_strength)
-        model = self.model
-        ids = [self.encode_text(t) for t in texts]
-        txt_seq, lens, _pool, cond = model.prefill.run(ids, ref, n_frames=int(max_frames) + 1, style_strength=st)
-        toks, n = model.ar_generate_tensors(cond, txt_seq, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                            anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds)
-        eos, B = model.eos_id, len(texts)
-        Ts = []
-        for i in range(B):
-            row = toks[i, : n[i]]
-            hit = (row == eos).nonzero()[0]
-            Ts.append(int(hit[0]) if hit.size else int(n[i]))
+        Ts, codes = self._batch_codes(texts, ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                      anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
+                                      seeds=seeds)
         out: List[torch.Tensor] = [torch.zeros(1, 1, 0, device=self.device) for _ in texts]
-        Tmax = max(Ts)
-        if Tmax == 0:
-            return out
-        # NAR refiner over the ragged batch (not causal: `lens` makes the padding act as each utterance's zero padding)
-        rvq1 = torch.from_numpy(toks[:, :Tmax].copy()).to(self.device)
-        codes = model.nar_refine(cond[:, :Tmax], rvq1.clamp_(0, eos - 1), lens=torch.tensor(Ts, dtype=torch.int32))  # [B, Tmax, Q]
-        # Mimi decode is causal and per-utterance: right-pad to the longest of a chunk, decode together, cut
-        live = sorted((i for i in range(B) if Ts[i] > 0), key=lambda i: -Ts[i])
-        hop = self.codec.engine.hop
-        cap = 12800  # frames per decode call (workspace bound)
-        while live:
-            chunk, frames = [], 0
-            while live and (not chunk or (len(chunk) + 1) * max(frames, Ts[live[0]]) <= cap):
-                frames = max(frames, Ts[live[0]])
-                chunk.append(live.pop(0))
-            idx = torch.tensor(chunk, device=self.device)
-            batch = codes[idx, :frames].permute(0, 2, 1).to(torch.int32)
-            keep = torch.arange(frames, device=self.device)[None, :] < torch.tensor([Ts[i] for i in chunk], device=self.device)[:, None]
-            batch = (batch * keep[:, None, :]).contiguous()  # padding frames decode code 0; their samples are cut below
-            wav = self.codec.engine.decode(batch)
-            # the padding past Ts[i] * hop holds decoded filler: lens keeps the time-stretch and the resampler from reading it
-            lens = [Ts[i] * hop for i in chunk]
+        for chunk, wav, lens in self._decode_chunks(codes, Ts):
             if stretch_on:
                 wav = stretch(wav.view(len(chunk), -1), speed, lens=lens).unsqueeze(1)
                 lens = [stretched_length(speed, n) for n in lens]
@@ -671,6 +642,100 @@ class SoproTTS:
             for j, i in enumerate(chunk):
                 out[i] = wav[j: j + 1, :, : lens[j]].clone()
         return out
+
+    @torch.inference_mode()
+    def synthesize_long(self, text: str, *, ref: PreparedReference, max_frames: int = 400, max_tokens: int = 64,
+                        pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                        style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
+                        seed: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
+                        loudness: Optional[float] = None) -> torch.Tensor:
+        """NEW: a text of any length -> one waveform [1, 1, N] f32 on the device.  The text is cut into segments of at
+        most `max_tokens` tokens (sopro_b200/longform.py::split_text: paragraphs, sentences, greedy packing); the
+        segments are generated side by side through the batch path, SEGMENT_GROUP at a time (segment i equals
+        synthesize(segment, seed=seed + i); without a seed the global generator is consumed segment after segment, as by
+        synthesize_batch), each decoded row is trimmed to its speech on the GPU, and the rows are joined with
+        `pause_ms` (in [0, 2000]) of silence between them and 10 ms raised-cosine edges.  The joined 24 kHz row then goes
+        through the chain of synthesize: stretch (`speed`, pauses included), resample (`sample_rate`), loudness (one
+        level for the whole passage).  Segments that produced no frames are skipped; if none did, the result is
+        [1, 1, 0].  Every argument is checked before any work."""
+        rs = self._resampler(sample_rate)
+        stretch_on = check_speed(speed) is not None
+        target = check_loudness(loudness)
+        LF.check_pause(pause_ms)
+        budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
+        segments = LF.split_text(text, self.tokenizer, budget)
+        if not segments:
+            raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
+        B, group = len(segments), int(LF.SEGMENT_GROUP)
+        ext = torch.zeros((B, 2), dtype=torch.int64, device=self.device)
+        rows: List[torch.Tensor] = [torch.zeros(0, device=self.device)] * B
+        for g0 in range(0, B, group):
+            part = segments[g0: g0 + group]
+            seeds = None if seed is None else [int(seed) + g0 + i for i in range(len(part))]
+            Ts, codes = self._batch_codes(part, ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                          anti_loop=anti_loop, style_strength=style_strength,
+                                          min_gen_frames=min_gen_frames, seeds=seeds)
+            for chunk, wav, lens in self._decode_chunks(codes, Ts):
+                flat = wav.view(len(chunk), -1)
+                ext[torch.tensor([g0 + i for i in chunk], device=self.device)] = LF.speech_extents(flat, lens=lens)
+                for j, i in enumerate(chunk):
+                    rows[g0 + i] = flat[j, : lens[j]]  # read in place by the join
+        wav = LF.join_segments(rows, ext, pause_ms)  # the one host read: the B extents
+        if wav.shape[-1] == 0:
+            return wav
+        if stretch_on:
+            wav = stretch(wav, speed)
+        if rs is not None:
+            wav = rs(wav)
+        if target is not None:
+            wav = normalize_loudness(wav, TARGET_SR if rs is None else rs.sr_out, target)
+        return wav
+
+    def _batch_codes(self, texts: Sequence[str], ref: PreparedReference, *, max_frames: int, top_p: float,
+                     temperature: float, anti_loop: bool, style_strength: Optional[float], min_gen_frames: Optional[int],
+                     seeds: Optional[Sequence[int]]) -> Tuple[List[int], Optional[torch.Tensor]]:
+        """B texts with one prepared reference: one batched prefill, one persistent AR launch, one ragged NAR pass ->
+        (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0 frames)."""
+        st = float(style_strength if style_strength is not None else self.cfg.style_strength)
+        model = self.model
+        ids = [self.encode_text(t) for t in texts]
+        txt_seq, lens, _pool, cond = model.prefill.run(ids, ref, n_frames=int(max_frames) + 1, style_strength=st)
+        toks, n = model.ar_generate_tensors(cond, txt_seq, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                            anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds)
+        eos, B = model.eos_id, len(texts)
+        Ts = []
+        for i in range(B):
+            row = toks[i, : n[i]]
+            hit = (row == eos).nonzero()[0]
+            Ts.append(int(hit[0]) if hit.size else int(n[i]))
+        Tmax = max(Ts)
+        if Tmax == 0:
+            return Ts, None
+        # NAR refiner over the ragged batch (not causal: `lens` makes the padding act as each utterance's zero padding)
+        rvq1 = torch.from_numpy(toks[:, :Tmax].copy()).to(self.device)
+        codes = model.nar_refine(cond[:, :Tmax], rvq1.clamp_(0, eos - 1), lens=torch.tensor(Ts, dtype=torch.int32))  # [B, Tmax, Q]
+        return Ts, codes
+
+    def _decode_chunks(self, codes: Optional[torch.Tensor], Ts: Sequence[int]) -> Iterator[Tuple[List[int], torch.Tensor, List[int]]]:
+        """Padded Mimi decodes of the utterances with frames -> yields (indices, wav [rows, 1, L], valid samples per
+        row), longest utterances first.  The padding past Ts[i] * hop holds decoded filler: every stage after the decode
+        takes the lens so it never reads it."""
+        if codes is None:
+            return
+        # Mimi decode is causal and per-utterance: right-pad to the longest of a chunk, decode together, cut
+        live = sorted((i for i in range(len(Ts)) if Ts[i] > 0), key=lambda i: -Ts[i])
+        hop = self.codec.engine.hop
+        cap = 12800  # frames per decode call (workspace bound)
+        while live:
+            chunk, frames = [], 0
+            while live and (not chunk or (len(chunk) + 1) * max(frames, Ts[live[0]]) <= cap):
+                frames = max(frames, Ts[live[0]])
+                chunk.append(live.pop(0))
+            idx = torch.tensor(chunk, device=self.device)
+            batch = codes[idx, :frames].permute(0, 2, 1).to(torch.int32)
+            keep = torch.arange(frames, device=self.device)[None, :] < torch.tensor([Ts[i] for i in chunk], device=self.device)[:, None]
+            batch = (batch * keep[:, None, :]).contiguous()  # padding frames decode code 0; their samples are cut by lens
+            yield chunk, self.codec.engine.decode(batch), [Ts[i] * hop for i in chunk]
 
     def stream(self, text: str, *, sample_rate: Optional[int] = None, speed: Optional[float] = None,
                **kwargs) -> Iterator[torch.Tensor]:

@@ -752,6 +752,7 @@ struct TeamCtx {
 // ---------------------------------------------------------------------------
 constexpr int kAttGroup = 256;
 constexpr int kAttG = 32;  // upper bound of the key groups (Dh >= 32)
+constexpr int kAttVU = 8;  // value rows per thread requested together
 
 __device__ __forceinline__ void group_sync(int grp) {
   asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "r"(kAttGroup) : "memory");
@@ -767,23 +768,47 @@ __device__ __forceinline__ void attention_item(const ArParams& p, const LayerDev
   const float* __restrict__ Kp = p.kc + kv_off;
   const float* __restrict__ Vp = p.vc + kv_off;
   const float scale = 1.0f / sqrtf((float)Dh);
-  // 1. scores
+  // Every L2 read of an item is a round trip of ~1-2k cycles on a busy GPU, and the item is on the step's critical path:
+  // the key rows of two score rounds, and kAttVU value rows per thread, are requested together.  The sums keep the
+  // order of one key, one value row at a time.
+  // 1. scores: keys l and l + 32 of a round pair, 8 threads per key
   {
     const int sub = gt & 7;
-    for (int l0 = 0; l0 < len; l0 += kAttGroup / 8) {
-      const int l = l0 + (gt >> 3);
-      float sdot = 0.f;
-      if (l < len) {
-        for (int d = sub * 4; d < Dh; d += 32) {
-          const float4 kk = __ldg(reinterpret_cast<const float4*>(Kp + (size_t)l * Dh + d));
-          const float4 qq = *reinterpret_cast<const float4*>(qs + d);
-          sdot += kk.x * qq.x + kk.y * qq.y + kk.z * qq.z + kk.w * qq.w;
+    for (int l0 = 0; l0 < len; l0 += 2 * (kAttGroup / 8)) {
+      const int la = l0 + (gt >> 3), lb = la + kAttGroup / 8;
+      float sa = 0.f, sb = 0.f;
+      for (int d0 = sub * 4; d0 < Dh; d0 += 4 * 32) {
+        float4 ka[4], kb[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int d = d0 + 32 * i;
+          ka[i] = (la < len && d < Dh) ? __ldg(reinterpret_cast<const float4*>(Kp + (size_t)la * Dh + d)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          kb[i] = (lb < len && d < Dh) ? __ldg(reinterpret_cast<const float4*>(Kp + (size_t)lb * Dh + d)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int d = d0 + 32 * i;
+          if (d < Dh) {
+            const float4 qq = *reinterpret_cast<const float4*>(qs + d);
+            if (la < len) {
+              const float4 kk = ka[i];
+              sa += kk.x * qq.x + kk.y * qq.y + kk.z * qq.z + kk.w * qq.w;
+            }
+            if (lb < len) {
+              const float4 kk = kb[i];
+              sb += kk.x * qq.x + kk.y * qq.y + kk.z * qq.z + kk.w * qq.w;
+            }
+          }
         }
       }
-      sdot += __shfl_xor_sync(0xffffffffu, sdot, 1);
-      sdot += __shfl_xor_sync(0xffffffffu, sdot, 2);
-      sdot += __shfl_xor_sync(0xffffffffu, sdot, 4);
-      if (sub == 0 && l < len) sc[l] = sdot * scale;
+      sa += __shfl_xor_sync(0xffffffffu, sa, 1);
+      sa += __shfl_xor_sync(0xffffffffu, sa, 2);
+      sa += __shfl_xor_sync(0xffffffffu, sa, 4);
+      sb += __shfl_xor_sync(0xffffffffu, sb, 1);
+      sb += __shfl_xor_sync(0xffffffffu, sb, 2);
+      sb += __shfl_xor_sync(0xffffffffu, sb, 4);
+      if (sub == 0 && la < len) sc[la] = sa * scale;
+      if (sub == 0 && lb < len) sc[lb] = sb * scale;
     }
   }
   group_sync(grp);
@@ -794,20 +819,32 @@ __device__ __forceinline__ void attention_item(const ArParams& p, const LayerDev
   float sum = 0.f;
   for (int l = lane; l < len; l += 32) sum += expf(sc[l] - mx);
   sum = warp_sum(sum);
-  // 3. partial outputs
+  // 3. partial outputs, keys l = g mod G in ascending order
   const int C4 = Dh >> 2;
   const int G = min(kAttGroup / C4, kAttG);
   {
     const int g = gt / C4, c = gt - g * C4;
     if (g < G) {
       float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int l = g; l < len; l += G) {
-        const float e = expf(sc[l] - mx);
-        const float4 v = __ldg(reinterpret_cast<const float4*>(Vp + (size_t)l * Dh + c * 4));
-        o.x += e * v.x;
-        o.y += e * v.y;
-        o.z += e * v.z;
-        o.w += e * v.w;
+      for (int l0 = g; l0 < len; l0 += kAttVU * G) {
+        float4 vr[kAttVU];
+#pragma unroll
+        for (int j = 0; j < kAttVU; ++j) {
+          const int l = l0 + j * G;
+          vr[j] = l < len ? __ldg(reinterpret_cast<const float4*>(Vp + (size_t)l * Dh + c * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int j = 0; j < kAttVU; ++j) {
+          const int l = l0 + j * G;
+          if (l < len) {
+            const float e = expf(sc[l] - mx);
+            const float4 v = vr[j];
+            o.x += e * v.x;
+            o.y += e * v.y;
+            o.z += e * v.z;
+            o.w += e * v.w;
+          }
+        }
       }
       *reinterpret_cast<float4*>(part + (size_t)g * Dh + c * 4) = o;
     }

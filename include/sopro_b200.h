@@ -739,6 +739,58 @@ int sopro_longform_extents(const float* x, int32_t B, int64_t x_stride, const in
 int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host, int64_t pause,
                         float* y, int64_t y_len, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Lossless FLAC output (RFC 9639; no reference counterpart: the reference's demo sends PCM16): mono, 16 bits per sample,
+ * at a rate sr, an integer in [4000, 192000].  Every choice is fixed, so the device's bytes equal
+ * oracle/flac_oracle.py's.
+ *   Input: each fp32 sample -> trunc(clamp(x, -1, 1) * 32767.0f) (wire.float_to_pcm16le's rule); NaN -> 0.
+ *   Stream: "fLaC", one metadata header (last 1, type 0, length 34), STREAMINFO: min / max block size (u16), min / max
+ *   frame bytes (u24), sr (u20), channels - 1 = 0 (u3), bits - 1 = 15 (u5), total samples (u36), MD5 all zero ("not
+ *   computed").  One-shot: fixed blocking, 4096-sample blocks (the last may be shorter), min = max block 4096, the exact
+ *   frame sizes (0 with no frame) and total.  Stream: variable blocking, min block 16, max 4096, frame sizes and total 0.
+ *   Frame header: 0xFF, 0xF8 (fixed) / 0xF9 (variable); block-size code 1100 for 4096, else 0110 + u8 (n - 1) when
+ *   n <= 256, else 0111 + u16 (n - 1); rate code 0100 8k, 0101 16k, 0110 22.05k, 0111 24k, 1000 32k, 1001 44.1k,
+ *   1010 48k, 1011 96k, 0001 88.2k, 0010 176.4k, 0011 192k, any other 0000 (from STREAMINFO); channels 0000, size
+ *   100, reserved 0; the frame number (fixed) or first sample's number (variable) in FLAC's UTF-8 coding; the block-size
+ *   bytes; CRC-8 (poly 0x07, init 0) over the header.
+ *   Subframe: 0, 6-bit type, wasted-bits flag 0.  Candidates in order CONSTANT (all samples equal), FIXED 0-4, LPC 1-12,
+ *   VERBATIM, order p only when p <= n; each sized exactly, the smallest wins, ties to the earlier.
+ *   LPC: R[l] = sum s[n] s[n - l] (l = 0 .. 12, int64, exact in double); none when R[0] = 0.  Levinson-Durbin in double,
+ *   one IEEE rounding per operation, err = R[0], for p = 1 .. 12: stop if !(err > 0) or err not finite;
+ *   acc = R[p] - a[j] R[p-1-j] (j = 0 .. p-2, in order); k = acc / err; a[j] -= k a[p-2-j] (from the old a); a[p-1] = k;
+ *   stop if any of these is not finite; err *= (1 - k k).  Precision 12: e = frexp exponent of max|a|,
+ *   shift = min(11 - e, 15), the order skipped when max|a| = 0 or shift < 0; error-feedback rounding
+ *   err' += a[j] 2^shift, q = clamp(round(err') (halves away from zero), -2048, 2047), err' -= q.  Residual
+ *   s[n] - ((sum q[j] s[n-1-j]) >> shift), arithmetic shift; fields precision - 1 (u4), shift (s5), q[0 .. p-1] (s12).
+ *   Residual coding: partitioned Rice, u = 2e or -2e - 1; a partition of m residuals costs m (k + 1) + sum(u >> k), k
+ *   the cheapest in 0 .. 14 (method 00, 4-bit parameters) or 0 .. 30 (method 01, 5-bit), ties to the smaller k, no
+ *   escapes; partition order o in 0 .. 8 with n % 2^o = 0 and (n >> o) >= p; per o the cheaper method (ties to 00), then
+ *   the cheapest o (ties to the smaller).  Zero pad to a byte, then CRC-16 (poly 0x8005, init 0) over the frame.
+ * A row's bytes depend only on its own samples. */
+typedef struct SoproFlacStream SoproFlacStream;
+/* host-only: the workspace bytes and the output bound (every row's worst case, VERBATIM plus headers) of one encode of
+ * B rows of at most max_len samples; SOPRO_ERR_INVALID for a refused rate or geometry (max_len < 2^36) */
+int sopro_flac_sizes(int32_t B, int64_t max_len, int32_t sr, int64_t* ws_bytes, int64_t* out_bytes);
+/* ragged batch, one launch of each kernel per 128 rows: row b of x [B][x_stride] f32 (device) has lens_host[b] samples
+ * (HOST i64; NULL = x_stride each); samples at or past lens[b] are not read.  ws: device, sopro_flac_sizes' bytes; out:
+ * device, at least its bound.  Row b's complete stream lands at out + row_off[b], row_bytes[b] bytes (device i64 [B]),
+ * the rows back to back in order.  A refused rate or geometry is SOPRO_ERR_INVALID before any launch.  No call
+ * synchronises or allocates. */
+int sopro_flac_encode(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, void* ws,
+                      uint8_t* out, int64_t* row_off, int64_t* row_bytes, void* stream);
+/* a stream of frames (variable blocking; the header is the stream STREAMINFO above).  Each push of n samples, after the
+ * carried ones, becomes 4096-sample frames and one remainder frame; a remainder under 16 samples (frames that short may
+ * only end a stream) is carried on the device to the next push.  push: ws / out sized by sopro_flac_sizes(1, n + 15);
+ * the frames' bytes -> out, their count -> *nbytes (device i64).  finish: the carried samples as the last frame (none
+ * when nothing is carried), then the state starts over at sample 0.  create allocates the 2 x 16-sample carry. */
+int sopro_flac_stream_create(int32_t sr, SoproFlacStream** out);
+int sopro_flac_stream_destroy(SoproFlacStream* s);
+int sopro_flac_stream_reset(SoproFlacStream* s, int32_t sr);
+/* host-only: samples carried to the next push (0 .. 15); -1 for NULL */
+int64_t sopro_flac_stream_carried(const SoproFlacStream* s);
+int sopro_flac_stream_push(SoproFlacStream* s, const float* x, int64_t n, void* ws, uint8_t* out, int64_t* nbytes, void* stream);
+int sopro_flac_stream_finish(SoproFlacStream* s, void* ws, uint8_t* out, int64_t* nbytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,10 +6,14 @@ Importing the package does not need a GPU; constructing a model does (no CPU fal
 from .config import SoproTTSConfig  # noqa: F401
 
 __version__ = "0.1.0"
-__all__ = ["SoproTTS", "SoproTTSConfig"]
+__all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac"]
 
 
 def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
+    if name in ("encode_flac", "FlacStreamEncoder", "encode_stream_flac"):
+        from . import flac
+
+        return getattr(flac, name)
     if name == "SoproTTS":
         from .model import SoproTTS
 

@@ -749,6 +749,15 @@ class SoproTTS:
 
         save_audio(path, wav_1xT, sr=int(sample_rate))
 
+    def save_flac(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
+        """Writes the waveform (one row on the device) as a lossless 16-bit FLAC file, encoded on the GPU
+        (sopro_b200/flac.py); `sample_rate`: the rate the waveform is at."""
+        from .flac import encode_flac
+
+        data = encode_flac(wav_1xT, sample_rate)
+        with open(path, "wb") as f:
+            f.write(data)
+
     def _resampler(self, sample_rate: Optional[int]) -> Optional[Resampler]:
         """None for the codec's own 24 kHz (no launch); otherwise this rate's cached resampler.  A refused rate raises
         ValueError here, before a caller has consumed any random draws."""

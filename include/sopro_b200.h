@@ -189,6 +189,13 @@ int sopro_ar_set_trace(sopro_ar_session_t* s, float* trace_blocks, float* trace_
  * start, then five per stage (activations staged, weight tiles done, whole CTA done, barrier
  * arrival posted, barrier released). NULL = off */
 int sopro_ar_set_timing(sopro_ar_session_t* s, int64_t* buf, int step);
+/* word timestamps: every later launch stores the text cross-attention weights it applies into probs (device f32,
+ * [steps][n_attn][batch][H][ld], n_attn = the attention layers in ascending order): for every step it computes and every
+ * key l < text_len[b], exp(s_l - max) / sum, a non-finite weight stored as 0.  Entries at l >= text_len[b], and steps a
+ * launch skips (every utterance of a team done), are not written.  The sampled tokens do not change.  NULL = off.
+ * ld < 1 with a buffer is SOPRO_ERR_INVALID; sopro_ar_begin and sopro_ar_run refuse ld < the batch's longest text
+ * (SOPRO_ERR_INVALID, before any launch). */
+int sopro_ar_set_attn_trace(sopro_ar_session_t* s, float* probs, int64_t ld);
 /* copy the sampled (pre-forcing) tokens into dst [batch, steps] i32 (device) */
 int sopro_ar_debug_sampled(sopro_ar_session_t* s, int32_t* dst, void* stream);
 /* copy the text K/V built by sopro_ar_begin into k_dst / v_dst, each
@@ -790,6 +797,22 @@ int sopro_flac_stream_reset(SoproFlacStream* s, int32_t sr);
 int64_t sopro_flac_stream_carried(const SoproFlacStream* s);
 int sopro_flac_stream_push(SoproFlacStream* s, const float* x, int64_t n, void* ws, uint8_t* out, int64_t* nbytes, void* stream);
 int sopro_flac_stream_finish(SoproFlacStream* s, void* ws, uint8_t* out, int64_t* nbytes, void* stream);
+
+/* ---- word alignment (no reference counterpart): the monotonic token -> frame path through the AR step's text
+ * cross-attention weights (sopro_ar_set_attn_trace).  Per utterance b of L = text_len[b] tokens and T = frames[b] frames:
+ *   A[t][l] = sum over s ascending, then h ascending, of (double) probs[t][s][b][h][l], starting from 0.0;
+ *   S[0][0] = A[0][0], S[0][l > 0] = -inf; for t >= 1 S[t][l] = A[t][l] + max(S[t-1][l], S[t-1][l-1]) (S[t-1][-1] = -inf),
+ *   the stay predecessor l winning ties; backtrack from (T-1, L-1).
+ * first [B][ld] (device i32): first[b][l] = the first frame of token l, which owns frames [first[l], first[l+1]) with
+ * first[L] := T; every token gets at least one frame.  Entries l >= L are -1, and so is the whole row when there is no
+ * path (T < L or T == 0, or a path that does not start at (0, 0)).  IEEE double additions and comparisons only. */
+/* host-only: the workspace bytes of one alignment; SOPRO_ERR_INVALID for bad geometry */
+int sopro_align_sizes(int32_t B, int32_t steps, int64_t ld, int64_t* ws_bytes);
+/* probs: device f32 [steps][n_attn][B][H][ld]; text_len_host, frames_host: HOST i32 [B], 1 <= text_len <= min(ld, 2048),
+ * 0 <= frames <= steps; ws: device, sopro_align_sizes' bytes.  One CTA per utterance, one launch per 128 utterances.
+ * Bad geometry is SOPRO_ERR_INVALID before any launch.  No call synchronises or allocates. */
+int sopro_align(const float* probs, int32_t steps, int32_t n_attn, int32_t B, int32_t H, int64_t ld, const int32_t* text_len_host,
+                const int32_t* frames_host, void* ws, int32_t* first, void* stream);
 
 #ifdef __cplusplus
 }

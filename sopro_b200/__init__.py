@@ -6,7 +6,7 @@ Importing the package does not need a GPU; constructing a model does (no CPU fal
 from .config import SoproTTSConfig  # noqa: F401
 
 __version__ = "0.1.0"
-__all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac"]
+__all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac", "WordTiming"]
 
 
 def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
@@ -18,6 +18,10 @@ def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
         from .model import SoproTTS
 
         return SoproTTS
+    if name == "WordTiming":
+        from .timestamps import WordTiming
+
+        return WordTiming
     if name == "PreparedReference":
         from .prefill import PreparedReference
 

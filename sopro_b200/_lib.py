@@ -160,6 +160,7 @@ SYMBOLS = {
     "sopro_ar_set_forced_tokens": (_I, [_VP, _VP]),
     "sopro_ar_set_trace": (_I, [_VP, _VP, _VP]),
     "sopro_ar_set_timing": (_I, [_VP, _VP, _I]),
+    "sopro_ar_set_attn_trace": (_I, [_VP, _VP, C.c_int64]),
     "sopro_ar_debug_sampled": (_I, [_VP, _VP, _VP]),
     "sopro_ar_debug_kv": (_I, [_VP, _VP, _VP, _VP]),
     "sopro_noise_create": (_I, [C.c_uint64, _VP]),
@@ -249,6 +250,8 @@ SYMBOLS = {
     "sopro_flac_stream_carried": (C.c_int64, [_VP]),
     "sopro_flac_stream_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP, _VP, _VP]),
     "sopro_flac_stream_finish": (_I, [_VP, _VP, _VP, _VP, _VP]),
+    "sopro_align_sizes": (_I, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_int64)]),
+    "sopro_align": (_I, [_VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _I32P, _I32P, _VP, _VP, _VP]),
 }
 
 _lib = None

@@ -160,6 +160,9 @@ struct sopro_ar_session {
   float* trace_logits = nullptr;
   long long* timing = nullptr;
   int timing_step = -1;
+  float* attn_trace = nullptr;  // word timestamps: [steps][n_attn][B][H][attn_ld] (null = off)
+  int64_t attn_ld = 0;
+  int max_len = 0;  // longest text of the current batch
   bool begun = false;
   std::vector<UttState> host_st;
   // pinned staging of begin()'s small uploads (text lengths, sampler parameters, initial states): the copies are asynchronous
@@ -563,7 +566,11 @@ int sopro_ar_begin(sopro_ar_session_t* s, int batch, int steps, const float* con
     sd[b].min_gen = q.min_gen_frames;
     sd[b].stop_on_first_eos = q.stop_on_first_eos;
   }
+  const int max_len = *std::max_element(lens.begin(), lens.end());
+  if (s->attn_trace && s->attn_ld < max_len)
+    return fail(SOPRO_ERR_INVALID, "attention trace row stride %lld < longest text %d", (long long)s->attn_ld, max_len);
   CK(cudaSetDevice(e->device));
+  s->max_len = max_len;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   s->B = batch;
   s->steps = steps;
@@ -778,7 +785,8 @@ static int build_tiles(sopro_ar_session* s, int P, int wbuf, bool tc, cudaStream
 
 template <typename WT, int TU, bool LL, bool TC = false>
 static int launch_ar_tu(sopro_ar_session* s, ArParams& p, size_t smem, int grid, cudaStream_t st) {
-  auto kern = ar_persistent_kernel<WT, TU, LL, TC>;
+  // the attention-trace export is its own instantiation, so the untraced kernel's code is not touched by it
+  auto kern = p.attn_trace ? ar_persistent_kernel<WT, TU, LL, TC, true> : ar_persistent_kernel<WT, TU, LL, TC, false>;
   CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem));
@@ -845,6 +853,9 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   p.seq_base = s->seq_base;
   p.timing = s->timing;
   p.timing_step = s->timing_step;
+  p.attn_trace = s->attn_trace;
+  p.attn_ld = s->attn_ld;
+  p.attn_step = (long long)e->n_attn * s->B * e->H * s->attn_ld;
   // ---- team geometry: g teams x P CTAs, Bt utterances per team
   int Bt = s->utts_per_team;
   if (Bt <= 0) {
@@ -1031,6 +1042,8 @@ int sopro_ar_run(sopro_ar_session_t* s, int n_steps, void* stream) {
   const int t0 = s->t_pos;
   const int t1 = std::min(s->steps, t0 + n_steps);
   if (t0 >= t1) return SOPRO_OK;
+  if (s->attn_trace && s->attn_ld < s->max_len)  // a trace set after sopro_ar_begin
+    return fail(SOPRO_ERR_INVALID, "attention trace row stride %lld < longest text %d", (long long)s->attn_ld, s->max_len);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int rc = e->cfg.weight_dtype == SOPRO_W_F32 ? launch_ar<float>(s, t0, t1, st)
                                                : launch_ar<__nv_bfloat16>(s, t0, t1, st);
@@ -1117,6 +1130,14 @@ int sopro_ar_set_trace(sopro_ar_session_t* s, float* trace_blocks, float* trace_
   if (!s) return fail(SOPRO_ERR_INVALID, "null session");
   s->trace_blocks = trace_blocks;
   s->trace_logits = trace_logits;
+  return SOPRO_OK;
+}
+
+int sopro_ar_set_attn_trace(sopro_ar_session_t* s, float* probs, int64_t ld) {
+  if (!s) return fail(SOPRO_ERR_INVALID, "null session");
+  if (probs && ld < 1) return fail(SOPRO_ERR_INVALID, "attention trace row stride must be >= 1 (got %lld)", (long long)ld);
+  s->attn_trace = probs;
+  s->attn_ld = probs ? ld : 0;
   return SOPRO_OK;
 }
 

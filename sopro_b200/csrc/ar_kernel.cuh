@@ -156,6 +156,10 @@ struct ArParams {
   int g, P, Bt;
   int PH;  // fused Q+attention stage: CTAs per head (P / H); rank r serves head r % H, utterances r / H + j*PH
   int t_begin, t_end;
+  // word timestamps (null = off): every cross-attention weight of step t, [steps][n_attn][B][H][attn_ld] fp32,
+  // attn_step = n_attn * B * H * attn_ld floats per step
+  float* attn_trace;
+  long long attn_ld, attn_step;
 };
 
 // ---------------------------------------------------------------------------
@@ -747,6 +751,8 @@ struct TeamCtx {
 //   3. output: thread (g, c) accumulates the keys l = g mod G for the float4 chunk c of the head dimension
 //      (G = 256 / (Dh/4) key groups, one L2 round trip with every load in flight)
 //   4. fixed-order sum over the key groups, normalise, nan_to_num (nn/text.py:128), store
+// TRACE (word timestamps, p.attn_trace set): the group's first warp also stores the weights exp(sc[l] - mx) / sum after 2.
+// The TRACE = false instantiations are the untraced kernels, unchanged.
 // Groups synchronise with named barriers (ids 1, 2), never with the CTA barrier.
 // smem per group: sc[Lp] | part[kAttG][Dh]
 // ---------------------------------------------------------------------------
@@ -754,10 +760,14 @@ constexpr int kAttGroup = 256;
 constexpr int kAttG = 32;  // upper bound of the key groups (Dh >= 32)
 constexpr int kAttVU = 8;  // value rows per thread requested together
 
+// word timestamps: the step the CTA is computing (written only by the TRACE instantiations)
+__shared__ int g_attn_step;
+
 __device__ __forceinline__ void group_sync(int grp) {
   asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "r"(kAttGroup) : "memory");
 }
 
+template <bool TRACE>
 __device__ __forceinline__ void attention_item(const ArParams& p, const LayerDev& L, int b, int h, const float* __restrict__ qs,
                                                float* __restrict__ sc, float* __restrict__ part, int grp, int gt, int ll,
                                                unsigned out_seq) {
@@ -819,6 +829,13 @@ __device__ __forceinline__ void attention_item(const ArParams& p, const LayerDev
   float sum = 0.f;
   for (int l = lane; l < len; l += 32) sum += expf(sc[l] - mx);
   sum = warp_sum(sum);
+  if (TRACE && gt < 32) {  // the weights the output applies (nan_to_num as in 4)
+    float* row = p.attn_trace + (size_t)g_attn_step * p.attn_step + (((size_t)L.attn_slot * p.B + b) * H + h) * p.attn_ld;
+    for (int l = lane; l < len; l += 32) {
+      const float w = expf(sc[l] - mx) / sum;
+      row[l] = isfinite(w) ? w : 0.f;
+    }
+  }
   // 3. partial outputs, keys l = g mod G in ascending order
   const int C4 = Dh >> 2;
   const int G = min(kAttGroup / C4, kAttG);
@@ -869,6 +886,7 @@ __host__ __device__ inline int att_group_floats(int Lmax, int Dh) { return ((Lma
 // The attention stage of the un-fused program (q comes from the q stage through the exchange buffer): work items
 // (utterance, head) round-robin over the team's CTAs, two items at a time per CTA.
 // smem: [qs[Dh] | sc | part] x 2 groups
+template <bool TRACE>
 __device__ __noinline__ void stage_attention(const ArParams& p, int li, int rank, int P, int b0, int nb,
                                              float* __restrict__ smem, int ll, unsigned q_seq, unsigned out_seq) {
   const LayerDev& L = p.layer[li];
@@ -899,7 +917,7 @@ __device__ __noinline__ void stage_attention(const ArParams& p, int li, int rank
       *reinterpret_cast<float4*>(qs + gt * 4) = q4;
     }
     group_sync(grp);
-    attention_item(p, L, b, h, qs, sc, part, grp, gt, ll, out_seq);
+    attention_item<TRACE>(p, L, b, h, qs, sc, part, grp, gt, ll, out_seq);
   }
   __syncthreads();
 }
@@ -1426,7 +1444,7 @@ __device__ __noinline__ void sample_utterance(const ArParams& p, int b, int t, f
 // stage fewer per attention layer than q-stage -> attention-stage.
 // smem (floats): xs[MU][D] | qh[MU][Dh] | [sc | part] x 2 groups,  MU = ceil(Bt / PH)
 // ---------------------------------------------------------------------------
-template <typename WT, bool LL>
+template <typename WT, bool LL, bool TRACE>
 __device__ __forceinline__ void stage_qatt(const ArParams& p, int li, const TeamCtx& tc, WeightRing& ring, int n_tiles,
                                            float* __restrict__ smem, const float* __restrict__ xsrc, unsigned x_seq,
                                            unsigned out_seq, Stamp& ts) {
@@ -1519,7 +1537,7 @@ __device__ __forceinline__ void stage_qatt(const ArParams& p, int li, const Team
 #pragma unroll 1
     for (int j = grp; j < n_my; j += 2) {
       const int u = gi + j * PH;
-      attention_item(p, L, tc.b0 + u, h, qh + (size_t)j * Dh, sc, part, grp, gt, LL ? 1 : 0, out_seq);
+      attention_item<TRACE>(p, L, tc.b0 + u, h, qh + (size_t)j * Dh, sc, part, grp, gt, LL ? 1 : 0, out_seq);
     }
   }
 }
@@ -1527,7 +1545,7 @@ __device__ __forceinline__ void stage_qatt(const ArParams& p, int li, const Team
 // ---------------------------------------------------------------------------
 // the persistent kernel: an interpreter over p.prog with one shared GEMV body
 // ---------------------------------------------------------------------------
-template <typename WT, int TU, bool LL, bool TC = false>
+template <typename WT, int TU, bool LL, bool TC = false, bool TRACE = false>
 __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid_constant__ ArParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ SamplerSmem ssm;
@@ -1608,6 +1626,7 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
       s_tok[threadIdx.x] = tok;
       s_done[threadIdx.x] = dn;
     }
+    if (TRACE && threadIdx.x == 0) g_attn_step = t;
     if (threadIdx.x < p.n_layers) {  // the only integer divisions of the step: one thread per layer
       const int dl = p.layer[threadIdx.x].dil;
       conv_phase[threadIdx.x] = t % dl;
@@ -1960,11 +1979,11 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
         }
         if (kind == K_GLU || kind == K_FFN2 || kind == K_O) x_seq = seq;
       } else if (kind == K_QATT) {
-        stage_qatt<WT, LL>(p, li, tc, ring, stage_tiles[si], act, cur, x_seq, seq, ts);
+        stage_qatt<WT, LL, TRACE>(p, li, tc, ring, stage_tiles[si], act, cur, x_seq, seq, ts);
       } else if (kind == K_ATT) {
         ts.mark();
         ts.mark();
-        stage_attention(p, li, tc.rank, tc.P, tc.b0, tc.nb, act, LL ? 1 : 0, seq - 1, seq);
+        stage_attention<TRACE>(p, li, tc.rank, tc.P, tc.b0, tc.nb, act, LL ? 1 : 0, seq - 1, seq);
       } else {  // K_SAMPLE: utterances round-robin over the team's CTAs
         ts.mark();
         ts.mark();

@@ -219,6 +219,17 @@ class ArSession:
         _lib.check(self.lib.sopro_ar_set_trace(self._h, blocks.data_ptr() if blocks is not None else None,
                                                logits.data_ptr() if logits is not None else None))
 
+    def set_attn_trace(self, probs: Optional[torch.Tensor]) -> None:
+        """Word timestamps: later launches store their text cross-attention weights into `probs`, a device f32 tensor
+        [steps, n_attn, batch, H, ld] (ld >= the batch's longest text); None turns the export off."""
+        if probs is None:
+            self._attn_trace = None
+            _lib.check(self.lib.sopro_ar_set_attn_trace(self._h, None, 0))
+            return
+        assert probs.dtype == torch.float32 and probs.is_contiguous() and probs.device == self.engine.device and probs.dim() == 5
+        self._attn_trace = probs
+        _lib.check(self.lib.sopro_ar_set_attn_trace(self._h, probs.data_ptr(), int(probs.shape[-1])))
+
     def set_timing(self, buf: Optional[torch.Tensor], step: int = -1) -> None:
         self._timing = buf
         _lib.check(self.lib.sopro_ar_set_timing(self._h, buf.data_ptr() if buf is not None else None, int(step)))

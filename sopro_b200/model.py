@@ -20,6 +20,7 @@ import torch
 
 from . import longform as LF
 from . import prefill as P
+from . import timestamps as TS
 from .codec import MimiCodec
 from .config import TARGET_SR, SoproTTSConfig
 from .engine import ArEngine, ArSession, Sampling
@@ -314,14 +315,16 @@ class SoproModel:
     def ar_chunks(self, prep: Dict[str, torch.Tensor], *, max_frames: int, chunk_frames: int = 0, top_p: float = 0.9,
                   temperature: float = 1.05, anti_loop: bool = True, loop_streak: int = 8, recovery_top_p: float = 0.85,
                   recovery_temp: float = 1.2, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-                  generator: Optional[torch.Generator] = None, progress: Optional[dict] = None):
+                  generator: Optional[torch.Generator] = None, progress: Optional[dict] = None,
+                  attn_trace: Optional[torch.Tensor] = None):
         """The persistent kernel driven `chunk_frames` frames per launch (0 = the whole utterance in one launch).
         Yields ``(tokens, finished, prefetch)`` per launch: the frames it produced (ints), whether the utterance is over
         (EOS past min_gen_frames, or max_frames reached), and a callable that enqueues the NEXT launch right away on the
         current CUDA stream -- a streaming consumer queues it behind its own NAR + Mimi work so it runs while the audio is
         handed out; without the call the next launch is enqueued when the generator is resumed.  Frames computed ahead
         of a consumer that stops early are abandoned: on exit the RNG is settled to ``progress["consumed"]`` frames
-        (default: every frame yielded), i.e. exactly the draws the reference would have made."""
+        (default: every frame yielded), i.e. exactly the draws the reference would have made.  `attn_trace` (word
+        timestamps): a [max_frames + 1, n_attn, 1, H, L] buffer that receives the text cross-attention weights."""
         cond, txt = prep["cond_ar"], prep["txt_seq"]
         steps = int(max_frames) + 1
         if cond.size(1) < steps:
@@ -354,6 +357,8 @@ class SoproModel:
             # the session keeps a pointer to this device tape; each launch's rows are drawn and uploaded just before it
             tape = torch.zeros(1, steps, nk, device=self.device)
             stage = torch.empty(steps, nk, pin_memory=True) if self.device.type == "cuda" else None
+            if attn_trace is not None:
+                ses.set_attn_trace(attn_trace)
             ses.begin(cond[:, :steps], txt, [L], tape, samp)
             t = 0
             while t < steps:
@@ -369,6 +374,8 @@ class SoproModel:
                 if finished:
                     break
         finally:
+            if attn_trace is not None:
+                ses.set_attn_trace(None)  # sessions are cached and shared
             self._release(ses)
             noise.settle(int(progress["consumed"]) if progress is not None and "consumed" in progress else st["yielded"])
 
@@ -376,7 +383,8 @@ class SoproModel:
     def ar_stream(self, prep: Dict[str, torch.Tensor], *, max_frames: int, top_p: float = 0.9, temperature: float = 1.05,
                   anti_loop: bool = True, loop_streak: int = 8, recovery_top_p: float = 0.85, recovery_temp: float = 1.2,
                   min_gen_frames: Optional[int] = None, launch_frames: int = 0, seed: Optional[int] = None,
-                  generator: Optional[torch.Generator] = None) -> Iterator[Tuple[int, int, bool]]:
+                  generator: Optional[torch.Generator] = None,
+                  attn_trace: Optional[torch.Tensor] = None) -> Iterator[Tuple[int, int, bool]]:
         """Yields (t, token, is_eos) like the reference generator (model.py:218-305).  The persistent kernel runs
         `launch_frames` frames per launch (0 = the whole utterance in one launch); a consumer that stops iterating
         early simply abandons the frames computed ahead, and the RNG is settled to the frames actually consumed."""
@@ -384,7 +392,7 @@ class SoproModel:
         gen = self.ar_chunks(prep, max_frames=max_frames, chunk_frames=launch_frames, top_p=top_p, temperature=temperature,
                              anti_loop=anti_loop, loop_streak=loop_streak, recovery_top_p=recovery_top_p,
                              recovery_temp=recovery_temp, min_gen_frames=min_gen_frames, seed=seed, generator=generator,
-                             progress=progress)
+                             progress=progress, attn_trace=attn_trace)
         t = 0
         try:
             for chunk, _finished, _prefetch in gen:
@@ -419,14 +427,18 @@ class SoproModel:
     @torch.no_grad()
     def ar_generate_tensors(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int, top_p: float = 0.9,
                             temperature: float = 1.05, anti_loop: bool = True, min_gen_frames: Optional[int] = None,
-                            seeds: Optional[Sequence[int]] = None, stop_on_first_eos: bool = True):
+                            seeds: Optional[Sequence[int]] = None, stop_on_first_eos: bool = True,
+                            attn_trace: Optional[torch.Tensor] = None):
         """B utterances in ONE persistent launch from batch tensors (cond [B, >=steps, D], txt [B, Lmax, D], lens).
-        -> (tokens [B, steps] int32 numpy, n_tokens [B])."""
+        -> (tokens [B, steps] int32 numpy, n_tokens [B]).  `attn_trace` (word timestamps): a [steps, n_attn, B, H, ld]
+        buffer, ld >= max(lens), that receives the text cross-attention weights."""
         B, steps = int(cond.shape[0]), int(max_frames) + 1
         samp = self._sampling(top_p, temperature, anti_loop, 8, 0.85, 1.2, min_gen_frames, stop_on_first_eos)
         nk = self._noise_cols(samp)
         ses = self._checkout(B, steps, max(int(x) for x in lens))
         try:
+            if attn_trace is not None:
+                ses.set_attn_trace(attn_trace)
             if seeds is None or steps < 64:
                 tapes = self._draw_tapes(B, steps, nk, seeds)  # host threads; the prefill kernels queued before run meanwhile
                 ses.begin(cond[:, :steps], txt, [int(x) for x in lens], tapes.to(self.device, non_blocking=True), samp)
@@ -465,6 +477,8 @@ class SoproModel:
                     ses.run(b - a)
             toks, n, _ = ses.read()
         finally:
+            if attn_trace is not None:
+                ses.set_attn_trace(None)  # sessions are cached and shared
             self._release(ses)
         return toks, n
 
@@ -491,12 +505,14 @@ class SoproModel:
     def generate_tokens(self, text_ids_1d: torch.Tensor, ref: PreparedReference, *, max_frames: int, device=None,
                         top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True, style_strength: float = 1.2,
                         min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-                        generator: Optional[torch.Generator] = None) -> torch.Tensor:
-        """reference model.py:349-401: prefill, AR until the first EOS, cut there, NAR refine -> [T, Q] int64."""
+                        generator: Optional[torch.Generator] = None, attn_trace: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """reference model.py:349-401: prefill, AR until the first EOS, cut there, NAR refine -> [T, Q] int64.
+        `attn_trace`: see ar_chunks."""
         prep = self.prepare_conditioning(text_ids_1d, ref, max_frames=max_frames, style_strength=style_strength)
         hist: List[int] = []
         for _t, tok, is_eos in self.ar_stream(prep, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                              anti_loop=anti_loop, min_gen_frames=min_gen_frames, seed=seed, generator=generator):
+                                              anti_loop=anti_loop, min_gen_frames=min_gen_frames, seed=seed, generator=generator,
+                                              attn_trace=attn_trace):
             hist.append(tok)
             if is_eos:
                 break
@@ -586,23 +602,33 @@ class SoproTTS:
                    temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                    ref_seconds: Optional[float] = None, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
                    generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
-                   speed: Optional[float] = None, loudness: Optional[float] = None) -> torch.Tensor:
+                   speed: Optional[float] = None, loudness: Optional[float] = None, word_timestamps: bool = False):
         """-> [1, 1, N] f32 on the device.  `sample_rate` (extension): the output rate in Hz (None = 24 kHz, the codec's
         own); another rate resamples the decoded waveform on the GPU (sopro_b200/resample.py).  `speed` (extension): the
         speaking rate in [0.25, 4.0] (None = the model's own); the 24 kHz waveform is time-stretched on the GPU with its
         pitch kept (sopro_b200/stretch.py), then resampled when `sample_rate` is set.  `loudness` (extension): a target
         integrated loudness in LUFS, [-60, 0] (None = the level the model produced); the final waveform is measured per
-        ITU-R BS.1770-4 and scaled on the GPU under a -1 dBFS sample-peak ceiling (sopro_b200/loudness.py)."""
+        ITU-R BS.1770-4 and scaled on the GPU under a -1 dBFS sample-peak ceiling (sopro_b200/loudness.py).
+        `word_timestamps` (extension): also return when each word is spoken, ``(wav, List[WordTiming])``, from the AR
+        step's text cross-attention (sopro_b200/timestamps.py); the audio is the same as without it."""
         rs = self._resampler(sample_rate)  # a refused rate raises before any work
-        stretch_on = check_speed(speed) is not None  # so does a refused speed
+        S = check_speed(speed)  # so does a refused speed
+        stretch_on = S is not None
         target = check_loudness(loudness)  # and a refused loudness target
         text_ids = self.encode_text(text)
+        trace = spans = None
+        if word_timestamps:
+            spans = self.tokenizer.encode_with_offsets(text)[1]
+            trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, 1, int(text_ids.numel()), self.device)
         if ref is None:
             ref = self.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
         tokens_tq = self.model.generate_tokens(
             text_ids, ref=ref, max_frames=max_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
             style_strength=float(style_strength if style_strength is not None else self.cfg.style_strength),
-            min_gen_frames=min_gen_frames, seed=seed, generator=generator)
+            min_gen_frames=min_gen_frames, seed=seed, generator=generator, attn_trace=trace)
+        words = None
+        if word_timestamps:
+            words = self._timings([text], [spans], trace, [int(text_ids.numel())], [int(tokens_tq.shape[0])], S)[0]
         wav = self.codec.decode_full(tokens_tq)
         if stretch_on:
             wav = stretch(wav, speed)
@@ -610,24 +636,31 @@ class SoproTTS:
             wav = rs(wav)
         if target is not None:
             wav = normalize_loudness(wav, TARGET_SR if rs is None else rs.sr_out, target)
-        return wav
+        return (wav, words) if word_timestamps else wav
 
     @torch.inference_mode()
     def synthesize_batch(self, texts: Sequence[str], *, ref: PreparedReference, max_frames: int = 400, top_p: float = 0.9,
                          temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                          min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                          sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                         loudness: Optional[float] = None) -> List[torch.Tensor]:
+                         loudness: Optional[float] = None, word_timestamps: bool = False):
         """NEW: B texts with one shared prepared reference -> B waveforms [1, 1, N_i].  One batched prefill, one
         persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, then
         loudness-normalised, in one ragged launch when `speed` / `sample_rate` / `loudness` is given); utterance i equals
-        synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness)."""
+        synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness).
+        `word_timestamps`: also return each utterance's word timings (see synthesize), ``(List[wav], List[List[WordTiming]])``."""
         rs = self._resampler(sample_rate)
-        stretch_on = check_speed(speed) is not None
+        S = check_speed(speed)
+        stretch_on = S is not None
         target = check_loudness(loudness)
+        tr: Optional[dict] = {} if word_timestamps else None
         Ts, codes = self._batch_codes(texts, ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
                                       anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
-                                      seeds=seeds)
+                                      seeds=seeds, trace_out=tr)
+        words = None
+        if word_timestamps:
+            spans = [self.tokenizer.encode_with_offsets(t)[1] for t in texts]
+            words = self._timings(texts, spans, tr["probs"], tr["lens"], Ts, S)
         out: List[torch.Tensor] = [torch.zeros(1, 1, 0, device=self.device) for _ in texts]
         for chunk, wav, lens in self._decode_chunks(codes, Ts):
             if stretch_on:
@@ -641,14 +674,14 @@ class SoproTTS:
                                          lens=lens).unsqueeze(1)
             for j, i in enumerate(chunk):
                 out[i] = wav[j: j + 1, :, : lens[j]].clone()
-        return out
+        return (out, words) if word_timestamps else out
 
     @torch.inference_mode()
     def synthesize_long(self, text: str, *, ref: PreparedReference, max_frames: int = 400, max_tokens: int = 64,
                         pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
                         style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
                         seed: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                        loudness: Optional[float] = None) -> torch.Tensor:
+                        loudness: Optional[float] = None, word_timestamps: bool = False):
         """NEW: a text of any length -> one waveform [1, 1, N] f32 on the device.  The text is cut into segments of at
         most `max_tokens` tokens (sopro_b200/longform.py::split_text: paragraphs, sentences, greedy packing); the
         segments are generated side by side through the batch path, SEGMENT_GROUP at a time (segment i equals
@@ -657,9 +690,11 @@ class SoproTTS:
         `pause_ms` (in [0, 2000]) of silence between them and 10 ms raised-cosine edges.  The joined 24 kHz row then goes
         through the chain of synthesize: stretch (`speed`, pauses included), resample (`sample_rate`), loudness (one
         level for the whole passage).  Segments that produced no frames are skipped; if none did, the result is
-        [1, 1, 0].  Every argument is checked before any work."""
+        [1, 1, 0].  Every argument is checked before any work.  `word_timestamps`: also return the passage's word timings
+        (see synthesize), ``(wav, List[WordTiming])``, their char spans in `text`."""
         rs = self._resampler(sample_rate)
-        stretch_on = check_speed(speed) is not None
+        S = check_speed(speed)
+        stretch_on = S is not None
         target = check_loudness(loudness)
         LF.check_pause(pause_ms)
         budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
@@ -669,39 +704,64 @@ class SoproTTS:
         B, group = len(segments), int(LF.SEGMENT_GROUP)
         ext = torch.zeros((B, 2), dtype=torch.int64, device=self.device)
         rows: List[torch.Tensor] = [torch.zeros(0, device=self.device)] * B
+        firsts: List = []
+        all_Ts: List[int] = []
         for g0 in range(0, B, group):
             part = segments[g0: g0 + group]
             seeds = None if seed is None else [int(seed) + g0 + i for i in range(len(part))]
+            tr: Optional[dict] = {} if word_timestamps else None
             Ts, codes = self._batch_codes(part, ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
                                           anti_loop=anti_loop, style_strength=style_strength,
-                                          min_gen_frames=min_gen_frames, seeds=seeds)
+                                          min_gen_frames=min_gen_frames, seeds=seeds, trace_out=tr)
+            if word_timestamps:
+                first = TS.align(tr["probs"], tr["lens"], Ts).cpu().numpy()
+                firsts.extend(first[i] for i in range(len(part)))
+                all_Ts.extend(Ts)
             for chunk, wav, lens in self._decode_chunks(codes, Ts):
                 flat = wav.view(len(chunk), -1)
                 ext[torch.tensor([g0 + i for i in chunk], device=self.device)] = LF.speech_extents(flat, lens=lens)
                 for j, i in enumerate(chunk):
                     rows[g0 + i] = flat[j, : lens[j]]  # read in place by the join
         wav = LF.join_segments(rows, ext, pause_ms)  # the one host read: the B extents
+        words = None
+        if word_timestamps:
+            spans = [self.tokenizer.encode_with_offsets(t)[1] for t in segments]
+            words = TS.long_timings(text, segments, spans, firsts, all_Ts, self.codec.engine.hop, ext.cpu().numpy(),
+                                    LF.pause_samples(pause_ms), S)
         if wav.shape[-1] == 0:
-            return wav
+            return (wav, words) if word_timestamps else wav
         if stretch_on:
             wav = stretch(wav, speed)
         if rs is not None:
             wav = rs(wav)
         if target is not None:
             wav = normalize_loudness(wav, TARGET_SR if rs is None else rs.sr_out, target)
-        return wav
+        return (wav, words) if word_timestamps else wav
+
+    def _timings(self, texts: Sequence[str], spans, probs: torch.Tensor, lens: Sequence[int], Ts: Sequence[int],
+                 S: Optional[int]) -> List[List[TS.WordTiming]]:
+        """The word timings of each utterance from its exported attention weights (one alignment launch)."""
+        first = TS.align(probs, lens, Ts).cpu().numpy()
+        hop = self.codec.engine.hop
+        return [TS.utterance_timings(t, sp, first[i], int(Ts[i]), hop, S) for i, (t, sp) in enumerate(zip(texts, spans))]
 
     def _batch_codes(self, texts: Sequence[str], ref: PreparedReference, *, max_frames: int, top_p: float,
                      temperature: float, anti_loop: bool, style_strength: Optional[float], min_gen_frames: Optional[int],
-                     seeds: Optional[Sequence[int]]) -> Tuple[List[int], Optional[torch.Tensor]]:
+                     seeds: Optional[Sequence[int]], trace_out: Optional[dict] = None) -> Tuple[List[int], Optional[torch.Tensor]]:
         """B texts with one prepared reference: one batched prefill, one persistent AR launch, one ragged NAR pass ->
-        (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0 frames)."""
+        (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0 frames).
+        `trace_out` (word timestamps): receives "probs", the AR launch's attention weights, and "lens", the text lengths."""
         st = float(style_strength if style_strength is not None else self.cfg.style_strength)
         model = self.model
         ids = [self.encode_text(t) for t in texts]
         txt_seq, lens, _pool, cond = model.prefill.run(ids, ref, n_frames=int(max_frames) + 1, style_strength=st)
+        trace = None
+        if trace_out is not None:
+            trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, len(texts), max(int(x) for x in lens), self.device)
+            trace_out["probs"], trace_out["lens"] = trace, [int(x) for x in lens]
         toks, n = model.ar_generate_tensors(cond, txt_seq, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                            anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds)
+                                            anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds,
+                                            attn_trace=trace)
         eos, B = model.eos_id, len(texts)
         Ts = []
         for i in range(B):

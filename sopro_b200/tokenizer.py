@@ -3,8 +3,11 @@ wrapped in BOS/EOS.  ``IdsTokenizer`` is the offline stand-in for synthetic chec
 integer ids, or a deterministic hash of each word into the vocabulary."""
 from __future__ import annotations
 
+import re
 import zlib
-from typing import List
+from typing import List, Optional, Tuple
+
+Span = Optional[Tuple[int, int]]
 
 
 class TextTokenizer:
@@ -26,6 +29,19 @@ class TextTokenizer:
             ids = [self.bos_id] + ids + [self.eos_id]
         return ids
 
+    def encode_with_offsets(self, text: str) -> Tuple[List[int], List[Span]]:
+        """(encode(text), the (start, end) character span of each id in `text`; BOS and EOS have none).  Raises when
+        the offsets pass of the fast tokenizer gives other ids than encode, rather than guessing."""
+        enc = self.tok(text, add_special_tokens=False, return_offsets_mapping=True)
+        ids = [int(i) for i in enc["input_ids"]]
+        spans: List[Span] = [(int(a), int(b)) for a, b in enc["offset_mapping"]]
+        if self.add_bos_eos and self.bos_id is not None and self.eos_id is not None:
+            ids = [self.bos_id] + ids + [self.eos_id]
+            spans = [None] + spans + [None]
+        if ids != self.encode(text):
+            raise ValueError("the tokenizer's offsets pass gives other ids than encode(); cannot map tokens to characters")
+        return ids, spans
+
 
 class IdsTokenizer:
     def __init__(self, vocab_size: int, add_bos_eos: bool = True):
@@ -38,3 +54,10 @@ class IdsTokenizer:
         for w in text.split():
             ids.append(int(w) % (self.vocab_size - 2) if w.lstrip("-").isdigit() else zlib.crc32(w.encode()) % (self.vocab_size - 2))
         return [self.bos_id] + ids + [self.eos_id] if self.add_bos_eos else ids
+
+    def encode_with_offsets(self, text: str) -> Tuple[List[int], List[Span]]:
+        """(encode(text), the (start, end) character span of each id in `text`; BOS and EOS have none)."""
+        spans: List[Span] = [(m.start(), m.end()) for m in re.finditer(r"\S+", text)]
+        if self.add_bos_eos:
+            spans = [None] + spans + [None]
+        return self.encode(text), spans

@@ -1,11 +1,17 @@
-"""ctypes binding of the C-ABI in include/sopro_b200.h (sopro_b200/lib/libsopro_b200.so).
+"""ctypes binding of the C-ABI in include/sopro_b200.h (sopro_b200/lib/libsopro_b200.so), and what every wrapper of
+it shares: the return-code checks, the stream argument, the rows of a batched output stage, and the chunk streams of the
+streaming stages with their pool.
 
 There is NO fallback: if the shared library is missing or fails to load, importing
 this module raises.  Build it with ./build.sh (or __graft_entry__.build())."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
+from typing import List, Optional, Sequence
+
+import torch
 
 MAX_AR_LAYERS = 16
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -278,3 +284,109 @@ def check(rc: int) -> None:
     if rc != 0:
         msg = load().sopro_last_error()
         raise SoproError(f"sopro_b200 error {rc}: {msg.decode() if msg else '?'}")
+
+
+def check_arg(rc: int) -> None:
+    """SOPRO_ERR_INVALID (a refused argument: a rate, a speed, a target, a geometry, an oversized push) is a ValueError;
+    anything else goes through check()."""
+    if rc == -1:
+        msg = load().sopro_last_error()
+        raise ValueError(msg.decode() if msg else "invalid argument")
+    check(rc)
+
+
+def stream_ptr(device: torch.device) -> int:
+    """The device's current CUDA stream, as the C ABI takes it."""
+    return int(torch.cuda.current_stream(device).cuda_stream)
+
+
+def rows(wav: torch.Tensor, lens: Optional[Sequence[int]], what: str):
+    """The input of a batched output stage: wav [..., L] on a CUDA device, its rows the leading dims flattened ->
+    (x fp32 contiguous [B, L], the leading dims, lens as c_int64 * B or None).  `lens`: valid samples per row.  `what`
+    names the stage in the error a CPU tensor raises."""
+    if wav.device.type != "cuda":
+        raise SoproError(f"{what} needs CUDA tensors; there is no CPU path")
+    L = int(wav.shape[-1])
+    lead = tuple(wav.shape[:-1])
+    B = math.prod(lead)
+    x = wav.detach().to(dtype=torch.float32).reshape(B, L).contiguous()
+    if lens is None:
+        return x, lead, None
+    if len(lens) != B:
+        raise ValueError(f"lens has {len(lens)} entries for {B} rows")
+    return x, lead, (C.c_int64 * B)(*[int(v) for v in lens])
+
+
+class ChunkStream:
+    """One utterance through a streaming stage, chunk by chunk: ``push(x)`` returns the outputs its input completes,
+    ``finish()`` the rest.  A subclass creates the device state ``_h`` on ``device`` and names its C symbols (``_ready``,
+    ``_push``, ``_finish``, ``_destroy``); ``_owner``, when set, is the object the state was created from, and closing
+    that one frees the state with it."""
+
+    _ready = _push = _finish = _destroy = ""
+    _not_ready = "the stream is finished (reset it) or n_more < 0"
+    _owner = None
+
+    def ready(self, n_more: int, final: bool = False) -> int:
+        """Outputs a push of n_more samples (followed by finish when `final`) would write."""
+        n = int(getattr(self.lib, self._ready)(self._h, int(n_more), 1 if final else 0))
+        if n < 0:
+            raise SoproError(self._not_ready)
+        return n
+
+    def push(self, x: torch.Tensor) -> torch.Tensor:
+        """x: the next samples (any shape, flattened; at most max_chunk) -> [k] f32 on the device."""
+        dev = self.device
+        x = x.detach().to(device=dev, dtype=torch.float32).reshape(-1).contiguous()
+        n = int(x.numel())
+        k = int(getattr(self.lib, self._ready)(self._h, n, 0))
+        y = torch.empty(max(k, 0), dtype=torch.float32, device=dev)
+        check_arg(getattr(self.lib, self._push)(self._h, x.data_ptr() if n else None, n, y.data_ptr() if k > 0 else None,
+                                                stream_ptr(dev)))
+        return y
+
+    def finish(self) -> torch.Tensor:
+        """The remaining outputs (the input's end zero padded) -> [k]; the stream then takes no push until reset()."""
+        dev = self.device
+        k = int(getattr(self.lib, self._ready)(self._h, 0, 1))
+        y = torch.empty(max(k, 0), dtype=torch.float32, device=dev)
+        check_arg(getattr(self.lib, self._finish)(self._h, y.data_ptr() if k > 0 else None, stream_ptr(dev)))
+        return y
+
+    def close(self) -> None:
+        if getattr(self, "_h", None) and (self._owner is None or getattr(self._owner, "_h", None)):
+            getattr(self.lib, self._destroy)(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class StatePool:
+    """Idle stream states, reused by the next utterance so that it allocates nothing.  ``checkout(max_chunk, *args)``
+    takes an idle state whose max_chunk covers the request and calls its ``reset(*args)``, or makes a new one with
+    ``make(max_chunk, *args)``; ``release`` keeps at most 4 idle."""
+
+    def __init__(self, make):
+        self._make = make
+        self._idle: List = []
+
+    def checkout(self, max_chunk: int, *args):
+        for i, s in enumerate(self._idle):
+            if s.max_chunk >= max_chunk:
+                del self._idle[i]
+                s.reset(*args)
+                return s
+        return self._make(max_chunk, *args)
+
+    def release(self, s) -> None:
+        if s is not None and len(self._idle) < 4:
+            self._idle.append(s)
+
+    def close(self) -> None:
+        for s in self._idle:
+            s.close()
+        self._idle = []

@@ -14,14 +14,10 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 
 #include "../../include/sopro_b200.h"
-
-namespace mimi {
-void set_error(const char* msg);  // the library's per-thread error message (ar_engine.cu)
-}
+#include "common.cuh"
 
 namespace {
 
@@ -30,23 +26,6 @@ constexpr int kThreads = 512;
 constexpr int kRowsPerLaunch = 128;      // utterances of one launch (their lengths travel as a kernel parameter)
 constexpr int kTileBytes = 128 * 1024;   // the A tile
 constexpr int kMaxTile = 64;             // steps of one A tile
-
-int afail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-
-#define ACK(call)                                                                                      \
-  do {                                                                                                 \
-    cudaError_t e__ = (call);                                                                          \
-    if (e__ != cudaSuccess)                                                                            \
-      return afail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
 
 struct AlignRows {
   int len[kRowsPerLaunch];
@@ -156,24 +135,24 @@ __global__ void __launch_bounds__(kThreads) align_kernel(const float* __restrict
 extern "C" {
 
 int sopro_align_sizes(int32_t B, int32_t steps, int64_t ld, int64_t* ws_bytes) {
-  if (!ws_bytes) return afail(SOPRO_ERR_INVALID, "align: null ws_bytes");
+  if (!ws_bytes) return fail(SOPRO_ERR_INVALID, "align: null ws_bytes");
   *ws_bytes = 0;
-  if (B < 1 || steps < 1 || ld < 1) return afail(SOPRO_ERR_INVALID, "align: B=%d, steps=%d, ld=%lld must be >= 1", B, steps, (long long)ld);
+  if (B < 1 || steps < 1 || ld < 1) return fail(SOPRO_ERR_INVALID, "align: B=%d, steps=%d, ld=%lld must be >= 1", B, steps, (long long)ld);
   *ws_bytes = (int64_t)B * steps * words_per_step(ld) * 4;
   return SOPRO_OK;
 }
 
 int sopro_align(const float* probs, int32_t steps, int32_t n_attn, int32_t B, int32_t H, int64_t ld, const int32_t* text_len_host,
                 const int32_t* frames_host, void* ws, int32_t* first, void* stream) {
-  if (!probs || !text_len_host || !frames_host || !ws || !first) return afail(SOPRO_ERR_INVALID, "align: null argument");
+  if (!probs || !text_len_host || !frames_host || !ws || !first) return fail(SOPRO_ERR_INVALID, "align: null argument");
   if (B < 1 || steps < 1 || n_attn < 1 || H < 1 || ld < 1)
-    return afail(SOPRO_ERR_INVALID, "align: B=%d, steps=%d, n_attn=%d, H=%d, ld=%lld must be >= 1", B, steps, n_attn, H, (long long)ld);
-  if ((long long)n_attn * H > 4096) return afail(SOPRO_ERR_INVALID, "align: n_attn x H = %lld > 4096", (long long)n_attn * H);
+    return fail(SOPRO_ERR_INVALID, "align: B=%d, steps=%d, n_attn=%d, H=%d, ld=%lld must be >= 1", B, steps, n_attn, H, (long long)ld);
+  if ((long long)n_attn * H > 4096) return fail(SOPRO_ERR_INVALID, "align: n_attn x H = %lld > 4096", (long long)n_attn * H);
   for (int b = 0; b < B; ++b) {
     if (text_len_host[b] < 1 || text_len_host[b] > std::min<int64_t>(ld, kMaxL))
-      return afail(SOPRO_ERR_INVALID, "align: text_len[%d]=%d not in [1, min(ld=%lld, %d)]", b, text_len_host[b], (long long)ld, kMaxL);
+      return fail(SOPRO_ERR_INVALID, "align: text_len[%d]=%d not in [1, min(ld=%lld, %d)]", b, text_len_host[b], (long long)ld, kMaxL);
     if (frames_host[b] < 0 || frames_host[b] > steps)
-      return afail(SOPRO_ERR_INVALID, "align: frames[%d]=%d not in [0, %d]", b, frames_host[b], steps);
+      return fail(SOPRO_ERR_INVALID, "align: frames[%d]=%d not in [0, %d]", b, frames_host[b], steps);
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int W = words_per_step(ld);
@@ -188,9 +167,9 @@ int sopro_align(const float* probs, int32_t steps, int32_t n_attn, int32_t B, in
     }
     // a CTA's own tile (tile_steps(own Lp) x own Lp) never exceeds this bound
     const size_t smem = (size_t)2 * Lp * 8 + std::min<size_t>((size_t)kMaxTile * Lp * 8, kTileBytes);
-    ACK(cudaFuncSetAttribute(align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     align_kernel<<<nb, kThreads, smem, st>>>(probs, steps, n_attn, B, H, ld, rows, b0, static_cast<unsigned*>(ws), W, first);
-    ACK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }

@@ -2,13 +2,13 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
 
 #include "../../include/sopro_b200.h"
+#include "common.cuh"
 #include "ar_kernel.cuh"
 
 using namespace sopro;
@@ -16,24 +16,6 @@ using namespace sopro;
 namespace {
 
 thread_local std::string g_err;
-
-int fail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-
-#define CK(call)                                                                          \
-  do {                                                                                    \
-    cudaError_t e__ = (call);                                                             \
-    if (e__ != cudaSuccess)                                                               \
-      return fail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), \
-                  __FILE__, __LINE__);                                                    \
-  } while (0)
 
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 

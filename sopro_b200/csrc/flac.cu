@@ -22,15 +22,11 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 
 #include "../../include/sopro_b200.h"
-
-namespace mimi {
-void set_error(const char* msg);  // the library's per-thread error message (ar_engine.cu)
-}
+#include "common.cuh"
 
 namespace {
 
@@ -48,23 +44,6 @@ constexpr int kMinRate = 4000, kMaxRate = 192000;
 constexpr int kStreamMin = 16;          // frames shorter than this may only end a stream
 
 enum Kind { kConst = 0, kVerbatim = 1, kFixed = 2, kLpc = 3 };
-
-int ffail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-
-#define FCK(call)                                                                                      \
-  do {                                                                                                 \
-    cudaError_t e__ = (call);                                                                          \
-    if (e__ != cudaSuccess)                                                                            \
-      return ffail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
 
 bool valid_rate(int sr) { return sr >= kMinRate && sr <= kMaxRate; }
 
@@ -762,7 +741,7 @@ int run(Job J, int B, const long long* lens, char* ws, const Layout& l, unsigned
   long long* foff = reinterpret_cast<long long*>(ws + l.foff);
   long long* cursor = reinterpret_cast<long long*>(ws + l.cursor);
   flac_zero_kernel<<<1, 1, 0, st>>>(cursor);
-  FCK(cudaGetLastError());
+  CK(cudaGetLastError());
   const Src src0 = J.src;
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
@@ -777,13 +756,13 @@ int run(Job J, int B, const long long* lens, char* ws, const Layout& l, unsigned
     const long long nblk = R.blk0[rows];
     if (nblk > 0) {
       flac_analysis_kernel<<<(unsigned)nblk, kT, 0, st>>>(J, R, desc);
-      FCK(cudaGetLastError());
+      CK(cudaGetLastError());
     }
     flac_layout_kernel<<<1, kLayT, 0, st>>>(J, R, desc, foff, cursor, out, row_off + b0, row_bytes + b0);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     if (nblk > 0) {
       flac_pack_kernel<<<(unsigned)nblk, kT, 0, st>>>(J, R, desc, foff, out);
-      FCK(cudaGetLastError());
+      CK(cudaGetLastError());
     }
   }
   return SOPRO_OK;
@@ -801,9 +780,9 @@ struct SoproFlacStream {
 extern "C" {
 
 int sopro_flac_sizes(int32_t B, int64_t max_len, int32_t sr, int64_t* ws_bytes, int64_t* out_bytes) {
-  if (!valid_rate(sr)) return ffail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
+  if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   if (B < 1 || max_len < 0 || max_len > kMaxLen)
-    return ffail(SOPRO_ERR_INVALID, "bad geometry: %d rows of at most %lld samples (at most %lld)", B, (long long)max_len, kMaxLen);
+    return fail(SOPRO_ERR_INVALID, "bad geometry: %d rows of at most %lld samples (at most %lld)", B, (long long)max_len, kMaxLen);
   if (ws_bytes) *ws_bytes = (int64_t)layout(B, max_len).total;
   if (out_bytes) *out_bytes = (int64_t)B * out_bound(max_len, true);
   return SOPRO_OK;
@@ -811,25 +790,25 @@ int sopro_flac_sizes(int32_t B, int64_t max_len, int32_t sr, int64_t* ws_bytes, 
 
 int sopro_flac_encode(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, void* ws,
                       uint8_t* out, int64_t* row_off, int64_t* row_bytes, void* stream) {
-  if (!valid_rate(sr)) return ffail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
+  if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return ffail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
-  if (!ws || !out || !row_off || !row_bytes) return ffail(SOPRO_ERR_INVALID, "null argument");
+    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
+  if (!ws || !out || !row_off || !row_bytes) return fail(SOPRO_ERR_INVALID, "null argument");
   long long most = 0;
   long long* lens = static_cast<long long*>(malloc(sizeof(long long) * B));
-  if (!lens) return ffail(SOPRO_ERR_INVALID, "out of host memory");
+  if (!lens) return fail(SOPRO_ERR_INVALID, "out of host memory");
   for (int b = 0; b < B; ++b) {
     lens[b] = lens_host ? lens_host[b] : x_stride;
     if (lens[b] < 0 || lens[b] > x_stride) {
       const long long v = lens[b];
       free(lens);
-      return ffail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, v, (long long)x_stride);
+      return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, v, (long long)x_stride);
     }
     most = std::max(most, lens[b]);
   }
   if (!x && most > 0) {
     free(lens);
-    return ffail(SOPRO_ERR_INVALID, "null argument");
+    return fail(SOPRO_ERR_INVALID, "null argument");
   }
   Job J{};
   J.src = Src{x, x_stride, nullptr, 0};
@@ -845,9 +824,9 @@ int sopro_flac_encode(const float* x, int32_t B, int64_t x_stride, const int64_t
 }
 
 int sopro_flac_stream_create(int32_t sr, SoproFlacStream** out) {
-  if (!out) return ffail(SOPRO_ERR_INVALID, "null argument");
+  if (!out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (!valid_rate(sr)) return ffail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
+  if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   SoproFlacStream* s = new SoproFlacStream();
   s->sr = sr;
   for (int i = 0; i < 2; ++i) {
@@ -855,7 +834,7 @@ int sopro_flac_stream_create(int32_t sr, SoproFlacStream** out) {
     if (e != cudaSuccess) {
       cudaFree(s->carry[0]);
       delete s;
-      return ffail(SOPRO_ERR_CUDA, "cudaMalloc failed: %s", cudaGetErrorString(e));
+      return fail(SOPRO_ERR_CUDA, "cudaMalloc failed: %s", cudaGetErrorString(e));
     }
   }
   *out = s;
@@ -871,8 +850,8 @@ int sopro_flac_stream_destroy(SoproFlacStream* s) {
 }
 
 int sopro_flac_stream_reset(SoproFlacStream* s, int32_t sr) {
-  if (!s) return ffail(SOPRO_ERR_INVALID, "null argument");
-  if (!valid_rate(sr)) return ffail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   s->sr = sr;
   s->carry_n = 0;
   s->samples = 0;
@@ -903,7 +882,7 @@ static int stream_encode(SoproFlacStream* s, const float* x, long long n, void* 
   if (rc != SOPRO_OK) return rc;
   if (keep > 0) {
     flac_carry_kernel<<<1, 32, 0, st>>>(s->carry[s->cur], s->carry_n, x, enc, (int)keep, s->carry[s->cur ^ 1]);
-    FCK(cudaGetLastError());
+    CK(cudaGetLastError());
     s->cur ^= 1;
   }
   s->carry_n = (int)keep;
@@ -912,13 +891,13 @@ static int stream_encode(SoproFlacStream* s, const float* x, long long n, void* 
 }
 
 int sopro_flac_stream_push(SoproFlacStream* s, const float* x, int64_t n, void* ws, uint8_t* out, int64_t* nbytes, void* stream) {
-  if (!s || !ws || !out || !nbytes || (!x && n > 0)) return ffail(SOPRO_ERR_INVALID, "null argument");
-  if (n < 0 || n > kMaxLen - s->samples - s->carry_n) return ffail(SOPRO_ERR_INVALID, "push of %lld samples refused", (long long)n);
+  if (!s || !ws || !out || !nbytes || (!x && n > 0)) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (n < 0 || n > kMaxLen - s->samples - s->carry_n) return fail(SOPRO_ERR_INVALID, "push of %lld samples refused", (long long)n);
   return stream_encode(s, x, n, ws, out, nbytes, false, stream);
 }
 
 int sopro_flac_stream_finish(SoproFlacStream* s, void* ws, uint8_t* out, int64_t* nbytes, void* stream) {
-  if (!s || !ws || !out || !nbytes) return ffail(SOPRO_ERR_INVALID, "null argument");
+  if (!s || !ws || !out || !nbytes) return fail(SOPRO_ERR_INVALID, "null argument");
   const int rc = stream_encode(s, nullptr, 0, ws, out, nbytes, true, stream);
   if (rc != SOPRO_OK) return rc;
   s->carry_n = 0;

@@ -18,16 +18,12 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <vector>
 
 #include "../../include/sopro_b200.h"
-
-namespace mimi {
-void set_error(const char* msg);  // the library's per-thread error message (ar_engine.cu)
-}
+#include "common.cuh"
 
 namespace {
 
@@ -40,27 +36,6 @@ constexpr int kRowsPerLaunch = 128;          // rows of one extents launch (thei
 constexpr int kSegsPerLaunch = 64;           // segments of one join launch
 constexpr long long kMaxLen = 1LL << 40;
 constexpr double kPi = 3.141592653589793;
-
-int lfail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-
-#define LCK(call)                                                                                      \
-  do {                                                                                                 \
-    cudaError_t e__ = (call);                                                                          \
-    if (e__ != cudaSuccess)                                                                            \
-      return lfail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
-struct RowLens {
-  long long v[kRowsPerLaunch];
-};
 
 // frame k's dB, the same value in every lane
 __device__ __forceinline__ double frame_db(const float* __restrict__ x, long long k, int lane) {
@@ -79,7 +54,7 @@ __device__ __forceinline__ double frame_db(const float* __restrict__ x, long lon
   return 10.0 * log10(s / (double)kFrame + 1e-10);
 }
 
-__global__ void __launch_bounds__(kExtThreads) extents_kernel(const float* __restrict__ x, long long x_stride, RowLens lens,
+__global__ void __launch_bounds__(kExtThreads) extents_kernel(const float* __restrict__ x, long long x_stride, RowLens<kRowsPerLaunch> lens,
                                                               long long* __restrict__ ext) {
   __shared__ double wmax[kExtWarps];
   __shared__ long long s_first, s_last;
@@ -174,56 +149,56 @@ int fade_len(long long span) { return (int)std::min<long long>(kFadeMax, span / 
 extern "C" {
 
 int sopro_longform_fade(int32_t F, float* f) {
-  if (F < 0 || F > kFadeMax) return lfail(SOPRO_ERR_INVALID, "fade length %d not in [0, %d]", F, kFadeMax);
-  if (F > 0 && !f) return lfail(SOPRO_ERR_INVALID, "null argument");
+  if (F < 0 || F > kFadeMax) return fail(SOPRO_ERR_INVALID, "fade length %d not in [0, %d]", F, kFadeMax);
+  if (F > 0 && !f) return fail(SOPRO_ERR_INVALID, "null argument");
   fade(F, f);
   return SOPRO_OK;
 }
 
 int sopro_longform_extents(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int64_t* ext, void* stream) {
-  if (!ext) return lfail(SOPRO_ERR_INVALID, "null argument");
+  if (!ext) return fail(SOPRO_ERR_INVALID, "null argument");
   if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return lfail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
+    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
   long long most = 0;
   for (int b = 0; b < B; ++b) {
     const long long len = lens_host ? lens_host[b] : x_stride;
     if (len < 0 || len > x_stride)
-      return lfail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
+      return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
     most = std::max(most, len);
   }
-  if (!x && most > 0) return lfail(SOPRO_ERR_INVALID, "null argument");
+  if (!x && most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens L{};
+    RowLens<kRowsPerLaunch> L{};
     for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
     extents_kernel<<<rows, kExtThreads, 0, st>>>(x + (long long)b0 * x_stride, x_stride, L,
                                                  reinterpret_cast<long long*>(ext) + 2LL * b0);
-    LCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }
 
 int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host, int64_t pause,
                         float* y, int64_t y_len, void* stream) {
-  if (!src || !lens_host || !ext_host) return lfail(SOPRO_ERR_INVALID, "null argument");
-  if (n_seg < 1) return lfail(SOPRO_ERR_INVALID, "n_seg = %d < 1", n_seg);
-  if (pause < 0 || pause > kMaxPause) return lfail(SOPRO_ERR_INVALID, "pause of %lld samples not in [0, %lld]", (long long)pause, kMaxPause);
+  if (!src || !lens_host || !ext_host) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (n_seg < 1) return fail(SOPRO_ERR_INVALID, "n_seg = %d < 1", n_seg);
+  if (pause < 0 || pause > kMaxPause) return fail(SOPRO_ERR_INVALID, "pause of %lld samples not in [0, %lld]", (long long)pause, kMaxPause);
   long long total = 0, last = -1;
   for (int i = 0; i < n_seg; ++i) {
     const long long len = lens_host[i], s = ext_host[2 * i], e = ext_host[2 * i + 1];
-    if (len < 0 || len > kMaxLen) return lfail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, 2^40]", i, len);
+    if (len < 0 || len > kMaxLen) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, 2^40]", i, len);
     if (s < 0 || s > e || e > len)
-      return lfail(SOPRO_ERR_INVALID, "extent [%lld, %lld) of segment %d is not inside its %lld samples", s, e, i, len);
-    if (e > s && !src[i]) return lfail(SOPRO_ERR_INVALID, "null source for segment %d", i);
+      return fail(SOPRO_ERR_INVALID, "extent [%lld, %lld) of segment %d is not inside its %lld samples", s, e, i, len);
+    if (e > s && !src[i]) return fail(SOPRO_ERR_INVALID, "null source for segment %d", i);
     if (e > s) {
       total += (last >= 0 ? pause : 0) + (e - s);
       last = i;
     }
   }
-  if (y_len != total) return lfail(SOPRO_ERR_INVALID, "y_len = %lld, the joined length is %lld", (long long)y_len, total);
+  if (y_len != total) return fail(SOPRO_ERR_INVALID, "y_len = %lld, the joined length is %lld", (long long)y_len, total);
   if (total == 0) return SOPRO_OK;
-  if (!y) return lfail(SOPRO_ERR_INVALID, "null argument");
+  if (!y) return fail(SOPRO_ERR_INVALID, "null argument");
   // each span's place in y, then one launch per (fade length, run of at most kSegsPerLaunch segments)
   std::vector<long long> off(n_seg, 0);
   std::vector<char> done(n_seg, 1);
@@ -240,7 +215,7 @@ int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* l
   auto launch = [&]() -> int {
     const unsigned gx = (unsigned)std::min<long long>((most + kJoinThreads - 1) / kJoinThreads, 1024);
     join_kernel<<<dim3(gx, a.nseg), kJoinThreads, 0, st>>>(a, y);
-    LCK(cudaGetLastError());
+    CK(cudaGetLastError());
     a.nseg = 0;
     most = 0;
     return SOPRO_OK;

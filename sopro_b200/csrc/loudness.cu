@@ -23,14 +23,10 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 
 #include "../../include/sopro_b200.h"
-
-namespace mimi {
-void set_error(const char* msg);  // the library's per-thread error message (ar_engine.cu)
-}
+#include "common.cuh"
 
 namespace {
 
@@ -42,23 +38,6 @@ constexpr int kRowsPerLaunch = 128;     // rows of a ragged batch per launch (th
 constexpr long long kMaxLen = 1LL << 40;
 constexpr int kMinRate = 4000, kMaxRate = 192000;
 constexpr double kPi = 3.141592653589793;
-
-int tfail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-
-#define TCK(call)                                                                                      \
-  do {                                                                                                 \
-    cudaError_t e__ = (call);                                                                          \
-    if (e__ != cudaSuccess)                                                                            \
-      return tfail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
 
 struct Mat {
   double m[4][4];
@@ -75,10 +54,6 @@ struct Gate {
   double abs_e;     // 10^((-70 + 0.691) / 10): the absolute gate as an energy
   double rel;       // 10^(-10 / 10): the relative gate's factor on the mean energy
   double ceil_amp;  // 10^(-1 / 20): the sample-peak ceiling
-};
-
-struct RowLens {
-  long long v[kRowsPerLaunch];
 };
 
 struct St {
@@ -263,7 +238,7 @@ struct Smem {
 };
 
 // pass 1: grid (R, rows); piece end states from zero state, and the CTA's aggregate
-__global__ void __launch_bounds__(kT) loud_scan_kernel(Filt f, const float* __restrict__ x, long long x_stride, RowLens lens,
+__global__ void __launch_bounds__(kT) loud_scan_kernel(Filt f, const float* __restrict__ x, long long x_stride, RowLens<kRowsPerLaunch> lens,
                                                        St* __restrict__ v, St* __restrict__ agg, long long R) {
   __shared__ Smem sm;
   const int b = blockIdx.y, tid = threadIdx.x;
@@ -285,7 +260,7 @@ __global__ void __launch_bounds__(kT) loud_scan_kernel(Filt f, const float* __re
 
 // per row, in increasing CTA order: carry_c = A^(P T) carry_{c-1} + agg_{c-1}, carry_0 = 0; the aggregates are staged
 // through shared memory kT at a time, so the serial chain waits on no global load
-__global__ void __launch_bounds__(kT) loud_carry_kernel(Filt f, RowLens lens, const St* __restrict__ agg, St* __restrict__ carry,
+__global__ void __launch_bounds__(kT) loud_carry_kernel(Filt f, RowLens<kRowsPerLaunch> lens, const St* __restrict__ agg, St* __restrict__ carry,
                                                         long long R) {
   __shared__ St buf[kT];
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -319,7 +294,7 @@ __global__ void __launch_bounds__(kT) loud_carry_kernel(Filt f, RowLens lens, co
 
 // pass 2: grid (R, rows); each piece re-filtered from its true start state; y^2 per piece and sub-block; max|x| per CTA
 __global__ void __launch_bounds__(kT) loud_energy_kernel(Filt f, int sbs, const float* __restrict__ x, long long x_stride,
-                                                         RowLens lens, const St* __restrict__ v, const St* __restrict__ carry,
+                                                         RowLens<kRowsPerLaunch> lens, const St* __restrict__ v, const St* __restrict__ carry,
                                                          double* __restrict__ e, float* __restrict__ cmax, long long R) {
   __shared__ Smem sm;
   __shared__ float wmax[kT / 32];
@@ -362,7 +337,7 @@ __global__ void __launch_bounds__(kT) loud_energy_kernel(Filt f, int sbs, const 
 
 // grid (ceil(nsb / 8), rows): warp w sums sub-block q = 8 blockIdx.x + w over the pieces it touches -- lane l the
 // pieces i0 + l, i0 + l + 32, ... in order, then a butterfly over the lanes (a fixed order that depends on q and s alone)
-__global__ void __launch_bounds__(kT) loud_subblock_kernel(int sbs, RowLens lens, const double* __restrict__ e, double* __restrict__ E,
+__global__ void __launch_bounds__(kT) loud_subblock_kernel(int sbs, RowLens<kRowsPerLaunch> lens, const double* __restrict__ e, double* __restrict__ E,
                                                            long long R, long long nsb_stride) {
   const int b = blockIdx.y, lane = threadIdx.x & 31;
   const long long s = sbs, q = (long long)blockIdx.x * (kT / 32) + (threadIdx.x >> 5);
@@ -399,7 +374,7 @@ __device__ __forceinline__ double block_z(const double* E, long long j, double i
 }
 
 // one CTA per row: blocks, both gates, L, max|x| and (normalize) the gain
-__global__ void __launch_bounds__(kT) loud_gate_kernel(Gate gt, RowLens lens, const float* __restrict__ cmax,
+__global__ void __launch_bounds__(kT) loud_gate_kernel(Gate gt, RowLens<kRowsPerLaunch> lens, const float* __restrict__ cmax,
                                                        const double* __restrict__ E, long long R, long long nsb_stride,
                                                        double* __restrict__ lufs, int normalize, double target,
                                                        float* __restrict__ gain) {
@@ -455,7 +430,7 @@ __global__ void __launch_bounds__(kT) loud_gate_kernel(Gate gt, RowLens lens, co
 }
 
 // y = g * x over [0, lens[b]); y may alias x
-__global__ void __launch_bounds__(kT) loud_apply_kernel(const float* x, long long x_stride, RowLens lens, const float* __restrict__ gain,
+__global__ void __launch_bounds__(kT) loud_apply_kernel(const float* x, long long x_stride, RowLens<kRowsPerLaunch> lens, const float* __restrict__ gain,
                                                         float* y, long long y_stride) {
   const int b = blockIdx.y;
   const long long n = lens.v[b];
@@ -466,22 +441,22 @@ __global__ void __launch_bounds__(kT) loud_apply_kernel(const float* x, long lon
 }
 
 int check_batch(const float* x, int B, long long x_stride, const int64_t* lens_host, int sr, void* ws, long long* most) {
-  if (!ws) return tfail(SOPRO_ERR_INVALID, "null argument");
-  if (!valid_rate(sr)) return tfail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
+  if (!ws) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return tfail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, x_stride);
+    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, x_stride);
   *most = 0;
   for (int b = 0; b < B; ++b) {
     const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride) return tfail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, x_stride);
+    if (len < 0 || len > x_stride) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, x_stride);
     *most = std::max(*most, len);
   }
-  if (!x && *most > 0) return tfail(SOPRO_ERR_INVALID, "null argument");
+  if (!x && *most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
   return SOPRO_OK;
 }
 
 // the meter over rows [b0, b0 + rows): L -> lufs[b0 ..], and with `normalize` g -> gain[b0 ..]
-int run_meter(const Filt& f, const Gate& gt, const Layout& l, const float* x, long long x_stride, const RowLens& L, int b0,
+int run_meter(const Filt& f, const Gate& gt, const Layout& l, const float* x, long long x_stride, const RowLens<kRowsPerLaunch>& L, int b0,
               int rows, char* ws, double* lufs, int normalize, double target, float* gain, cudaStream_t st) {
   St* v = reinterpret_cast<St*>(ws + l.v) + (long long)b0 * l.R * kT;
   double* e = reinterpret_cast<double*>(ws + l.e) + 2LL * b0 * l.R * kT;
@@ -493,18 +468,18 @@ int run_meter(const Filt& f, const Gate& gt, const Layout& l, const float* x, lo
   if (l.R > 0) {
     const dim3 grid((unsigned)l.R, rows);
     loud_scan_kernel<<<grid, kT, 0, st>>>(f, xb, x_stride, L, v, agg, l.R);
-    TCK(cudaGetLastError());
+    CK(cudaGetLastError());
     loud_carry_kernel<<<rows, kT, 0, st>>>(f, L, agg, carry, l.R);
-    TCK(cudaGetLastError());
+    CK(cudaGetLastError());
     loud_energy_kernel<<<grid, kT, 0, st>>>(f, gt.s, xb, x_stride, L, v, carry, e, cmax, l.R);
-    TCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   if (l.nsb > 0) {
     loud_subblock_kernel<<<dim3((unsigned)((l.nsb + kT / 32 - 1) / (kT / 32)), rows), kT, 0, st>>>(gt.s, L, e, E, l.R, l.nsb);
-    TCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   loud_gate_kernel<<<rows, kT, 0, st>>>(gt, L, cmax, E, l.R, l.nsb, lufs + b0, normalize, target, gain ? gain + b0 : nullptr);
-  TCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -515,14 +490,14 @@ bool valid_target(double T) { return T >= -60.0 && T <= 0.0; }  // also refuses 
 extern "C" {
 
 int sopro_loudness_filter(int32_t sr, double* c) {
-  if (!c) return tfail(SOPRO_ERR_INVALID, "null argument");
-  if (!valid_rate(sr)) return tfail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
+  if (!c) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   coeffs(sr, c);
   return SOPRO_OK;
 }
 
 int sopro_loudness_target(double T) {
-  if (!valid_target(T)) return tfail(SOPRO_ERR_INVALID, "loudness target must be a real number in [-60, 0] LUFS (got %g)", T);
+  if (!valid_target(T)) return fail(SOPRO_ERR_INVALID, "loudness target must be a real number in [-60, 0] LUFS (got %g)", T);
   return SOPRO_OK;
 }
 
@@ -536,14 +511,14 @@ int sopro_loudness_measure(const float* x, int32_t B, int64_t x_stride, const in
   long long most = 0;
   const int rc = check_batch(x, B, x_stride, lens_host, sr, ws, &most);
   if (rc != SOPRO_OK) return rc;
-  if (!lufs_dev) return tfail(SOPRO_ERR_INVALID, "null argument");
+  if (!lufs_dev) return fail(SOPRO_ERR_INVALID, "null argument");
   const Filt f = make_filt(sr);
   const Gate gt = make_gate(sr);
   const Layout l = layout(B, most, sr);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens L{};
+    RowLens<kRowsPerLaunch> L{};
     for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
     const int r = run_meter(f, gt, l, x, x_stride, L, b0, rows, static_cast<char*>(ws), lufs_dev, 0, 0.0, nullptr, st);
     if (r != SOPRO_OK) return r;
@@ -553,12 +528,12 @@ int sopro_loudness_measure(const float* x, int32_t B, int64_t x_stride, const in
 
 int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, double T,
                              float* y, int64_t y_stride, void* ws, double* lufs_dev, float* gain_dev, void* stream) {
-  if (!valid_target(T)) return tfail(SOPRO_ERR_INVALID, "loudness target must be a real number in [-60, 0] LUFS (got %g)", T);
+  if (!valid_target(T)) return fail(SOPRO_ERR_INVALID, "loudness target must be a real number in [-60, 0] LUFS (got %g)", T);
   long long most = 0;
   const int rc = check_batch(x, B, x_stride, lens_host, sr, ws, &most);
   if (rc != SOPRO_OK) return rc;
-  if (!y && most > 0) return tfail(SOPRO_ERR_INVALID, "null argument");
-  if (B > 1 && y_stride < most) return tfail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld samples", (long long)y_stride, most);
+  if (!y && most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B > 1 && y_stride < most) return fail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld samples", (long long)y_stride, most);
   const Filt f = make_filt(sr);
   const Gate gt = make_gate(sr);
   const Layout l = layout(B, most, sr);
@@ -568,7 +543,7 @@ int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const 
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens L{};
+    RowLens<kRowsPerLaunch> L{};
     for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
     const int r = run_meter(f, gt, l, x, x_stride, L, b0, rows, w, lufs, 1, T, gain, st);
     if (r != SOPRO_OK) return r;
@@ -576,7 +551,7 @@ int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const 
       const long long gx = std::min<long long>((most + kT - 1) / kT, 4096);
       loud_apply_kernel<<<dim3((unsigned)gx, rows), kT, 0, st>>>(x + (long long)b0 * x_stride, x_stride, L, gain + b0,
                                                                   y + (long long)b0 * y_stride, y_stride);
-      TCK(cudaGetLastError());
+      CK(cudaGetLastError());
     }
   }
   return SOPRO_OK;

@@ -25,7 +25,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -34,12 +33,10 @@
 #include <vector>
 
 #include "../../include/sopro_b200.h"
+#include "common.cuh"
 #include "mimi_tc.cuh"
 
 namespace mimi {
-
-// shared with ar_engine.cu through sopro_last_error()
-void set_error(const char* msg);
 
 enum { EPI_NONE = 0, EPI_GELU = 1, EPI_RES_SCALE = 2, EPI_RES = 3 };
 
@@ -442,22 +439,6 @@ __global__ void __launch_bounds__(256) final_conv_h_kernel(const __nv_bfloat16* 
 using namespace mimi;
 
 namespace {
-int mfail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-#define MCK(call)                                                                                      \
-  do {                                                                                                 \
-    cudaError_t e__ = (call);                                                                          \
-    if (e__ != cudaSuccess)                                                                            \
-      return mfail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
 uint16_t bf16_rne(float f) {
   uint32_t u;
   memcpy(&u, &f, 4);
@@ -563,20 +544,20 @@ sopro_mimi::Layer pack_layer(const sopro_mimi_layer_weights_t& L, int C, int FF,
 extern "C" {
 
 int sopro_mimi_create(const sopro_mimi_config_t* cfg, const sopro_mimi_weights_t* w, int device, sopro_mimi_t** out) {
-  if (!cfg || !w || !out) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
   int ndev = 0;
   cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0) return mfail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the Mimi decoder has no CPU fallback");
-  if (device < 0 || device >= ndev) return mfail(SOPRO_ERR_INVALID, "device %d out of range", device);
+  if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the Mimi decoder has no CPU fallback");
+  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
-  MCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return mfail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  CK(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int C = cfg->hidden, Dc = cfg->codebook_dim, Q = cfg->n_q, V = cfg->vocab, NL = cfg->n_layers, FF = cfg->ffn;
   if (C % 64 || Dc % 4 || C != 2 * Dc || NL < 1 || cfg->n_ratios < 1 || cfg->n_ratios > 8 || cfg->n_heads < 1 || C % cfg->n_heads ||
       (C / cfg->n_heads) % 4 || FF % 16)
-    return mfail(SOPRO_ERR_INVALID, "unsupported Mimi geometry (hidden=%d codebook_dim=%d)", C, Dc);
-  MCK(cudaSetDevice(device));
+    return fail(SOPRO_ERR_INVALID, "unsupported Mimi geometry (hidden=%d codebook_dim=%d)", C, Dc);
+  CK(cudaSetDevice(device));
   sopro_mimi* m = new sopro_mimi();
   m->device = device;
   m->cfg = *cfg;
@@ -645,13 +626,13 @@ int sopro_mimi_create(const sopro_mimi_config_t* cfg, const sopro_mimi_weights_t
     cudaFree(m->dev);
     cudaFree(m->dev_h);
     delete m;
-    return mfail(SOPRO_ERR_UNSUPPORTED, "driver has no cuTensorMapEncodeTiled entry point");
+    return fail(SOPRO_ERR_UNSUPPORTED, "driver has no cuTensorMapEncodeTiled entry point");
   }
   if (err != cudaSuccess) {
     if (m->dev) cudaFree(m->dev);
     if (m->dev_h) cudaFree(m->dev_h);
     delete m;
-    return mfail(SOPRO_ERR_CUDA, "Mimi weight upload failed: %s", cudaGetErrorString(err));
+    return fail(SOPRO_ERR_CUDA, "Mimi weight upload failed: %s", cudaGetErrorString(err));
   }
   *out = m;
   return SOPRO_OK;
@@ -682,8 +663,8 @@ int64_t sopro_mimi_samples_per_frame(const sopro_mimi_t* m) {
 }
 
 int sopro_mimi_set_precision(sopro_mimi_t* m, int precision) {
-  if (!m) return mfail(SOPRO_ERR_INVALID, "null argument");
-  if (precision != SOPRO_MIMI_FP32 && precision != SOPRO_MIMI_BF16_TC) return mfail(SOPRO_ERR_INVALID, "unknown precision %d", precision);
+  if (!m) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (precision != SOPRO_MIMI_FP32 && precision != SOPRO_MIMI_BF16_TC) return fail(SOPRO_ERR_INVALID, "unknown precision %d", precision);
   m->precision = precision;
   return SOPRO_OK;
 }
@@ -713,9 +694,9 @@ int make_rope(const sopro_mimi_config_t& c, int n, float** tab, int* tab_n, cuda
       h[(size_t)t * (Dh / 2) + d] = cosf(f);
       h[(size_t)(n + t) * (Dh / 2) + d] = sinf(f);
     }
-  MCK(cudaMalloc(tab, h.size() * 4));
-  MCK(cudaMemcpyAsync(*tab, h.data(), h.size() * 4, cudaMemcpyHostToDevice, st));
-  MCK(cudaStreamSynchronize(st));
+  CK(cudaMalloc(tab, h.size() * 4));
+  CK(cudaMemcpyAsync(*tab, h.data(), h.size() * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaStreamSynchronize(st));
   *tab_n = n;
   return SOPRO_OK;
 }
@@ -749,7 +730,7 @@ int mimi_prepare(sopro_mimi* m, int B, int T, cudaStream_t st) {
     m->ws = nullptr;
     m->ws_bytes = 0;
     cudaError_t e = cudaMalloc(&m->ws, need);
-    if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "Mimi workspace %zu MB: %s", need >> 20, cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "Mimi workspace %zu MB: %s", need >> 20, cudaGetErrorString(e));
     m->ws_bytes = need;
   }
   return SOPRO_OK;
@@ -767,14 +748,14 @@ int check_tc_geometry(const sopro_mimi* m) {
     ok = ok && tc::supported(S.ratio * S.cout, 2 * S.cin, S.cin) && tc::supported(hid, c.res_kernel * S.cout, S.cout) &&
          tc::supported(S.cout, hid, hid);
   }
-  return ok ? (int)SOPRO_OK : mfail(SOPRO_ERR_UNSUPPORTED, "tensor-core mode: unsupported Mimi geometry (use SOPRO_MIMI_FP32)");
+  return ok ? (int)SOPRO_OK : fail(SOPRO_ERR_UNSUPPORTED, "tensor-core mode: unsupported Mimi geometry (use SOPRO_MIMI_FP32)");
 }
 
 // ---- the layer sequence shared by the one-shot decode, the streaming step and the encoder.  These routines only
 //      enqueue kernels (no allocation, upload or synchronisation): the one-shot decode runs them under graph capture.
 
 int launch_gemm(const GemmOp& op, int B, cudaStream_t st) {
-  if (op.K % 16 || op.Cin % 4) return mfail(SOPRO_ERR_INVALID, "igemm: K=%d Cin=%d not aligned", op.K, op.Cin);
+  if (op.K % 16 || op.Cin % 4) return fail(SOPRO_ERR_INVALID, "igemm: K=%d Cin=%d not aligned", op.K, op.Cin);
   if (op.N % 64 == 0 || op.N > 32) {
     dim3 grid((op.M + 63) / 64, (op.N + 63) / 64, B);
     igemm_kernel<64><<<grid, 256, 0, st>>>(op);
@@ -782,7 +763,7 @@ int launch_gemm(const GemmOp& op, int B, cudaStream_t st) {
     dim3 grid((op.M + 63) / 64, (op.N + 31) / 32, B);
     igemm_kernel<32><<<grid, 256, 0, st>>>(op);
   }
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -815,7 +796,7 @@ int gemm_tc(const Operand& a, int cin, int taps, const __nv_bfloat16* W, const f
   o.c_bs = a.M * N; o.M = (int)a.M; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = 1; o.pad = taps - 1 - a.ctx;
   o.bias_mod = bias_mod; o.epi = epi; o.out_elu = out_elu;
   cudaError_t e = tc::launch(a.p, a.M + a.ctx, W, o, a.B, st);
-  if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core GEMM (N=%d K=%d): %s", N, o.K, cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "tensor-core GEMM (N=%d K=%d): %s", N, o.K, cudaGetErrorString(e));
   return SOPRO_OK;
 }
 static_assert((int)EPI_NONE == tc::EPI_NONE && (int)EPI_GELU == tc::EPI_GELU && (int)EPI_RES_SCALE == tc::EPI_RES_SCALE &&
@@ -872,16 +853,16 @@ int run_layers(const sopro_mimi_config_t& c, const std::vector<sopro_mimi::Layer
       if (tc_attn) {
         if constexpr (tc_mode) {  // q goes to ln (dead until the next LayerNorm)
           rope_pack_kernel<tc::kAttnDh><<<dim3((T2 + 31) / 32, B), 256, pack_bytes, st>>>(b.qkv, rope, ln, b.k, b.vt, T2, T2p, rope_T2, C, H);
-          MCK(cudaGetLastError());
+          CK(cudaGetLastError());
           cudaError_t ae = tc::launch_attn(ln, b.k, b.vt, att, B, T2, T2p, C, H, c.window, st);
-          if (ae != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core attention: %s", cudaGetErrorString(ae));
+          if (ae != cudaSuccess) return fail(SOPRO_ERR_CUDA, "tensor-core attention: %s", cudaGetErrorString(ae));
         }
       } else {
         float* kr = ring ? ring->k + li * (size_t)R * C : nullptr;
         float* vr = ring ? ring->v + li * (size_t)R * C : nullptr;
         rope_kernel<<<dim3(T2, B), 256, 0, st>>>(b.qkv, rope, T2, rope_T2, C, H, pos0, kr, vr, R);
         attn_kernel<<<dim3((T2 + 7) / 8, H, B), 256, asm_bytes, st>>>(b.qkv, att, T2, C, H, c.window, pos0, kr, vr, R);
-        MCK(cudaGetLastError());
+        CK(cudaGetLastError());
       }
       if ((rc = lin(att, C, L.wo, L.wo_h, C, EPI_RES_SCALE, Wd + L.ls1, x, nullptr))) return rc;
       layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, Wd + L.ln2w, Wd + L.ln2b, ln, rows, C, c.norm_eps);
@@ -973,7 +954,7 @@ int seanet_f32(const sopro_mimi* m, const SeanetBufs& b, int B, long long T2, Ta
   }
   final_conv_kernel<<<dim3((unsigned)((Tn + 255) / 256), B), 256, 0, st>>>(cur.rows<float>(ch), Wd + m->lw, Wd + m->lb, wav, Tn, ch,
                                                                             c.last_kernel, -cur.ctx);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -989,7 +970,7 @@ int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, l
   int ch = c.num_filters << c.n_ratios, rc;
   const long long n4 = (long long)B * T2 * C / 4;
   cast_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(x, b.in.rows<__nv_bfloat16>(C), n4);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   if ((rc = gemm_tc(b.in.operand(Tn, B), C, c.kernel, Wh + m->c0w_h, Wd + m->c0b, ch, ch, tc::EPI_NONE, nullptr, nullptr, nullptr,
                     b.a0.rows<__nv_bfloat16>(ch), 1, st)))
     return rc;
@@ -1017,7 +998,7 @@ int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, l
       ro.pad = c.res_kernel - 1 - sb.z.ctx;
       ro.out_elu = 1;
       cudaError_t fe = tc::launch_resblock(sb.z.p, Wh + S.r1w_h, Wh + S.r2w_h, hid, ro, B, st);
-      if (fe != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "fused ResnetBlock (stage %zu): %s", si, cudaGetErrorString(fe));
+      if (fe != cudaSuccess) return fail(SOPRO_ERR_CUDA, "fused ResnetBlock (stage %zu): %s", si, cudaGetErrorString(fe));
     } else {  // conv k=3 -> ELU(h) bf16, then the 1x1 conv + fp32 skip
       if ((rc = gemm_tc(sb.z.operand(Tn, B), S.cout, c.res_kernel, Wh + S.r1w_h, Wd + S.r1b, hid, hid, tc::EPI_NONE, nullptr, nullptr,
                         nullptr, sb.h.rows<__nv_bfloat16>(hid), 1, st)))
@@ -1034,7 +1015,7 @@ int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, l
   const int per = 256 - (c.last_kernel - 1);
   final_conv_h_kernel<<<dim3((unsigned)((Tn + per - 1) / per), B), 256, (size_t)(c.last_kernel * 256 + c.last_kernel * ch) * 4, st>>>(
       cur.rows<__nv_bfloat16>(ch), Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, -cur.ctx);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -1063,11 +1044,11 @@ int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, 
   __nv_bfloat16* h2 = h1 + bufsz;
   // ---- RVQ + projection + upsample (small; fp32 in both modes)
   rvq_gather_kernel<<<dim3(T, B), 256, 0, st>>>(codes, Wd + m->embed, b0, c.n_q, T, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   int rc;
   if ((rc = gemm_f32({b0, T, 0, B}, C, 1, Wd + m->rvq_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, b1, 0, st))) return rc;
   upsample_kernel<<<dim3(T2, B), 256, 0, st>>>(b1, Wd + m->up_w, x, T, C, nullptr);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   // ---- transformer: b1 (idle until the SEANet) takes the attention output; tensor-core mode: the LayerNorm copy and
   //      q in h0, k in h1, v^T and the MLP hidden in h2
   LayerBufs lb{};
@@ -1092,22 +1073,22 @@ int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, 
 extern "C" {
 
 int sopro_mimi_decode(sopro_mimi_t* m, const int32_t* codes, int B, int T, float* wav, void* stream) {
-  if (!m || !codes || !wav) return mfail(SOPRO_ERR_INVALID, "null argument");
-  if (B < 1 || T < 1) return mfail(SOPRO_ERR_INVALID, "B and T must be >= 1");
-  if (B > 65535) return mfail(SOPRO_ERR_INVALID, "B must be <= 65535");
-  if ((long long)T * sopro_mimi_samples_per_frame(m) > 0x7fffffffLL) return mfail(SOPRO_ERR_INVALID, "sequence too long for one launch");
+  if (!m || !codes || !wav) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || T < 1) return fail(SOPRO_ERR_INVALID, "B and T must be >= 1");
+  if (B > 65535) return fail(SOPRO_ERR_INVALID, "B must be <= 65535");
+  if ((long long)T * sopro_mimi_samples_per_frame(m) > 0x7fffffffLL) return fail(SOPRO_ERR_INVALID, "sequence too long for one launch");
   int rc;
   if (m->precision == SOPRO_MIMI_BF16_TC && (rc = check_tc_geometry(m))) return rc;
-  MCK(cudaSetDevice(m->device));
+  CK(cudaSetDevice(m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if ((rc = mimi_prepare(m, B, T, st))) return rc;
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  MCK(cudaStreamIsCapturing(st, &cap));
+  CK(cudaStreamIsCapturing(st, &cap));
   if (!m->graphs || (long long)B * T > kGraphFrames || cap != cudaStreamCaptureStatusNone) return mimi_enqueue(m, codes, B, T, wav, st);
   const size_t nc = (size_t)B * m->cfg.n_q * T, nw = (size_t)B * T * (size_t)sopro_mimi_samples_per_frame(m);
   if (!m->g_codes) {
-    MCK(cudaMalloc(&m->g_codes, (size_t)kGraphFrames * m->cfg.n_q * 4));
-    MCK(cudaMalloc(&m->g_wav, (size_t)kGraphFrames * (size_t)sopro_mimi_samples_per_frame(m) * 4));
+    CK(cudaMalloc(&m->g_codes, (size_t)kGraphFrames * m->cfg.n_q * 4));
+    CK(cudaMalloc(&m->g_wav, (size_t)kGraphFrames * (size_t)sopro_mimi_samples_per_frame(m) * 4));
   }
   cudaGraphExec_t exec = nullptr;
   for (auto& r : m->replays)
@@ -1115,8 +1096,8 @@ int sopro_mimi_decode(sopro_mimi_t* m, const int32_t* codes, int B, int T, float
   if (!exec) {
     if (m->replays.size() >= 32) drop_replays(m);
     // captured on a private stream (the caller's may be the legacy default stream, which cannot capture)
-    if (!m->cap_stream) MCK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-    MCK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
+    if (!m->cap_stream) CK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
+    CK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
     rc = mimi_enqueue(m, m->g_codes, B, T, m->g_wav, m->cap_stream);
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(m->cap_stream, &graph);
@@ -1124,15 +1105,15 @@ int sopro_mimi_decode(sopro_mimi_t* m, const int32_t* codes, int B, int T, float
       if (graph) cudaGraphDestroy(graph);
       return rc;
     }
-    if (ce != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "Mimi graph capture: %s", cudaGetErrorString(ce));
+    if (ce != cudaSuccess) return fail(SOPRO_ERR_CUDA, "Mimi graph capture: %s", cudaGetErrorString(ce));
     ce = cudaGraphInstantiate(&exec, graph, 0);
     cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "Mimi graph instantiate: %s", cudaGetErrorString(ce));
+    if (ce != cudaSuccess) return fail(SOPRO_ERR_CUDA, "Mimi graph instantiate: %s", cudaGetErrorString(ce));
     m->replays.push_back({B, T, m->precision, exec});
   }
-  MCK(cudaMemcpyAsync(m->g_codes, codes, nc * 4, cudaMemcpyDeviceToDevice, st));
-  MCK(cudaGraphLaunch(exec, st));
-  MCK(cudaMemcpyAsync(wav, m->g_wav, nw * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(m->g_codes, codes, nc * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaGraphLaunch(exec, st));
+  CK(cudaMemcpyAsync(wav, m->g_wav, nw * 4, cudaMemcpyDeviceToDevice, st));
   return SOPRO_OK;
 }
 
@@ -1250,12 +1231,12 @@ int stream_step(sopro_mimi_stream* s, const int32_t* codes, int n, int code_stri
   if (rc) return rc;
   // ---- RVQ + projection + upsample
   rvq_gather_kernel<<<dim3(n, 1), 256, 0, st>>>(codes, Wd + m->embed, s->S, c.n_q, code_stride, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   if ((rc = gemm_f32({s->S, n, 0, 1}, C, 1, Wd + m->rvq_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, s->E, 0, st))) return rc;
   float* x = s->XC + (size_t)(c.kernel - 1) * C;  // residual stream: the rows behind conv0's context rows
   upsample_kernel<<<dim3(T2, 1), 256, 0, st>>>(s->E, Wd + m->up_w, x, n, C, s->up_prev);
-  MCK(cudaGetLastError());
-  MCK(cudaMemcpyAsync(s->up_prev, s->E + (size_t)(n - 1) * C, (size_t)C * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(s->up_prev, s->E + (size_t)(n - 1) * C, (size_t)C * 4, cudaMemcpyDeviceToDevice, st));
   // ---- transformer: K/V of the new positions go to the rings, queries attend over the ring
   const KVRing ring{s->kring, s->vring, s->R, pos0};
   if ((rc = run_layers(c, m->layers, tcm, Wd, m->dev_h, m->rope, m->rope_T2, x, 1, T2, s->tr, &ring, st))) return rc;
@@ -1263,7 +1244,7 @@ int stream_step(sopro_mimi_stream* s, const int32_t* codes, int n, int code_stri
   TailShift ts{};
   if ((rc = tcm ? seanet_tc(m, x, s->sea, 1, T2, &ts, wav, st) : seanet_f32(m, s->sea, 1, T2, &ts, wav, st))) return rc;
   tail_shift_kernel<<<ts.n, 256, 16384, st>>>(ts);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   s->frames += n;
   return SOPRO_OK;
 }
@@ -1272,10 +1253,10 @@ int stream_step(sopro_mimi_stream* s, const int32_t* codes, int n, int code_stri
 extern "C" {
 
 int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_stream_t** out) {
-  if (!m || !out) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!m || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (max_chunk_frames < 1 || max_chunk_frames > 256) return mfail(SOPRO_ERR_INVALID, "max_chunk_frames must be in [1, 256]");
-  MCK(cudaSetDevice(m->device));
+  if (max_chunk_frames < 1 || max_chunk_frames > 256) return fail(SOPRO_ERR_INVALID, "max_chunk_frames must be in [1, 256]");
+  CK(cudaSetDevice(m->device));
   sopro_mimi_stream* s = new sopro_mimi_stream();
   s->m = m;
   s->max_n = max_chunk_frames;
@@ -1284,20 +1265,20 @@ int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_s
   stream_layout(s, nullptr);
   if ((size_t)(m->cfg.kernel - 1) * m->cfg.hidden * 4 > 16384) {
     delete s;
-    return mfail(SOPRO_ERR_UNSUPPORTED, "conv context rows exceed the tail-shift staging buffer");
+    return fail(SOPRO_ERR_UNSUPPORTED, "conv context rows exceed the tail-shift staging buffer");
   }
   cudaError_t e = cudaMalloc(&s->slab, s->slab_bytes);
   if (e != cudaSuccess) {
     const size_t mb = s->slab_bytes >> 20;
     delete s;
-    return mfail(SOPRO_ERR_CUDA, "stream state %zu MB: %s", mb, cudaGetErrorString(e));
+    return fail(SOPRO_ERR_CUDA, "stream state %zu MB: %s", mb, cudaGetErrorString(e));
   }
   stream_layout(s, s->slab);
   e = cudaMemset(s->slab, 0, s->state_bytes);
   if (e != cudaSuccess) {
     cudaFree(s->slab);
     delete s;
-    return mfail(SOPRO_ERR_CUDA, "stream state init: %s", cudaGetErrorString(e));
+    return fail(SOPRO_ERR_CUDA, "stream state init: %s", cudaGetErrorString(e));
   }
   *out = s;
   return SOPRO_OK;
@@ -1313,21 +1294,21 @@ int sopro_mimi_stream_destroy(sopro_mimi_stream_t* s) {
 }
 
 int sopro_mimi_stream_reset(sopro_mimi_stream_t* s, void* stream) {
-  if (!s) return mfail(SOPRO_ERR_INVALID, "null argument");
-  MCK(cudaSetDevice(s->m->device));
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(s->m->device));
   if (s->precision != s->m->precision) {  // the buffers are laid out per arithmetic mode
     s->precision = s->m->precision;
     size_t old = s->slab_bytes;
     stream_layout(s, nullptr);
     if (s->slab_bytes > old) {
-      MCK(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));
+      CK(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));
       cudaFree(s->slab);
       s->slab = nullptr;
-      MCK(cudaMalloc(&s->slab, s->slab_bytes));
+      CK(cudaMalloc(&s->slab, s->slab_bytes));
     }
     stream_layout(s, s->slab);
   }
-  MCK(cudaMemsetAsync(s->slab, 0, s->state_bytes, reinterpret_cast<cudaStream_t>(stream)));
+  CK(cudaMemsetAsync(s->slab, 0, s->state_bytes, reinterpret_cast<cudaStream_t>(stream)));
   s->frames = 0;
   return SOPRO_OK;
 }
@@ -1335,16 +1316,16 @@ int sopro_mimi_stream_reset(sopro_mimi_stream_t* s, void* stream) {
 int64_t sopro_mimi_stream_frames(const sopro_mimi_stream_t* s) { return s ? s->frames : -1; }
 
 int sopro_mimi_decode_step(sopro_mimi_stream_t* s, const int32_t* codes, int n, float* wav, void* stream) {
-  if (!s || !codes || !wav) return mfail(SOPRO_ERR_INVALID, "null argument");
-  if (n < 1) return mfail(SOPRO_ERR_INVALID, "n must be >= 1");
+  if (!s || !codes || !wav) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (n < 1) return fail(SOPRO_ERR_INVALID, "n must be >= 1");
   if (s->precision != s->m->precision)
-    return mfail(SOPRO_ERR_STATE, "the decoder's precision changed since this stream started: call sopro_mimi_stream_reset");
-  if (2 * (s->frames + n) > 0x3fffffffLL) return mfail(SOPRO_ERR_INVALID, "stream too long");
+    return fail(SOPRO_ERR_STATE, "the decoder's precision changed since this stream started: call sopro_mimi_stream_reset");
+  if (2 * (s->frames + n) > 0x3fffffffLL) return fail(SOPRO_ERR_INVALID, "stream too long");
   if (s->precision == SOPRO_MIMI_BF16_TC) {
     const int rc = check_tc_geometry(s->m);
     if (rc) return rc;
   }
-  MCK(cudaSetDevice(s->m->device));
+  CK(cudaSetDevice(s->m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int64_t hop = sopro_mimi_samples_per_frame(s->m);
   for (int done = 0; done < n; done += s->max_n) {  // codes are [n_q][n]: a sub-chunk starts at column `done`
@@ -1356,24 +1337,24 @@ int sopro_mimi_decode_step(sopro_mimi_stream_t* s, const int32_t* codes, int n, 
 }
 
 int sopro_mimi_decode_step_host(sopro_mimi_stream_t* s, const int32_t* codes_host, int n, float* wav_host, void* stream) {
-  if (!s || !codes_host || !wav_host) return mfail(SOPRO_ERR_INVALID, "null argument");
-  if (n < 1 || n > 65536) return mfail(SOPRO_ERR_INVALID, "n must be in [1, 65536]");
+  if (!s || !codes_host || !wav_host) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (n < 1 || n > 65536) return fail(SOPRO_ERR_INVALID, "n must be in [1, 65536]");
   const sopro_mimi_config_t& c = s->m->cfg;
   for (size_t i = 0; i < (size_t)n * c.n_q; ++i)
     if (codes_host[i] < 0 || codes_host[i] >= c.vocab)
-      return mfail(SOPRO_ERR_INVALID, "code %d at flat index %zu is outside [0, %d)", codes_host[i], i, c.vocab);
-  MCK(cudaSetDevice(s->m->device));
+      return fail(SOPRO_ERR_INVALID, "code %d at flat index %zu is outside [0, %d)", codes_host[i], i, c.vocab);
+  CK(cudaSetDevice(s->m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const size_t nc = (size_t)n * c.n_q, nw = (size_t)n * (size_t)sopro_mimi_samples_per_frame(s->m);
   cudaFree(s->codes_dev);
   s->codes_dev = nullptr;
-  MCK(cudaMalloc(&s->codes_dev, nc * 4 + nw * 4));
+  CK(cudaMalloc(&s->codes_dev, nc * 4 + nw * 4));
   s->wav_dev = reinterpret_cast<float*>(s->codes_dev + nc);
-  MCK(cudaMemcpyAsync(s->codes_dev, codes_host, nc * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s->codes_dev, codes_host, nc * 4, cudaMemcpyHostToDevice, st));
   const int rc = sopro_mimi_decode_step(s, s->codes_dev, n, s->wav_dev, stream);
   if (rc) return rc;
-  MCK(cudaMemcpyAsync(wav_host, s->wav_dev, nw * 4, cudaMemcpyDeviceToHost, st));
-  MCK(cudaStreamSynchronize(st));
+  CK(cudaMemcpyAsync(wav_host, s->wav_dev, nw * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   return SOPRO_OK;
 }
 
@@ -1382,19 +1363,19 @@ int sopro_mimi_decode_step_host(sopro_mimi_stream_t* s, const int32_t* codes_hos
 extern "C" {
 
 int sopro_mimi_check(sopro_mimi_t* m, void* stream) {
-  if (!m) return mfail(SOPRO_ERR_INVALID, "null argument");
-  MCK(cudaSetDevice(m->device));
+  if (!m) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int flag = 0;
-  MCK(cudaMemcpyAsync(&flag, m->bad_code, 4, cudaMemcpyDeviceToHost, st));
-  MCK(cudaMemsetAsync(m->bad_code, 0, 4, st));
-  MCK(cudaStreamSynchronize(st));
-  if (flag) return mfail(SOPRO_ERR_INVALID, "a decode since the last check read a code outside [0, %d) (clamped)", m->cfg.vocab);
+  CK(cudaMemcpyAsync(&flag, m->bad_code, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemsetAsync(m->bad_code, 0, 4, st));
+  CK(cudaStreamSynchronize(st));
+  if (flag) return fail(SOPRO_ERR_INVALID, "a decode since the last check read a code outside [0, %d) (clamped)", m->cfg.vocab);
   return SOPRO_OK;
 }
 
 int sopro_mimi_set_graphs(sopro_mimi_t* m, int enabled) {
-  if (!m) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!m) return fail(SOPRO_ERR_INVALID, "null argument");
   m->graphs = enabled != 0;
   return SOPRO_OK;
 }
@@ -1402,36 +1383,36 @@ int sopro_mimi_set_graphs(sopro_mimi_t* m, int enabled) {
 int sopro_debug_tc_gemm(const void* X, int B, int64_t rows, int cin, int taps, int dil, int pad, const void* W, int N,
                         const float* bias, int bias_mod, int epi, const float* R, const float* scale, float* out_f32,
                         void* out_bf16, int out_elu, void* stream) {
-  if (!X || !W || (!out_f32 && !out_bf16)) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!X || !W || (!out_f32 && !out_bf16)) return fail(SOPRO_ERR_INVALID, "null argument");
   if (B < 1 || B > 65535 || rows < 1 || rows > 0x7fffffffLL || !tc::supported(N, taps * cin, cin))
-    return mfail(SOPRO_ERR_INVALID, "tc gemm: unsupported shape (rows=%lld cin=%d taps=%d N=%d)", (long long)rows, cin, taps, N);
+    return fail(SOPRO_ERR_INVALID, "tc gemm: unsupported shape (rows=%lld cin=%d taps=%d N=%d)", (long long)rows, cin, taps, N);
   tc::TcOp o{};
   o.bias = bias; o.R = R; o.scale = scale; o.out_f32 = out_f32; o.out_bf16 = reinterpret_cast<__nv_bfloat16*>(out_bf16);
   o.c_bs = rows * N; o.M = (int)rows; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = dil; o.pad = pad;
   o.bias_mod = bias_mod > 0 ? bias_mod : N; o.epi = epi; o.out_elu = out_elu;
   cudaError_t e = tc::launch(X, rows, W, o, B, reinterpret_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core GEMM launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "tensor-core GEMM launch: %s", cudaGetErrorString(e));
   return SOPRO_OK;
 }
 
 int sopro_debug_tc_attn(const void* q, const void* k, const void* vt, void* out, int B, int T2, int64_t T2p, int C, int H, int window,
                         void* stream) {
-  if (!q || !k || !vt || !out) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!q || !k || !vt || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   if (B < 1 || B > 65535 || T2 < 1 || T2p < T2 || T2p % 8 != 0 || !tc::attn_supported(C, H, window))
-    return mfail(SOPRO_ERR_INVALID, "tc attention: unsupported shape (B=%d T2=%d T2p=%lld C=%d H=%d window=%d)", B, T2, (long long)T2p,
-                 C, H, window);
+    return fail(SOPRO_ERR_INVALID, "tc attention: unsupported shape (B=%d T2=%d T2p=%lld C=%d H=%d window=%d)", B, T2, (long long)T2p,
+                C, H, window);
   cudaError_t e = tc::launch_attn(q, k, vt, static_cast<__nv_bfloat16*>(out), B, T2, T2p, C, H, window,
                                   reinterpret_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "tensor-core attention launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "tensor-core attention launch: %s", cudaGetErrorString(e));
   return SOPRO_OK;
 }
 
 int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2, const float* Z,
                             float* out_f32, void* out_bf16, int B, int M, int ctx, int hid, int taps, int out_elu, void* stream) {
-  if (!X || !W1 || !W2 || !bias1 || !bias2 || !Z || (!out_f32 && !out_bf16)) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!X || !W1 || !W2 || !bias1 || !bias2 || !Z || (!out_f32 && !out_bf16)) return fail(SOPRO_ERR_INVALID, "null argument");
   if (B < 1 || B > 65535 || M < 1 || taps < 1 || ctx < 0 || ctx > taps - 1 || (long long)M + ctx > 0x7fffffffLL ||
       !tc::resblock_supported(hid, 2 * hid) || (2 * hid * taps) % 64 != 0)
-    return mfail(SOPRO_ERR_INVALID, "fused ResnetBlock: unsupported shape (B=%d M=%d ctx=%d hid=%d taps=%d)", B, M, ctx, hid, taps);
+    return fail(SOPRO_ERR_INVALID, "fused ResnetBlock: unsupported shape (B=%d M=%d ctx=%d hid=%d taps=%d)", B, M, ctx, hid, taps);
   // the operand geometry of seanet_tc: ctx context rows in front of the M rows, the causal zero pad covers the rest
   tc::ResOp ro{};
   ro.bias1 = bias1;
@@ -1445,46 +1426,46 @@ int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const
   ro.pad = taps - 1 - ctx;
   ro.out_elu = out_elu;
   cudaError_t e = tc::launch_resblock(X, W1, W2, hid, ro, B, reinterpret_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "fused ResnetBlock launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "fused ResnetBlock launch: %s", cudaGetErrorString(e));
   return SOPRO_OK;
 }
 
 int sopro_debug_rope_pack(const float* qkv, const float* table, int tab_T2, void* qh, void* kh, void* vt, int B, int T2, int C, int H,
                           void* stream) {
-  if (!qkv || !table || !qh || !kh || !vt) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!qkv || !table || !qh || !kh || !vt) return fail(SOPRO_ERR_INVALID, "null argument");
   const size_t pack_bytes = (size_t)32 * (C + 2) * 2;
   if (B < 1 || B > 65535 || T2 < 1 || tab_T2 < T2 || H < 1 || C != H * tc::kAttnDh || pack_bytes > 48 * 1024)
-    return mfail(SOPRO_ERR_INVALID, "rope pack: unsupported shape (B=%d T2=%d tab_T2=%d C=%d H=%d)", B, T2, tab_T2, C, H);
+    return fail(SOPRO_ERR_INVALID, "rope pack: unsupported shape (B=%d T2=%d tab_T2=%d C=%d H=%d)", B, T2, tab_T2, C, H);
   const long long T2p = (T2 + 7) / 8 * 8;  // as run_layers pitches v^T
   rope_pack_kernel<tc::kAttnDh><<<dim3((T2 + 31) / 32, B), 256, pack_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(
       qkv, table, static_cast<__nv_bfloat16*>(qh), static_cast<__nv_bfloat16*>(kh), static_cast<__nv_bfloat16*>(vt), T2, T2p, tab_T2, C, H);
-  MCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
 int sopro_mimi_decode_host(sopro_mimi_t* m, const int32_t* codes_host, int B, int T, float* wav_host, void* stream) {
-  if (!m || !codes_host || !wav_host) return mfail(SOPRO_ERR_INVALID, "null argument");
-  MCK(cudaSetDevice(m->device));
+  if (!m || !codes_host || !wav_host) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (B < 1 || T < 1) return mfail(SOPRO_ERR_INVALID, "B and T must be >= 1");
+  if (B < 1 || T < 1) return fail(SOPRO_ERR_INVALID, "B and T must be >= 1");
   const size_t nc = (size_t)B * m->cfg.n_q * T;
   const size_t nw = (size_t)B * T * sopro_mimi_samples_per_frame(m);
   for (size_t i = 0; i < nc; ++i)
     if (codes_host[i] < 0 || codes_host[i] >= m->cfg.vocab)
-      return mfail(SOPRO_ERR_INVALID, "code %d at flat index %zu is outside [0, %d)", codes_host[i], i, m->cfg.vocab);
+      return fail(SOPRO_ERR_INVALID, "code %d at flat index %zu is outside [0, %d)", codes_host[i], i, m->cfg.vocab);
   if (m->codes_cap < nc * 4 + nw * 4) {
     cudaFree(m->codes_dev);
     m->codes_dev = nullptr;
     m->codes_cap = 0;
-    MCK(cudaMalloc(&m->codes_dev, nc * 4 + nw * 4));
+    CK(cudaMalloc(&m->codes_dev, nc * 4 + nw * 4));
     m->codes_cap = nc * 4 + nw * 4;
   }
   float* wav_dev = reinterpret_cast<float*>(m->codes_dev + nc);
-  MCK(cudaMemcpyAsync(m->codes_dev, codes_host, nc * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(m->codes_dev, codes_host, nc * 4, cudaMemcpyHostToDevice, st));
   int rc = sopro_mimi_decode(m, m->codes_dev, B, T, wav_dev, stream);
   if (rc) return rc;
-  MCK(cudaMemcpyAsync(wav_host, wav_dev, nw * 4, cudaMemcpyDeviceToHost, st));
-  MCK(cudaStreamSynchronize(st));
+  CK(cudaMemcpyAsync(wav_host, wav_dev, nw * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   return SOPRO_OK;
 }
 
@@ -1651,21 +1632,21 @@ extern "C" {
 
 int sopro_mimi_encoder_create(const sopro_mimi_config_t* cfg, const sopro_mimi_encoder_weights_t* w, int device,
                               sopro_mimi_encoder_t** out) {
-  if (!cfg || !w || !out) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
   int ndev = 0;
   cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0) return mfail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the Mimi encoder has no CPU fallback");
-  if (device < 0 || device >= ndev) return mfail(SOPRO_ERR_INVALID, "device %d out of range", device);
+  if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the Mimi encoder has no CPU fallback");
+  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
-  MCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return mfail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  CK(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int C = cfg->hidden, Dc = cfg->codebook_dim, Q = cfg->n_q, V = cfg->vocab, NL = cfg->n_layers, FF = cfg->ffn, F0 = cfg->num_filters;
   if (C % 64 || Dc != 256 || C != 2 * Dc || NL < 1 || NL > SOPRO_MIMI_MAX_LAYERS || cfg->n_ratios < 1 || cfg->n_ratios > SOPRO_MIMI_MAX_RATIOS ||
       cfg->n_heads < 1 || C % cfg->n_heads || (C / cfg->n_heads) % 4 || FF % 16 || F0 % 16 || cfg->compress != 2 || Q < 1 || cfg->n_sem < 1 ||
       cfg->n_sem > Q || cfg->kernel < 1 || cfg->kernel > 16)
-    return mfail(SOPRO_ERR_INVALID, "unsupported Mimi encoder geometry (hidden=%d codebook_dim=%d)", C, Dc);
-  MCK(cudaSetDevice(device));
+    return fail(SOPRO_ERR_INVALID, "unsupported Mimi encoder geometry (hidden=%d codebook_dim=%d)", C, Dc);
+  CK(cudaSetDevice(device));
   sopro_mimi_encoder* e = new sopro_mimi_encoder();
   e->device = device;
   e->cfg = *cfg;
@@ -1712,7 +1693,7 @@ int sopro_mimi_encoder_create(const sopro_mimi_config_t* cfg, const sopro_mimi_e
   if (err != cudaSuccess) {
     if (e->dev) cudaFree(e->dev);
     delete e;
-    return mfail(SOPRO_ERR_CUDA, "Mimi encoder weight upload failed: %s", cudaGetErrorString(err));
+    return fail(SOPRO_ERR_CUDA, "Mimi encoder weight upload failed: %s", cudaGetErrorString(err));
   }
   *out = e;
   return SOPRO_OK;
@@ -1737,10 +1718,10 @@ int64_t sopro_mimi_encoded_frames(const sopro_mimi_encoder_t* e, int64_t n_sampl
 }
 
 int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_samples, int32_t* codes, float* latent, void* stream) {
-  if (!e || !wav || !codes) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!e || !wav || !codes) return fail(SOPRO_ERR_INVALID, "null argument");
   if (n_samples < 1 || n_samples > kEncMaxSamples)
-    return mfail(SOPRO_ERR_INVALID, "n_samples=%lld outside [1, %lld]", (long long)n_samples, kEncMaxSamples);
-  MCK(cudaSetDevice(e->device));
+    return fail(SOPRO_ERR_INVALID, "n_samples=%lld outside [1, %lld]", (long long)n_samples, kEncMaxSamples);
+  CK(cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
   const sopro_mimi_config_t& c = e->cfg;
   const int C = c.hidden, Dc = c.codebook_dim;
@@ -1753,7 +1734,7 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
     e->ws = nullptr;
     e->ws_bytes = 0;
     cudaError_t ae = cudaMalloc(&e->ws, P.need);
-    if (ae != cudaSuccess) return mfail(SOPRO_ERR_CUDA, "Mimi encoder workspace %zu MB: %s", P.need >> 20, cudaGetErrorString(ae));
+    if (ae != cudaSuccess) return fail(SOPRO_ERR_CUDA, "Mimi encoder workspace %zu MB: %s", P.need >> 20, cudaGetErrorString(ae));
     e->ws_bytes = P.need;
   }
   float* b0 = e->ws;
@@ -1769,7 +1750,7 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
   {
     const long long tot = n_samples * c.num_filters;
     enc_conv0_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(wav, Wd + e->c0w, Wd + e->c0b, cur, n_samples, c.num_filters, c.kernel);
-    MCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   int ch = c.num_filters;
   for (int s = 0; s < c.n_ratios; ++s) {
@@ -1781,7 +1762,7 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
       return rc;
     if ((rc = gemm_f32({hid, Ls, 0, 1}, ch / 2, 1, Wd + S.r2w, Wd + S.r2b, ch, ch, EPI_RES, cur, nullptr, cur, 1, st))) return rc;
     // ELU + conv kernel 2r stride r: zero rows up to a multiple of r, then 2 taps over [Lp/r][r*ch]
-    if (Lp > Ls) MCK(cudaMemsetAsync(cur + (size_t)Ls * ch, 0, (size_t)(Lp - Ls) * ch * 4, st));
+    if (Lp > Ls) CK(cudaMemsetAsync(cur + (size_t)Ls * ch, 0, (size_t)(Lp - Ls) * ch * 4, st));
     if ((rc = gemm_f32({cur, Lp / r, 0, 1}, r * ch, 2, Wd + S.dw, Wd + S.db, 2 * ch, 2 * ch, EPI_NONE, nullptr, nullptr, nxt, 1, st)))
       return rc;
     std::swap(cur, nxt);
@@ -1801,24 +1782,24 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
     const int rows = 2 * T + 2;
     const long long tot = (long long)rows * C;
     replicate_pad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(x, b0, T2, C, 2, rows);
-    MCK(cudaGetLastError());
+    CK(cudaGetLastError());
     float* lat = latent ? latent : b1;
     // 2 taps over the T + 1 row pairs [rows/2][2C]: the first pair (the left padding) is the context of output row 0
     if ((rc = gemm_f32({b0, T, 1, 1}, 2 * C, 2, Wd + e->down_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, lat, 0, st))) return rc;
     // ---- quantizer: both input projections in one GEMM, then the residual search
     if ((rc = gemm_f32({lat, T, 0, 1}, C, 1, Wd + e->inproj, nullptr, 2 * Dc, 2 * Dc, EPI_NONE, nullptr, nullptr, b2, 0, st))) return rc;
     rvq_encode_kernel<8><<<T, 256, 0, st>>>(b2, Wd + e->embed, codes, T, c.n_q, c.n_sem, c.vocab);
-    MCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }
 
 int sopro_mimi_encode_host(sopro_mimi_encoder_t* e, const float* wav_host, int64_t n_samples, int32_t* codes_host,
                            float* latent_host, void* stream) {
-  if (!e || !wav_host || !codes_host) return mfail(SOPRO_ERR_INVALID, "null argument");
+  if (!e || !wav_host || !codes_host) return fail(SOPRO_ERR_INVALID, "null argument");
   if (n_samples < 1 || n_samples > kEncMaxSamples)
-    return mfail(SOPRO_ERR_INVALID, "n_samples=%lld outside [1, %lld]", (long long)n_samples, kEncMaxSamples);
-  MCK(cudaSetDevice(e->device));
+    return fail(SOPRO_ERR_INVALID, "n_samples=%lld outside [1, %lld]", (long long)n_samples, kEncMaxSamples);
+  CK(cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
   const long long T = enc_plan(e->cfg, n_samples).T;
   const size_t nc = (size_t)e->cfg.n_q * T, nl = (size_t)T * e->cfg.hidden;
@@ -1826,29 +1807,29 @@ int sopro_mimi_encode_host(sopro_mimi_encoder_t* e, const float* wav_host, int64
     cudaFree(e->wav_dev);
     e->wav_dev = nullptr;
     e->wav_cap = 0;
-    MCK(cudaMalloc(&e->wav_dev, (size_t)n_samples * 4));
+    CK(cudaMalloc(&e->wav_dev, (size_t)n_samples * 4));
     e->wav_cap = (size_t)n_samples;
   }
   if (e->codes_cap < nc) {
     cudaFree(e->codes_dev);
     e->codes_dev = nullptr;
     e->codes_cap = 0;
-    MCK(cudaMalloc(&e->codes_dev, nc * 4));
+    CK(cudaMalloc(&e->codes_dev, nc * 4));
     e->codes_cap = nc;
   }
   if (latent_host && e->lat_cap < nl) {
     cudaFree(e->lat_dev);
     e->lat_dev = nullptr;
     e->lat_cap = 0;
-    MCK(cudaMalloc(&e->lat_dev, nl * 4));
+    CK(cudaMalloc(&e->lat_dev, nl * 4));
     e->lat_cap = nl;
   }
-  MCK(cudaMemcpyAsync(e->wav_dev, wav_host, (size_t)n_samples * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(e->wav_dev, wav_host, (size_t)n_samples * 4, cudaMemcpyHostToDevice, st));
   const int rc = sopro_mimi_encode(e, e->wav_dev, n_samples, e->codes_dev, latent_host ? e->lat_dev : nullptr, st);
   if (rc) return rc;
-  MCK(cudaMemcpyAsync(codes_host, e->codes_dev, nc * 4, cudaMemcpyDeviceToHost, st));
-  if (latent_host) MCK(cudaMemcpyAsync(latent_host, e->lat_dev, nl * 4, cudaMemcpyDeviceToHost, st));
-  MCK(cudaStreamSynchronize(st));
+  CK(cudaMemcpyAsync(codes_host, e->codes_dev, nc * 4, cudaMemcpyDeviceToHost, st));
+  if (latent_host) CK(cudaMemcpyAsync(latent_host, e->lat_dev, nl * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   return SOPRO_OK;
 }
 

@@ -7,37 +7,17 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
 
 #include "../../include/sopro_b200.h"
+#include "common.cuh"
 #include "dense_f32.cuh"
 #include "mimi_tc.cuh"  // tc::launch: the wgmma / TMA implicit-GEMM kernel, reused for the exact split products
 
-namespace mimi {
-void set_error(const char* msg);  // ar_engine.cu: the string behind sopro_last_error()
-}
-
 namespace pstage {
-
-int fail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-#define PCK(call)                                                                                                       \
-  do {                                                                                                                  \
-    cudaError_t e__ = (call);                                                                                           \
-    if (e__ != cudaSuccess)                                                                                             \
-      return pstage::fail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
 
 struct FArena {
   std::vector<float> host;
@@ -102,7 +82,7 @@ int launch_dense(dense::DenseOp op, int groups, cudaStream_t st, int edge = 0, i
     // a function attribute belongs to the current device's context: set once per device
     static unsigned long long attr_done = 0;
     if (tc::attr_needed(attr_done))
-      PCK(cudaFuncSetAttribute(dense::dense_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 2048 * 4));
+      CK(cudaFuncSetAttribute(dense::dense_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 2048 * 4));
     if (parts_out) *parts_out = parts;
     dense::dense_skinny_kernel<<<dim3(parts, 1, groups), dense::kSkinnyThreads, smem, st>>>(op, cols);
   } else {
@@ -116,7 +96,7 @@ int launch_dense(dense::DenseOp op, int groups, cudaStream_t st, int edge = 0, i
     else if (e == 64) dense::dense_tile_kernel<64, 64><<<grid, dense::kTileThreads, 0, st>>>(op);
     else dense::dense_tile_kernel<32, 32><<<grid, dense::kTileThreads, 0, st>>>(op);
   }
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -305,7 +285,7 @@ int ssm_block_tc(const float* W, const BlockOff& o, const uint16_t* T, const Blo
   if ((rc = launch_tc6(a3, T + t.w1, W + o.b1, nullptr, v, M, 4 * D, D, tc::EPI_GELU, st))) return rc;
   split3_rows_kernel<<<rb, 256, 0, st>>>(v, nullptr, a3, M, 4 * D);
   if ((rc = launch_tc6(a3, T + t.w2, W + o.b2, x, x, M, D, 4 * D, tc::EPI_RES, st))) return rc;
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -320,7 +300,7 @@ int ssm_block(const float* W, const BlockOff& o, float* x, float* h, float* hid,
   if (rc) return rc;
   const int total = (k - 1) * dil, left = causal ? total : total / 2;
   dense::dwconv_res_kernel<<<dim3(Tmax, B), 128, 0, st>>>(h, x, W + o.dw_w, W + o.dw_b, x, lens, Tmax, D, k, dil, left);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   g = dense::DenseOp{};
   g.A = x; g.W = W + o.w1; g.bias = W + o.b1; g.norm_w = W + o.ffn_norm_w; g.C = hid; g.M = M; g.N = 4 * D; g.K = D; g.ldc = 4 * D;
   g.epi = dense::EPI_GELU;
@@ -445,7 +425,7 @@ int sopro_nar_create(const sopro_nar_config_t* cfg, const sopro_nar_weights_t* w
   if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the NAR refiner has no CPU fallback");
   if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
-  PCK(cudaGetDeviceProperties(&prop, device));
+  CK(cudaGetDeviceProperties(&prop, device));
   if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int D = cfg->d_model, NL = cfg->n_layers, k = cfg->kernel, Q = cfg->n_codebooks, V = cfg->codebook_size, Hn = cfg->head_dim,
             AH = cfg->adapter_hidden, NS = cfg->n_stages;
@@ -467,7 +447,7 @@ int sopro_nar_create(const sopro_nar_config_t* cfg, const sopro_nar_weights_t* w
         return fail(SOPRO_ERR_INVALID, "NAR stage %d head %d: null weight or codebook out of range", s, j);
     covered += cfg->stage_count[s];
   }
-  PCK(cudaSetDevice(device));
+  CK(cudaSetDevice(device));
   sopro_nar* n = new sopro_nar();
   n->device = device;
   n->cfg = *cfg;
@@ -628,7 +608,7 @@ int sopro_debug_dense(const float* A, const float* W, const float* bias, const f
   int rc = launch_dense(op, groups, st, kernel, &parts);
   if (rc || !amax) return rc;
   dense::argmax_finish_kernel<<<dim3((unsigned)((M + 127) / 128), groups), 128, 0, st>>>(op.amax_val, op.amax_idx, M, parts, ids, groups);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -641,7 +621,7 @@ int sopro_debug_tc6(const float* X, const float* norm_w, const uint16_t* W6, con
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   __nv_bfloat16* a3 = static_cast<__nv_bfloat16*>(A3);
   split3_rows_kernel<<<(unsigned)((M + 7) / 8), 256, 0, st>>>(X, norm_w, a3, M, K);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return launch_tc6(a3, W6, bias, R, C, M, N, K, epi, st);
 }
 
@@ -651,7 +631,7 @@ int sopro_debug_dwconv_res(const float* h, const float* x, const float* w, const
   if (B < 1 || B > 65535 || Tmax < 1 || D < 1 || k < 1 || k > 64 || dil < 1 || left < 0 || left > (k - 1) * dil)
     return fail(SOPRO_ERR_INVALID, "debug dwconv: bad shape B=%d Tmax=%d D=%d k=%d dil=%d left=%d", B, Tmax, D, k, dil, left);
   dense::dwconv_res_kernel<<<dim3(Tmax, B), 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(h, x, w, bias, out, lens, Tmax, D, k, dil, left);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -660,7 +640,7 @@ int sopro_debug_argmax_heads(const float* logits, int64_t rows, int heads, int V
   if (rows < 1 || rows > 0x3fffffffLL || heads < 1 || V < 4 || V % 4 || Q < heads)
     return fail(SOPRO_ERR_INVALID, "debug argmax heads: bad shape rows=%lld heads=%d V=%d Q=%d", (long long)rows, heads, V, Q);
   argmax_heads_kernel<<<(unsigned)((rows * heads + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(logits, rows, heads, V, codes, Q);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -693,7 +673,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
   const sopro_nar_config_t& c = n->cfg;
   const int D = c.d_model, Q = c.n_codebooks, V = c.codebook_size, Hn = c.head_dim;
   if (cond_batch_stride < (int64_t)Tmax * D) return fail(SOPRO_ERR_INVALID, "cond_batch_stride smaller than Tmax*d_model");
-  PCK(cudaSetDevice(n->device));
+  CK(cudaSetDevice(n->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long M = (long long)B * Tmax;
   int max_heads = 1;
@@ -713,7 +693,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
   const size_t flog = use_tc ? (size_t)mc * max_heads * V : 0;
   const size_t need = std::max(n->reserve_bytes, (al(fx) + al(fh) + al(fhid) + al(fz) + 2 * al(famax) + al(fa3) + al(flog)) * 4);
   if (n->ws_bytes < need) {
-    PCK(cudaStreamSynchronize(st));
+    CK(cudaStreamSynchronize(st));
     nar_drop_replays(n);  // the graphs hold pointers into the old workspace
     cudaFree(n->ws);
     n->ws = nullptr;
@@ -736,7 +716,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
   float* logits = amax_v + 2 * al(famax) + al(fa3);
   const float* W = n->dev;
   set_first_codebook_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(rvq1, codes, M, Q);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   float* trace = n->trace_z;
   for (const auto& S : n->stages) {
     EmbedMix em{};
@@ -744,7 +724,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
     em.norm_w = W + n->adapter_norm_w; em.mul = W + S.mul; em.add = W + S.add; em.out = x; em.mix0 = S.mix0; em.mix1 = S.mix1;
     em.Tmax = Tmax; em.D = D; em.Q = Q; em.V = V; em.n_prev = S.n_prev;
     nar_embed_mix_kernel<<<(unsigned)((M + 7) / 8), 256, 0, st>>>(em, M);
-    PCK(cudaGetLastError());
+    CK(cudaGetLastError());
     int rc;
     if (use_tc) {
       for (int i = 0; i < c.n_layers; ++i)
@@ -753,7 +733,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
       split3_rows_kernel<<<rb, 256, 0, st>>>(x, W + n->norm_w, a3, M, D);
       if ((rc = launch_tc6(a3, n->tcw + n->tc_pre, W + n->pre_b, nullptr, z, M, Hn, D, tc::EPI_NONE, st))) return rc;
       if (trace) {
-        PCK(cudaMemcpyAsync(trace, z, (size_t)M * Hn * 4, cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(trace, z, (size_t)M * Hn * 4, cudaMemcpyDeviceToDevice, st));
         trace += (size_t)M * Hn;
       }
       split3_rows_kernel<<<rb, 256, 0, st>>>(z, nullptr, a3, M, Hn);
@@ -763,7 +743,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
           return rc;
         argmax_heads_kernel<<<(unsigned)((rows * S.count + 7) / 8), 256, 0, st>>>(logits, rows, S.count, V, codes + m0 * Q + S.first, Q);
       }
-      PCK(cudaGetLastError());
+      CK(cudaGetLastError());
       continue;
     }
     for (int i = 0; i < c.n_layers; ++i)
@@ -773,7 +753,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
     g.epi = dense::EPI_BIAS;
     if ((rc = launch_dense(g, 1, st))) return rc;
     if (trace) {
-      PCK(cudaMemcpyAsync(trace, z, (size_t)M * Hn * 4, cudaMemcpyDeviceToDevice, st));
+      CK(cudaMemcpyAsync(trace, z, (size_t)M * Hn * 4, cudaMemcpyDeviceToDevice, st));
       trace += (size_t)M * Hn;
     }
     g = dense::DenseOp{};
@@ -782,7 +762,7 @@ static int nar_refine_impl(sopro_nar_t* n, const float* cond, int64_t cond_batch
     const int parts = argmax_parts((int)M, V, S.count);
     if ((rc = launch_dense(g, S.count, st))) return rc;
     dense::argmax_finish_kernel<<<dim3((unsigned)((M + 127) / 128), S.count), 128, 0, st>>>(amax_v, amax_i, (int)M, parts, codes + S.first, Q);
-    PCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }
@@ -800,17 +780,17 @@ int sopro_nar_refine(sopro_nar_t* n, const float* cond, int64_t cond_batch_strid
   if (!n || !cond || !rvq1 || !codes) return fail(SOPRO_ERR_INVALID, "null argument");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  PCK(cudaSetDevice(n->device));
-  PCK(cudaStreamIsCapturing(st, &cap));
+  CK(cudaSetDevice(n->device));
+  CK(cudaStreamIsCapturing(st, &cap));
   // one utterance's streaming window: replay the whole pass (113..217 launches) from a graph over static buffers
   if (!n->graphs || B != 1 || Tmax < 1 || Tmax > kNarGraphRows || lens || n->forced || n->trace_z || cap != cudaStreamCaptureStatusNone)
     return nar_refine_impl(n, cond, cond_batch_stride, rvq1, lens, B, Tmax, codes, stream);
   const sopro_nar_config_t& c = n->cfg;
   const int D = c.d_model, Q = c.n_codebooks;
   if (!n->g_cond) {
-    PCK(cudaMalloc(&n->g_cond, (size_t)kNarGraphRows * D * 4));
-    PCK(cudaMalloc(&n->g_rvq1, (size_t)kNarGraphRows * 4));
-    PCK(cudaMalloc(&n->g_codes, (size_t)kNarGraphRows * Q * 4));
+    CK(cudaMalloc(&n->g_cond, (size_t)kNarGraphRows * D * 4));
+    CK(cudaMalloc(&n->g_rvq1, (size_t)kNarGraphRows * 4));
+    CK(cudaMalloc(&n->g_codes, (size_t)kNarGraphRows * Q * 4));
   }
   // no graph-sized call may reallocate the workspace: reserve the largest graph shape of either arithmetic path once
   if (n->reserve_bytes == 0) {
@@ -827,8 +807,8 @@ int sopro_nar_refine(sopro_nar_t* n, const float* cond, int64_t cond_batch_strid
     // warm-up outside the capture (first use of a kernel sets function attributes), then capture on a private stream
     int rc = nar_refine_impl(n, cond, cond_batch_stride, rvq1, nullptr, 1, Tmax, codes, stream);
     if (rc) return rc;
-    if (!n->cap_stream) PCK(cudaStreamCreateWithFlags(&n->cap_stream, cudaStreamNonBlocking));
-    PCK(cudaStreamBeginCapture(n->cap_stream, cudaStreamCaptureModeThreadLocal));
+    if (!n->cap_stream) CK(cudaStreamCreateWithFlags(&n->cap_stream, cudaStreamNonBlocking));
+    CK(cudaStreamBeginCapture(n->cap_stream, cudaStreamCaptureModeThreadLocal));
     rc = nar_refine_impl(n, n->g_cond, (int64_t)Tmax * D, n->g_rvq1, nullptr, 1, Tmax, n->g_codes, n->cap_stream);
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(n->cap_stream, &graph);
@@ -844,13 +824,13 @@ int sopro_nar_refine(sopro_nar_t* n, const float* cond, int64_t cond_batch_strid
     return SOPRO_OK;  // the eager warm-up produced this call's result
   }
   // replays from different caller streams share the static buffers: each waits for the previous one to finish
-  if (!n->g_done) PCK(cudaEventCreateWithFlags(&n->g_done, cudaEventDisableTiming));
-  else PCK(cudaStreamWaitEvent(st, n->g_done, 0));
-  PCK(cudaMemcpyAsync(n->g_cond, cond, (size_t)Tmax * D * 4, cudaMemcpyDeviceToDevice, st));
-  PCK(cudaMemcpyAsync(n->g_rvq1, rvq1, (size_t)Tmax * 4, cudaMemcpyDeviceToDevice, st));
-  PCK(cudaGraphLaunch(exec, st));
-  PCK(cudaMemcpyAsync(codes, n->g_codes, (size_t)Tmax * Q * 4, cudaMemcpyDeviceToDevice, st));
-  PCK(cudaEventRecord(n->g_done, st));
+  if (!n->g_done) CK(cudaEventCreateWithFlags(&n->g_done, cudaEventDisableTiming));
+  else CK(cudaStreamWaitEvent(st, n->g_done, 0));
+  CK(cudaMemcpyAsync(n->g_cond, cond, (size_t)Tmax * D * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(n->g_rvq1, rvq1, (size_t)Tmax * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaGraphLaunch(exec, st));
+  CK(cudaMemcpyAsync(codes, n->g_codes, (size_t)Tmax * Q * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaEventRecord(n->g_done, st));
   return SOPRO_OK;
 }
 
@@ -1029,7 +1009,7 @@ int sopro_prefill_create(const sopro_prefill_config_t* cfg, const sopro_prefill_
   if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the prefill has no CPU fallback");
   if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
-  PCK(cudaGetDeviceProperties(&prop, device));
+  CK(cudaGetDeviceProperties(&prop, device));
   if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int D = cfg->d_model, NL = cfg->n_layers_text, k = cfg->text_kernel, SV = cfg->sv_dim, RL = cfg->ref_layers, H = cfg->ref_heads;
   if (D < 32 || D > 512 || D % 16 || NL < 0 || NL > SOPRO_MAX_SSM_LAYERS || k < 1 || k > 64 || SV < 16 || SV % 16 || RL < 0 ||
@@ -1042,7 +1022,7 @@ int sopro_prefill_create(const sopro_prefill_config_t* cfg, const sopro_prefill_
     return fail(SOPRO_ERR_INVALID, "prefill: null weight pointer");
   for (int i = 0; i < RL; ++i)
     if (!w->ref_layer[i].nq_w || !w->ref_layer[i].q_w || !w->ref_layer[i].o_w) return fail(SOPRO_ERR_INVALID, "ref layer %d: null weight", i);
-  PCK(cudaSetDevice(device));
+  CK(cudaSetDevice(device));
   sopro_prefill* p = new sopro_prefill();
   p->device = device;
   p->cfg = *cfg;
@@ -1095,14 +1075,14 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
   if (B < 1 || Lmax < 1 || Lmax > c.max_text_len || n_frames < 1 || n_frames > c.max_frames_pos || (long long)B * n_frames > 0x3fffffffLL)
     return fail(SOPRO_ERR_INVALID, "bad B=%d Lmax=%d (max %d) n_frames=%d (max %d)", B, Lmax, c.max_text_len, n_frames, c.max_frames_pos);
   if (c.ref_layers > 0 && (!ref_k || !ref_v || Tr < 1 || Tr > 4096)) return fail(SOPRO_ERR_INVALID, "reference K/V missing or Tr=%d out of range", Tr);
-  PCK(cudaSetDevice(p->device));
+  CK(cudaSetDevice(p->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long Mt = (long long)B * Lmax, Mc = (long long)B * n_frames;
   auto al = [](size_t x) { return (x + 63) / 64 * 64; };
   const size_t rows = (size_t)std::max(Mt, Mc);
   const size_t need = (al(rows * D) * 3 + al(rows * 4 * D) + al((size_t)B * D) + al((size_t)B * 2 * D)) * 4;
   if (p->ws_bytes < need) {
-    PCK(cudaStreamSynchronize(st));
+    CK(cudaStreamSynchronize(st));
     cudaFree(p->ws);
     p->ws = nullptr;
     p->ws_bytes = 0;
@@ -1120,13 +1100,13 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
   int rc;
   // ---- text encoder
   text_embed_kernel<<<dim3(Lmax, B), 128, 0, st>>>(text_ids, text_len, W + p->text_emb, W + p->text_pos, x, Lmax, D, c.text_vocab);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   for (int i = 0; i < c.n_layers_text; ++i)
     if ((rc = ssm_block(W, p->blk[i], x, h, hid, text_len, B, Lmax, D, c.text_kernel, 1, false, st))) return rc;
   dense::rmsnorm_rows_kernel<<<(unsigned)((Mt + 7) / 8), 256, 0, st>>>(x, W + p->text_norm_w, nullptr, nullptr, txt_seq, Mt, D);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   mean_pool_kernel<<<B, 128, 0, st>>>(txt_seq, text_len, txt_pool, Lmax, D);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   // ---- FiLM parameters from the speaker vector(s)
   const int Bf = sv_shared ? 1 : B;
   dense::DenseOp g{};
@@ -1137,26 +1117,26 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
   if ((rc = launch_dense(g, 1, st))) return rc;
   film_rows_kernel<<<(unsigned)((Mc + 7) / 8), 256, 0, st>>>(txt_pool, W + p->frame_pos, W + p->film_ln_w, W + p->film_ln_b, film, sv_shared ? 1 : 0,
                                                             style_strength, x, Mc, n_frames, D);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   // ---- reference cross-attention stack
   const size_t rsmem = (size_t)8 * (2 * D + ((Tr + 3) & ~3)) * 4;
   if (c.ref_layers > 0 && rsmem > 48 * 1024) {
     static unsigned long long attr_done = 0;  // per device, like every function attribute
-    if (tc::attr_needed(attr_done)) PCK(cudaFuncSetAttribute(ref_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    if (tc::attr_needed(attr_done)) CK(cudaFuncSetAttribute(ref_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
   for (int i = 0; i < c.ref_layers; ++i) {
     g = dense::DenseOp{};
     g.A = x; g.W = W + p->ref[i].q_w; g.norm_w = W + p->ref[i].nq_w; g.C = q; g.M = (int)Mc; g.N = D; g.K = D; g.ldc = D; g.epi = dense::EPI_BIAS;
     if ((rc = launch_dense(g, 1, st))) return rc;
     ref_attn_kernel<<<(unsigned)((Mc + 7) / 8), 256, rsmem, st>>>(q, x, ref_k[i], ref_v[i], h, Mc, D, H, Tr);
-    PCK(cudaGetLastError());
+    CK(cudaGetLastError());
     g = dense::DenseOp{};
     g.A = h; g.W = W + p->ref[i].o_w; g.R = x; g.C = x; g.M = (int)Mc; g.N = D; g.K = D; g.ldc = D; g.epi = dense::EPI_RES_GATE;
     g.gate = p->ref[i].gate_eff;
     if ((rc = launch_dense(g, 1, st))) return rc;
   }
   dense::rmsnorm_rows_kernel<<<(unsigned)((Mc + 7) / 8), 256, 0, st>>>(x, W + p->cond_norm_w, nullptr, nullptr, cond_ar, Mc, D);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -1312,7 +1292,7 @@ int sopro_refprep_create(const sopro_refprep_config_t* cfg, const sopro_refprep_
   if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the reference preparation has no CPU fallback");
   if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
-  PCK(cudaGetDeviceProperties(&prop, device));
+  CK(cudaGetDeviceProperties(&prop, device));
   if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
   const int D = cfg->d_model, d = cfg->sv_embed_dim, SV = cfg->sv_dim, Q = cfg->n_codebooks, V = cfg->codebook_size, NL = cfg->ref_enc_layers,
             RL = cfg->ref_layers, H = cfg->ref_heads;
@@ -1327,7 +1307,7 @@ int sopro_refprep_create(const sopro_refprep_config_t* cfg, const sopro_refprep_
     if (!block_ok(w->ref_block[i])) return fail(SOPRO_ERR_INVALID, "reference encoder block %d: null weight", i);
   for (int i = 0; i < RL; ++i)
     if (!w->layer[i].nkv_w || !w->layer[i].k_w || !w->layer[i].v_w) return fail(SOPRO_ERR_INVALID, "ref layer %d: null weight", i);
-  PCK(cudaSetDevice(device));
+  CK(cudaSetDevice(device));
   sopro_refprep* p = new sopro_refprep();
   p->device = device;
   p->cfg = *cfg;
@@ -1394,14 +1374,14 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
   if (c.ref_layers > 0 && (!ref_k || !ref_v)) return fail(SOPRO_ERR_INVALID, "ref_k / ref_v missing");
   for (int i = 0; i < c.ref_layers; ++i)
     if (!ref_k[i] || !ref_v[i]) return fail(SOPRO_ERR_INVALID, "ref_k[%d] / ref_v[%d] is null", i, i);
-  PCK(cudaSetDevice(p->device));
+  CK(cudaSetDevice(p->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int D = c.d_model, d = c.sv_embed_dim, SV = c.sv_dim, Q = c.n_codebooks, V = c.codebook_size, H = c.ref_heads;
   auto al = [](size_t x) { return (x + 63) / 64 * 64; };
   const size_t rows = (size_t)Tr;
   const size_t need = (al(rows * D) * 3 + al(rows * 4 * D) + al(2 * (size_t)d) + al((size_t)SV)) * 4;
   if (p->ws_bytes < need) {
-    PCK(cudaStreamSynchronize(st));
+    CK(cudaStreamSynchronize(st));
     cudaFree(p->ws);
     p->ws = nullptr;
     p->ws_bytes = 0;
@@ -1420,27 +1400,27 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
   dense::DenseOp g{};
   // ---- Token2SV (d <= D: the [Tr][d] buffers live in x / h / q)
   codes_mix_kernel<<<Tr, 128, Q * sizeof(int), st>>>(tokens, W + p->sv_emb, W + p->sv_w, x, Q, V, d, p->bad);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   const int left = (c.sv_kernel - 1) / 2;
   dwconv_gelu_kernel<<<Tr, 128, 0, st>>>(x, W + p->dw0_w, W + p->dw0_b, h, Tr, d, c.sv_kernel, left);
   dwconv_gelu_kernel<<<Tr, 128, 0, st>>>(h, W + p->dw1_w, W + p->dw1_b, x, Tr, d, c.sv_kernel, left);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   g.A = x; g.W = W + p->pool_w0; g.bias = W + p->pool_b0; g.C = q; g.M = Tr; g.N = d; g.K = d; g.ldc = d; g.epi = dense::EPI_BIAS;
   if ((rc = launch_dense(g, 1, st))) return rc;
   attn_stats_pool_kernel<<<1, 256, (size_t)Tr * 4, st>>>(q, x, W + p->pool_w2, p->pool_b2, stats, Tr, d);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   g = dense::DenseOp{};
   g.A = stats; g.W = W + p->proj_w; g.bias = W + p->proj_b; g.C = e; g.M = 1; g.N = SV; g.K = 2 * d; g.ldc = SV; g.epi = dense::EPI_BIAS;
   if ((rc = launch_dense(g, 1, st))) return rc;
   l2_normalize_kernel<<<1, 32, 0, st>>>(e, sv, SV, 1e-6f);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   // ---- reference encoder
   codes_mix_kernel<<<Tr, 128, Q * sizeof(int), st>>>(tokens, W + p->cb_embed, W + p->ref_w, x, Q, V, D, p->bad);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   for (int i = 0; i < c.ref_enc_layers; ++i)
     if ((rc = ssm_block(W, p->blk[i], x, h, hid, nullptr, 1, Tr, D, c.ref_enc_kernel, 1, false, st))) return rc;
   dense::rmsnorm_rows_kernel<<<(unsigned)((Tr + 7) / 8), 256, 0, st>>>(x, W + p->ref_norm_w, nullptr, nullptr, ref_seq, (long long)Tr, D);
-  PCK(cudaGetLastError());
+  CK(cudaGetLastError());
   // ---- cached K / V of every reference cross-attention layer, heads-major
   const long long tot = (long long)Tr * D;
   for (int i = 0; i < c.ref_layers; ++i) {
@@ -1450,7 +1430,7 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
       g.ldc = D; g.epi = dense::EPI_BIAS;
       if ((rc = launch_dense(g, 1, st))) return rc;
       heads_major_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(h, kv ? ref_v[i] : ref_k[i], Tr, H, D / H);
-      PCK(cudaGetLastError());
+      CK(cudaGetLastError());
     }
   }
   return SOPRO_OK;
@@ -1459,13 +1439,13 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
 /* Synchronises `stream`; SOPRO_ERR_INVALID if a run since the last check met a code outside [0, codebook_size). */
 int sopro_refprep_check(sopro_refprep_t* p, void* stream) {
   if (!p) return fail(SOPRO_ERR_INVALID, "null argument");
-  PCK(cudaSetDevice(p->device));
+  CK(cudaSetDevice(p->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int bad = 0;
-  PCK(cudaMemcpyAsync(&bad, p->bad, 4, cudaMemcpyDeviceToHost, st));
-  PCK(cudaStreamSynchronize(st));
+  CK(cudaMemcpyAsync(&bad, p->bad, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   if (bad) {
-    PCK(cudaMemsetAsync(p->bad, 0, 4, st));
+    CK(cudaMemsetAsync(p->bad, 0, 4, st));
     return fail(SOPRO_ERR_INVALID, "reference codes outside [0, %d)", p->cfg.codebook_size);
   }
   return SOPRO_OK;

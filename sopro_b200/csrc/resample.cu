@@ -13,17 +13,13 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <numeric>
 #include <vector>
 
 #include "../../include/sopro_b200.h"
-
-namespace mimi {
-void set_error(const char* msg);  // the library's per-thread error message (ar_engine.cu)
-}
+#include "common.cuh"
 
 namespace {
 
@@ -38,23 +34,6 @@ constexpr int kRowsPerLaunch = 256;      // rows of a ragged batch per launch (t
 constexpr int kMaxSmemBytes = 4 * (kInSmemFloats + kTabSmemFloats + 2 + 2 * kMaxReduced);
 constexpr double kPi = 3.141592653589793;
 
-int rfail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-
-#define RCK(call)                                                                                      \
-  do {                                                                                                 \
-    cudaError_t e__ = (call);                                                                          \
-    if (e__ != cudaSuccess)                                                                            \
-      return rfail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
 struct Geo {
   int o, n, width;  // reduced input / output rates, left context of a block's window
   int S;            // row stride of the tap table (the longest span)
@@ -68,10 +47,6 @@ struct Src {
   const float* a;
   const float* b;
   long long a_base, split, limit;
-};
-
-struct RowLens {
-  long long v[kRowsPerLaunch];
 };
 
 // rates -> (o, n, width), or a message on refusal.  Pure host arithmetic.
@@ -105,7 +80,7 @@ struct Filter {
 // torchaudio's _get_sinc_resample_kernel in double (same operation order), rounded to fp32, zeros trimmed per phase
 int make_filter(int32_t sr_in, int32_t sr_out, Filter* f) {
   char why[256];
-  if (!reduce_rates(sr_in, sr_out, &f->o, &f->n, &f->width, why, sizeof(why))) return rfail(SOPRO_ERR_INVALID, "%s", why);
+  if (!reduce_rates(sr_in, sr_out, &f->o, &f->n, &f->width, why, sizeof(why))) return fail(SOPRO_ERR_INVALID, "%s", why);
   const int o = f->o, n = f->n, width = f->width, full = 2 * width + o;
   const double base = std::min(o, n) * 0.99, scale = base / o;
   std::vector<std::vector<float>> rows(n);
@@ -130,7 +105,7 @@ int make_filter(int32_t sr_in, int32_t sr_out, Filter* f) {
         b = i;
       }
     }
-    if (a < 0) return rfail(SOPRO_ERR_INVALID, "phase %d of %d -> %d has no nonzero tap", p, sr_in, sr_out);
+    if (a < 0) return fail(SOPRO_ERR_INVALID, "phase %d of %d -> %d has no nonzero tap", p, sr_in, sr_out);
     f->first[p] = a;
     f->span[p] = b - a + 1;
     rows[p].assign(k.begin() + (a - lo), k.begin() + (b - lo + 1));
@@ -196,7 +171,7 @@ __device__ __forceinline__ void resample_tile(const Geo& g, const float* __restr
 
 // one-shot, ragged batch: grid (tiles of the longest row, rows); row b reads x[b][0, lens[b]) only
 __global__ void __launch_bounds__(kThreads) resample_batch_kernel(Geo g, const float* __restrict__ tab, const int2* __restrict__ meta,
-                                                                  const float* __restrict__ x, long long x_stride, RowLens lens,
+                                                                  const float* __restrict__ x, long long x_stride, RowLens<kRowsPerLaunch> lens,
                                                                   float* __restrict__ y, long long y_stride) {
   const int b = blockIdx.y;
   const long long len = lens.v[b];
@@ -242,7 +217,7 @@ int launch_stream(sopro_resampler_stream_t* s, const Src& src, long long j_begin
   if (j_end <= j_begin) return SOPRO_OK;
   const unsigned tiles = (unsigned)((j_end - j_begin + g.tile - 1) / g.tile);
   resample_stream_kernel<<<tiles, kThreads, s->r->smem, st>>>(g, s->r->tab, s->r->meta, src, j_begin, j_end, y);
-  RCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 }  // namespace
@@ -250,7 +225,7 @@ int launch_stream(sopro_resampler_stream_t* s, const Src& src, long long j_begin
 extern "C" {
 
 int sopro_resampler_filter(int32_t sr_in, int32_t sr_out, int32_t* geometry, int32_t* first, int32_t* span, float* taps) {
-  if (!geometry) return rfail(SOPRO_ERR_INVALID, "null argument");
+  if (!geometry) return fail(SOPRO_ERR_INVALID, "null argument");
   Filter f;
   const int rc = make_filter(sr_in, sr_out, &f);
   if (rc != SOPRO_OK) return rc;
@@ -272,19 +247,19 @@ int64_t sopro_resampled_length(int32_t sr_in, int32_t sr_out, int64_t n_in) {
 }
 
 int sopro_resampler_create(int32_t sr_in, int32_t sr_out, int device, sopro_resampler_t** out) {
-  if (!out) return rfail(SOPRO_ERR_INVALID, "null argument");
+  if (!out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
   Filter f;
   const int rc = make_filter(sr_in, sr_out, &f);  // refuses a rate before anything touches the device
   if (rc != SOPRO_OK) return rc;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
-    return rfail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the resampler has no CPU fallback");
-  if (device < 0 || device >= ndev) return rfail(SOPRO_ERR_INVALID, "device %d out of range", device);
+    return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the resampler has no CPU fallback");
+  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp prop;
-  RCK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return rfail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
-  RCK(cudaSetDevice(device));
+  CK(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  CK(cudaSetDevice(device));
   Geo g{f.o, f.n, f.width, f.S, 0, f.n * f.S <= kTabSmemFloats ? 1 : 0};
   for (int per = kMaxPerThread; per >= 1; per /= 2) {  // the largest tile whose input window fits the staging budget
     g.tile = per * kThreads;
@@ -306,7 +281,7 @@ int sopro_resampler_create(int32_t sr_in, int32_t sr_out, int device, sopro_resa
     cudaFree(r->tab);
     cudaFree(r->meta);
     delete r;
-    return rfail(SOPRO_ERR_CUDA, "resampler setup failed: %s", cudaGetErrorString(e));
+    return fail(SOPRO_ERR_CUDA, "resampler setup failed: %s", cudaGetErrorString(e));
   }
   *out = r;
   return SOPRO_OK;
@@ -323,36 +298,36 @@ int sopro_resampler_destroy(sopro_resampler_t* r) {
 
 int sopro_resample(sopro_resampler_t* r, const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, float* y,
                    int64_t y_stride, void* stream) {
-  if (!r || !x || !y) return rfail(SOPRO_ERR_INVALID, "null argument");
+  if (!r || !x || !y) return fail(SOPRO_ERR_INVALID, "null argument");
   const Geo& g = r->g;
-  if (B < 1 || x_stride < 0 || x_stride > (1LL << 40)) return rfail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
+  if (B < 1 || x_stride < 0 || x_stride > (1LL << 40)) return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
   long long most = 0;
   for (int b = 0; b < B; ++b) {
     const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride) return rfail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
+    if (len < 0 || len > x_stride) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
     most = std::max(most, out_len(g.o, g.n, len));
   }
-  if (B > 1 && y_stride < most) return rfail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld outputs", (long long)y_stride, most);
+  if (B > 1 && y_stride < most) return fail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld outputs", (long long)y_stride, most);
   if (most == 0) return SOPRO_OK;
-  RCK(cudaSetDevice(r->device));
+  CK(cudaSetDevice(r->device));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const unsigned tiles = (unsigned)((most + g.tile - 1) / g.tile);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens L{};
+    RowLens<kRowsPerLaunch> L{};
     for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
     resample_batch_kernel<<<dim3(tiles, rows), kThreads, r->smem, st>>>(g, r->tab, r->meta, x + (long long)b0 * x_stride, x_stride, L,
                                                                         y + (long long)b0 * y_stride, y_stride);
-    RCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }
 
 int sopro_resampler_stream_create(sopro_resampler_t* r, int64_t max_chunk, sopro_resampler_stream_t** out) {
-  if (!r || !out) return rfail(SOPRO_ERR_INVALID, "null argument");
+  if (!r || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (max_chunk < 1 || max_chunk > (1LL << 32)) return rfail(SOPRO_ERR_INVALID, "max_chunk must be in [1, 2^32]");
-  RCK(cudaSetDevice(r->device));
+  if (max_chunk < 1 || max_chunk > (1LL << 32)) return fail(SOPRO_ERR_INVALID, "max_chunk must be in [1, 2^32]");
+  CK(cudaSetDevice(r->device));
   sopro_resampler_stream* s = new sopro_resampler_stream();
   s->r = r;
   s->max_chunk = max_chunk;
@@ -362,7 +337,7 @@ int sopro_resampler_stream_create(sopro_resampler_t* r, int64_t max_chunk, sopro
   if (e != cudaSuccess) {
     cudaFree(s->carry[0]);
     delete s;
-    return rfail(SOPRO_ERR_CUDA, "resampler stream state: %s", cudaGetErrorString(e));
+    return fail(SOPRO_ERR_CUDA, "resampler stream state: %s", cudaGetErrorString(e));
   }
   *out = s;
   return SOPRO_OK;
@@ -378,7 +353,7 @@ int sopro_resampler_stream_destroy(sopro_resampler_stream_t* s) {
 }
 
 int sopro_resampler_stream_reset(sopro_resampler_stream_t* s) {
-  if (!s) return rfail(SOPRO_ERR_INVALID, "null argument");
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
   s->n_seen = s->q_done = 0;
   s->cur = 0;
   s->finished = false;
@@ -394,14 +369,14 @@ int64_t sopro_resampler_stream_ready(const sopro_resampler_stream_t* s, int64_t 
 }
 
 int sopro_resampler_push(sopro_resampler_stream_t* s, const float* x, int64_t n, float* y, void* stream) {
-  if (!s) return rfail(SOPRO_ERR_INVALID, "null argument");
-  if (s->finished) return rfail(SOPRO_ERR_STATE, "push after finish: reset the stream first");
-  if (n < 0 || n > s->max_chunk) return rfail(SOPRO_ERR_INVALID, "push of %lld samples: must be in [0, max_chunk = %lld]", (long long)n, s->max_chunk);
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (s->finished) return fail(SOPRO_ERR_STATE, "push after finish: reset the stream first");
+  if (n < 0 || n > s->max_chunk) return fail(SOPRO_ERR_INVALID, "push of %lld samples: must be in [0, max_chunk = %lld]", (long long)n, s->max_chunk);
   if (n == 0) return SOPRO_OK;
   const Geo& g = s->r->g;
   const long long n_seen = s->n_seen + n, q_done = blocks_ready(g, n_seen);
-  if (!x || (q_done > s->q_done && !y)) return rfail(SOPRO_ERR_INVALID, "null argument");
-  RCK(cudaSetDevice(s->r->device));
+  if (!x || (q_done > s->q_done && !y)) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(s->r->device));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long base = s->q_done * g.o - g.width;  // logical index of carry[cur][0]
   const Src src{s->carry[s->cur], x, base, s->n_seen, n_seen};
@@ -412,10 +387,10 @@ int sopro_resampler_push(sopro_resampler_stream_t* s, const float* x, int64_t n,
   float* dst = s->carry[s->cur ^ 1];
   long long k = nbase;
   if (k < s->n_seen) {
-    RCK(cudaMemcpyAsync(dst, s->carry[s->cur] + (k - base), (size_t)(s->n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst, s->carry[s->cur] + (k - base), (size_t)(s->n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
     k = s->n_seen;
   }
-  RCK(cudaMemcpyAsync(dst + (k - nbase), x + (k - s->n_seen), (size_t)(n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(dst + (k - nbase), x + (k - s->n_seen), (size_t)(n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
   s->cur ^= 1;
   s->n_seen = n_seen;
   s->q_done = q_done;
@@ -423,12 +398,12 @@ int sopro_resampler_push(sopro_resampler_stream_t* s, const float* x, int64_t n,
 }
 
 int sopro_resampler_finish(sopro_resampler_stream_t* s, float* y, void* stream) {
-  if (!s) return rfail(SOPRO_ERR_INVALID, "null argument");
-  if (s->finished) return rfail(SOPRO_ERR_STATE, "finish after finish: reset the stream first");
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (s->finished) return fail(SOPRO_ERR_STATE, "finish after finish: reset the stream first");
   const Geo& g = s->r->g;
   const long long j_end = out_len(g.o, g.n, s->n_seen), j_begin = (long long)g.n * s->q_done;
-  if (j_end > j_begin && !y) return rfail(SOPRO_ERR_INVALID, "null argument");
-  RCK(cudaSetDevice(s->r->device));
+  if (j_end > j_begin && !y) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(s->r->device));
   const Src src{s->carry[s->cur], nullptr, s->q_done * g.o - g.width, s->n_seen, s->n_seen};
   const int rc = launch_stream(s, src, j_begin, j_end, y, reinterpret_cast<cudaStream_t>(stream));
   if (rc != SOPRO_OK) return rc;

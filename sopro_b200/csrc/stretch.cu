@@ -18,16 +18,12 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <vector>
 
 #include "../../include/sopro_b200.h"
-
-namespace mimi {
-void set_error(const char* msg);  // the library's per-thread error message (ar_engine.cu)
-}
+#include "common.cuh"
 
 namespace {
 
@@ -45,23 +41,6 @@ static_assert(kN % kWarps == 0 && kCandPad >= kCand && kHs == kHalf, "geometry")
 static_assert(kCandPad - 1 + kN - 1 + 1 <= kWin, "the search's last register load stays in the window");
 constexpr double kPi = 3.141592653589793;
 
-int tfail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  mimi::set_error(buf);
-  return code;
-}
-
-#define TCK(call)                                                                                      \
-  do {                                                                                                 \
-    cudaError_t e__ = (call);                                                                          \
-    if (e__ != cudaSuccess)                                                                            \
-      return tfail(SOPRO_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
 // where the input sample at logical index i comes from: [0, split) from a (a[i - a_base]), [split, limit) from b
 // (b[i - split]), zero elsewhere -- the one-shot path has a single source, a stream its carried tail and the new chunk
 struct Src {
@@ -72,10 +51,6 @@ struct Src {
 
 struct Window {
   float w[kN];
-};
-
-struct RowLens {
-  long long v[kRowsPerLaunch];
 };
 
 // the stream's device-resident state between launches
@@ -246,7 +221,7 @@ __device__ void stretch_frames(const Src& src, int S, long long k_begin, long lo
 }
 
 // one-shot, ragged batch: one CTA per row; row b reads x[b][0, lens[b]) only
-__global__ void __launch_bounds__(kThreads, 1) stretch_batch_kernel(Window wp, const float* __restrict__ x, long long x_stride, RowLens lens,
+__global__ void __launch_bounds__(kThreads, 1) stretch_batch_kernel(Window wp, const float* __restrict__ x, long long x_stride, RowLens<kRowsPerLaunch> lens,
                                                                     int S, float* __restrict__ y, long long y_stride,
                                                                     int* __restrict__ offsets, long long k_stride) {
   const int b = blockIdx.x;
@@ -311,7 +286,7 @@ int launch_stream(sopro_stretch_stream* s, const Src& src, long long k_begin, lo
   if (k_end <= k_begin) return SOPRO_OK;
   static const Window wp = make_window();
   stretch_stream_kernel<<<1, kThreads, 0, st>>>(wp, src, s->S, k_begin, k_end, s->state, y, emitted(s), m_end);
-  TCK(cudaGetLastError());
+  CK(cudaGetLastError());
   return SOPRO_OK;
 }
 
@@ -321,9 +296,9 @@ bool valid_S(int32_t S) { return S >= kMinS && S <= kMaxS; }
 extern "C" {
 
 int sopro_stretch_speed(double speed, int32_t* S) {
-  if (!S) return tfail(SOPRO_ERR_INVALID, "null argument");
+  if (!S) return fail(SOPRO_ERR_INVALID, "null argument");
   if (!(speed >= 0.25 && speed <= 4.0))  // also refuses NaN
-    return tfail(SOPRO_ERR_INVALID, "speed must be a real number in [0.25, 4.0] (got %g)", speed);
+    return fail(SOPRO_ERR_INVALID, "speed must be a real number in [0.25, 4.0] (got %g)", speed);
   *S = (int32_t)std::nearbyint(speed * kOne);  // exact product (a power of two), rounded half to even
   return SOPRO_OK;
 }
@@ -342,7 +317,7 @@ int64_t sopro_stretch_positions(int32_t S, int64_t n_in, int64_t* a) {
 }
 
 int sopro_stretch_window(float* w) {
-  if (!w) return tfail(SOPRO_ERR_INVALID, "null argument");
+  if (!w) return fail(SOPRO_ERR_INVALID, "null argument");
   const Window wp = make_window();
   std::memcpy(w, wp.w, sizeof(wp.w));
   return SOPRO_OK;
@@ -350,41 +325,41 @@ int sopro_stretch_window(float* w) {
 
 int sopro_stretch(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t S, float* y, int64_t y_stride,
                   int32_t* offsets, void* stream) {
-  if (!x || !y) return tfail(SOPRO_ERR_INVALID, "null argument");
-  if (!valid_S(S)) return tfail(SOPRO_ERR_INVALID, "S = %d not in [%d, %d] (speed 0.25 .. 4 in 1/65536 steps)", S, kMinS, kMaxS);
+  if (!x || !y) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (!valid_S(S)) return fail(SOPRO_ERR_INVALID, "S = %d not in [%d, %d] (speed 0.25 .. 4 in 1/65536 steps)", S, kMinS, kMaxS);
   if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return tfail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
+    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
   long long most = 0;
   for (int b = 0; b < B; ++b) {
     const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride) return tfail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
+    if (len < 0 || len > x_stride) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
     most = std::max(most, out_len(S, len));
   }
-  if (B > 1 && y_stride < most) return tfail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld outputs", (long long)y_stride, most);
+  if (B > 1 && y_stride < most) return fail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld outputs", (long long)y_stride, most);
   if (most == 0) return SOPRO_OK;
   const long long k_max = n_frames(most);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   static const Window wp = make_window();
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens L{};
+    RowLens<kRowsPerLaunch> L{};
     for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
     stretch_batch_kernel<<<rows, kThreads, 0, st>>>(wp, x + (long long)b0 * x_stride, x_stride, L, S, y + (long long)b0 * y_stride,
                                                     y_stride, offsets ? offsets + (long long)b0 * k_max : nullptr, k_max);
-    TCK(cudaGetLastError());
+    CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }
 
 int sopro_stretch_stream_create(int64_t max_chunk, int device, sopro_stretch_stream_t** out) {
-  if (!out) return tfail(SOPRO_ERR_INVALID, "null argument");
+  if (!out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (max_chunk < 1 || max_chunk > (1LL << 32)) return tfail(SOPRO_ERR_INVALID, "max_chunk must be in [1, 2^32]");
+  if (max_chunk < 1 || max_chunk > (1LL << 32)) return fail(SOPRO_ERR_INVALID, "max_chunk must be in [1, 2^32]");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
-    return tfail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the time-stretch has no CPU fallback");
-  if (device < 0 || device >= ndev) return tfail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  TCK(cudaSetDevice(device));
+    return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the time-stretch has no CPU fallback");
+  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
+  CK(cudaSetDevice(device));
   sopro_stretch_stream* s = new sopro_stretch_stream();
   s->device = device;
   s->max_chunk = max_chunk;
@@ -395,7 +370,7 @@ int sopro_stretch_stream_create(int64_t max_chunk, int device, sopro_stretch_str
     cudaFree(s->carry[0]);
     cudaFree(s->carry[1]);
     delete s;
-    return tfail(SOPRO_ERR_CUDA, "stretch stream state: %s", cudaGetErrorString(e));
+    return fail(SOPRO_ERR_CUDA, "stretch stream state: %s", cudaGetErrorString(e));
   }
   *out = s;
   return SOPRO_OK;
@@ -412,8 +387,8 @@ int sopro_stretch_stream_destroy(sopro_stretch_stream_t* s) {
 }
 
 int sopro_stretch_stream_reset(sopro_stretch_stream_t* s, int32_t S) {
-  if (!s) return tfail(SOPRO_ERR_INVALID, "null argument");
-  if (!valid_S(S)) return tfail(SOPRO_ERR_INVALID, "S = %d not in [%d, %d]", S, kMinS, kMaxS);
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (!valid_S(S)) return fail(SOPRO_ERR_INVALID, "S = %d not in [%d, %d]", S, kMinS, kMaxS);
   s->S = S;
   s->n_seen = s->k_done = 0;
   s->cur = 0;
@@ -429,15 +404,15 @@ int64_t sopro_stretch_stream_ready(const sopro_stretch_stream_t* s, int64_t n_mo
 }
 
 int sopro_stretch_push(sopro_stretch_stream_t* s, const float* x, int64_t n, float* y, void* stream) {
-  if (!s) return tfail(SOPRO_ERR_INVALID, "null argument");
-  if (s->S == 0) return tfail(SOPRO_ERR_STATE, "push before reset: set the speed first");
-  if (s->finished) return tfail(SOPRO_ERR_STATE, "push after finish: reset the stream first");
-  if (n < 0 || n > s->max_chunk) return tfail(SOPRO_ERR_INVALID, "push of %lld samples: must be in [0, max_chunk = %lld]", (long long)n, s->max_chunk);
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (s->S == 0) return fail(SOPRO_ERR_STATE, "push before reset: set the speed first");
+  if (s->finished) return fail(SOPRO_ERR_STATE, "push after finish: reset the stream first");
+  if (n < 0 || n > s->max_chunk) return fail(SOPRO_ERR_INVALID, "push of %lld samples: must be in [0, max_chunk = %lld]", (long long)n, s->max_chunk);
   if (n == 0) return SOPRO_OK;
   const long long n_seen = s->n_seen + n, k_done = frames_ready(s->S, s->k_done, n_seen);
   const long long n_out = std::max(0LL, k_done - 1) * kHs - emitted(s);
-  if (!x || (n_out > 0 && !y)) return tfail(SOPRO_ERR_INVALID, "null argument");
-  TCK(cudaSetDevice(s->device));
+  if (!x || (n_out > 0 && !y)) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(s->device));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long base = tail_base(s->k_done, s->S);  // logical index of carry[cur][0]
   const Src src{s->carry[s->cur], x, base, s->n_seen, n_seen};
@@ -448,10 +423,10 @@ int sopro_stretch_push(sopro_stretch_stream_t* s, const float* x, int64_t n, flo
   float* dst = s->carry[s->cur ^ 1];
   long long k = nbase;
   if (k < s->n_seen) {
-    TCK(cudaMemcpyAsync(dst, s->carry[s->cur] + (k - base), (size_t)(s->n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst, s->carry[s->cur] + (k - base), (size_t)(s->n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
     k = s->n_seen;
   }
-  TCK(cudaMemcpyAsync(dst + (k - nbase), x + (k - s->n_seen), (size_t)(n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(dst + (k - nbase), x + (k - s->n_seen), (size_t)(n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
   s->cur ^= 1;
   s->n_seen = n_seen;
   s->k_done = k_done;
@@ -459,12 +434,12 @@ int sopro_stretch_push(sopro_stretch_stream_t* s, const float* x, int64_t n, flo
 }
 
 int sopro_stretch_finish(sopro_stretch_stream_t* s, float* y, void* stream) {
-  if (!s) return tfail(SOPRO_ERR_INVALID, "null argument");
-  if (s->S == 0) return tfail(SOPRO_ERR_STATE, "finish before reset: set the speed first");
-  if (s->finished) return tfail(SOPRO_ERR_STATE, "finish after finish: reset the stream first");
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (s->S == 0) return fail(SOPRO_ERR_STATE, "finish before reset: set the speed first");
+  if (s->finished) return fail(SOPRO_ERR_STATE, "finish after finish: reset the stream first");
   const long long M = out_len(s->S, s->n_seen), K = n_frames(M);
-  if (M > emitted(s) && !y) return tfail(SOPRO_ERR_INVALID, "null argument");
-  TCK(cudaSetDevice(s->device));
+  if (M > emitted(s) && !y) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(s->device));
   const Src src{s->carry[s->cur], nullptr, tail_base(s->k_done, s->S), s->n_seen, s->n_seen};
   const int rc = launch_stream(s, src, s->k_done, K, y, M, reinterpret_cast<cudaStream_t>(stream));
   if (rc != SOPRO_OK) return rc;

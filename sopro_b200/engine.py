@@ -44,10 +44,6 @@ def _f32(t: torch.Tensor) -> torch.Tensor:
     return t.detach().to(device="cpu", dtype=torch.float32).contiguous()
 
 
-def _stream_ptr(device: torch.device) -> int:
-    return int(torch.cuda.current_stream(device).cuda_stream)
-
-
 class ArEngine:
     def __init__(self, cfg: SoproTTSConfig, state_dict: Dict[str, torch.Tensor], device: Union[int, str, torch.device] = 0,
                  weight_dtype: str = "fp32"):
@@ -162,19 +158,19 @@ class ArSession:
         lens = (C.c_int32 * B)(*[int(x) for x in text_len])
         _lib.check(self.lib.sopro_ar_begin(
             self._h, B, steps, cond_ar.data_ptr(), txt_seq.data_ptr(), int(txt_seq.shape[1]), lens,
-            noise.data_ptr(), int(noise.shape[2]), arr, _stream_ptr(self.engine.device)))
+            noise.data_ptr(), int(noise.shape[2]), arr, _lib.stream_ptr(self.engine.device)))
         self.batch, self.steps = int(B), int(steps)
 
     def run(self, n_steps: Optional[int] = None) -> None:
         _lib.check(self.lib.sopro_ar_run(self._h, int(n_steps if n_steps is not None else self.steps),
-                                         _stream_ptr(self.engine.device)))
+                                         _lib.stream_ptr(self.engine.device)))
 
     def read(self):
         toks = np.zeros((self.batch, self.steps), dtype=np.int32)
         n = np.zeros((self.batch,), dtype=np.int32)
         done = np.zeros((self.batch,), dtype=np.int32)
         _lib.check(self.lib.sopro_ar_read(self._h, toks.ctypes.data, n.ctypes.data, done.ctypes.data,
-                                          _stream_ptr(self.engine.device)))
+                                          _lib.stream_ptr(self.engine.device)))
         return toks, n, done
 
     @property
@@ -201,7 +197,7 @@ class ArSession:
         n = np.zeros((B,), dtype=np.int32)
         _lib.check(self.lib.sopro_ar_generate_host(
             self._h, B, steps, pc, pt, int(stx[1]), lens, pn, int(sn[2]), arr, toks.ctypes.data, n.ctypes.data,
-            _stream_ptr(self.engine.device)))
+            _lib.stream_ptr(self.engine.device)))
         self.batch, self.steps = B, steps
         return toks, n
 
@@ -236,7 +232,7 @@ class ArSession:
 
     def sampled(self) -> torch.Tensor:
         out = torch.empty((self.batch, self.steps), dtype=torch.int32, device=self.engine.device)
-        _lib.check(self.lib.sopro_ar_debug_sampled(self._h, out.data_ptr(), _stream_ptr(self.engine.device)))
+        _lib.check(self.lib.sopro_ar_debug_sampled(self._h, out.data_ptr(), _lib.stream_ptr(self.engine.device)))
         return out
 
     def kv(self):
@@ -246,7 +242,7 @@ class ArSession:
         shape = (n_attn, self.batch, cfg.AR_HEADS, Lp, int(cfg.d_model) // cfg.AR_HEADS)
         ko = torch.empty(shape, dtype=torch.float32, device=self.engine.device)
         vo = torch.empty(shape, dtype=torch.float32, device=self.engine.device)
-        _lib.check(self.lib.sopro_ar_debug_kv(self._h, ko.data_ptr(), vo.data_ptr(), _stream_ptr(self.engine.device)))
+        _lib.check(self.lib.sopro_ar_debug_kv(self._h, ko.data_ptr(), vo.data_ptr(), _lib.stream_ptr(self.engine.device)))
         return ko, vo
 
     def close(self) -> None:

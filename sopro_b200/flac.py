@@ -20,19 +20,11 @@ BLOCK = 4096
 STREAM_MIN_BLOCK = 16
 
 
-def _check(rc: int) -> None:
-    """SOPRO_ERR_INVALID (a refused rate or geometry) is a ValueError; anything else a SoproError."""
-    if rc == -1:
-        msg = _lib.load().sopro_last_error()
-        raise ValueError(msg.decode() if msg else "invalid argument")
-    _lib.check(rc)
-
-
 def sizes(rows: int, max_len: int, sample_rate: int):
     """-> (workspace bytes, output bound in bytes) of one encode of `rows` rows of at most max_len samples.  Host only;
     ValueError for a refused rate or geometry."""
     ws, out = C.c_int64(0), C.c_int64(0)
-    _check(_lib.load().sopro_flac_sizes(int(rows), int(max_len), _rate(sample_rate), C.byref(ws), C.byref(out)))
+    _lib.check_arg(_lib.load().sopro_flac_sizes(int(rows), int(max_len), _rate(sample_rate), C.byref(ws), C.byref(out)))
     return int(ws.value), int(out.value)
 
 
@@ -60,10 +52,6 @@ def _to_host(dev: torch.Tensor, n: int):
     return host.numpy()[:n]
 
 
-def _stream_ptr(device: torch.device) -> int:
-    return int(torch.cuda.current_stream(device).cuda_stream)
-
-
 def encode_flac(wav: Union[torch.Tensor, Sequence[torch.Tensor]], sample_rate: int,
                 lens: Optional[Sequence[int]] = None) -> Union[bytes, List[bytes]]:
     """-> one FLAC stream (bytes) for a single row (any shape with one row of samples, e.g. [1, 1, N] or [N]), or a list
@@ -73,13 +61,9 @@ def encode_flac(wav: Union[torch.Tensor, Sequence[torch.Tensor]], sample_rate: i
     sr = _rate(sample_rate)
     single = isinstance(wav, torch.Tensor) and lens is None and (wav.dim() <= 1 or wav.shape[:-1].numel() == 1)
     if isinstance(wav, torch.Tensor):
-        x = _cuda(wav)
-        L = int(x.shape[-1]) if x.dim() else 1
-        B = int(x.shape[:-1].numel()) if x.dim() else 1
-        x = x.reshape(B, L).contiguous()
-        lv = [L] * B if lens is None else [int(v) for v in lens]
-        if len(lv) != B:
-            raise ValueError(f"lens has {len(lv)} entries for {B} rows")
+        x, _lead, lp = _lib.rows(wav.reshape(1) if wav.dim() == 0 else wav, lens, "FLAC encoding")
+        B, L = x.shape
+        lv = [L] * B if lp is None else list(lp)
     else:
         if lens is not None:
             raise ValueError("lens goes with a [B, L] tensor, not a list of rows")
@@ -101,8 +85,8 @@ def encode_flac(wav: Union[torch.Tensor, Sequence[torch.Tensor]], sample_rate: i
     out = torch.empty(max(out_n, 1), dtype=torch.uint8, device=dev)
     meta = torch.empty(2 * B, dtype=torch.int64, device=dev)  # row offsets, then row sizes
     with torch.cuda.device(dev):
-        _check(_lib.load().sopro_flac_encode(x.data_ptr(), B, L, (C.c_int64 * B)(*lv), sr, ws.data_ptr(), out.data_ptr(),
-                                             meta.data_ptr(), meta.data_ptr() + 8 * B, _stream_ptr(dev)))
+        _lib.check_arg(_lib.load().sopro_flac_encode(x.data_ptr(), B, L, (C.c_int64 * B)(*lv), sr, ws.data_ptr(), out.data_ptr(),
+                                                     meta.data_ptr(), meta.data_ptr() + 8 * B, _lib.stream_ptr(dev)))
         m = meta.cpu().tolist()
         total = m[B - 1] + m[2 * B - 1]
         blob = _to_host(out, total)
@@ -120,7 +104,7 @@ class FlacStreamEncoder:
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         h = _lib._VP()
         with torch.cuda.device(self.device):
-            _check(_lib.load().sopro_flac_stream_create(self.sample_rate, C.byref(h)))
+            _lib.check_arg(_lib.load().sopro_flac_stream_create(self.sample_rate, C.byref(h)))
         self._h = h
         self._nbytes = torch.zeros(1, dtype=torch.int64, device=self.device)
 
@@ -144,12 +128,12 @@ class FlacStreamEncoder:
         out = torch.empty(max(out_n, 1), dtype=torch.uint8, device=self.device)
         lib = _lib.load()
         with torch.cuda.device(self.device):
-            sp = _stream_ptr(self.device)
+            sp = _lib.stream_ptr(self.device)
             if x is None:
-                _check(lib.sopro_flac_stream_finish(self._h, ws.data_ptr(), out.data_ptr(), self._nbytes.data_ptr(), sp))
+                _lib.check_arg(lib.sopro_flac_stream_finish(self._h, ws.data_ptr(), out.data_ptr(), self._nbytes.data_ptr(), sp))
             else:
-                _check(lib.sopro_flac_stream_push(self._h, x.data_ptr(), n, ws.data_ptr(), out.data_ptr(),
-                                                  self._nbytes.data_ptr(), sp))
+                _lib.check_arg(lib.sopro_flac_stream_push(self._h, x.data_ptr(), n, ws.data_ptr(), out.data_ptr(),
+                                                          self._nbytes.data_ptr(), sp))
             return _to_host(out, int(self._nbytes.item())).tobytes()
 
     def push(self, chunk: torch.Tensor) -> bytes:

@@ -30,14 +30,6 @@ _TERMINATOR = re.compile("[.!?…]+[\"'”’)\\]]*")   # a maximal run of . ! ?
 _CLAUSE = re.compile("[,;:—–](?= )")                   # a clause mark followed by whitespace
 
 
-def _check(rc: int) -> None:
-    """SOPRO_ERR_INVALID (bad geometry) is a ValueError; anything else a SoproError."""
-    if rc == -1:
-        msg = _lib.load().sopro_last_error()
-        raise ValueError(msg.decode() if msg else "invalid argument")
-    _lib.check(rc)
-
-
 # ---- text segmentation (host)
 
 def _sentences(par: str) -> List[str]:
@@ -157,7 +149,7 @@ def fade_length(span: int) -> int:
 def fade_window(F: int) -> np.ndarray:
     """The F fp32 fade taps the join uses: 0.5 - 0.5 cos(pi (i + 0.5) / F) in double, rounded once.  Host only."""
     f = np.zeros(int(F), dtype=np.float32)
-    _check(_lib.load().sopro_longform_fade(int(F), f.ctypes.data if F else None))
+    _lib.check_arg(_lib.load().sopro_longform_fade(int(F), f.ctypes.data if F else None))
     return f
 
 
@@ -167,29 +159,17 @@ def joined_length(extents, pause: int) -> int:
     return sum(spans) + max(0, len(spans) - 1) * int(pause)
 
 
-def _stream_ptr(device: torch.device) -> int:
-    return int(torch.cuda.current_stream(device).cuda_stream)
-
-
 def speech_extents(wav: torch.Tensor, lens: Optional[Sequence[int]] = None) -> torch.Tensor:
     """wav [..., L] 24 kHz on a CUDA device (rows = the leading dims flattened) -> int64 [rows, 2] (start, end) of each
     row's speech, on the device (nothing synchronises).  `lens`: valid samples per row (a ragged batch); samples past
     lens[b] are not read."""
-    if wav.device.type != "cuda":
-        raise _lib.SoproError("speech extents need CUDA tensors; there is no CPU path")
-    L = int(wav.shape[-1])
-    B = math.prod(tuple(wav.shape[:-1]))
-    x = wav.detach().to(dtype=torch.float32).reshape(B, L).contiguous()
+    x, _lead, lp = _lib.rows(wav, lens, "speech extents")
+    B, L = x.shape
     ext = torch.empty((B, 2), dtype=torch.int64, device=x.device)
     if B == 0:
         return ext
-    lp = None
-    if lens is not None:
-        if len(lens) != B:
-            raise ValueError(f"lens has {len(lens)} entries for {B} rows")
-        lp = (C.c_int64 * B)(*[int(v) for v in lens])
     with torch.cuda.device(x.device):
-        _check(_lib.load().sopro_longform_extents(x.data_ptr(), B, L, lp, ext.data_ptr(), _stream_ptr(x.device)))
+        _lib.check_arg(_lib.load().sopro_longform_extents(x.data_ptr(), B, L, lp, ext.data_ptr(), _lib.stream_ptr(x.device)))
     return ext
 
 
@@ -227,6 +207,6 @@ def join_segments(rows_or_chunks: Union[torch.Tensor, Sequence[torch.Tensor]], e
     src = (C.c_void_p * n)(*[r.data_ptr() if r.numel() else None for r in rows])
     lens = (C.c_int64 * n)(*[int(r.numel()) for r in rows])
     with torch.cuda.device(dev):
-        _check(_lib.load().sopro_longform_join(src, n, lens, ext.ctypes.data, P, y.data_ptr() if N else None, N,
-                                               _stream_ptr(dev)))
+        _lib.check_arg(_lib.load().sopro_longform_join(src, n, lens, ext.ctypes.data, P, y.data_ptr() if N else None, N,
+                                                       _lib.stream_ptr(dev)))
     return y

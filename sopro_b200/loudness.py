@@ -8,8 +8,6 @@ synchronises with the host.  A target is a real number in [-60, 0] LUFS; ``check
 kernels are sopro_b200/csrc/loudness.cu, the contract is in include/sopro_b200.h."""
 from __future__ import annotations
 
-import ctypes as C
-import math
 import numbers
 from typing import Optional, Sequence, Tuple, Union
 
@@ -20,14 +18,6 @@ from . import _lib
 from .resample import _rate
 
 
-def _check(rc: int) -> None:
-    """SOPRO_ERR_INVALID (a refused target or rate) is a ValueError; anything else a SoproError."""
-    if rc == -1:
-        msg = _lib.load().sopro_last_error()
-        raise ValueError(msg.decode() if msg else "invalid argument")
-    _lib.check(rc)
-
-
 def check_loudness(target) -> Optional[float]:
     """None for None (no normalisation), else the target as a float; ValueError for anything but a real number in
     [-60, 0].  Host only, nothing allocated."""
@@ -35,7 +25,7 @@ def check_loudness(target) -> Optional[float]:
         return None
     if isinstance(target, (bool, np.bool_)) or not isinstance(target, numbers.Real):
         raise ValueError(f"loudness must be a real number in [-60, 0] LUFS, got {target!r}")
-    _check(_lib.load().sopro_loudness_target(float(target)))
+    _lib.check_arg(_lib.load().sopro_loudness_target(float(target)))
     return float(target)
 
 
@@ -43,7 +33,7 @@ def loudness_filter(sample_rate: int) -> Tuple[np.ndarray, np.ndarray, np.ndarra
     """The K-weighting biquads the kernels use at this rate, in float64: (b1, a1, b2, a2), each [3] with a[0] = 1.
     Host only."""
     c = np.zeros(10, dtype=np.float64)
-    _check(_lib.load().sopro_loudness_filter(_rate(sample_rate), c.ctypes.data))
+    _lib.check_arg(_lib.load().sopro_loudness_filter(_rate(sample_rate), c.ctypes.data))
     one = np.ones(1)
     return c[0:3].copy(), np.concatenate([one, c[3:5]]), c[5:8].copy(), np.concatenate([one, c[8:10]])
 
@@ -58,35 +48,24 @@ def workspace_bytes(rows: int, max_len: int, sample_rate: int) -> int:
 
 
 def _rows(wav: torch.Tensor, lens: Optional[Sequence[int]]):
-    if wav.device.type != "cuda":
-        raise _lib.SoproError("loudness metering needs CUDA tensors; there is no CPU path")
-    L = int(wav.shape[-1])
-    lead = tuple(wav.shape[:-1])
-    B = math.prod(lead)
-    x = wav.detach().to(dtype=torch.float32).reshape(B, L).contiguous()
-    if lens is None:
-        return x, lead, B, L, None, L
-    if len(lens) != B:
-        raise ValueError(f"lens has {len(lens)} entries for {B} rows")
-    lv = [int(v) for v in lens]
-    return x, lead, B, L, (C.c_int64 * B)(*lv), max(lv, default=0)
-
-
-def _stream_ptr(device: torch.device) -> int:
-    return int(torch.cuda.current_stream(device).cuda_stream)
+    """-> the rows (see _lib.rows) and the longest row's valid samples, which sizes the workspace."""
+    x, lead, lp = _lib.rows(wav, lens, "loudness metering")
+    most = int(x.shape[1]) if lp is None else max(lp, default=0)
+    return x, lead, lp, most
 
 
 def measure_loudness(wav: torch.Tensor, sample_rate: int, lens: Optional[Sequence[int]] = None) -> torch.Tensor:
     """wav [..., L] on a CUDA device (rows = the leading dims flattened) -> float64 [...] LUFS on the device, -inf for a
     row with no gated block.  `lens`: valid samples per row (a ragged batch); samples past lens[b] are not read."""
     sr = _rate(sample_rate)
-    x, lead, B, L, lp, most = _rows(wav, lens)
+    x, lead, lp, most = _rows(wav, lens)
+    B, L = x.shape
     lufs = torch.empty(B, dtype=torch.float64, device=x.device)
     if B:
         ws = torch.empty(workspace_bytes(B, most, sr), dtype=torch.uint8, device=x.device)
         with torch.cuda.device(x.device):
-            _check(_lib.load().sopro_loudness_measure(x.data_ptr(), B, L, lp, sr, ws.data_ptr(), lufs.data_ptr(),
-                                                      _stream_ptr(x.device)))
+            _lib.check_arg(_lib.load().sopro_loudness_measure(x.data_ptr(), B, L, lp, sr, ws.data_ptr(), lufs.data_ptr(),
+                                                              _lib.stream_ptr(x.device)))
     return lufs.reshape(lead)
 
 
@@ -100,14 +79,15 @@ def normalize_loudness(wav: torch.Tensor, sample_rate: int, target, lens: Option
     if T is None:
         raise ValueError("loudness target is None: there is nothing to normalise to")
     sr = _rate(sample_rate)
-    x, lead, B, L, lp, most = _rows(wav, lens)
-    y = torch.empty((B, L), dtype=torch.float32, device=x.device) if lp is None else torch.zeros((B, L), dtype=torch.float32,
-                                                                                                   device=x.device)
+    x, lead, lp, most = _rows(wav, lens)
+    B, L = x.shape
+    y = (torch.empty if lp is None else torch.zeros)((B, L), dtype=torch.float32, device=x.device)
     gain = torch.empty(B, dtype=torch.float32, device=x.device)
     if B:
         ws = torch.empty(workspace_bytes(B, most, sr), dtype=torch.uint8, device=x.device)
         with torch.cuda.device(x.device):
-            _check(_lib.load().sopro_loudness_normalize(x.data_ptr(), B, L, lp, sr, T, y.data_ptr(), L, ws.data_ptr(),
-                                                        None, gain.data_ptr(), _stream_ptr(x.device)))
+            _lib.check_arg(_lib.load().sopro_loudness_normalize(x.data_ptr(), B, L, lp, sr, T, y.data_ptr(), L,
+                                                                ws.data_ptr(), None, gain.data_ptr(),
+                                                                _lib.stream_ptr(x.device)))
     y = y.reshape(*lead, L)
     return (y, gain.reshape(lead)) if return_gain else y

@@ -21,15 +21,16 @@ import torch
 from . import longform as LF
 from . import prefill as P
 from . import timestamps as TS
+from ._lib import StatePool
 from .codec import MimiCodec
 from .config import TARGET_SR, SoproTTSConfig
 from .engine import ArEngine, ArSession, Sampling
 from .nar import NarEngine
 from .prefill_cuda import PrefillEngine, RefPrepEngine
 from .prefill import PreparedReference
-from .loudness import check_loudness, normalize_loudness
+from .output import OutputChain
 from .resample import Resampler, check_rates
-from .stretch import StretchPool, check_speed, stretch, stretched_length
+from .stretch import StretchStream
 from .weights import load_safetensors, read_safetensors_cfg
 
 
@@ -531,7 +532,8 @@ class SoproTTS:
         self.codec = codec
         self.device = torch.device(device)
         self._resamplers: Dict[int, Resampler] = {}  # output rate -> its resampler (tap table on the device)
-        self._stretch_pool = StretchPool(self.device)  # idle time-stretch stream states, shared by every speed
+        dev = self.device
+        self._stretch_pool = StatePool(lambda n, speed: StretchStream(n, dev, speed))  # idle time-stretch states, any speed
 
     # ---- construction
     @classmethod
@@ -611,10 +613,7 @@ class SoproTTS:
         ITU-R BS.1770-4 and scaled on the GPU under a -1 dBFS sample-peak ceiling (sopro_b200/loudness.py).
         `word_timestamps` (extension): also return when each word is spoken, ``(wav, List[WordTiming])``, from the AR
         step's text cross-attention (sopro_b200/timestamps.py); the audio is the same as without it."""
-        rs = self._resampler(sample_rate)  # a refused rate raises before any work
-        S = check_speed(speed)  # so does a refused speed
-        stretch_on = S is not None
-        target = check_loudness(loudness)  # and a refused loudness target
+        post = OutputChain(self, sample_rate, speed, loudness)  # a refused rate, speed or target raises before any work
         text_ids = self.encode_text(text)
         trace = spans = None
         if word_timestamps:
@@ -628,14 +627,8 @@ class SoproTTS:
             min_gen_frames=min_gen_frames, seed=seed, generator=generator, attn_trace=trace)
         words = None
         if word_timestamps:
-            words = self._timings([text], [spans], trace, [int(text_ids.numel())], [int(tokens_tq.shape[0])], S)[0]
-        wav = self.codec.decode_full(tokens_tq)
-        if stretch_on:
-            wav = stretch(wav, speed)
-        if rs is not None:
-            wav = rs(wav)
-        if target is not None:
-            wav = normalize_loudness(wav, TARGET_SR if rs is None else rs.sr_out, target)
+            words = self._timings([text], [spans], trace, [int(text_ids.numel())], [int(tokens_tq.shape[0])], post.S)[0]
+        wav, _ = post(self.codec.decode_full(tokens_tq))
         return (wav, words) if word_timestamps else wav
 
     @torch.inference_mode()
@@ -649,10 +642,7 @@ class SoproTTS:
         loudness-normalised, in one ragged launch when `speed` / `sample_rate` / `loudness` is given); utterance i equals
         synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness).
         `word_timestamps`: also return each utterance's word timings (see synthesize), ``(List[wav], List[List[WordTiming]])``."""
-        rs = self._resampler(sample_rate)
-        S = check_speed(speed)
-        stretch_on = S is not None
-        target = check_loudness(loudness)
+        post = OutputChain(self, sample_rate, speed, loudness)
         tr: Optional[dict] = {} if word_timestamps else None
         Ts, codes = self._batch_codes(texts, ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
                                       anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
@@ -660,18 +650,10 @@ class SoproTTS:
         words = None
         if word_timestamps:
             spans = [self.tokenizer.encode_with_offsets(t)[1] for t in texts]
-            words = self._timings(texts, spans, tr["probs"], tr["lens"], Ts, S)
+            words = self._timings(texts, spans, tr["probs"], tr["lens"], Ts, post.S)
         out: List[torch.Tensor] = [torch.zeros(1, 1, 0, device=self.device) for _ in texts]
         for chunk, wav, lens in self._decode_chunks(codes, Ts):
-            if stretch_on:
-                wav = stretch(wav.view(len(chunk), -1), speed, lens=lens).unsqueeze(1)
-                lens = [stretched_length(speed, n) for n in lens]
-            if rs is not None:
-                wav = rs(wav.view(len(chunk), -1), lens=lens).unsqueeze(1)
-                lens = [rs.length(n) for n in lens]
-            if target is not None:
-                wav = normalize_loudness(wav.view(len(chunk), -1), TARGET_SR if rs is None else rs.sr_out, target,
-                                         lens=lens).unsqueeze(1)
+            wav, lens = post(wav, lens)  # [rows, 1, L]: one ragged launch per stage
             for j, i in enumerate(chunk):
                 out[i] = wav[j: j + 1, :, : lens[j]].clone()
         return (out, words) if word_timestamps else out
@@ -692,10 +674,7 @@ class SoproTTS:
         level for the whole passage).  Segments that produced no frames are skipped; if none did, the result is
         [1, 1, 0].  Every argument is checked before any work.  `word_timestamps`: also return the passage's word timings
         (see synthesize), ``(wav, List[WordTiming])``, their char spans in `text`."""
-        rs = self._resampler(sample_rate)
-        S = check_speed(speed)
-        stretch_on = S is not None
-        target = check_loudness(loudness)
+        post = OutputChain(self, sample_rate, speed, loudness)
         LF.check_pause(pause_ms)
         budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
         segments = LF.split_text(text, self.tokenizer, budget)
@@ -727,15 +706,10 @@ class SoproTTS:
         if word_timestamps:
             spans = [self.tokenizer.encode_with_offsets(t)[1] for t in segments]
             words = TS.long_timings(text, segments, spans, firsts, all_Ts, self.codec.engine.hop, ext.cpu().numpy(),
-                                    LF.pause_samples(pause_ms), S)
+                                    LF.pause_samples(pause_ms), post.S)
         if wav.shape[-1] == 0:
             return (wav, words) if word_timestamps else wav
-        if stretch_on:
-            wav = stretch(wav, speed)
-        if rs is not None:
-            wav = rs(wav)
-        if target is not None:
-            wav = normalize_loudness(wav, TARGET_SR if rs is None else rs.sr_out, target)
+        wav, _ = post(wav)
         return (wav, words) if word_timestamps else wav
 
     def _timings(self, texts: Sequence[str], spans, probs: torch.Tensor, lens: Sequence[int], Ts: Sequence[int],

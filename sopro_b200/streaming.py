@@ -10,8 +10,8 @@ from typing import Iterator, List, Optional
 import torch
 
 from .codec import MimiDecodeState, MimiStreamDecoder
+from .output import OutputChain
 from .prefill import PreparedReference
-from .stretch import check_speed
 
 
 @dataclass
@@ -56,8 +56,7 @@ class SoproTTSStreamer:
         stream, right after its Mimi step, so the chunks concatenate to the one-shot stretch and resample of the 24 kHz
         stream bit for bit; the last chunk also carries both tails."""
         tts, model = self.tts, self.tts.model
-        rs = tts._resampler(sample_rate)  # a refused rate raises before the prefill
-        stretch_on = check_speed(speed) is not None  # so does a refused speed
+        post = OutputChain(tts, sample_rate, speed)  # a refused rate or speed raises before the prefill
         text_ids = tts.encode_text(text)
         if ref is None:
             ref = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
@@ -70,11 +69,8 @@ class SoproTTSStreamer:
         hist: List[int] = []
         emitted = 0
         state = self.mimi_stream.new_state()
-        # stretch / resampler states: their tails carry at most one frame's window / the filter window; pushes are
-        # bounded by one chunk's samples (a stretch push can yield up to 4x that, so the resampler pushes are split)
-        max_push = self.mimi_stream.max_chunk_frames * tts.codec.engine.hop
-        sstate = tts._stretch_pool.checkout(max_push, speed) if stretch_on else None
-        rstate = rs.checkout_stream(max_push) if rs is not None else None
+        # the stretch / resampler states' pushes are bounded by one chunk's samples
+        post_state = post.stream(self.mimi_stream.max_chunk_frames * tts.codec.engine.hop)
         on_gpu = tts.device.type == "cuda"
         main = torch.cuda.current_stream(tts.device) if on_gpu else None
         side = torch.cuda.Stream(tts.device) if on_gpu else None
@@ -91,16 +87,7 @@ class SoproTTSStreamer:
                 win = model.nar_refine(prep["cond_ar"][:, lo:end, :], toks).squeeze(0)
                 wav, state = self.mimi_stream.decode_step(win[emitted - lo:, :], state, _trusted=True)  # our own NAR's codes
                 emitted = end
-            if sstate is not None and (wav is not None or last):
-                parts = [sstate.push(wav[:, i: i + max_push]) for i in range(0, wav.shape[1], max_push)] if wav is not None else []
-                if last:
-                    parts.append(sstate.finish())
-                wav = torch.cat(parts).unsqueeze(0) if len(parts) > 1 else parts[0].unsqueeze(0)
-            if rstate is not None and (wav is not None or last):
-                parts = [rstate.push(wav[:, i: i + max_push]) for i in range(0, wav.shape[1], max_push)] if wav is not None else []
-                if last:
-                    parts.append(rstate.finish())
-                wav = torch.cat(parts).unsqueeze(0) if len(parts) > 1 else parts[0].unsqueeze(0)
+            wav = post_state.finish(wav) if last else post_state.push(wav)
             return wav if wav is not None and wav.numel() > 0 else None
 
         progress = {"consumed": 0}
@@ -137,18 +124,14 @@ class SoproTTSStreamer:
         finally:
             chunks.close()
             self.mimi_stream.release(state)
-            if sstate is not None:
-                tts._stretch_pool.release(sstate)
-            if rstate is not None:
-                rs.release_stream(rstate)
+            post_state.release()
 
 
 @torch.inference_mode()
 def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
            ref: Optional[PreparedReference] = None, chunk_frames: int = 6, sample_rate: Optional[int] = None,
            speed: Optional[float] = None, **kwargs) -> Iterator[torch.Tensor]:
-    tts._resampler(sample_rate)  # a refused rate or speed raises at the call, not at the first chunk
-    check_speed(speed)
+    OutputChain(tts, sample_rate, speed)  # a refused rate or speed raises at the call, not at the first chunk
     streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
     return streamer.stream(text, ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref=ref,
                            chunk_frames=chunk_frames, sample_rate=sample_rate, speed=speed, **kwargs)

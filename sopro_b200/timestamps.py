@@ -46,14 +46,6 @@ class WordTiming:
     char_end: int
 
 
-def _check(rc: int) -> None:
-    """SOPRO_ERR_INVALID (bad geometry) is a ValueError; anything else a SoproError."""
-    if rc == -1:
-        msg = _lib.load().sopro_last_error()
-        raise ValueError(msg.decode() if msg else "invalid argument")
-    _lib.check(rc)
-
-
 # ---- the device part
 
 def trace_buffer(cfg, steps: int, batch: int, ld: int, device) -> torch.Tensor:
@@ -74,14 +66,14 @@ def align(probs: torch.Tensor, text_len: Sequence[int], frames: Sequence[int]) -
         raise ValueError(f"{len(text_len)} text lengths and {len(frames)} frame counts for {B} utterances")
     lib = _lib.load()
     ws_bytes = C.c_int64()
-    _check(lib.sopro_align_sizes(B, steps, ld, C.byref(ws_bytes)))
+    _lib.check_arg(lib.sopro_align_sizes(B, steps, ld, C.byref(ws_bytes)))
     lens = (C.c_int32 * B)(*[int(v) for v in text_len])
     fr = (C.c_int32 * B)(*[int(v) for v in frames])
     ws = torch.empty(int(ws_bytes.value), dtype=torch.uint8, device=probs.device)
     first = torch.empty((B, ld), dtype=torch.int32, device=probs.device)
     with torch.cuda.device(probs.device):
-        _check(lib.sopro_align(probs.data_ptr(), steps, n_attn, B, H, ld, lens, fr, ws.data_ptr(), first.data_ptr(),
-                               int(torch.cuda.current_stream(probs.device).cuda_stream)))
+        _lib.check_arg(lib.sopro_align(probs.data_ptr(), steps, n_attn, B, H, ld, lens, fr, ws.data_ptr(), first.data_ptr(),
+                                       _lib.stream_ptr(probs.device)))
     return first
 
 

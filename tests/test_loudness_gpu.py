@@ -260,8 +260,8 @@ def test_synthesize_loudness_equals_normalize_of_synthesize(mode, target, speed,
         assert torch.equal(w, s)
 
 
-def test_no_loudness_makes_no_launch(monkeypatch):
-    import sopro_b200.model as model_mod
+def test_no_loudness_makes_no_launch_in_the_chain(monkeypatch):
+    import sopro_b200.output as output_mod
 
     tts, ref, text = _api()
     kw = dict(ref=ref, max_frames=16, min_gen_frames=10 ** 9)
@@ -272,7 +272,7 @@ def test_no_loudness_makes_no_launch(monkeypatch):
     def boom(*a, **k):
         raise AssertionError("the loudness stage ran without a target")
 
-    monkeypatch.setattr(model_mod, "normalize_loudness", boom)
+    monkeypatch.setattr(output_mod, "normalize_loudness", boom)
     assert torch.equal(tts.synthesize(text, seed=3, loudness=None, **kw), base)
     assert all(torch.equal(a, b) for a, b in zip(tts.synthesize_batch(texts, seeds=[1, 2], loudness=None, **kw), base_b))
     with pytest.raises(AssertionError):

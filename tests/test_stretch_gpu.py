@@ -324,9 +324,8 @@ def test_interleaved_and_abandoned_stretched_streams():
     assert len(again) == len(solo_a) and all(torch.equal(x, y) for x, y in zip(again, solo_a))
 
 
-def test_bypass_speeds_return_todays_outputs_without_a_launch(monkeypatch):
-    import sopro_b200.model as model_mod
-    from sopro_b200.stretch import StretchPool
+def test_bypass_speeds_return_todays_outputs_without_a_stretch_in_the_chain(monkeypatch):
+    import sopro_b200.output as output_mod
 
     tts, ref, text = _api()
     kw = dict(ref=ref, max_frames=16, min_gen_frames=10 ** 9)
@@ -338,8 +337,8 @@ def test_bypass_speeds_return_todays_outputs_without_a_launch(monkeypatch):
     def boom(*a, **k):
         raise AssertionError("the time-stretch ran on a bypass speed")
 
-    monkeypatch.setattr(model_mod, "stretch", boom)
-    monkeypatch.setattr(StretchPool, "checkout", boom)
+    monkeypatch.setattr(output_mod, "stretch", boom)
+    monkeypatch.setattr(tts._stretch_pool, "checkout", boom)
     for speed in (None, 1.0, 1, 1 + 0.4 / 65536):
         assert torch.equal(tts.synthesize(text, seed=3, speed=speed, **kw), base)
         assert all(torch.equal(a, b) for a, b in zip(tts.synthesize_batch(texts, seeds=[1, 2], speed=speed, **kw), base_b))

@@ -12,6 +12,7 @@ additionally accepts ``seed=`` / ``generator=`` (an extension) to leave the glob
 """
 from __future__ import annotations
 
+import contextlib
 import os
 import threading
 from typing import Dict, Iterator, List, Optional, Sequence, Tuple
@@ -30,6 +31,7 @@ from .prefill_cuda import PrefillEngine, RefPrepEngine
 from .prefill import PreparedReference
 from .output import OutputChain
 from .resample import Resampler, check_rates
+from .sampling import TapeFeed
 from .stretch import StretchStream
 from .weights import load_safetensors, read_safetensors_cfg
 
@@ -69,130 +71,19 @@ def _complete_state_dict(cfg: SoproTTSConfig, sd: Dict[str, torch.Tensor]) -> Di
     return out
 
 
-_TAPE_POOL = None
-
-
-def _tape_pool():
-    """Host threads that draw noise tapes (the Exp(1) draws release the GIL)."""
-    global _TAPE_POOL
-    if _TAPE_POOL is None:
-        from concurrent.futures import ThreadPoolExecutor
-
-        _TAPE_POOL = ThreadPoolExecutor(max_workers=max(1, len(os.sched_getaffinity(0))))
-    return _TAPE_POOL
-
-
-_NATIVE_NOISE = None
-
-
-def _native_noise_ok() -> bool:
-    """The host-side mt19937 tape generator of the library (csrc/noise_host.cu) is used for private generators when it
-    reproduces THIS torch build's CPU exponential_ bit for bit (checked once per process; a torch built with another
-    sampling kernel falls back to torch itself)."""
-    global _NATIVE_NOISE
-    if _NATIVE_NOISE is None:
-        try:
-            import ctypes as C
-
-            from . import _lib
-
-            lib = _lib.load()
-            h = C.c_void_p()
-            _lib.check(lib.sopro_noise_create(C.c_uint64(987654321), C.byref(h)))
-            got = torch.empty(3, 7)
-            _lib.check(lib.sopro_noise_rows(h, 3, 97, 7, got.data_ptr()))
-            lib.sopro_noise_destroy(h)
-            want = torch.empty(3, 97).exponential_(1.0, generator=torch.Generator().manual_seed(987654321))[:, :7]
-            _NATIVE_NOISE = bool(torch.equal(got, want))
-        except Exception:
-            _NATIVE_NOISE = False
-    return _NATIVE_NOISE
-
-
-class _Noise:
-    """The Exp(1) draws `steps` successive torch.multinomial calls would consume (see sopro_b200/sampling.py),
-    produced block by block as the kernel launches need them (a [n, V] draw equals n successive [V] draws), with
-    the bookkeeping needed to leave the generator exactly where the reference would leave it."""
-
-    def __init__(self, steps: int, vocab: int, seed: Optional[int], generator: Optional[torch.Generator]):
-        self.steps, self.vocab = int(steps), int(vocab)
-        self.private = seed is not None
-        self.gen = torch.Generator().manual_seed(int(seed)) if seed is not None else (generator or torch.default_generator)
-        self.marks: List[Tuple[int, torch.Tensor]] = []  # (first row of a block, generator state before it)
-        self.drawn = 0
-        self._native = None  # private generators: the library's host-side mt19937 (bit-equal to torch, skips unread draws)
-        if seed is not None and int(seed) >= 0 and _native_noise_ok():  # (negative seeds: torch's own remapping, torch's path)
-            import ctypes as C
-
-            from . import _lib
-
-            self._lib = _lib.load()
-            h = C.c_void_p()
-            _lib.check(self._lib.sopro_noise_create(C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), C.byref(h)))
-            self._native = h
-
-    def __del__(self):
-        if getattr(self, "_native", None) is not None:
-            self._lib.sopro_noise_destroy(self._native)
-            self._native = None
-
-    def rows_keep(self, upto: int, keep: int) -> torch.Tensor:
-        """Rows [drawn, upto), first `keep` columns -> [n, keep] (empty when already drawn)."""
-        upto = min(int(upto), self.steps)
-        n = upto - self.drawn
-        if n <= 0:
-            return torch.empty(0, int(keep))
-        if self._native is not None:
-            out = torch.empty(n, int(keep))
-            self.rows_into(upto, keep, out.numpy())
-            return out
-        return self.rows(upto)[:, : int(keep)]
-
-    def rows_into(self, upto: int, keep: int, out) -> None:
-        """Rows [drawn, upto), first `keep` columns, written into the float32 numpy array `out` [n, keep] (C-contiguous)."""
-        upto = min(int(upto), self.steps)
-        n = upto - self.drawn
-        if n <= 0:
-            return
-        if self._native is not None:
-            assert out.flags["C_CONTIGUOUS"] and out.shape == (n, keep)
-            from . import _lib
-
-            _lib.check(self._lib.sopro_noise_rows(self._native, n, self.vocab, int(keep), out.ctypes.data))
-            self.drawn = upto
-        else:
-            out[...] = self.rows(upto)[:, :keep].numpy()
-
-    def rows(self, upto: int) -> torch.Tensor:
-        """Draw rows [drawn, upto) -> [n, V] (empty when already drawn)."""
-        upto = min(int(upto), self.steps)
-        n = upto - self.drawn
-        if n <= 0:
-            return torch.empty(0, self.vocab)
-        if not self.private:
-            self.marks.append((self.drawn, self.gen.get_state()))
-        if self._native is not None:
-            out = torch.empty(n, self.vocab)
-            self.rows_into(upto, self.vocab, out.numpy())
-            return out
-        self.drawn = upto
-        return torch.empty(n, self.vocab).exponential_(1.0, generator=self.gen)
-
-    @property
-    def tape(self) -> torch.Tensor:
-        """All rows at once (only valid before any block has been drawn)."""
-        assert self.drawn == 0
-        return self.rows(self.steps)
-
-    def settle(self, steps_used: int) -> None:
-        """Rewind to the state after exactly `steps_used` draws (the reference stops drawing when it stops stepping)."""
-        if self.private or steps_used >= self.drawn:
-            return
-        start, state = [m for m in self.marks if m[0] <= steps_used][-1]
-        self.gen.set_state(state)
-        if steps_used > start:
-            torch.empty(int(steps_used - start), self.vocab).exponential_(1.0, generator=self.gen)
-        self.drawn = int(steps_used)
+def _growing_blocks(steps: int) -> List[Tuple[int, int]]:
+    """Block edges of a seeded batch: the host draws block k+1 of the tapes while the device generates block k, so
+    only the first, short block is exposed (and that one overlaps the prefill).  Block k+1 must be drawn faster than
+    the device generates block k: the host draws ~10 steps per ms (64 utterances, 16 threads), the kernel runs ~6
+    steps per ms -> blocks grow by 1.5x."""
+    edges, a, step = [], 0, 24
+    while a < steps:
+        b = min(steps, a + step)
+        if steps - b < 24:
+            b = steps
+        edges.append((a, b))
+        a, step = b, (step * 3) // 2
+    return edges
 
 
 class SoproModel:
@@ -228,30 +119,47 @@ class SoproModel:
     def eval(self):
         return self
 
-    def _checkout(self, batch: int, steps: int, text_len: int) -> ArSession:
-        """An idle session of this geometry (a fresh one when every cached one is in use); pair with _release."""
+    @contextlib.contextmanager
+    def _lease(self, batch: int, steps: int, text_len: int, attn_trace: Optional[torch.Tensor]) -> Iterator[ArSession]:
+        """An idle session of this geometry (a fresh one when every cached one is in use), held for the `with` block,
+        with `attn_trace` (word timestamps) set on it for that time: sessions are cached and shared."""
         key = (int(batch), int(steps), (int(text_len) + 63) // 64 * 64)
         with self._sessions_lock:
-            for ses in self._sessions.get(key, []):
-                if id(ses) not in self._sessions_busy:
-                    self._sessions_busy.add(id(ses))
-                    return ses
-            # evict idle sessions of other geometries beyond 8 cached (never one a live generator holds)
-            idle = [(k, x) for k, v in self._sessions.items() for x in v if id(x) not in self._sessions_busy and k != key]
-            total = sum(len(v) for v in self._sessions.values())
-            while total >= 8 and idle:
-                k, x = idle.pop(0)
-                self._sessions[k].remove(x)
-                x.close()
-                total -= 1
-            ses = self.engine.session(*key)
-            self._sessions.setdefault(key, []).append(ses)
+            ses = next((x for x in self._sessions.get(key, []) if id(x) not in self._sessions_busy), None)
+            if ses is None:
+                # evict idle sessions of other geometries beyond 8 cached (never one a live generator holds)
+                idle = [(k, x) for k, v in self._sessions.items() for x in v if id(x) not in self._sessions_busy and k != key]
+                total = sum(len(v) for v in self._sessions.values())
+                while total >= 8 and idle:
+                    k, x = idle.pop(0)
+                    self._sessions[k].remove(x)
+                    x.close()
+                    total -= 1
+                ses = self.engine.session(*key)
+                self._sessions.setdefault(key, []).append(ses)
             self._sessions_busy.add(id(ses))
-            return ses
+        try:
+            if attn_trace is not None:
+                ses.set_attn_trace(attn_trace)
+            yield ses
+        finally:
+            if attn_trace is not None:
+                ses.set_attn_trace(None)
+            with self._sessions_lock:
+                self._sessions_busy.discard(id(ses))
 
-    def _release(self, ses: ArSession) -> None:
-        with self._sessions_lock:
-            self._sessions_busy.discard(id(ses))
+    @staticmethod
+    def _launch_blocks(ses: ArSession, feed: TapeFeed, edges: Sequence[Tuple[int, int]], cond: torch.Tensor,
+                       txt: torch.Tensor, lens: Sequence[int], samp: Sampling) -> Iterator[int]:
+        """Runs the session block by block, (a, b) edges: each block's noise rows are drawn and queued for upload just
+        before its launch.  The session is begun before the first block is drawn, so that the device work of `begin`
+        (state resets, the text K/V) runs while the host draws.  Yields each block's end once it is enqueued."""
+        for a, b in edges:
+            if a == 0:
+                ses.begin(cond, txt, lens, feed.dev, samp)
+            feed.fill(b)
+            ses.run(b - a)
+            yield b
 
     # ---- prefill
     @torch.no_grad()
@@ -331,54 +239,35 @@ class SoproModel:
         if cond.size(1) < steps:
             raise ValueError(f"cond_ar has {cond.size(1)} rows, need max_frames+1 = {steps}")
         L = int(txt.size(1))
-        noise = _Noise(steps, self.cfg.ar_vocab(), seed, generator)
         samp = self._sampling(top_p, temperature, anti_loop, loop_streak, recovery_top_p, recovery_temp, min_gen_frames, False)
-        nk = self._noise_cols(samp)
-        ses = self._checkout(1, steps, L)
         per = steps if chunk_frames <= 0 else int(chunk_frames)
         st = {"launched": 0, "read": 0, "yielded": 0}
+        with TapeFeed(1, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device,
+                      None if seed is None else [seed], generator) as feed, self._lease(1, steps, L, attn_trace) as ses:
+            launches = self._launch_blocks(ses, feed, [(a, min(steps, a + per)) for a in range(0, steps, per)],
+                                           cond[:, :steps], txt, [L], samp)
 
-        def launch():
-            """Draw + upload the noise rows of the next launch and enqueue it (no-op while one is in flight)."""
-            if st["launched"] >= steps or st["launched"] > st["read"]:
-                return
-            lo = noise.drawn
-            blk = noise.rows_keep(st["launched"] + per, nk)
-            if blk.size(0):
-                n_new = int(blk.size(0))
-                if stage is not None:  # pinned staging rows: the upload is asynchronous, ordered before the launch on this stream
-                    stage[lo: lo + n_new].copy_(blk)
-                    tape[0, lo: lo + n_new].copy_(stage[lo: lo + n_new], non_blocking=True)
-                else:
-                    tape[0, lo: lo + n_new].copy_(blk)
-            ses.run(per)
-            st["launched"] = min(steps, st["launched"] + per)
+            def launch():
+                """Enqueue the next launch (no-op while one is in flight)."""
+                if st["launched"] < steps and st["launched"] <= st["read"]:
+                    st["launched"] = next(launches)
 
-        try:
-            # the session keeps a pointer to this device tape; each launch's rows are drawn and uploaded just before it
-            tape = torch.zeros(1, steps, nk, device=self.device)
-            stage = torch.empty(steps, nk, pin_memory=True) if self.device.type == "cuda" else None
-            if attn_trace is not None:
-                ses.set_attn_trace(attn_trace)
-            ses.begin(cond[:, :steps], txt, [L], tape, samp)
-            t = 0
-            while t < steps:
-                launch()
-                toks, n, done = ses.read()  # synchronises the stream the launch ran on
-                upto = int(n[0])
-                st["read"] = st["launched"]
-                chunk = [int(x) for x in toks[0, t:upto]]
-                finished = bool(done[0]) or upto >= steps or upto < st["launched"]
-                t = upto
-                st["yielded"] = upto
-                yield chunk, finished, (launch if not finished else (lambda: None))
-                if finished:
-                    break
-        finally:
-            if attn_trace is not None:
-                ses.set_attn_trace(None)  # sessions are cached and shared
-            self._release(ses)
-            noise.settle(int(progress["consumed"]) if progress is not None and "consumed" in progress else st["yielded"])
+            try:
+                t = 0
+                while t < steps:
+                    launch()
+                    toks, n, done = ses.read()  # synchronises the stream the launch ran on
+                    upto = int(n[0])
+                    st["read"] = st["launched"]
+                    chunk = [int(x) for x in toks[0, t:upto]]
+                    finished = bool(done[0]) or upto >= steps or upto < st["launched"]
+                    t = upto
+                    st["yielded"] = upto
+                    yield chunk, finished, (launch if not finished else (lambda: None))
+                    if finished:
+                        break
+            finally:
+                feed.settle(int(progress["consumed"]) if progress is not None and "consumed" in progress else st["yielded"])
 
     @torch.no_grad()
     def ar_stream(self, prep: Dict[str, torch.Tensor], *, max_frames: int, top_p: float = 0.9, temperature: float = 1.05,
@@ -404,103 +293,25 @@ class SoproModel:
         finally:
             gen.close()
 
-    def _draw_tapes(self, B: int, steps: int, nk: int, seeds: Optional[Sequence[int]]) -> torch.Tensor:
-        """[B, steps, nk] Exp(1) draws: utterance i's rows are what `steps` multinomial calls consume after
-        torch.manual_seed(seeds[i]) (private generators, drawn on host threads -- the draws release the GIL); without
-        seeds the global generator is consumed utterance after utterance, full length each."""
-        V = self.cfg.ar_vocab()
-        out = torch.empty((B, steps, nk), dtype=torch.float32, pin_memory=torch.cuda.is_available())
-        if seeds is None:
-            for i in range(B):
-                out[i] = _Noise(steps, V, None, None).tape[:, :nk]
-            return out
-        from concurrent.futures import ThreadPoolExecutor
-
-        view = out.numpy()  # worker threads are outside the caller's inference_mode: write through numpy
-
-        def one(i):
-            _Noise(steps, V, int(seeds[i]), None).rows_into(steps, nk, view[i])
-
-        with ThreadPoolExecutor(max_workers=min(B, max(1, len(os.sched_getaffinity(0))))) as ex:
-            list(ex.map(one, range(B)))
-        return out
-
     @torch.no_grad()
     def ar_generate_tensors(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int, top_p: float = 0.9,
                             temperature: float = 1.05, anti_loop: bool = True, min_gen_frames: Optional[int] = None,
                             seeds: Optional[Sequence[int]] = None, stop_on_first_eos: bool = True,
                             attn_trace: Optional[torch.Tensor] = None):
-        """B utterances in ONE persistent launch from batch tensors (cond [B, >=steps, D], txt [B, Lmax, D], lens).
-        -> (tokens [B, steps] int32 numpy, n_tokens [B]).  `attn_trace` (word timestamps): a [steps, n_attn, B, H, ld]
-        buffer, ld >= max(lens), that receives the text cross-attention weights."""
+        """B utterances in ONE persistent kernel run from batch tensors (cond [B, >=steps, D], txt [B, Lmax, D], lens).
+        -> (tokens [B, steps] int32 numpy, n_tokens [B]).  With `seeds` and at least 64 steps the run is launched in
+        growing blocks (the kernel resumes from its device state), each block's tapes drawn on host threads while the
+        device generates the block before; otherwise in one launch.  `attn_trace` (word timestamps): a
+        [steps, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text cross-attention weights."""
         B, steps = int(cond.shape[0]), int(max_frames) + 1
         samp = self._sampling(top_p, temperature, anti_loop, 8, 0.85, 1.2, min_gen_frames, stop_on_first_eos)
-        nk = self._noise_cols(samp)
-        ses = self._checkout(B, steps, max(int(x) for x in lens))
-        try:
-            if attn_trace is not None:
-                ses.set_attn_trace(attn_trace)
-            if seeds is None or steps < 64:
-                tapes = self._draw_tapes(B, steps, nk, seeds)  # host threads; the prefill kernels queued before run meanwhile
-                ses.begin(cond[:, :steps], txt, [int(x) for x in lens], tapes.to(self.device, non_blocking=True), samp)
-                ses.run()
-            else:
-                # Private generators: the tape is drawn in growing blocks of steps and the persistent kernel is launched
-                # block by block (it resumes from its device state), so the host draws block k+1 while the device
-                # generates block k; only the first, short block is exposed (and that one overlaps the prefill).
-                V = self.cfg.ar_vocab()
-                gens = [_Noise(steps, V, int(seeds[i]), None) for i in range(B)]
-                host = torch.empty((B, steps, nk), dtype=torch.float32, pin_memory=torch.cuda.is_available())
-                view = host.numpy()
-                dev = torch.empty((B, steps, nk), dtype=torch.float32, device=self.device)
-                pool = _tape_pool()
-
-                def draw(a: int, b: int) -> None:
-                    def one(i):
-                        gens[i].rows_into(b, nk, view[i, a:b])
-                    list(pool.map(one, range(B)))
-                    dev[:, a:b].copy_(host[:, a:b], non_blocking=True)
-
-                # block k+1 must be drawn faster than the device generates block k: the host draws ~10 steps per ms
-                # (64 utterances, 16 threads), the kernel runs ~6 steps per ms -> blocks grow by 1.5x
-                edges, a, step = [], 0, 24
-                while a < steps:
-                    b = min(steps, a + step)
-                    if steps - b < 24:
-                        b = steps
-                    edges.append((a, b))
-                    a, step = b, (step * 3) // 2
-                draw(*edges[0])
-                ses.begin(cond[:, :steps], txt, [int(x) for x in lens], dev, samp)
-                ses.run(edges[0][1])
-                for a, b in edges[1:]:
-                    draw(a, b)
-                    ses.run(b - a)
+        edges = _growing_blocks(steps) if seeds is not None and steps >= 64 else [(0, steps)]
+        with TapeFeed(B, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device, seeds) as feed, \
+                self._lease(B, steps, max(int(x) for x in lens), attn_trace) as ses:
+            for _ in self._launch_blocks(ses, feed, edges, cond[:, :steps], txt, [int(x) for x in lens], samp):
+                pass
             toks, n, _ = ses.read()
-        finally:
-            if attn_trace is not None:
-                ses.set_attn_trace(None)  # sessions are cached and shared
-            self._release(ses)
         return toks, n
-
-    @torch.no_grad()
-    def ar_generate_batch(self, preps: Sequence[Dict[str, torch.Tensor]], *, max_frames: int, top_p: float = 0.9,
-                          temperature: float = 1.05, anti_loop: bool = True, min_gen_frames: Optional[int] = None,
-                          seeds: Optional[Sequence[int]] = None, stop_on_first_eos: bool = True) -> List[List[int]]:
-        """NEW capability (the reference is batch-1): B independent utterances in ONE persistent launch.  Utterance i
-        equals the reference run alone with seed seeds[i] (SURVEY.md §0.3).  Without seeds the global generator is
-        consumed utterance after utterance, full length each."""
-        B, steps = len(preps), int(max_frames) + 1
-        D = int(self.cfg.d_model)
-        lens = [int(p["txt_seq"].size(1)) for p in preps]
-        cond = torch.stack([p["cond_ar"][0, :steps] for p in preps])
-        txt = torch.zeros(B, max(lens), D, device=self.device)
-        for i, p in enumerate(preps):
-            txt[i, : lens[i]] = p["txt_seq"][0]
-        toks, n = self.ar_generate_tensors(cond, txt, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                           anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds,
-                                           stop_on_first_eos=stop_on_first_eos)
-        return [toks[i, : n[i]].tolist() for i in range(B)]
 
     @torch.no_grad()
     def generate_tokens(self, text_ids_1d: torch.Tensor, ref: PreparedReference, *, max_frames: int, device=None,

@@ -118,6 +118,22 @@ def test_batch_synthesis_equals_single():
         assert torch.equal(single, w)
 
 
+def test_batch_synthesis_equals_single_across_noise_blocks():
+    """At 101 steps a seeded batch draws its tapes and launches in blocks of 24, 36 and 41 frames (synthesize runs one
+    launch); each utterance still equals synthesize(text, seed=s) bit for bit."""
+    tts, _ = _tts()
+    cfg, sd, inp = e2e_inputs()
+    ref = tts.prepare_reference(ref_tokens_tq=inp["ref_tokens_tq"])
+    texts = [TEXT, " ".join(str(i) for i in range(3, 40, 3)), "5 9", " ".join(str(11 * i + 2) for i in range(30))]
+    seeds = [1, 2, 3, 4]
+    wavs = tts.synthesize_batch(texts, ref=ref, max_frames=100, seeds=seeds)
+    frames = [w.shape[-1] // 1920 for w in wavs]
+    assert max(frames) > 24, f"no utterance ran past the first block: {frames}"
+    for t, s, w in zip(texts, seeds, wavs):
+        single = tts.synthesize(t, ref=ref, max_frames=100, seed=s)
+        assert torch.equal(single, w)
+
+
 def test_prepared_reference_roundtrips_through_torch_save():
     tts, _ = _tts()
     cfg, sd, inp = e2e_inputs()

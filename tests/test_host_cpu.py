@@ -122,20 +122,22 @@ def test_wav_roundtrip(tmp_path):
     assert sr * 0.9 < trimmed.shape[-1] < wav.numel()
 
 
-def test_noise_blocks_equal_one_tape_and_settle_rewinds():
+def test_noise_tape_blocks_equal_one_tape_and_settle_rewinds():
     """ar_stream draws the sampler's Exp(1) rows launch by launch: the blocks must concatenate to the one-shot tape
     (== what `steps` multinomial calls consume) and settle() must leave the global generator after exactly the
     consumed rows."""
-    from sopro_b200.model import _Noise
+    from sopro_b200.sampling import NoiseTape
 
     V = 2049
     torch.manual_seed(3)
     full = torch.empty(20, V).exponential_(1.0)
     after_full = torch.get_rng_state()
     torch.manual_seed(3)
-    n = _Noise(20, V, None, None)
-    got = torch.cat([n.rows(up) for up in (6, 12, 18, 24)])
-    assert torch.equal(got, full) and torch.equal(torch.get_rng_state(), after_full)
+    n = NoiseTape(20, V, V)
+    got = np.zeros((20, V), dtype=np.float32)
+    for up in (6, 12, 18, 24):
+        n.draw(up, got)
+    assert torch.equal(torch.from_numpy(got), full) and torch.equal(torch.get_rng_state(), after_full)
     n.settle(8)
     state = torch.get_rng_state()
     torch.manual_seed(3)
@@ -143,8 +145,11 @@ def test_noise_blocks_equal_one_tape_and_settle_rewinds():
     assert torch.equal(state, torch.get_rng_state())
     # a private seed never touches the global generator
     before = torch.get_rng_state()
-    p = _Noise(5, V, 11, None)
-    assert torch.equal(p.tape, torch.empty(5, V).exponential_(1.0, generator=torch.Generator().manual_seed(11)))
+    p = NoiseTape(5, V, V, seed=11)
+    tape = np.zeros((5, V), dtype=np.float32)
+    p.draw(5, tape)
+    p.close()
+    assert torch.equal(torch.from_numpy(tape), torch.empty(5, V).exponential_(1.0, generator=torch.Generator().manual_seed(11)))
     assert torch.equal(before, torch.get_rng_state())
 
 
@@ -180,14 +185,14 @@ def test_missing_checkpoint_tensors_get_reference_defaults_or_one_clear_error():
     assert "ar.head.weight" in str(ei.value) and "cond_norm.weight" in str(ei.value)
 
 
-def test_native_noise_tape_is_bit_equal_to_torch_and_skips_the_unread_draws():
+def test_native_noise_tape_draws_are_bit_equal_to_torch_and_skip_the_unread_draws():
     """csrc/noise_host.cu (host-side mt19937 + ATen's uniform -> -log1p(-u) transform) against this torch build's CPU
     exponential_: same bits for private generators, also when only the first `keep` columns of each row are materialised
-    and across blocks of rows; the Python _Noise wrapper uses it only after this check (model._native_noise_ok)."""
+    and across blocks of rows; the Python NoiseTape wrapper uses it only after this check (sampling._native_noise_ok)."""
     import ctypes as C
 
     from sopro_b200 import _lib
-    from sopro_b200.model import _Noise, _native_noise_ok
+    from sopro_b200.sampling import NoiseTape, _native_noise_ok
 
     lib = _lib.load()
     for seed in (0, 1, 1234, 2 ** 31 + 7, 2 ** 40 + 3):
@@ -201,10 +206,14 @@ def test_native_noise_tape_is_bit_equal_to_torch_and_skips_the_unread_draws():
             assert torch.equal(got, want), (seed, n, V, keep)
         lib.sopro_noise_destroy(h)
     assert _native_noise_ok()
-    a = _Noise(40, 2049, 77, None)
-    first, second = a.rows_keep(13, 50), a.rows_keep(40, 50)
+    a = NoiseTape(40, 2049, 50, seed=77)
+    assert a._native is not None  # a private seed >= 0 draws through the library
+    got = np.zeros((40, 50), dtype=np.float32)
+    a.draw(13, got)
+    a.draw(40, got)
+    a.close()
     ref = torch.empty(40, 2049).exponential_(1.0, generator=torch.Generator().manual_seed(77))[:, :50]
-    assert torch.equal(torch.cat([first, second]), ref)
+    assert torch.equal(torch.from_numpy(got), ref)
 
 
 def test_ctypes_mirrors_match_the_header_layout(tmp_path):

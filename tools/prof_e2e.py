@@ -83,7 +83,12 @@ with torch.inference_mode():
     ids64 = [tts.encode_text(x) for x in texts]
     t, preps = timed(lambda: tts.model.prepare_conditioning_batch(ids64, ref, max_frames=400, style_strength=cfg.style_strength), n=3, warm=1)
     print(f"prefill batch 64       {t:8.3f} ms")
-    t, tapes = timed(lambda: tts.model._draw_tapes(64, 401, 50, list(range(64))), n=3, warm=1)
-    print(f"draw 64 noise tapes    {t:8.3f} ms")
+    from sopro_b200.sampling import TapeFeed
+
+    def draw_tapes():
+        with TapeFeed(64, 401, cfg.ar_vocab(), 50, dev, list(range(64))) as feed:
+            feed.fill(401)
+    t, _ = timed(draw_tapes, n=3, warm=1)
+    print(f"draw+upload 64 tapes   {t:8.3f} ms")
     t, _ = timed(lambda: tts.synthesize_batch(texts, ref=ref, max_frames=400, seeds=list(range(64)), min_gen_frames=10 ** 9), n=3, warm=1)
     print(f"synthesize_batch(64)   {t:8.3f} ms")

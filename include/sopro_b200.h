@@ -560,6 +560,13 @@ int sopro_refprep_destroy(sopro_refprep_t* p);
  * pointers, each [H, Tr, D/H] (PreparedReference.ref_kv_caches[i]["k"/"v"], model.py:45-50). */
 int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* sv, float* ref_seq, float* const* ref_k,
                       float* const* ref_v, void* stream);
+/* Token2SV alone over a ragged batch (best-of-N synthesis scores its takes with it): B code sequences -> B unit speaker
+ * vectors, and optionally their cosine with one reference vector.  tokens: device int32 [B][Tmax][Q]; lens_host: B ints
+ * in [1, Tmax], Tmax <= 4096; sv: device f32 [B][sv_dim]; ref_sv: device f32 [sv_dim] or NULL; cos: device f32 [B]
+ * (written only when ref_sv is given).  Row b equals, bit for bit, the sv sopro_refprep_run gives for its lens_host[b]
+ * frames alone.  Codes outside [0, codebook_size) are reported by sopro_refprep_check. */
+int sopro_refprep_speaker_vectors(sopro_refprep_t* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host,
+                                  float* sv, const float* ref_sv, float* cos, void* stream);
 /* synchronises `stream`; SOPRO_ERR_INVALID if a run since the last check met a code outside [0, codebook_size) (the
  * reference's embedding lookup raises IndexError); clears the flag */
 int sopro_refprep_check(sopro_refprep_t* p, void* stream);

@@ -6,7 +6,8 @@
 //
 //   dense_tile_kernel    C[M][N] = epi(prologue(A)[M][K] . W[N][K]^T): 128x128x16 tiles, 8x8 outputs per thread
 //   dense_skinny_kernel  the same contract for M <= 16 rows (streaming windows, time-to-first-audio): the rows
-//                        live in shared memory, one warp per output column, lanes split K
+//                        live in shared memory, one warp per output column, lanes split K; more rows in blocks of 16
+//                        (grid.y), where a row's reduction order must not depend on M (Token2SV of a batch)
 //   prologue             optional RMSNorm of the A rows (nn/blocks.py:32-37) and/or a vector added to every row
 //   epilogues            bias | bias+GELU(erf) | bias+residual | GLU (value . sigmoid(gate), nn/blocks.py:16-23) |
 //                        argmax partials (value desc, index asc == torch.argmax's first maximum)
@@ -321,7 +322,16 @@ __device__ __forceinline__ float reduce_transposed(float (&v)[N], int lane) {
 }
 
 __global__ void __launch_bounds__(kSkinnyThreads) dense_skinny_kernel(const DenseOp op_in, int cols_per_cta) {
-  const DenseOp op = group_of(op_in);
+  DenseOp op = group_of(op_in);
+  // more than 16 rows (never with the argmax epilogue): blockIdx.y = block of 16 rows, each row computed exactly as in
+  // a launch of its own
+  if (blockIdx.y) {
+    const size_t r0 = (size_t)blockIdx.y * kSkinnyRows;
+    op.A += r0 * op.K;
+    op.C += r0 * op.ldc;
+    if (op.R) op.R += r0 * op.ldc;
+    op.M -= (int)r0;
+  }
   extern __shared__ __align__(16) float xs[];  // [16][K]
   __shared__ float s_best_v[kSkinnyThreads / 32][kSkinnyRows];
   __shared__ int s_best_i[kSkinnyThreads / 32][kSkinnyRows];

@@ -64,13 +64,16 @@ int tile_edge(int M, int N, int groups, int epi) {
 }
 
 // C = epi(prologue(A) . W^T): picks the skinny kernel for M <= 16 rows, a tile kernel otherwise.
-// groups > 1 (argmax heads): blockIdx.z = group.  edge (tests): 0 = that choice, 16 = the skinny kernel, 32 / 64 / 128 = that
-// tile edge.  parts_out: the argmax partial slots per row the launch writes.
+// groups > 1 (argmax heads): blockIdx.z = group.  edge: 0 = that choice, 16 = the skinny kernel (more than 16 rows in
+// blocks of 16, each row with the reduction order of a launch of <= 16 rows), 32 / 64 / 128 = that tile edge (tests).
+// parts_out: the argmax partial slots per row the launch writes.
 int launch_dense(dense::DenseOp op, int groups, cudaStream_t st, int edge = 0, int* parts_out = nullptr) {
   if (op.K % 16 || op.M < 1 || op.N < 1) return fail(SOPRO_ERR_INVALID, "dense: bad shape M=%d N=%d K=%d", op.M, op.N, op.K);
   if (edge == 0) edge = op.M <= dense::kSkinnyRows ? 16 : tile_edge(op.M, op.N, groups, op.epi);
   if (edge == 16) {
-    if (op.M > dense::kSkinnyRows) return fail(SOPRO_ERR_INVALID, "dense: M=%d too many rows for the skinny kernel", op.M);
+    const int row_blocks = (op.M + dense::kSkinnyRows - 1) / dense::kSkinnyRows;
+    if ((row_blocks > 1 && op.epi == dense::EPI_ARGMAX) || row_blocks > 65535)
+      return fail(SOPRO_ERR_INVALID, "dense: M=%d too many rows for the skinny kernel", op.M);
     const int ncol = op.epi == dense::EPI_GLU ? op.N / 2 : op.N;
     // about two waves of CTAs over the GPU, at least one column per warp
     int cols = std::max(8, (ncol * groups + 295) / 296);
@@ -84,7 +87,7 @@ int launch_dense(dense::DenseOp op, int groups, cudaStream_t st, int edge = 0, i
     if (tc::attr_needed(attr_done))
       CK(cudaFuncSetAttribute(dense::dense_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 2048 * 4));
     if (parts_out) *parts_out = parts;
-    dense::dense_skinny_kernel<<<dim3(parts, 1, groups), dense::kSkinnyThreads, smem, st>>>(op, cols);
+    dense::dense_skinny_kernel<<<dim3(parts, row_blocks, groups), dense::kSkinnyThreads, smem, st>>>(op, cols);
   } else {
     const int e = edge;
     if ((e != 32 && e != 64 && e != 128) || (e == 32 && op.epi == dense::EPI_GLU))
@@ -1156,12 +1159,25 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
 // =================================================================================================
 namespace pstage {
 
-// out[t][c] = sum_q w[q] * emb[(q*V + tok[t][q]) * dim + c], q ascending (the reference's loop order); a code outside
-// [0, V) is clamped and flagged
+// Token2SV's batch of B sequences is PACKED: rows[2b] = the first row of sequence b in the [frames][d] buffers,
+// rows[2b+1] = its length.  Every kernel then runs over valid frames only, and the pooling projection is one dense
+// launch over them (a padded layout would compute every padding frame of a ragged batch: one 4096-frame take beside
+// fifteen 40-frame ones would be 16 x 4096 rows instead of 4696).
+
+// out[r][c] = sum_q w[q] * emb[(q*V + tok[b][t][q]) * dim + c], q ascending (the reference's loop order); a code outside
+// [0, V) is clamped and flagged.  Frame t = blockIdx.x of sequence b = blockIdx.y, tok [B][T][Q]; rows null: r = t
+// (one sequence), otherwise r = rows[2b] + t and frames past rows[2b+1] are skipped
 __global__ void __launch_bounds__(128) codes_mix_kernel(const int* __restrict__ tok, const float* __restrict__ emb,
                                                         const float* __restrict__ w, float* __restrict__ out, int Q, int V, int dim,
-                                                        int* __restrict__ bad) {
-  const int t = blockIdx.x;
+                                                        int* __restrict__ bad, const int* __restrict__ rows = nullptr, int T = 0) {
+  const int t = blockIdx.x, b = blockIdx.y;
+  size_t r = t;
+  if (rows) {
+    if (t >= rows[2 * b + 1]) return;
+    r = (size_t)rows[2 * b] + t;
+    tok += (size_t)b * T * Q;
+  }
+  out += r * dim;
   extern __shared__ int ids[];
   for (int q = threadIdx.x; q < Q; q += blockDim.x) {
     int id = tok[(size_t)t * Q + q];
@@ -1175,33 +1191,42 @@ __global__ void __launch_bounds__(128) codes_mix_kernel(const int* __restrict__ 
   for (int c = threadIdx.x; c < dim; c += blockDim.x) {
     float acc = 0.f;
     for (int q = 0; q < Q; ++q) acc = __fadd_rn(acc, __fmul_rn(__ldg(w + q), __ldg(emb + ((size_t)q * V + ids[q]) * dim + c)));
-    out[(size_t)t * dim + c] = acc;
+    out[c] = acc;
   }
 }
 
-// y[t][c] = gelu(bias[c] + sum_j x[t + j - left][c] * w[c][j])   (DepthwiseConv1d non-causal + GELU, zero padding)
+// y[t][c] = gelu(bias[c] + sum_j x[t + j - left][c] * w[c][j])   (DepthwiseConv1d non-causal + GELU, zero padding at
+// both ends of each sequence): frame t = blockIdx.x of packed sequence b = blockIdx.y
 __global__ void __launch_bounds__(128) dwconv_gelu_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                                          const float* __restrict__ bias, float* __restrict__ y, int T, int D, int k,
-                                                          int left) {
-  const int t = blockIdx.x;
+                                                          const float* __restrict__ bias, float* __restrict__ y,
+                                                          const int* __restrict__ rows, int D, int k, int left) {
+  const int t = blockIdx.x, b = blockIdx.y, T = rows[2 * b + 1];
+  if (t >= T) return;
+  const size_t base = rows[2 * b];
+  x += base * D;
   for (int c = threadIdx.x; c < D; c += blockDim.x) {
     float acc = 0.f;
     for (int j = 0; j < k; ++j) {
       const int r = t + j - left;
       if (r >= 0 && r < T) acc = fmaf(x[(size_t)r * D + c], __ldg(w + c * k + j), acc);
     }
-    y[(size_t)t * D + c] = dense::gelu_erf(acc + __ldg(bias + c));
+    y[(base + t) * D + c] = dense::gelu_erf(acc + __ldg(bias + c));
   }
 }
 
 // AttentiveStatsPool tail: u [T][D] = W0 h + b0 (from the dense kernel); logits[t] = w2 . tanh(u[t]) + b2; a = softmax_t;
-// mu = sum_t a h; std = sqrt(max(sum_t a (h - mu)^2, 1e-6)); out = [mu | std]  (one CTA; T floats of shared memory)
+// mu = sum_t a h; std = sqrt(max(sum_t a (h - mu)^2, 1e-6)); out = [mu | std]  (one CTA per packed sequence
+// b = blockIdx.x, out [B][2D]; T floats of shared memory)
 __global__ void __launch_bounds__(256) attn_stats_pool_kernel(const float* __restrict__ u, const float* __restrict__ h,
-                                                              const float* __restrict__ w2, float b2, float* __restrict__ out, int T,
-                                                              int D) {
+                                                              const float* __restrict__ w2, float b2, float* __restrict__ out,
+                                                              const int* __restrict__ rows, int D) {
   extern __shared__ float a[];
   __shared__ float red[8];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x, T = rows[2 * b + 1];
+  u += (size_t)rows[2 * b] * D;
+  h += (size_t)rows[2 * b] * D;
+  out += (size_t)b * 2 * D;
   for (int t = warp; t < T; t += 8) {
     float s = 0.f;
     for (int c = lane; c < D; c += 32) s = fmaf(__ldg(w2 + c), tanhf(u[(size_t)t * D + c]), s);
@@ -1245,15 +1270,28 @@ __global__ void __launch_bounds__(256) attn_stats_pool_kernel(const float* __res
   }
 }
 
-// F.normalize(e, eps): e / max(||e||, eps), one warp
-__global__ void l2_normalize_kernel(const float* __restrict__ e, float* __restrict__ out, int n, float eps) {
+// F.normalize(e, eps): e / max(||e||, eps), one warp per row b = blockIdx.x of e / out [B][n]; with ref [n], also
+// cos[b] = out[b] . ref (the rows and ref are unit vectors, so this is their cosine)
+__global__ void l2_normalize_kernel(const float* __restrict__ e, float* __restrict__ out, int n, float eps,
+                                    const float* __restrict__ ref, float* __restrict__ cos) {
   const int lane = threadIdx.x;
+  e += (size_t)blockIdx.x * n;
+  out += (size_t)blockIdx.x * n;
   float s = 0.f;
   for (int i = lane; i < n; i += 32) s = fmaf(e[i], e[i], s);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   const float d = fmaxf(sqrtf(s), eps);
-  for (int i = lane; i < n; i += 32) out[i] = e[i] / d;
+  float c = 0.f;
+  for (int i = lane; i < n; i += 32) {
+    const float v = e[i] / d;
+    out[i] = v;
+    if (ref) c = fmaf(v, __ldg(ref + i), c);
+  }
+  if (!ref) return;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if (lane == 0) cos[blockIdx.x] = c;
 }
 
 // [T][H*Dh] -> [H][T][Dh]
@@ -1281,6 +1319,76 @@ struct sopro_refprep {
   size_t ws_bytes = 0;
   int* bad = nullptr;
 };
+
+namespace pstage {
+
+size_t al64(size_t x) { return (x + 63) / 64 * 64; }
+
+// the workspace holds at least `need` bytes (a grown one replaces the old once the stream is done with it)
+int grow_ws(sopro_refprep* p, size_t need, cudaStream_t st) {
+  if (p->ws_bytes >= need) return SOPRO_OK;
+  CK(cudaStreamSynchronize(st));
+  cudaFree(p->ws);
+  p->ws = nullptr;
+  p->ws_bytes = 0;
+  cudaError_t e = cudaMalloc(&p->ws, need);
+  if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "reference-preparation workspace: %s", cudaGetErrorString(e));
+  p->ws_bytes = need;
+  return SOPRO_OK;
+}
+
+// Token2SV of B code sequences, tokens [B][Tmax][Q], lens[b] (host) frames each -> sv [B][SV], and cos [B] when ref_sv
+// is given.  x / h / q: [sum lens][d] each, stats [B][2d], e [B][SV], rows: 2B ints (device).  A row's result does not
+// depend on the batch: the convolutions and the pooling stay inside each sequence, and both matmuls run each row in the
+// reduction order it gets alone -- a sequence of <= 16 frames (and the B-row projection) on the skinny kernel in blocks
+// of 16 rows, longer sequences on the tile kernel, whose order does not depend on M.  So the long sequences are packed
+// first, the short ones after them, and the pooling matmul is one launch per kind.
+int token2sv(sopro_refprep* p, const int32_t* tokens, int B, int Tmax, const int32_t* lens, float* sv, const float* ref_sv, float* cos,
+             float* x, float* h, float* q, float* stats, float* e, int* rows, cudaStream_t st) {
+  const sopro_refprep_config_t& c = p->cfg;
+  const int d = c.sv_embed_dim, SV = c.sv_dim, Q = c.n_codebooks, V = c.codebook_size;
+  std::vector<int> host(2 * (size_t)B);
+  int n_long = 0, total = 0;
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int b = 0; b < B; ++b) {
+      if ((lens[b] > dense::kSkinnyRows) != (pass == 0)) continue;
+      host[2 * b] = total;
+      host[2 * b + 1] = lens[b];
+      total += lens[b];
+    }
+    if (pass == 0) n_long = total;
+  }
+  CK(cudaMemcpyAsync(rows, host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const float* W = p->dev;
+  const dim3 frames(Tmax, B);
+  codes_mix_kernel<<<frames, 128, Q * sizeof(int), st>>>(tokens, W + p->sv_emb, W + p->sv_w, x, Q, V, d, p->bad, rows, Tmax);
+  CK(cudaGetLastError());
+  const int left = (c.sv_kernel - 1) / 2;
+  dwconv_gelu_kernel<<<frames, 128, 0, st>>>(x, W + p->dw0_w, W + p->dw0_b, h, rows, d, c.sv_kernel, left);
+  dwconv_gelu_kernel<<<frames, 128, 0, st>>>(h, W + p->dw1_w, W + p->dw1_b, x, rows, d, c.sv_kernel, left);
+  CK(cudaGetLastError());
+  int rc;
+  dense::DenseOp g{};
+  g.W = W + p->pool_w0; g.bias = W + p->pool_b0; g.N = d; g.K = d; g.ldc = d; g.epi = dense::EPI_BIAS;
+  if (n_long > 0) {  // > 16 rows: the tile kernel
+    g.A = x; g.C = q; g.M = n_long;
+    if ((rc = launch_dense(g, 1, st))) return rc;
+  }
+  if (total > n_long) {
+    g.A = x + (size_t)n_long * d; g.C = q + (size_t)n_long * d; g.M = total - n_long;
+    if ((rc = launch_dense(g, 1, st, 16))) return rc;
+  }
+  attn_stats_pool_kernel<<<B, 256, (size_t)Tmax * 4, st>>>(q, x, W + p->pool_w2, p->pool_b2, stats, rows, d);
+  CK(cudaGetLastError());
+  g = dense::DenseOp{};
+  g.A = stats; g.W = W + p->proj_w; g.bias = W + p->proj_b; g.C = e; g.M = B; g.N = SV; g.K = 2 * d; g.ldc = SV; g.epi = dense::EPI_BIAS;
+  if ((rc = launch_dense(g, 1, st, 16))) return rc;
+  l2_normalize_kernel<<<B, 32, 0, st>>>(e, sv, SV, 1e-6f, ref_sv, cos);
+  CK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+}  // namespace pstage
 
 extern "C" {
 
@@ -1377,45 +1485,25 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
   CK(cudaSetDevice(p->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int D = c.d_model, d = c.sv_embed_dim, SV = c.sv_dim, Q = c.n_codebooks, V = c.codebook_size, H = c.ref_heads;
-  auto al = [](size_t x) { return (x + 63) / 64 * 64; };
+  const auto al = al64;
   const size_t rows = (size_t)Tr;
-  const size_t need = (al(rows * D) * 3 + al(rows * 4 * D) + al(2 * (size_t)d) + al((size_t)SV)) * 4;
-  if (p->ws_bytes < need) {
-    CK(cudaStreamSynchronize(st));
-    cudaFree(p->ws);
-    p->ws = nullptr;
-    p->ws_bytes = 0;
-    cudaError_t e = cudaMalloc(&p->ws, need);
-    if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "reference-preparation workspace: %s", cudaGetErrorString(e));
-    p->ws_bytes = need;
-  }
+  const size_t need = (al(rows * D) * 3 + al(rows * 4 * D) + al(2 * (size_t)d) + al((size_t)SV) + al(2)) * 4;
+  int rc;
+  if ((rc = grow_ws(p, need, st))) return rc;
   float* x = p->ws;
   float* h = x + al(rows * D);
   float* q = h + al(rows * D);
   float* hid = q + al(rows * D);
   float* stats = hid + al(rows * 4 * D);  // [2d]
   float* e = stats + al(2 * (size_t)d);   // [SV]
+  int* seq_rows = reinterpret_cast<int*>(e + al((size_t)SV));
   const float* W = p->dev;
-  int rc;
   dense::DenseOp g{};
-  // ---- Token2SV (d <= D: the [Tr][d] buffers live in x / h / q)
-  codes_mix_kernel<<<Tr, 128, Q * sizeof(int), st>>>(tokens, W + p->sv_emb, W + p->sv_w, x, Q, V, d, p->bad);
-  CK(cudaGetLastError());
-  const int left = (c.sv_kernel - 1) / 2;
-  dwconv_gelu_kernel<<<Tr, 128, 0, st>>>(x, W + p->dw0_w, W + p->dw0_b, h, Tr, d, c.sv_kernel, left);
-  dwconv_gelu_kernel<<<Tr, 128, 0, st>>>(h, W + p->dw1_w, W + p->dw1_b, x, Tr, d, c.sv_kernel, left);
-  CK(cudaGetLastError());
-  g.A = x; g.W = W + p->pool_w0; g.bias = W + p->pool_b0; g.C = q; g.M = Tr; g.N = d; g.K = d; g.ldc = d; g.epi = dense::EPI_BIAS;
-  if ((rc = launch_dense(g, 1, st))) return rc;
-  attn_stats_pool_kernel<<<1, 256, (size_t)Tr * 4, st>>>(q, x, W + p->pool_w2, p->pool_b2, stats, Tr, d);
-  CK(cudaGetLastError());
-  g = dense::DenseOp{};
-  g.A = stats; g.W = W + p->proj_w; g.bias = W + p->proj_b; g.C = e; g.M = 1; g.N = SV; g.K = 2 * d; g.ldc = SV; g.epi = dense::EPI_BIAS;
-  if ((rc = launch_dense(g, 1, st))) return rc;
-  l2_normalize_kernel<<<1, 32, 0, st>>>(e, sv, SV, 1e-6f);
-  CK(cudaGetLastError());
+  // ---- Token2SV: the batched path with B = 1 (d <= D: the [Tr][d] buffers live in x / h / q)
+  const int32_t len = Tr;
+  if ((rc = token2sv(p, tokens, 1, Tr, &len, sv, nullptr, nullptr, x, h, q, stats, e, seq_rows, st))) return rc;
   // ---- reference encoder
-  codes_mix_kernel<<<Tr, 128, Q * sizeof(int), st>>>(tokens, W + p->cb_embed, W + p->ref_w, x, Q, V, D, p->bad);
+  codes_mix_kernel<<<Tr, 128, Q * sizeof(int), st>>>(tokens, W + p->cb_embed, W + p->ref_w, x, Q, V, D, p->bad, nullptr, 0);
   CK(cudaGetLastError());
   for (int i = 0; i < c.ref_enc_layers; ++i)
     if ((rc = ssm_block(W, p->blk[i], x, h, hid, nullptr, 1, Tr, D, c.ref_enc_kernel, 1, false, st))) return rc;
@@ -1434,6 +1522,33 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
     }
   }
   return SOPRO_OK;
+}
+
+int sopro_refprep_speaker_vectors(sopro_refprep_t* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host,
+                                  float* sv, const float* ref_sv, float* cos, void* stream) {
+  if (!p || !tokens || !lens_host || !sv) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535) return fail(SOPRO_ERR_INVALID, "B=%d outside [1, 65535]", B);
+  if (Tmax < 1 || Tmax > 4096) return fail(SOPRO_ERR_INVALID, "Tmax=%d outside [1, 4096]", Tmax);
+  if (ref_sv && !cos) return fail(SOPRO_ERR_INVALID, "ref_sv given without cos");
+  size_t total = 0;
+  for (int b = 0; b < B; ++b) {
+    if (lens_host[b] < 1 || lens_host[b] > Tmax) return fail(SOPRO_ERR_INVALID, "lens[%d]=%d outside [1, %d]", b, lens_host[b], Tmax);
+    total += (size_t)lens_host[b];
+  }
+  CK(cudaSetDevice(p->device));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t d = p->cfg.sv_embed_dim, SV = p->cfg.sv_dim, nb = (size_t)B;
+  const auto al = pstage::al64;
+  const size_t need = (al(total * d) * 3 + al(nb * 2 * d) + al(nb * SV) + al(2 * nb)) * 4;
+  int rc;
+  if ((rc = pstage::grow_ws(p, need, st))) return rc;
+  float* x = p->ws;
+  float* h = x + al(total * d);
+  float* q = h + al(total * d);
+  float* stats = q + al(total * d);
+  float* e = stats + al(nb * 2 * d);
+  int* rows = reinterpret_cast<int*>(e + al(nb * SV));
+  return pstage::token2sv(p, tokens, B, Tmax, lens_host, sv, ref_sv, cos, x, h, q, stats, e, rows, st);
 }
 
 /* Synchronises `stream`; SOPRO_ERR_INVALID if a run since the last check met a code outside [0, codebook_size). */

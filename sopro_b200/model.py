@@ -21,6 +21,7 @@ import torch
 
 from . import longform as LF
 from . import prefill as P
+from . import rerank
 from . import timestamps as TS
 from ._lib import StatePool
 from .codec import MimiCodec
@@ -297,16 +298,17 @@ class SoproModel:
     def ar_generate_tensors(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int, top_p: float = 0.9,
                             temperature: float = 1.05, anti_loop: bool = True, min_gen_frames: Optional[int] = None,
                             seeds: Optional[Sequence[int]] = None, stop_on_first_eos: bool = True,
-                            attn_trace: Optional[torch.Tensor] = None):
+                            attn_trace: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None):
         """B utterances in ONE persistent kernel run from batch tensors (cond [B, >=steps, D], txt [B, Lmax, D], lens).
         -> (tokens [B, steps] int32 numpy, n_tokens [B]).  With `seeds` and at least 64 steps the run is launched in
         growing blocks (the kernel resumes from its device state), each block's tapes drawn on host threads while the
         device generates the block before; otherwise in one launch.  `attn_trace` (word timestamps): a
-        [steps, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text cross-attention weights."""
+        [steps, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text cross-attention weights.  Without
+        `seeds` the tapes draw from `generator` (None: the global one)."""
         B, steps = int(cond.shape[0]), int(max_frames) + 1
         samp = self._sampling(top_p, temperature, anti_loop, 8, 0.85, 1.2, min_gen_frames, stop_on_first_eos)
         edges = _growing_blocks(steps) if seeds is not None and steps >= 64 else [(0, steps)]
-        with TapeFeed(B, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device, seeds) as feed, \
+        with TapeFeed(B, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device, seeds, generator) as feed, \
                 self._lease(B, steps, max(int(x) for x in lens), attn_trace) as ses:
             for _ in self._launch_blocks(ses, feed, edges, cond[:, :steps], txt, [int(x) for x in lens], samp):
                 pass
@@ -415,7 +417,8 @@ class SoproTTS:
                    temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                    ref_seconds: Optional[float] = None, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
                    generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
-                   speed: Optional[float] = None, loudness: Optional[float] = None, word_timestamps: bool = False):
+                   speed: Optional[float] = None, loudness: Optional[float] = None, word_timestamps: bool = False,
+                   best_of: int = 1):
         """-> [1, 1, N] f32 on the device.  `sample_rate` (extension): the output rate in Hz (None = 24 kHz, the codec's
         own); another rate resamples the decoded waveform on the GPU (sopro_b200/resample.py).  `speed` (extension): the
         speaking rate in [0.25, 4.0] (None = the model's own); the 24 kHz waveform is time-stretched on the GPU with its
@@ -423,19 +426,36 @@ class SoproTTS:
         integrated loudness in LUFS, [-60, 0] (None = the level the model produced); the final waveform is measured per
         ITU-R BS.1770-4 and scaled on the GPU under a -1 dBFS sample-peak ceiling (sopro_b200/loudness.py).
         `word_timestamps` (extension): also return when each word is spoken, ``(wav, List[WordTiming])``, from the AR
-        step's text cross-attention (sopro_b200/timestamps.py); the audio is the same as without it."""
+        step's text cross-attention (sopro_b200/timestamps.py); the audio is the same as without it.
+        `best_of` (extension): generate that many takes side by side in one batch (take k with seed + k) and keep the
+        one rerank.choose picks: takes that ended with an EOS and have at least one frame per text token first, then
+        the highest cosine between the take's speaker vector and the reference voice's; only that take is decoded.
+        The result equals synthesize(seed=seed + k) for the picked k.  Without a seed the takes draw from the generator
+        as synthesize_batch of the takes would.  That the cosine picks better-sounding takes is not measured."""
         post = OutputChain(self, sample_rate, speed, loudness)  # a refused rate, speed or target raises before any work
+        n_best = self._check_best_of(best_of, 1)
         text_ids = self.encode_text(text)
         trace = spans = None
         if word_timestamps:
             spans = self.tokenizer.encode_with_offsets(text)[1]
-            trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, 1, int(text_ids.numel()), self.device)
+            if n_best == 1:
+                trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, 1, int(text_ids.numel()), self.device)
         if ref is None:
             ref = self.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
-        tokens_tq = self.model.generate_tokens(
-            text_ids, ref=ref, max_frames=max_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
-            style_strength=float(style_strength if style_strength is not None else self.cfg.style_strength),
-            min_gen_frames=min_gen_frames, seed=seed, generator=generator, attn_trace=trace)
+        if n_best == 1:
+            tokens_tq = self.model.generate_tokens(
+                text_ids, ref=ref, max_frames=max_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
+                style_strength=float(style_strength if style_strength is not None else self.cfg.style_strength),
+                min_gen_frames=min_gen_frames, seed=seed, generator=generator, attn_trace=trace)
+        else:
+            tr: Optional[dict] = {} if word_timestamps else None
+            Ts, codes = self._best_codes([text], ref, n_best, seeds=None if seed is None else [int(seed)], trace_out=tr,
+                                         generator=generator, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                         anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+            tokens_tq = (codes[0, : Ts[0]] if codes is not None
+                         else torch.zeros((0, int(self.cfg.num_codebooks)), dtype=torch.long, device=self.device))
+            if word_timestamps:
+                trace = tr["probs"]
         words = None
         if word_timestamps:
             words = self._timings([text], [spans], trace, [int(text_ids.numel())], [int(tokens_tq.shape[0])], post.S)[0]
@@ -447,17 +467,20 @@ class SoproTTS:
                          temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                          min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                          sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                         loudness: Optional[float] = None, word_timestamps: bool = False):
+                         loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1):
         """NEW: B texts with one shared prepared reference -> B waveforms [1, 1, N_i].  One batched prefill, one
         persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, then
         loudness-normalised, in one ragged launch when `speed` / `sample_rate` / `loudness` is given); utterance i equals
         synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness).
-        `word_timestamps`: also return each utterance's word timings (see synthesize), ``(List[wav], List[List[WordTiming]])``."""
+        `word_timestamps`: also return each utterance's word timings (see synthesize), ``(List[wav], List[List[WordTiming]])``.
+        `best_of`: each text's takes are generated in the same pass (B x best_of rows, take k of text i with seed
+        seeds[i] + k) and only the picked take of each text is decoded (see synthesize)."""
         post = OutputChain(self, sample_rate, speed, loudness)
+        n_best = self._check_best_of(best_of, len(texts))
         tr: Optional[dict] = {} if word_timestamps else None
-        Ts, codes = self._batch_codes(texts, ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                      anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
-                                      seeds=seeds, trace_out=tr)
+        Ts, codes = self._best_codes(texts, ref, n_best, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                     anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
+                                     seeds=seeds, trace_out=tr)
         words = None
         if word_timestamps:
             spans = [self.tokenizer.encode_with_offsets(t)[1] for t in texts]
@@ -474,7 +497,7 @@ class SoproTTS:
                         pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
                         style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
                         seed: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                        loudness: Optional[float] = None, word_timestamps: bool = False):
+                        loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1):
         """NEW: a text of any length -> one waveform [1, 1, N] f32 on the device.  The text is cut into segments of at
         most `max_tokens` tokens (sopro_b200/longform.py::split_text: paragraphs, sentences, greedy packing); the
         segments are generated side by side through the batch path, SEGMENT_GROUP at a time (segment i equals
@@ -484,14 +507,21 @@ class SoproTTS:
         through the chain of synthesize: stretch (`speed`, pauses included), resample (`sample_rate`), loudness (one
         level for the whole passage).  Segments that produced no frames are skipped; if none did, the result is
         [1, 1, 0].  Every argument is checked before any work.  `word_timestamps`: also return the passage's word timings
-        (see synthesize), ``(wav, List[WordTiming])``, their char spans in `text`."""
+        (see synthesize), ``(wav, List[WordTiming])``, their char spans in `text`.  `best_of`: each segment picks its own
+        take (see synthesize; take k of segment i with seed seed + i + k) and the join sees only the picked ones; a
+        group then holds fewer segments when group x best_of rows would exceed the batch limit."""
         post = OutputChain(self, sample_rate, speed, loudness)
+        n_best = self._check_best_of(best_of, 1)
         LF.check_pause(pause_ms)
         budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
         segments = LF.split_text(text, self.tokenizer, budget)
         if not segments:
             raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
         B, group = len(segments), int(LF.SEGMENT_GROUP)
+        if n_best > 1:
+            limit = self._batch_limit()
+            if limit is not None:
+                group = max(1, min(group, limit // n_best))
         ext = torch.zeros((B, 2), dtype=torch.int64, device=self.device)
         rows: List[torch.Tensor] = [torch.zeros(0, device=self.device)] * B
         firsts: List = []
@@ -500,9 +530,9 @@ class SoproTTS:
             part = segments[g0: g0 + group]
             seeds = None if seed is None else [int(seed) + g0 + i for i in range(len(part))]
             tr: Optional[dict] = {} if word_timestamps else None
-            Ts, codes = self._batch_codes(part, ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                          anti_loop=anti_loop, style_strength=style_strength,
-                                          min_gen_frames=min_gen_frames, seeds=seeds, trace_out=tr)
+            Ts, codes = self._best_codes(part, ref, n_best, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                         anti_loop=anti_loop, style_strength=style_strength,
+                                         min_gen_frames=min_gen_frames, seeds=seeds, trace_out=tr)
             if word_timestamps:
                 first = TS.align(tr["probs"], tr["lens"], Ts).cpu().numpy()
                 firsts.extend(first[i] for i in range(len(part)))
@@ -530,12 +560,60 @@ class SoproTTS:
         hop = self.codec.engine.hop
         return [TS.utterance_timings(t, sp, first[i], int(Ts[i]), hop, S) for i, (t, sp) in enumerate(zip(texts, spans))]
 
+    def _best_codes(self, texts: Sequence[str], ref: PreparedReference, best_of: int, *, seeds: Optional[Sequence[int]],
+                    trace_out: Optional[dict] = None, generator: Optional[torch.Generator] = None,
+                    **kw) -> Tuple[List[int], Optional[torch.Tensor]]:
+        """_batch_codes with `best_of` candidates per text (sopro_b200/rerank.py): text i's candidate k is row i*N + k
+        of ONE _batch_codes pass, with seed seeds[i] + k; every take is scored with one Token2SV launch against
+        ref.sv_ref, rerank.choose picks one per text, and only the picked rows are returned (the trace too), so the
+        caller decodes those alone.  best_of = 1 is _batch_codes itself."""
+        N = int(best_of)
+        if N == 1:
+            return self._batch_codes(texts, ref, seeds=seeds, trace_out=trace_out, generator=generator, **kw)
+        rows = [t for t in texts for _ in range(N)]
+        tr: Optional[dict] = {} if trace_out is not None else None
+        info: dict = {}
+        Ts, codes = self._batch_codes(rows, ref, seeds=rerank.candidate_seeds(seeds, N), trace_out=tr, generator=generator,
+                                      info=info, **kw)
+        cos = [0.0] * len(rows)
+        live = [r for r in range(len(rows)) if Ts[r] > 0]
+        if live:  # the takes with frames, in one launch
+            _sv, c = self.model.refprep.speaker_vectors(codes[torch.tensor(live, device=codes.device)], [Ts[r] for r in live],
+                                                        ref.sv_ref)
+            for r, v in zip(live, c.tolist()):
+                cos[r] = v
+        picks = []
+        for i in range(len(texts)):
+            a = i * N
+            picks.append(a + rerank.choose(Ts[a: a + N], info["stopped"][a: a + N], info["text_lens"][a], cos[a: a + N]))
+        Ts = [Ts[p] for p in picks]
+        if tr is not None:
+            trace_out["probs"] = tr["probs"][:, :, picks].contiguous()
+            trace_out["lens"] = [tr["lens"][p] for p in picks]
+        if max(Ts) == 0:
+            return Ts, None
+        return Ts, codes[torch.tensor(picks, device=codes.device)]
+
+    def _batch_limit(self) -> Optional[int]:
+        """The AR session's batch limit (SMs x 16 utterances per team)."""
+        dev = self.model.device
+        return torch.cuda.get_device_properties(dev).multi_processor_count * 16 if dev.type == "cuda" else None
+
+    def _check_best_of(self, best_of, rows: int) -> int:
+        """best_of checked, and the rows it makes checked against the batch limit, before any work."""
+        n = rerank.check_best_of(best_of)
+        if n > 1:
+            rerank.check_rows(rows * n, self._batch_limit())
+        return n
+
     def _batch_codes(self, texts: Sequence[str], ref: PreparedReference, *, max_frames: int, top_p: float,
                      temperature: float, anti_loop: bool, style_strength: Optional[float], min_gen_frames: Optional[int],
-                     seeds: Optional[Sequence[int]], trace_out: Optional[dict] = None) -> Tuple[List[int], Optional[torch.Tensor]]:
+                     seeds: Optional[Sequence[int]], trace_out: Optional[dict] = None, generator: Optional[torch.Generator] = None,
+                     info: Optional[dict] = None) -> Tuple[List[int], Optional[torch.Tensor]]:
         """B texts with one prepared reference: one batched prefill, one persistent AR launch, one ragged NAR pass ->
         (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0 frames).
-        `trace_out` (word timestamps): receives "probs", the AR launch's attention weights, and "lens", the text lengths."""
+        `trace_out` (word timestamps): receives "probs", the AR launch's attention weights, and "lens", the text lengths.
+        `info` (best-of-N): receives "stopped", whether each row sampled an EOS, and "text_lens"."""
         st = float(style_strength if style_strength is not None else self.cfg.style_strength)
         model = self.model
         ids = [self.encode_text(t) for t in texts]
@@ -546,13 +624,16 @@ class SoproTTS:
             trace_out["probs"], trace_out["lens"] = trace, [int(x) for x in lens]
         toks, n = model.ar_generate_tensors(cond, txt_seq, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
                                             anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds,
-                                            attn_trace=trace)
+                                            attn_trace=trace, generator=generator)
         eos, B = model.eos_id, len(texts)
-        Ts = []
+        Ts, stopped = [], []
         for i in range(B):
             row = toks[i, : n[i]]
             hit = (row == eos).nonzero()[0]
             Ts.append(int(hit[0]) if hit.size else int(n[i]))
+            stopped.append(bool(hit.size))
+        if info is not None:
+            info["stopped"], info["text_lens"] = stopped, [int(x) for x in lens]
         Tmax = max(Ts)
         if Tmax == 0:
             return Ts, None
@@ -584,6 +665,8 @@ class SoproTTS:
 
     def stream(self, text: str, *, sample_rate: Optional[int] = None, speed: Optional[float] = None,
                **kwargs) -> Iterator[torch.Tensor]:
+        """Chunks of one utterance as they are generated (sopro_b200/streaming.py).  There is no `best_of` here: a
+        stream plays its take while it is generated, so it cannot choose among takes before playing one."""
         from .streaming import stream as _stream
 
         return _stream(self, text, sample_rate=sample_rate, speed=speed, **kwargs)

@@ -4,7 +4,7 @@ once-per-voice reference preparation in front of it (sopro_refprep_*; reference 
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, List, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -175,6 +175,35 @@ class RefPrepEngine:
         except _lib.SoproError as e:
             raise IndexError(str(e)) from None  # the reference's embedding lookup raises IndexError
         return sv, seq, [{"k": k, "v": v, "key_padding_mask": None} for k, v in zip(ks, vs)]
+
+    def speaker_vectors(self, codes: torch.Tensor, lens: Sequence[int], ref_sv: Optional[torch.Tensor] = None
+                        ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """Token2SV of a ragged batch in one pass: codes [B, Tmax, Q] (row b's first lens[b] frames) -> (sv [B, sv_dim],
+        cos [B] with `ref_sv` [sv_dim] or [1, sv_dim], else None) on the device.  Row b equals ``run(codes[b, :lens[b]])[0]``
+        bit for bit.  Refused geometry raises ValueError before any launch; a code outside the codebook IndexError."""
+        if codes.dim() != 3 or int(codes.shape[2]) != self.Q:
+            raise ValueError(f"codes must be [B, Tmax, {self.Q}], got {tuple(codes.shape)}")
+        B, Tmax = int(codes.shape[0]), int(codes.shape[1])
+        ln = torch.tensor([int(x) for x in lens], dtype=torch.int32)
+        if int(ln.numel()) != B:
+            raise ValueError(f"{int(ln.numel())} lengths for {B} sequences")
+        ref = None
+        if ref_sv is not None:
+            ref = ref_sv.to(self.device, torch.float32).reshape(-1).contiguous()
+            if int(ref.numel()) != self.sv_dim:
+                raise ValueError(f"ref_sv must hold {self.sv_dim} values, got {int(ref.numel())}")
+        tok = codes.to(self.device, torch.int32).contiguous()
+        sv = torch.empty((max(B, 1), self.sv_dim), dtype=torch.float32, device=self.device)
+        cos = torch.empty(max(B, 1), dtype=torch.float32, device=self.device) if ref is not None else None
+        st = int(torch.cuda.current_stream(self.device).cuda_stream)
+        _lib.check_arg(self.lib.sopro_refprep_speaker_vectors(self._h, tok.data_ptr(), B, Tmax, ln.data_ptr(), sv.data_ptr(),
+                                                               None if ref is None else ref.data_ptr(),
+                                                               None if cos is None else cos.data_ptr(), st))
+        try:
+            _lib.check(self.lib.sopro_refprep_check(self._h, st))  # also keeps `tok` and `ref` alive until read
+        except _lib.SoproError as e:
+            raise IndexError(str(e)) from None
+        return sv, cos
 
     def close(self) -> None:
         if getattr(self, "_h", None):

@@ -821,6 +821,63 @@ int sopro_align_sizes(int32_t B, int32_t steps, int64_t ld, int64_t* ws_bytes);
 int sopro_align(const float* probs, int32_t steps, int32_t n_attn, int32_t B, int32_t H, int64_t ld, const int32_t* text_len_host,
                 const int32_t* frames_host, void* ws, int32_t* first, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Watermark (no reference counterpart): a keyed spread-spectrum mark on 24 kHz audio, and its detector.  A key is an
+ * integer in [0, 2^32).
+ *   Pattern: P = SOPRO_WATERMARK_PERIOD samples.  The real-DFT bins k with LO_HZ <= k 24000 / P <= HI_HZ (k = 342 ..
+ *   1194) get unit magnitude and phase 2 pi u_k, u_k = (z >> 11) 2^-53 for splitmix64's outputs z seeded with the key,
+ *   one per bin in bin order; every other bin is zero.  p[n] = sum_k cos(2 pi k n / P + 2 pi u_k) in double, scaled to
+ *   unit RMS, rounded to fp32 once.
+ *   Embed: blocks of SOPRO_WATERMARK_BLOCK samples from the utterance's first sample; r_j = sqrt(sum x^2 / count) over
+ *   block j (a trailing partial block over its own samples), summed in double in a fixed order that depends only on
+ *   the block's samples; g_j = fp32(a min(r_{j-1}, r_j)), r_{-1} = 0, a = 10^(LEVEL_DB / 20);
+ *   y[n] = fma(g_{j(n)}, p[n mod P], x[n]), and y = x bit for bit where g = 0.
+ *   Detect: r_j as above from the clip's first sample; w_j = 1 / r_j where r_j > max(10^(FLOOR_DB / 20) max_j r_j, 1e-6),
+ *   else 0; F[k] = sum over n = k (mod P) of w_{j(n)} x[n] (double, stored fp32); c[l] = sum_k F[k] p[(k + l) mod P]
+ *   for every lag l (fp32, direct); score = max c / sqrt(mean c^2) (0 when c = 0), offset = the first argmax (the
+ *   pattern's phase at the clip's first sample), detected = score >= THRESHOLD.
+ * A row's results depend only on its own samples.  No call synchronises or allocates, except stream_create. */
+#define SOPRO_WATERMARK_PERIOD 8192
+#define SOPRO_WATERMARK_BLOCK 240
+#define SOPRO_WATERMARK_LO_HZ 1000
+#define SOPRO_WATERMARK_HI_HZ 3500
+#define SOPRO_WATERMARK_LEVEL_DB (-30.0)
+#define SOPRO_WATERMARK_FLOOR_DB (-40.0)
+#define SOPRO_WATERMARK_THRESHOLD 7.0
+typedef struct sopro_watermark_stream sopro_watermark_stream_t;
+/* host-only: the key's pattern -> out [P] f32 (host); SOPRO_ERR_INVALID for a key outside [0, 2^32) */
+int sopro_watermark_pattern(int64_t key, float* out);
+/* host-only: the device workspace bytes of one embed / one detect of B rows of at most max_len samples (either
+ * pointer may be NULL); SOPRO_ERR_INVALID for bad geometry */
+int sopro_watermark_sizes(int32_t B, int64_t max_len, int64_t* embed_ws, int64_t* detect_ws);
+/* ragged batch, two launches per 128 rows: row b of x [B][x_stride] f32 (device) has lens_host[b] samples (HOST i64;
+ * NULL = x_stride each); samples at or past lens[b] are not read.  pattern: device f32 [P].  Row b's marked samples go to
+ * y + b * y_stride (device; y_stride >= the longest row when B > 1); the rest of the row is not written. */
+int sopro_watermark_embed(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, const float* pattern, float* y,
+                          int64_t y_stride, void* ws, void* stream);
+/* ragged batch as the embed; per row score -> score [B] (device f32), offset -> offset [B] (device i64), the decision
+ * -> detected [B] (device u8, 0 or 1).  Four launches per 128 rows. */
+int sopro_watermark_detect(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, const float* pattern, void* ws,
+                           float* score, int64_t* offset, uint8_t* detected, void* stream);
+/* Streaming embed: one utterance pushed in chunks of at most max_chunk samples.  A push emits every complete block
+ * (held + n rounded down to a multiple of BLOCK), holding back at most BLOCK - 1 samples; finish emits the held ones as
+ * the last, partial block.  The concatenated outputs equal sopro_watermark_embed of the concatenated input bit for bit,
+ * under any chunk schedule.  The state on the device: the held samples and the last block's r; output counts are host
+ * arithmetic.  Calls on one state must be ordered (one CUDA stream). */
+int sopro_watermark_stream_create(int64_t max_chunk, int device, sopro_watermark_stream_t** out);
+int sopro_watermark_stream_destroy(sopro_watermark_stream_t* s);
+/* back to sample 0 with this key's pattern (device f32 [P], kept alive by the caller until the next reset; host-only).
+ * A new state takes no push until its first reset. */
+int sopro_watermark_stream_reset(sopro_watermark_stream_t* s, const float* pattern);
+/* outputs the next call writes: a push of n_more samples (final == 0), or a push followed by finish (final != 0); < 0 on
+ * bad arguments, before the first reset or after finish */
+int64_t sopro_watermark_stream_ready(const sopro_watermark_stream_t* s, int64_t n_more, int final);
+/* x [n] f32 (device) -> y (device) receives stream_ready(s, n, 0) outputs.  n > max_chunk: SOPRO_ERR_INVALID, nothing
+ * launched, state unchanged.  After finish: SOPRO_ERR_STATE until a reset. */
+int sopro_watermark_push(sopro_watermark_stream_t* s, const float* x, int64_t n, float* y, void* stream);
+/* the held samples, marked -> y (device); SOPRO_ERR_STATE when called twice without a reset */
+int sopro_watermark_finish(sopro_watermark_stream_t* s, float* y, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,7 +6,8 @@ Importing the package does not need a GPU; constructing a model does (no CPU fal
 from .config import SoproTTSConfig  # noqa: F401
 
 __version__ = "0.1.0"
-__all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac", "WordTiming"]
+__all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac", "WordTiming",
+           "detect_watermark"]
 
 
 def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
@@ -14,6 +15,10 @@ def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
         from . import flac
 
         return getattr(flac, name)
+    if name == "detect_watermark":
+        from .watermark import detect_watermark
+
+        return detect_watermark
     if name == "SoproTTS":
         from .model import SoproTTS
 

@@ -259,6 +259,16 @@ SYMBOLS = {
     "sopro_flac_stream_finish": (_I, [_VP, _VP, _VP, _VP, _VP]),
     "sopro_align_sizes": (_I, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_int64)]),
     "sopro_align": (_I, [_VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _I32P, _I32P, _VP, _VP, _VP]),
+    "sopro_watermark_pattern": (_I, [C.c_int64, _VP]),
+    "sopro_watermark_sizes": (_I, [C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "sopro_watermark_embed": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
+    "sopro_watermark_detect": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "sopro_watermark_stream_create": (_I, [C.c_int64, _I, C.POINTER(_VP)]),
+    "sopro_watermark_stream_destroy": (_I, [_VP]),
+    "sopro_watermark_stream_reset": (_I, [_VP, _VP]),
+    "sopro_watermark_stream_ready": (C.c_int64, [_VP, C.c_int64, _I]),
+    "sopro_watermark_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP]),
+    "sopro_watermark_finish": (_I, [_VP, _VP, _VP]),
 }
 
 _lib = None

@@ -34,6 +34,7 @@ from .output import OutputChain
 from .resample import Resampler, check_rates
 from .sampling import TapeFeed
 from .stretch import StretchStream
+from .watermark import WatermarkStream
 from .weights import load_safetensors, read_safetensors_cfg
 
 
@@ -347,6 +348,7 @@ class SoproTTS:
         self._resamplers: Dict[int, Resampler] = {}  # output rate -> its resampler (tap table on the device)
         dev = self.device
         self._stretch_pool = StatePool(lambda n, speed: StretchStream(n, dev, speed))  # idle time-stretch states, any speed
+        self._watermark_pool = StatePool(lambda n, key: WatermarkStream(n, dev, key))  # idle watermark states, any key
 
     # ---- construction
     @classmethod
@@ -418,7 +420,7 @@ class SoproTTS:
                    ref_seconds: Optional[float] = None, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
                    generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
                    speed: Optional[float] = None, loudness: Optional[float] = None, word_timestamps: bool = False,
-                   best_of: int = 1):
+                   best_of: int = 1, watermark: Optional[int] = None):
         """-> [1, 1, N] f32 on the device.  `sample_rate` (extension): the output rate in Hz (None = 24 kHz, the codec's
         own); another rate resamples the decoded waveform on the GPU (sopro_b200/resample.py).  `speed` (extension): the
         speaking rate in [0.25, 4.0] (None = the model's own); the 24 kHz waveform is time-stretched on the GPU with its
@@ -431,8 +433,11 @@ class SoproTTS:
         one rerank.choose picks: takes that ended with an EOS and have at least one frame per text token first, then
         the highest cosine between the take's speaker vector and the reference voice's; only that take is decoded.
         The result equals synthesize(seed=seed + k) for the picked k.  Without a seed the takes draw from the generator
-        as synthesize_batch of the takes would.  That the cosine picks better-sounding takes is not measured."""
-        post = OutputChain(self, sample_rate, speed, loudness)  # a refused rate, speed or target raises before any work
+        as synthesize_batch of the takes would.  That the cosine picks better-sounding takes is not measured.
+        `watermark` (extension): a key, an integer in [0, 2^32) (None = no mark); the 24 kHz waveform, after the
+        time-stretch, carries a keyed spread-spectrum mark 30 dB below the local signal level, which
+        sopro_b200.detect_watermark finds with the same key (sopro_b200/watermark.py)."""
+        post = OutputChain(self, sample_rate, speed, loudness, watermark)  # a refused argument raises before any work
         n_best = self._check_best_of(best_of, 1)
         text_ids = self.encode_text(text)
         trace = spans = None
@@ -467,15 +472,17 @@ class SoproTTS:
                          temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                          min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                          sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                         loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1):
+                         loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1,
+                         watermark: Optional[int] = None):
         """NEW: B texts with one shared prepared reference -> B waveforms [1, 1, N_i].  One batched prefill, one
         persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, then
         loudness-normalised, in one ragged launch when `speed` / `sample_rate` / `loudness` is given); utterance i equals
         synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness).
         `word_timestamps`: also return each utterance's word timings (see synthesize), ``(List[wav], List[List[WordTiming]])``.
         `best_of`: each text's takes are generated in the same pass (B x best_of rows, take k of text i with seed
-        seeds[i] + k) and only the picked take of each text is decoded (see synthesize)."""
-        post = OutputChain(self, sample_rate, speed, loudness)
+        seeds[i] + k) and only the picked take of each text is decoded (see synthesize).  `watermark`: every
+        utterance carries the key's mark (see synthesize)."""
+        post = OutputChain(self, sample_rate, speed, loudness, watermark)
         n_best = self._check_best_of(best_of, len(texts))
         tr: Optional[dict] = {} if word_timestamps else None
         Ts, codes = self._best_codes(texts, ref, n_best, max_frames=max_frames, top_p=top_p, temperature=temperature,
@@ -497,7 +504,8 @@ class SoproTTS:
                         pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
                         style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
                         seed: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                        loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1):
+                        loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1,
+                        watermark: Optional[int] = None):
         """NEW: a text of any length -> one waveform [1, 1, N] f32 on the device.  The text is cut into segments of at
         most `max_tokens` tokens (sopro_b200/longform.py::split_text: paragraphs, sentences, greedy packing); the
         segments are generated side by side through the batch path, SEGMENT_GROUP at a time (segment i equals
@@ -509,8 +517,9 @@ class SoproTTS:
         [1, 1, 0].  Every argument is checked before any work.  `word_timestamps`: also return the passage's word timings
         (see synthesize), ``(wav, List[WordTiming])``, their char spans in `text`.  `best_of`: each segment picks its own
         take (see synthesize; take k of segment i with seed seed + i + k) and the join sees only the picked ones; a
-        group then holds fewer segments when group x best_of rows would exceed the batch limit."""
-        post = OutputChain(self, sample_rate, speed, loudness)
+        group then holds fewer segments when group x best_of rows would exceed the batch limit.  `watermark`: the joined
+        passage carries the key's mark (see synthesize)."""
+        post = OutputChain(self, sample_rate, speed, loudness, watermark)
         n_best = self._check_best_of(best_of, 1)
         LF.check_pause(pause_ms)
         budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
@@ -664,12 +673,12 @@ class SoproTTS:
             yield chunk, self.codec.engine.decode(batch), [Ts[i] * hop for i in chunk]
 
     def stream(self, text: str, *, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-               **kwargs) -> Iterator[torch.Tensor]:
+               watermark: Optional[int] = None, **kwargs) -> Iterator[torch.Tensor]:
         """Chunks of one utterance as they are generated (sopro_b200/streaming.py).  There is no `best_of` here: a
         stream plays its take while it is generated, so it cannot choose among takes before playing one."""
         from .streaming import stream as _stream
 
-        return _stream(self, text, sample_rate=sample_rate, speed=speed, **kwargs)
+        return _stream(self, text, sample_rate=sample_rate, speed=speed, watermark=watermark, **kwargs)
 
     def save_wav(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
         """`sample_rate`: the rate the waveform is at (the one passed to synthesize / stream)."""

@@ -1,6 +1,6 @@
-"""The output chain every synthesis entry point runs on the decoded 24 kHz audio: time-stretch (``speed``), then resample
-(``sample_rate``), then loudness normalisation (``loudness``).  A stage whose argument is a bypass runs nothing and
-allocates nothing.  ``synthesize``, ``synthesize_batch`` and ``synthesize_long`` call the chain on whole rows; ``stream``
+"""The output chain every synthesis entry point runs on the decoded 24 kHz audio: time-stretch (``speed``), then the
+watermark (``watermark``), then resample (``sample_rate``), then loudness normalisation (``loudness``).  A stage whose
+argument is a bypass runs nothing and allocates nothing.  ``synthesize``, ``synthesize_batch`` and ``synthesize_long`` call the chain on whole rows; ``stream``
 feeds each chunk through a per-utterance state of stream states, which concatenates to the one-shot result bit for bit
 (loudness has no streaming form: it needs the whole utterance)."""
 from __future__ import annotations
@@ -12,19 +12,21 @@ import torch
 from .config import TARGET_SR
 from .loudness import check_loudness, normalize_loudness
 from .stretch import check_speed, stretch, stretched_length
+from .watermark import check_watermark, embed_watermark
 
 
 class OutputChain:
     """Built per call from the caller's arguments.  Construction checks them in a fixed order, rate, then speed, then
-    loudness, and raises ValueError for a refused one before any other work (no random draw, nothing read from `tts`
+    loudness, then the watermark key, and raises ValueError for a refused one before any other work (no random draw, nothing read from `tts`
     but its resampler cache).  ``sample_rate``: the rate of the returned audio; ``S``: the stretch's fixed-point speed,
     None on a bypass (word timestamps scale their samples by it)."""
 
     def __init__(self, tts, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                 loudness: Optional[float] = None):
+                 loudness: Optional[float] = None, watermark: Optional[int] = None):
         self.rs = tts._resampler(sample_rate)
         self.S = check_speed(speed)
         self.target = check_loudness(loudness)
+        self.key = check_watermark(watermark)
         self.tts, self.speed = tts, speed
         self.sample_rate = TARGET_SR if self.rs is None else self.rs.sr_out
 
@@ -35,6 +37,8 @@ class OutputChain:
         if self.S is not None:
             wav = stretch(wav, self.speed, lens=lens)
             lens = None if lens is None else [stretched_length(self.speed, n) for n in lens]
+        if self.key is not None:
+            wav = embed_watermark(wav, self.key, lens=lens)
         if self.rs is not None:
             wav = self.rs(wav, lens=lens)
             lens = None if lens is None else [self.rs.length(n) for n in lens]
@@ -48,7 +52,7 @@ class OutputChain:
 
 
 class ChainStream:
-    """One utterance's stretch and resampler stream states, checked out of their pools (none on a bypass) and given
+    """One utterance's stretch, watermark and resampler stream states, checked out of their pools (none on a bypass) and given
     back by ``release``.  Pushes go to a state in pieces of at most max_push samples: a stretch push can yield up to 4x
     its input."""
 
@@ -58,6 +62,9 @@ class ChainStream:
         if chain.S is not None:
             pool = chain.tts._stretch_pool
             self._stages.append((pool.checkout(self.max_push, chain.speed), pool))
+        if chain.key is not None:
+            pool = chain.tts._watermark_pool
+            self._stages.append((pool.checkout(self.max_push, chain.key), pool))
         if chain.rs is not None:
             pool = chain.rs.pool
             self._stages.append((pool.checkout(self.max_push), pool))

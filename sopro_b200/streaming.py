@@ -50,13 +50,14 @@ class SoproTTSStreamer:
                chunk_frames: Optional[int] = None, nar_context_frames: Optional[int] = None,
                min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
                generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
-               speed: Optional[float] = None) -> Iterator[torch.Tensor]:
+               speed: Optional[float] = None, watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
         """`sample_rate` (extension): chunks at this rate (None = 24 kHz).  `speed` (extension): the speaking rate in
-        [0.25, 4.0] (None = the model's own).  Each chunk's audio goes through a time-stretch stream, then a resampler
-        stream, right after its Mimi step, so the chunks concatenate to the one-shot stretch and resample of the 24 kHz
-        stream bit for bit; the last chunk also carries both tails."""
+        [0.25, 4.0] (None = the model's own).  `watermark` (extension): a key in [0, 2^32) to mark the audio with (None =
+        no mark).  Each chunk's audio goes through a time-stretch stream, a watermark stream, then a resampler stream,
+        right after its Mimi step, so the chunks concatenate to the one-shot stretch, mark and resample of the 24 kHz
+        stream bit for bit; the last chunk also carries their tails."""
         tts, model = self.tts, self.tts.model
-        post = OutputChain(tts, sample_rate, speed)  # a refused rate or speed raises before the prefill
+        post = OutputChain(tts, sample_rate, speed, watermark=watermark)  # a refused argument raises before the prefill
         text_ids = tts.encode_text(text)
         if ref is None:
             ref = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
@@ -130,8 +131,8 @@ class SoproTTSStreamer:
 @torch.inference_mode()
 def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
            ref: Optional[PreparedReference] = None, chunk_frames: int = 6, sample_rate: Optional[int] = None,
-           speed: Optional[float] = None, **kwargs) -> Iterator[torch.Tensor]:
-    OutputChain(tts, sample_rate, speed)  # a refused rate or speed raises at the call, not at the first chunk
+           speed: Optional[float] = None, watermark: Optional[int] = None, **kwargs) -> Iterator[torch.Tensor]:
+    OutputChain(tts, sample_rate, speed, watermark=watermark)  # a refused argument raises at the call, not at the first chunk
     streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
     return streamer.stream(text, ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref=ref,
-                           chunk_frames=chunk_frames, sample_rate=sample_rate, speed=speed, **kwargs)
+                           chunk_frames=chunk_frames, sample_rate=sample_rate, speed=speed, watermark=watermark, **kwargs)

@@ -121,13 +121,6 @@ int sopro_ar_session_destroy(sopro_ar_session_t* s);
 /* Launch geometry override (0 = automatic): utterances per CTA team. */
 int sopro_ar_session_set_team(sopro_ar_session_t* s, int utts_per_team);
 
-/* Arithmetic unit of the step's contractions: 0 or -1 = fp32 FMA tiles -- the default and the faster one at
- * the 22..86 weight rows a CTA owns per stage; 1 = tensor cores (wgmma, every fp32 activation split into three exact bf16
- * terms against bf16 weights, fp32 accumulation) or fail when the launch cannot use them (needs bf16 weight storage,
- * d_model % 64 == 0, teams of 5..8 utterances).  -1 also honours the environment variable SOPRO_AR_TC=1.  Both produce the
- * reference's token ids (tests/test_ar_gpu.py). */
-int sopro_ar_session_set_contraction(sopro_ar_session_t* s, int mode);
-
 /* Start `batch` utterances.  Zeroes the rings, builds the text K/V caches on the
  * device (TextXAttnBlock.build_kv_cache, nn/text.py:75-83), resets history.
  *   cond_ar   [batch, steps, D] f32   prep["cond_ar"] rows 0..steps-1 (model.py:272)
@@ -201,10 +194,8 @@ int sopro_ar_debug_sampled(sopro_ar_session_t* s, int32_t* dst, void* stream);
 /* copy the text K/V built by sopro_ar_begin into k_dst / v_dst, each
  * [n_attn_layers, batch, H, Lpad, Dh] f32 (device), Lpad = max_text_len rounded up to 4 */
 int sopro_ar_debug_kv(sopro_ar_session_t* s, float* k_dst, float* v_dst, void* stream);
-/* Host-only views of the operand images the engines build (no device needed): the tensor-core image of an AR step matrix
- * W [N][K] ([K / D slices][groups of 8 rows][D / 64 chunks][8 x 128 B, 16-byte units XOR row]; glu: group = 4 channels, value
- * rows then gate rows) and the NAR refiner's W6 [N][6K] (bf16 terms of the six product pairs mm, lh, hl, mh, hm, hh). */
-int sopro_debug_pack_umma(const float* W, int N, int K, int d_model, int glu, uint8_t* out, int64_t bytes);
+/* Host-only view of an operand image the NAR engine builds (no device needed): W6 [N][6K] of W [N][K] (bf16 terms of the
+ * six product pairs mm, lh, hl, mh, hm, hh). */
 int sopro_debug_pack_w6(const float* W, int N, int K, uint16_t* out);
 /* The kernel's sampler (sample_token, sampling.py:24-93) on ONE logits row, outside the step: HOST buffers; `hist` = the
  * n_hist tokens generated so far (repetition penalty looks at the last 50), `noise` = the Exp(1) draws of this step (first

@@ -156,7 +156,6 @@ SYMBOLS = {
     "sopro_ar_session_create": (_I, [_VP, _I, _I, _I, C.POINTER(_VP)]),
     "sopro_ar_session_destroy": (_I, [_VP]),
     "sopro_ar_session_set_team": (_I, [_VP, _I]),
-    "sopro_ar_session_set_contraction": (_I, [_VP, _I]),
     "sopro_ar_begin": (_I, [_VP, _I, _I, _VP, _VP, _I, _I32P, _VP, _I, C.POINTER(ArSampling), _VP]),
     "sopro_ar_run": (_I, [_VP, _I, _VP]),
     "sopro_ar_outputs": (_I, [_VP, C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP)]),
@@ -172,7 +171,6 @@ SYMBOLS = {
     "sopro_noise_create": (_I, [C.c_uint64, _VP]),
     "sopro_noise_rows": (_I, [_VP, _I, _I, _I, _VP]),
     "sopro_noise_destroy": (_I, [_VP]),
-    "sopro_debug_pack_umma": (_I, [_VP, _I, _I, _I, _I, _VP, C.c_int64]),
     "sopro_debug_pack_w6": (_I, [_VP, _I, _I, _VP]),
     "sopro_debug_sample": (_I, [_VP, _I, _VP, _I, _VP, _I, _VP, _I, _I, _VP]),
     "sopro_mimi_create": (_I, [C.POINTER(MimiConfigC), C.POINTER(MimiWeights), _I, C.POINTER(_VP)]),

@@ -30,31 +30,6 @@ uint16_t f32_to_bf16_rne(float f) {
 
 struct Arena {
   std::vector<unsigned char> host;
-  // Tensor-core operand IMAGE of W[N][K] (bf16): what wgmma reads from shared memory after a plain 1-D bulk copy.
-  //   [K / D slices][G groups of 8 rows][D / 64 chunks][8 rows x 128 B], 16-byte unit j of row r stored at unit j ^ r
-  //   (128-byte swizzle, K-major).  glu: group g = channels 4g..4g+3, rows 0..3 their value rows, 4..7 their gate rows.
-  size_t add_packed(const float* src, int N, int K, int D, bool glu, int* groups_out) {
-    const int G = glu ? D / 4 : (N + 7) / 8, S = K / D, KSC = D / 64;
-    const size_t off = add((size_t)S * G * KSC * 1024);
-    unsigned char* base = host.data() + off;
-    memset(base, 0, (size_t)S * G * KSC * 1024);
-    for (int sl = 0; sl < S; ++sl)
-      for (int g = 0; g < G; ++g)
-        for (int rr = 0; rr < 8; ++rr) {
-          const int row = glu ? (rr < 4 ? 4 * g + rr : D + 4 * g + (rr - 4)) : 8 * g + rr;
-          if (row >= N) continue;
-          for (int c = 0; c < KSC; ++c) {
-            unsigned char* blk = base + (((size_t)sl * G + g) * KSC + c) * 1024 + (size_t)rr * 128;
-            for (int j = 0; j < 8; ++j) {
-              uint16_t* d = reinterpret_cast<uint16_t*>(blk + ((j ^ rr) << 4));
-              const float* sp = src + (size_t)row * K + (size_t)sl * D + c * 64 + j * 8;
-              for (int e = 0; e < 8; ++e) d[e] = f32_to_bf16_rne(sp[e]);
-            }
-          }
-        }
-    *groups_out = G;
-    return off;
-  }
   size_t add(size_t bytes) {
     const size_t off = align_up(host.size(), 256);
     host.resize(off + bytes);
@@ -99,20 +74,12 @@ struct sopro_engine {
   const float* epi[kMaxLayers]{};  // packed [D][KcE]: dwconv taps, dwconv bias, GLU value bias, GLU gate bias
   int KcP = 0, KcE = 0;
   long long ring_floats_per_utt = 0;
-  // tensor-core operand images of the step matrices (bf16 engines with D % 64 == 0; null otherwise)
-  bool tc_ok = false;
-  const unsigned char* tc_glu[kMaxLayers]{};
-  const unsigned char* tc_w1[kMaxLayers]{};
-  const unsigned char* tc_w2[kMaxLayers]{};
-  const unsigned char* tc_wo[kMaxLayers]{};
-  const unsigned char* tc_head = nullptr;
 };
 
 struct sopro_ar_session {
   sopro_engine* e = nullptr;
   int max_batch = 0, max_steps = 0, Lmax = 0;
   int utts_per_team = 0;  // 0 = auto
-  int tc_mode = -1;       // -1 auto, 0 FMA path, 1 tensor cores required
   // device buffers
   float *ring = nullptr, *xa = nullptr, *xb = nullptr, *hbuf = nullptr, *qbuf = nullptr, *abuf = nullptr,
         *logits = nullptr, *kc = nullptr, *vc = nullptr;
@@ -126,7 +93,7 @@ struct sopro_ar_session {
   int* n_tiles = nullptr;     // [n_sms]
   unsigned char* stage_tiles = nullptr;  // [n_sms][kMaxStages]
   std::vector<unsigned char> h_stage_tiles;
-  int tile_P = -1, tile_wbuf = -1, tile_qatt = -1, tile_tc = -1;
+  int tile_P = -1, tile_wbuf = -1, tile_qatt = -1;
   bool qatt = false;  // this launch geometry uses the fused q + attention stage
   std::vector<TileDesc> h_tiles;
   std::vector<int> h_ntiles;
@@ -269,23 +236,6 @@ int sopro_engine_create(const sopro_ar_config_t* cfg, const sopro_ar_weights_t* 
   const size_t off_emb = A.add((size_t)(V + 1) * D * 4);
   memcpy(A.host.data() + off_emb, w->cb_embed, (size_t)V * D * 4);
   memcpy(A.host.data() + off_emb + (size_t)V * D * 4, w->cb_embed + (size_t)w->bos_row * D, (size_t)D * 4);
-  // second copy of the step matrices as tensor-core operand images (batched launches, DESIGN.md §3)
-  struct TcOff {
-    size_t glu, w1, w2, wo;
-  } tco[kMaxLayers];
-  size_t tco_head = 0;
-  const bool tc_ok = wd == SOPRO_W_BF16 && D % 64 == 0 && D % 8 == 0;
-  if (tc_ok) {
-    int G = 0;
-    for (int i = 0; i < NL; ++i) {
-      const sopro_ar_layer_weights_t& L = w->layer[i];
-      tco[i].glu = A.add_packed(L.glu_w, 2 * D, D, D, true, &G);
-      tco[i].w1 = A.add_packed(L.ffn_w1, 4 * D, D, D, false, &G);
-      tco[i].w2 = A.add_packed(L.ffn_w2, D, 4 * D, D, false, &G);
-      tco[i].wo = cfg->has_attn[i] ? A.add_packed(L.o_w, D, D, D, false, &G) : 0;
-    }
-    tco_head = A.add_packed(w->head_w, V, D, D, false, &G);
-  }
 
   e->dev_bytes = align_up(A.host.size(), 256);
   cudaError_t err = cudaMalloc(&e->dev, e->dev_bytes);
@@ -330,16 +280,6 @@ int sopro_engine_create(const sopro_ar_config_t* cfg, const sopro_ar_weights_t* 
       ++n_attn;
     }
     ring_off += (long long)D * L.dil * e->KcP;  // conv state per utterance: [D][dil][KcP]
-  }
-  e->tc_ok = tc_ok;
-  if (tc_ok) {
-    for (int i = 0; i < NL; ++i) {
-      e->tc_glu[i] = e->dev + tco[i].glu;
-      e->tc_w1[i] = e->dev + tco[i].w1;
-      e->tc_w2[i] = e->dev + tco[i].w2;
-      e->tc_wo[i] = cfg->has_attn[i] ? e->dev + tco[i].wo : nullptr;
-    }
-    e->tc_head = e->dev + tco_head;
   }
   e->n_attn = n_attn;
   e->ring_floats_per_utt = ring_off;
@@ -457,25 +397,6 @@ int sopro_ar_session_set_team(sopro_ar_session_t* s, int utts_per_team) {
   if (utts_per_team < 0 || utts_per_team > kMaxUttPerTeam)
     return fail(SOPRO_ERR_INVALID, "utts_per_team must be in [0,%d]", kMaxUttPerTeam);
   s->utts_per_team = utts_per_team;
-  return SOPRO_OK;
-}
-
-// test hook (host only): the tensor-core operand image of W [N][K] (see Arena::add_packed) -> out, `bytes` = its size
-int sopro_debug_pack_umma(const float* W, int N, int K, int D, int glu, uint8_t* out, int64_t bytes) {
-  if (!W || !out || N < 1 || K < 1 || D < 64 || D % 64 || K % D) return fail(SOPRO_ERR_INVALID, "bad argument");
-  Arena A;
-  int G = 0;
-  const size_t off = A.add_packed(W, N, K, D, glu != 0, &G);
-  const size_t need = (size_t)(K / D) * G * (D / 64) * 1024;
-  if ((int64_t)need != bytes) return fail(SOPRO_ERR_INVALID, "image is %zu bytes, caller expects %lld", need, (long long)bytes);
-  memcpy(out, A.host.data() + off, need);
-  return SOPRO_OK;
-}
-
-int sopro_ar_session_set_contraction(sopro_ar_session_t* s, int mode) {
-  if (!s) return fail(SOPRO_ERR_INVALID, "null session");
-  if (mode < -1 || mode > 1) return fail(SOPRO_ERR_INVALID, "contraction mode must be -1, 0 or 1");
-  s->tc_mode = mode;
   return SOPRO_OK;
 }
 
@@ -617,7 +538,6 @@ struct StageW {
   int N, K, parts;    // parts = 2 for the GLU (value rows + gate rows of the same channels)
   const float* epi;   // GLU: packed [D][KcE] epilogue rows; else the bias vector [N] (or null)
   bool by_head;       // fused q + attention stage: rank r gets ALL rows of head r % H (ranks >= H * (P / H): none)
-  const unsigned char* packed;  // tensor-core operand image of the matrix (null: row-major FMA tiles)
 };
 
 // the fused q-projection + attention stage needs at least one CTA per head
@@ -626,92 +546,35 @@ static bool use_qatt(const sopro_engine* e, int P) {
   return !off && P >= e->H;
 }
 
-static int build_tiles(sopro_ar_session* s, int P, int wbuf, bool tc, cudaStream_t st) {
+static int build_tiles(sopro_ar_session* s, int P, int wbuf, cudaStream_t st) {
   sopro_engine* e = s->e;
   const bool qatt = s->qatt;
-  if (s->tile_P == P && s->tile_wbuf == wbuf && s->tile_qatt == (int)qatt && s->tile_tc == (int)tc) return SOPRO_OK;
+  if (s->tile_P == P && s->tile_wbuf == wbuf && s->tile_qatt == (int)qatt) return SOPRO_OK;
   const size_t wsz = e->cfg.weight_dtype == SOPRO_W_F32 ? 4 : 2;
   std::vector<StageW> prog;
   int si = 0;  // must mirror the stage program built in launch_ar
   for (int i = 0; i < e->n_layers; ++i) {
     const LayerDev& L = e->layer[i];
-    prog.push_back({si++, L.glu_w, e->D, e->D, 2, e->epi[i], false, tc ? e->tc_glu[i] : nullptr});
-    prog.push_back({si++, L.w1, e->F, e->D, 1, L.b1, false, tc ? e->tc_w1[i] : nullptr});
-    prog.push_back({si++, L.w2, e->D, e->F, 1, L.b2, false, tc ? e->tc_w2[i] : nullptr});
+    prog.push_back({si++, L.glu_w, e->D, e->D, 2, e->epi[i], false});
+    prog.push_back({si++, L.w1, e->F, e->D, 1, L.b1, false});
+    prog.push_back({si++, L.w2, e->D, e->F, 1, L.b2, false});
     if (L.has_attn) {
       if (qatt) {
-        prog.push_back({si++, L.wq, e->D, e->D, 1, nullptr, true, nullptr});
+        prog.push_back({si++, L.wq, e->D, e->D, 1, nullptr, true});
       } else {
-        prog.push_back({si++, L.wq, e->D, e->D, 1, nullptr, false, nullptr});
+        prog.push_back({si++, L.wq, e->D, e->D, 1, nullptr, false});
         si++;  // attention core: no weights
       }
-      prog.push_back({si++, L.wo, e->D, e->D, 1, nullptr, false, tc ? e->tc_wo[i] : nullptr});
+      prog.push_back({si++, L.wo, e->D, e->D, 1, nullptr, false});
     }
   }
-  prog.push_back({si++, e->head_w, e->V, e->D, 1, e->head_b, false, tc ? e->tc_head : nullptr});
+  prog.push_back({si++, e->head_w, e->V, e->D, 1, e->head_b, false});
   s->h_stage_tiles.assign((size_t)P * kMaxStages, 0);
   s->h_tiles.assign((size_t)P * kMaxTilesPerStep, TileDesc{});
   s->h_ntiles.assign(P, 0);
-  const int KSC = e->D / 64;  // 64-wide K chunks per K slice of the tensor-core images
   for (int r = 0; r < P; ++r) {
     int n = 0;
     for (const StageW& sw : prog) {
-      if (sw.packed) {
-        // ---- tensor-core tiles.  Outputs are dealt to the ranks in units of 8 rows (GLU: 8 channels = 2 groups of 4), a
-        // tile = consecutive 8-row groups of one K slice (contiguous in the image: one bulk copy), at most 16 groups
-        // (the instruction reads 128 rows) and what fits a ring buffer with its epilogue constants.
-        const bool glu = sw.parts == 2;
-        const int units = glu ? e->D / 8 : (sw.N + 7) / 8;
-        const int u0 = (int)(((long long)units * r) / P), u1 = (int)(((long long)units * (r + 1)) / P);
-        const int g0 = glu ? 2 * u0 : u0, g1 = glu ? 2 * u1 : u1;
-        const int G = glu ? e->D / 4 : (sw.N + 7) / 8, S = sw.K / e->D;
-        const size_t gbytes = (size_t)KSC * 1024;
-        const size_t epi_g = glu ? (size_t)4 * e->KcE * 4 : 32;
-        const int gmax = (int)std::min<size_t>(8, ((size_t)wbuf - 64) / (gbytes + epi_g));  // M = 64: at most 8 groups
-        if (gmax < 1) return fail(SOPRO_ERR_INVALID, "weight buffer %d B cannot hold one 8-row group (%zu B)", wbuf, gbytes);
-        const int ng = g1 - g0;
-        const int ntile = (ng + gmax - 1) / gmax;
-        for (int it = 0, ga = g0; it < ntile; ++it) {
-          const int per = (g1 - ga + (ntile - it) - 1) / (ntile - it);
-          // two K slices of the same rows share a tile when they fit (parts 0 and 1: the image keeps slices apart)
-          const int spt = (S > 1 && 2 * ((size_t)per * gbytes) + (size_t)per * epi_g + 64 <= (size_t)wbuf) ? 2 : 1;
-          for (int sl = 0; sl < S; sl += spt) {
-            if (n >= kMaxTilesPerStep) return fail(SOPRO_ERR_INVALID, "more than %d weight tiles per step (P=%d, wbuf=%d)", kMaxTilesPerStep, P, wbuf);
-            TileDesc& t = s->h_tiles[(size_t)r * kMaxTilesPerStep + n++];
-            t.src0 = reinterpret_cast<unsigned long long>(sw.packed + (((size_t)sl * G + ga) * KSC) * 1024);
-            t.bytes0 = (unsigned)((size_t)per * gbytes);
-            const bool two = spt == 2 && sl + 1 < S;
-            t.src1 = two ? reinterpret_cast<unsigned long long>(sw.packed + (((size_t)(sl + 1) * G + ga) * KSC) * 1024) : 0ull;
-            t.bytes1 = two ? t.bytes0 : 0u;
-            t.ngrp = per;
-            t.kc0 = sl * KSC;
-            t.flags = (sl == 0 ? 1 : 0) | (sl + (two ? 2 : 1) >= S ? 2 : 0);
-            if (glu) {
-              t.row0 = 4 * ga;
-              t.nrows = 4 * per;
-              t.src2 = reinterpret_cast<unsigned long long>(sw.epi + (size_t)t.row0 * e->KcE);
-              t.bytes2 = (unsigned)((size_t)t.nrows * e->KcE * 4);
-              t.off2 = 0;
-            } else {
-              t.row0 = 8 * ga;
-              t.nrows = std::min(sw.N - t.row0, 8 * per);
-              t.src2 = 0;
-              t.bytes2 = 0;
-              t.off2 = 0;
-              if (sw.epi) {
-                const int lo = t.row0 / 4 * 4, hi = (t.row0 + t.nrows + 3) / 4 * 4;
-                t.src2 = reinterpret_cast<unsigned long long>(sw.epi + lo);
-                t.bytes2 = (unsigned)((hi - lo) * 4);
-                t.off2 = t.row0 - lo;
-              }
-            }
-            if (++s->h_stage_tiles[(size_t)r * kMaxStages + sw.stage] == 255)
-              return fail(SOPRO_ERR_INVALID, "more than 254 weight tiles in one stage");
-          }
-          ga += per;
-        }
-        continue;
-      }
       int n0 = (int)(((long long)sw.N * r) / P), n1 = (int)(((long long)sw.N * (r + 1)) / P);
       if (sw.by_head) {
         const int PH = P / e->H;
@@ -746,9 +609,6 @@ static int build_tiles(sopro_ar_session* s, int P, int wbuf, bool tc, cudaStream
         }
         t.row0 = a;
         t.nrows = nr;
-        t.ngrp = 0;
-        t.kc0 = 0;
-        t.flags = 3;
         if (++s->h_stage_tiles[(size_t)r * kMaxStages + sw.stage] == 255)
           return fail(SOPRO_ERR_INVALID, "more than 254 weight tiles in one stage");
       }
@@ -761,14 +621,13 @@ static int build_tiles(sopro_ar_session* s, int P, int wbuf, bool tc, cudaStream
   s->tile_P = P;
   s->tile_wbuf = wbuf;
   s->tile_qatt = (int)qatt;
-  s->tile_tc = (int)tc;
   return SOPRO_OK;
 }
 
-template <typename WT, int TU, bool LL, bool TC = false>
+template <typename WT, int TU, bool LL>
 static int launch_ar_tu(sopro_ar_session* s, ArParams& p, size_t smem, int grid, cudaStream_t st) {
   // the attention-trace export is its own instantiation, so the untraced kernel's code is not touched by it
-  auto kern = p.attn_trace ? ar_persistent_kernel<WT, TU, LL, TC, true> : ar_persistent_kernel<WT, TU, LL, TC, false>;
+  auto kern = p.attn_trace ? ar_persistent_kernel<WT, TU, LL, true> : ar_persistent_kernel<WT, TU, LL, false>;
   CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem));
@@ -865,13 +724,6 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   p.Bt = Bt;
   p.t_begin = t_begin;
   p.t_end = t_end;
-  // ---- tensor cores for the contractions?  Needs bf16 weight storage, an engine with operand images, teams of 5..8
-  // utterances (one 8-utterance B operand) and the fused q + attention stage (Wq stays on the FMA path).  OPT-IN
-  // (sopro_ar_session_set_contraction(1) or SOPRO_AR_TC=1): exact, but not the default -- a CTA owns only 22..86 weight
-  // rows per stage, so most of every 64-row instruction is idle work and the operand-building stage-in is extra.
-  static const int tc_env = getenv("SOPRO_AR_TC") ? atoi(getenv("SOPRO_AR_TC")) : -1;
-  const bool tc_want = s->tc_mode == 1 || (s->tc_mode == -1 && tc_env == 1);
-  bool tc = tc_want && e->tc_ok && Bt >= 5 && Bt <= 8 && use_qatt(e, P);
   const size_t kSmemCap = 213 * 1024;  // 227 KB minus static shared memory (sampler scratch, mbarriers) and alignment slack
   const size_t table_bytes = (size_t)kMaxTilesPerStep * sizeof(TileDesc);
   const size_t wsz = e->cfg.weight_dtype == SOPRO_W_F32 ? 4 : 2;
@@ -881,75 +733,47 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   size_t act_bytes = 0, wbuf = 0;
   int nbuf = 0, PH = 1;
   bool qatt = use_qatt(e, P);
-  if (tc) {
-    // [ring | B operand (F / 64 chunks of 4 KB; the K = D stages use the first D / 64, their fp32 staging rows and the
-    //  dwconv tap scratch sit behind those) | tile table]
-    const size_t ksc = (size_t)e->D / 64;
-    const size_t bt_full = (size_t)(e->F / 64) * 4096;
-    const size_t glu_need = ksc * 4096 + (size_t)2 * Bt * e->D * 4 + (size_t)64 * 8 * e->KcP * 4;
-    PH = P / e->H;
-    const size_t need_att = need_att_base + (size_t)((Bt + PH - 1) / PH) * (e->D + e->Dh) * 4;
-    // + the accumulator scratch at the end of the region
-    act_bytes = align_up(std::max(std::max(bt_full, glu_need), std::max(need_att, need_smp)), 1024) + kTcDBytes;
-    if (act_bytes + table_bytes + 3 * 8192 > kSmemCap) {
-      tc = false;
-    } else {
-      const size_t avail = kSmemCap - act_bytes - table_bytes;
-      nbuf = 2;
-      wbuf = (avail / nbuf) / 1024 * 1024;
-      if (wbuf < ksc * 1024 + 1024 || (size_t)e->Dh * e->D * wsz + 64 > (size_t)nbuf * wbuf) tc = false;
-      // the instruction reads 8 groups from a tile's start: that span must stay inside the allocation
-      if (tc && (size_t)(nbuf - 1) * wbuf + 8 * ksc * 1024 > (size_t)nbuf * wbuf + act_bytes) tc = false;
-      // the one-pass stage-in of the normalised stages holds 3 element pairs per thread
-      if ((size_t)8 * e->D > (size_t)3 * kThreads * 2) tc = false;
-    }
-  }
-  if (!tc) {
-    const size_t need_act = std::max((size_t)Bt * e->F * 4, (size_t)2 * Bt * e->D * 4 + (size_t)kWarps * kTapSlots * e->KcP * 4);
-    auto slice_bytes = [&](int N, int K, int parts) {
-      const size_t rows = (size_t)((N + P - 1) / P);
-      return rows * K * wsz * parts + (parts == 2 ? rows * e->KcE * 4 : rows * 4) + 32;
-    };
-    size_t full = std::max(std::max(slice_bytes(e->D, e->D, 2), slice_bytes(e->F, e->D, 1)),
-                           std::max(slice_bytes(e->D, e->F, 1), slice_bytes(e->V, e->D, 1)));
-    full = align_up(full, 128);
-    // The fused q + attention stage (one exchange and one GEMV stage fewer per attention layer) streams a whole head's
-    // Wq rows through every serving CTA: taken when that head tile fits at most two ring buffers (batched launches); a
-    // batch-1 launch, whose CTAs (one per SM) hold slivers of every matrix, keeps the q stage spread over all CTAs.
-    for (;;) {
-      size_t need_att = need_att_base;
-      PH = qatt ? P / e->H : 1;
-      if (qatt) need_att += (size_t)((Bt + PH - 1) / PH) * (e->D + e->Dh) * 4;  // + the fused stage's x rows and q rows
-      act_bytes = align_up(std::max(need_act, std::max(need_att, need_smp)), 128);
-      if (act_bytes + table_bytes + 2 * 4096 > kSmemCap) {
-        if (qatt) {
-          qatt = false;
-          continue;
-        }
-        return fail(SOPRO_ERR_INVALID, "shared memory: activations need %zu B (Bt=%d, Lmax=%d), nothing left for weights",
-                    act_bytes, Bt, s->Lmax);
-      }
-      const size_t avail = kSmemCap - act_bytes - table_bytes;
-      if (2 * full <= avail) {
-        wbuf = full;
-        nbuf = (int)std::min<size_t>(kMaxWBuf, avail / wbuf);
-      } else {
-        wbuf = (avail / 2) / 128 * 128;
-        nbuf = 2;
-      }
-      if (qatt && (size_t)e->Dh * e->D * wsz + 64 > 2 * wbuf) {
+  const size_t need_act = std::max((size_t)Bt * e->F * 4, (size_t)2 * Bt * e->D * 4 + (size_t)kWarps * kTapSlots * e->KcP * 4);
+  auto slice_bytes = [&](int N, int K, int parts) {
+    const size_t rows = (size_t)((N + P - 1) / P);
+    return rows * K * wsz * parts + (parts == 2 ? rows * e->KcE * 4 : rows * 4) + 32;
+  };
+  size_t full = std::max(std::max(slice_bytes(e->D, e->D, 2), slice_bytes(e->F, e->D, 1)),
+                         std::max(slice_bytes(e->D, e->F, 1), slice_bytes(e->V, e->D, 1)));
+  full = align_up(full, 128);
+  // The fused q + attention stage (one exchange and one GEMV stage fewer per attention layer) streams a whole head's
+  // Wq rows through every serving CTA: taken when that head tile fits at most two ring buffers (batched launches); a
+  // batch-1 launch, whose CTAs (one per SM) hold slivers of every matrix, keeps the q stage spread over all CTAs.
+  for (;;) {
+    size_t need_att = need_att_base;
+    PH = qatt ? P / e->H : 1;
+    if (qatt) need_att += (size_t)((Bt + PH - 1) / PH) * (e->D + e->Dh) * 4;  // + the fused stage's x rows and q rows
+    act_bytes = align_up(std::max(need_act, std::max(need_att, need_smp)), 128);
+    if (act_bytes + table_bytes + 2 * 4096 > kSmemCap) {
+      if (qatt) {
         qatt = false;
         continue;
       }
-      break;
+      return fail(SOPRO_ERR_INVALID, "shared memory: activations need %zu B (Bt=%d, Lmax=%d), nothing left for weights",
+                  act_bytes, Bt, s->Lmax);
     }
+    const size_t avail = kSmemCap - act_bytes - table_bytes;
+    if (2 * full <= avail) {
+      wbuf = full;
+      nbuf = (int)std::min<size_t>(kMaxWBuf, avail / wbuf);
+    } else {
+      wbuf = (avail / 2) / 128 * 128;
+      nbuf = 2;
+    }
+    if (qatt && (size_t)e->Dh * e->D * wsz + 64 > 2 * wbuf) {
+      qatt = false;
+      continue;
+    }
+    break;
   }
-  if (s->tc_mode == 1 && !tc)
-    return fail(SOPRO_ERR_INVALID, "tensor-core contraction requested but this launch cannot use it (bf16 weights, d_model %% 64 == 0, "
-                                   "teams of 5..8 utterances: Bt=%d, P=%d)", Bt, P);
   p.PH = PH;
   s->qatt = qatt;
-  int rc = build_tiles(s, P, (int)wbuf, tc, st);
+  int rc = build_tiles(s, P, (int)wbuf, st);
   if (rc != SOPRO_OK) return rc;
   p.tiles = s->tiles;
   p.n_tiles = s->n_tiles;
@@ -957,17 +781,8 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   p.nbuf = nbuf;
   p.wbuf_bytes = (int)wbuf;
   p.act_bytes = (int)act_bytes;
-  p.tc = tc ? 1 : 0;
-  p.ksc = e->D / 64;
-  if (tc) {
-    p.ring_off = 0;
-    p.act_off = (int)((size_t)nbuf * wbuf);
-    p.table_off = (int)((size_t)nbuf * wbuf + act_bytes);
-  } else {
-    p.act_off = 0;
-    p.ring_off = (int)act_bytes;
-    p.table_off = (int)(act_bytes + (size_t)nbuf * wbuf);
-  }
+  p.ring_off = (int)act_bytes;
+  p.table_off = (int)(act_bytes + (size_t)nbuf * wbuf);
   const size_t smem = act_bytes + (size_t)nbuf * wbuf + table_bytes + 1024;  // + slack for the 1024-byte alignment
   // ---- stage program of one step
   {
@@ -998,9 +813,6 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   bool ll = Bt <= 8;
   if (sync_env && strcmp(sync_env, "barrier") == 0) ll = false;
   if (sync_env && strcmp(sync_env, "ll") == 0) ll = true;
-  if constexpr (sizeof(WT) == 2) {
-    if (tc) return ll ? launch_ar_tu<WT, 8, true, true>(s, p, smem, grid, st) : launch_ar_tu<WT, 8, false, true>(s, p, smem, grid, st);
-  }
   if (ll) {
     if (Bt >= 8) return launch_ar_tu<WT, 8, true>(s, p, smem, grid, st);
     if (Bt >= 4) return launch_ar_tu<WT, 4, true>(s, p, smem, grid, st);

@@ -28,8 +28,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "wgmma.cuh"
-
 namespace sopro {
 
 constexpr int kThreads = 512;
@@ -40,7 +38,7 @@ constexpr int kCand = 128;  // candidate slots of the sampler's top-k
 constexpr int kMaxUttPerTeam = 32;
 constexpr int kMaxVocab = 8 * kThreads;
 constexpr int kTapSlots = 16;     // dwconv tap rows staged per warp in the GLU stage (channels per task x utterances)
-constexpr int kTimingSlots = 224;  // [0,160) stage stamps, [160,192) sampler phases, [192,224) attention phases
+constexpr int kTimingSlots = 224;  // [0,160) stage stamps, [160,192) sampler phases, the rest spare
 constexpr int kMaxStages = 6 * kMaxLayers + 2;
 constexpr int kMaxTilesPerStep = 128;
 constexpr int kMaxWBuf = 8;
@@ -98,10 +96,9 @@ struct TileDesc {
   int off2;                 // float index of the tile's first row inside part 2
   int row0;                 // first output feature of the tile
   int nrows;
-  int ngrp;                 // tensor-core tiles: 8-row groups in part 0 (0 = row-major tile of the FMA path)
-  int kc0;                  // tensor-core tiles: first 64-wide K chunk of the B operand this tile contracts with
-  int flags;                // tensor-core tiles: bit 0 = first K slice of its rows (accumulator reset), bit 1 = last (epilogue)
+  int pad[4];               // 64 bytes per tile: the shared-memory table is 8 KB, and the weight ring gets what it leaves
 };
+static_assert(sizeof(TileDesc) == 64, "the weight ring is sized around an 8 KB tile table");
 
 struct StageOp {
   unsigned char kind, layer;
@@ -146,11 +143,8 @@ struct ArParams {
   const int* n_tiles;     // [P] tiles per step of each rank
   const unsigned char* stage_tiles;  // [P][kMaxStages] tiles of each stage
   int nbuf, wbuf_bytes, act_bytes;
-  // dynamic shared-memory map (bytes from the 1024-byte aligned base): FMA path [act | ring | table]; tensor-core
-  // path [ring | B operand + staging | table]
-  int act_off, ring_off, table_off;
-  int tc;   // 1: the GEMV stages contract on the tensor cores (wgmma; bf16 weights, teams of <= 8 utterances)
-  int ksc;  // tensor-core path: 64-wide K chunks per K slice (= D / 64); a [.. x F] matrix is F / D slices
+  // dynamic shared-memory map [act | ring | table]: bytes from the 1024-byte aligned base (act is at 0)
+  int ring_off, table_off;
   long long* timing;  // debug: [grid][kTimingSlots] clock64 stamps of step `timing_step` (null = off)
   int timing_step;
   int g, P, Bt;
@@ -339,151 +333,6 @@ __device__ __forceinline__ float4 ldsw4<__nv_bfloat16>(unsigned a) {
   r.z = __uint_as_float(y << 16);
   r.w = __uint_as_float(y & 0xffff0000u);
   return r;
-}
-
-// ---------------------------------------------------------------------------
-// Tensor-core (wgmma) contraction of the batched launches (bf16 weight storage, teams of <= 8 utterances).
-//   D[64 rows x 32] (+)= A[64 x 16] . B[32 x 16]^T per instruction, fp32 accumulation in the registers of warpgroup 0.
-//   A = this CTA's weight rows: the host stores them as the shared-memory IMAGE the tensor core reads (K-major,
-//       128-byte swizzle, 8-row groups of [K chunks][8 x 128 B]; group stride = SBO), so the 1-D TMA bulk copy of the
-//       weight ring delivers a ready operand.  A tile has <= 8 groups; the instruction always reads 64 rows, the rows
-//       past the tile are whatever follows in shared memory and only reach accumulator rows nobody reads.
-//   B = the team's activations, each fp32 value split into THREE bf16 terms x = hi + mid + lo (exact: 3 x 8 mantissa
-//       bits): B row 4u + s holds term s of utterance u (row 4u + 3 is zero).  bf16 x bf16 products are exact in fp32,
-//       so D column 4u+0..2 summed = sum_k w[k] * x[k] with fp32 accumulation -- the same arithmetic as the FMA path
-//       up to the order of the fp32 additions.
-//   The finished accumulator goes through a [64][kTcDPitch] fp32 scratch in shared memory (behind the activation
-//   region) to the epilogue threads, one (row, two utterances) per thread.
-// ---------------------------------------------------------------------------
-constexpr int kTcCols = 32;            // B rows = accumulator columns of one instruction
-constexpr int kTcBChunk = 32 * 128;    // bytes of one 64-wide K chunk of the B operand
-constexpr int kTcDPitch = kTcCols + 1;  // accumulator scratch row pitch (floats)
-constexpr int kTcDBytes = 9 * 1024;     // accumulator scratch, 1024-byte multiple
-static_assert(64 * kTcDPitch * 4 <= kTcDBytes, "accumulator scratch");
-// shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups `sbo` bytes apart
-__device__ __forceinline__ unsigned long long tc_desc(unsigned addr, unsigned sbo) { return wg::desc_sw128(addr, sbo); }
-__device__ __forceinline__ void sts128(unsigned a, unsigned x, unsigned y, unsigned z, unsigned w) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
-}
-// 8 consecutive k of utterance u (K-chunk `chunk`, 16-byte unit `unit`) -> the three bf16 terms, stored swizzled
-__device__ __forceinline__ void tc_store_split8(unsigned bt, int u, int chunk, int unit, const float (&x)[8]) {
-  unsigned hi[4], mi[4], lo[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const float a = x[2 * e], b = x[2 * e + 1];
-    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    const float ra = a - __low2float(h), rb = b - __high2float(h);
-    const __nv_bfloat162 m = __floats2bfloat162_rn(ra, rb);
-    const __nv_bfloat162 l = __floats2bfloat162_rn(ra - __low2float(m), rb - __high2float(m));
-    hi[e] = *reinterpret_cast<const unsigned*>(&h);
-    mi[e] = *reinterpret_cast<const unsigned*>(&m);
-    lo[e] = *reinterpret_cast<const unsigned*>(&l);
-  }
-  // B row n = 4u + s: 8-row group n >> 3, row r = n & 7 of the group; 16-byte unit index XOR r (128-byte swizzle)
-  const int n0 = 4 * u, r0 = n0 & 7;
-  const unsigned base = bt + (unsigned)chunk * (unsigned)kTcBChunk + (unsigned)(n0 >> 3) * 1024u;
-  sts128(base + (unsigned)(r0 + 0) * 128u + (unsigned)((unit ^ (r0 + 0)) << 4), hi[0], hi[1], hi[2], hi[3]);
-  sts128(base + (unsigned)(r0 + 1) * 128u + (unsigned)((unit ^ (r0 + 1)) << 4), mi[0], mi[1], mi[2], mi[3]);
-  sts128(base + (unsigned)(r0 + 2) * 128u + (unsigned)((unit ^ (r0 + 2)) << 4), lo[0], lo[1], lo[2], lo[3]);
-  sts128(base + (unsigned)(r0 + 3) * 128u + (unsigned)((unit ^ (r0 + 3)) << 4), 0u, 0u, 0u, 0u);
-}
-// B operand from fp32 rows in shared memory ([nb][K], already normalised)
-__device__ __forceinline__ void tc_btile_from_rows(const float* __restrict__ rows, int nb, int K, unsigned bt) {
-  const int upr = K >> 3;  // 16-byte units per row
-  for (int idx = threadIdx.x; idx < nb * upr; idx += kThreads) {
-    const int u = idx / upr, j8 = idx - u * upr;
-    const float4 a = *reinterpret_cast<const float4*>(rows + (size_t)u * K + j8 * 8);
-    const float4 b = *reinterpret_cast<const float4*>(rows + (size_t)u * K + j8 * 8 + 4);
-    const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    tc_store_split8(bt, u, j8 >> 3, j8 & 7, x);
-  }
-}
-// One 4-byte word (k, k+1 of one split term) of B row n: chunk k / 64, 16-byte unit (k % 64) / 8 XOR (n & 7)
-__device__ __forceinline__ unsigned tc_b_word_addr(unsigned bt, int n, int k) {
-  const int r = n & 7;
-  return bt + (unsigned)(k >> 6) * (unsigned)kTcBChunk + (unsigned)(n >> 3) * 1024u + (unsigned)r * 128u +
-         (unsigned)(((((k & 63) >> 3) ^ r) << 4) + ((k & 7) << 1));
-}
-__device__ __forceinline__ void sts32(unsigned a, unsigned v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-// two consecutive elements (k even) of utterance u -> the three bf16 terms + the zero row: four conflict-free 4-byte stores
-// (a warp's 64 consecutive k fill one 128-byte row of the operand per term)
-__device__ __forceinline__ void tc_store_split2(unsigned bt, int u, int k, float a, float b) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  const float ra = a - __low2float(h), rb = b - __high2float(h);
-  const __nv_bfloat162 m = __floats2bfloat162_rn(ra, rb);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(ra - __low2float(m), rb - __high2float(m));
-  sts32(tc_b_word_addr(bt, 4 * u + 0, k), *reinterpret_cast<const unsigned*>(&h));
-  sts32(tc_b_word_addr(bt, 4 * u + 1, k), *reinterpret_cast<const unsigned*>(&m));
-  sts32(tc_b_word_addr(bt, 4 * u + 2, k), *reinterpret_cast<const unsigned*>(&l));
-  sts32(tc_b_word_addr(bt, 4 * u + 3, k), 0u);
-}
-// Stage-in of the tensor-core path in ONE pass over the exchange buffer: every thread polls (LL) / loads its element pairs
-// with coalesced 16-byte requests, all in flight; with a norm weight the rows' sums of squares meet through a
-// [row][K / 64] table of warp partials (summed in a fixed order) and one block barrier; then each thread normalises,
-// splits and stores its own pairs into the B operand.  No fp32 staging copy of the activations.
-//   raw_copy: un-normalised rows as plain floats (the GLU stage's residual operand), or null
-//   part:     shared [kMaxUttPerTeam * 32] floats
-template <bool LL, int NJ>
-__device__ __forceinline__ void tc_stage_in(const float* __restrict__ src, int nb, int K, int e_begin, int total, unsigned seq,
-                                            const float* __restrict__ norm_w, float* __restrict__ raw_copy, float* __restrict__ part,
-                                            unsigned bt) {
-  // elements [e_begin, total) of the [nb][K] block, NJ pairs per thread (e_begin = 0 whenever norm_w / raw_copy is set)
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float2 x[NJ];
-  if (LL) {
-    uint4 v[NJ];
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int e = e_begin + threadIdx.x * 2 + j * (kThreads * 2);
-      if (e < total) v[j] = ll_load2(src + (size_t)e * 2);
-    }
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int e = e_begin + threadIdx.x * 2 + j * (kThreads * 2);
-      if (e < total) {
-        while (v[j].y != seq || v[j].w != seq) v[j] = ll_load2(src + (size_t)e * 2);
-        x[j] = make_float2(__uint_as_float(v[j].x), __uint_as_float(v[j].z));
-      } else {
-        x[j] = make_float2(0.f, 0.f);
-      }
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int e = e_begin + threadIdx.x * 2 + j * (kThreads * 2);
-      x[j] = e < total ? __ldcg(reinterpret_cast<const float2*>(src + e)) : make_float2(0.f, 0.f);
-    }
-  }
-  const int cpr = K >> 6;  // 64-element chunks (= warps' spans) per row
-  if (norm_w || raw_copy) {
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int e = e_begin + threadIdx.x * 2 + j * (kThreads * 2);
-      if (raw_copy && e < total) *reinterpret_cast<float2*>(raw_copy + e) = x[j];
-      if (norm_w) {
-        const float ss = warp_sum(x[j].x * x[j].x + x[j].y * x[j].y);
-        const int ci = warp + j * kWarps;  // chunk index: row ci / cpr, slot ci % cpr
-        if (lane == 0 && ci * 64 < total) part[ci] = ss;
-      }
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int j = 0; j < NJ; ++j) {
-    const int e = e_begin + threadIdx.x * 2 + j * (kThreads * 2);
-    if (e >= total) continue;
-    const int u = e / K, k = e - u * K;
-    float a = x[j].x, b = x[j].y;
-    if (norm_w) {
-      float ss = 0.f;
-      for (int c = 0; c < cpr; ++c) ss += part[u * cpr + c];
-      const float inv = 1.0f / sqrtf(ss / (float)K + 1e-6f);
-      const float2 w = __ldg(reinterpret_cast<const float2*>(norm_w + k));
-      a = (a * inv) * w.x;
-      b = (b * inv) * w.y;
-    }
-    tc_store_split2(bt, u, k, a, b);
-  }
 }
 
 // The weight ring of a CTA: nbuf shared buffers filled by TMA in tile order.  Tile i lives in
@@ -1545,7 +1394,7 @@ __device__ __forceinline__ void stage_qatt(const ArParams& p, int li, const Team
 // ---------------------------------------------------------------------------
 // the persistent kernel: an interpreter over p.prog with one shared GEMV body
 // ---------------------------------------------------------------------------
-template <typename WT, int TU, bool LL, bool TC = false, bool TRACE = false>
+template <typename WT, int TU, bool LL, bool TRACE = false>
 __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid_constant__ ArParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ SamplerSmem ssm;
@@ -1553,13 +1402,11 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
   __shared__ unsigned char stage_tiles[kMaxStages];
   __shared__ int conv_phase[kMaxLayers], conv_slot[kMaxLayers];
   __shared__ int s_tok[kMaxUttPerTeam], s_done[kMaxUttPerTeam];
-  __shared__ float tc_part[TC ? 8 * 32 : 1];  // tensor-core stage-in: per-row partial sums of squares
   constexpr int EL = LL ? 2 : 1;  // floats per activation element in the exchange buffers
-  // the tensor-core instantiations (TC: bf16 weights, TU == 8) carry no FMA tile loop and vice versa
-  static_assert(!TC || (TU == 8 && sizeof(WT) == 2), "tensor-core path: bf16 weights, 8-utterance B operand");
-  // dynamic shared memory, 1024-byte aligned (the swizzled tensor-core operands need it): p.act_off / ring_off / table_off
+  // dynamic shared memory [act | p.ring_off: ring | p.table_off: table] from a 1024-byte aligned base, so that no address
+  // in the map depends on the static shared memory in front of it (the bulk copies into the ring need 16-byte alignment)
   unsigned char* const smem_base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* act = reinterpret_cast<float*>(smem_base + p.act_off);  // [nb][max(D,F)] (or 2 x [nb][D] + tap scratch)
+  float* act = reinterpret_cast<float*>(smem_base);  // [nb][max(D,F)] (or 2 x [nb][D] + tap scratch)
   TeamCtx tc;
   tc.team = blockIdx.x / p.P;
   tc.rank = blockIdx.x % p.P;
@@ -1572,16 +1419,9 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
   unsigned* bar = p.barrier + (size_t)tc.team * 32;
   unsigned epoch = 0;
   const int D = p.D, F = p.F;
-  constexpr bool use_tc = TC;
   const unsigned act_s = smem_u32(act);
-  // tensor-core path: the act region starts with the B operand ([F / 64 chunks][32 rows x 128 B]); the fp32 staging rows
-  // of the K = D stages sit behind the D / 64 chunks those stages use (the FFN2 stage, K = F, converts straight from
-  // the exchange buffer and needs no staging), the dwconv tap scratch behind them
-  float* gact = use_tc ? act + (size_t)p.ksc * (kTcBChunk / 4) : act;
-  const unsigned gact_s = smem_u32(gact);
-  float* xraw = gact + (size_t)tc.nb * D;  // second [nb][D] buffer (GLU stage only)
-  const unsigned scratch_s = gact_s + (unsigned)(2 * tc.nb * D) * 4u;  // GLU stage: dwconv tap rows
-  float* const tcd = reinterpret_cast<float*>(smem_base + p.act_off + p.act_bytes - kTcDBytes);  // tensor-core path only
+  float* xraw = act + (size_t)tc.nb * D;  // second [nb][D] buffer (GLU stage only)
+  const unsigned scratch_s = act_s + (unsigned)(2 * tc.nb * D) * 4u;  // GLU stage: dwconv tap rows
   const int n_ut = (tc.nb + TU - 1) / TU;
   // ---- weight ring: [act region][nbuf x wbuf][tile table]
   WeightRing ring;
@@ -1694,44 +1534,27 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
           for (int u = warp; u < tc.nb; u += kWarps) {
             const int b = tc.b0 + u;
             const float* cr = p.cond + ((size_t)b * p.steps + t) * D;
-            for (int k = lane * 4; k < D; k += 128) cp_async16(gact_s + (unsigned)(u * D + k) * 4u, cr + k);
+            for (int k = lane * 4; k < D; k += 128) cp_async16(act_s + (unsigned)(u * D + k) * 4u, cr + k);
             const int row = (t == 0) ? p.V : s_tok[u];
             const float* er = p.emb + (size_t)row * D;
-            for (int k = lane * 4; k < D; k += 128) cp_async16(gact_s + (unsigned)((tc.nb + u) * D + k) * 4u, er + k);
+            for (int k = lane * 4; k < D; k += 128) cp_async16(act_s + (unsigned)((tc.nb + u) * D + k) * 4u, er + k);
           }
           cp_async_commit();
           cp_async_wait0();
           __syncwarp();
           for (int u = warp; u < tc.nb; u += kWarps) {
             for (int k = lane * 4; k < D; k += 128) {
-              const float4 c = *reinterpret_cast<float4*>(gact + (size_t)u * D + k);
+              const float4 c = *reinterpret_cast<float4*>(act + (size_t)u * D + k);
               const float4 e = *reinterpret_cast<float4*>(xraw + (size_t)u * D + k);
               const float4 x = make_float4(c.x + e.x, c.y + e.y, c.z + e.z, c.w + e.w);
-              *reinterpret_cast<float4*>(gact + (size_t)u * D + k) = x;
+              *reinterpret_cast<float4*>(act + (size_t)u * D + k) = x;
               *reinterpret_cast<float4*>(xraw + (size_t)u * D + k) = x;
             }
           }
           __syncwarp();
         }
-        if (use_tc && src) {
-          // one pass: poll, (sum of squares, normalise,) split into three bf16 terms, store into the B operand
-          const float* xs = src + (size_t)tc.b0 * K * EL;
-          float* raw = kind == K_GLU ? xraw : nullptr;
-          if (norm_w || raw) {  // K = D: the whole block in one round (the rows' sums of squares need all of it)
-            tc_stage_in<LL, 3>(xs, tc.nb, K, 0, tc.nb * K, src_seq, norm_w, raw, tc_part, act_s);
-          } else {              // K = F: rounds of 6 pairs per thread
-            for (int e0 = 0; e0 < tc.nb * K; e0 += 6 * kThreads * 2)
-              tc_stage_in<LL, 6>(xs, tc.nb, K, e0, min(tc.nb * K, e0 + 6 * kThreads * 2), src_seq, nullptr, nullptr, tc_part, act_s);
-          }
-        } else {
-          stage_rows<LL>(src ? src + (size_t)tc.b0 * K * EL : nullptr, tc.nb, K, gact, norm_w,
-                         (kind == K_GLU && src) ? xraw : nullptr, src_seq);
-          if (use_tc) {  // layer 0: x was built in shared memory
-            __syncthreads();
-            tc_btile_from_rows(gact, tc.nb, K, act_s);
-          }
-        }
-        if (use_tc) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> tensor-core reads
+        stage_rows<LL>(src ? src + (size_t)tc.b0 * K * EL : nullptr, tc.nb, K, act, norm_w,
+                       (kind == K_GLU && src) ? xraw : nullptr, src_seq);
         __syncthreads();
         ts.mark();  // activations staged
         // ---- this CTA's rows, tile by tile from the weight ring
@@ -1740,237 +1563,104 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
         float* state = p.ring + L.ring_off;
         const int dil = L.dil;
         const int phase = conv_phase[li], slot_now = conv_slot[li];
-        if constexpr (TC) {
-          // ================= tensor-core tiles: epilogue thread = (accumulator row, two utterances)
-          const int q = warp & 3, jc = warp >> 2;  // rows 16q..16q+15 (lanes 0..15); columns 8jc..8jc+7 = utterances 2jc, 2jc+1
-          const int rt = lane < 16 ? 16 * q + lane : 64;  // row of the tile (64 = none)
-          float dacc[kTcCols / 2];  // warpgroup 0: the accumulator, carried across the tiles of one output row block
-          long long* tdbg = (ts.buf && (si == 1 || si == 7)) ? ts.buf + (si == 1 ? 192 : 208) : nullptr;  // tile phase stamps
-          int tdn = 0;
-#define TCMARK() do { if (tdbg && tdn < 16) tdbg[tdn++] = clock64(); } while (0)
-          TCMARK();
 #pragma unroll 1
-          for (int ti = stage_tiles[si]; ti > 0; --ti) {
-            const TileDesc* td;
-            const unsigned wb = ring.acquire(td);
-            TCMARK();  // weights landed
-            const bool last = (td->flags & 2) != 0;
-            // GLU: a group of 8 operand rows = 4 channels (value rows 0..3, their gate rows 4..7)
-            const int g8 = rt & 7;
-            const int ri = glu ? ((rt >> 3) * 4 + (g8 & 3)) : rt;  // row (GLU: channel) index inside the tile
-            const bool row_ok = rt < td->ngrp * 8 && ri < td->nrows && (!glu || g8 < 4);
-            const int r = td->row0 + (row_ok ? ri : 0);             // output feature (GLU: channel)
-            const unsigned epi_s = wb + td->bytes0 + td->bytes1;
-            float res_v[2] = {0.f, 0.f};
-            float* rbp[2] = {nullptr, nullptr};
-            if (last) {  // epilogue operands: their latency hides under the contraction
+      for (int ti = stage_tiles[si]; ti > 0; --ti) {
+        const TileDesc* td;
+        const unsigned wb = ring.acquire(td);
+        const int nr = td->nrows;
+        // a task = R weight rows x TU utterances; GLU: R/2 channels (value rows, then their gate rows)
+        constexpr int R = (TU == 8) ? 4 : 2;
+        constexpr int RC = R / 2;
+        const int n_rt = glu ? (nr + RC - 1) / RC : (nr + R - 1) / R;
+        const unsigned epi_s = wb + td->bytes0 + td->bytes1;
+#pragma unroll 1
+        for (int task = warp; task < n_rt * n_ut; task += kWarps) {
+          const int rt = n_ut == 1 ? task : (int)((unsigned)task / (unsigned)n_ut);
+          const int u0 = (task - rt * n_ut) * TU;
+          unsigned wr[R];
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int u = 2 * jc + e;
-                const bool mine = row_ok && u < tc.nb;
-                const int b = tc.b0 + (mine ? u : 0);
-                if (glu) {
-                  rbp[e] = state + (((size_t)b * D + r) * dil + phase) * p.KcP;
-                  if (mine) {
-                    const unsigned tap_w = scratch_s + (unsigned)((ri * 8 + u) * p.KcP) * 4u;
-                    for (int q4 = 0; q4 < p.KcP; q4 += 4) cp_async16(tap_w + (unsigned)q4 * 4u, rbp[e] + q4);
-                  }
-                } else if (mine && (kind == K_FFN2 || kind == K_O)) {
-                  res_v[e] = ldcg1(dst + ((size_t)b * ld_dst + r) * EL);  // own rows, written at an earlier stage
-                }
-              }
-              cp_async_commit();
-            }
-            // ---- the contraction: warpgroup 0 issues (K slices of the tile) x (D / 64) x 4 instructions [64 x 32 x 16]
-            if (warp < 4) {
-              const bool first = (td->flags & 1) != 0;
-              const int nsl = td->bytes1 ? 2 : 1;  // part 1 = the same rows' next K slice
-              wg::fence();
-#pragma unroll 1
-              for (int sl = 0; sl < nsl; ++sl) {
-                const unsigned long long da = tc_desc(wb + (unsigned)sl * td->bytes0, (unsigned)p.ksc * 1024u);
-                const unsigned long long db = tc_desc(act_s + (unsigned)(td->kc0 + sl * p.ksc) * (unsigned)kTcBChunk, 1024u);
-#pragma unroll 1
-                for (int c = 0; c < p.ksc; ++c) {
-#pragma unroll
-                  for (int k = 0; k < 4; ++k)
-                    wg::mma_ss<kTcCols>(dacc, da + (unsigned long long)(c * 64 + k * 2), db + (unsigned long long)(c * (kTcBChunk >> 4) + k * 2),
-                                        (first && sl == 0 && c == 0 && k == 0) ? 0u : 1u);
-                }
-              }
-              wg::commit();
-              TCMARK();  // instructions issued
-              wg::wait<0>();  // also: the weight buffer may be released
-              wg::fence_regs(dacc);
-              if (last) {
-#pragma unroll
-                for (int i = 0; i < kTcCols / 2; ++i)
-                  tcd[(16 * warp + (lane >> 2) + 8 * ((i >> 1) & 1)) * kTcDPitch + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)] = dacc[i];
-              }
-            }
-            TCMARK();  // accumulator complete
-            if (last) {
-              __syncthreads();
-              float vv[2] = {0.f, 0.f};
-              if (rt < 64) {  // x = hi + mid + lo: add the small terms first
-                const float* dr = tcd + rt * kTcDPitch + 8 * jc;
-                vv[0] = (dr[2] + dr[1]) + dr[0];
-                vv[1] = (dr[6] + dr[5]) + dr[4];
-              }
-              cp_async_wait0();
-              TCMARK();  // accumulator in registers
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                float v = vv[e];
-                const float gate_v = __shfl_xor_sync(0xffffffffu, v, 4);  // GLU: the gate row sits 4 lanes up
-                const int u = 2 * jc + e;
-                const bool mine = row_ok && u < tc.nb;
-                if (!mine) continue;
-                const int b = tc.b0 + u;
-                float* d = dst + ((size_t)b * ld_dst + r) * EL;
-                if (glu) {
-                  const int Kc = p.Kc;
-                  const unsigned er = epi_s + (unsigned)(ri * p.KcE) * 4u;  // [w0..w(Kc-1), dw_b, b_value, b_gate]
-                  const unsigned tap_w = scratch_s + (unsigned)((ri * 8 + u) * p.KcP) * 4u;
-                  const float a = v + lds32(er + (unsigned)(Kc + 1) * 4u);
-                  const float gt = gate_v + lds32(er + (unsigned)(Kc + 2) * 4u);
-                  const float h = a * sigmoid_ref(gt);
-                  rbp[e][slot_now] = h;
-                  float y = 0.f;
-                  int pos = slot_now + 1;
-#pragma unroll 1
-                  for (int j = 0; j < Kc - 1; ++j) {
-                    if (pos == Kc) pos = 0;
-                    y += lds32(tap_w + (unsigned)pos * 4u) * lds32(er + (unsigned)j * 4u);
-                    ++pos;
-                  }
-                  y += h * lds32(er + (unsigned)(Kc - 1) * 4u);
-                  y += lds32(er + (unsigned)Kc * 4u);
-                  v = xraw[(size_t)u * D + r] + y;
-                } else {
-                  const float bias_v = (kind == K_Q || kind == K_O) ? 0.f : lds32(epi_s + (unsigned)(td->off2 + ri) * 4u);
-                  if (kind == K_FFN1) {
-                    v = gelu_erf(v + bias_v);
-                  } else if (kind == K_FFN2) {
-                    v = res_v[e] + (v + bias_v);
-                    if (trace) trace[(size_t)b * D + r] = v;
-                  } else if (kind == K_O) {
-                    v = res_v[e] + scale * v;
-                    if (trace) trace[(size_t)b * D + r] = v;
-                  } else if (kind == K_HEAD) {
-                    v += bias_v;
-                    if (trace) trace[(size_t)b * p.V + r] = v;
-                  }
-                }
-                if (LL) ll_store(d, v, seq);
-                else *d = v;
-              }
-            }
-            TCMARK();  // epilogue done (thread 0)
-            ring.release();  // (block barrier inside) every warp has read its accumulator columns before the next reset
-            TCMARK();  // released
-          }
-#undef TCMARK
-        } else {
-#pragma unroll 1
-        for (int ti = stage_tiles[si]; ti > 0; --ti) {
-          const TileDesc* td;
-          const unsigned wb = ring.acquire(td);
-          const int nr = td->nrows;
-          // a task = R weight rows x TU utterances; GLU: R/2 channels (value rows, then their gate rows)
-          constexpr int R = (TU == 8) ? 4 : 2;
-          constexpr int RC = R / 2;
-          const int n_rt = glu ? (nr + RC - 1) / RC : (nr + R - 1) / R;
-          const unsigned epi_s = wb + td->bytes0 + td->bytes1;
-#pragma unroll 1
-          for (int task = warp; task < n_rt * n_ut; task += kWarps) {
-            const int rt = n_ut == 1 ? task : (int)((unsigned)task / (unsigned)n_ut);
-            const int u0 = (task - rt * n_ut) * TU;
-            unsigned wr[R];
-#pragma unroll
-            for (int jr = 0; jr < R; ++jr) {
-              if (glu) {
-                const int ch = min(rt * RC + (jr % RC), nr - 1);
-                wr[jr] = wb + (jr < RC ? 0u : td->bytes0) + (unsigned)ch * row_bytes;
-              } else {
-                wr[jr] = wb + (unsigned)min(rt * R + jr, nr - 1) * row_bytes;
-              }
-            }
-            const int ub = min(u0, max(tc.nb - TU, 0));
-            // after the transposed reduction lane L owns output o = (L >> SH) & (R*TU-1) = i*TU + uu
-            constexpr int NOUT = R * TU;
-            constexpr int LOG2N = (NOUT == 2 ? 1 : NOUT == 4 ? 2 : NOUT == 8 ? 3 : NOUT == 16 ? 4 : 5);
-            constexpr int SH = 5 - LOG2N;
-            const int o = (lane >> SH) & (NOUT - 1);
-            const int i = o / TU, uu = o % TU;
-            const bool writer = (lane & ((1 << SH) - 1)) == 0;
-            const int ri = glu ? rt * RC + i : rt * R + i;
-            const int u = ub + uu;
-            const bool mine = writer && (glu ? i < RC : true) && ri < nr && u >= u0 && u < tc.nb;
-            const int r = td->row0 + ri;  // output feature (GLU: channel)
-            const int b = tc.b0 + (mine ? u : 0);
-            float* d = dst + ((size_t)b * ld_dst + (mine ? r : td->row0)) * EL;
-            // operands of the epilogue are requested before the K loop: their latency hides under it
-            float res_v = 0.f;
-            float* rb = nullptr;
-            // one tap row per (channel of the task, utterance): kTapSlots = 16 rows per warp (RC <= 2 channels x TU <= 8)
-            const unsigned tap_w = scratch_s + (unsigned)warp * (unsigned)(kTapSlots * p.KcP * 4) +
-                                   (unsigned)((i % RC) * TU + uu) * (unsigned)(p.KcP * 4);
+          for (int jr = 0; jr < R; ++jr) {
             if (glu) {
-              // conv state row of (utterance, channel, phase): [KcP] floats, see DESIGN.md §2
-              rb = state + (((size_t)b * D + (mine ? r : td->row0)) * dil + phase) * p.KcP;
-              if (mine)
-                for (int q = 0; q < p.KcP; q += 4) cp_async16(tap_w + (unsigned)q * 4u, rb + q);
-            } else if (mine && (kind == K_FFN2 || kind == K_O)) {
-              res_v = ldcg1(d);  // own slice: written by this CTA at an earlier stage (value word)
+              const int ch = min(rt * RC + (jr % RC), nr - 1);
+              wr[jr] = wb + (jr < RC ? 0u : td->bytes0) + (unsigned)ch * row_bytes;
+            } else {
+              wr[jr] = wb + (unsigned)min(rt * R + jr, nr - 1) * row_bytes;
             }
-            cp_async_commit();
-            float v = warp_rows_s<R, TU, WT>(wr, gact_s + (unsigned)ub * (unsigned)K * 4u, K, lane);
-            // GLU: the gate total of (channel i, utterance uu) lives in the lanes of output (RC + i)*TU + uu
-            const float gate_v = __shfl_sync(0xffffffffu, v, (((RC + (i % RC)) * TU + uu) << SH) & 31);
-            cp_async_wait0();
-            if (mine) {
-              if (glu) {
-                const int Kc = p.Kc;
-                const unsigned er = epi_s + (unsigned)(ri * p.KcE) * 4u;  // [w0..w(Kc-1), dw_b, b_value, b_gate]
-                const float a = v + lds32(er + (unsigned)(Kc + 1) * 4u);
-                const float gt = gate_v + lds32(er + (unsigned)(Kc + 2) * 4u);
-                const float h = a * sigmoid_ref(gt);
-                rb[slot_now] = h;  // slot (t / dil) mod Kc of frame t inside its phase
-                float y = 0.f;
-                int pos = slot_now + 1;  // oldest tap: frame t - (Kc-1)*dil
-#pragma unroll 1
-                for (int j = 0; j < Kc - 1; ++j) {
-                  if (pos == Kc) pos = 0;
-                  y += lds32(tap_w + (unsigned)pos * 4u) * lds32(er + (unsigned)j * 4u);
-                  ++pos;
-                }
-                y += h * lds32(er + (unsigned)(Kc - 1) * 4u);
-                y += lds32(er + (unsigned)Kc * 4u);
-                v = xraw[(size_t)u * D + r] + y;
-              } else {
-                const float bias_v = (kind == K_Q || kind == K_O) ? 0.f : lds32(epi_s + (unsigned)(td->off2 + ri) * 4u);
-                if (kind == K_FFN1) {
-                  v = gelu_erf(v + bias_v);
-                } else if (kind == K_FFN2) {
-                  v = res_v + (v + bias_v);
-                  if (trace) trace[(size_t)b * D + r] = v;
-                } else if (kind == K_O) {
-                  v = res_v + scale * v;
-                  if (trace) trace[(size_t)b * D + r] = v;
-                } else if (kind == K_HEAD) {
-                  v += bias_v;
-                  if (trace) trace[(size_t)b * p.V + r] = v;
-                }
-              }
-              if (LL) ll_store(d, v, seq);
-              else *d = v;
-            }
-            __syncwarp();  // the tap scratch is reused by the next task of this warp
           }
-          ring.release();
+          const int ub = min(u0, max(tc.nb - TU, 0));
+          // after the transposed reduction lane L owns output o = (L >> SH) & (R*TU-1) = i*TU + uu
+          constexpr int NOUT = R * TU;
+          constexpr int LOG2N = (NOUT == 2 ? 1 : NOUT == 4 ? 2 : NOUT == 8 ? 3 : NOUT == 16 ? 4 : 5);
+          constexpr int SH = 5 - LOG2N;
+          const int o = (lane >> SH) & (NOUT - 1);
+          const int i = o / TU, uu = o % TU;
+          const bool writer = (lane & ((1 << SH) - 1)) == 0;
+          const int ri = glu ? rt * RC + i : rt * R + i;
+          const int u = ub + uu;
+          const bool mine = writer && (glu ? i < RC : true) && ri < nr && u >= u0 && u < tc.nb;
+          const int r = td->row0 + ri;  // output feature (GLU: channel)
+          const int b = tc.b0 + (mine ? u : 0);
+          float* d = dst + ((size_t)b * ld_dst + (mine ? r : td->row0)) * EL;
+          // operands of the epilogue are requested before the K loop: their latency hides under it
+          float res_v = 0.f;
+          float* rb = nullptr;
+          // one tap row per (channel of the task, utterance): kTapSlots = 16 rows per warp (RC <= 2 channels x TU <= 8)
+          const unsigned tap_w = scratch_s + (unsigned)warp * (unsigned)(kTapSlots * p.KcP * 4) +
+                                 (unsigned)((i % RC) * TU + uu) * (unsigned)(p.KcP * 4);
+          if (glu) {
+            // conv state row of (utterance, channel, phase): [KcP] floats, see DESIGN.md §2
+            rb = state + (((size_t)b * D + (mine ? r : td->row0)) * dil + phase) * p.KcP;
+            if (mine)
+              for (int q = 0; q < p.KcP; q += 4) cp_async16(tap_w + (unsigned)q * 4u, rb + q);
+          } else if (mine && (kind == K_FFN2 || kind == K_O)) {
+            res_v = ldcg1(d);  // own slice: written by this CTA at an earlier stage (value word)
+          }
+          cp_async_commit();
+          float v = warp_rows_s<R, TU, WT>(wr, act_s + (unsigned)ub * (unsigned)K * 4u, K, lane);
+          // GLU: the gate total of (channel i, utterance uu) lives in the lanes of output (RC + i)*TU + uu
+          const float gate_v = __shfl_sync(0xffffffffu, v, (((RC + (i % RC)) * TU + uu) << SH) & 31);
+          cp_async_wait0();
+          if (mine) {
+            if (glu) {
+              const int Kc = p.Kc;
+              const unsigned er = epi_s + (unsigned)(ri * p.KcE) * 4u;  // [w0..w(Kc-1), dw_b, b_value, b_gate]
+              const float a = v + lds32(er + (unsigned)(Kc + 1) * 4u);
+              const float gt = gate_v + lds32(er + (unsigned)(Kc + 2) * 4u);
+              const float h = a * sigmoid_ref(gt);
+              rb[slot_now] = h;  // slot (t / dil) mod Kc of frame t inside its phase
+              float y = 0.f;
+              int pos = slot_now + 1;  // oldest tap: frame t - (Kc-1)*dil
+#pragma unroll 1
+              for (int j = 0; j < Kc - 1; ++j) {
+                if (pos == Kc) pos = 0;
+                y += lds32(tap_w + (unsigned)pos * 4u) * lds32(er + (unsigned)j * 4u);
+                ++pos;
+              }
+              y += h * lds32(er + (unsigned)(Kc - 1) * 4u);
+              y += lds32(er + (unsigned)Kc * 4u);
+              v = xraw[(size_t)u * D + r] + y;
+            } else {
+              const float bias_v = (kind == K_Q || kind == K_O) ? 0.f : lds32(epi_s + (unsigned)(td->off2 + ri) * 4u);
+              if (kind == K_FFN1) {
+                v = gelu_erf(v + bias_v);
+              } else if (kind == K_FFN2) {
+                v = res_v + (v + bias_v);
+                if (trace) trace[(size_t)b * D + r] = v;
+              } else if (kind == K_O) {
+                v = res_v + scale * v;
+                if (trace) trace[(size_t)b * D + r] = v;
+              } else if (kind == K_HEAD) {
+                v += bias_v;
+                if (trace) trace[(size_t)b * p.V + r] = v;
+              }
+            }
+            if (LL) ll_store(d, v, seq);
+            else *d = v;
+          }
+          __syncwarp();  // the tap scratch is reused by the next task of this warp
         }
-        }
+        ring.release();
+      }
         ts.mark();  // tiles done
         if (glu) {
           float* tmp = cur;

@@ -137,11 +137,6 @@ class ArSession:
     def set_team(self, utts_per_team: int) -> None:
         _lib.check(self.lib.sopro_ar_session_set_team(self._h, int(utts_per_team)))
 
-    def set_contraction(self, mode: int) -> None:
-        """-1 / 0: packed-fp32 FMA tiles (default; -1 honours SOPRO_AR_TC=1); 1: tensor cores (wgmma, exact three-way
-        bf16 split of the activations against bf16 weights) -- exact but slower at this kernel's tile sizes."""
-        _lib.check(self.lib.sopro_ar_session_set_contraction(self._h, int(mode)))
-
     def _dev(self, t: torch.Tensor) -> torch.Tensor:
         t = t.to(device=self.engine.device, dtype=torch.float32).contiguous()
         self._keep.append(t)

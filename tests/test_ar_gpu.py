@@ -106,12 +106,10 @@ def test_teacher_forced_logits_and_blocks(name):
     assert sampled == gold.tolist()
 
 
-@pytest.mark.parametrize("mode", [1, 0])
-def test_batched_bf16_reference_case_on_both_contraction_units(mode):
-    """The reference fixture default_bf16 replicated over a team of 8 utterances, through the tensor-core contraction
-    (mode 1: tensor cores, every fp32 activation split into three exact bf16 terms) and through the packed-fp32 FMA path
-    (mode 0) of the same launch geometry: teacher-forced logits and per-block residuals within the fixture tolerances
-    (3e-5 / 2e-5 of the peak, fp32 accumulation-order noise), and every sampled token is the reference's."""
+def test_batched_bf16_reference_case_over_a_team_of_eight():
+    """The reference fixture default_bf16 replicated over a team of 8 utterances: teacher-forced logits and per-block
+    residuals within the fixture tolerances (3e-5 / 2e-5 of the peak, fp32 accumulation-order noise), and every sampled
+    token is the reference's."""
     spec, cfg, sd, inp, g, eng, steps, tape = _case("default_bf16")
     B, L = 8, inp["txt_seq"].shape[1]
     gold = torch.from_numpy(g["tokens"].astype(np.int32))
@@ -122,7 +120,6 @@ def test_batched_bf16_reference_case_on_both_contraction_units(mode):
     tr_b = torch.zeros(steps, int(cfg.n_layers_ar), B, int(cfg.d_model), device=dev)
     tr_l = torch.zeros(steps, B, cfg.ar_vocab(), device=dev)
     ses = eng.session(B, steps, L)
-    ses.set_contraction(mode)
     ses.set_forced(forced)
     ses.set_trace(tr_b, tr_l)
     ses.begin(inp["cond_ar"].expand(B, -1, -1).contiguous(), inp["txt_seq"].expand(B, -1, -1).contiguous(), [L] * B,
@@ -147,10 +144,9 @@ def test_batched_bf16_reference_case_on_both_contraction_units(mode):
 
 
 @pytest.mark.parametrize("n_utts", [8, 19, 5])
-def test_tensor_core_teams_match_the_oracle(n_utts):
-    """bf16 weight storage, ragged texts, full and partially filled teams (19 -> 7 + 7 + 5 utterances) with the tensor-core
-    contraction REQUIRED (set_contraction(1) fails loudly when a launch cannot use it): every utterance equals the CPU
-    oracle run alone on it."""
+def test_bf16_ragged_teams_match_the_oracle(n_utts):
+    """bf16 weight storage, ragged texts, full and partially filled teams (19 -> 7 + 7 + 5 utterances), a resumed
+    launch: every utterance equals the CPU oracle run alone on it."""
     spec = AR_CASES["default_bf16"]
     cfg, sd, _ = ar_case_inputs(spec)
     eng = _engine(cfg, sd, "bf16", _wkey(spec))
@@ -160,28 +156,12 @@ def test_tensor_core_teams_match_the_oracle(n_utts):
     samp = O.ArSampling(min_gen_frames=10 ** 9)
     want = _oracle_batch(sd, cfg, cond, txt, tapes, lens, samp, steps)
     ses = eng.session(n, steps, max(lens))
-    ses.set_contraction(1)
     ses.begin(cond, txt, lens, tapes[:, :, :50].contiguous(), _sampling(samp, cfg))
-    ses.run(11)  # resumed launches carry the tensor-core state too
+    ses.run(11)
     ses.run()
     toks, nn, done = ses.read()
     bad = [i for i in range(n) if toks[i, : nn[i]].tolist() != want[i]]
     assert not bad, f"utterances {bad} differ from the oracle"
-    ses.close()
-
-
-def test_tensor_core_contraction_is_refused_where_it_cannot_run():
-    from sopro_b200._lib import SoproError
-
-    spec = AR_CASES["default_fp32"]
-    cfg, sd, inp = ar_case_inputs(spec)
-    eng = _engine(cfg, sd, "fp32", _wkey(spec))
-    ses = eng.session(8, 4, 8)
-    ses.set_contraction(1)
-    cond, txt, tapes = _batch_inputs(cfg, 8, 4, [8] * 8)
-    ses.begin(cond, txt, [8] * 8, tapes[:, :, :50].contiguous(), _sampling(O.ArSampling(min_gen_frames=10 ** 9), cfg))
-    with pytest.raises(SoproError, match="tensor-core"):
-        ses.run()
     ses.close()
 
 

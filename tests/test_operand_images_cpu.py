@@ -1,5 +1,5 @@
-"""Host-built operand images (no GPU): the NAR refiner's exact three-way bf16 split of the weights (W6) and the AR step's
-tensor-core image (K-major, 128-byte swizzle) decode back to the matrices they were built from."""
+"""Host-built operand images (no GPU): the NAR refiner's exact three-way bf16 split of the weights (W6) decodes back to
+the matrix it was built from."""
 import ctypes as C
 
 import numpy as np
@@ -32,35 +32,3 @@ def test_w6_is_an_exact_three_term_split_in_the_pair_order():
     assert np.array_equal((h + m + l).astype(np.float32), W)           # exact: 3 x 8 mantissa bits cover fp32's 24
     assert np.array_equal(out[:, 1], _bf16_rne(W))                     # h = round-to-nearest-even bf16 of w
     assert np.all(np.abs(m) <= np.abs(h) * 2.0 ** -8 + 1e-45) and np.all(np.abs(l) <= np.abs(h) * 2.0 ** -16 + 1e-45)
-
-
-def _decode_umma(img, N, K, D, glu):
-    """Undo Arena::add_packed: -> W [N][K] as float32 from bf16."""
-    KSC, S = D // 64, K // D
-    G = D // 4 if glu else (N + 7) // 8
-    img = img.reshape(S, G, KSC, 8, 8, 8)  # [slice][group][chunk][row r][unit position][8 bf16]
-    W = np.zeros((N, K), dtype=np.float32)
-    for sl in range(S):
-        for g in range(G):
-            for rr in range(8):
-                row = (4 * g + rr if rr < 4 else N // 2 + 4 * g + rr - 4) if glu else 8 * g + rr
-                if row >= N:
-                    assert not img[sl, g, :, rr].any()  # padding rows are zero
-                    continue
-                for c in range(KSC):
-                    for j in range(8):
-                        W[row, sl * D + c * 64 + j * 8: sl * D + c * 64 + j * 8 + 8] = _bf16_to_f32(img[sl, g, c, rr, j ^ rr])
-    return W
-
-
-def test_tensor_core_image_round_trips_with_the_128_byte_swizzle():
-    lib = _lib.load()
-    D = 128
-    for N, K, glu in ((2 * D, D, 1), (4 * D, D, 0), (D, 4 * D, 0), (37, D, 0)):
-        W = (hash_uniform(N * K, 99 + N) * np.float32(2.0)).astype(np.float32).reshape(N, K)
-        G = D // 4 if glu else (N + 7) // 8
-        nbytes = (K // D) * G * (D // 64) * 1024
-        img = np.zeros(nbytes // 2, dtype=np.uint16)
-        _lib.check(lib.sopro_debug_pack_umma(W.ctypes.data, N, K, D, glu, img.ctypes.data, nbytes))
-        got = _decode_umma(img, N, K, D, bool(glu))
-        assert np.array_equal(got, _bf16_to_f32(_bf16_rne(W))), (N, K, glu)

@@ -87,11 +87,10 @@ def test_exported_weights_match_the_float64_oracle(name):
     print(f"{name}: max |w - w64| = {err:.2e} over {T} steps")
 
 
-def _generate(eng, inp, cfg, spec, B, steps, L_list, trace, team=0, mode=-1, chunks=None, txt=None):
+def _generate(eng, inp, cfg, spec, B, steps, L_list, trace, team=0, chunks=None, txt=None):
     ses = eng.session(B, steps, max(L_list))
     if team:
         ses.set_team(team)
-    ses.set_contraction(mode)
     tape = O.noise_tape(spec["noise_seed"], steps, cfg.ar_vocab())[:, :50].contiguous()
     cond = inp["cond_ar"][:, :steps].expand(B, -1, -1).contiguous()
     txt = inp["txt_seq"].expand(B, -1, -1).contiguous() if txt is None else txt
@@ -109,17 +108,17 @@ def _generate(eng, inp, cfg, spec, B, steps, L_list, trace, team=0, mode=-1, chu
     return toks, n
 
 
-@pytest.mark.parametrize("name,B,team,mode", [
-    ("default_fp32", 1, 0, -1), ("default_bf16", 1, 0, -1), ("default_fp32", 64, 0, 0), ("default_bf16", 64, 0, 0),
-    ("default_bf16", 64, 8, 1), ("default_fp32", 16, 16, 0), ("default_bf16", 16, 8, 1)])
-def test_tokens_unchanged_with_the_export_on(name, B, team, mode):
+@pytest.mark.parametrize("name,B,team", [
+    ("default_fp32", 1, 0), ("default_bf16", 1, 0), ("default_fp32", 64, 0), ("default_bf16", 64, 0),
+    ("default_bf16", 64, 8), ("default_fp32", 16, 16), ("default_bf16", 16, 8)])
+def test_tokens_unchanged_with_the_export_on(name, B, team):
     spec, cfg, sd, inp, eng = _engine(name)
     steps = 121
     L = int(inp["txt_seq"].shape[1])
     lens = [L - (b % 5) for b in range(B)]
-    off, _ = _generate(eng, inp, cfg, spec, B, steps, lens, None, team, mode)
+    off, _ = _generate(eng, inp, cfg, spec, B, steps, lens, None, team)
     tr = _trace(cfg, steps, B, L)
-    on, _ = _generate(eng, inp, cfg, spec, B, steps, lens, tr, team, mode)
+    on, _ = _generate(eng, inp, cfg, spec, B, steps, lens, tr, team)
     assert np.array_equal(on, off)
     w = tr.cpu().numpy()
     for b in (0, B - 1):

@@ -19,7 +19,7 @@ def stage_names(cfg, fused):
     return names + ["head", "sample"]
 
 
-def run(B, wdtype, team=0, mode=-1, steps=64, L=52, step=40):
+def run(B, wdtype, team=0, steps=64, L=52, step=40):
     spec = AR_CASES["default_bf16" if wdtype == "bf16" else "default_fp32"]
     cfg, sd, _ = ar_case_inputs(spec)
     eng = ArEngine(cfg, sd, 0, wdtype)
@@ -29,7 +29,6 @@ def run(B, wdtype, team=0, mode=-1, steps=64, L=52, step=40):
     noise = torch.empty(B, steps, 50).exponential_(1.0, generator=torch.Generator().manual_seed(0))
     ses = eng.session(B, steps, L)
     if team: ses.set_team(team)
-    ses.set_contraction(mode)
     buf = torch.zeros(eng.num_sms, 224, dtype=torch.int64, device="cuda")
     ses.set_timing(buf, step)
     ses.begin(cond, txt, [L] * B, noise, Sampling(min_gen_frames=2**31 - 1))
@@ -40,7 +39,7 @@ def run(B, wdtype, team=0, mode=-1, steps=64, L=52, step=40):
     names = stage_names(cfg, fused)
     ns = len(names)
     clk = 1.0  # cycles
-    print(f"== B={B} {wdtype} team={team} contraction={mode}: per-stage cycles (median / max over CTAs)")
+    print(f"== B={B} {wdtype} team={team}: per-stage cycles (median / max over CTAs)")
     tot = np.zeros(5)
     for s_i, nm in enumerate(names):
         base = 1 + 5 * s_i
@@ -54,20 +53,13 @@ def run(B, wdtype, team=0, mode=-1, steps=64, L=52, step=40):
     sm = t[int(np.argmax(t[:, 161] > 0)), 160:170]  # the CTA that ran a sampler
     print("  sampler phases (CTA 0):", [int(b - a) for a, b in zip(sm[:-1], sm[1:])],
           "= fetch, penalise, max, exp+sum, probs, lower bound, compaction, sort/top-p/draw, bookkeeping")
-    if mode != 0 and wdtype == "bf16" and B >= 8:
-        for nm, base in (("L0.ffn1", 192), ("L1.o", 208)):
-            for cta in (0, 5, 11):
-                row = t[cta, base:base + 16]
-                row = row[row > 0]
-                print(f"  tc tile phases {nm} CTA {cta}:", [int(b - a) for a, b in zip(row[:-1], row[1:])],
-                      "= per tile: wait weights, issue, accumulate, tmem->regs, epilogue, release")
     span = (t[:, 5 * ns] - t[:, 0])
     print(f"  step span cycles median {np.median(span[span>0]):.0f}; sums of medians stage-in {tot[0]:.0f} tiles {tot[1]:.0f} tail {tot[2]:.0f} post {tot[3]:.0f} wait {tot[4]:.0f}")
 
 
 if __name__ == "__main__":
-    cfgs = [(1, "fp32", 0, -1), (64, "bf16", 0, -1)]
+    cfgs = [(1, "fp32", 0), (64, "bf16", 0)]
     if len(sys.argv) > 1:  # e.g. 64:bf16:8 1:fp32:0
-        cfgs = [(int(a.split(":")[0]), a.split(":")[1], int(a.split(":")[2]), int(a.split(":")[3]) if a.count(":") > 2 else -1) for a in sys.argv[1:]]
+        cfgs = [(int(a.split(":")[0]), a.split(":")[1], int(a.split(":")[2])) for a in sys.argv[1:]]
     for c in cfgs:
         run(*c)

@@ -189,6 +189,13 @@ int sopro_ar_set_timing(sopro_ar_session_t* s, int64_t* buf, int step);
  * ld < 1 with a buffer is SOPRO_ERR_INVALID; sopro_ar_begin and sopro_ar_run refuse ld < the batch's longest text
  * (SOPRO_ERR_INVALID, before any launch). */
 int sopro_ar_set_attn_trace(sopro_ar_session_t* s, float* probs, int64_t ld);
+/* warp task shape of the GEMV stages of later launches: 0 = picked per stage from the launch geometry (the default),
+ * 1 = always R rows x TU utterances (wide), 2 = R x TU/2 (narrow) in every GEMV stage but GLU (teams of one utterance
+ * stay wide).  The outputs are bit-identical in every mode. */
+int sopro_ar_session_set_task_shape(sopro_ar_session_t* s, int mode);
+/* the stage program of the last launch: kinds[i] (0 GLU, 1 FFN1, 2 FFN2, 3 Q, 4 O, 5 HEAD, 6 ATT, 7 SAMPLE, 8 fused
+ * Q+ATT) and shapes[i] (0 wide, 1 narrow) of its first min(cap, *n_stage) stages; *n_stage = 0 before any launch.  HOST. */
+int sopro_ar_session_stage_shapes(sopro_ar_session_t* s, int32_t* kinds, int32_t* shapes, int cap, int32_t* n_stage);
 /* copy the sampled (pre-forcing) tokens into dst [batch, steps] i32 (device) */
 int sopro_ar_debug_sampled(sopro_ar_session_t* s, int32_t* dst, void* stream);
 /* copy the text K/V built by sopro_ar_begin into k_dst / v_dst, each

@@ -166,6 +166,8 @@ SYMBOLS = {
     "sopro_ar_set_trace": (_I, [_VP, _VP, _VP]),
     "sopro_ar_set_timing": (_I, [_VP, _VP, _I]),
     "sopro_ar_set_attn_trace": (_I, [_VP, _VP, C.c_int64]),
+    "sopro_ar_session_set_task_shape": (_I, [_VP, _I]),
+    "sopro_ar_session_stage_shapes": (_I, [_VP, _I32P, _I32P, _I, _I32P]),
     "sopro_ar_debug_sampled": (_I, [_VP, _VP, _VP]),
     "sopro_ar_debug_kv": (_I, [_VP, _VP, _VP, _VP]),
     "sopro_noise_create": (_I, [C.c_uint64, _VP]),

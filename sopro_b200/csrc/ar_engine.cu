@@ -80,6 +80,9 @@ struct sopro_ar_session {
   sopro_engine* e = nullptr;
   int max_batch = 0, max_steps = 0, Lmax = 0;
   int utts_per_team = 0;  // 0 = auto
+  int task_shape = 0;     // 0 = picked per stage by launch_ar, 1 = always wide, 2 = always narrow (test hook)
+  StageOp last_prog[kMaxStages]{};  // the stage program of the last launch (with each stage's task shape)
+  int last_n_stage = 0;
   // device buffers
   float *ring = nullptr, *xa = nullptr, *xb = nullptr, *hbuf = nullptr, *qbuf = nullptr, *abuf = nullptr,
         *logits = nullptr, *kc = nullptr, *vc = nullptr;
@@ -400,6 +403,24 @@ int sopro_ar_session_set_team(sopro_ar_session_t* s, int utts_per_team) {
   return SOPRO_OK;
 }
 
+int sopro_ar_session_set_task_shape(sopro_ar_session_t* s, int mode) {
+  if (!s) return fail(SOPRO_ERR_INVALID, "null session");
+  if (mode < 0 || mode > 2) return fail(SOPRO_ERR_INVALID, "task shape mode must be 0 (auto), 1 (wide) or 2 (narrow)");
+  s->task_shape = mode;
+  return SOPRO_OK;
+}
+
+int sopro_ar_session_stage_shapes(sopro_ar_session_t* s, int32_t* kinds, int32_t* shapes, int cap, int32_t* n_stage) {
+  if (!s) return fail(SOPRO_ERR_INVALID, "null session");
+  if (cap < 0 || (cap > 0 && (!kinds || !shapes))) return fail(SOPRO_ERR_INVALID, "stage_shapes: bad output buffers");
+  for (int i = 0; i < s->last_n_stage && i < cap; ++i) {
+    kinds[i] = s->last_prog[i].kind;
+    shapes[i] = s->last_prog[i].shape;
+  }
+  if (n_stage) *n_stage = s->last_n_stage;
+  return SOPRO_OK;
+}
+
 }  // extern "C"
 
 template <typename WT>
@@ -624,6 +645,44 @@ static int build_tiles(sopro_ar_session* s, int P, int wbuf, cudaStream_t st) {
   return SOPRO_OK;
 }
 
+// Task shape of every weight stage (ar_kernel.cuh, TaskShape).  Task i of a tile runs on warp i mod 16, and warp w issues
+// from scheduler w mod 4, so scheduler 0 carries ceil(tasks / 4) tasks of R x TUE outputs x K MACs each.  A stage takes
+// narrow when its busiest scheduler, summed over the stage's tiles and maximised over the team's ranks, carries less
+// work even after weighting by its 1.2x shared-memory bytes per MAC (1.5 against 1.25 B): measured at batch 64 (DESIGN.md
+// §3), a narrow HEAD (272 against 288 output-units per scheduler) is slower, FFN2 and O (48 against 64) are faster.
+// A tie keeps the wide shape.  The fused q + attention stage keeps its own tiles.
+static void pick_task_shapes(sopro_ar_session* s, ArParams& p, int P, int TU, int Bt) {
+  const int R = TU == 8 ? 4 : 2, RC = R / 2;
+  std::vector<int> first(P, 0);  // each rank's first tile of the stage
+  for (int si = 0; si < p.n_stage; ++si) {
+    StageOp& op = p.prog[si];
+    op.shape = SHAPE_WIDE;
+    const bool gemv = op.kind <= K_HEAD;
+    const int K = op.kind == K_FFN2 ? s->e->F : s->e->D;
+    long long load[2] = {0, 0};  // [wide, narrow]
+    for (int r = 0; r < P; ++r) {
+      const int nt = s->h_stage_tiles[(size_t)r * kMaxStages + si];
+      long long l[2] = {0, 0};
+      for (int j = 0; gemv && j < nt; ++j) {
+        const int nr = s->h_tiles[(size_t)r * kMaxTilesPerStep + first[r] + j].nrows;
+        const int n_rt = op.kind == K_GLU ? (nr + RC - 1) / RC : (nr + R - 1) / R;
+        for (int w = 0; w < 2; ++w) {
+          const int tue = w ? std::max(TU / 2, 1) : TU;
+          const long long tasks = (long long)n_rt * ((Bt + tue - 1) / tue);
+          l[w] += (tasks + 3) / 4 * R * tue * K;
+        }
+      }
+      first[r] += nt;
+      load[0] = std::max(load[0], l[0]);
+      load[1] = std::max(load[1], l[1]);
+    }
+    if (!gemv || TU < 2 || op.kind == K_GLU) continue;  // GLU is always wide: its narrow tiles measured slower
+    if (s->task_shape == 2 || (s->task_shape == 0 && 6 * load[1] < 5 * load[0])) op.shape = SHAPE_NARROW;
+  }
+  std::copy(p.prog, p.prog + p.n_stage, s->last_prog);
+  s->last_n_stage = p.n_stage;
+}
+
 template <typename WT, int TU, bool LL>
 static int launch_ar_tu(sopro_ar_session* s, ArParams& p, size_t smem, int grid, cudaStream_t st) {
   // the attention-trace export is its own instantiation, so the untraced kernel's code is not touched by it
@@ -805,6 +864,8 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
     p.prog[n++] = {K_SAMPLE, 0};
     p.n_stage = n;
   }
+  const int TU = Bt >= 8 ? 8 : Bt >= 4 ? 4 : Bt >= 2 ? 2 : 1;
+  pick_task_shapes(s, p, P, TU, Bt);
   const int grid = g * P;
   // activation exchange: LL protocol (flag-in-data, no barrier) for small teams, where the step is latency
   // bound; team barrier for large teams, where LL's doubled activation traffic costs more than the barrier
@@ -814,14 +875,14 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   if (sync_env && strcmp(sync_env, "barrier") == 0) ll = false;
   if (sync_env && strcmp(sync_env, "ll") == 0) ll = true;
   if (ll) {
-    if (Bt >= 8) return launch_ar_tu<WT, 8, true>(s, p, smem, grid, st);
-    if (Bt >= 4) return launch_ar_tu<WT, 4, true>(s, p, smem, grid, st);
-    if (Bt >= 2) return launch_ar_tu<WT, 2, true>(s, p, smem, grid, st);
+    if (TU == 8) return launch_ar_tu<WT, 8, true>(s, p, smem, grid, st);
+    if (TU == 4) return launch_ar_tu<WT, 4, true>(s, p, smem, grid, st);
+    if (TU == 2) return launch_ar_tu<WT, 2, true>(s, p, smem, grid, st);
     return launch_ar_tu<WT, 1, true>(s, p, smem, grid, st);
   }
-  if (Bt >= 8) return launch_ar_tu<WT, 8, false>(s, p, smem, grid, st);
-  if (Bt >= 4) return launch_ar_tu<WT, 4, false>(s, p, smem, grid, st);
-  if (Bt >= 2) return launch_ar_tu<WT, 2, false>(s, p, smem, grid, st);
+  if (TU == 8) return launch_ar_tu<WT, 8, false>(s, p, smem, grid, st);
+  if (TU == 4) return launch_ar_tu<WT, 4, false>(s, p, smem, grid, st);
+  if (TU == 2) return launch_ar_tu<WT, 2, false>(s, p, smem, grid, st);
   return launch_ar_tu<WT, 1, false>(s, p, smem, grid, st);
 }
 

@@ -43,6 +43,8 @@ constexpr int kMaxStages = 6 * kMaxLayers + 2;
 constexpr int kMaxTilesPerStep = 128;
 constexpr int kMaxWBuf = 8;
 
+__host__ __device__ constexpr int ilog2(int n) { return n > 1 ? 1 + ilog2(n / 2) : 0; }
+
 // fma of an element pair, one rounding per element
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
@@ -100,8 +102,12 @@ struct TileDesc {
 };
 static_assert(sizeof(TileDesc) == 64, "the weight ring is sized around an 8 KB tile table");
 
+// Warp task of a GEMV stage: R weight rows x TU utterances (wide) or R x TU/2 (narrow, TU >= 2).  The host picks
+// the shape per stage (launch_ar); both accumulate every output in the same order, so the choice never changes a bit.
+enum TaskShape { SHAPE_WIDE = 0, SHAPE_NARROW = 1 };
+
 struct StageOp {
-  unsigned char kind, layer;
+  unsigned char kind, layer, shape;
 };
 
 struct ArParams {
@@ -442,7 +448,8 @@ __device__ __forceinline__ float reduce_transposed<1>(float (&v)[1], int lane) {
   return warp_sum(v[0]);
 }
 
-template <int R, int TU, typename WT>
+// UNROLL: K-loop unroll (the narrow task shape passes 1: the step's instructions must stay near the instruction cache)
+template <int R, int TU, typename WT, int UNROLL = (R * TU >= 32 ? 1 : 3)>
 __device__ __forceinline__ float warp_rows_s(const unsigned (&w)[R], unsigned act, int K, int lane) {
   float2 acc[R][TU];
 #pragma unroll
@@ -450,7 +457,7 @@ __device__ __forceinline__ float warp_rows_s(const unsigned (&w)[R], unsigned ac
 #pragma unroll
     for (int u = 0; u < TU; ++u) acc[r][u] = make_float2(0.f, 0.f);
   // big register tiles (64 float2 accumulators) leave no room for unrolled loads
-#pragma unroll(R * TU >= 32 ? 1 : 3)
+#pragma unroll(UNROLL)
   for (int k = lane * 4; k < K; k += 128) {
     float4 wv[R];
 #pragma unroll
@@ -1422,7 +1429,6 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
   const unsigned act_s = smem_u32(act);
   float* xraw = act + (size_t)tc.nb * D;  // second [nb][D] buffer (GLU stage only)
   const unsigned scratch_s = act_s + (unsigned)(2 * tc.nb * D) * 4u;  // GLU stage: dwconv tap rows
-  const int n_ut = (tc.nb + TU - 1) / TU;
   // ---- weight ring: [act region][nbuf x wbuf][tile table]
   WeightRing ring;
   {
@@ -1563,20 +1569,27 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
         float* state = p.ring + L.ring_off;
         const int dil = L.dil;
         const int phase = conv_phase[li], slot_now = conv_slot[li];
+        // a task = R weight rows x tue utterances (tue = TU, or TU / 2 for a narrow stage); GLU: R/2 channels (value
+        // rows, then their gate rows).  Only the K loop and its reduction are compiled once per shape.
+        constexpr int R = (TU == 8) ? 4 : 2;
+        constexpr int RC = R / 2;
+        constexpr int TUN = TU >= 2 ? TU / 2 : TU;  // the TU = 1 instantiation has one shape
+        const bool narrow = TUN != TU && p.prog[si].shape == SHAPE_NARROW;
+        const int lg_tue = narrow ? ilog2(TUN) : ilog2(TU);
+        const int tue = 1 << lg_tue;
+        const int sh = 5 - ilog2(R) - lg_tue;  // after the transposed reduction lane L owns output (L >> sh) & (R*tue-1)
+        const int n_ut = (tc.nb + tue - 1) >> lg_tue;
 #pragma unroll 1
       for (int ti = stage_tiles[si]; ti > 0; --ti) {
         const TileDesc* td;
         const unsigned wb = ring.acquire(td);
         const int nr = td->nrows;
-        // a task = R weight rows x TU utterances; GLU: R/2 channels (value rows, then their gate rows)
-        constexpr int R = (TU == 8) ? 4 : 2;
-        constexpr int RC = R / 2;
         const int n_rt = glu ? (nr + RC - 1) / RC : (nr + R - 1) / R;
         const unsigned epi_s = wb + td->bytes0 + td->bytes1;
 #pragma unroll 1
         for (int task = warp; task < n_rt * n_ut; task += kWarps) {
           const int rt = n_ut == 1 ? task : (int)((unsigned)task / (unsigned)n_ut);
-          const int u0 = (task - rt * n_ut) * TU;
+          const int u0 = (task - rt * n_ut) << lg_tue;
           unsigned wr[R];
 #pragma unroll
           for (int jr = 0; jr < R; ++jr) {
@@ -1587,14 +1600,10 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
               wr[jr] = wb + (unsigned)min(rt * R + jr, nr - 1) * row_bytes;
             }
           }
-          const int ub = min(u0, max(tc.nb - TU, 0));
-          // after the transposed reduction lane L owns output o = (L >> SH) & (R*TU-1) = i*TU + uu
-          constexpr int NOUT = R * TU;
-          constexpr int LOG2N = (NOUT == 2 ? 1 : NOUT == 4 ? 2 : NOUT == 8 ? 3 : NOUT == 16 ? 4 : 5);
-          constexpr int SH = 5 - LOG2N;
-          const int o = (lane >> SH) & (NOUT - 1);
-          const int i = o / TU, uu = o % TU;
-          const bool writer = (lane & ((1 << SH) - 1)) == 0;
+          const int ub = min(u0, max(tc.nb - tue, 0));
+          const int o = (lane >> sh) & ((R << lg_tue) - 1);  // = i*tue + uu
+          const int i = o >> lg_tue, uu = o & (tue - 1);
+          const bool writer = (lane & ((1 << sh) - 1)) == 0;
           const int ri = glu ? rt * RC + i : rt * R + i;
           const int u = ub + uu;
           const bool mine = writer && (glu ? i < RC : true) && ri < nr && u >= u0 && u < tc.nb;
@@ -1604,9 +1613,9 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
           // operands of the epilogue are requested before the K loop: their latency hides under it
           float res_v = 0.f;
           float* rb = nullptr;
-          // one tap row per (channel of the task, utterance): kTapSlots = 16 rows per warp (RC <= 2 channels x TU <= 8)
+          // one tap row per (channel of the task, utterance): kTapSlots = 16 rows per warp (RC <= 2 channels x tue <= 8)
           const unsigned tap_w = scratch_s + (unsigned)warp * (unsigned)(kTapSlots * p.KcP * 4) +
-                                 (unsigned)((i % RC) * TU + uu) * (unsigned)(p.KcP * 4);
+                                 (unsigned)((i % RC) * tue + uu) * (unsigned)(p.KcP * 4);
           if (glu) {
             // conv state row of (utterance, channel, phase): [KcP] floats, see DESIGN.md §2
             rb = state + (((size_t)b * D + (mine ? r : td->row0)) * dil + phase) * p.KcP;
@@ -1616,9 +1625,10 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
             res_v = ldcg1(d);  // own slice: written by this CTA at an earlier stage (value word)
           }
           cp_async_commit();
-          float v = warp_rows_s<R, TU, WT>(wr, act_s + (unsigned)ub * (unsigned)K * 4u, K, lane);
-          // GLU: the gate total of (channel i, utterance uu) lives in the lanes of output (RC + i)*TU + uu
-          const float gate_v = __shfl_sync(0xffffffffu, v, (((RC + (i % RC)) * TU + uu) << SH) & 31);
+          const unsigned xa = act_s + (unsigned)ub * (unsigned)K * 4u;
+          float v = narrow ? warp_rows_s<R, TUN, WT, 1>(wr, xa, K, lane) : warp_rows_s<R, TU, WT>(wr, xa, K, lane);
+          // GLU: the gate total of (channel i, utterance uu) lives in the lanes of output (RC + i)*tue + uu
+          const float gate_v = __shfl_sync(0xffffffffu, v, (((RC + (i % RC)) * tue + uu) << sh) & 31);
           cp_async_wait0();
           if (mine) {
             if (glu) {

@@ -225,6 +225,19 @@ class ArSession:
         self._timing = buf
         _lib.check(self.lib.sopro_ar_set_timing(self._h, buf.data_ptr() if buf is not None else None, int(step)))
 
+    STAGE_KINDS = ("glu", "ffn1", "ffn2", "q", "o", "head", "att", "sample", "qatt")
+
+    def set_task_shape(self, mode: int) -> None:
+        """GEMV warp task shape of later launches: 0 = picked per stage (default), 1 = always wide, 2 = narrow wherever
+        the kernel has it (every GEMV stage but GLU, teams of at least two utterances)."""
+        _lib.check(self.lib.sopro_ar_session_set_task_shape(self._h, int(mode)))
+
+    def stage_shapes(self):
+        """[(kind, "wide" | "narrow")] of every stage of the last launch, in program order."""
+        kinds, shapes, n = (C.c_int32 * 128)(), (C.c_int32 * 128)(), C.c_int32()
+        _lib.check(self.lib.sopro_ar_session_stage_shapes(self._h, kinds, shapes, 128, C.byref(n)))
+        return [(self.STAGE_KINDS[kinds[i]], ("wide", "narrow")[shapes[i]]) for i in range(n.value)]
+
     def sampled(self) -> torch.Tensor:
         out = torch.empty((self.batch, self.steps), dtype=torch.int32, device=self.engine.device)
         _lib.check(self.lib.sopro_ar_debug_sampled(self._h, out.data_ptr(), _lib.stream_ptr(self.engine.device)))

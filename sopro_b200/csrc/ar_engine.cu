@@ -133,17 +133,8 @@ int sopro_engine_create(const sopro_ar_config_t* cfg, const sopro_ar_weights_t* 
                         sopro_engine_t** out) {
   if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0)
-    return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device (%s); this engine has no CPU fallback",
-                ce == cudaSuccess ? "device count 0" : cudaGetErrorString(ce));
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range [0,%d)", device, ndev);
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9)
-    return fail(SOPRO_ERR_UNSUPPORTED, "device %d is sm_%d%d; this build targets sm_90a only", device, prop.major,
-                prop.minor);
+  const int rc = open_device(device, "the AR engine");
+  if (rc != SOPRO_OK) return rc;
   const int D = cfg->d_model, NL = cfg->n_layers, Kc = cfg->kernel, H = cfg->n_heads, V = cfg->vocab;
   if (D <= 0 || D % 4 != 0) return fail(SOPRO_ERR_INVALID, "d_model must be a positive multiple of 4 (got %d)", D);
   if (NL <= 0 || NL > kMaxLayers) return fail(SOPRO_ERR_INVALID, "n_layers must be in [1,%d]", kMaxLayers);
@@ -157,11 +148,12 @@ int sopro_engine_create(const sopro_ar_config_t* cfg, const sopro_ar_weights_t* 
   if (w->cb_embed_rows < V || w->bos_row < 0 || w->bos_row >= w->cb_embed_rows)
     return fail(SOPRO_ERR_INVALID, "cb_embed has %lld rows, need >= vocab %d and a valid bos_row",
                 (long long)w->cb_embed_rows, V);
-  CK(cudaSetDevice(device));
+  int n_sms = 0;
+  CK(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device));
 
   sopro_engine* e = new sopro_engine();
   e->device = device;
-  e->n_sms = prop.multiProcessorCount;
+  e->n_sms = n_sms;
   e->cfg = *cfg;
   e->D = D;
   e->F = 4 * D;

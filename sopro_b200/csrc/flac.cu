@@ -23,10 +23,9 @@
 
 #include <algorithm>
 #include <cstdio>
-#include <cstdlib>
 
 #include "../../include/sopro_b200.h"
-#include "common.cuh"
+#include "chunk_stream.cuh"
 
 namespace {
 
@@ -697,15 +696,6 @@ __global__ void __launch_bounds__(kT) flac_pack_kernel(Job J, Rows Rw, const Des
   for (int j = tid; j < d.bytes; j += kT) o[j] = (unsigned char)get_byte(sm.w, j);
 }
 
-// the stream's carry: dst[i] = (carry ++ x)[from + i] for i < cnt (cnt < 16)
-__global__ void flac_carry_kernel(const float* carry, int carry_n, const float* x, long long from, int cnt, float* dst) {
-  const int i = threadIdx.x;
-  if (i < cnt) {
-    const long long g = from + i;
-    dst[i] = g < carry_n ? carry[g] : x[g - carry_n];
-  }
-}
-
 __global__ void flac_zero_kernel(long long* p) { *p = 0; }
 
 // workspace: the descriptors, the frame offsets and the cursor of one launch's blocks
@@ -734,8 +724,9 @@ long long out_bound(long long n, bool header) {
   return (header ? kInfoBytes : 0) + blocks_of(n) * (kMaxHdr + 1 + 2) + 2 * n;
 }
 
-// rows [0, B) of the job in launches of 128 rows; row b's bytes land at out + row_off[b], its size in row_bytes[b]
-int run(Job J, int B, const long long* lens, char* ws, const Layout& l, unsigned char* out, long long* row_off,
+// rows [0, B) of the job in launches of 128 rows, row b lens[b] samples long (x_stride each when lens is null); row b's
+// bytes land at out + row_off[b], its size in row_bytes[b]
+int run(Job J, int B, const int64_t* lens, long long x_stride, char* ws, const Layout& l, unsigned char* out, long long* row_off,
         long long* row_bytes, cudaStream_t st) {
   Desc* desc = reinterpret_cast<Desc*>(ws + l.desc);
   long long* foff = reinterpret_cast<long long*>(ws + l.foff);
@@ -745,10 +736,11 @@ int run(Job J, int B, const long long* lens, char* ws, const Layout& l, unsigned
   const Src src0 = J.src;
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
+    const RowLens<kRowsPerLaunch> L = row_lens<kRowsPerLaunch>(lens, x_stride, b0, rows);
     Rows R{};
     R.blk0[0] = 0;
     for (int i = 0; i < rows; ++i) {
-      R.len[i] = lens[b0 + i];
+      R.len[i] = L.v[i];
       R.blk0[i + 1] = R.blk0[i] + blocks_of(R.len[i]);
     }
     J.rows = rows;
@@ -770,11 +762,11 @@ int run(Job J, int B, const long long* lens, char* ws, const Layout& l, unsigned
 
 }  // namespace
 
+// the tail holds the carried samples [samples, samples + carried), samples emitted in frames so far being the next
+// frame's number
 struct SoproFlacStream {
   int sr = 0;
-  float* carry[2] = {nullptr, nullptr};
-  int cur = 0, carry_n = 0;
-  long long samples = 0;  // samples emitted in frames so far: the next frame's number
+  chunk::Tail tail;
 };
 
 extern "C" {
@@ -791,25 +783,10 @@ int sopro_flac_sizes(int32_t B, int64_t max_len, int32_t sr, int64_t* ws_bytes, 
 int sopro_flac_encode(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, void* ws,
                       uint8_t* out, int64_t* row_off, int64_t* row_bytes, void* stream) {
   if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
-  if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
   if (!ws || !out || !row_off || !row_bytes) return fail(SOPRO_ERR_INVALID, "null argument");
   long long most = 0;
-  long long* lens = static_cast<long long*>(malloc(sizeof(long long) * B));
-  if (!lens) return fail(SOPRO_ERR_INVALID, "out of host memory");
-  for (int b = 0; b < B; ++b) {
-    lens[b] = lens_host ? lens_host[b] : x_stride;
-    if (lens[b] < 0 || lens[b] > x_stride) {
-      const long long v = lens[b];
-      free(lens);
-      return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, v, (long long)x_stride);
-    }
-    most = std::max(most, lens[b]);
-  }
-  if (!x && most > 0) {
-    free(lens);
-    return fail(SOPRO_ERR_INVALID, "null argument");
-  }
+  const int rc = check_rows(x, B, x_stride, lens_host, kMaxLen, &most);
+  if (rc != SOPRO_OK) return rc;
   Job J{};
   J.src = Src{x, x_stride, nullptr, 0};
   J.variable = 0;
@@ -817,10 +794,8 @@ int sopro_flac_encode(const float* x, int32_t B, int64_t x_stride, const int64_t
   J.sr = sr;
   J.sr_code = rate_code(sr);
   J.header = 1;
-  const int rc = run(J, B, lens, static_cast<char*>(ws), layout(B, most), out, reinterpret_cast<long long*>(row_off),
-                     reinterpret_cast<long long*>(row_bytes), reinterpret_cast<cudaStream_t>(stream));
-  free(lens);
-  return rc;
+  return run(J, B, lens_host, x_stride, static_cast<char*>(ws), layout(B, most), out, reinterpret_cast<long long*>(row_off),
+             reinterpret_cast<long long*>(row_bytes), reinterpret_cast<cudaStream_t>(stream));
 }
 
 int sopro_flac_stream_create(int32_t sr, SoproFlacStream** out) {
@@ -829,13 +804,10 @@ int sopro_flac_stream_create(int32_t sr, SoproFlacStream** out) {
   if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   SoproFlacStream* s = new SoproFlacStream();
   s->sr = sr;
-  for (int i = 0; i < 2; ++i) {
-    const cudaError_t e = cudaMalloc(&s->carry[i], kStreamMin * sizeof(float));
-    if (e != cudaSuccess) {
-      cudaFree(s->carry[0]);
-      delete s;
-      return fail(SOPRO_ERR_CUDA, "cudaMalloc failed: %s", cudaGetErrorString(e));
-    }
+  const cudaError_t e = s->tail.alloc(kStreamMin);
+  if (e != cudaSuccess) {
+    sopro_flac_stream_destroy(s);
+    return fail(SOPRO_ERR_CUDA, "flac stream state: %s", cudaGetErrorString(e));
   }
   *out = s;
   return SOPRO_OK;
@@ -843,8 +815,7 @@ int sopro_flac_stream_create(int32_t sr, SoproFlacStream** out) {
 
 int sopro_flac_stream_destroy(SoproFlacStream* s) {
   if (!s) return SOPRO_OK;
-  cudaFree(s->carry[0]);
-  cudaFree(s->carry[1]);
+  s->tail.release();
   delete s;
   return SOPRO_OK;
 }
@@ -853,17 +824,16 @@ int sopro_flac_stream_reset(SoproFlacStream* s, int32_t sr) {
   if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
   if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
   s->sr = sr;
-  s->carry_n = 0;
-  s->samples = 0;
+  s->tail.restart(0);
   return SOPRO_OK;
 }
 
-int64_t sopro_flac_stream_carried(const SoproFlacStream* s) { return s ? s->carry_n : -1; }
+int64_t sopro_flac_stream_carried(const SoproFlacStream* s) { return s ? s->tail.held() : -1; }
 
 static int stream_encode(SoproFlacStream* s, const float* x, long long n, void* ws, uint8_t* out, int64_t* nbytes, bool last,
                          void* stream) {
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const long long total = s->carry_n + n;
+  const long long total = s->tail.held() + n;
   long long keep = total % kBlock;
   if (last || keep >= kStreamMin) keep = 0;
   const long long enc = total - keep;
@@ -871,28 +841,20 @@ static int stream_encode(SoproFlacStream* s, const float* x, long long n, void* 
   const Layout l = layout(1, total);
   long long* roff = reinterpret_cast<long long*>(w + l.roff);
   Job J{};
-  J.src = Src{x, 0, s->carry[s->cur], s->carry_n};
+  J.src = Src{x, 0, s->tail.data(), (int)s->tail.held()};
   J.variable = 1;
-  J.num0 = s->samples;
+  J.num0 = s->tail.base;
   J.sr = s->sr;
   J.sr_code = rate_code(s->sr);
   J.header = 0;
-  const long long lens[1] = {enc};
-  int rc = run(J, 1, lens, w, l, out, roff, reinterpret_cast<long long*>(nbytes), st);
-  if (rc != SOPRO_OK) return rc;
-  if (keep > 0) {
-    flac_carry_kernel<<<1, 32, 0, st>>>(s->carry[s->cur], s->carry_n, x, enc, (int)keep, s->carry[s->cur ^ 1]);
-    CK(cudaGetLastError());
-    s->cur ^= 1;
-  }
-  s->carry_n = (int)keep;
-  s->samples += enc;
-  return SOPRO_OK;
+  const int64_t lens[1] = {enc};
+  const int rc = run(J, 1, lens, 0, w, l, out, roff, reinterpret_cast<long long*>(nbytes), st);
+  return rc == SOPRO_OK ? s->tail.keep(s->tail.base + enc, x, n, st) : rc;
 }
 
 int sopro_flac_stream_push(SoproFlacStream* s, const float* x, int64_t n, void* ws, uint8_t* out, int64_t* nbytes, void* stream) {
   if (!s || !ws || !out || !nbytes || (!x && n > 0)) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (n < 0 || n > kMaxLen - s->samples - s->carry_n) return fail(SOPRO_ERR_INVALID, "push of %lld samples refused", (long long)n);
+  if (n < 0 || n > kMaxLen - s->tail.seen) return fail(SOPRO_ERR_INVALID, "push of %lld samples refused", (long long)n);
   return stream_encode(s, x, n, ws, out, nbytes, false, stream);
 }
 
@@ -900,8 +862,7 @@ int sopro_flac_stream_finish(SoproFlacStream* s, void* ws, uint8_t* out, int64_t
   if (!s || !ws || !out || !nbytes) return fail(SOPRO_ERR_INVALID, "null argument");
   const int rc = stream_encode(s, nullptr, 0, ws, out, nbytes, true, stream);
   if (rc != SOPRO_OK) return rc;
-  s->carry_n = 0;
-  s->samples = 0;
+  s->tail.restart(0);
   return SOPRO_OK;
 }
 

@@ -157,22 +157,14 @@ int sopro_longform_fade(int32_t F, float* f) {
 
 int sopro_longform_extents(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int64_t* ext, void* stream) {
   if (!ext) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
   long long most = 0;
-  for (int b = 0; b < B; ++b) {
-    const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride)
-      return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
-    most = std::max(most, len);
-  }
-  if (!x && most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
+  const int rc = check_rows(x, B, x_stride, lens_host, kMaxLen, &most);
+  if (rc != SOPRO_OK) return rc;
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens<kRowsPerLaunch> L{};
-    for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
-    extents_kernel<<<rows, kExtThreads, 0, st>>>(x + (long long)b0 * x_stride, x_stride, L,
+    extents_kernel<<<rows, kExtThreads, 0, st>>>(x + (long long)b0 * x_stride, x_stride,
+                                                 row_lens<kRowsPerLaunch>(lens_host, x_stride, b0, rows),
                                                  reinterpret_cast<long long*>(ext) + 2LL * b0);
     CK(cudaGetLastError());
   }

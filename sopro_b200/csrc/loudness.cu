@@ -443,16 +443,7 @@ __global__ void __launch_bounds__(kT) loud_apply_kernel(const float* x, long lon
 int check_batch(const float* x, int B, long long x_stride, const int64_t* lens_host, int sr, void* ws, long long* most) {
   if (!ws) return fail(SOPRO_ERR_INVALID, "null argument");
   if (!valid_rate(sr)) return fail(SOPRO_ERR_INVALID, "sample rate %d not in [%d, %d]", sr, kMinRate, kMaxRate);
-  if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, x_stride);
-  *most = 0;
-  for (int b = 0; b < B; ++b) {
-    const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, x_stride);
-    *most = std::max(*most, len);
-  }
-  if (!x && *most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
-  return SOPRO_OK;
+  return check_rows(x, B, x_stride, lens_host, kMaxLen, most);
 }
 
 // the meter over rows [b0, b0 + rows): L -> lufs[b0 ..], and with `normalize` g -> gain[b0 ..]
@@ -518,8 +509,7 @@ int sopro_loudness_measure(const float* x, int32_t B, int64_t x_stride, const in
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens<kRowsPerLaunch> L{};
-    for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
+    const RowLens<kRowsPerLaunch> L = row_lens<kRowsPerLaunch>(lens_host, x_stride, b0, rows);
     const int r = run_meter(f, gt, l, x, x_stride, L, b0, rows, static_cast<char*>(ws), lufs_dev, 0, 0.0, nullptr, st);
     if (r != SOPRO_OK) return r;
   }
@@ -530,10 +520,9 @@ int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const 
                              float* y, int64_t y_stride, void* ws, double* lufs_dev, float* gain_dev, void* stream) {
   if (!valid_target(T)) return fail(SOPRO_ERR_INVALID, "loudness target must be a real number in [-60, 0] LUFS (got %g)", T);
   long long most = 0;
-  const int rc = check_batch(x, B, x_stride, lens_host, sr, ws, &most);
+  int rc = check_batch(x, B, x_stride, lens_host, sr, ws, &most);
+  if (rc == SOPRO_OK) rc = check_out_rows(y, B, y_stride, most);
   if (rc != SOPRO_OK) return rc;
-  if (!y && most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (B > 1 && y_stride < most) return fail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld samples", (long long)y_stride, most);
   const Filt f = make_filt(sr);
   const Gate gt = make_gate(sr);
   const Layout l = layout(B, most, sr);
@@ -543,8 +532,7 @@ int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const 
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens<kRowsPerLaunch> L{};
-    for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
+    const RowLens<kRowsPerLaunch> L = row_lens<kRowsPerLaunch>(lens_host, x_stride, b0, rows);
     const int r = run_meter(f, gt, l, x, x_stride, L, b0, rows, w, lufs, 1, T, gain, st);
     if (r != SOPRO_OK) return r;
     if (most > 0) {

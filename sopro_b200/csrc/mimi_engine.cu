@@ -546,18 +546,12 @@ extern "C" {
 int sopro_mimi_create(const sopro_mimi_config_t* cfg, const sopro_mimi_weights_t* w, int device, sopro_mimi_t** out) {
   if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the Mimi decoder has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  const int rc = open_device(device, "the Mimi decoder");
+  if (rc != SOPRO_OK) return rc;
   const int C = cfg->hidden, Dc = cfg->codebook_dim, Q = cfg->n_q, V = cfg->vocab, NL = cfg->n_layers, FF = cfg->ffn;
   if (C % 64 || Dc % 4 || C != 2 * Dc || NL < 1 || cfg->n_ratios < 1 || cfg->n_ratios > 8 || cfg->n_heads < 1 || C % cfg->n_heads ||
       (C / cfg->n_heads) % 4 || FF % 16)
     return fail(SOPRO_ERR_INVALID, "unsupported Mimi geometry (hidden=%d codebook_dim=%d)", C, Dc);
-  CK(cudaSetDevice(device));
   sopro_mimi* m = new sopro_mimi();
   m->device = device;
   m->cfg = *cfg;
@@ -1634,19 +1628,13 @@ int sopro_mimi_encoder_create(const sopro_mimi_config_t* cfg, const sopro_mimi_e
                               sopro_mimi_encoder_t** out) {
   if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the Mimi encoder has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  const int rc = open_device(device, "the Mimi encoder");
+  if (rc != SOPRO_OK) return rc;
   const int C = cfg->hidden, Dc = cfg->codebook_dim, Q = cfg->n_q, V = cfg->vocab, NL = cfg->n_layers, FF = cfg->ffn, F0 = cfg->num_filters;
   if (C % 64 || Dc != 256 || C != 2 * Dc || NL < 1 || NL > SOPRO_MIMI_MAX_LAYERS || cfg->n_ratios < 1 || cfg->n_ratios > SOPRO_MIMI_MAX_RATIOS ||
       cfg->n_heads < 1 || C % cfg->n_heads || (C / cfg->n_heads) % 4 || FF % 16 || F0 % 16 || cfg->compress != 2 || Q < 1 || cfg->n_sem < 1 ||
       cfg->n_sem > Q || cfg->kernel < 1 || cfg->kernel > 16)
     return fail(SOPRO_ERR_INVALID, "unsupported Mimi encoder geometry (hidden=%d codebook_dim=%d)", C, Dc);
-  CK(cudaSetDevice(device));
   sopro_mimi_encoder* e = new sopro_mimi_encoder();
   e->device = device;
   e->cfg = *cfg;

@@ -423,13 +423,8 @@ extern "C" {
 int sopro_nar_create(const sopro_nar_config_t* cfg, const sopro_nar_weights_t* w, int device, sopro_nar_t** out) {
   if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the NAR refiner has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  const int rc = open_device(device, "the NAR refiner");
+  if (rc != SOPRO_OK) return rc;
   const int D = cfg->d_model, NL = cfg->n_layers, k = cfg->kernel, Q = cfg->n_codebooks, V = cfg->codebook_size, Hn = cfg->head_dim,
             AH = cfg->adapter_hidden, NS = cfg->n_stages;
   if (D < 32 || D > 512 || D % 16 || Hn % 16 || NL < 1 || NL > SOPRO_MAX_SSM_LAYERS || k < 1 || k > 64 || Q < 2 || Q > SOPRO_NAR_MAX_CODEBOOKS ||
@@ -450,7 +445,6 @@ int sopro_nar_create(const sopro_nar_config_t* cfg, const sopro_nar_weights_t* w
         return fail(SOPRO_ERR_INVALID, "NAR stage %d head %d: null weight or codebook out of range", s, j);
     covered += cfg->stage_count[s];
   }
-  CK(cudaSetDevice(device));
   sopro_nar* n = new sopro_nar();
   n->device = device;
   n->cfg = *cfg;
@@ -1007,13 +1001,8 @@ extern "C" {
 int sopro_prefill_create(const sopro_prefill_config_t* cfg, const sopro_prefill_weights_t* w, int device, sopro_prefill_t** out) {
   if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the prefill has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  const int rc = open_device(device, "the prefill");
+  if (rc != SOPRO_OK) return rc;
   const int D = cfg->d_model, NL = cfg->n_layers_text, k = cfg->text_kernel, SV = cfg->sv_dim, RL = cfg->ref_layers, H = cfg->ref_heads;
   if (D < 32 || D > 512 || D % 16 || NL < 0 || NL > SOPRO_MAX_SSM_LAYERS || k < 1 || k > 64 || SV < 16 || SV % 16 || RL < 0 ||
       RL > SOPRO_PREFILL_MAX_REF_LAYERS || H < 1 || D % H || (D / H) % 4 || cfg->text_vocab < 1 || cfg->max_text_len < 1 || cfg->max_frames_pos < 1)
@@ -1025,7 +1014,6 @@ int sopro_prefill_create(const sopro_prefill_config_t* cfg, const sopro_prefill_
     return fail(SOPRO_ERR_INVALID, "prefill: null weight pointer");
   for (int i = 0; i < RL; ++i)
     if (!w->ref_layer[i].nq_w || !w->ref_layer[i].q_w || !w->ref_layer[i].o_w) return fail(SOPRO_ERR_INVALID, "ref layer %d: null weight", i);
-  CK(cudaSetDevice(device));
   sopro_prefill* p = new sopro_prefill();
   p->device = device;
   p->cfg = *cfg;
@@ -1395,13 +1383,8 @@ extern "C" {
 int sopro_refprep_create(const sopro_refprep_config_t* cfg, const sopro_refprep_weights_t* w, int device, sopro_refprep_t** out) {
   if (!cfg || !w || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev <= 0) return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the reference preparation has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
+  const int rc = open_device(device, "the reference preparation");
+  if (rc != SOPRO_OK) return rc;
   const int D = cfg->d_model, d = cfg->sv_embed_dim, SV = cfg->sv_dim, Q = cfg->n_codebooks, V = cfg->codebook_size, NL = cfg->ref_enc_layers,
             RL = cfg->ref_layers, H = cfg->ref_heads;
   if (D < 32 || D > 512 || D % 16 || d < 16 || d % 16 || SV < 16 || SV % 16 || Q < 1 || Q > 64 || V < 1 || NL < 0 || NL > SOPRO_MAX_SSM_LAYERS ||
@@ -1415,7 +1398,6 @@ int sopro_refprep_create(const sopro_refprep_config_t* cfg, const sopro_refprep_
     if (!block_ok(w->ref_block[i])) return fail(SOPRO_ERR_INVALID, "reference encoder block %d: null weight", i);
   for (int i = 0; i < RL; ++i)
     if (!w->layer[i].nkv_w || !w->layer[i].k_w || !w->layer[i].v_w) return fail(SOPRO_ERR_INVALID, "ref layer %d: null weight", i);
-  CK(cudaSetDevice(device));
   sopro_refprep* p = new sopro_refprep();
   p->device = device;
   p->cfg = *cfg;

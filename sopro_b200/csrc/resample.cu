@@ -19,9 +19,12 @@
 #include <vector>
 
 #include "../../include/sopro_b200.h"
-#include "common.cuh"
+#include "chunk_stream.cuh"
 
 namespace {
+
+using chunk::Src;
+using chunk::src_at;
 
 constexpr int kThreads = 256;
 constexpr int kMaxPerThread = 8;         // outputs per thread: tiles of up to 2048 outputs per CTA
@@ -39,14 +42,6 @@ struct Geo {
   int S;            // row stride of the tap table (the longest span)
   int tile;         // outputs per CTA
   int tab_smem;     // the tap table and the phase spans are staged in shared memory
-};
-
-// where the input sample at logical index k comes from: [0, split) from a (a[k - a_base]), [split, limit) from b
-// (b[k - split]), zero elsewhere -- the one-shot path has a single source, a stream its carried tail and the new chunk
-struct Src {
-  const float* a;
-  const float* b;
-  long long a_base, split, limit;
 };
 
 // rates -> (o, n, width), or a message on refusal.  Pure host arithmetic.
@@ -117,11 +112,6 @@ int make_filter(int32_t sr_in, int32_t sr_out, Filter* f) {
 }
 
 long long out_len(int o, int n, long long n_in) { return (n * n_in + o - 1) / o; }
-
-__device__ __forceinline__ float src_at(const Src& s, long long k) {
-  if (k < 0 || k >= s.limit) return 0.0f;
-  return k < s.split ? s.a[k - s.a_base] : s.b[k - s.split];
-}
 
 // One output sample: its phase's nonzero taps against the staged input from the span's first sample on, one fp32 FMA
 // chain in increasing input index.  Every output of either kernel is summed here.
@@ -200,13 +190,10 @@ struct sopro_resampler {
   size_t smem = 0;
 };
 
-struct sopro_resampler_stream {
+// the tail holds the logical input [q_done * o - width, n_seen) of the utterance
+struct sopro_resampler_stream : chunk::ChunkStream {
   sopro_resampler* r = nullptr;
-  long long max_chunk = 0;
-  float* carry[2] = {nullptr, nullptr};  // ping-pong: logical input [q_done * o - width, n_seen) of the utterance
-  int cur = 0;
-  long long n_seen = 0, q_done = 0;      // input samples pushed, blocks of n outputs emitted
-  bool finished = false;
+  long long q_done = 0;  // blocks of n outputs emitted
 };
 
 namespace {
@@ -250,16 +237,9 @@ int sopro_resampler_create(int32_t sr_in, int32_t sr_out, int device, sopro_resa
   if (!out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
   Filter f;
-  const int rc = make_filter(sr_in, sr_out, &f);  // refuses a rate before anything touches the device
+  int rc = make_filter(sr_in, sr_out, &f);  // refuses a rate before anything touches the device
+  if (rc == SOPRO_OK) rc = open_device(device, "the resampler");
   if (rc != SOPRO_OK) return rc;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
-    return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the resampler has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9) return fail(SOPRO_ERR_UNSUPPORTED, "device is sm_%d%d; this build targets sm_90a only", prop.major, prop.minor);
-  CK(cudaSetDevice(device));
   Geo g{f.o, f.n, f.width, f.S, 0, f.n * f.S <= kTabSmemFloats ? 1 : 0};
   for (int per = kMaxPerThread; per >= 1; per /= 2) {  // the largest tile whose input window fits the staging budget
     g.tile = per * kThreads;
@@ -300,23 +280,19 @@ int sopro_resample(sopro_resampler_t* r, const float* x, int32_t B, int64_t x_st
                    int64_t y_stride, void* stream) {
   if (!r || !x || !y) return fail(SOPRO_ERR_INVALID, "null argument");
   const Geo& g = r->g;
-  if (B < 1 || x_stride < 0 || x_stride > (1LL << 40)) return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
   long long most = 0;
-  for (int b = 0; b < B; ++b) {
-    const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
-    most = std::max(most, out_len(g.o, g.n, len));
-  }
-  if (B > 1 && y_stride < most) return fail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld outputs", (long long)y_stride, most);
+  int rc = check_rows(x, B, x_stride, lens_host, 1LL << 40, &most);
+  if (rc != SOPRO_OK) return rc;
+  most = out_len(g.o, g.n, most);  // out_len is monotone in the row length
+  if ((rc = check_out_rows(y, B, y_stride, most)) != SOPRO_OK) return rc;
   if (most == 0) return SOPRO_OK;
   CK(cudaSetDevice(r->device));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const unsigned tiles = (unsigned)((most + g.tile - 1) / g.tile);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens<kRowsPerLaunch> L{};
-    for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
-    resample_batch_kernel<<<dim3(tiles, rows), kThreads, r->smem, st>>>(g, r->tab, r->meta, x + (long long)b0 * x_stride, x_stride, L,
+    resample_batch_kernel<<<dim3(tiles, rows), kThreads, r->smem, st>>>(g, r->tab, r->meta, x + (long long)b0 * x_stride, x_stride,
+                                                                        row_lens<kRowsPerLaunch>(lens_host, x_stride, b0, rows),
                                                                         y + (long long)b0 * y_stride, y_stride);
     CK(cudaGetLastError());
   }
@@ -324,88 +300,57 @@ int sopro_resample(sopro_resampler_t* r, const float* x, int32_t B, int64_t x_st
 }
 
 int sopro_resampler_stream_create(sopro_resampler_t* r, int64_t max_chunk, sopro_resampler_stream_t** out) {
-  if (!r || !out) return fail(SOPRO_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (max_chunk < 1 || max_chunk > (1LL << 32)) return fail(SOPRO_ERR_INVALID, "max_chunk must be in [1, 2^32]");
+  if (!r) return fail(SOPRO_ERR_INVALID, "null argument");
+  const int rc = chunk::check_create(max_chunk, out);
+  if (rc != SOPRO_OK) return rc;
   CK(cudaSetDevice(r->device));
   sopro_resampler_stream* s = new sopro_resampler_stream();
   s->r = r;
-  s->max_chunk = max_chunk;
-  const size_t cap = (size_t)(2 * r->g.width + r->g.o);  // the carried tail is always shorter (header)
-  cudaError_t e = cudaMalloc(&s->carry[0], cap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&s->carry[1], cap * 4);
-  if (e != cudaSuccess) {
-    cudaFree(s->carry[0]);
-    delete s;
-    return fail(SOPRO_ERR_CUDA, "resampler stream state: %s", cudaGetErrorString(e));
-  }
-  *out = s;
-  return SOPRO_OK;
+  s->restart(-r->g.width);
+  // the carried tail is always shorter than 2 width + o (header)
+  return chunk::create(s, max_chunk, (size_t)(2 * r->g.width + r->g.o), "resampler", out);
 }
 
-int sopro_resampler_stream_destroy(sopro_resampler_stream_t* s) {
-  if (!s) return SOPRO_OK;
-  cudaSetDevice(s->r->device);
-  cudaFree(s->carry[0]);
-  cudaFree(s->carry[1]);
-  delete s;
-  return SOPRO_OK;
-}
+int sopro_resampler_stream_destroy(sopro_resampler_stream_t* s) { return chunk::destroy(s); }
 
 int sopro_resampler_stream_reset(sopro_resampler_stream_t* s) {
   if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
-  s->n_seen = s->q_done = 0;
-  s->cur = 0;
-  s->finished = false;
+  s->restart(-s->r->g.width);
+  s->q_done = 0;
   return SOPRO_OK;
 }
 
 int64_t sopro_resampler_stream_ready(const sopro_resampler_stream_t* s, int64_t n_more, int final) {
-  if (!s || n_more < 0 || s->finished) return -1;
+  if (!chunk::can_run(s, n_more)) return -1;
   const Geo& g = s->r->g;
   const long long done = (long long)g.n * s->q_done;
-  if (final) return out_len(g.o, g.n, s->n_seen + n_more) - done;
-  return (long long)g.n * blocks_ready(g, s->n_seen + n_more) - done;
+  if (final) return out_len(g.o, g.n, s->tail.seen + n_more) - done;
+  return (long long)g.n * blocks_ready(g, s->tail.seen + n_more) - done;
 }
 
 int sopro_resampler_push(sopro_resampler_stream_t* s, const float* x, int64_t n, float* y, void* stream) {
-  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (s->finished) return fail(SOPRO_ERR_STATE, "push after finish: reset the stream first");
-  if (n < 0 || n > s->max_chunk) return fail(SOPRO_ERR_INVALID, "push of %lld samples: must be in [0, max_chunk = %lld]", (long long)n, s->max_chunk);
-  if (n == 0) return SOPRO_OK;
+  int rc = chunk::check_push(s, n);
+  if (rc != SOPRO_OK || n == 0) return rc;
   const Geo& g = s->r->g;
-  const long long n_seen = s->n_seen + n, q_done = blocks_ready(g, n_seen);
-  if (!x || (q_done > s->q_done && !y)) return fail(SOPRO_ERR_INVALID, "null argument");
-  CK(cudaSetDevice(s->r->device));
+  const long long q_done = blocks_ready(g, s->tail.seen + n);
+  if ((rc = chunk::check_io(x, n, y, q_done - s->q_done)) != SOPRO_OK) return rc;
+  CK(cudaSetDevice(s->tail.device));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const long long base = s->q_done * g.o - g.width;  // logical index of carry[cur][0]
-  const Src src{s->carry[s->cur], x, base, s->n_seen, n_seen};
-  int rc = launch_stream(s, src, (long long)g.n * s->q_done, (long long)g.n * q_done, y, st);
+  rc = launch_stream(s, s->tail.src(x, n), (long long)g.n * s->q_done, (long long)g.n * q_done, y, st);
+  if (rc == SOPRO_OK) rc = s->tail.keep(q_done * g.o - g.width, x, n, st);
   if (rc != SOPRO_OK) return rc;
-  // the new tail [q_done * o - width, n_seen) into the other buffer: what is left of the old tail, then of the chunk
-  const long long nbase = q_done * g.o - g.width;
-  float* dst = s->carry[s->cur ^ 1];
-  long long k = nbase;
-  if (k < s->n_seen) {
-    CK(cudaMemcpyAsync(dst, s->carry[s->cur] + (k - base), (size_t)(s->n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
-    k = s->n_seen;
-  }
-  CK(cudaMemcpyAsync(dst + (k - nbase), x + (k - s->n_seen), (size_t)(n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
-  s->cur ^= 1;
-  s->n_seen = n_seen;
   s->q_done = q_done;
   return SOPRO_OK;
 }
 
 int sopro_resampler_finish(sopro_resampler_stream_t* s, float* y, void* stream) {
-  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (s->finished) return fail(SOPRO_ERR_STATE, "finish after finish: reset the stream first");
+  int rc = chunk::check_finish(s);
+  if (rc != SOPRO_OK) return rc;
   const Geo& g = s->r->g;
-  const long long j_end = out_len(g.o, g.n, s->n_seen), j_begin = (long long)g.n * s->q_done;
-  if (j_end > j_begin && !y) return fail(SOPRO_ERR_INVALID, "null argument");
-  CK(cudaSetDevice(s->r->device));
-  const Src src{s->carry[s->cur], nullptr, s->q_done * g.o - g.width, s->n_seen, s->n_seen};
-  const int rc = launch_stream(s, src, j_begin, j_end, y, reinterpret_cast<cudaStream_t>(stream));
+  const long long j_end = out_len(g.o, g.n, s->tail.seen), j_begin = (long long)g.n * s->q_done;
+  if ((rc = chunk::check_io(nullptr, 0, y, j_end - j_begin)) != SOPRO_OK) return rc;
+  CK(cudaSetDevice(s->tail.device));
+  rc = launch_stream(s, s->tail.src(nullptr, 0), j_begin, j_end, y, reinterpret_cast<cudaStream_t>(stream));
   if (rc != SOPRO_OK) return rc;
   s->finished = true;
   return SOPRO_OK;

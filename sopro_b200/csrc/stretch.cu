@@ -23,9 +23,12 @@
 #include <vector>
 
 #include "../../include/sopro_b200.h"
-#include "common.cuh"
+#include "chunk_stream.cuh"
 
 namespace {
+
+using chunk::Src;
+using chunk::src_at;
 
 constexpr int kN = 480, kHs = 240, kHalf = kN / 2, kDelta = 160, kCand = 2 * kDelta + 1;
 constexpr int kMinS = 16384, kMaxS = 262144, kOne = 65536;  // speed 0.25 .. 4.0 in 1/65536 steps
@@ -40,14 +43,6 @@ constexpr long long kMaxLen = 1LL << 40;
 static_assert(kN % kWarps == 0 && kCandPad >= kCand && kHs == kHalf, "geometry");
 static_assert(kCandPad - 1 + kN - 1 + 1 <= kWin, "the search's last register load stays in the window");
 constexpr double kPi = 3.141592653589793;
-
-// where the input sample at logical index i comes from: [0, split) from a (a[i - a_base]), [split, limit) from b
-// (b[i - split]), zero elsewhere -- the one-shot path has a single source, a stream its carried tail and the new chunk
-struct Src {
-  const float* a;
-  const float* b;
-  long long a_base, split, limit;
-};
 
 struct Window {
   float w[kN];
@@ -70,11 +65,6 @@ Window make_window() {
     w.w[n] = (float)(s * s);
   }
   return w;
-}
-
-__device__ __forceinline__ float src_at(const Src& s, long long i) {
-  if (i < 0 || i >= s.limit) return 0.0f;
-  return i < s.split ? s.a[i - s.a_base] : s.b[i - s.split];
 }
 
 // (score, d) beats (s2, d2): the larger score; on a tie the smaller |d|, then the negative d
@@ -267,15 +257,14 @@ static_assert(kCarryCap >= 2 * kLead + 4 * kHs + 2 && kCarryCap >= 2 * kLead + k
 
 }  // namespace
 
-struct sopro_stretch_stream {
-  int device = 0;
-  long long max_chunk = 0;
-  int S = 0;                             // 0 until the first reset
-  float* carry[2] = {nullptr, nullptr};  // ping-pong: logical input [tail_base(k_done), n_seen) of the utterance
+// the tail holds the logical input [tail_base(k_done), n_seen) of the utterance
+struct sopro_stretch_stream : chunk::ChunkStream {
+  int S = 0;
   Carry* state = nullptr;
-  int cur = 0;
-  long long n_seen = 0, k_done = 0;      // input samples pushed, frames computed
-  bool finished = false;
+  long long k_done = 0;  // frames computed
+
+  cudaError_t alloc_own() { return cudaMalloc(&state, sizeof(Carry)); }
+  void free_own() { cudaFree(state); }
 };
 
 namespace {
@@ -327,121 +316,74 @@ int sopro_stretch(const float* x, int32_t B, int64_t x_stride, const int64_t* le
                   int32_t* offsets, void* stream) {
   if (!x || !y) return fail(SOPRO_ERR_INVALID, "null argument");
   if (!valid_S(S)) return fail(SOPRO_ERR_INVALID, "S = %d not in [%d, %d] (speed 0.25 .. 4 in 1/65536 steps)", S, kMinS, kMaxS);
-  if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, (long long)x_stride);
   long long most = 0;
-  for (int b = 0; b < B; ++b) {
-    const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, (long long)x_stride);
-    most = std::max(most, out_len(S, len));
-  }
-  if (B > 1 && y_stride < most) return fail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld outputs", (long long)y_stride, most);
+  int rc = check_rows(x, B, x_stride, lens_host, kMaxLen, &most);
+  if (rc != SOPRO_OK) return rc;
+  most = out_len(S, most);  // out_len is monotone in the row length
+  if ((rc = check_out_rows(y, B, y_stride, most)) != SOPRO_OK) return rc;
   if (most == 0) return SOPRO_OK;
   const long long k_max = n_frames(most);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   static const Window wp = make_window();
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    RowLens<kRowsPerLaunch> L{};
-    for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
-    stretch_batch_kernel<<<rows, kThreads, 0, st>>>(wp, x + (long long)b0 * x_stride, x_stride, L, S, y + (long long)b0 * y_stride,
-                                                    y_stride, offsets ? offsets + (long long)b0 * k_max : nullptr, k_max);
+    stretch_batch_kernel<<<rows, kThreads, 0, st>>>(wp, x + (long long)b0 * x_stride, x_stride,
+                                                    row_lens<kRowsPerLaunch>(lens_host, x_stride, b0, rows), S,
+                                                    y + (long long)b0 * y_stride, y_stride,
+                                                    offsets ? offsets + (long long)b0 * k_max : nullptr, k_max);
     CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }
 
 int sopro_stretch_stream_create(int64_t max_chunk, int device, sopro_stretch_stream_t** out) {
-  if (!out) return fail(SOPRO_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (max_chunk < 1 || max_chunk > (1LL << 32)) return fail(SOPRO_ERR_INVALID, "max_chunk must be in [1, 2^32]");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
-    return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the time-stretch has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  CK(cudaSetDevice(device));
+  int rc = chunk::check_create(max_chunk, out);
+  if (rc == SOPRO_OK) rc = open_device(device, "the time-stretch");
+  if (rc != SOPRO_OK) return rc;
   sopro_stretch_stream* s = new sopro_stretch_stream();
-  s->device = device;
-  s->max_chunk = max_chunk;
-  cudaError_t e = cudaMalloc(&s->carry[0], kCarryCap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&s->carry[1], kCarryCap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&s->state, sizeof(Carry));
-  if (e != cudaSuccess) {
-    cudaFree(s->carry[0]);
-    cudaFree(s->carry[1]);
-    delete s;
-    return fail(SOPRO_ERR_CUDA, "stretch stream state: %s", cudaGetErrorString(e));
-  }
-  *out = s;
-  return SOPRO_OK;
+  s->unset = "speed";
+  return chunk::create(s, max_chunk, kCarryCap, "stretch", out);
 }
 
-int sopro_stretch_stream_destroy(sopro_stretch_stream_t* s) {
-  if (!s) return SOPRO_OK;
-  cudaSetDevice(s->device);
-  cudaFree(s->carry[0]);
-  cudaFree(s->carry[1]);
-  cudaFree(s->state);
-  delete s;
-  return SOPRO_OK;
-}
+int sopro_stretch_stream_destroy(sopro_stretch_stream_t* s) { return chunk::destroy(s); }
 
 int sopro_stretch_stream_reset(sopro_stretch_stream_t* s, int32_t S) {
   if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
   if (!valid_S(S)) return fail(SOPRO_ERR_INVALID, "S = %d not in [%d, %d]", S, kMinS, kMaxS);
   s->S = S;
-  s->n_seen = s->k_done = 0;
-  s->cur = 0;
-  s->finished = false;
+  s->restart(tail_base(0, S));
+  s->k_done = 0;
   return SOPRO_OK;
 }
 
 int64_t sopro_stretch_stream_ready(const sopro_stretch_stream_t* s, int64_t n_more, int final) {
-  if (!s || n_more < 0 || s->finished || s->S == 0) return -1;
-  const long long n = s->n_seen + n_more;
+  if (!chunk::can_run(s, n_more)) return -1;
+  const long long n = s->tail.seen + n_more;
   if (final) return out_len(s->S, n) - emitted(s);
   return std::max(0LL, frames_ready(s->S, s->k_done, n) - 1) * kHs - emitted(s);
 }
 
 int sopro_stretch_push(sopro_stretch_stream_t* s, const float* x, int64_t n, float* y, void* stream) {
-  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (s->S == 0) return fail(SOPRO_ERR_STATE, "push before reset: set the speed first");
-  if (s->finished) return fail(SOPRO_ERR_STATE, "push after finish: reset the stream first");
-  if (n < 0 || n > s->max_chunk) return fail(SOPRO_ERR_INVALID, "push of %lld samples: must be in [0, max_chunk = %lld]", (long long)n, s->max_chunk);
-  if (n == 0) return SOPRO_OK;
-  const long long n_seen = s->n_seen + n, k_done = frames_ready(s->S, s->k_done, n_seen);
-  const long long n_out = std::max(0LL, k_done - 1) * kHs - emitted(s);
-  if (!x || (n_out > 0 && !y)) return fail(SOPRO_ERR_INVALID, "null argument");
-  CK(cudaSetDevice(s->device));
+  int rc = chunk::check_push(s, n);
+  if (rc != SOPRO_OK || n == 0) return rc;
+  const long long k_done = frames_ready(s->S, s->k_done, s->tail.seen + n);
+  if ((rc = chunk::check_io(x, n, y, std::max(0LL, k_done - 1) * kHs - emitted(s))) != SOPRO_OK) return rc;
+  CK(cudaSetDevice(s->tail.device));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const long long base = tail_base(s->k_done, s->S);  // logical index of carry[cur][0]
-  const Src src{s->carry[s->cur], x, base, s->n_seen, n_seen};
-  const int rc = launch_stream(s, src, s->k_done, k_done, y, 1LL << 62, st);
+  rc = launch_stream(s, s->tail.src(x, n), s->k_done, k_done, y, 1LL << 62, st);
+  if (rc == SOPRO_OK) rc = s->tail.keep(tail_base(k_done, s->S), x, n, st);
   if (rc != SOPRO_OK) return rc;
-  // the new tail [tail_base(k_done), n_seen) into the other buffer: what is left of the old tail, then of the chunk
-  const long long nbase = tail_base(k_done, s->S);
-  float* dst = s->carry[s->cur ^ 1];
-  long long k = nbase;
-  if (k < s->n_seen) {
-    CK(cudaMemcpyAsync(dst, s->carry[s->cur] + (k - base), (size_t)(s->n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
-    k = s->n_seen;
-  }
-  CK(cudaMemcpyAsync(dst + (k - nbase), x + (k - s->n_seen), (size_t)(n_seen - k) * 4, cudaMemcpyDeviceToDevice, st));
-  s->cur ^= 1;
-  s->n_seen = n_seen;
   s->k_done = k_done;
   return SOPRO_OK;
 }
 
 int sopro_stretch_finish(sopro_stretch_stream_t* s, float* y, void* stream) {
-  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (s->S == 0) return fail(SOPRO_ERR_STATE, "finish before reset: set the speed first");
-  if (s->finished) return fail(SOPRO_ERR_STATE, "finish after finish: reset the stream first");
-  const long long M = out_len(s->S, s->n_seen), K = n_frames(M);
-  if (M > emitted(s) && !y) return fail(SOPRO_ERR_INVALID, "null argument");
-  CK(cudaSetDevice(s->device));
-  const Src src{s->carry[s->cur], nullptr, tail_base(s->k_done, s->S), s->n_seen, s->n_seen};
-  const int rc = launch_stream(s, src, s->k_done, K, y, M, reinterpret_cast<cudaStream_t>(stream));
+  int rc = chunk::check_finish(s);
+  if (rc != SOPRO_OK) return rc;
+  const long long M = out_len(s->S, s->tail.seen), K = n_frames(M);
+  if ((rc = chunk::check_io(nullptr, 0, y, M - emitted(s))) != SOPRO_OK) return rc;
+  CK(cudaSetDevice(s->tail.device));
+  rc = launch_stream(s, s->tail.src(nullptr, 0), s->k_done, K, y, M, reinterpret_cast<cudaStream_t>(stream));
   if (rc != SOPRO_OK) return rc;
   s->finished = true;
   return SOPRO_OK;

@@ -17,7 +17,7 @@
 #include <vector>
 
 #include "../../include/sopro_b200.h"
-#include "common.cuh"
+#include "chunk_stream.cuh"
 
 namespace {
 
@@ -239,51 +239,38 @@ Layout layout(int B, long long max_len) {
   return l;
 }
 
-int check_batch(const float* x, int B, long long x_stride, const int64_t* lens_host, const float* pattern, void* ws, long long* most) {
-  if (!pattern || !ws) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (B < 1 || x_stride < 0 || x_stride > kMaxLen)
-    return fail(SOPRO_ERR_INVALID, "bad batch geometry (B=%d, x_stride=%lld)", B, x_stride);
-  *most = 0;
-  for (int b = 0; b < B; ++b) {
-    const long long len = lens_host ? lens_host[b] : x_stride;
-    if (len < 0 || len > x_stride) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, x_stride = %lld]", b, len, x_stride);
-    *most = std::max(*most, len);
-  }
-  if (!x && *most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
-  return SOPRO_OK;
-}
-
-RowLens<kRowsPerLaunch> row_lens(const int64_t* lens_host, long long x_stride, int b0, int rows) {
-  RowLens<kRowsPerLaunch> L{};
-  for (int i = 0; i < rows; ++i) L.v[i] = lens_host ? lens_host[b0 + i] : x_stride;
-  return L;
-}
-
 // carried partial block: fewer than kBlk samples
 constexpr long long kCarryCap = kBlk;
 
 }  // namespace
 
-struct sopro_watermark_stream {
-  int device = 0;
-  long long max_chunk = 0;
-  const float* pattern = nullptr;        // the key's table (device); null until the first reset
-  float* carry[2] = {nullptr, nullptr};  // ping-pong: samples [done, n_seen) of the utterance
-  double* r = nullptr;                   // [max_chunk / kBlk + 2]: one push's blocks, after the one before them
-  double* r_last = nullptr;              // the last complete block's r
-  int cur = 0;
-  long long n_seen = 0, done = 0;        // samples pushed; samples emitted
-  bool finished = false;
+// the tail holds the held partial block: samples [done, n_seen) of the utterance
+struct sopro_watermark_stream : chunk::ChunkStream {
+  const float* pattern = nullptr;  // the key's table (device)
+  double* r = nullptr;             // [max_chunk / kBlk + 2]: one push's blocks, after the one before them
+  double* r_last = nullptr;        // the last complete block's r
+
+  cudaError_t alloc_own() {
+    const cudaError_t e = cudaMalloc(&r, (size_t)(max_chunk / kBlk + 2) * sizeof(double));
+    return e == cudaSuccess ? cudaMalloc(&r_last, sizeof(double)) : e;
+  }
+  void free_own() {
+    cudaFree(r);
+    cudaFree(r_last);
+  }
 };
 
 namespace {
-// the span [done, done + count) of s marked -> y, its nb blocks' RMS first (the last one over last_count samples)
-int stream_launch(sopro_watermark_stream* s, const Src& src, int nb, int last_count, long long count, float* y, cudaStream_t st) {
+// the tail followed by x: the span [done, done + count) marked -> y, its nb blocks' RMS first (the last one over
+// last_count samples)
+int stream_launch(sopro_watermark_stream* s, const float* x, int nb, int last_count, long long count, float* y, cudaStream_t st) {
   if (nb == 0) return SOPRO_OK;
-  wm_stream_rms_kernel<<<(nb + kWarps - 1) / kWarps, kT, 0, st>>>(src, nb, last_count, s->r_last, s->done > 0 ? 1 : 0, s->r);
+  const long long done = s->tail.base;
+  const Src src{s->tail.data(), x, s->tail.held()};
+  wm_stream_rms_kernel<<<(nb + kWarps - 1) / kWarps, kT, 0, st>>>(src, nb, last_count, s->r_last, done > 0 ? 1 : 0, s->r);
   CK(cudaGetLastError());
   const long long gx = std::min<long long>((count + kT - 1) / kT, 4096);
-  wm_stream_apply_kernel<<<(unsigned)gx, kT, 0, st>>>(src, count, s->done, nb, s->r, s->pattern, level(), y, s->r_last);
+  wm_stream_apply_kernel<<<(unsigned)gx, kT, 0, st>>>(src, count, done, nb, s->r, s->pattern, level(), y, s->r_last);
   CK(cudaGetLastError());
   return SOPRO_OK;
 }
@@ -331,11 +318,11 @@ int sopro_watermark_sizes(int32_t B, int64_t max_len, int64_t* embed_ws, int64_t
 
 int sopro_watermark_embed(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, const float* pattern, float* y,
                           int64_t y_stride, void* ws, void* stream) {
+  if (!pattern || !ws) return fail(SOPRO_ERR_INVALID, "null argument");
   long long most = 0;
-  const int rc = check_batch(x, B, x_stride, lens_host, pattern, ws, &most);
+  int rc = check_rows(x, B, x_stride, lens_host, kMaxLen, &most);
+  if (rc == SOPRO_OK) rc = check_out_rows(y, B, y_stride, most);
   if (rc != SOPRO_OK) return rc;
-  if (!y && most > 0) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (B > 1 && y_stride < most) return fail(SOPRO_ERR_INVALID, "y_stride %lld < the longest row's %lld samples", (long long)y_stride, most);
   if (most == 0) return SOPRO_OK;
   const Layout l = layout(B, most);
   double* r = reinterpret_cast<double*>(static_cast<char*>(ws) + l.r);
@@ -344,7 +331,7 @@ int sopro_watermark_embed(const float* x, int32_t B, int64_t x_stride, const int
   const long long gx = std::min<long long>((most + kT - 1) / kT, 4096);
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    const RowLens<kRowsPerLaunch> L = row_lens(lens_host, x_stride, b0, rows);
+    const RowLens<kRowsPerLaunch> L = row_lens<kRowsPerLaunch>(lens_host, x_stride, b0, rows);
     double* rb = r + (long long)b0 * l.nblk;
     wm_rms_kernel<<<dim3((unsigned)((l.nblk + kWarps - 1) / kWarps), rows), kT, 0, st>>>(x + (long long)b0 * x_stride, x_stride, L,
                                                                                           rb, l.nblk);
@@ -358,8 +345,9 @@ int sopro_watermark_embed(const float* x, int32_t B, int64_t x_stride, const int
 
 int sopro_watermark_detect(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, const float* pattern, void* ws,
                            float* score, int64_t* offset, uint8_t* detected, void* stream) {
+  if (!pattern || !ws) return fail(SOPRO_ERR_INVALID, "null argument");
   long long most = 0;
-  const int rc = check_batch(x, B, x_stride, lens_host, pattern, ws, &most);
+  const int rc = check_rows(x, B, x_stride, lens_host, kMaxLen, &most);
   if (rc != SOPRO_OK) return rc;
   if (!score || !offset || !detected) return fail(SOPRO_ERR_INVALID, "null argument");
   const Layout l = layout(B, most);
@@ -371,7 +359,7 @@ int sopro_watermark_detect(const float* x, int32_t B, int64_t x_stride, const in
   const double fr = floor_ratio();
   for (int b0 = 0; b0 < B; b0 += kRowsPerLaunch) {
     const int rows = std::min(kRowsPerLaunch, B - b0);
-    const RowLens<kRowsPerLaunch> L = row_lens(lens_host, x_stride, b0, rows);
+    const RowLens<kRowsPerLaunch> L = row_lens<kRowsPerLaunch>(lens_host, x_stride, b0, rows);
     const float* xb = x + (long long)b0 * x_stride;
     double* rb = r + (long long)b0 * l.nblk;
     float* Fb = F + (long long)b0 * kP;
@@ -391,95 +379,49 @@ int sopro_watermark_detect(const float* x, int32_t B, int64_t x_stride, const in
 }
 
 int sopro_watermark_stream_create(int64_t max_chunk, int device, sopro_watermark_stream_t** out) {
-  if (!out) return fail(SOPRO_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (max_chunk < 1 || max_chunk > (1LL << 32)) return fail(SOPRO_ERR_INVALID, "max_chunk must be in [1, 2^32]");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
-    return fail(SOPRO_ERR_UNSUPPORTED, "no CUDA device; the watermark has no CPU fallback");
-  if (device < 0 || device >= ndev) return fail(SOPRO_ERR_INVALID, "device %d out of range", device);
-  CK(cudaSetDevice(device));
+  int rc = chunk::check_create(max_chunk, out);
+  if (rc == SOPRO_OK) rc = open_device(device, "the watermark");
+  if (rc != SOPRO_OK) return rc;
   sopro_watermark_stream* s = new sopro_watermark_stream();
-  s->device = device;
-  s->max_chunk = max_chunk;
-  cudaError_t e = cudaMalloc(&s->carry[0], kCarryCap * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&s->carry[1], kCarryCap * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&s->r, (size_t)(max_chunk / kBlk + 2) * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&s->r_last, sizeof(double));
-  if (e != cudaSuccess) {
-    cudaFree(s->carry[0]);
-    cudaFree(s->carry[1]);
-    cudaFree(s->r);
-    delete s;
-    return fail(SOPRO_ERR_CUDA, "watermark stream state: %s", cudaGetErrorString(e));
-  }
-  *out = s;
-  return SOPRO_OK;
+  s->unset = "key";
+  return chunk::create(s, max_chunk, kCarryCap, "watermark", out);
 }
 
-int sopro_watermark_stream_destroy(sopro_watermark_stream_t* s) {
-  if (!s) return SOPRO_OK;
-  cudaSetDevice(s->device);
-  cudaFree(s->carry[0]);
-  cudaFree(s->carry[1]);
-  cudaFree(s->r);
-  cudaFree(s->r_last);
-  delete s;
-  return SOPRO_OK;
-}
+int sopro_watermark_stream_destroy(sopro_watermark_stream_t* s) { return chunk::destroy(s); }
 
 int sopro_watermark_stream_reset(sopro_watermark_stream_t* s, const float* pattern) {
   if (!s || !pattern) return fail(SOPRO_ERR_INVALID, "null argument");
   s->pattern = pattern;
-  s->n_seen = s->done = 0;
-  s->cur = 0;
-  s->finished = false;
+  s->restart(0);
   return SOPRO_OK;
 }
 
 int64_t sopro_watermark_stream_ready(const sopro_watermark_stream_t* s, int64_t n_more, int final) {
-  if (!s || n_more < 0 || s->finished || !s->pattern) return -1;
-  const long long n = s->n_seen + n_more - s->done;
+  if (!chunk::can_run(s, n_more)) return -1;
+  const long long n = s->tail.held() + n_more;
   return final ? n : n / kBlk * kBlk;
 }
 
 int sopro_watermark_push(sopro_watermark_stream_t* s, const float* x, int64_t n, float* y, void* stream) {
-  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (!s->pattern) return fail(SOPRO_ERR_STATE, "push before reset: set the key first");
-  if (s->finished) return fail(SOPRO_ERR_STATE, "push after finish: reset the stream first");
-  if (n < 0 || n > s->max_chunk) return fail(SOPRO_ERR_INVALID, "push of %lld samples: must be in [0, max_chunk = %lld]", (long long)n, s->max_chunk);
-  if (n == 0) return SOPRO_OK;
-  const long long held = s->n_seen - s->done, total = held + n, count = total / kBlk * kBlk;
-  if (!x || (count > 0 && !y)) return fail(SOPRO_ERR_INVALID, "null argument");
-  CK(cudaSetDevice(s->device));
+  int rc = chunk::check_push(s, n);
+  if (rc != SOPRO_OK || n == 0) return rc;
+  const long long count = (s->tail.held() + n) / kBlk * kBlk;
+  if ((rc = chunk::check_io(x, n, y, count)) != SOPRO_OK) return rc;
+  CK(cudaSetDevice(s->tail.device));
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const Src src{s->carry[s->cur], x, held};
-  const int rc = stream_launch(s, src, (int)(count / kBlk), 0, count, y, st);
-  if (rc != SOPRO_OK) return rc;
-  // the new partial block [count, total) of the span into the other buffer: what is left of the carried one, then the chunk
-  float* dst = s->carry[s->cur ^ 1];
-  long long k = count;
-  if (k < held) {
-    CK(cudaMemcpyAsync(dst, s->carry[s->cur] + k, (size_t)(held - k) * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    k = held;
-  }
-  if (total > k) CK(cudaMemcpyAsync(dst + (k - count), x + (k - held), (size_t)(total - k) * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  s->cur ^= 1;
-  s->n_seen += n;
-  s->done += count;
-  return SOPRO_OK;
+  rc = stream_launch(s, x, (int)(count / kBlk), 0, count, y, st);
+  if (rc == SOPRO_OK) rc = s->tail.keep(s->tail.base + count, x, n, st);  // the new partial block
+  return rc;
 }
 
 int sopro_watermark_finish(sopro_watermark_stream_t* s, float* y, void* stream) {
-  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (!s->pattern) return fail(SOPRO_ERR_STATE, "finish before reset: set the key first");
-  if (s->finished) return fail(SOPRO_ERR_STATE, "finish after finish: reset the stream first");
-  const long long held = s->n_seen - s->done;
-  if (held > 0 && !y) return fail(SOPRO_ERR_INVALID, "null argument");
+  int rc = chunk::check_finish(s);
+  if (rc != SOPRO_OK) return rc;
+  const long long held = s->tail.held();
+  if ((rc = chunk::check_io(nullptr, 0, y, held)) != SOPRO_OK) return rc;
   if (held > 0) {
-    CK(cudaSetDevice(s->device));
-    const Src src{s->carry[s->cur], nullptr, held};
-    const int rc = stream_launch(s, src, 1, (int)held, held, y, reinterpret_cast<cudaStream_t>(stream));
+    CK(cudaSetDevice(s->tail.device));
+    rc = stream_launch(s, nullptr, 1, (int)held, held, y, reinterpret_cast<cudaStream_t>(stream));
     if (rc != SOPRO_OK) return rc;
   }
   s->finished = true;

@@ -355,6 +355,34 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
 /* same with HOST buffers; synchronises the stream */
 int sopro_mimi_encode_host(sopro_mimi_encoder_t* e, const float* wav_host, int64_t n_samples, int32_t* codes_host,
                            float* latent_host, void* stream);
+/* A ragged batch of clips in one pass: row b of wav [B][stride] f32 @24 kHz (device) has lens_host[b] samples (HOST i64,
+ * each in [1, 14 400 000]); samples past lens[b] are not read.  Tmax = sopro_mimi_encoded_frames(longest row) -> codes
+ * [B][n_q][Tmax] i32 (device): row b's first T_b = sopro_mimi_encoded_frames(lens[b]) frames are written, the rest
+ * are left as they were.  `latent` (optional, device [B][Tmax][hidden] f32): rows past T_b hold padding values.
+ * Row b equals sopro_mimi_encode of that clip alone, codes and latent, bit for bit.  The batch is padded to the longest
+ * row rounded up to 2 * prod(ratios) samples; B times that must be at most 14 400 000 (the single call's bound).
+ * B < 1, a length out of range, stride < the longest row, an oversized batch or a null pointer: SOPRO_ERR_INVALID
+ * before any launch.  Uploads the B lengths (HOST -> device copy on `stream`); no synchronisation. */
+int sopro_mimi_encode_batch(sopro_mimi_encoder_t* e, const float* wav, int32_t B, int64_t stride, const int64_t* lens_host,
+                            int32_t* codes, float* latent, void* stream);
+
+/* ---- voice ingestion (MimiCodec.encode_file's host-side preparation, reference codec/mimi.py:44-57, on the device for
+ * a ragged batch of clips, each at its own sample rate; no reference counterpart for the batch).
+ *   Trim: the energy VAD of the reference's trim_silence_energy (audio.py:30-87) at the clip's rate sr:
+ *   flen = max(1, floor(sr * 25 / 1000)), hop = max(1, floor(sr * 10 / 1000)), pad = floor(sr * 30 / 1000); frames
+ *   k < K = floor((n - flen) / hop) + 1; e_k = sum x^2 / flen summed in fp64 (a fixed order per frame), dB_k =
+ *   10 log10(e_k + 1e-10); thr = max(max_k dB_k - 40, -40); frame k is voiced when dB_k > thr; start = max(0, first hop
+ *   - pad), end = min(n, last hop + flen + pad).  The extent is (0, n) when n < floor(sr * 0.1) or n < flen, no frame
+ *   is voiced, or end - start < floor(sr / 2).  The reference sums in fp32, so a frame whose dB lies within rounding of
+ *   the threshold may be classified differently there.
+ *   Pack: row b of dst [B][dst_stride] = the lens_host[b] samples at src[b], zeros up to dst_stride. */
+/* rows: HOST array of B device pointers, row b of lens_host[b] samples (HOST i64) at rates_host[b] Hz (HOST i32, in
+ * [4000, 192000]) -> ext [B][2] (device i64).  One launch per 64 rows; no call synchronises or allocates. */
+int sopro_ingest_trim(const float* const* rows, int32_t B, const int64_t* lens_host, const int32_t* rates_host, int64_t* ext,
+                      void* stream);
+/* src: HOST array of B device pointers (row b's first sample, read in place); lens_host[b] in [0, dst_stride].  One
+ * launch per 128 rows; no call synchronises or allocates. */
+int sopro_ingest_pack(const float* const* src, int32_t B, const int64_t* lens_host, float* dst, int64_t dst_stride, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * NAR refiner: SoproTTSModel.nar_refine (reference model.py:307-347) over NARSinglePass.forward_stage

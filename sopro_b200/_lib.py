@@ -194,6 +194,9 @@ SYMBOLS = {
     "sopro_mimi_encoded_frames": (C.c_int64, [_VP, C.c_int64]),
     "sopro_mimi_encode": (_I, [_VP, _VP, C.c_int64, _VP, _VP, _VP]),
     "sopro_mimi_encode_host": (_I, [_VP, _VP, C.c_int64, _VP, _VP, _VP]),
+    "sopro_mimi_encode_batch": (_I, [_VP, _VP, C.c_int32, C.c_int64, _VP, _VP, _VP, _VP]),
+    "sopro_ingest_trim": (_I, [_VP, C.c_int32, _VP, _VP, _VP, _VP]),
+    "sopro_ingest_pack": (_I, [_VP, C.c_int32, _VP, _VP, C.c_int64, _VP]),
     "sopro_nar_create": (_I, [_VP, _VP, _I, C.POINTER(_VP)]),
     "sopro_nar_destroy": (_I, [_VP]),
     "sopro_nar_set_forced": (_I, [_VP, _VP]),

@@ -7,8 +7,9 @@ read from when none is passed in."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -119,6 +120,47 @@ class MimiEncoderEngine:
                                               int(torch.cuda.current_stream(self.device).cuda_stream)))
         codes = codes.to(torch.long)
         return (codes, lat) if return_latent else codes
+
+    def encode_batch(self, wav_bl: torch.Tensor, lens: Sequence[int], *, return_latent: bool = False):
+        """A ragged batch wav [B, L] f32 @24 kHz (row b's first lens[b] samples) -> codes: a list of [Q, T_b] int64 on
+        the engine's device (and, on request, the latents [T_b, 512]).  Row b equals ``encode`` of its samples alone, bit
+        for bit.  The rows run longest first in padded calls of at most ENC_MAX_SAMPLES samples each."""
+        from .ingest import ENC_MAX_SAMPLES
+
+        wav_bl = wav_bl.to(device=self.device, dtype=torch.float32)
+        B, L = wav_bl.shape
+        lens = [int(n) for n in lens]
+        if len(lens) != B:
+            raise ValueError(f"lens has {len(lens)} entries for {B} rows")
+        if any(n < 1 or n > L for n in lens):
+            raise ValueError(f"every length must be in [1, {L}]")
+        Ts = [self.frames(n) for n in lens]
+        unit = 2 * math.prod(UPSAMPLING_RATIOS)
+        codes: List[Optional[torch.Tensor]] = [None] * B
+        lats: List[Optional[torch.Tensor]] = [None] * B
+        live = sorted(range(B), key=lambda i: -lens[i])
+        st = int(torch.cuda.current_stream(self.device).cuda_stream)
+        while live:
+            pad = -(-lens[live[0]] // unit) * unit
+            k = max(1, min(len(live), ENC_MAX_SAMPLES // pad))
+            idx, live = live[:k], live[k:]
+            if idx == list(range(idx[0], idx[0] + k)):
+                x = wav_bl[idx[0]: idx[0] + k]
+            else:
+                x = wav_bl[torch.tensor(idx, device=self.device)]
+            if x.stride(-1) != 1:
+                x = x.contiguous()
+            Tm = Ts[idx[0]]
+            c = torch.empty((k, self.num_quantizers, Tm), dtype=torch.int32, device=self.device)
+            lat = torch.empty((k, Tm, 512), dtype=torch.float32, device=self.device) if return_latent else None
+            _lib.check_arg(self.lib.sopro_mimi_encode_batch(self._h, x.data_ptr(), k, int(x.stride(0)),
+                                                            (C.c_int64 * k)(*[lens[i] for i in idx]), c.data_ptr(),
+                                                            lat.data_ptr() if lat is not None else None, st))
+            for j, i in enumerate(idx):
+                codes[i] = c[j, :, : Ts[i]].to(torch.long)
+                if lat is not None:
+                    lats[i] = lat[j, : Ts[i]]
+        return (codes, lats) if return_latent else codes
 
     def encode_host(self, wav: np.ndarray) -> np.ndarray:
         wav = np.ascontiguousarray(wav, dtype=np.float32).reshape(-1)
@@ -324,6 +366,7 @@ class MimiCodec:
         self._num_quantizers = int(num_quantizers)
         self.engine = MimiEngine(state_dict, self.device, num_quantizers=self._num_quantizers, precision=precision)
         self._encoder: Optional[MimiEncoderEngine] = None
+        self._in_resamplers: Dict[int, "Resampler"] = {}  # clip rate -> 24 kHz (prepare_wavs)
         enc = ("encoder.", "encoder_transformer.", "downsample.", "quantizer.")
         self._encoder_sd = ({k: v for k, v in state_dict.items() if k.startswith(enc)}
                             if all(k in state_dict for k in ENCODER_KEYS) else None)
@@ -363,6 +406,57 @@ class MimiCodec:
         """mono waveform @24 kHz ([n], [1, n] or [1, 1, n]) -> codes [T, Q] int64 on the device: the model call of
         ``encode_file`` (reference codec/mimi.py:59-62), on the CUDA encoder."""
         return self.encoder.encode(wav).permute(1, 0).contiguous()
+
+    @torch.no_grad()
+    def prepare_wavs(self, wavs: Sequence[torch.Tensor], sample_rates: Sequence[int],
+                     crop_seconds: Optional[float] = None) -> Tuple[torch.Tensor, List[int]]:
+        """``encode_file``'s preparation of a ragged batch on the device: clips [n] or [C, n] (any device, channels
+        averaged), each at its own rate -> (wav [B, L] f32 @24 kHz on the device, valid samples per row; zeros past them).
+        Per clip: energy trim at its rate (one launch for the batch), resample to 24 kHz (one launch per distinct rate;
+        a 24 kHz clip is not resampled), centre crop to `crop_seconds` as encode_file does (None or <= 0: no crop).  The
+        one host read is the B trim extents.  The trim sums in fp64 where the reference's torch ops sum in fp32, so only
+        a frame within rounding of the threshold can be classified differently from ``encode_file``; the resampler is
+        §5d's (DESIGN.md), not torchaudio's fp32 kernel."""
+        from . import ingest
+        from .resample import Resampler
+
+        wavs, sample_rates = list(wavs), list(sample_rates)
+        if not wavs or len(sample_rates) != len(wavs):
+            raise ValueError(f"{len(wavs)} clips with {len(sample_rates)} sample rates")
+        rates = [ingest._check_wav(w, sr, i) for i, (w, sr) in enumerate(zip(wavs, sample_rates))]
+        win = ingest.crop_samples(crop_seconds)
+        rows = ingest.mono_rows(wavs, self.device)
+        ext = ingest.trim_extents(rows, rates).tolist()  # the one host read
+        B = len(rows)
+        src, n24 = [0] * B, [0] * B
+        keep = []  # resampled rows, alive until the last pack has been enqueued
+        by_rate: Dict[int, List[int]] = {}
+        for b, (s, e) in enumerate(ext):
+            if rates[b] == TARGET_SR:
+                src[b], n24[b] = rows[b].data_ptr() + 4 * s, e - s
+            else:
+                by_rate.setdefault(rates[b], []).append(b)
+        for sr, idx in by_rate.items():
+            lens = [ext[b][1] - ext[b][0] for b in idx]
+            x = ingest.pack([rows[b].data_ptr() + 4 * ext[b][0] for b in idx], lens,
+                            torch.empty((len(idx), max(lens)), dtype=torch.float32, device=self.device))
+            rs = self._in_resamplers.get(sr)
+            if rs is None:
+                rs = self._in_resamplers[sr] = Resampler(sr, TARGET_SR, self.device)
+            y = rs(x, lens)
+            keep.append(y)
+            for j, b in enumerate(idx):
+                src[b], n24[b] = y[j].data_ptr(), rs.length(lens[j])
+        plan = [ingest.crop_plan(n, win) for n in n24]
+        out = torch.empty((B, max(n for _, n in plan)), dtype=torch.float32, device=self.device)
+        ingest.pack([src[b] + 4 * plan[b][0] for b in range(B)], [n for _, n in plan], out)
+        return out, [n for _, n in plan]
+
+    @torch.no_grad()
+    def encode_wavs(self, wav_bl: torch.Tensor, lens: Sequence[int]) -> List[torch.Tensor]:
+        """A ragged batch @24 kHz (``prepare_wavs``' result) -> codes [T_b, Q] int64 per row on the device, each equal
+        to ``encode_wav`` of the row's samples alone, bit for bit (batched Mimi encoder, sopro_mimi_encode_batch)."""
+        return [c.permute(1, 0).contiguous() for c in self.encoder.encode_batch(wav_bl, lens)]
 
     @torch.no_grad()
     def decode_full(self, codes_tq: torch.Tensor) -> torch.Tensor:

@@ -1473,43 +1473,75 @@ int sopro_mimi_decode_host(sopro_mimi_t* m, const int32_t* codes_host, int B, in
 // tap at superrow -1).
 // =====================================================================================================================
 namespace mimi {
-// first conv: wav [L] -> y [L][F], kernel k, causal (left zero pad k-1), weight [F][k]
+// A batch of clips (sopro_mimi_encode_batch) is right-padded to one length and every kernel runs over all its rows.
+// Everything in the encoder is causal, so a clip's valid prefix never reads its padding, except where a kernel below
+// takes the clip's own lengths: `info` [B][NS] int, row b = (rows entering stage s for s = 0..n_ratios, the last being
+// the transformer positions T2, then the frames T) of clip b.  A single clip passes info = null and B = 1.
+constexpr int enc_info_cols(int n_ratios) { return n_ratios + 2; }
+
+// first conv: wav [L] -> y [L][F], kernel k, causal (left zero pad k-1), weight [F][k].  Batch (grid.y = B): clip b's
+// samples are wav + b * wav_stride, info[b][0] of them (zero past that), its rows y + b * L * F.
 __global__ void enc_conv0_kernel(const float* __restrict__ wav, const float* __restrict__ w, const float* __restrict__ bias,
-                                 float* __restrict__ y, long long L, int F, int k) {
+                                 float* __restrict__ y, long long L, int F, int k, long long wav_stride, const int* __restrict__ info,
+                                 int NS) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L * F) return;
+  const int b = blockIdx.y;
+  const long long n = info ? info[b * NS] : L;
+  wav += (long long)b * wav_stride;
   const long long t = i / F;
   const int c = (int)(i - t * F);
   float acc = __ldg(bias + c);
   for (int j = 0; j < k; ++j) {
     const long long ti = t + j - (k - 1);
-    if (ti >= 0) acc = fmaf(__ldg(w + c * k + j), __ldg(wav + ti), acc);
+    if (ti >= 0 && ti < n) acc = fmaf(__ldg(w + c * k + j), __ldg(wav + ti), acc);
   }
-  y[i] = acc;
+  y[(long long)b * L * F + i] = acc;
 }
 
-// replicate padding for the 25 -> 12.5 Hz conv: y rows [0, left) = x[0], [left, left+T) = x, [left+T, rows) = x[T-1]
-__global__ void replicate_pad_kernel(const float* __restrict__ x, float* __restrict__ y, int T, int C, int left, int rows) {
+// MimiConv1d's extra padding of clip b (grid.y) before the stride-r conv of stage s: rows [L, roundup(L, r)) of its
+// [stride rows][ch] block are zeroed, L = info[b][s]
+__global__ void enc_zero_tail_kernel(float* __restrict__ x, long long stride, int ch, int r, const int* __restrict__ info, int NS, int s) {
+  const int b = blockIdx.y;
+  const long long L = info[b * NS + s], Lp = (L + r - 1) / r * r;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long row = L + i / ch;
+  if (row < Lp) x[(long long)b * stride * ch + row * ch + (i % ch)] = 0.f;
+}
+
+// replicate padding for the 25 -> 12.5 Hz conv: y rows [0, left) = x[0], [left, left+T) = x, [left+T, rows) = x[T-1].
+// Batch (grid.y = B): clip b's x rows are x + b * T * C (T = the padded positions), its y rows y + b * rows * C, and its
+// own last position info[b][NS - 2] - 1 is the one replicated.
+__global__ void replicate_pad_kernel(const float* __restrict__ x, float* __restrict__ y, int T, int C, int left, int rows,
+                                     const int* __restrict__ info, int NS) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)rows * C) return;
+  const int b = blockIdx.y;
+  const int Tb = info ? info[b * NS + NS - 2] : T;
   const int r = (int)(i / C), c = (int)(i - (long long)r * C);
   int src = r - left;
-  src = src < 0 ? 0 : (src >= T ? T - 1 : src);
-  y[i] = x[(size_t)src * C + c];
+  src = src < 0 ? 0 : (src >= Tb ? Tb - 1 : src);
+  y[(size_t)b * rows * C + i] = x[(size_t)b * T * C + (size_t)src * C + c];
 }
 
 // Residual nearest-neighbour search (MimiResidualVectorQuantizer.encode :1262-1280 with MimiEuclideanCodebook.quantize
 // :1197-1203): one CTA per frame, the residual (Dc = 32*DPL floats) in registers, lane-sliced; a warp scans every 8th
 // code vector, squared distance summed directly (the reference's cdist goes through |x|^2+|e|^2-2xe, same minimiser),
 // lowest index wins ties (torch.argmin).  proj [T][2*Dc] = [semantic input_proj | acoustic input_proj] of the latent.
+// Batch (grid.y = B): clip b's proj rows are proj + b * T * 2Dc and its codes codes + b * n_q * T; frames at or past
+// its own info[b][NS - 1] are skipped.
 template <int DPL>
 __global__ void __launch_bounds__(256) rvq_encode_kernel(const float* __restrict__ proj, const float* __restrict__ embed,
-                                                         int* __restrict__ codes, int T, int n_q, int n_sem, int V) {
+                                                         int* __restrict__ codes, int T, int n_q, int n_sem, int V,
+                                                         const int* __restrict__ info, int NS) {
   constexpr int Dc = 32 * DPL;
   __shared__ float best_d[8];
   __shared__ int best_i[8];
   __shared__ int winner;
-  const int t = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.y;
+  if (info && t >= info[b * NS + NS - 1]) return;  // uniform across the CTA
+  proj += (size_t)b * T * 2 * Dc;
+  codes += (size_t)b * n_q * T;
   float r[DPL];
   for (int q = 0; q < n_q; ++q) {
     if (q == 0 || q == n_sem) {
@@ -1586,6 +1618,8 @@ struct sopro_mimi_encoder {
   int* codes_dev = nullptr;
   float* lat_dev = nullptr;
   size_t wav_cap = 0, codes_cap = 0, lat_cap = 0;
+  int* info_dev = nullptr;    // the per-clip lengths of a batch (see enc_info_cols)
+  size_t info_cap = 0;
 };
 
 namespace {
@@ -1619,6 +1653,93 @@ EncPlan enc_plan(const sopro_mimi_config_t& c, long long n) {
   p.xsz = ((size_t)T2 * c.hidden + 63) / 64 * 64;
   p.need = (3 * p.buf + 2 * p.xsz) * 4;
   return p;
+}
+
+// The encode sequence over B clips laid out by plan P (a clip alone: P of its length, B = 1, info = null; a batch: P
+// of the padded length, whose every stage length is then a multiple of its stride, and info the clips' own lengths).
+// Only enqueues kernels, after the RoPE table and the workspace have been sized.
+int encode_run(sopro_mimi_encoder* e, const EncPlan& P, int B, const float* wav, long long wav_stride, const int* info,
+               int32_t* codes, float* latent, cudaStream_t st) {
+  const sopro_mimi_config_t& c = e->cfg;
+  const int C = c.hidden, Dc = c.codebook_dim, NS = enc_info_cols(c.n_ratios);
+  const int T2 = (int)P.len[c.n_ratios], T = (int)P.T;
+  int rc;
+  float* b0 = e->ws;
+  float* b1 = b0 + B * P.buf;
+  float* b2 = b1 + B * P.buf;
+  float* x = b2 + B * P.buf;
+  float* ln = x + B * P.xsz;
+  const float* Wd = e->dev;
+  // ---- SEANet encoder
+  float* cur = b0;   // stage input [len][ch]
+  float* hid = b1;   // resblock hidden [len][ch/2]
+  float* nxt = b2;
+  {
+    const long long tot = P.len[0] * c.num_filters;
+    enc_conv0_kernel<<<dim3((unsigned)((tot + 255) / 256), B), 256, 0, st>>>(wav, Wd + e->c0w, Wd + e->c0b, cur, P.len[0],
+                                                                           c.num_filters, c.kernel, wav_stride, info, NS);
+    CK(cudaGetLastError());
+  }
+  int ch = c.num_filters;
+  for (int s = 0; s < c.n_ratios; ++s) {
+    const sopro_mimi_encoder::Stage& S = e->stages[s];
+    const long long Ls = P.len[s], Lp = P.padded[s];
+    const int r = S.ratio;
+    // ResnetBlock (:412-451): x + conv1(ELU(conv3(ELU(x))))
+    if ((rc = gemm_f32({cur, Ls, 0, B}, ch, c.res_kernel, Wd + S.r1w, Wd + S.r1b, ch / 2, ch / 2, EPI_NONE, nullptr, nullptr, hid, 1, st)))
+      return rc;
+    if ((rc = gemm_f32({hid, Ls, 0, B}, ch / 2, 1, Wd + S.r2w, Wd + S.r2b, ch, ch, EPI_RES, cur, nullptr, cur, 1, st))) return rc;
+    // ELU + conv kernel 2r stride r: zero rows up to a multiple of r, then 2 taps over [Lp/r][r*ch]
+    if (info && r > 1) {
+      enc_zero_tail_kernel<<<dim3((unsigned)(((r - 1) * ch + 255) / 256), B), 256, 0, st>>>(cur, Lp, ch, r, info, NS, s);
+      CK(cudaGetLastError());
+    } else if (!info && Lp > Ls) {
+      CK(cudaMemsetAsync(cur + (size_t)Ls * ch, 0, (size_t)(Lp - Ls) * ch * 4, st));
+    }
+    if ((rc = gemm_f32({cur, Lp / r, 0, B}, r * ch, 2, Wd + S.dw, Wd + S.db, 2 * ch, 2 * ch, EPI_NONE, nullptr, nullptr, nxt, 1, st)))
+      return rc;
+    std::swap(cur, nxt);
+    ch *= 2;
+  }
+  // ELU + conv k3 -> residual stream x [T2][C]
+  if ((rc = gemm_f32({cur, T2, 0, B}, ch, c.last_kernel, Wd + e->lw, Wd + e->lb, C, C, EPI_NONE, nullptr, nullptr, x, 1, st))) return rc;
+  // ---- encoder transformer (MimiTransformerLayer.forward :966-993), fp32 path of the decoder
+  LayerBufs lb{};
+  lb.ln = ln;
+  lb.qkv = b0;
+  lb.att = b1;
+  lb.hid = b0;
+  if ((rc = run_layers(c, e->layers, false, Wd, nullptr, e->rope, e->rope_T2, x, B, T2, lb, nullptr, st))) return rc;
+  // ---- 25 -> 12.5 Hz: kernel 4, stride 2, no bias, replicate padding (2 rows left, 0 or 1 right)
+  {
+    const int rows = 2 * T + 2;
+    const long long tot = (long long)rows * C;
+    replicate_pad_kernel<<<dim3((unsigned)((tot + 255) / 256), B), 256, 0, st>>>(x, b0, T2, C, 2, rows, info, NS);
+    CK(cudaGetLastError());
+    float* lat = latent ? latent : b1;
+    // 2 taps over the T + 1 row pairs [rows/2][2C]: the first pair (the left padding) is the context of output row 0
+    if ((rc = gemm_f32({b0, T, 1, B}, 2 * C, 2, Wd + e->down_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, lat, 0, st))) return rc;
+    // ---- quantizer: both input projections in one GEMM, then the residual search
+    if ((rc = gemm_f32({lat, T, 0, B}, C, 1, Wd + e->inproj, nullptr, 2 * Dc, 2 * Dc, EPI_NONE, nullptr, nullptr, b2, 0, st))) return rc;
+    rvq_encode_kernel<8><<<dim3(T, B), 256, 0, st>>>(b2, Wd + e->embed, codes, T, c.n_q, c.n_sem, c.vocab, info, NS);
+    CK(cudaGetLastError());
+  }
+  return SOPRO_OK;
+}
+
+// the RoPE table for T2 positions and a workspace of `need` bytes
+int encode_prepare(sopro_mimi_encoder* e, int T2, size_t need, cudaStream_t st) {
+  int rc;
+  if (e->rope_T2 < T2 && (rc = make_rope(e->cfg, std::max(T2, 256), &e->rope, &e->rope_T2, st))) return rc;
+  if (e->ws_bytes < need) {
+    cudaFree(e->ws);
+    e->ws = nullptr;
+    e->ws_bytes = 0;
+    cudaError_t ae = cudaMalloc(&e->ws, need);
+    if (ae != cudaSuccess) return fail(SOPRO_ERR_CUDA, "Mimi encoder workspace %zu MB: %s", need >> 20, cudaGetErrorString(ae));
+    e->ws_bytes = need;
+  }
+  return SOPRO_OK;
 }
 }  // namespace
 
@@ -1696,6 +1817,7 @@ int sopro_mimi_encoder_destroy(sopro_mimi_encoder_t* e) {
   cudaFree(e->wav_dev);
   cudaFree(e->codes_dev);
   cudaFree(e->lat_dev);
+  cudaFree(e->info_dev);
   delete e;
   return SOPRO_OK;
 }
@@ -1711,75 +1833,52 @@ int sopro_mimi_encode(sopro_mimi_encoder_t* e, const float* wav, int64_t n_sampl
     return fail(SOPRO_ERR_INVALID, "n_samples=%lld outside [1, %lld]", (long long)n_samples, kEncMaxSamples);
   CK(cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
+  const EncPlan P = enc_plan(e->cfg, n_samples);
+  const int rc = encode_prepare(e, (int)P.len[e->cfg.n_ratios], P.need, st);
+  if (rc) return rc;
+  return encode_run(e, P, 1, wav, n_samples, nullptr, codes, latent, st);
+}
+
+int sopro_mimi_encode_batch(sopro_mimi_encoder_t* e, const float* wav, int32_t B, int64_t stride, const int64_t* lens_host,
+                            int32_t* codes, float* latent, void* stream) {
+  if (!e || !wav || !lens_host || !codes) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1) return fail(SOPRO_ERR_INVALID, "B = %d < 1", B);
+  long long most = 0;
+  for (int b = 0; b < B; ++b) {
+    if (lens_host[b] < 1 || lens_host[b] > kEncMaxSamples)
+      return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld outside [1, %lld]", b, (long long)lens_host[b], kEncMaxSamples);
+    most = std::max(most, (long long)lens_host[b]);
+  }
+  if (stride < most) return fail(SOPRO_ERR_INVALID, "stride %lld < the longest row's %lld samples", (long long)stride, most);
   const sopro_mimi_config_t& c = e->cfg;
-  const int C = c.hidden, Dc = c.codebook_dim;
-  const EncPlan P = enc_plan(c, n_samples);
-  const int T2 = (int)P.len[c.n_ratios], T = (int)P.T;
-  int rc;
-  if (e->rope_T2 < T2 && (rc = make_rope(c, std::max(T2, 256), &e->rope, &e->rope_T2, st))) return rc;
-  if (e->ws_bytes < P.need) {
-    cudaFree(e->ws);
-    e->ws = nullptr;
-    e->ws_bytes = 0;
-    cudaError_t ae = cudaMalloc(&e->ws, P.need);
-    if (ae != cudaSuccess) return fail(SOPRO_ERR_CUDA, "Mimi encoder workspace %zu MB: %s", P.need >> 20, cudaGetErrorString(ae));
-    e->ws_bytes = P.need;
+  const int NS = mimi::enc_info_cols(c.n_ratios);
+  // pad to a multiple of every stride (2 * prod(ratios)): then no stage of the padded plan pads, and every clip's rows sit
+  // at one pitch per stage
+  long long unit = 2;
+  for (int s = 0; s < c.n_ratios; ++s) unit *= c.ratios[s];
+  const long long Lpad = (most + unit - 1) / unit * unit;
+  if (Lpad * B > kEncMaxSamples)
+    return fail(SOPRO_ERR_INVALID, "B = %d rows padded to %lld samples exceed %lld samples", B, Lpad, kEncMaxSamples);
+  const EncPlan P = enc_plan(c, Lpad);
+  std::vector<int> info((size_t)B * NS);
+  for (int b = 0; b < B; ++b) {
+    const EncPlan p = enc_plan(c, lens_host[b]);
+    for (int s = 0; s <= c.n_ratios; ++s) info[(size_t)b * NS + s] = (int)p.len[s];
+    info[(size_t)b * NS + NS - 1] = (int)p.T;
   }
-  float* b0 = e->ws;
-  float* b1 = b0 + P.buf;
-  float* b2 = b1 + P.buf;
-  float* x = b2 + P.buf;
-  float* ln = x + P.xsz;
-  const float* Wd = e->dev;
-  // ---- SEANet encoder
-  float* cur = b0;   // stage input [len][ch]
-  float* hid = b1;   // resblock hidden [len][ch/2]
-  float* nxt = b2;
-  {
-    const long long tot = n_samples * c.num_filters;
-    enc_conv0_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(wav, Wd + e->c0w, Wd + e->c0b, cur, n_samples, c.num_filters, c.kernel);
-    CK(cudaGetLastError());
+  CK(cudaSetDevice(e->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (e->info_cap < info.size()) {
+    cudaFree(e->info_dev);
+    e->info_dev = nullptr;
+    e->info_cap = 0;
+    CK(cudaMalloc(&e->info_dev, info.size() * sizeof(int)));
+    e->info_cap = info.size();
   }
-  int ch = c.num_filters;
-  for (int s = 0; s < c.n_ratios; ++s) {
-    const sopro_mimi_encoder::Stage& S = e->stages[s];
-    const long long Ls = P.len[s], Lp = P.padded[s];
-    const int r = S.ratio;
-    // ResnetBlock (:412-451): x + conv1(ELU(conv3(ELU(x))))
-    if ((rc = gemm_f32({cur, Ls, 0, 1}, ch, c.res_kernel, Wd + S.r1w, Wd + S.r1b, ch / 2, ch / 2, EPI_NONE, nullptr, nullptr, hid, 1, st)))
-      return rc;
-    if ((rc = gemm_f32({hid, Ls, 0, 1}, ch / 2, 1, Wd + S.r2w, Wd + S.r2b, ch, ch, EPI_RES, cur, nullptr, cur, 1, st))) return rc;
-    // ELU + conv kernel 2r stride r: zero rows up to a multiple of r, then 2 taps over [Lp/r][r*ch]
-    if (Lp > Ls) CK(cudaMemsetAsync(cur + (size_t)Ls * ch, 0, (size_t)(Lp - Ls) * ch * 4, st));
-    if ((rc = gemm_f32({cur, Lp / r, 0, 1}, r * ch, 2, Wd + S.dw, Wd + S.db, 2 * ch, 2 * ch, EPI_NONE, nullptr, nullptr, nxt, 1, st)))
-      return rc;
-    std::swap(cur, nxt);
-    ch *= 2;
-  }
-  // ELU + conv k3 -> residual stream x [T2][C]
-  if ((rc = gemm_f32({cur, T2, 0, 1}, ch, c.last_kernel, Wd + e->lw, Wd + e->lb, C, C, EPI_NONE, nullptr, nullptr, x, 1, st))) return rc;
-  // ---- encoder transformer (MimiTransformerLayer.forward :966-993), fp32 path of the decoder
-  LayerBufs lb{};
-  lb.ln = ln;
-  lb.qkv = b0;
-  lb.att = b1;
-  lb.hid = b0;
-  if ((rc = run_layers(c, e->layers, false, Wd, nullptr, e->rope, e->rope_T2, x, 1, T2, lb, nullptr, st))) return rc;
-  // ---- 25 -> 12.5 Hz: kernel 4, stride 2, no bias, replicate padding (2 rows left, 0 or 1 right)
-  {
-    const int rows = 2 * T + 2;
-    const long long tot = (long long)rows * C;
-    replicate_pad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(x, b0, T2, C, 2, rows);
-    CK(cudaGetLastError());
-    float* lat = latent ? latent : b1;
-    // 2 taps over the T + 1 row pairs [rows/2][2C]: the first pair (the left padding) is the context of output row 0
-    if ((rc = gemm_f32({b0, T, 1, 1}, 2 * C, 2, Wd + e->down_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, lat, 0, st))) return rc;
-    // ---- quantizer: both input projections in one GEMM, then the residual search
-    if ((rc = gemm_f32({lat, T, 0, 1}, C, 1, Wd + e->inproj, nullptr, 2 * Dc, 2 * Dc, EPI_NONE, nullptr, nullptr, b2, 0, st))) return rc;
-    rvq_encode_kernel<8><<<T, 256, 0, st>>>(b2, Wd + e->embed, codes, T, c.n_q, c.n_sem, c.vocab);
-    CK(cudaGetLastError());
-  }
-  return SOPRO_OK;
+  CK(cudaMemcpyAsync(e->info_dev, info.data(), info.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const int rc = encode_prepare(e, (int)P.len[c.n_ratios], (size_t)B * P.need, st);
+  if (rc) return rc;
+  return encode_run(e, P, B, wav, stride, e->info_dev, codes, latent, st);
 }
 
 int sopro_mimi_encode_host(sopro_mimi_encoder_t* e, const float* wav_host, int64_t n_samples, int32_t* codes_host,

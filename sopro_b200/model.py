@@ -19,6 +19,7 @@ from typing import Dict, Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
+from . import ingest
 from . import longform as LF
 from . import prefill as P
 from . import rerank
@@ -411,6 +412,27 @@ class SoproTTS:
                           ref_seconds: Optional[float] = None) -> PreparedReference:
         tokens_tq = self.encode_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
         return self.model.prepare_reference(tokens_tq, device=self.device)
+
+    @torch.inference_mode()
+    def prepare_references(self, clips: Sequence[ingest.Clip], *, sample_rates=None,
+                           ref_seconds: Optional[float] = None) -> List[PreparedReference]:
+        """(extension) Many reference voices in one batched pass, from files or in-memory audio -> one PreparedReference
+        per clip, in order.  `clips`: paths (read with audio.load_audio_file) and / or float tensors [n] or [C, n] on
+        any device (channels averaged).  `sample_rates`: one rate per clip (None for a path, which has its own), or one
+        int for every tensor clip.  `ref_seconds`: as in prepare_reference (None = 12 s, <= 0 = no crop).  One voice from
+        memory: ``prepare_references([wav], sample_rates=[sr])[0]``.
+        encode_file's steps run on the GPU for the whole batch (energy trim at each clip's rate, resample to 24 kHz,
+        centre crop, a batched Mimi encode whose every row equals encode_wav of that row alone), then prepare_reference
+        per voice.  Against prepare_reference(ref_audio_path=...) the trim decisions can differ only at a frame within
+        rounding of the threshold, and the resampler is this library's (DESIGN.md §5d, §5l).  Every argument is checked,
+        and the files read, before any device work."""
+        ingest.crop_samples(ref_seconds)
+        wavs, rates = ingest.load_clips(clips, sample_rates)
+        if ref_seconds is None:
+            ref_seconds = ingest.DEFAULT_REF_SECONDS
+        wav_bl, lens = self.codec.prepare_wavs(wavs, rates, ref_seconds)
+        codes = self.codec.encode_wavs(wav_bl, lens)
+        return [self.model.prepare_reference(c, device=self.device) for c in codes]
 
     # ---- synthesis (model.py:531-580)
     @torch.inference_mode()

@@ -536,6 +536,17 @@ int sopro_prefill_destroy(sopro_prefill_t* p);
 int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, const float* sv,
                       int sv_shared, const float* const* ref_k, const float* const* ref_v, int Tr, float style_strength,
                       int n_frames, float* txt_seq, float* txt_pool, float* cond_ar, void* stream);
+/* The same prefill with a voice per text: B texts over a table of n_voices (1 <= n_voices <= B) prepared references.
+ * voice_of: HOST int32 [B], text b speaks voice voice_of[b] in [0, n_voices); sv: DEVICE f32 [n_voices, sv_dim], voice v's
+ * speaker vector; tr: HOST int32 [n_voices], voice v's reference frames, each in [1, 4096]; ref_k / ref_v: HOST arrays of
+ * ref_layers * n_voices device pointers, entry i * n_voices + v = voice v's cached K / V of reference layer i [H, tr[v], D/H].
+ * The other arguments and the outputs are sopro_prefill_run's.  Text b's rows equal, bit for bit, the rows of a
+ * sopro_prefill_run of the same texts with voice voice_of[b] alone (sv_shared = 1).  The table is copied to the device
+ * on `stream` with no host synchronisation; the host arrays may be released when the call returns. */
+int sopro_prefill_run_voices(sopro_prefill_t* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, int n_voices,
+                             const int32_t* voice_of, const float* sv, const int32_t* tr, const float* const* ref_k,
+                             const float* const* ref_v, float style_strength, int n_frames, float* txt_seq, float* txt_pool,
+                             float* cond_ar, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Reference preparation: SoproTTSModel.prepare_reference (reference model.py:152-170), once per voice, from the
@@ -593,6 +604,11 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
  * frames alone.  Codes outside [0, codebook_size) are reported by sopro_refprep_check. */
 int sopro_refprep_speaker_vectors(sopro_refprep_t* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host,
                                   float* sv, const float* ref_sv, float* cos, void* stream);
+/* sopro_refprep_speaker_vectors scored against a reference vector per row (best-of-N over texts in different voices):
+ * ref_sv: device f32 [B][sv_dim], cos[b] = sv[b] . ref_sv[b]; both required.  Each row's sv and cos equal, bit for bit,
+ * those of sopro_refprep_speaker_vectors with ref_sv[b] as its one vector. */
+int sopro_refprep_speaker_vectors_per_row(sopro_refprep_t* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host,
+                                          float* sv, const float* ref_sv, float* cos, void* stream);
 /* synchronises `stream`; SOPRO_ERR_INVALID if a run since the last check met a code outside [0, codebook_size) (the
  * reference's embedding lookup raises IndexError); clears the flag */
 int sopro_refprep_check(sopro_refprep_t* p, void* stream);

@@ -870,10 +870,10 @@ __global__ void __launch_bounds__(128) mean_pool_kernel(const float* __restrict_
 }
 
 // one warp per (b, t) row: base = pool[b] + frame_pos[t]; LayerNorm (eps 1e-5, biased variance) * w + bias;
-// y = ln * (1 + s*tanh(gamma[b])) + s*tanh(beta[b])         (film rows [Bf][2D], Bf = B or 1)
+// y = ln * (1 + s*tanh(gamma[v])) + s*tanh(beta[v]), v = voice_of[b]      (film rows [n_voices][2D])
 __global__ void __launch_bounds__(256) film_rows_kernel(const float* __restrict__ pool, const float* __restrict__ fpos,
                                                         const float* __restrict__ ln_w, const float* __restrict__ ln_b,
-                                                        const float* __restrict__ film, int film_shared, float strength,
+                                                        const float* __restrict__ film, const int* __restrict__ voice_of, float strength,
                                                         float* __restrict__ y, long long rows, int T, int D) {
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -899,7 +899,7 @@ __global__ void __launch_bounds__(256) film_rows_kernel(const float* __restrict_
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) var += __shfl_xor_sync(0xffffffffu, var, o);
   const float inv = 1.0f / sqrtf(var / (float)D + 1e-5f);
-  const float* f = film + (film_shared ? 0 : b * 2 * D);
+  const float* f = film + (size_t)voice_of[b] * 2 * D;
   n = 0;
   for (int k = lane; k < D; k += 32, ++n) {
     const float ln = (v[n] - mean) * inv * __ldg(ln_w + k) + __ldg(ln_b + k);
@@ -910,15 +910,21 @@ __global__ void __launch_bounds__(256) film_rows_kernel(const float* __restrict_
 // Cached reference cross-attention core + RMS matching, one warp per query row (nn/ref.py:84-101):
 //   per head: s_j = q.K_j / sqrt(dh); p = softmax(s); a = sum_j p_j V_j; nan_to_num
 //   a *= clamp(rms(x) / rms(a), 0, 10) over the full row (both heads)
-// K, V: [H][Tr][dh] (one shared reference voice).  Shared memory per warp: q [D] | p [Tr] | a [D].
+// Row `row` belongs to utterance b = row / T, which speaks voice v = voice_of[b]: K = Kv[v], V = Vv[v], both [H][Tr][dh]
+// with Tr = tr_of[v].  A row's arithmetic depends on its voice alone (the loops run to that voice's Tr), so it equals
+// the row of a launch with that one voice.  Shared memory per warp: q [D] | p [Tr_max] | a [D].
 __global__ void __launch_bounds__(256) ref_attn_kernel(const float* __restrict__ q, const float* __restrict__ x,
-                                                       const float* __restrict__ Kc, const float* __restrict__ Vc,
-                                                       float* __restrict__ out, long long rows, int D, int H, int Tr) {
+                                                       const int* __restrict__ voice_of, const int* __restrict__ tr_of,
+                                                       const float* const* __restrict__ Kv, const float* const* __restrict__ Vv,
+                                                       float* __restrict__ out, long long rows, int T, int D, int H, int Tr_max) {
   extern __shared__ float rsm[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * 8 + warp;
   if (row >= rows) return;
-  const int dh = D / H, Trp = (Tr + 3) & ~3;  // padded: the per-warp regions stay 16-byte aligned
+  const int v = voice_of[row / T], Tr = tr_of[v];
+  const float* __restrict__ Kc = Kv[v];
+  const float* __restrict__ Vc = Vv[v];
+  const int dh = D / H, Trp = (Tr_max + 3) & ~3;  // padded: the per-warp regions stay 16-byte aligned
   float* qs = rsm + (size_t)warp * (2 * D + Trp);
   float* ps = qs + D;
   float* as = ps + Trp;
@@ -1057,21 +1063,42 @@ int sopro_prefill_destroy(sopro_prefill_t* p) {
   return SOPRO_OK;
 }
 
-int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, const float* sv,
-                      int sv_shared, const float* const* ref_k, const float* const* ref_v, int Tr, float style_strength, int n_frames,
-                      float* txt_seq, float* txt_pool, float* cond_ar, void* stream) {
-  if (!p || !text_ids || !text_len || !sv || !txt_seq || !txt_pool || !cond_ar) return fail(SOPRO_ERR_INVALID, "null argument");
+}  // extern "C"
+
+namespace pstage {
+
+// The prefill of B texts over a table of n_voices voices: text b speaks voice voice_of[b] (host), voice v has speaker
+// vector sv[v] (device [n_voices][SV]), tr[v] reference frames (host) and, for reference layer i, cached K / V at
+// ref_k[i * n_voices + v] / ref_v[...] (host arrays of device pointers).  The one-voice call is n_voices = 1.
+int prefill_core(sopro_prefill* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, int n_voices,
+                 const int32_t* voice_of, const float* sv, const int32_t* tr, const float* const* ref_k, const float* const* ref_v,
+                 float style_strength, int n_frames, float* txt_seq, float* txt_pool, float* cond_ar, cudaStream_t st) {
+  if (!p || !text_ids || !text_len || !sv || !txt_seq || !txt_pool || !cond_ar || !voice_of) return fail(SOPRO_ERR_INVALID, "null argument");
   const sopro_prefill_config_t& c = p->cfg;
-  const int D = c.d_model, SV = c.sv_dim, H = c.ref_heads;
+  const int D = c.d_model, SV = c.sv_dim, H = c.ref_heads, RL = c.ref_layers;
   if (B < 1 || Lmax < 1 || Lmax > c.max_text_len || n_frames < 1 || n_frames > c.max_frames_pos || (long long)B * n_frames > 0x3fffffffLL)
     return fail(SOPRO_ERR_INVALID, "bad B=%d Lmax=%d (max %d) n_frames=%d (max %d)", B, Lmax, c.max_text_len, n_frames, c.max_frames_pos);
-  if (c.ref_layers > 0 && (!ref_k || !ref_v || Tr < 1 || Tr > 4096)) return fail(SOPRO_ERR_INVALID, "reference K/V missing or Tr=%d out of range", Tr);
+  if (n_voices < 1 || n_voices > B) return fail(SOPRO_ERR_INVALID, "n_voices=%d outside [1, B=%d]", n_voices, B);
+  for (int b = 0; b < B; ++b)
+    if (voice_of[b] < 0 || voice_of[b] >= n_voices) return fail(SOPRO_ERR_INVALID, "voice_of[%d]=%d outside [0, %d)", b, voice_of[b], n_voices);
+  int Tr_max = 1;
+  if (RL > 0) {
+    if (!ref_k || !ref_v || !tr) return fail(SOPRO_ERR_INVALID, "reference K/V missing");
+    for (int v = 0; v < n_voices; ++v) {
+      if (tr[v] < 1 || tr[v] > 4096) return fail(SOPRO_ERR_INVALID, "reference K/V missing or Tr=%d out of range", tr[v]);
+      Tr_max = std::max(Tr_max, (int)tr[v]);
+      for (int i = 0; i < RL; ++i)
+        if (!ref_k[(size_t)i * n_voices + v] || !ref_v[(size_t)i * n_voices + v])
+          return fail(SOPRO_ERR_INVALID, "reference K/V of layer %d, voice %d is null", i, v);
+    }
+  }
   CK(cudaSetDevice(p->device));
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long Mt = (long long)B * Lmax, Mc = (long long)B * n_frames;
   auto al = [](size_t x) { return (x + 63) / 64 * 64; };
   const size_t rows = (size_t)std::max(Mt, Mc);
-  const size_t need = (al(rows * D) * 3 + al(rows * 4 * D) + al((size_t)B * D) + al((size_t)B * 2 * D)) * 4;
+  // the voice table: K pointers [RL][n_voices] | V pointers [RL][n_voices] | tr [n_voices] | voice_of [B]
+  const size_t n_ptr = (size_t)RL * n_voices, tab_bytes = 2 * n_ptr * sizeof(void*) + ((size_t)n_voices + B) * sizeof(int);
+  const size_t need = (al(rows * D) * 3 + al(rows * 4 * D) + al((size_t)B * D) + al((size_t)B * 2 * D) + al((tab_bytes + 3) / 4)) * 4;
   if (p->ws_bytes < need) {
     CK(cudaStreamSynchronize(st));
     cudaFree(p->ws);
@@ -1085,8 +1112,25 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
   float* h = x + al(rows * D);
   float* q = h + al(rows * D);
   float* hid = q + al(rows * D);
-  float* fmid = hid + al(rows * 4 * D);  // [B][D] FiLM hidden
-  float* film = fmid + al((size_t)B * D);  // [B][2D]
+  float* fmid = hid + al(rows * 4 * D);           // [n_voices][D] FiLM hidden
+  float* film = fmid + al((size_t)B * D);         // [n_voices][2D]
+  char* tab = reinterpret_cast<char*>(film + al((size_t)B * 2 * D));
+  const float* const* kv_dev = reinterpret_cast<const float* const*>(tab);
+  const int* tr_dev = reinterpret_cast<const int*>(tab + 2 * n_ptr * sizeof(void*));
+  const int* voice_dev = tr_dev + n_voices;
+  {
+    // one copy from pageable memory: cudaMemcpyAsync has staged the bytes when it returns, so `host` may go
+    std::vector<char> host(tab_bytes);
+    if (n_ptr) {
+      memcpy(host.data(), ref_k, n_ptr * sizeof(void*));
+      memcpy(host.data() + n_ptr * sizeof(void*), ref_v, n_ptr * sizeof(void*));
+    }
+    std::vector<int> tr_h(n_voices, 1);
+    if (RL > 0) std::copy(tr, tr + n_voices, tr_h.begin());
+    memcpy(host.data() + 2 * n_ptr * sizeof(void*), tr_h.data(), (size_t)n_voices * sizeof(int));
+    memcpy(host.data() + 2 * n_ptr * sizeof(void*) + (size_t)n_voices * sizeof(int), voice_of, (size_t)B * sizeof(int));
+    CK(cudaMemcpyAsync(tab, host.data(), tab_bytes, cudaMemcpyHostToDevice, st));
+  }
   const float* W = p->dev;
   int rc;
   // ---- text encoder
@@ -1098,28 +1142,29 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
   CK(cudaGetLastError());
   mean_pool_kernel<<<B, 128, 0, st>>>(txt_seq, text_len, txt_pool, Lmax, D);
   CK(cudaGetLastError());
-  // ---- FiLM parameters from the speaker vector(s)
-  const int Bf = sv_shared ? 1 : B;
+  // ---- FiLM parameters of every voice, on the skinny kernel whatever n_voices is: each voice's row then has the
+  // reduction order of a one-voice (M = 1) launch (the tile kernel, taken above 16 rows by default, sums in another)
   dense::DenseOp g{};
-  g.A = sv; g.W = W + p->film_w0; g.bias = W + p->film_b0; g.C = fmid; g.M = Bf; g.N = D; g.K = SV; g.ldc = D; g.epi = dense::EPI_GELU;
-  if ((rc = launch_dense(g, 1, st))) return rc;
+  g.A = sv; g.W = W + p->film_w0; g.bias = W + p->film_b0; g.C = fmid; g.M = n_voices; g.N = D; g.K = SV; g.ldc = D; g.epi = dense::EPI_GELU;
+  if ((rc = launch_dense(g, 1, st, 16))) return rc;
   g = dense::DenseOp{};
-  g.A = fmid; g.W = W + p->film_w2; g.bias = W + p->film_b2; g.C = film; g.M = Bf; g.N = 2 * D; g.K = D; g.ldc = 2 * D; g.epi = dense::EPI_BIAS;
-  if ((rc = launch_dense(g, 1, st))) return rc;
-  film_rows_kernel<<<(unsigned)((Mc + 7) / 8), 256, 0, st>>>(txt_pool, W + p->frame_pos, W + p->film_ln_w, W + p->film_ln_b, film, sv_shared ? 1 : 0,
+  g.A = fmid; g.W = W + p->film_w2; g.bias = W + p->film_b2; g.C = film; g.M = n_voices; g.N = 2 * D; g.K = D; g.ldc = 2 * D; g.epi = dense::EPI_BIAS;
+  if ((rc = launch_dense(g, 1, st, 16))) return rc;
+  film_rows_kernel<<<(unsigned)((Mc + 7) / 8), 256, 0, st>>>(txt_pool, W + p->frame_pos, W + p->film_ln_w, W + p->film_ln_b, film, voice_dev,
                                                             style_strength, x, Mc, n_frames, D);
   CK(cudaGetLastError());
   // ---- reference cross-attention stack
-  const size_t rsmem = (size_t)8 * (2 * D + ((Tr + 3) & ~3)) * 4;
-  if (c.ref_layers > 0 && rsmem > 48 * 1024) {
+  const size_t rsmem = (size_t)8 * (2 * D + ((Tr_max + 3) & ~3)) * 4;
+  if (RL > 0 && rsmem > 48 * 1024) {
     static unsigned long long attr_done = 0;  // per device, like every function attribute
     if (tc::attr_needed(attr_done)) CK(cudaFuncSetAttribute(ref_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
-  for (int i = 0; i < c.ref_layers; ++i) {
+  for (int i = 0; i < RL; ++i) {
     g = dense::DenseOp{};
     g.A = x; g.W = W + p->ref[i].q_w; g.norm_w = W + p->ref[i].nq_w; g.C = q; g.M = (int)Mc; g.N = D; g.K = D; g.ldc = D; g.epi = dense::EPI_BIAS;
     if ((rc = launch_dense(g, 1, st))) return rc;
-    ref_attn_kernel<<<(unsigned)((Mc + 7) / 8), 256, rsmem, st>>>(q, x, ref_k[i], ref_v[i], h, Mc, D, H, Tr);
+    ref_attn_kernel<<<(unsigned)((Mc + 7) / 8), 256, rsmem, st>>>(q, x, voice_dev, tr_dev, kv_dev + (size_t)i * n_voices,
+                                                                  kv_dev + n_ptr + (size_t)i * n_voices, h, Mc, n_frames, D, H, Tr_max);
     CK(cudaGetLastError());
     g = dense::DenseOp{};
     g.A = h; g.W = W + p->ref[i].o_w; g.R = x; g.C = x; g.M = (int)Mc; g.N = D; g.K = D; g.ldc = D; g.epi = dense::EPI_RES_GATE;
@@ -1129,6 +1174,38 @@ int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t
   dense::rmsnorm_rows_kernel<<<(unsigned)((Mc + 7) / 8), 256, 0, st>>>(x, W + p->cond_norm_w, nullptr, nullptr, cond_ar, Mc, D);
   CK(cudaGetLastError());
   return SOPRO_OK;
+}
+
+}  // namespace pstage
+
+extern "C" {
+
+int sopro_prefill_run(sopro_prefill_t* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, const float* sv,
+                      int sv_shared, const float* const* ref_k, const float* const* ref_v, int Tr, float style_strength, int n_frames,
+                      float* txt_seq, float* txt_pool, float* cond_ar, void* stream) {
+  if (!p || !text_ids || !text_len || !sv || !txt_seq || !txt_pool || !cond_ar) return fail(SOPRO_ERR_INVALID, "null argument");
+  // one voice (sv_shared), or one speaker vector per text over the same K / V: a table of B voices that differ in sv only
+  const int nb = std::max(B, 1), nv = sv_shared ? 1 : nb, RL = p->cfg.ref_layers;
+  std::vector<int32_t> voice_of(nb), tr(nv, Tr);
+  for (int b = 0; b < nb; ++b) voice_of[b] = sv_shared ? 0 : b;
+  std::vector<const float*> kp((size_t)RL * nv), vp((size_t)RL * nv);
+  const bool kv = ref_k && ref_v;
+  for (int i = 0; kv && i < RL; ++i)
+    for (int v = 0; v < nv; ++v) {
+      kp[(size_t)i * nv + v] = ref_k[i];
+      vp[(size_t)i * nv + v] = ref_v[i];
+    }
+  return pstage::prefill_core(p, text_ids, text_len, B, Lmax, nv, voice_of.data(), sv, tr.data(), kv ? kp.data() : nullptr,
+                              kv ? vp.data() : nullptr, style_strength, n_frames, txt_seq, txt_pool, cond_ar,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sopro_prefill_run_voices(sopro_prefill_t* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, int n_voices,
+                             const int32_t* voice_of, const float* sv, const int32_t* tr, const float* const* ref_k,
+                             const float* const* ref_v, float style_strength, int n_frames, float* txt_seq, float* txt_pool,
+                             float* cond_ar, void* stream) {
+  return pstage::prefill_core(p, text_ids, text_len, B, Lmax, n_voices, voice_of, sv, tr, ref_k, ref_v, style_strength, n_frames, txt_seq,
+                              txt_pool, cond_ar, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
@@ -1258,13 +1335,15 @@ __global__ void __launch_bounds__(256) attn_stats_pool_kernel(const float* __res
   }
 }
 
-// F.normalize(e, eps): e / max(||e||, eps), one warp per row b = blockIdx.x of e / out [B][n]; with ref [n], also
-// cos[b] = out[b] . ref (the rows and ref are unit vectors, so this is their cosine)
+// F.normalize(e, eps): e / max(||e||, eps), one warp per row b = blockIdx.x of e / out [B][n]; with ref, also
+// cos[b] = out[b] . ref[b * ref_stride .. + n) (the rows and ref are unit vectors, so this is their cosine; ref_stride 0:
+// every row against the one vector ref [n])
 __global__ void l2_normalize_kernel(const float* __restrict__ e, float* __restrict__ out, int n, float eps,
-                                    const float* __restrict__ ref, float* __restrict__ cos) {
+                                    const float* __restrict__ ref, int ref_stride, float* __restrict__ cos) {
   const int lane = threadIdx.x;
   e += (size_t)blockIdx.x * n;
   out += (size_t)blockIdx.x * n;
+  if (ref) ref += (size_t)blockIdx.x * ref_stride;
   float s = 0.f;
   for (int i = lane; i < n; i += 32) s = fmaf(e[i], e[i], s);
 #pragma unroll
@@ -1326,13 +1405,13 @@ int grow_ws(sopro_refprep* p, size_t need, cudaStream_t st) {
 }
 
 // Token2SV of B code sequences, tokens [B][Tmax][Q], lens[b] (host) frames each -> sv [B][SV], and cos [B] when ref_sv
-// is given.  x / h / q: [sum lens][d] each, stats [B][2d], e [B][SV], rows: 2B ints (device).  A row's result does not
+// is given (row b against ref_sv + b * ref_stride).  x / h / q: [sum lens][d] each, stats [B][2d], e [B][SV], rows: 2B ints (device).  A row's result does not
 // depend on the batch: the convolutions and the pooling stay inside each sequence, and both matmuls run each row in the
 // reduction order it gets alone -- a sequence of <= 16 frames (and the B-row projection) on the skinny kernel in blocks
 // of 16 rows, longer sequences on the tile kernel, whose order does not depend on M.  So the long sequences are packed
 // first, the short ones after them, and the pooling matmul is one launch per kind.
-int token2sv(sopro_refprep* p, const int32_t* tokens, int B, int Tmax, const int32_t* lens, float* sv, const float* ref_sv, float* cos,
-             float* x, float* h, float* q, float* stats, float* e, int* rows, cudaStream_t st) {
+int token2sv(sopro_refprep* p, const int32_t* tokens, int B, int Tmax, const int32_t* lens, float* sv, const float* ref_sv, int ref_stride,
+             float* cos, float* x, float* h, float* q, float* stats, float* e, int* rows, cudaStream_t st) {
   const sopro_refprep_config_t& c = p->cfg;
   const int d = c.sv_embed_dim, SV = c.sv_dim, Q = c.n_codebooks, V = c.codebook_size;
   std::vector<int> host(2 * (size_t)B);
@@ -1371,7 +1450,7 @@ int token2sv(sopro_refprep* p, const int32_t* tokens, int B, int Tmax, const int
   g = dense::DenseOp{};
   g.A = stats; g.W = W + p->proj_w; g.bias = W + p->proj_b; g.C = e; g.M = B; g.N = SV; g.K = 2 * d; g.ldc = SV; g.epi = dense::EPI_BIAS;
   if ((rc = launch_dense(g, 1, st, 16))) return rc;
-  l2_normalize_kernel<<<B, 32, 0, st>>>(e, sv, SV, 1e-6f, ref_sv, cos);
+  l2_normalize_kernel<<<B, 32, 0, st>>>(e, sv, SV, 1e-6f, ref_sv, ref_stride, cos);
   CK(cudaGetLastError());
   return SOPRO_OK;
 }
@@ -1483,7 +1562,7 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
   dense::DenseOp g{};
   // ---- Token2SV: the batched path with B = 1 (d <= D: the [Tr][d] buffers live in x / h / q)
   const int32_t len = Tr;
-  if ((rc = token2sv(p, tokens, 1, Tr, &len, sv, nullptr, nullptr, x, h, q, stats, e, seq_rows, st))) return rc;
+  if ((rc = token2sv(p, tokens, 1, Tr, &len, sv, nullptr, 0, nullptr, x, h, q, stats, e, seq_rows, st))) return rc;
   // ---- reference encoder
   codes_mix_kernel<<<Tr, 128, Q * sizeof(int), st>>>(tokens, W + p->cb_embed, W + p->ref_w, x, Q, V, D, p->bad, nullptr, 0);
   CK(cudaGetLastError());
@@ -1506,8 +1585,13 @@ int sopro_refprep_run(sopro_refprep_t* p, const int32_t* tokens, int Tr, float* 
   return SOPRO_OK;
 }
 
-int sopro_refprep_speaker_vectors(sopro_refprep_t* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host,
-                                  float* sv, const float* ref_sv, float* cos, void* stream) {
+}  // extern "C"
+
+namespace pstage {
+
+// sopro_refprep_speaker_vectors with row b scored against ref_sv + b * ref_stride (0: one vector for every row)
+int speaker_vectors(sopro_refprep* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host, float* sv,
+                    const float* ref_sv, int ref_stride, float* cos, cudaStream_t st) {
   if (!p || !tokens || !lens_host || !sv) return fail(SOPRO_ERR_INVALID, "null argument");
   if (B < 1 || B > 65535) return fail(SOPRO_ERR_INVALID, "B=%d outside [1, 65535]", B);
   if (Tmax < 1 || Tmax > 4096) return fail(SOPRO_ERR_INVALID, "Tmax=%d outside [1, 4096]", Tmax);
@@ -1518,19 +1602,34 @@ int sopro_refprep_speaker_vectors(sopro_refprep_t* p, const int32_t* tokens, int
     total += (size_t)lens_host[b];
   }
   CK(cudaSetDevice(p->device));
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const size_t d = p->cfg.sv_embed_dim, SV = p->cfg.sv_dim, nb = (size_t)B;
-  const auto al = pstage::al64;
+  const auto al = al64;
   const size_t need = (al(total * d) * 3 + al(nb * 2 * d) + al(nb * SV) + al(2 * nb)) * 4;
   int rc;
-  if ((rc = pstage::grow_ws(p, need, st))) return rc;
+  if ((rc = grow_ws(p, need, st))) return rc;
   float* x = p->ws;
   float* h = x + al(total * d);
   float* q = h + al(total * d);
   float* stats = q + al(total * d);
   float* e = stats + al(nb * 2 * d);
   int* rows = reinterpret_cast<int*>(e + al(nb * SV));
-  return pstage::token2sv(p, tokens, B, Tmax, lens_host, sv, ref_sv, cos, x, h, q, stats, e, rows, st);
+  return token2sv(p, tokens, B, Tmax, lens_host, sv, ref_sv, ref_stride, cos, x, h, q, stats, e, rows, st);
+}
+
+}  // namespace pstage
+
+extern "C" {
+
+int sopro_refprep_speaker_vectors(sopro_refprep_t* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host,
+                                  float* sv, const float* ref_sv, float* cos, void* stream) {
+  return pstage::speaker_vectors(p, tokens, B, Tmax, lens_host, sv, ref_sv, 0, cos, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sopro_refprep_speaker_vectors_per_row(sopro_refprep_t* p, const int32_t* tokens, int32_t B, int32_t Tmax, const int32_t* lens_host,
+                                          float* sv, const float* ref_sv, float* cos, void* stream) {
+  if (!ref_sv || !cos) return fail(SOPRO_ERR_INVALID, "ref_sv and cos are required");
+  return pstage::speaker_vectors(p, tokens, B, Tmax, lens_host, sv, ref_sv, p ? p->cfg.sv_dim : 0, cos,
+                                 reinterpret_cast<cudaStream_t>(stream));
 }
 
 /* Synchronises `stream`; SOPRO_ERR_INVALID if a run since the last check met a code outside [0, codebook_size). */

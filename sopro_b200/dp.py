@@ -77,9 +77,14 @@ class DataParallelTTS:
         return shard_range(n_items, self.rank, self.world)
 
     def synthesize_batch(self, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int]] = None, **kw):
-        """-> (waveforms of THIS rank's utterances, (lo, hi)): texts[lo:hi] of the global batch."""
+        """-> (waveforms of THIS rank's utterances, (lo, hi)): texts[lo:hi] of the global batch.  `ref`: one prepared
+        reference, or one per text of the global batch (sliced with the texts)."""
+        per_text = isinstance(ref, Sequence) and not isinstance(ref, (str, bytes))
+        if per_text and len(ref) != len(texts):  # refused on every rank alike, before any work
+            raise ValueError(f"ref holds {len(ref)} voices for {len(texts)} texts; pass one PreparedReference or one per text")
         lo, hi = self.shard(len(texts))
         if hi <= lo:
             return [], (lo, hi)
-        wavs = self.tts.synthesize_batch(list(texts[lo:hi]), ref=ref, seeds=None if seeds is None else list(seeds[lo:hi]), **kw)
+        mine = list(ref[lo:hi]) if per_text else ref
+        wavs = self.tts.synthesize_batch(list(texts[lo:hi]), ref=mine, seeds=None if seeds is None else list(seeds[lo:hi]), **kw)
         return wavs, (lo, hi)

@@ -15,7 +15,7 @@ from __future__ import annotations
 import contextlib
 import os
 import threading
-from typing import Dict, Iterator, List, Optional, Sequence, Tuple
+from typing import Dict, Iterator, List, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -24,6 +24,7 @@ from . import longform as LF
 from . import prefill as P
 from . import rerank
 from . import timestamps as TS
+from . import voices
 from ._lib import StatePool
 from .codec import MimiCodec
 from .config import TARGET_SR, SoproTTSConfig
@@ -490,22 +491,28 @@ class SoproTTS:
         return (wav, words) if word_timestamps else wav
 
     @torch.inference_mode()
-    def synthesize_batch(self, texts: Sequence[str], *, ref: PreparedReference, max_frames: int = 400, top_p: float = 0.9,
+    def synthesize_batch(self, texts: Sequence[str], *, ref: Union[PreparedReference, Sequence[PreparedReference]],
+                         max_frames: int = 400, top_p: float = 0.9,
                          temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                          min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                          sample_rate: Optional[int] = None, speed: Optional[float] = None,
                          loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1,
                          watermark: Optional[int] = None):
-        """NEW: B texts with one shared prepared reference -> B waveforms [1, 1, N_i].  One batched prefill, one
-        persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, then
+        """NEW: B texts -> B waveforms [1, 1, N_i].  `ref`: one prepared reference for every text, or a sequence of B, a
+        voice per text (texts that pass the same object share its K / V; sopro_b200/voices.py).  One batched prefill,
+        one persistent AR launch, one ragged NAR pass, padded Mimi decodes (each time-stretched, then resampled, then
         loudness-normalised, in one ragged launch when `speed` / `sample_rate` / `loudness` is given); utterance i equals
-        synthesize(texts[i], seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness).
+        synthesize(texts[i], ref=ref[i] (or ref), seed=seeds[i], sample_rate=sample_rate, speed=speed, loudness=loudness).
         `word_timestamps`: also return each utterance's word timings (see synthesize), ``(List[wav], List[List[WordTiming]])``.
         `best_of`: each text's takes are generated in the same pass (B x best_of rows, take k of text i with seed
-        seeds[i] + k) and only the picked take of each text is decoded (see synthesize).  `watermark`: every
-        utterance carries the key's mark (see synthesize)."""
+        seeds[i] + k, in text i's voice) and only the picked take of each text is decoded (see synthesize; text i's takes
+        are scored against its own voice's sv_ref).  `watermark`: every utterance carries the key's mark (see
+        synthesize).  A `ref` sequence of the wrong length (ValueError), an element that is not a PreparedReference
+        (TypeError), a voice of another geometry or outside [1, 4096] reference frames (ValueError) or with a key
+        padding mask (NotImplementedError) is refused before any device work or random draw."""
         post = OutputChain(self, sample_rate, speed, loudness, watermark)
         n_best = self._check_best_of(best_of, len(texts))
+        voices.check_voices(ref, len(texts), **voices.geometry(self.cfg))
         tr: Optional[dict] = {} if word_timestamps else None
         Ts, codes = self._best_codes(texts, ref, n_best, max_frames=max_frames, top_p=top_p, temperature=temperature,
                                      anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
@@ -591,26 +598,30 @@ class SoproTTS:
         hop = self.codec.engine.hop
         return [TS.utterance_timings(t, sp, first[i], int(Ts[i]), hop, S) for i, (t, sp) in enumerate(zip(texts, spans))]
 
-    def _best_codes(self, texts: Sequence[str], ref: PreparedReference, best_of: int, *, seeds: Optional[Sequence[int]],
+    def _best_codes(self, texts: Sequence[str], ref, best_of: int, *, seeds: Optional[Sequence[int]],
                     trace_out: Optional[dict] = None, generator: Optional[torch.Generator] = None,
                     **kw) -> Tuple[List[int], Optional[torch.Tensor]]:
         """_batch_codes with `best_of` candidates per text (sopro_b200/rerank.py): text i's candidate k is row i*N + k
-        of ONE _batch_codes pass, with seed seeds[i] + k; every take is scored with one Token2SV launch against
-        ref.sv_ref, rerank.choose picks one per text, and only the picked rows are returned (the trace too), so the
-        caller decodes those alone.  best_of = 1 is _batch_codes itself."""
+        of ONE _batch_codes pass, with seed seeds[i] + k and text i's voice; every take is scored with one Token2SV
+        launch against its text's voice's sv_ref, rerank.choose picks one per text, and only the picked rows are returned
+        (the trace too), so the caller decodes those alone.  best_of = 1 is _batch_codes itself."""
         N = int(best_of)
         if N == 1:
             return self._batch_codes(texts, ref, seeds=seeds, trace_out=trace_out, generator=generator, **kw)
+        slots, of = voices.voice_slots(ref, len(texts))
         rows = [t for t in texts for _ in range(N)]
+        row_ref = slots[0] if len(slots) == 1 else [slots[of[r // N]] for r in range(len(rows))]
         tr: Optional[dict] = {} if trace_out is not None else None
         info: dict = {}
-        Ts, codes = self._batch_codes(rows, ref, seeds=rerank.candidate_seeds(seeds, N), trace_out=tr, generator=generator,
+        Ts, codes = self._batch_codes(rows, row_ref, seeds=rerank.candidate_seeds(seeds, N), trace_out=tr, generator=generator,
                                       info=info, **kw)
         cos = [0.0] * len(rows)
         live = [r for r in range(len(rows)) if Ts[r] > 0]
         if live:  # the takes with frames, in one launch
+            sv_ref = slots[0].sv_ref if len(slots) == 1 else torch.cat(
+                [slots[of[r // N]].sv_ref.to(codes.device, torch.float32).reshape(1, -1) for r in live])
             _sv, c = self.model.refprep.speaker_vectors(codes[torch.tensor(live, device=codes.device)], [Ts[r] for r in live],
-                                                        ref.sv_ref)
+                                                        sv_ref)
             for r, v in zip(live, c.tolist()):
                 cos[r] = v
         picks = []
@@ -637,11 +648,12 @@ class SoproTTS:
             rerank.check_rows(rows * n, self._batch_limit())
         return n
 
-    def _batch_codes(self, texts: Sequence[str], ref: PreparedReference, *, max_frames: int, top_p: float,
+    def _batch_codes(self, texts: Sequence[str], ref, *, max_frames: int, top_p: float,
                      temperature: float, anti_loop: bool, style_strength: Optional[float], min_gen_frames: Optional[int],
                      seeds: Optional[Sequence[int]], trace_out: Optional[dict] = None, generator: Optional[torch.Generator] = None,
                      info: Optional[dict] = None) -> Tuple[List[int], Optional[torch.Tensor]]:
-        """B texts with one prepared reference: one batched prefill, one persistent AR launch, one ragged NAR pass ->
+        """B texts with one prepared reference, or one each (`ref` as in synthesize_batch): one batched prefill, one
+        persistent AR launch, one ragged NAR pass ->
         (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0 frames).
         `trace_out` (word timestamps): receives "probs", the AR launch's attention weights, and "lens", the text lengths.
         `info` (best-of-N): receives "stopped", whether each row sampled an EOS, and "text_lens"."""

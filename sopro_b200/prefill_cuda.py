@@ -1,5 +1,5 @@
 """Host side of the CUDA prefill (libsopro_b200.so: sopro_prefill_*; reference model.py:172-216): text encoder,
-FiLM, cached reference cross-attention and cond_norm for B texts sharing one prepared reference voice -- and of the
+FiLM, cached reference cross-attention and cond_norm for B texts over a table of prepared reference voices -- and of the
 once-per-voice reference preparation in front of it (sopro_refprep_*; reference model.py:152-170)."""
 from __future__ import annotations
 
@@ -8,7 +8,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from . import _lib
+from . import _lib, voices
 from .config import SoproTTSConfig
 from .nar import _f32, fill_ssm_block
 
@@ -58,9 +58,11 @@ class PrefillEngine:
         del keep
 
     def run(self, text_ids: Sequence[torch.Tensor], ref, *, n_frames: int, style_strength: float):
-        """text_ids: B 1-D id tensors; ref: PreparedReference (shared).  -> txt_seq [B, Lmax, D], lens (list),
-        txt_pool [B, D], cond_ar [B, n_frames, D] on the device."""
+        """text_ids: B 1-D id tensors; ref: one PreparedReference for every text, or a sequence of B (a voice per text;
+        rows that pass the same object share its K / V).  -> txt_seq [B, Lmax, D], lens (list), txt_pool [B, D],
+        cond_ar [B, n_frames, D] on the device.  Text b's rows equal, bit for bit, those of run(text_ids, ref[b])."""
         B = len(text_ids)
+        slots, voice_of = voices.check_voices(ref, B, **voices.geometry(self.cfg))
         lens = [int(t.numel()) for t in text_ids]
         if min(lens) < 1:
             raise ValueError("empty text")
@@ -72,30 +74,45 @@ class PrefillEngine:
             ids[i, : lens[i]] = t.to("cpu", torch.int32)
         ids = ids.to(self.device, non_blocking=True)
         ln = torch.tensor(lens, dtype=torch.int32).to(self.device, non_blocking=True)
-        sv = ref.sv_ref.to(self.device, torch.float32).reshape(-1, ref.sv_ref.shape[-1]).contiguous()
-        ks: List[torch.Tensor] = []
-        vs: List[torch.Tensor] = []
-        Tr = 1
-        for c in ref.ref_kv_caches[: self.n_ref]:
-            if c.get("key_padding_mask") is not None:
-                raise NotImplementedError("prepared references with a key padding mask are not produced by prepare_reference")
-            k = c["k"].to(self.device, torch.float32)
-            v = c["v"].to(self.device, torch.float32)
-            if k.dim() == 4:
-                if k.size(0) != 1:
-                    raise ValueError("the prefill batches texts over ONE shared prepared reference")
-                k, v = k[0], v[0]
-            ks.append(k.contiguous())
-            vs.append(v.contiguous())
-            Tr = int(k.shape[1])
-        kp = (C.c_void_p * max(1, self.n_ref))(*[int(k.data_ptr()) for k in ks])
-        vp = (C.c_void_p * max(1, self.n_ref))(*[int(v.data_ptr()) for v in vs])
+        svs = [r.sv_ref.to(self.device, torch.float32).reshape(-1, r.sv_ref.shape[-1]) for r in slots]
+        if len(slots) == 1 and svs[0].shape[0] > 1:
+            voice_of = list(range(B))  # one PreparedReference with a speaker vector per text over one K / V
+        sv = torch.cat(svs).contiguous()
+        nv = int(sv.shape[0])
+        ks: List[List[torch.Tensor]] = []  # [voice][layer]
+        vs: List[List[torch.Tensor]] = []
+        trs: List[int] = []
+        for r in slots:
+            kl, vl, Tr = [], [], 1
+            for c in r.ref_kv_caches[: self.n_ref]:
+                if c.get("key_padding_mask") is not None:
+                    raise NotImplementedError("prepared references with a key padding mask are not produced by prepare_reference")
+                k = c["k"].to(self.device, torch.float32)
+                v = c["v"].to(self.device, torch.float32)
+                if k.dim() == 4:
+                    if k.size(0) != 1:
+                        raise ValueError("the prefill batches texts over ONE shared prepared reference")
+                    k, v = k[0], v[0]
+                kl.append(k.contiguous())
+                vl.append(v.contiguous())
+                Tr = int(k.shape[1])
+            ks.append(kl)
+            vs.append(vl)
+            trs.append(Tr)
+        if len(slots) < nv:  # the speaker vectors share the one voice's K / V
+            ks, vs, trs = ks * nv, vs * nv, trs * nv
+        n = max(1, self.n_ref * nv)
+        kp = (C.c_void_p * n)(*[int(ks[v][i].data_ptr()) for i in range(self.n_ref) for v in range(nv)])
+        vp = (C.c_void_p * n)(*[int(vs[v][i].data_ptr()) for i in range(self.n_ref) for v in range(nv)])
+        vmap = (C.c_int32 * B)(*voice_of)
+        tr = (C.c_int32 * nv)(*trs)
         txt_seq = torch.empty((B, Lmax, self.D), dtype=torch.float32, device=self.device)
         txt_pool = torch.empty((B, self.D), dtype=torch.float32, device=self.device)
         cond = torch.empty((B, int(n_frames), self.D), dtype=torch.float32, device=self.device)
-        _lib.check(self.lib.sopro_prefill_run(self._h, ids.data_ptr(), ln.data_ptr(), B, Lmax, sv.data_ptr(), 1 if sv.shape[0] == 1 else 0,
-                                              kp, vp, Tr, float(style_strength), int(n_frames), txt_seq.data_ptr(), txt_pool.data_ptr(),
-                                              cond.data_ptr(), int(torch.cuda.current_stream(self.device).cuda_stream)))
+        _lib.check(self.lib.sopro_prefill_run_voices(self._h, ids.data_ptr(), ln.data_ptr(), B, Lmax, nv, vmap, sv.data_ptr(), tr,
+                                                     kp, vp, float(style_strength), int(n_frames), txt_seq.data_ptr(),
+                                                     txt_pool.data_ptr(), cond.data_ptr(),
+                                                     int(torch.cuda.current_stream(self.device).cuda_stream)))
         self._keep = (ids, ln, sv, ks, vs)  # alive until the stream has consumed them
         return txt_seq, lens, txt_pool, cond
 
@@ -179,26 +196,32 @@ class RefPrepEngine:
     def speaker_vectors(self, codes: torch.Tensor, lens: Sequence[int], ref_sv: Optional[torch.Tensor] = None
                         ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """Token2SV of a ragged batch in one pass: codes [B, Tmax, Q] (row b's first lens[b] frames) -> (sv [B, sv_dim],
-        cos [B] with `ref_sv` [sv_dim] or [1, sv_dim], else None) on the device.  Row b equals ``run(codes[b, :lens[b]])[0]``
-        bit for bit.  Refused geometry raises ValueError before any launch; a code outside the codebook IndexError."""
+        cos [B] with `ref_sv`, else None) on the device.  `ref_sv`: [sv_dim] or [1, sv_dim], one vector for every row,
+        or [B, sv_dim], row b's own (cos[b] against ref_sv[b]).  Row b equals ``run(codes[b, :lens[b]])[0]`` bit for bit,
+        and its cos the one-vector call's with its vector.  Refused geometry raises ValueError before any launch; a code
+        outside the codebook IndexError."""
         if codes.dim() != 3 or int(codes.shape[2]) != self.Q:
             raise ValueError(f"codes must be [B, Tmax, {self.Q}], got {tuple(codes.shape)}")
         B, Tmax = int(codes.shape[0]), int(codes.shape[1])
         ln = torch.tensor([int(x) for x in lens], dtype=torch.int32)
         if int(ln.numel()) != B:
             raise ValueError(f"{int(ln.numel())} lengths for {B} sequences")
-        ref = None
+        ref, per_row = None, False
         if ref_sv is not None:
-            ref = ref_sv.to(self.device, torch.float32).reshape(-1).contiguous()
-            if int(ref.numel()) != self.sv_dim:
-                raise ValueError(f"ref_sv must hold {self.sv_dim} values, got {int(ref.numel())}")
+            per_row = ref_sv.dim() == 2 and int(ref_sv.shape[0]) > 1
+            ref = ref_sv.to(self.device, torch.float32).contiguous() if per_row else \
+                ref_sv.to(self.device, torch.float32).reshape(-1).contiguous()
+            want = (B, self.sv_dim) if per_row else (self.sv_dim,)
+            if tuple(ref.shape) != want:
+                raise ValueError(f"ref_sv must be [{self.sv_dim}], [1, {self.sv_dim}] or [B={B}, {self.sv_dim}], "
+                                 f"got {tuple(ref_sv.shape)}")
         tok = codes.to(self.device, torch.int32).contiguous()
         sv = torch.empty((max(B, 1), self.sv_dim), dtype=torch.float32, device=self.device)
         cos = torch.empty(max(B, 1), dtype=torch.float32, device=self.device) if ref is not None else None
         st = int(torch.cuda.current_stream(self.device).cuda_stream)
-        _lib.check_arg(self.lib.sopro_refprep_speaker_vectors(self._h, tok.data_ptr(), B, Tmax, ln.data_ptr(), sv.data_ptr(),
-                                                               None if ref is None else ref.data_ptr(),
-                                                               None if cos is None else cos.data_ptr(), st))
+        fn = self.lib.sopro_refprep_speaker_vectors_per_row if per_row else self.lib.sopro_refprep_speaker_vectors
+        _lib.check_arg(fn(self._h, tok.data_ptr(), B, Tmax, ln.data_ptr(), sv.data_ptr(), None if ref is None else ref.data_ptr(),
+                          None if cos is None else cos.data_ptr(), st))
         try:
             _lib.check(self.lib.sopro_refprep_check(self._h, st))  # also keeps `tok` and `ref` alive until read
         except _lib.SoproError as e:

@@ -920,6 +920,40 @@ int sopro_watermark_push(sopro_watermark_stream_t* s, const float* x, int64_t n,
 /* the held samples, marked -> y (device); SOPRO_ERR_STATE when called twice without a reset */
 int sopro_watermark_finish(sopro_watermark_stream_t* s, float* y, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Reference-voice denoising (no reference counterpart): a stationary-noise Wiener suppressor with the decision-directed
+ * a priori SNR estimate (Ephraim-Malah), for SoproTTS.prepare_references(denoise=True).  Each row of n samples at
+ * 24 kHz on its own:
+ *   Frames: N = SOPRO_DENOISE_FRAME, R = SOPRO_DENOISE_HOP; w[j] = sqrt(0.5 - 0.5 cos(2 pi j / N)) (periodic sqrt-Hann)
+ *   for analysis and synthesis; M = ceil(n / R) + 1 frames, frame m covering samples [(m - 1) R, (m + 1) R) with zeros
+ *   outside [0, n); X[m][k], k = 0 .. N/2, and P[m][k] = |X|^2.
+ *   Noise, once per row: E[m] = sum of P[m][k], in double with k ascending.  Of the C = floor(n / R) - 1 frames wholly
+ *   inside the row (m = 1 .. C), the K = max(1, floor(C / 10)) with the smallest E, ties to the lower m; lambda[k] = the
+ *   mean of their P[m][k], summed in double with m ascending.
+ *   Gain, per bin, in double: gamma = P / lambda; xi[0] = max(gamma[0] - 1, 0);
+ *   xi[m] = 0.98 G[m-1]^2 gamma[m-1] + 0.02 max(gamma[m] - 1, 0); G[m] = max(xi / (1 + xi), 0.1) (a -20 dB floor);
+ *   G = 1 in every frame of a bin where lambda = 0.
+ *   Synthesis: G X, inverse real FFT, times w; y[i] = frame q's second half + frame q + 1's first half, q = floor(i / R),
+ *   added in that order.
+ *   A row with n < N or a non-finite E[m] comes back unchanged.  w^2 at hop N/2 sums to 1, so G = 1 reconstructs the
+ *   input in exact arithmetic.
+ * The device FFT is a 512-point shared-memory radix-2 transform in fp32 (twiddles and window computed in double, rounded
+ * once); E, lambda and the recursion run in double.  Every sum runs in an order fixed by the row's own positions, so a
+ * row's output is the same alone and in any batch, bit for bit.  No call synchronises or allocates. */
+#define SOPRO_DENOISE_FRAME 512
+#define SOPRO_DENOISE_HOP 256
+/* host-only: the device workspace bytes of one call over B rows of at most max_len samples; SOPRO_ERR_INVALID for bad
+ * geometry (B < 1, max_len outside [0, 2^36]) or a null ws_bytes */
+int sopro_denoise_sizes(int32_t B, int64_t max_len, int64_t* ws_bytes);
+/* ragged batch, five launches per 128 rows: row b of x [B][x_stride] f32 (device) has lens_host[b] samples (HOST i64;
+ * NULL = x_stride each); samples at or past lens[b] are not read.  Row b of y (device, y + b * y_stride, y_stride >=
+ * x_stride when B > 1) receives lens[b] outputs, then zeros up to x_stride.  ws: device, sopro_denoise_sizes(B, the
+ * longest row) bytes; on return it begins with sel [B][Kmax] i32, Kmax = K of the longest row (1 below N): row b's
+ * selected noise frames in ascending order, then -1 (all -1 for a row that passed through) -- a test hook.  y must not
+ * overlap x.  Bad geometry or a null pointer is SOPRO_ERR_INVALID before any launch. */
+int sopro_denoise(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, void* ws, float* y, int64_t y_stride,
+                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,7 +7,7 @@ from .config import SoproTTSConfig  # noqa: F401
 
 __version__ = "0.1.0"
 __all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac", "WordTiming",
-           "detect_watermark"]
+           "detect_watermark", "denoise"]
 
 
 def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
@@ -19,6 +19,10 @@ def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
         from .watermark import detect_watermark
 
         return detect_watermark
+    if name == "denoise":
+        from .denoising import denoise
+
+        return denoise
     if name == "SoproTTS":
         from .model import SoproTTS
 

@@ -274,6 +274,8 @@ SYMBOLS = {
     "sopro_watermark_stream_ready": (C.c_int64, [_VP, C.c_int64, _I]),
     "sopro_watermark_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP]),
     "sopro_watermark_finish": (_I, [_VP, _VP, _VP]),
+    "sopro_denoise_sizes": (_I, [C.c_int32, C.c_int64, C.POINTER(C.c_int64)]),
+    "sopro_denoise": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP, C.c_int64, _VP]),
 }
 
 _lib = None

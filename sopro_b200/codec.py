@@ -409,17 +409,22 @@ class MimiCodec:
 
     @torch.no_grad()
     def prepare_wavs(self, wavs: Sequence[torch.Tensor], sample_rates: Sequence[int],
-                     crop_seconds: Optional[float] = None) -> Tuple[torch.Tensor, List[int]]:
+                     crop_seconds: Optional[float] = None, denoise: bool = False) -> Tuple[torch.Tensor, List[int]]:
         """``encode_file``'s preparation of a ragged batch on the device: clips [n] or [C, n] (any device, channels
         averaged), each at its own rate -> (wav [B, L] f32 @24 kHz on the device, valid samples per row; zeros past them).
         Per clip: energy trim at its rate (one launch for the batch), resample to 24 kHz (one launch per distinct rate;
         a 24 kHz clip is not resampled), centre crop to `crop_seconds` as encode_file does (None or <= 0: no crop).  The
         one host read is the B trim extents.  The trim sums in fp64 where the reference's torch ops sum in fp32, so only
         a frame within rounding of the threshold can be classified differently from ``encode_file``; the resampler is
-        §5d's (DESIGN.md), not torchaudio's fp32 kernel."""
+        §5d's (DESIGN.md), not torchaudio's fp32 kernel.
+        `denoise` (extension): after the resample, each trimmed clip goes through ``denoising.denoise`` (DESIGN.md §5n)
+        before the crop, so that the noise estimate sees the whole clip; 24 kHz clips are then packed too, since the
+        denoiser writes a new buffer.  The clips are denoised in groups of at most ENC_MAX_SAMPLES padded samples."""
         from . import ingest
+        from .denoising import check_denoise
         from .resample import Resampler
 
+        check_denoise(denoise)
         wavs, sample_rates = list(wavs), list(sample_rates)
         if not wavs or len(sample_rates) != len(wavs):
             raise ValueError(f"{len(wavs)} clips with {len(sample_rates)} sample rates")
@@ -432,7 +437,7 @@ class MimiCodec:
         keep = []  # resampled rows, alive until the last pack has been enqueued
         by_rate: Dict[int, List[int]] = {}
         for b, (s, e) in enumerate(ext):
-            if rates[b] == TARGET_SR:
+            if rates[b] == TARGET_SR and not denoise:
                 src[b], n24[b] = rows[b].data_ptr() + 4 * s, e - s
             else:
                 by_rate.setdefault(rates[b], []).append(b)
@@ -440,17 +445,35 @@ class MimiCodec:
             lens = [ext[b][1] - ext[b][0] for b in idx]
             x = ingest.pack([rows[b].data_ptr() + 4 * ext[b][0] for b in idx], lens,
                             torch.empty((len(idx), max(lens)), dtype=torch.float32, device=self.device))
-            rs = self._in_resamplers.get(sr)
-            if rs is None:
-                rs = self._in_resamplers[sr] = Resampler(sr, TARGET_SR, self.device)
-            y = rs(x, lens)
+            if sr == TARGET_SR:
+                y, n = x, lens
+            else:
+                rs = self._in_resamplers.get(sr)
+                if rs is None:
+                    rs = self._in_resamplers[sr] = Resampler(sr, TARGET_SR, self.device)
+                y, n = rs(x, lens), [rs.length(v) for v in lens]
+            if denoise:
+                y = self._denoise_rows(y, n)
             keep.append(y)
             for j, b in enumerate(idx):
-                src[b], n24[b] = y[j].data_ptr(), rs.length(lens[j])
+                src[b], n24[b] = y[j].data_ptr(), n[j]
         plan = [ingest.crop_plan(n, win) for n in n24]
         out = torch.empty((B, max(n for _, n in plan)), dtype=torch.float32, device=self.device)
         ingest.pack([src[b] + 4 * plan[b][0] for b in range(B)], [n for _, n in plan], out)
         return out, [n for _, n in plan]
+
+    @staticmethod
+    def _denoise_rows(y: torch.Tensor, lens: Sequence[int]) -> torch.Tensor:
+        """denoising.denoise of the ragged batch y [k, L], in consecutive groups of at most ENC_MAX_SAMPLES padded
+        samples (the rows' results do not depend on the grouping) -> a new [k, L]."""
+        from .denoising import denoise
+        from .ingest import ENC_MAX_SAMPLES
+
+        out = torch.empty_like(y)
+        per = max(1, ENC_MAX_SAMPLES // max(1, int(y.shape[1])))
+        for i in range(0, int(y.shape[0]), per):
+            out[i: i + per] = denoise(y[i: i + per], lens[i: i + per])
+        return out
 
     @torch.no_grad()
     def encode_wavs(self, wav_bl: torch.Tensor, lens: Sequence[int]) -> List[torch.Tensor]:

@@ -28,6 +28,7 @@ from . import voices
 from ._lib import StatePool
 from .codec import MimiCodec
 from .config import TARGET_SR, SoproTTSConfig
+from .denoising import check_denoise
 from .engine import ArEngine, ArSession, Sampling
 from .nar import NarEngine
 from .prefill_cuda import PrefillEngine, RefPrepEngine
@@ -416,7 +417,7 @@ class SoproTTS:
 
     @torch.inference_mode()
     def prepare_references(self, clips: Sequence[ingest.Clip], *, sample_rates=None,
-                           ref_seconds: Optional[float] = None) -> List[PreparedReference]:
+                           ref_seconds: Optional[float] = None, denoise: bool = False) -> List[PreparedReference]:
         """(extension) Many reference voices in one batched pass, from files or in-memory audio -> one PreparedReference
         per clip, in order.  `clips`: paths (read with audio.load_audio_file) and / or float tensors [n] or [C, n] on
         any device (channels averaged).  `sample_rates`: one rate per clip (None for a path, which has its own), or one
@@ -426,12 +427,18 @@ class SoproTTS:
         centre crop, a batched Mimi encode whose every row equals encode_wav of that row alone), then prepare_reference
         per voice.  Against prepare_reference(ref_audio_path=...) the trim decisions can differ only at a frame within
         rounding of the threshold, and the resampler is this library's (DESIGN.md §5d, §5l).  Every argument is checked,
-        and the files read, before any device work."""
+        and the files read, before any device work.
+        `denoise` (extension): remove stationary background noise (fans, hum, room tone) from each trimmed 24 kHz clip
+        before the crop, with a CUDA Wiener suppressor whose noise estimate is the quietest tenth of the clip's frames
+        (sopro_b200/denoising.py, DESIGN.md §5n).  It assumes the clip pauses: one that never does loses some of its own
+        stationary content.  Whether it improves a clone has not been measured.  One denoised voice from a file:
+        ``prepare_references([path], denoise=True)[0]`` (prepare_reference keeps the reference's signature)."""
+        check_denoise(denoise)
         ingest.crop_samples(ref_seconds)
         wavs, rates = ingest.load_clips(clips, sample_rates)
         if ref_seconds is None:
             ref_seconds = ingest.DEFAULT_REF_SECONDS
-        wav_bl, lens = self.codec.prepare_wavs(wavs, rates, ref_seconds)
+        wav_bl, lens = self.codec.prepare_wavs(wavs, rates, ref_seconds, denoise=denoise)
         codes = self.codec.encode_wavs(wav_bl, lens)
         return [self.model.prepare_reference(c, device=self.device) for c in codes]
 

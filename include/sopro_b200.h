@@ -308,12 +308,20 @@ int sopro_mimi_check(sopro_mimi_t* m, void* stream);
  * One stream = one utterance; streams of one decoder are independent; the arithmetic mode is the decoder's at
  * create / reset time. */
 typedef struct sopro_mimi_stream sopro_mimi_stream_t;
-int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_stream_t** out);
+/* A stream of `rows` utterances in [1, 65535] decoded side by side: every step advances all rows by the same number of
+ * frames, and each row's state sits in its own slice of every buffer, so each kernel reads and writes only its own
+ * row and sums in a fixed order: row b's samples equal a one-row stream fed row b's codes, bit for bit, in both
+ * arithmetic modes.  A row whose utterance has ended can be fed code 0 and its samples dropped (the decoder is causal:
+ * its earlier samples do not change).  Device memory grows linearly with rows (sopro_mimi_stream_bytes). */
+int sopro_mimi_stream_create_rows(sopro_mimi_t* m, int max_chunk_frames, int rows, sopro_mimi_stream_t** out);
+int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_stream_t** out);  /* rows = 1 */
 int sopro_mimi_stream_destroy(sopro_mimi_stream_t* s);
 int sopro_mimi_stream_reset(sopro_mimi_stream_t* s, void* stream);     /* back to frame 0 (MimiDecodeState()) */
 int64_t sopro_mimi_stream_frames(const sopro_mimi_stream_t* s);        /* MimiDecodeState.frames_seen */
-/* the next n frames: codes [n_q, n] i32 (device) -> wav [n*1920] f32 (device); any n >= 1 (longer than
- * max_chunk_frames is processed in pieces) */
+int64_t sopro_mimi_stream_rows(const sopro_mimi_stream_t* s);
+int64_t sopro_mimi_stream_bytes(const sopro_mimi_stream_t* s);         /* device bytes the stream holds */
+/* the next n frames of every row: codes [rows, n_q, n] i32 (device) -> wav [rows, n*1920] f32 (device); any n >= 1
+ * (longer than max_chunk_frames is processed in pieces).  One row: codes [n_q, n] -> wav [n*1920]. */
 int sopro_mimi_decode_step(sopro_mimi_stream_t* s, const int32_t* codes, int n, float* wav, void* stream);
 int sopro_mimi_decode_step_host(sopro_mimi_stream_t* s, const int32_t* codes_host, int n, float* wav_host, void* stream);
 

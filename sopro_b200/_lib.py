@@ -184,9 +184,12 @@ SYMBOLS = {
     "sopro_mimi_set_graphs": (_I, [_VP, _I]),
     "sopro_mimi_check": (_I, [_VP, _VP]),
     "sopro_mimi_stream_create": (_I, [_VP, _I, C.POINTER(_VP)]),
+    "sopro_mimi_stream_create_rows": (_I, [_VP, _I, _I, C.POINTER(_VP)]),
     "sopro_mimi_stream_destroy": (_I, [_VP]),
     "sopro_mimi_stream_reset": (_I, [_VP, _VP]),
     "sopro_mimi_stream_frames": (C.c_int64, [_VP]),
+    "sopro_mimi_stream_rows": (C.c_int64, [_VP]),
+    "sopro_mimi_stream_bytes": (C.c_int64, [_VP]),
     "sopro_mimi_decode_step": (_I, [_VP, _VP, _I, _VP, _VP]),
     "sopro_mimi_decode_step_host": (_I, [_VP, _VP, _I, _VP, _VP]),
     "sopro_mimi_encoder_create": (_I, [C.POINTER(MimiConfigC), C.POINTER(MimiEncoderWeights), _I, C.POINTER(_VP)]),

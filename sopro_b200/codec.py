@@ -284,8 +284,9 @@ class MimiEngine:
         """Raises if any decode since the last check met an out-of-range code (device-side sticky flag)."""
         _lib.check(self.lib.sopro_mimi_check(self._h, int(torch.cuda.current_stream(self.device).cuda_stream)))
 
-    def stream(self, max_chunk_frames: int = 16) -> "MimiStream":
-        return MimiStream(self, max_chunk_frames)
+    def stream(self, max_chunk_frames: int = 16, rows: int = 1) -> "MimiStream":
+        """A decode state of `rows` utterances stepped side by side (see MimiStream)."""
+        return MimiStream(self, max_chunk_frames, rows)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -300,37 +301,52 @@ class MimiEngine:
 
 
 class MimiStream:
-    """Persistent decode state of one utterance on the device (K/V rings, upsampler frame, conv context rows):
-    ``step(codes [Q, n])`` returns the next n*hop samples in O(n) work.  See include/sopro_b200.h."""
+    """Persistent decode state of `rows` utterances on the device (per row: K/V rings, upsampler frame, conv context
+    rows): ``step(codes [Q, n])`` (one row) or ``step(codes [rows, Q, n])`` returns the next n*hop samples of every row
+    in O(rows * n) work.  Row b's samples equal a one-row stream fed row b's codes, bit for bit; a row whose utterance
+    has ended can be fed code 0 and its samples dropped.  See include/sopro_b200.h."""
 
-    def __init__(self, engine: MimiEngine, max_chunk_frames: int = 16):
+    def __init__(self, engine: MimiEngine, max_chunk_frames: int = 16, rows: int = 1):
         self.engine, self.lib = engine, engine.lib
         h = C.c_void_p()
-        _lib.check(self.lib.sopro_mimi_stream_create(engine._h, int(max_chunk_frames), C.byref(h)))
+        _lib.check(self.lib.sopro_mimi_stream_create_rows(engine._h, int(max_chunk_frames), int(rows), C.byref(h)))
         self._h = h
+        self.rows = int(rows)
 
     @property
     def frames(self) -> int:
         return int(self.lib.sopro_mimi_stream_frames(self._h))
 
+    @property
+    def state_bytes(self) -> int:
+        """Device bytes this state holds."""
+        return int(self.lib.sopro_mimi_stream_bytes(self._h))
+
     def reset(self) -> None:
         _lib.check(self.lib.sopro_mimi_stream_reset(self._h, int(torch.cuda.current_stream(self.engine.device).cuda_stream)))
 
     def step(self, codes_qn: torch.Tensor, trusted: bool = False) -> torch.Tensor:
+        """codes [Q, n] (a one-row state) or [rows, Q, n] -> wav [1, n*hop] or [rows, n*hop]."""
         codes = self.engine._validated(codes_qn, trusted)
-        Q, n = codes.shape
+        if codes.dim() == 2:
+            codes = codes.unsqueeze(0)
+        if codes.dim() != 3 or int(codes.shape[0]) != self.rows:
+            raise ValueError(f"a stream of {self.rows} row(s) takes codes [{self.rows}, Q, n]"
+                             + (" or [Q, n]" if self.rows == 1 else "") + f", got {tuple(codes_qn.shape)}")
+        _rows, Q, n = codes.shape
         if Q != self.engine.num_quantizers:
             raise ValueError(f"expected {self.engine.num_quantizers} codebooks, got {Q}")
-        wav = torch.empty((1, n * self.engine.hop), dtype=torch.float32, device=self.engine.device)
+        wav = torch.empty((self.rows, n * self.engine.hop), dtype=torch.float32, device=self.engine.device)
         if n:
             _lib.check(self.lib.sopro_mimi_decode_step(self._h, codes.data_ptr(), int(n), wav.data_ptr(),
                                                        int(torch.cuda.current_stream(self.engine.device).cuda_stream)))
         return wav
 
     def step_host(self, codes_qn: np.ndarray) -> np.ndarray:
-        codes = np.ascontiguousarray(codes_qn, dtype=np.int32)
-        Q, n = codes.shape
-        wav = np.empty((1, n * self.engine.hop), dtype=np.float32)
+        """Host buffers: codes [Q, n] or [rows, Q, n] -> wav [rows, n*hop]."""
+        codes = np.ascontiguousarray(codes_qn, dtype=np.int32).reshape(self.rows, self.engine.num_quantizers, -1)
+        n = codes.shape[2]
+        wav = np.empty((self.rows, n * self.engine.hop), dtype=np.float32)
         _lib.check(self.lib.sopro_mimi_decode_step_host(self._h, codes.ctypes.data, int(n), wav.ctypes.data,
                                                         int(torch.cuda.current_stream(self.engine.device).cuda_stream)))
         return wav
@@ -506,40 +522,59 @@ class MimiStreamDecoder:
     the waveform's peak from its own decode_full (measured: tests/golden/measure_stream_distance.py, DESIGN.md §5).
     Here the state carries everything a causal decoder needs (K/V rings, upsampler frame, the left context of every
     conv), so each chunk costs O(chunk) and the chunks concatenate to exactly the non-streaming waveform.
-    ``overlap_frames`` is accepted for signature compatibility; nothing is re-decoded."""
+    ``overlap_frames`` is accepted for signature compatibility; nothing is re-decoded.
+
+    A state can also hold several utterances stepped side by side (``new_state(rows)``, codes [rows, n, Q]; see
+    MimiStream).  Released states are kept for reuse by their row count, at most MAX_IDLE_STATES of them holding at
+    most MAX_IDLE_ROWS rows in all; the oldest go first."""
+
+    MAX_IDLE_STATES = 4
+    MAX_IDLE_ROWS = 256
 
     def __init__(self, codec: MimiCodec, max_chunk_frames: int = 16):
         self.codec = codec
         self.max_chunk_frames = int(max_chunk_frames)
-        self._idle: list = []  # device streams of finished utterances, reused after a reset (no allocation per stream())
+        self._idle: list = []  # device streams of finished utterances, oldest first, reused after a reset
 
-    def new_state(self) -> MimiDecodeState:
-        """A fresh state; reuses the device buffers of a released one when available."""
+    def new_state(self, rows: int = 1) -> MimiDecodeState:
+        """A fresh state of `rows` utterances; reuses the device buffers of a released one of that many rows when
+        available (no allocation on the time-to-first-audio path)."""
         st = MimiDecodeState()
-        if self._idle:
-            st.decoder_past_key_values = self._idle.pop()
-            st.decoder_past_key_values.reset()
+        for i in range(len(self._idle) - 1, -1, -1):
+            if getattr(self._idle[i], "rows", 1) == int(rows):
+                st.decoder_past_key_values = self._idle.pop(i)
+                st.decoder_past_key_values.reset()
+                break
         return st
 
     def release(self, state: Optional[MimiDecodeState]) -> None:
         """Hand a finished utterance's device buffers back for reuse."""
-        if state is not None and state.decoder_past_key_values is not None and len(self._idle) < 4:
-            self._idle.append(state.decoder_past_key_values)
-            state.decoder_past_key_values = None
+        if state is None or state.decoder_past_key_values is None:
+            return
+        dev, state.decoder_past_key_values = state.decoder_past_key_values, None
+        self._idle.append(dev)
+        while len(self._idle) > self.MAX_IDLE_STATES or sum(getattr(x, "rows", 1) for x in self._idle) > self.MAX_IDLE_ROWS:
+            old = self._idle.pop(0)
+            if hasattr(old, "close"):
+                old.close()
 
     @torch.inference_mode()
     def decode_step(self, codes_chunk_tq: torch.Tensor, state: Optional[MimiDecodeState] = None, *,
                     overlap_frames: int = 2, _trusted: bool = False) -> Tuple[torch.Tensor, MimiDecodeState]:
+        """codes [n, Q] of one utterance -> wav [1, n*hop]; or codes [rows, n, Q] of a state's rows -> wav [rows, n*hop]
+        (the state takes its row count from the first chunk it decodes)."""
         if state is None:
             state = MimiDecodeState()
-        n_new = int(codes_chunk_tq.size(0))
+        rows = 1 if codes_chunk_tq.dim() == 2 else int(codes_chunk_tq.size(0))
+        n_new = int(codes_chunk_tq.size(-2))
         if n_new == 0:
-            return torch.zeros(1, 0, device=self.codec.device), state
+            return torch.zeros(rows, 0, device=self.codec.device), state
         if state.decoder_past_key_values is None:
-            state.decoder_past_key_values = self.codec.engine.stream(self.max_chunk_frames)
+            state.decoder_past_key_values = (self.codec.engine.stream(self.max_chunk_frames) if rows == 1 else
+                                             self.codec.engine.stream(self.max_chunk_frames, rows))
         chunk = codes_chunk_tq.to(self.codec.device)
-        wav_new = state.decoder_past_key_values.step(chunk.permute(1, 0), _trusted)
+        wav_new = state.decoder_past_key_values.step(chunk.transpose(-1, -2), _trusted)
         state.frames_seen += n_new
         state.samples_emitted += int(wav_new.size(1))
-        state.tail_codes_tq = chunk[-max(int(overlap_frames), 0):].detach() if overlap_frames > 0 else None
+        state.tail_codes_tq = chunk[..., -max(int(overlap_frames), 0):, :].detach() if overlap_frames > 0 else None
         return wav_new, state

@@ -24,6 +24,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -159,16 +160,16 @@ __global__ void __launch_bounds__(256) igemm_kernel(const GemmOp op) {
   }
 }
 
-// RVQ lookup-sum: codes [B][Q][T] -> S [B][T][2*Dc] = [semantic sum | acoustic sum]
+// RVQ lookup-sum: codes [B][Q][code_T] (frames [0, T) of each row) -> S [B][T][2*Dc] = [semantic sum | acoustic sum]
 // A code outside [0, vocab) (an uncut EOS id, a negative pad) is clamped and recorded in *bad (sticky, read by
 // sopro_mimi_check): the gather never leaves the table.  The reference's embedding lookup raises IndexError there.
 __global__ void rvq_gather_kernel(const int* __restrict__ codes, const float* __restrict__ embed, float* __restrict__ S,
-                                  int Q, int T, int Dc, int vocab, int n_sem, int* __restrict__ bad) {
+                                  int Q, int T, int code_T, int Dc, int vocab, int n_sem, int* __restrict__ bad) {
   const int t = blockIdx.x, b = blockIdx.y;
   for (int c = threadIdx.x; c < Dc; c += blockDim.x) {
     float s0 = 0.f, s1 = 0.f;
     for (int q = 0; q < Q; ++q) {
-      int code = codes[((size_t)b * Q + q) * T + t];
+      int code = codes[((size_t)b * Q + q) * code_T + t];
       if (code < 0 || code >= vocab) {
         if (c == 0) atomicOr(bad, 1);
         code = min(max(code, 0), vocab - 1);
@@ -184,7 +185,7 @@ __global__ void rvq_gather_kernel(const int* __restrict__ codes, const float* __
 }
 
 // depthwise ConvTranspose k=4 s=2, causal: y[2t+r][c] = x[t][c]*w[c][r] + x[t-1][c]*w[c][r+2]
-// `prev` (streaming, B = 1): the frame before x[0] (zeros at the start of a stream), else null
+// `prev` (streaming): [B][C], each row's frame before x[0] (zeros at the start of a stream), else null
 __global__ void upsample_kernel(const float* __restrict__ x, const float* __restrict__ w, float* __restrict__ y, int T,
                                 int C, const float* __restrict__ prev) {
   const int to = blockIdx.x, b = blockIdx.y;  // output row 0..2T-1
@@ -193,7 +194,7 @@ __global__ void upsample_kernel(const float* __restrict__ x, const float* __rest
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float v = xb[(size_t)t * C + c] * __ldg(w + c * 4 + r);
     if (t > 0) v += xb[(size_t)(t - 1) * C + c] * __ldg(w + c * 4 + r + 2);
-    else if (prev) v += prev[c] * __ldg(w + c * 4 + r + 2);
+    else if (prev) v += prev[(size_t)b * C + c] * __ldg(w + c * 4 + r + 2);
     y[((size_t)b * 2 * T + to) * C + c] = v;
   }
 }
@@ -225,17 +226,18 @@ __global__ void layernorm_kernel(const float* __restrict__ x, const float* __res
   for (int c = lane; c < C; c += 32) put(y + row * C + c, (xr[c] - mean) * inv * __ldg(w + c) + __ldg(bb + c));
 }
 
-__global__ void cast_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, long long n4) {
+// n4 float4s of item blockIdx.y: x + item * x_bs -> y + item * y_bs (strides in elements, multiples of 4)
+__global__ void cast_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, long long n4, long long x_bs, long long y_bs) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n4) return;
-  const float4 v = reinterpret_cast<const float4*>(x)[i];
+  const float4 v = reinterpret_cast<const float4*>(x + blockIdx.y * x_bs)[i];
   const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-  reinterpret_cast<uint2*>(y)[i] = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+  reinterpret_cast<uint2*>(y + blockIdx.y * y_bs)[i] = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
 }
 
 // RoPE in place on the q and k thirds of QKV [rows][3C]; rope table [T2][Dh/2] cos, then sin
-// Streaming (kring != null, B = 1): row t sits at absolute position pos0 + t; its rotated key and its value are also
-// appended to the layer's K/V ring at slot (pos0 + t) % R.
+// Streaming (kring != null): row t sits at absolute position pos0 + t; its rotated key and its value are also
+// appended to item b's ring of the layer, [B][R][C], at slot (pos0 + t) % R.
 __global__ void rope_kernel(float* __restrict__ qkv, const float* __restrict__ cs, int T2, int tab_T2, int C, int H,
                             int pos0, float* __restrict__ kring, float* __restrict__ vring, int R) {
   const int t = blockIdx.x, b = blockIdx.y;
@@ -255,7 +257,7 @@ __global__ void rope_kernel(float* __restrict__ qkv, const float* __restrict__ c
   }
   if (kring) {
     __syncthreads();
-    const size_t slot = (size_t)((pos0 + t) % R) * C;
+    const size_t slot = ((size_t)b * R + (pos0 + t) % R) * C;
     for (int c4 = threadIdx.x * 4; c4 < C; c4 += blockDim.x * 4) {
       *reinterpret_cast<float4*>(kring + slot + c4) = *reinterpret_cast<const float4*>(row + C + c4);
       *reinterpret_cast<float4*>(vring + slot + c4) = *reinterpret_cast<const float4*>(row + 2 * C + c4);
@@ -307,9 +309,9 @@ __global__ void __launch_bounds__(256) rope_pack_kernel(const float* __restrict_
 }
 
 // causal sliding-window attention, one warp per (b, h, query); QKV rotated; out [B][T2][C]
-// Streaming (kring != null, B = 1): query row i sits at absolute position pos0 + i and the keys / values of positions
-// [pos - window + 1, pos] are read from the layer's ring (slot = position % R); the arithmetic and its order are the
-// full decode's, so a chunked decode equals the full decode's prefix bit for bit in fp32 mode.
+// Streaming (kring != null): query row i sits at absolute position pos0 + i and the keys / values of positions
+// [pos - window + 1, pos] are read from item b's ring of the layer (slot = position % R); the arithmetic and its order
+// are the full decode's, so a chunked decode equals the full decode's prefix bit for bit in fp32 mode.
 template <typename OutT>
 __global__ void __launch_bounds__(256) attn_kernel(const float* __restrict__ qkv, OutT* __restrict__ out, int T2, int C,
                                                    int H, int window, int pos0, const float* __restrict__ kring,
@@ -323,6 +325,10 @@ __global__ void __launch_bounds__(256) attn_kernel(const float* __restrict__ qkv
   if (i >= T2) return;
   const float* base = qkv + (size_t)b * T2 * 3 * C;
   const float* q = base + (size_t)i * 3 * C + h * Dh;
+  // keys / values of position p: row p % R of item b's ring (streaming), else row p of the QKV rows
+  const float* kb = kring ? kring + (size_t)b * R * C + h * Dh : base + C + h * Dh;
+  const float* vb = vring ? vring + (size_t)b * R * C + h * Dh : base + 2 * C + h * Dh;
+  const int kv_ld = kring ? C : 3 * C, kv_mod = kring ? R : INT_MAX;
   for (int d = lane; d < Dh; d += 32) qs[d] = q[d];
   __syncwarp();
   const int ia = pos0 + i;  // absolute position
@@ -331,7 +337,7 @@ __global__ void __launch_bounds__(256) attn_kernel(const float* __restrict__ qkv
   const float scale = 1.0f / sqrtf((float)Dh);
   float mx = -INFINITY;
   for (int jj = lane; jj < nk; jj += 32) {
-    const float* kr = kring ? kring + (size_t)((j0 + jj) % R) * C + h * Dh : base + (size_t)(j0 + jj) * 3 * C + C + h * Dh;
+    const float* kr = kb + (size_t)((j0 + jj) % kv_mod) * kv_ld;
     float s = 0.f;
     for (int d = 0; d < Dh; d += 4) {
       const float4 kk = *reinterpret_cast<const float4*>(kr + d);
@@ -355,24 +361,20 @@ __global__ void __launch_bounds__(256) attn_kernel(const float* __restrict__ qkv
   const float inv = 1.0f / sum;
   for (int d = lane; d < Dh; d += 32) {
     float o = 0.f;
-    if (vring) {
-      for (int jj = 0; jj < nk; ++jj) o += (sc[jj] * inv) * vring[(size_t)((j0 + jj) % R) * C + h * Dh + d];
-    } else {
-      for (int jj = 0; jj < nk; ++jj) o += (sc[jj] * inv) * base[(size_t)(j0 + jj) * 3 * C + 2 * C + h * Dh + d];
-    }
+    for (int jj = 0; jj < nk; ++jj) o += (sc[jj] * inv) * vb[(size_t)((j0 + jj) % kv_mod) * kv_ld + d];
     put(out + ((size_t)b * T2 + i) * C + h * Dh + d, o);
   }
 }
 
 // final conv: ELU -> causal conv k taps, Cin -> 1
 // rows r >= lo are readable (lo = 0: the causal zero pad; streaming: lo = -(taps-1), the carried context rows sit in
-// front of x)
+// front of x); item b of x starts at x + b * x_bs, its output at y + b * y_bs
 __global__ void final_conv_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
-                                  float* __restrict__ y, long long Tn, int Cin, int taps, int lo) {
+                                  float* __restrict__ y, long long Tn, int Cin, int taps, int lo, long long x_bs, long long y_bs) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (t >= Tn) return;
-  const float* xb = x + (size_t)b * Tn * Cin;
+  const float* xb = x + (size_t)b * x_bs;
   float acc = __ldg(bias);
   for (int j = 0; j < taps; ++j) {
     const long long r = t + j - (taps - 1);
@@ -384,7 +386,7 @@ __global__ void final_conv_kernel(const float* __restrict__ x, const float* __re
       acc += elu1(v.x) * ww.x + elu1(v.y) * ww.y + elu1(v.z) * ww.z + elu1(v.w) * ww.w;
     }
   }
-  y[(size_t)b * Tn + t] = acc;
+  y[(size_t)b * y_bs + t] = acc;
 }
 
 // final conv on the bf16 activation [B][Tn][Cin] that already went through ELU (tensor-core mode): one thread per
@@ -392,7 +394,7 @@ __global__ void final_conv_kernel(const float* __restrict__ x, const float* __re
 // through shared memory.  256 - (taps-1) outputs per block.
 __global__ void __launch_bounds__(256) final_conv_h_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w,
                                                            const float* __restrict__ bias, float* __restrict__ y, long long Tn,
-                                                           int Cin, int taps, int lo) {
+                                                           int Cin, int taps, int lo, long long x_bs, long long y_bs) {
   extern __shared__ float fsm[];  // [taps][256] partial dots, then [taps*Cin] weights
   float* sp = fsm;
   float* sw = fsm + taps * 256;
@@ -404,7 +406,7 @@ __global__ void __launch_bounds__(256) final_conv_h_kernel(const __nv_bfloat16* 
 #pragma unroll
   for (int j = 0; j < 8; ++j) acc[j] = 0.f;
   if (r >= lo && r < Tn) {
-    const uint4* xr = reinterpret_cast<const uint4*>(x + ((long long)b * Tn + r) * Cin);
+    const uint4* xr = reinterpret_cast<const uint4*>(x + (long long)b * x_bs + r * Cin);
     for (int c = 0; c < Cin; c += 8) {
       const uint4 v = xr[c >> 3];
       const uint32_t u[4] = {v.x, v.y, v.z, v.w};
@@ -430,7 +432,7 @@ __global__ void __launch_bounds__(256) final_conv_h_kernel(const __nv_bfloat16* 
   if (tid >= halo && r < Tn) {  // output sample r: tap j reads row r + j - halo
     float o = __ldg(bias);
     for (int j = 0; j < taps; ++j) o += sp[j * 256 + tid - halo + j];
-    y[(size_t)b * Tn + r] = o;
+    y[(size_t)b * y_bs + r] = o;
   }
 }
 
@@ -761,33 +763,38 @@ int launch_gemm(const GemmOp& op, int B, cudaStream_t st) {
   return SOPRO_OK;
 }
 
-// A channel-last GEMM operand: B items of [ctx + M] rows each.  The first ctx rows of an item are left context (the
-// rows a stream carried over from its previous chunk); with ctx = 0 the causal zero padding stands in for them.
+// A channel-last GEMM operand: B items of [ctx + M] rows each, item b at p + b * pitch rows (pitch 0: ctx + M, the
+// items back to back).  The first ctx rows of an item are left context (the rows a stream carried over from its
+// previous chunk); with ctx = 0 the causal zero padding stands in for them.
 struct Operand {
   const void* p;  // first context row of item 0
   long long M;
   int ctx, B;
+  long long pitch;
+  long long rows_per_item() const { return pitch > 0 ? pitch : M + ctx; }
 };
 
 // fp32 implicit GEMM (a causal conv of `taps` taps; a Linear with taps = 1) over an operand of cin channels:
-// pad = taps - 1 - ctx zero rows, Min = M + ctx readable rows.  elu: ELU on the operand load.
+// pad = taps - 1 - ctx zero rows, Min = M + ctx readable rows.  elu: ELU on the operand load.  Item b of the output
+// (and of R) starts c_pitch (r_pitch) rows of N after item b - 1 (0: M rows).
 int gemm_f32(const Operand& a, int cin, int taps, const float* W, const float* bias, int N, int bias_mod, int epi, const float* R,
-             const float* scale, float* out, int elu, cudaStream_t st) {
+             const float* scale, float* out, int elu, cudaStream_t st, long long c_pitch = 0, long long r_pitch = 0) {
   GemmOp g{};
   g.A = static_cast<const float*>(a.p); g.W = W; g.C = out; g.R = R; g.bias = bias; g.scale = scale;
   g.M = (int)a.M; g.N = N; g.K = taps * cin; g.Min = (int)(a.M + a.ctx); g.Cin = cin; g.taps = taps; g.dil = 1; g.pad = taps - 1 - a.ctx;
   g.ldc = N; g.bias_mod = bias_mod; g.epi = epi; g.a_elu = elu;
-  g.a_bs = (a.M + a.ctx) * cin; g.c_bs = a.M * N; g.r_bs = a.M * N;
+  g.a_bs = a.rows_per_item() * cin; g.c_bs = (c_pitch > 0 ? c_pitch : a.M) * N; g.r_bs = (r_pitch > 0 ? r_pitch : a.M) * N;
   return launch_gemm(g, a.B, st);
 }
 
 // tensor-core implicit GEMM over a bf16 operand (ELU already applied by its producer where the layer wants it), same
-// operand geometry; fp32 and / or bf16 output, the bf16 copy through ELU when out_elu
+// operand geometry; fp32 and / or bf16 output (the same pitch), the bf16 copy through ELU when out_elu
 int gemm_tc(const Operand& a, int cin, int taps, const __nv_bfloat16* W, const float* bias, int N, int bias_mod, int epi, const float* R,
-            const float* scale, float* of, __nv_bfloat16* oh, int out_elu, cudaStream_t st) {
+            const float* scale, float* of, __nv_bfloat16* oh, int out_elu, cudaStream_t st, long long c_pitch = 0, long long r_pitch = 0) {
   tc::TcOp o{};
   o.bias = bias; o.R = R; o.scale = scale; o.out_f32 = of; o.out_bf16 = oh;
-  o.c_bs = a.M * N; o.M = (int)a.M; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = 1; o.pad = taps - 1 - a.ctx;
+  o.c_bs = (c_pitch > 0 ? c_pitch : a.M) * N; o.r_bs = (r_pitch > 0 ? r_pitch : a.M) * N; o.a_pitch = a.rows_per_item();
+  o.M = (int)a.M; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = 1; o.pad = taps - 1 - a.ctx;
   o.bias_mod = bias_mod; o.epi = epi; o.out_elu = out_elu;
   cudaError_t e = tc::launch(a.p, a.M + a.ctx, W, o, a.B, st);
   if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "tensor-core GEMM (N=%d K=%d): %s", N, o.K, cudaGetErrorString(e));
@@ -805,8 +812,8 @@ struct LayerBufs {
   __nv_bfloat16 *k, *vt;  // [rows][C], [B][C][T2 rounded up to 8]
 };
 
-// A stream's K/V rings: layer l holds the rotated key / the value of position p in row p % R of k / v + l*R*C;
-// row 0 of the chunk is position pos0
+// A stream's K/V rings [n_layers][B][R][C]: item b of layer l holds the rotated key / the value of position p in row
+// p % R of k / v + (l*B + b)*R*C; row 0 of the chunk is position pos0
 struct KVRing {
   float *k, *v;
   int R, pos0;
@@ -852,8 +859,8 @@ int run_layers(const sopro_mimi_config_t& c, const std::vector<sopro_mimi::Layer
           if (ae != cudaSuccess) return fail(SOPRO_ERR_CUDA, "tensor-core attention: %s", cudaGetErrorString(ae));
         }
       } else {
-        float* kr = ring ? ring->k + li * (size_t)R * C : nullptr;
-        float* vr = ring ? ring->v + li * (size_t)R * C : nullptr;
+        float* kr = ring ? ring->k + li * (size_t)B * R * C : nullptr;
+        float* vr = ring ? ring->v + li * (size_t)B * R * C : nullptr;
         rope_kernel<<<dim3(T2, B), 256, 0, st>>>(b.qkv, rope, T2, rope_T2, C, H, pos0, kr, vr, R);
         attn_kernel<<<dim3((T2 + 7) / 8, H, B), 256, asm_bytes, st>>>(b.qkv, att, T2, C, H, c.window, pos0, kr, vr, R);
         CK(cudaGetLastError());
@@ -872,23 +879,26 @@ int run_layers(const sopro_mimi_config_t& c, const std::vector<sopro_mimi::Layer
 
 }  // namespace
 
-// Context rows a stream moves to the front of its conv operand buffers after a step (the parameter of
-// tail_shift_kernel, so outside the anonymous namespace)
+// Context rows a stream moves to the front of each row's slice of its conv operand buffers after a step (the
+// parameter of tail_shift_kernel, so outside the anonymous namespace)
 struct TailShift {
   void* base[16];
+  long long pitch_bytes[16];             // one stream row's slice of the buffer
   int row_bytes[16], ctx[16], rows[16];  // rows = new rows written behind the ctx rows this step
   int n;
 };
 
 namespace {
 
-// A SEANet activation buffer: `ctx` rows of left context in front of the rows a pass writes
+// A SEANet activation buffer: `ctx` rows of left context in front of the rows a pass writes, item b at p + b * pitch
+// rows (pitch 0: ctx + the pass's rows, the items back to back)
 struct Buf {
   void* p;
   int ctx;
+  long long pitch;
   template <typename T>
-  T* rows(int cols) const { return static_cast<T*>(p) + (size_t)ctx * cols; }  // the first row a pass writes
-  Operand operand(long long M, int B) const { return {p, M, ctx, B}; }
+  T* rows(int cols) const { return static_cast<T*>(p) + (size_t)ctx * cols; }  // the first row item 0's pass writes
+  Operand operand(long long M, int B) const { return {p, M, ctx, B, pitch}; }
 };
 
 // Buffers of one SEANet decoder pass.  fp32 mode: every buffer is fp32 and `h` holds the raw ResnetBlock hidden.
@@ -907,6 +917,7 @@ struct SeanetBufs {
 void carry(TailShift* ts, const Buf& b, int row_bytes, long long rows) {
   if (!ts) return;
   ts->base[ts->n] = b.p;
+  ts->pitch_bytes[ts->n] = b.pitch * row_bytes;
   ts->row_bytes[ts->n] = row_bytes;
   ts->ctx[ts->n] = b.ctx;
   ts->rows[ts->n] = (int)rows;
@@ -916,13 +927,13 @@ void carry(TailShift* ts, const Buf& b, int row_bytes, long long rows) {
 // SEANet decoder in fp32: conv0, per stage ELU -> ConvTranspose (stride r, kernel 2r: a 2-tap GEMM with r*Cout columns)
 // and the ResnetBlock z + conv1(ELU(conv3(ELU(z)))), then ELU -> final conv into wav [B][T2 * prod(ratios)].  The
 // tail shift of every buffer that holds a conv operand is recorded in *ts when ts is given.
-int seanet_f32(const sopro_mimi* m, const SeanetBufs& b, int B, long long T2, TailShift* ts, float* wav, cudaStream_t st) {
+int seanet_f32(const sopro_mimi* m, const SeanetBufs& b, int B, long long T2, TailShift* ts, float* wav, long long wav_pitch, cudaStream_t st) {
   const sopro_mimi_config_t& c = m->cfg;
   const float* Wd = m->dev;
   long long Tn = T2;
   int ch = c.num_filters << c.n_ratios, rc;
   if ((rc = gemm_f32(b.in.operand(Tn, B), c.hidden, c.kernel, Wd + m->c0w, Wd + m->c0b, ch, ch, EPI_NONE, nullptr, nullptr,
-                     b.a0.rows<float>(ch), 0, st)))
+                     b.a0.rows<float>(ch), 0, st, b.a0.pitch)))
     return rc;
   carry(ts, b.in, c.hidden * 4, Tn);
   carry(ts, b.a0, ch * 4, Tn);
@@ -931,15 +942,17 @@ int seanet_f32(const sopro_mimi* m, const SeanetBufs& b, int B, long long T2, Ta
     const sopro_mimi::Stage& S = m->stages[si];
     const SeanetBufs::Stage& sb = b.stage[si];
     const int hid = S.cout / c.compress;
+    // the ConvTranspose's S.ratio output rows of an input row are its S.ratio * S.cout columns: the output pitch in
+    // input rows is z's pitch / S.ratio (stream layouts keep it whole)
     if ((rc = gemm_f32(cur.operand(Tn, B), S.cin, 2, Wd + S.tw, Wd + S.tb, S.ratio * S.cout, S.cout, EPI_NONE, nullptr, nullptr,
-                       sb.z.rows<float>(S.cout), 1, st)))
+                       sb.z.rows<float>(S.cout), 1, st, sb.z.pitch / S.ratio)))
       return rc;
     Tn *= S.ratio;
     if ((rc = gemm_f32(sb.z.operand(Tn, B), S.cout, c.res_kernel, Wd + S.r1w, Wd + S.r1b, hid, hid, EPI_NONE, nullptr, nullptr,
-                       sb.h.rows<float>(hid), 1, st)))
+                       sb.h.rows<float>(hid), 1, st, sb.h.pitch)))
       return rc;
     if ((rc = gemm_f32(sb.h.operand(Tn, B), hid, 1, Wd + S.r2w, Wd + S.r2b, S.cout, S.cout, EPI_RES, sb.z.rows<float>(S.cout), nullptr,
-                       sb.o.rows<float>(S.cout), 1, st)))
+                       sb.o.rows<float>(S.cout), 1, st, sb.o.pitch, sb.z.pitch)))
       return rc;
     carry(ts, sb.z, S.cout * 4, Tn);
     carry(ts, sb.o, S.cout * 4, Tn);
@@ -947,7 +960,8 @@ int seanet_f32(const sopro_mimi* m, const SeanetBufs& b, int B, long long T2, Ta
     ch = S.cout;
   }
   final_conv_kernel<<<dim3((unsigned)((Tn + 255) / 256), B), 256, 0, st>>>(cur.rows<float>(ch), Wd + m->lw, Wd + m->lb, wav, Tn, ch,
-                                                                            c.last_kernel, -cur.ctx);
+                                                                            c.last_kernel, -cur.ctx, cur.operand(Tn, B).rows_per_item() * ch,
+                                                                            wav_pitch > 0 ? wav_pitch : Tn);
   CK(cudaGetLastError());
   return SOPRO_OK;
 }
@@ -955,18 +969,20 @@ int seanet_f32(const sopro_mimi* m, const SeanetBufs& b, int B, long long T2, Ta
 // SEANet decoder in tensor-core mode (check_tc_geometry passed), from the fp32 residual stream x [B][T2][C].
 // Activations that feed a contraction travel as bf16 with the consumer's ELU already applied; the ResnetBlock skip
 // stays fp32.  A ResnetBlock runs in one launch when the fused kernel takes its geometry, else conv by conv.
-int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, long long T2, TailShift* ts, float* wav, cudaStream_t st) {
+int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, long long T2, TailShift* ts, float* wav, long long wav_pitch,
+              cudaStream_t st) {
   const sopro_mimi_config_t& c = m->cfg;
   const int C = c.hidden;
   const float* Wd = m->dev;
   const __nv_bfloat16* Wh = m->dev_h;
   long long Tn = T2;
   int ch = c.num_filters << c.n_ratios, rc;
-  const long long n4 = (long long)B * T2 * C / 4;
-  cast_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(x, b.in.rows<__nv_bfloat16>(C), n4);
+  const long long n4 = T2 * C / 4;  // x [B][T2][C] packed -> each item's rows of `in`
+  cast_bf16_kernel<<<dim3((unsigned)((n4 + 255) / 256), B), 256, 0, st>>>(x, b.in.rows<__nv_bfloat16>(C), n4, T2 * C,
+                                                                          b.in.operand(Tn, B).rows_per_item() * C);
   CK(cudaGetLastError());
   if ((rc = gemm_tc(b.in.operand(Tn, B), C, c.kernel, Wh + m->c0w_h, Wd + m->c0b, ch, ch, tc::EPI_NONE, nullptr, nullptr, nullptr,
-                    b.a0.rows<__nv_bfloat16>(ch), 1, st)))
+                    b.a0.rows<__nv_bfloat16>(ch), 1, st, b.a0.pitch)))
     return rc;
   carry(ts, b.in, C * 2, Tn);
   carry(ts, b.a0, ch * 2, Tn);
@@ -976,8 +992,9 @@ int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, l
     const SeanetBufs::Stage& sb = b.stage[si];
     const int hid = S.cout / c.compress;
     // ELU -> ConvTranspose: fp32 skip zf, bf16 ELU(z) for the ResnetBlock
+    // (zf, which has no context rows, is laid out with z's pitch: one GEMM writes both)
     if ((rc = gemm_tc(cur.operand(Tn, B), S.cin, 2, Wh + S.tw_h, Wd + S.tb, S.ratio * S.cout, S.cout, tc::EPI_NONE, nullptr, nullptr,
-                      sb.zf, sb.z.rows<__nv_bfloat16>(S.cout), 1, st)))
+                      sb.zf, sb.z.rows<__nv_bfloat16>(S.cout), 1, st, sb.z.pitch / S.ratio)))
       return rc;
     Tn *= S.ratio;
     if (tc::resblock_supported(hid, S.cout) && (S.cout * c.res_kernel) % 64 == 0) {
@@ -991,14 +1008,17 @@ int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, l
       ro.taps = c.res_kernel;
       ro.pad = c.res_kernel - 1 - sb.z.ctx;
       ro.out_elu = 1;
+      ro.a_pitch = sb.z.pitch;
+      ro.z_bs = sb.z.pitch * S.cout;
+      ro.o_bs = sb.o.pitch * S.cout;
       cudaError_t fe = tc::launch_resblock(sb.z.p, Wh + S.r1w_h, Wh + S.r2w_h, hid, ro, B, st);
       if (fe != cudaSuccess) return fail(SOPRO_ERR_CUDA, "fused ResnetBlock (stage %zu): %s", si, cudaGetErrorString(fe));
     } else {  // conv k=3 -> ELU(h) bf16, then the 1x1 conv + fp32 skip
       if ((rc = gemm_tc(sb.z.operand(Tn, B), S.cout, c.res_kernel, Wh + S.r1w_h, Wd + S.r1b, hid, hid, tc::EPI_NONE, nullptr, nullptr,
-                        nullptr, sb.h.rows<__nv_bfloat16>(hid), 1, st)))
+                        nullptr, sb.h.rows<__nv_bfloat16>(hid), 1, st, sb.h.pitch)))
         return rc;
       if ((rc = gemm_tc(sb.h.operand(Tn, B), hid, 1, Wh + S.r2w_h, Wd + S.r2b, S.cout, S.cout, tc::EPI_RES, sb.zf, nullptr, nullptr,
-                        sb.o.rows<__nv_bfloat16>(S.cout), 1, st)))
+                        sb.o.rows<__nv_bfloat16>(S.cout), 1, st, sb.o.pitch, sb.z.pitch)))
         return rc;
     }
     carry(ts, sb.z, S.cout * 2, Tn);
@@ -1008,7 +1028,8 @@ int seanet_tc(const sopro_mimi* m, const float* x, const SeanetBufs& b, int B, l
   }
   const int per = 256 - (c.last_kernel - 1);
   final_conv_h_kernel<<<dim3((unsigned)((Tn + per - 1) / per), B), 256, (size_t)(c.last_kernel * 256 + c.last_kernel * ch) * 4, st>>>(
-      cur.rows<__nv_bfloat16>(ch), Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, -cur.ctx);
+      cur.rows<__nv_bfloat16>(ch), Wd + m->lw, Wd + m->lb, wav, Tn, ch, c.last_kernel, -cur.ctx, cur.operand(Tn, B).rows_per_item() * ch,
+      wav_pitch > 0 ? wav_pitch : Tn);
   CK(cudaGetLastError());
   return SOPRO_OK;
 }
@@ -1037,7 +1058,7 @@ int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, 
   __nv_bfloat16* h1 = h0 + bufsz;
   __nv_bfloat16* h2 = h1 + bufsz;
   // ---- RVQ + projection + upsample (small; fp32 in both modes)
-  rvq_gather_kernel<<<dim3(T, B), 256, 0, st>>>(codes, Wd + m->embed, b0, c.n_q, T, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
+  rvq_gather_kernel<<<dim3(T, B), 256, 0, st>>>(codes, Wd + m->embed, b0, c.n_q, T, T, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
   CK(cudaGetLastError());
   int rc;
   if ((rc = gemm_f32({b0, T, 0, B}, C, 1, Wd + m->rvq_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, b1, 0, st))) return rc;
@@ -1056,11 +1077,11 @@ int mimi_enqueue(sopro_mimi* m, const int32_t* codes, int B, int T, float* wav, 
   // ---- SEANet decoder over ping-pong buffers, no context rows.  fp32: x -> b0, per stage b0 -> b1 -> b2 -> b0.
   //      Tensor-core: bf16 copy of x in h2 -> h0, per stage h0 -> h1 (+ fp32 skip b1) -> [h2] -> h0
   SeanetBufs sb{};
-  sb.in = {use_tc ? (void*)h2 : x, 0};
-  sb.a0 = {use_tc ? (void*)h0 : b0, 0};
+  sb.in = {use_tc ? (void*)h2 : x, 0, 0};
+  sb.a0 = {use_tc ? (void*)h0 : b0, 0, 0};
   for (int i = 0; i < c.n_ratios; ++i)
-    sb.stage[i] = use_tc ? SeanetBufs::Stage{{h1, 0}, {h2, 0}, {h0, 0}, b1} : SeanetBufs::Stage{{b1, 0}, {b2, 0}, {b0, 0}, nullptr};
-  return use_tc ? seanet_tc(m, x, sb, B, T2, nullptr, wav, st) : seanet_f32(m, sb, B, T2, nullptr, wav, st);
+    sb.stage[i] = use_tc ? SeanetBufs::Stage{{h1, 0, 0}, {h2, 0, 0}, {h0, 0, 0}, b1} : SeanetBufs::Stage{{b1, 0, 0}, {b2, 0, 0}, {b0, 0, 0}, nullptr};
+  return use_tc ? seanet_tc(m, x, sb, B, T2, nullptr, wav, 0, st) : seanet_f32(m, sb, B, T2, nullptr, wav, 0, st);
 }
 }  // namespace
 
@@ -1127,33 +1148,37 @@ int sopro_mimi_decode(sopro_mimi_t* m, const int32_t* codes, int B, int T, float
 // computes each output element in the same order as the full decode: in fp32 mode the chunks are bit-identical to the
 // full decode's prefix.  Work per chunk is O(chunk), not O(prefix).
 // ---------------------------------------------------------------------------------------------
-// one block per buffer: rows [rows, rows + ctx) -> [0, ctx) (through shared memory: the ranges may overlap)
+// one block per (buffer, stream row): rows [rows, rows + ctx) -> [0, ctx) of the row's slice (through shared memory:
+// the ranges may overlap)
 __global__ void __launch_bounds__(256) tail_shift_kernel(const TailShift ts) {
   extern __shared__ uint4 tsm[];
   const int i = blockIdx.x;
   const int n16 = ts.ctx[i] * ts.row_bytes[i] / 16;
-  const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(ts.base[i]) + (size_t)ts.rows[i] * ts.row_bytes[i]);
-  uint4* dst = reinterpret_cast<uint4*>(ts.base[i]);
+  unsigned char* base = reinterpret_cast<unsigned char*>(ts.base[i]) + (size_t)blockIdx.y * (size_t)ts.pitch_bytes[i];
+  const uint4* src = reinterpret_cast<const uint4*>(base + (size_t)ts.rows[i] * ts.row_bytes[i]);
+  uint4* dst = reinterpret_cast<uint4*>(base);
   for (int e = threadIdx.x; e < n16; e += blockDim.x) tsm[e] = src[e];
   __syncthreads();
   for (int e = threadIdx.x; e < n16; e += blockDim.x) dst[e] = tsm[e];
 }
 
+// `rows` utterances decoded side by side, frame count shared.  Every per-utterance buffer is [rows][pitch][...] with a
+// pitch fixed at create time, so a stream row's state never moves and every kernel reads and writes only its own row.
 struct sopro_mimi_stream {
   sopro_mimi* m = nullptr;
-  int max_n = 0, precision = 0, R = 0;
+  int max_n = 0, precision = 0, R = 0, rows = 1;
   long long frames = 0;
   unsigned char* slab = nullptr;
   size_t slab_bytes = 0, state_bytes = 0;
   // ---- state (zeroed by reset): [up_prev | K rings | V rings | conv-context rows at the front of the buffers below]
-  float* up_prev = nullptr;
-  float *kring = nullptr, *vring = nullptr;  // [n_layers][R][C]
+  float* up_prev = nullptr;                  // [rows][C]
+  float *kring = nullptr, *vring = nullptr;  // [n_layers][rows][R][C]
   // ---- chunk buffers
-  float *S = nullptr, *E = nullptr, *XC = nullptr;  // XC: [conv0 context | residual stream of the chunk]
+  float *S = nullptr, *E = nullptr, *X = nullptr;  // [rows][n][2Dc], [rows][n][C], residual stream [rows][2n][C]
   LayerBufs tr{};  // transformer scratch (ln, att, hid: bf16 views in tensor-core mode)
-  // SEANet buffers, each conv operand [taps-1 context rows | Tn rows] (fp32 raw | bf16 ELU'd): in [2 + T2][C],
-  // a0 [1 + T2][16F], z [2 + Tn][cout], o [ctx + Tn][cout] with ctx = 1 (next ConvTranspose) or taps-1 (final conv);
-  // h [Tn][cout/2] and zf [Tn][cout] (tensor-core mode) have no context
+  // SEANet buffers, each conv operand [rows][taps-1 context rows | Tn rows] (fp32 raw | bf16 ELU'd): in [2 + T2][C]
+  // (a copy of X), a0 [1 + T2][16F], z [2 + Tn][cout], o [ctx + Tn][cout] with ctx = 1 (next ConvTranspose) or taps-1
+  // (final conv); h [Tn][cout/2] has no context, zf [Tn][cout] (tensor-core mode) none either but z's pitch
   SeanetBufs sea{};
   int* codes_dev = nullptr;
   float* wav_dev = nullptr;
@@ -1173,26 +1198,30 @@ struct SlabPlan {
 void stream_layout(sopro_mimi_stream* s, unsigned char* base) {
   const sopro_mimi_config_t& c = s->m->cfg;
   const bool tcm = s->precision == SOPRO_MIMI_BF16_TC;
-  const size_t C = c.hidden, FF = c.ffn, n = s->max_n, T2 = 2 * n, NL = c.n_layers;
+  const size_t C = c.hidden, FF = c.ffn, n = s->max_n, T2 = 2 * n, NL = c.n_layers, rows = s->rows;
   const size_t es = tcm ? 2 : 4;  // element size of the conv operands
   SlabPlan P;
   auto at = [&](size_t o) { return base ? base + o : nullptr; };
+  // a buffer of `ctx` context rows and up to Tn chunk rows per stream row, the pitch a multiple of `unit` rows
+  auto buf = [&](int ctx, size_t Tn, size_t cols, size_t esz, size_t unit) -> Buf {
+    const size_t pitch = (ctx + Tn + unit - 1) / unit * unit;
+    return {at(P.take(rows * pitch * cols * esz)), ctx, (long long)pitch};
+  };
   // state first
-  s->up_prev = (float*)at(P.take(C * 4));
-  s->kring = (float*)at(P.take(NL * s->R * C * 4));
-  s->vring = (float*)at(P.take(NL * s->R * C * 4));
-  // conv operand buffers: the context rows at their fronts are state too, so they come next
-  const int k0 = c.kernel - 1;
-  s->XC = (float*)at(P.take((k0 + T2) * C * 4));
-  s->sea.in = {tcm ? at(P.take((k0 + T2) * C * 2)) : (void*)s->XC, k0};
+  s->up_prev = (float*)at(P.take(rows * C * 4));
+  s->kring = (float*)at(P.take(NL * rows * s->R * C * 4));
+  s->vring = (float*)at(P.take(NL * rows * s->R * C * 4));
+  // conv operand buffers: the context rows at their fronts are state too, so they come next.  A ConvTranspose output's
+  // pitch is a whole number of its input rows (the GEMM writes ratio rows per input row).
+  s->sea.in = buf(c.kernel - 1, T2, C, es, 1);
   size_t ch = (size_t)c.num_filters << c.n_ratios, Tn = T2;
-  s->sea.a0 = {at(P.take((1 + Tn) * ch * es)), 1};
+  s->sea.a0 = buf(1, Tn, ch, es, 1);
   for (int i = 0; i < c.n_ratios; ++i) {
     const size_t cout = ch / 2;
     Tn *= c.ratios[i];
     const int ctx_o = i + 1 == c.n_ratios ? c.last_kernel - 1 : 1;
-    s->sea.stage[i].z = {at(P.take((c.res_kernel - 1 + Tn) * cout * es)), c.res_kernel - 1};
-    s->sea.stage[i].o = {at(P.take((ctx_o + Tn) * cout * es)), ctx_o};
+    s->sea.stage[i].z = buf(c.res_kernel - 1, Tn, cout, es, c.ratios[i]);
+    s->sea.stage[i].o = buf(ctx_o, Tn, cout, es, 1);
     ch = cout;
   }
   s->state_bytes = P.off;  // everything up to here is zeroed by reset (a superset of the state proper)
@@ -1201,43 +1230,52 @@ void stream_layout(sopro_mimi_stream* s, unsigned char* base) {
   for (int i = 0; i < c.n_ratios; ++i) {
     const size_t cout = ch / 2;
     Tn *= c.ratios[i];
-    s->sea.stage[i].zf = tcm ? (float*)at(P.take(Tn * cout * 4)) : nullptr;
-    s->sea.stage[i].h = {at(P.take(Tn * (cout / c.compress) * 4)), 0};  // fp32 mode: fp32; tensor-core mode: bf16 (unfused blocks)
+    const size_t zp = s->sea.stage[i].z.pitch;
+    s->sea.stage[i].zf = tcm ? (float*)at(P.take(rows * zp * cout * 4)) : nullptr;
+    s->sea.stage[i].h = buf(0, Tn, cout / c.compress, 4, 1);  // fp32 mode: fp32; tensor-core mode: bf16 (unfused blocks)
     ch = cout;
   }
-  s->S = (float*)at(P.take(n * C * 4));
-  s->E = (float*)at(P.take(n * C * 4));
-  s->tr.ln = at(P.take(T2 * C * 4));
-  s->tr.qkv = (float*)at(P.take(T2 * 3 * C * 4));
-  s->tr.att = at(P.take(T2 * C * 4));
-  s->tr.hid = at(P.take(T2 * FF * 4));
+  s->S = (float*)at(P.take(rows * n * C * 4));
+  s->E = (float*)at(P.take(rows * n * C * 4));
+  s->X = (float*)at(P.take(rows * T2 * C * 4));
+  s->tr.ln = at(P.take(rows * T2 * C * 4));
+  s->tr.qkv = (float*)at(P.take(rows * T2 * 3 * C * 4));
+  s->tr.att = at(P.take(rows * T2 * C * 4));
+  s->tr.hid = at(P.take(rows * T2 * FF * 4));
   s->slab_bytes = P.off;
 }
 
-int stream_step(sopro_mimi_stream* s, const int32_t* codes, int n, int code_stride, float* wav, cudaStream_t st) {
+// n <= max_n frames of every row: codes [rows][n_q][code_T], frames [0, n) -> wav [rows][wav_pitch], samples [0, n*hop)
+int stream_step(sopro_mimi_stream* s, const int32_t* codes, int n, int code_T, float* wav, long long wav_pitch, cudaStream_t st) {
   sopro_mimi* m = s->m;
   const sopro_mimi_config_t& c = m->cfg;
-  const int C = c.hidden, T2 = 2 * n;
+  const int C = c.hidden, T2 = 2 * n, B = s->rows;
   const float* Wd = m->dev;
   const bool tcm = s->precision == SOPRO_MIMI_BF16_TC;
   const int pos0 = (int)(2 * s->frames);
   int rc = ensure_rope(m, std::max(4096, 2 * (pos0 + T2)), st);
   if (rc) return rc;
-  // ---- RVQ + projection + upsample
-  rvq_gather_kernel<<<dim3(n, 1), 256, 0, st>>>(codes, Wd + m->embed, s->S, c.n_q, code_stride, c.codebook_dim, c.vocab, c.n_sem, m->bad_code);
+  // ---- RVQ + projection + upsample; each row's last frame is the next step's upsampler context
+  rvq_gather_kernel<<<dim3(n, B), 256, 0, st>>>(codes, Wd + m->embed, s->S, c.n_q, n, code_T, c.codebook_dim, c.vocab, c.n_sem,
+                                                m->bad_code);
   CK(cudaGetLastError());
-  if ((rc = gemm_f32({s->S, n, 0, 1}, C, 1, Wd + m->rvq_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, s->E, 0, st))) return rc;
-  float* x = s->XC + (size_t)(c.kernel - 1) * C;  // residual stream: the rows behind conv0's context rows
-  upsample_kernel<<<dim3(T2, 1), 256, 0, st>>>(s->E, Wd + m->up_w, x, n, C, s->up_prev);
+  if ((rc = gemm_f32({s->S, n, 0, B, 0}, C, 1, Wd + m->rvq_w, nullptr, C, C, EPI_NONE, nullptr, nullptr, s->E, 0, st))) return rc;
+  upsample_kernel<<<dim3(T2, B), 256, 0, st>>>(s->E, Wd + m->up_w, s->X, n, C, s->up_prev);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(s->up_prev, s->E + (size_t)(n - 1) * C, (size_t)C * 4, cudaMemcpyDeviceToDevice, st));
-  // ---- transformer: K/V of the new positions go to the rings, queries attend over the ring
+  CK(cudaMemcpy2DAsync(s->up_prev, (size_t)C * 4, s->E + (size_t)(n - 1) * C, (size_t)n * C * 4, (size_t)C * 4, B,
+                       cudaMemcpyDeviceToDevice, st));
+  // ---- transformer: K/V of the new positions go to each row's rings, queries attend over them
   const KVRing ring{s->kring, s->vring, s->R, pos0};
-  if ((rc = run_layers(c, m->layers, tcm, Wd, m->dev_h, m->rope, m->rope_T2, x, 1, T2, s->tr, &ring, st))) return rc;
-  // ---- SEANet decoder over [context | chunk] buffers, then every buffer's last context rows move to its front
+  if ((rc = run_layers(c, m->layers, tcm, Wd, m->dev_h, m->rope, m->rope_T2, s->X, B, T2, s->tr, &ring, st))) return rc;
+  // ---- SEANet decoder over [context | chunk] buffers, then every buffer's last context rows move to its front.  fp32
+  //      mode: the residual stream goes behind conv0's context rows here (tensor-core mode: its bf16 cast does)
+  if (!tcm)
+    CK(cudaMemcpy2DAsync(s->sea.in.rows<float>(C), (size_t)s->sea.in.pitch * C * 4, s->X, (size_t)T2 * C * 4, (size_t)T2 * C * 4, B,
+                         cudaMemcpyDeviceToDevice, st));
   TailShift ts{};
-  if ((rc = tcm ? seanet_tc(m, x, s->sea, 1, T2, &ts, wav, st) : seanet_f32(m, s->sea, 1, T2, &ts, wav, st))) return rc;
-  tail_shift_kernel<<<ts.n, 256, 16384, st>>>(ts);
+  if ((rc = tcm ? seanet_tc(m, s->X, s->sea, B, T2, &ts, wav, wav_pitch, st) : seanet_f32(m, s->sea, B, T2, &ts, wav, wav_pitch, st)))
+    return rc;
+  tail_shift_kernel<<<dim3(ts.n, B), 256, 16384, st>>>(ts);
   CK(cudaGetLastError());
   s->frames += n;
   return SOPRO_OK;
@@ -1246,14 +1284,16 @@ int stream_step(sopro_mimi_stream* s, const int32_t* codes, int n, int code_stri
 
 extern "C" {
 
-int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_stream_t** out) {
+int sopro_mimi_stream_create_rows(sopro_mimi_t* m, int max_chunk_frames, int rows, sopro_mimi_stream_t** out) {
   if (!m || !out) return fail(SOPRO_ERR_INVALID, "null argument");
   *out = nullptr;
   if (max_chunk_frames < 1 || max_chunk_frames > 256) return fail(SOPRO_ERR_INVALID, "max_chunk_frames must be in [1, 256]");
+  if (rows < 1 || rows > 65535) return fail(SOPRO_ERR_INVALID, "rows must be in [1, 65535]");
   CK(cudaSetDevice(m->device));
   sopro_mimi_stream* s = new sopro_mimi_stream();
   s->m = m;
   s->max_n = max_chunk_frames;
+  s->rows = rows;
   s->precision = m->precision;
   s->R = (m->cfg.window + 2 * max_chunk_frames + 7) / 8 * 8;
   stream_layout(s, nullptr);
@@ -1276,6 +1316,10 @@ int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_s
   }
   *out = s;
   return SOPRO_OK;
+}
+
+int sopro_mimi_stream_create(sopro_mimi_t* m, int max_chunk_frames, sopro_mimi_stream_t** out) {
+  return sopro_mimi_stream_create_rows(m, max_chunk_frames, 1, out);
 }
 
 int sopro_mimi_stream_destroy(sopro_mimi_stream_t* s) {
@@ -1309,22 +1353,27 @@ int sopro_mimi_stream_reset(sopro_mimi_stream_t* s, void* stream) {
 
 int64_t sopro_mimi_stream_frames(const sopro_mimi_stream_t* s) { return s ? s->frames : -1; }
 
+int64_t sopro_mimi_stream_rows(const sopro_mimi_stream_t* s) { return s ? s->rows : -1; }
+
+int64_t sopro_mimi_stream_bytes(const sopro_mimi_stream_t* s) { return s ? (int64_t)s->slab_bytes : -1; }
+
 int sopro_mimi_decode_step(sopro_mimi_stream_t* s, const int32_t* codes, int n, float* wav, void* stream) {
   if (!s || !codes || !wav) return fail(SOPRO_ERR_INVALID, "null argument");
   if (n < 1) return fail(SOPRO_ERR_INVALID, "n must be >= 1");
   if (s->precision != s->m->precision)
     return fail(SOPRO_ERR_STATE, "the decoder's precision changed since this stream started: call sopro_mimi_stream_reset");
   if (2 * (s->frames + n) > 0x3fffffffLL) return fail(SOPRO_ERR_INVALID, "stream too long");
+  const int64_t hop = sopro_mimi_samples_per_frame(s->m);
+  if ((long long)n * hop > 0x7fffffffLL) return fail(SOPRO_ERR_INVALID, "n too large for one call");
   if (s->precision == SOPRO_MIMI_BF16_TC) {
     const int rc = check_tc_geometry(s->m);
     if (rc) return rc;
   }
   CK(cudaSetDevice(s->m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int64_t hop = sopro_mimi_samples_per_frame(s->m);
-  for (int done = 0; done < n; done += s->max_n) {  // codes are [n_q][n]: a sub-chunk starts at column `done`
+  for (int done = 0; done < n; done += s->max_n) {  // codes are [rows][n_q][n]: a sub-chunk starts at column `done`
     const int k = std::min(s->max_n, n - done);
-    const int rc = stream_step(s, codes + done, k, n, wav + (size_t)done * hop, st);
+    const int rc = stream_step(s, codes + done, k, n, wav + (size_t)done * hop, (long long)n * hop, st);
     if (rc) return rc;
   }
   return SOPRO_OK;
@@ -1334,12 +1383,12 @@ int sopro_mimi_decode_step_host(sopro_mimi_stream_t* s, const int32_t* codes_hos
   if (!s || !codes_host || !wav_host) return fail(SOPRO_ERR_INVALID, "null argument");
   if (n < 1 || n > 65536) return fail(SOPRO_ERR_INVALID, "n must be in [1, 65536]");
   const sopro_mimi_config_t& c = s->m->cfg;
-  for (size_t i = 0; i < (size_t)n * c.n_q; ++i)
+  for (size_t i = 0; i < (size_t)s->rows * n * c.n_q; ++i)
     if (codes_host[i] < 0 || codes_host[i] >= c.vocab)
       return fail(SOPRO_ERR_INVALID, "code %d at flat index %zu is outside [0, %d)", codes_host[i], i, c.vocab);
   CK(cudaSetDevice(s->m->device));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t nc = (size_t)n * c.n_q, nw = (size_t)n * (size_t)sopro_mimi_samples_per_frame(s->m);
+  const size_t nc = (size_t)s->rows * n * c.n_q, nw = (size_t)s->rows * n * (size_t)sopro_mimi_samples_per_frame(s->m);
   cudaFree(s->codes_dev);
   s->codes_dev = nullptr;
   CK(cudaMalloc(&s->codes_dev, nc * 4 + nw * 4));

@@ -37,7 +37,9 @@ struct TcOp {
   const float* scale;  // LayerScale [N] or null
   float* out_f32;      // [B][M][N] or null
   __nv_bfloat16* out_bf16;  // [B][M][N] or null
-  long long c_bs;      // batch stride of R / outputs (elements)
+  long long c_bs;      // batch stride of the outputs (elements)
+  long long r_bs;      // batch stride of R (elements; 0 = c_bs)
+  long long a_pitch;   // rows per batch item of X (0 = Min: items packed back to back)
   int M, N, K, Cin, dil, pad, bias_mod, epi, out_elu;
   int stages;          // filled in by launch()
   int tap_col[8];      // A column offset of tap j (0 everywhere for convolutions; the NAR refiner's exact three-way bf16 split
@@ -196,7 +198,7 @@ __global__ void __launch_bounds__(kGemmThreads, BN >= 128 ? 1 : 2) igemm_tc_kern
     if (op.epi == EPI_GELU) {
       v = make_float4(gelu_erf(v.x), gelu_erf(v.y), gelu_erf(v.z), gelu_erf(v.w));
     } else if (op.epi == EPI_RES_SCALE || op.epi == EPI_RES) {
-      const float4 rv = *reinterpret_cast<const float4*>(op.R + row + n);  // may alias out_f32 (in-place residual)
+      const float4 rv = *reinterpret_cast<const float4*>(op.R + (size_t)b * (size_t)op.r_bs + (size_t)m * op.N + n);  // may alias out_f32
       if (op.epi == EPI_RES_SCALE) {
         const float4 sv = __ldg(reinterpret_cast<const float4*>(op.scale + n));
         v = make_float4(fmaf(sv.x, v.x, rv.x), fmaf(sv.y, v.y, rv.y), fmaf(sv.z, v.z, rv.z), fmaf(sv.w, v.w, rv.w));
@@ -225,11 +227,13 @@ __global__ void __launch_bounds__(kGemmThreads, BN >= 128 ? 1 : 2) igemm_tc_kern
 struct ResOp {
   const float* bias1;  // [HID]
   const float* bias2;  // [2*HID]
-  const float* Z;      // fp32 skip [B][M][2*HID]
-  float* out_f32;      // [B][M][2*HID] or null
+  const float* Z;      // fp32 skip [B][M][2*HID], item b at Z + b * z_bs
+  float* out_f32;      // [B][M][2*HID] or null, item b at b * o_bs
   __nv_bfloat16* out_bf16;  // [B][M][2*HID] or null, through ELU when out_elu
   int M, taps, pad, out_elu, stages;
   int Min;  // rows of the bf16 input X (0 = M; streaming: M + taps - 1 with pad = 0, the context rows in front)
+  long long a_pitch;     // rows per batch item of X (0 = Min)
+  long long z_bs, o_bs;  // batch strides of Z and of the outputs (elements; 0 = M * 2*HID)
 };
 
 template <int HID>
@@ -365,9 +369,9 @@ __global__ void __launch_bounds__(kGemmThreads, HID <= 64 ? 2 : 1) resblock_tc_k
     for (int r = 64 * g + tg / TPR; r < 64 * g + 64; r += RPP) {
       const int m = m0 + r;
       if (m >= op.M) break;
-      const size_t row = ((size_t)b * (size_t)op.M + (size_t)m) * COUT;
+      const size_t row = (size_t)b * (size_t)op.o_bs + (size_t)m * COUT;
       const float4 a = *reinterpret_cast<const float4*>(et + r * Cfg::kEpiPitch + cl);
-      const float4 zv = *reinterpret_cast<const float4*>(op.Z + row + c);
+      const float4 zv = *reinterpret_cast<const float4*>(op.Z + (size_t)b * (size_t)op.z_bs + (size_t)m * COUT + c);
       const float4 bv = __ldg(reinterpret_cast<const float4*>(op.bias2 + c));
       float4 v = make_float4(zv.x + (a.x + bv.x), zv.y + (a.y + bv.y), zv.z + (a.z + bv.z), zv.w + (a.w + bv.w));
       if (op.out_f32) *reinterpret_cast<float4*>(op.out_f32 + row + c) = v;
@@ -537,12 +541,13 @@ inline EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// activations [B][rows][cin] bf16, box = bk channels x 128 rows x 1 batch
-inline bool make_act_map(CUtensorMap* tm, const void* base, int B, long long rows, int cin, int bk = kBK) {
+// activations [B][rows][cin] bf16, item b at base + b * pitch rows (pitch 0 = rows), box = bk channels x 128 rows x
+// 1 batch; rows past `rows` of an item read as zeros
+inline bool make_act_map(CUtensorMap* tm, const void* base, int B, long long rows, int cin, int bk = kBK, long long pitch = 0) {
   EncodeTiledFn fn = encode_tiled_fn();
   if (!fn) return false;
   const cuuint64_t dims[3] = {(cuuint64_t)cin, (cuuint64_t)rows, (cuuint64_t)B};
-  const cuuint64_t strides[2] = {(cuuint64_t)cin * 2, (cuuint64_t)rows * (cuuint64_t)cin * 2};
+  const cuuint64_t strides[2] = {(cuuint64_t)cin * 2, (cuuint64_t)(pitch > 0 ? pitch : rows) * (cuuint64_t)cin * 2};
   const cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)kBM, 1};
   const cuuint32_t es[3] = {1, 1, 1};
   return fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -618,8 +623,10 @@ inline cudaError_t launch_resblock_t(const void* X, const void* W1, const void* 
   }
   const int cout = Cfg::kCout, K1 = op.taps * cout, nk = K1 / kBK;
   op.stages = nk < Cfg::kMaxStages ? nk : Cfg::kMaxStages;
+  if (op.z_bs == 0) op.z_bs = (long long)op.M * cout;
+  if (op.o_bs == 0) op.o_bs = (long long)op.M * cout;
   CUtensorMap tmA, tmW1, tmW2;
-  if (!make_act_map(&tmA, X, B, op.Min > 0 ? op.Min : op.M, cout) || !make_weight_map(&tmW1, W1, HID, K1, HID) ||
+  if (!make_act_map(&tmA, X, B, op.Min > 0 ? op.Min : op.M, cout, kBK, op.a_pitch) || !make_weight_map(&tmW1, W1, HID, K1, HID) ||
       !make_weight_map(&tmW2, W2, cout, HID, cout, Cfg::kBKH))
     return cudaErrorInvalidValue;
   dim3 grid((unsigned)((op.M + kBM - 1) / kBM), (unsigned)B);
@@ -650,6 +657,7 @@ inline cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmW, con
     if (e != cudaSuccess) return e;
   }
   TcOp o = op;
+  if (o.r_bs == 0) o.r_bs = o.c_bs;
   const int nk = op.K / BK;
   o.stages = nk < Cfg::kMaxStages ? nk : Cfg::kMaxStages;
   // short-K layers are bound by their epilogues: two stages leave room for a third resident CTA per SM
@@ -663,7 +671,7 @@ inline cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmW, con
 inline cudaError_t launch(const void* X, long long Min, const void* W, const TcOp& op, int B, cudaStream_t st, int a_cols = 0) {
   const int BN = pick_bn(op.N), BK = pick_bk(op.Cin);
   CUtensorMap tmA, tmW;
-  if (!make_act_map(&tmA, X, B, Min, a_cols > 0 ? a_cols : op.Cin, BK) || !make_weight_map(&tmW, W, op.N, op.K, BN, BK))
+  if (!make_act_map(&tmA, X, B, Min, a_cols > 0 ? a_cols : op.Cin, BK, op.a_pitch) || !make_weight_map(&tmW, W, op.N, op.K, BN, BK))
     return cudaErrorInvalidValue;
   if (BK == 64) {
     switch (BN) {

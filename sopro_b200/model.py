@@ -238,19 +238,44 @@ class SoproModel:
         handed out; without the call the next launch is enqueued when the generator is resumed.  Frames computed ahead
         of a consumer that stops early are abandoned: on exit the RNG is settled to ``progress["consumed"]`` frames
         (default: every frame yielded), i.e. exactly the draws the reference would have made.  `attn_trace` (word
-        timestamps): a [max_frames + 1, n_attn, 1, H, L] buffer that receives the text cross-attention weights."""
-        cond, txt = prep["cond_ar"], prep["txt_seq"]
-        steps = int(max_frames) + 1
+        timestamps): a [max_frames + 1, n_attn, 1, H, L] buffer that receives the text cross-attention weights.
+        The one-row case of ar_chunk_rows."""
+        rows = self.ar_chunk_rows(prep["cond_ar"], prep["txt_seq"], [int(prep["txt_seq"].size(1))], max_frames=max_frames,
+                                  chunk_frames=chunk_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
+                                  loop_streak=loop_streak, recovery_top_p=recovery_top_p, recovery_temp=recovery_temp,
+                                  min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator,
+                                  progress=progress, attn_trace=attn_trace)
+        try:
+            for toks, finished, prefetch in rows:
+                yield toks[0], finished[0], prefetch
+        finally:
+            rows.close()
+
+    @torch.no_grad()
+    def ar_chunk_rows(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int,
+                      chunk_frames: int = 0, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                      loop_streak: int = 8, recovery_top_p: float = 0.85, recovery_temp: float = 1.2,
+                      min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
+                      generator: Optional[torch.Generator] = None, progress: Optional[dict] = None,
+                      attn_trace: Optional[torch.Tensor] = None):
+        """ar_chunks over B utterances in one session (cond [B, >= steps, D], txt [B, Lmax, D], lens): every launch
+        advances all of them by the same `chunk_frames` steps.  Yields ``(tokens, finished, prefetch)`` with one list of
+        new frames and one finished flag per row.  `seeds` gives row i the private generator of seeds[i]; without them
+        the rows draw from `generator` (None: the global one) as ar_generate_tensors does: one row's tape block by
+        block, settled on exit to ``progress["consumed"]`` frames as in ar_chunks; several rows' tapes in full, row
+        after row, before the first launch, and never settled."""
+        B, steps = int(cond.size(0)), int(max_frames) + 1
         if cond.size(1) < steps:
             raise ValueError(f"cond_ar has {cond.size(1)} rows, need max_frames+1 = {steps}")
-        L = int(txt.size(1))
         samp = self._sampling(top_p, temperature, anti_loop, loop_streak, recovery_top_p, recovery_temp, min_gen_frames, False)
         per = steps if chunk_frames <= 0 else int(chunk_frames)
         st = {"launched": 0, "read": 0, "yielded": 0}
-        with TapeFeed(1, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device,
-                      None if seed is None else [seed], generator) as feed, self._lease(1, steps, L, attn_trace) as ses:
+        lens = [int(x) for x in lens]
+        with TapeFeed(B, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device,
+                      None if seeds is None else [int(x) for x in seeds], generator) as feed, \
+                self._lease(B, steps, max(lens), attn_trace) as ses:
             launches = self._launch_blocks(ses, feed, [(a, min(steps, a + per)) for a in range(0, steps, per)],
-                                           cond[:, :steps], txt, [L], samp)
+                                           cond[:, :steps], txt, lens, samp)
 
             def launch():
                 """Enqueue the next launch (no-op while one is in flight)."""
@@ -258,21 +283,25 @@ class SoproModel:
                     st["launched"] = next(launches)
 
             try:
-                t = 0
-                while t < steps:
+                t = [0] * B
+                over = [False] * B
+                while not all(over):
                     launch()
                     toks, n, done = ses.read()  # synchronises the stream the launch ran on
-                    upto = int(n[0])
                     st["read"] = st["launched"]
-                    chunk = [int(x) for x in toks[0, t:upto]]
-                    finished = bool(done[0]) or upto >= steps or upto < st["launched"]
-                    t = upto
-                    st["yielded"] = upto
-                    yield chunk, finished, (launch if not finished else (lambda: None))
-                    if finished:
-                        break
+                    chunks, finished = [], []
+                    for b in range(B):
+                        upto = int(n[b])
+                        chunks.append([] if over[b] else [int(x) for x in toks[b, t[b]:upto]])
+                        over[b] = over[b] or bool(done[b]) or upto >= steps or upto < st["launched"]
+                        finished.append(over[b])
+                        t[b] = upto
+                    st["yielded"] = max(t)
+                    end = all(over)
+                    yield chunks, finished, (launch if not end else (lambda: None))
             finally:
-                feed.settle(int(progress["consumed"]) if progress is not None and "consumed" in progress else st["yielded"])
+                if B == 1:
+                    feed.settle(int(progress["consumed"]) if progress is not None and "consumed" in progress else st["yielded"])
 
     @torch.no_grad()
     def ar_stream(self, prep: Dict[str, torch.Tensor], *, max_frames: int, top_p: float = 0.9, temperature: float = 1.05,
@@ -720,6 +749,35 @@ class SoproTTS:
         from .streaming import stream as _stream
 
         return _stream(self, text, sample_rate=sample_rate, speed=speed, watermark=watermark, **kwargs)
+
+    def stream_batch(self, texts: Sequence[str], *, ref: Union[PreparedReference, Sequence[PreparedReference]],
+                     seeds: Optional[Sequence[int]] = None, max_frames: int = 400, top_p: float = 0.9,
+                     temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
+                     min_gen_frames: Optional[int] = None, chunk_frames: int = 6, nar_context_frames: Optional[int] = None,
+                     sample_rate: Optional[int] = None, speed: Optional[float] = None,
+                     watermark: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor, bool]]:
+        """NEW: many texts streamed side by side through one chunk loop (sopro_b200/streaming.py): one AR launch of
+        `chunk_frames` frames for every row, one ragged NAR pass and one batched Mimi stream step per chunk.  Yields
+        ``(i, wav [1, n] on the device at the output rate, last)``; within a chunk the rows come in index order.  Row i
+        yields its non-empty chunks in order, then exactly one item with last=True, which carries the tails of its
+        output chain and may be [1, 0].  `ref`: one prepared voice for every text, or one per text (as in
+        synthesize_batch); the sampling settings are shared.  With `seeds`, row i's chunks equal
+        ``list(stream(texts[i], ref=ref[i] (or ref), seed=seeds[i], ...))`` bit for bit, the last item being the stream's
+        final chunk (or empty when the stream yielded nothing more).  Without seeds the rows draw their noise as
+        synthesize_batch(texts) does, every tape in full, row after row, from the global generator; that draw happens
+        before the first AR launch, so time to first audio wants seeds (one text behaves exactly as stream(), generator
+        included).  There is no loudness (it needs the whole utterance), best_of (see stream) or word_timestamps.
+        Refused before any device work or random draw: empty `texts`, `seeds` of another length, a wrong `ref`
+        sequence, `chunk_frames` outside [1, 256], a refused sample_rate / speed / watermark, more texts than
+        min(the AR batch limit, 256).  Closing the generator early releases its AR session, noise tapes, Mimi state and
+        output-chain states."""
+        from .streaming import stream_batch as _stream_batch
+
+        return _stream_batch(self, texts, ref=ref, seeds=seeds, max_frames=max_frames, top_p=top_p,
+                             temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
+                             min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
+                             nar_context_frames=nar_context_frames, sample_rate=sample_rate, speed=speed,
+                             watermark=watermark)
 
     def save_wav(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
         """`sample_rate`: the rate the waveform is at (the one passed to synthesize / stream)."""

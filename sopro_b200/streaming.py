@@ -5,7 +5,7 @@ persistent launch + one NAR window + one Mimi decode."""
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Iterator, List, Optional
+from typing import Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -56,76 +56,136 @@ class SoproTTSStreamer:
         no mark).  Each chunk's audio goes through a time-stretch stream, a watermark stream, then a resampler stream,
         right after its Mimi step, so the chunks concatenate to the one-shot stretch, mark and resample of the 24 kHz
         stream bit for bit; the last chunk also carries their tails."""
-        tts, model = self.tts, self.tts.model
+        tts = self.tts
         post = OutputChain(tts, sample_rate, speed, watermark=watermark)  # a refused argument raises before the prefill
         text_ids = tts.encode_text(text)
         if ref is None:
             ref = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
-        prep = model.prepare_conditioning(
-            text_ids, ref, max_frames=max_frames,
-            style_strength=float(style_strength if style_strength is not None else tts.cfg.style_strength))
+        rows = self.stream_rows([text_ids], ref, post, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                anti_loop=anti_loop, style_strength=style_strength, chunk_frames=chunk_frames,
+                                nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames,
+                                seeds=None if seed is None else [seed], generator=generator)
+        try:
+            for _i, wav, _last in rows:
+                if wav is not None:
+                    yield wav
+        finally:
+            rows.close()
+
+    @torch.inference_mode()
+    def stream_rows(self, text_ids: Sequence[torch.Tensor], ref, post: OutputChain, *, max_frames: int = 400,
+                    top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                    style_strength: Optional[float] = None, chunk_frames: Optional[int] = None,
+                    nar_context_frames: Optional[int] = None, min_gen_frames: Optional[int] = None,
+                    seeds: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None
+                    ) -> Iterator[Tuple[int, Optional[torch.Tensor], bool]]:
+        """The chunk loop of B utterances (`ref`: one prepared voice, or one per text) -> ``(i, wav or None, last)``:
+        per launch, in row order, each live row's chunk (None when it has no samples), the row's last item once with
+        last=True.  All rows advance in lockstep, `chunk_frames` AR frames per launch, so the NAR window [lo, end) is
+        shared by the live rows (only a row that ends in this launch has a shorter one) and runs as one ragged NAR pass;
+        one Mimi step decodes every row (a row that has ended is fed code 0 and its samples are dropped), then each row's
+        samples go through its own output-chain stream.  Row i's chunks are those of this loop over text i alone."""
+        tts, model = self.tts, self.tts.model
+        B = len(text_ids)
+        st_ = float(style_strength if style_strength is not None else tts.cfg.style_strength)
+        txt, lens, _pool, cond = model.prefill.run(list(text_ids), ref, n_frames=int(max_frames) + 1, style_strength=st_)
+        if B == 1:
+            txt = txt[:, : int(lens[0])]
         cf = int(chunk_frames if chunk_frames is not None else self.cfg.chunk_frames)
         ctx = nar_context_frames if nar_context_frames is not None else self.cfg.nar_context_frames
         ctx = int(model.rf_nar() if ctx is None else ctx)
-        hist: List[int] = []
+        hop = tts.codec.engine.hop
+        hist: List[List[int]] = [[] for _ in range(B)]
+        ended = [False] * B
         emitted = 0
-        state = self.mimi_stream.new_state()
+        state = self.mimi_stream.new_state(B)
         # the stretch / resampler states' pushes are bounded by one chunk's samples
-        post_state = post.stream(self.mimi_stream.max_chunk_frames * tts.codec.engine.hop)
+        posts = []
         on_gpu = tts.device.type == "cuda"
         main = torch.cuda.current_stream(tts.device) if on_gpu else None
         side = torch.cuda.Stream(tts.device) if on_gpu else None
 
-        def refine_and_emit(end: int, last: bool) -> Optional[torch.Tensor]:
+        def refine_and_emit(ends: List[int], last: List[bool], live: List[int]) -> List[Optional[torch.Tensor]]:
             """NAR over the new frames + `ctx` frames of left context, Mimi stream step on the new frames' codes
-            (reference streaming.py:81-104), then the stretch and resampler pushes (and, on the last chunk, their
-            finishes); enqueued on the side stream."""
+            (reference streaming.py:81-104), then each live row's stretch and resampler pushes (and, on its last chunk,
+            their finishes); enqueued on the side stream."""
             nonlocal emitted, state
-            wav = None
+            out: List[Optional[torch.Tensor]] = [None] * B
+            end = max(ends[b] for b in live)
+            rows_wav = None
             if end > emitted:
                 lo = max(0, emitted - ctx)
-                toks = torch.as_tensor(hist[lo:end], device=tts.device, dtype=torch.long).unsqueeze(0)
-                win = model.nar_refine(prep["cond_ar"][:, lo:end, :], toks).squeeze(0)
-                wav, state = self.mimi_stream.decode_step(win[emitted - lo:, :], state, _trusted=True)  # our own NAR's codes
-                emitted = end
-            wav = post_state.finish(wav) if last else post_state.push(wav)
-            return wav if wav is not None and wav.numel() > 0 else None
+                if B == 1:
+                    toks = torch.as_tensor(hist[0][lo:end], device=tts.device, dtype=torch.long).unsqueeze(0)
+                    win = model.nar_refine(cond[:, lo:end, :], toks).squeeze(0)
+                    rows_wav, state = self.mimi_stream.decode_step(win[emitted - lo:, :], state, _trusted=True)  # our own NAR's codes
+                else:
+                    run = [b for b in live if ends[b] > emitted]
+                    W = end - lo
+                    toks = torch.zeros((len(run), W), dtype=torch.long)
+                    for j, b in enumerate(run):
+                        toks[j, : ends[b] - lo] = torch.as_tensor(hist[b][lo:ends[b]], dtype=torch.long)
+                    idx = torch.tensor(run, device=tts.device)
+                    win = model.nar_refine(cond[idx, lo:end, :], toks.to(tts.device),
+                                           lens=torch.tensor([ends[b] - lo for b in run], dtype=torch.int32))
+                    n = end - emitted
+                    keep = (torch.arange(n)[None, :] < torch.tensor([ends[b] - emitted for b in run])[:, None]).to(tts.device)
+                    codes = torch.zeros((B, n, win.shape[2]), dtype=torch.long, device=tts.device)
+                    codes[idx] = win[:, emitted - lo:, :] * keep[:, :, None]  # a finished row's frames decode code 0
+                    rows_wav, state = self.mimi_stream.decode_step(codes, state, _trusted=True)
+            for b in live:
+                wav = rows_wav[b: b + 1, : (ends[b] - emitted) * hop] if rows_wav is not None and ends[b] > emitted else None
+                wav = posts[b].finish(wav) if last[b] else posts[b].push(wav)
+                out[b] = wav if wav is not None and wav.numel() > 0 else None
+            emitted = end
+            return out
 
         progress = {"consumed": 0}
-        chunks = model.ar_chunks(prep, max_frames=max_frames, chunk_frames=cf, top_p=top_p, temperature=temperature,
-                                 anti_loop=anti_loop, min_gen_frames=min_gen_frames, seed=seed, generator=generator,
-                                 progress=progress)
+        chunks = model.ar_chunk_rows(cond, txt, lens, max_frames=max_frames, chunk_frames=cf, top_p=top_p,
+                                     temperature=temperature, anti_loop=anti_loop, min_gen_frames=min_gen_frames,
+                                     seeds=seeds, generator=generator, progress=progress)
         try:
-            for toks, finished, prefetch in chunks:
-                # the stream ends at the first EOS regardless of min_gen_frames (reference streaming.py:114-115)
-                stop = model.eos_id in toks
-                if stop:
-                    toks = toks[: toks.index(model.eos_id)]
-                progress["consumed"] += len(toks) + (1 if stop else 0)  # the reference also draws for the EOS step
-                hist.extend(toks)
-                last = stop or finished
-                end = len(hist) if last else (len(hist) // cf) * cf
-                wav = None
+            for _ in range(B):
+                posts.append(post.stream(self.mimi_stream.max_chunk_frames * hop))
+            for toks_rows, finished, prefetch in chunks:
+                live = [b for b in range(B) if not ended[b]]
+                ends, last = [0] * B, [False] * B
+                for b in live:
+                    toks = toks_rows[b]
+                    # the stream ends at the first EOS regardless of min_gen_frames (reference streaming.py:114-115)
+                    stop = model.eos_id in toks
+                    if stop:
+                        toks = toks[: toks.index(model.eos_id)]
+                    if B == 1:
+                        progress["consumed"] += len(toks) + (1 if stop else 0)  # the reference also draws for the EOS step
+                    hist[b].extend(toks)
+                    last[b] = stop or finished[b]
+                    ends[b] = len(hist[b]) if last[b] else (len(hist[b]) // cf) * cf
+                done = all(last[b] for b in live)
                 if on_gpu:
                     side.wait_stream(main)
                     with torch.cuda.stream(side):
-                        wav = refine_and_emit(end, last)
-                    if not last:
+                        wavs = refine_and_emit(ends, last, live)
+                    if not done:
                         main.wait_stream(side)  # AR(k+1) behind chunk k's NAR + Mimi, never in front of them
                         prefetch()
                     side.synchronize()
-                    if wav is not None:
-                        wav.record_stream(main)
+                    for w in wavs:
+                        if w is not None:
+                            w.record_stream(main)
                 else:
-                    wav = refine_and_emit(end, last)
-                if wav is not None:
-                    yield wav
-                if last:
+                    wavs = refine_and_emit(ends, last, live)
+                for b in live:
+                    if wavs[b] is not None or last[b]:
+                        yield b, wavs[b], last[b]
+                    ended[b] = last[b]
+                if done:
                     break
         finally:
             chunks.close()
             self.mimi_stream.release(state)
-            post_state.release()
+            for p in posts:
+                p.release()
 
 
 @torch.inference_mode()
@@ -136,3 +196,50 @@ def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_t
     streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
     return streamer.stream(text, ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref=ref,
                            chunk_frames=chunk_frames, sample_rate=sample_rate, speed=speed, watermark=watermark, **kwargs)
+
+
+MAX_STREAM_ROWS = 256  # a Mimi stream state holds tens of MB per row (DESIGN.md §5o)
+
+
+def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int]] = None, max_frames: int = 400,
+                 top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                 style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None, chunk_frames: int = 6,
+                 nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
+                 watermark: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor, bool]]:
+    """SoproTTS.stream_batch: every argument is checked here, before any device work or random draw; the returned
+    generator runs SoproTTSStreamer.stream_rows over the texts."""
+    from . import voices
+
+    if isinstance(texts, str) or not isinstance(texts, Sequence):
+        raise TypeError(f"texts must be a sequence of strings, got {type(texts).__name__}")
+    texts = list(texts)
+    if not texts:
+        raise ValueError("texts is empty: stream_batch needs at least one text")
+    limit = tts._batch_limit()
+    limit = MAX_STREAM_ROWS if limit is None else min(int(limit), MAX_STREAM_ROWS)
+    if len(texts) > limit:
+        raise ValueError(f"{len(texts)} texts; stream_batch streams at most {limit} side by side on this device")
+    if seeds is not None:
+        seeds = [int(x) for x in seeds]
+        if len(seeds) != len(texts):
+            raise ValueError(f"{len(seeds)} seeds for {len(texts)} texts")
+    voices.check_voices(ref, len(texts), **voices.geometry(tts.cfg))
+    if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int):
+        raise TypeError(f"chunk_frames must be an int, got {type(chunk_frames).__name__}")
+    if not 1 <= chunk_frames <= 256:
+        raise ValueError(f"chunk_frames must be in [1, 256], got {chunk_frames}")
+    post = OutputChain(tts, sample_rate, speed, watermark=watermark)
+    streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
+
+    def rows_of():
+        ids = [tts.encode_text(t) for t in texts]
+        rows = streamer.stream_rows(ids, ref, post, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                    anti_loop=anti_loop, style_strength=style_strength, chunk_frames=chunk_frames,
+                                    nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames, seeds=seeds)
+        try:
+            for i, wav, last in rows:
+                yield i, (wav if wav is not None else torch.zeros(1, 0, device=tts.device)), last
+        finally:
+            rows.close()
+
+    return rows_of()

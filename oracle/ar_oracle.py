@@ -23,6 +23,8 @@ from typing import Dict, Iterator, List, Optional, Sequence, Tuple
 import torch
 import torch.nn.functional as F
 
+from oracle.dense_probes import rel_errors
+
 Tensor = torch.Tensor
 SD = Dict[str, Tensor]
 
@@ -30,12 +32,18 @@ SD = Dict[str, Tensor]
 # ---------------------------------------------------------------------------
 # building blocks
 # ---------------------------------------------------------------------------
+def _acc(t: Tensor) -> Tensor:
+    """The compute type: float64 stays float64 (the float64 oracle), everything else is computed in fp32 as the
+    reference does."""
+    return t if t.dtype == torch.float64 else t.float()
+
+
 def rms_norm(x: Tensor, w: Tensor, eps: float = 1e-6) -> Tensor:
-    """nn/blocks.py:32-37 — fp32 mean of squares, rsqrt, scale by weight."""
-    x32 = x.float()
+    """nn/blocks.py:32-37 — fp32 mean of squares, rsqrt, scale by weight (float64 for float64 input)."""
+    x32 = _acc(x)
     var = x32.pow(2).mean(dim=-1, keepdim=True)
     y32 = x32 * torch.rsqrt(var + eps)
-    y32 = y32 * w.float()
+    y32 = y32 * w.to(x32.dtype)
     return y32.to(dtype=x.dtype)
 
 
@@ -88,8 +96,8 @@ def text_kv_cache(sd: SD, p: str, txt_seq: Tensor, n_heads: int) -> Tuple[Tensor
 
 
 def xattn_step(sd: SD, p: str, x: Tensor, k: Tensor, v: Tensor, keep: Optional[Tensor], n_heads: int) -> Tensor:
-    """nn/text.py:93-131 — pre-norm q, fp32 SDPA over the cached text K/V with a
-    boolean keep-mask, nan_to_num, out-proj, x + tanh(gate)*a."""
+    """nn/text.py:93-131 — pre-norm q, fp32 SDPA (float64 for float64 input) over the
+    cached text K/V with a boolean keep-mask, nan_to_num, out-proj, x + tanh(gate)*a."""
     q = _heads(F.linear(rms_norm(x, sd[p + "nq.weight"]), sd[p + "q_proj.weight"]), n_heads)
     mask = None
     if keep is not None:
@@ -99,7 +107,7 @@ def xattn_step(sd: SD, p: str, x: Tensor, k: Tensor, v: Tensor, keep: Optional[T
             keep = keep.clone()
             keep[bad, 0] = True
         mask = keep[:, None, None, :]
-    a = F.scaled_dot_product_attention(q.float(), k.float(), v.float(), attn_mask=mask, dropout_p=0.0, is_causal=False)
+    a = F.scaled_dot_product_attention(_acc(q), _acc(k), _acc(v), attn_mask=mask, dropout_p=0.0, is_causal=False)
     a = torch.nan_to_num(a, nan=0.0, posinf=0.0, neginf=0.0).to(x.dtype)
     B, H, T, Dh = a.shape
     a = a.transpose(1, 2).contiguous().view(B, T, H * Dh)
@@ -138,6 +146,66 @@ def ar_step(sd: SD, cfg, x: Tensor, st: ArState, trace: Optional[dict] = None) -
             trace[f"h{i}"] = h.clone()
     h = rms_norm(h, sd["ar.norm.weight"])
     return F.linear(h, sd["ar.head.weight"], sd["ar.head.bias"])
+
+
+@dataclass
+class ArTrace:
+    """What a teacher-forced run of ar_step computed, in the kernel's trace layouts."""
+    blocks: Tensor                    # [steps, n_layers, B, D] residual after every layer
+    logits: Tensor                    # [steps, B, V]
+    kv: Dict[int, Tuple[Tensor, Tensor]]  # attention layer -> text (K, V), each [B, H, Lmax, Dh]
+
+
+def ar_teacher_forced(sd: SD, cfg, cond_ar: Tensor, txt_seq: Tensor, text_len: Sequence[int], forced: Tensor,
+                      dtype: torch.dtype = torch.float32) -> ArTrace:
+    """A ragged batch through ar_step with the tokens forced, every tensor cast to ``dtype`` (float64: the float64
+    oracle; float32: the reference's arithmetic).
+
+    cond_ar [B, steps, D], txt_seq [B, Lmax, D] (rows past text_len[b] are padding, masked out through the keep-mask),
+    forced [B, steps] token ids: step 0 takes the BOS row, step t the embedding row of forced[:, t - 1] (EOS =
+    codebook_size is fed back as table row codebook_size, model.py:266-272)."""
+    sd = {k: v.to(dtype) for k, v in sd.items()}
+    cond_ar, txt_seq = cond_ar.to(dtype), txt_seq.to(dtype)
+    B, steps, _D = cond_ar.shape
+    keep = torch.arange(txt_seq.size(1))[None, :] < torch.as_tensor(list(text_len))[:, None]
+    st = ar_init_state(sd, cfg, txt_seq, keep, batch=B)
+    emb = sd["cb_embed.emb.weight"]
+    bos_row = int(cfg.num_codebooks) * int(cfg.codebook_size)
+    n_layers = int(cfg.n_layers_ar)
+    blocks = torch.empty((steps, n_layers, B, int(cfg.d_model)), dtype=dtype)
+    logits = torch.empty((steps, B, int(cfg.ar_vocab())), dtype=dtype)
+    for t in range(steps):
+        rows = torch.full((B,), bos_row, dtype=torch.long) if t == 0 else forced[:, t - 1].long()
+        tr: dict = {}
+        logits[t] = ar_step(sd, cfg, cond_ar[:, t: t + 1] + emb[rows].unsqueeze(1), st, tr)[:, 0]
+        for i in range(n_layers):
+            blocks[t, i] = tr[f"h{i}"][:, 0]
+    return ArTrace(blocks=blocks, logits=logits, kv=dict(st.kv))
+
+
+def ar_trace_labels(cfg) -> List[str]:
+    """Names of the quantities ar_trace_errors compares, in its order."""
+    attn = list(cfg.ar_attn_layers())
+    return ([f"h{i}" for i in range(int(cfg.n_layers_ar))] + ["logits"] + [f"k{i}" for i in attn]
+            + [f"v{i}" for i in attn])
+
+
+def ar_trace_errors(got: ArTrace, ref: ArTrace, text_len: Sequence[int]) -> Tensor:
+    """[B, len(ar_trace_labels), 2] float64: for every utterance, the max and RMS error of each layer's residual, of
+    the logits, and of every attention layer's text K and V rows [:text_len[b]], against ``ref``, relative to that
+    utterance's own peak and RMS (dense_probes.rel_errors) over all its steps."""
+    B = got.logits.size(1)
+    n_layers = got.blocks.size(1)
+    out = torch.empty((B, n_layers + 1 + 2 * len(ref.kv), 2), dtype=torch.float64)
+    for b in range(B):
+        L = int(text_len[b])
+        pairs = [(got.blocks[:, i, b], ref.blocks[:, i, b]) for i in range(n_layers)]
+        pairs.append((got.logits[:, b], ref.logits[:, b]))
+        pairs += [(got.kv[i][0][b, :, :L], ref.kv[i][0][b, :, :L]) for i in ref.kv]
+        pairs += [(got.kv[i][1][b, :, :L], ref.kv[i][1][b, :, :L]) for i in ref.kv]
+        for j, (z, z64) in enumerate(pairs):
+            out[b, j] = torch.tensor(rel_errors(z, z64), dtype=torch.float64)
+    return out
 
 
 # ---------------------------------------------------------------------------

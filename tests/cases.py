@@ -86,6 +86,23 @@ def ar_case_inputs(spec: dict):
     return cfg, sd, inp
 
 
+def ar_forced_batch(cfg: SoproTTSConfig, lens: List[int], steps: int, key: int, pad: float = 30.0):
+    """A teacher-forced ragged batch: cond_ar [B, steps, D]; txt_seq [B, max(lens), D] whose rows past lens[b] are
+    padding of pad x unit-variance values (pad = 0: zeros); forced ids [B, steps] int32 in [0, codebook_size), with
+    EOS (= codebook_size) every 37th step from a per-utterance offset."""
+    D, B, Lm, eos = int(cfg.d_model), len(lens), max(lens), int(cfg.codebook_size)
+    k = int(key) * 1000
+    cond = torch.stack([_unit(steps * D, k + b).view(steps, D) for b in range(B)])
+    txt = (_unit(B * Lm * D, k + 500) * float(pad)).view(B, Lm, D)
+    for b, L in enumerate(lens):
+        txt[b, :L] = _unit(L * D, k + 600 + b).view(L, D)
+    u = torch.from_numpy(hash_uniform(B * steps, k + 900)).double().view(B, steps) * 0.5 + 0.5
+    forced = (u * eos).long().clamp(max=eos - 1)
+    t = torch.arange(steps)[None, :]
+    forced[(t + 11 * torch.arange(B)[:, None]) % 37 == 5] = eos
+    return cond, txt, forced.to(torch.int32)
+
+
 # ---------------------------------------------------------------------------
 # sampler known-answer cases (reference: sampling.py:24-93)
 # ---------------------------------------------------------------------------

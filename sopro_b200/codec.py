@@ -562,9 +562,12 @@ class MimiStreamDecoder:
     def decode_step(self, codes_chunk_tq: torch.Tensor, state: Optional[MimiDecodeState] = None, *,
                     overlap_frames: int = 2, _trusted: bool = False) -> Tuple[torch.Tensor, MimiDecodeState]:
         """codes [n, Q] of one utterance -> wav [1, n*hop]; or codes [rows, n, Q] of a state's rows -> wav [rows, n*hop]
-        (the state takes its row count from the first chunk it decodes)."""
+        (the state takes its row count from the first chunk it decodes).  Codes [1, n, Q] are one utterance's: the state
+        is a one-row stream, stepped with [Q, n] like any one-utterance chunk."""
         if state is None:
             state = MimiDecodeState()
+        if codes_chunk_tq.dim() == 3 and codes_chunk_tq.size(0) == 1:
+            codes_chunk_tq = codes_chunk_tq[0]
         rows = 1 if codes_chunk_tq.dim() == 2 else int(codes_chunk_tq.size(0))
         n_new = int(codes_chunk_tq.size(-2))
         if n_new == 0:

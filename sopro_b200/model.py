@@ -26,7 +26,7 @@ from . import rerank
 from . import timestamps as TS
 from . import voices
 from ._lib import StatePool
-from .codec import MimiCodec
+from .codec import MimiCodec, MimiStreamDecoder
 from .config import TARGET_SR, SoproTTSConfig
 from .denoising import check_denoise
 from .engine import ArEngine, ArSession, Sampling
@@ -183,22 +183,13 @@ class SoproModel:
     def prepare_conditioning(self, text_ids_1d: torch.Tensor, ref: PreparedReference, *, max_frames: int, device=None,
                              style_strength: float = 1.2) -> Dict[str, torch.Tensor]:
         """reference model.py:174-216 on the CUDA prefill engine (sopro_b200/csrc/nar_engine.cu: ~25 fused fp32 kernels)."""
-        return self.prepare_conditioning_batch([text_ids_1d], ref, max_frames=max_frames, style_strength=style_strength)[0]
-
-    @torch.no_grad()
-    def prepare_conditioning_batch(self, text_ids: Sequence[torch.Tensor], ref: PreparedReference, *, max_frames: int,
-                                   style_strength: float = 1.2) -> List[Dict[str, torch.Tensor]]:
-        """NEW (the reference is batch-1): the prefill of B texts that share one prepared reference in ONE pass; element i
-        is the `prep` dict of model.py:210-216 for text i (views into the batch tensors)."""
-        txt_seq, lens, txt_pool, cond = self.prefill.run(text_ids, ref, n_frames=int(max_frames) + 1, style_strength=float(style_strength))
+        txt_seq, lens, txt_pool, cond = self.prefill.run([text_ids_1d], ref, n_frames=int(max_frames) + 1,
+                                                         style_strength=float(style_strength))
         sv = ref.sv_ref.to(self.device)
         if sv.dim() == 1:
             sv = sv.unsqueeze(0)
-        out = []
-        for i, L in enumerate(lens):
-            out.append({"txt_seq": txt_seq[i: i + 1, :L], "text_mask": torch.ones((1, L), dtype=torch.bool, device=self.device),
-                        "txt_pool": txt_pool[i: i + 1], "sv_ref": sv, "cond_ar": cond[i: i + 1]})
-        return out
+        return {"txt_seq": txt_seq, "text_mask": torch.ones((1, lens[0]), dtype=torch.bool, device=self.device),
+                "txt_pool": txt_pool, "sv_ref": sv, "cond_ar": cond}
 
     @torch.no_grad()
     def nar_refine(self, cond_seq: torch.Tensor, rvq1_1xT: torch.Tensor, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -226,44 +217,25 @@ class SoproModel:
         return int(samp.top_k) if (samp.top_p < 1.0 and samp.recovery_top_p < 1.0) else int(self.cfg.ar_vocab())
 
     @torch.no_grad()
-    def ar_chunks(self, prep: Dict[str, torch.Tensor], *, max_frames: int, chunk_frames: int = 0, top_p: float = 0.9,
-                  temperature: float = 1.05, anti_loop: bool = True, loop_streak: int = 8, recovery_top_p: float = 0.85,
-                  recovery_temp: float = 1.2, min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-                  generator: Optional[torch.Generator] = None, progress: Optional[dict] = None,
-                  attn_trace: Optional[torch.Tensor] = None):
-        """The persistent kernel driven `chunk_frames` frames per launch (0 = the whole utterance in one launch).
-        Yields ``(tokens, finished, prefetch)`` per launch: the frames it produced (ints), whether the utterance is over
-        (EOS past min_gen_frames, or max_frames reached), and a callable that enqueues the NEXT launch right away on the
-        current CUDA stream -- a streaming consumer queues it behind its own NAR + Mimi work so it runs while the audio is
-        handed out; without the call the next launch is enqueued when the generator is resumed.  Frames computed ahead
-        of a consumer that stops early are abandoned: on exit the RNG is settled to ``progress["consumed"]`` frames
-        (default: every frame yielded), i.e. exactly the draws the reference would have made.  `attn_trace` (word
-        timestamps): a [max_frames + 1, n_attn, 1, H, L] buffer that receives the text cross-attention weights.
-        The one-row case of ar_chunk_rows."""
-        rows = self.ar_chunk_rows(prep["cond_ar"], prep["txt_seq"], [int(prep["txt_seq"].size(1))], max_frames=max_frames,
-                                  chunk_frames=chunk_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
-                                  loop_streak=loop_streak, recovery_top_p=recovery_top_p, recovery_temp=recovery_temp,
-                                  min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator,
-                                  progress=progress, attn_trace=attn_trace)
-        try:
-            for toks, finished, prefetch in rows:
-                yield toks[0], finished[0], prefetch
-        finally:
-            rows.close()
-
-    @torch.no_grad()
     def ar_chunk_rows(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int,
                       chunk_frames: int = 0, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
                       loop_streak: int = 8, recovery_top_p: float = 0.85, recovery_temp: float = 1.2,
                       min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                       generator: Optional[torch.Generator] = None, progress: Optional[dict] = None,
                       attn_trace: Optional[torch.Tensor] = None):
-        """ar_chunks over B utterances in one session (cond [B, >= steps, D], txt [B, Lmax, D], lens): every launch
-        advances all of them by the same `chunk_frames` steps.  Yields ``(tokens, finished, prefetch)`` with one list of
-        new frames and one finished flag per row.  `seeds` gives row i the private generator of seeds[i]; without them
-        the rows draw from `generator` (None: the global one) as ar_generate_tensors does: one row's tape block by
-        block, settled on exit to ``progress["consumed"]`` frames as in ar_chunks; several rows' tapes in full, row
-        after row, before the first launch, and never settled."""
+        """The persistent kernel over B utterances in one session (cond [B, >= steps, D], txt [B, Lmax, D], lens),
+        driven `chunk_frames` frames per launch (0 = the whole utterance in one launch): every launch advances all of
+        them by the same steps.  Yields ``(tokens, finished, prefetch)`` per launch: one list of new frames (ints) and
+        one finished flag (EOS past min_gen_frames, or max_frames reached) per row, and a callable that enqueues the NEXT
+        launch right away on the current CUDA stream -- a streaming consumer queues it behind its own NAR + Mimi work so
+        it runs while the audio is handed out; without the call the next launch is enqueued when the generator is
+        resumed.  `seeds` gives row i the private generator of seeds[i]; without them the rows draw from `generator`
+        (None: the global one) as ar_generate_tensors does: one row's tape block by block, several rows' tapes in full,
+        row after row, before the first launch.  One row's frames computed ahead of a consumer that stops early are
+        abandoned: on exit its generator is settled to ``progress["consumed"]`` frames (default: every frame yielded),
+        i.e. exactly the draws the reference would have made; several rows' are never settled.  `attn_trace` (word
+        timestamps): a [max_frames + 1, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text
+        cross-attention weights."""
         B, steps = int(cond.size(0)), int(max_frames) + 1
         if cond.size(1) < steps:
             raise ValueError(f"cond_ar has {cond.size(1)} rows, need max_frames+1 = {steps}")
@@ -313,14 +285,15 @@ class SoproModel:
         `launch_frames` frames per launch (0 = the whole utterance in one launch); a consumer that stops iterating
         early simply abandons the frames computed ahead, and the RNG is settled to the frames actually consumed."""
         progress = {"consumed": 0}
-        gen = self.ar_chunks(prep, max_frames=max_frames, chunk_frames=launch_frames, top_p=top_p, temperature=temperature,
-                             anti_loop=anti_loop, loop_streak=loop_streak, recovery_top_p=recovery_top_p,
-                             recovery_temp=recovery_temp, min_gen_frames=min_gen_frames, seed=seed, generator=generator,
-                             progress=progress, attn_trace=attn_trace)
+        gen = self.ar_chunk_rows(prep["cond_ar"], prep["txt_seq"], [int(prep["txt_seq"].size(1))], max_frames=max_frames,
+                                 chunk_frames=launch_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
+                                 loop_streak=loop_streak, recovery_top_p=recovery_top_p, recovery_temp=recovery_temp,
+                                 min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator,
+                                 progress=progress, attn_trace=attn_trace)
         t = 0
         try:
-            for chunk, _finished, _prefetch in gen:
-                for tok in chunk:
+            for rows, _finished, _prefetch in gen:
+                for tok in rows[0]:
                     progress["consumed"] = t + 1
                     yield t, tok, tok == self.eos_id
                     t += 1
@@ -331,13 +304,16 @@ class SoproModel:
     def ar_generate_tensors(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int, top_p: float = 0.9,
                             temperature: float = 1.05, anti_loop: bool = True, min_gen_frames: Optional[int] = None,
                             seeds: Optional[Sequence[int]] = None, stop_on_first_eos: bool = True,
-                            attn_trace: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None):
+                            attn_trace: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None,
+                            settle: bool = False):
         """B utterances in ONE persistent kernel run from batch tensors (cond [B, >=steps, D], txt [B, Lmax, D], lens).
         -> (tokens [B, steps] int32 numpy, n_tokens [B]).  With `seeds` and at least 64 steps the run is launched in
         growing blocks (the kernel resumes from its device state), each block's tapes drawn on host threads while the
         device generates the block before; otherwise in one launch.  `attn_trace` (word timestamps): a
         [steps, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text cross-attention weights.  Without
-        `seeds` the tapes draw from `generator` (None: the global one)."""
+        `seeds` the tapes draw from `generator` (None: the global one), every tape in full, row after row; `settle`
+        (one row, with stop_on_first_eos) then leaves the generator after exactly the draws of the frames generated, up
+        to and including the first EOS, as the reference's generate_tokens does."""
         B, steps = int(cond.shape[0]), int(max_frames) + 1
         samp = self._sampling(top_p, temperature, anti_loop, 8, 0.85, 1.2, min_gen_frames, stop_on_first_eos)
         edges = _growing_blocks(steps) if seeds is not None and steps >= 64 else [(0, steps)]
@@ -346,31 +322,65 @@ class SoproModel:
             for _ in self._launch_blocks(ses, feed, edges, cond[:, :steps], txt, [int(x) for x in lens], samp):
                 pass
             toks, n, _ = ses.read()
+            if settle:
+                feed.settle(int(n[0]))
         return toks, n
+
+    @torch.no_grad()
+    def generate_codes(self, text_ids: Sequence[torch.Tensor], ref, *, max_frames: int, top_p: float = 0.9,
+                       temperature: float = 1.05, anti_loop: bool = True, style_strength: float = 1.2,
+                       min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
+                       generator: Optional[torch.Generator] = None, settle: bool = False,
+                       attn_trace: Optional[torch.Tensor] = None,
+                       info: Optional[dict] = None) -> Tuple[List[int], Optional[torch.Tensor]]:
+        """NEW (the reference is batch-1): B texts with one prepared reference, or one each (`ref` as in
+        SoproTTS.synthesize_batch): one batched prefill, one persistent AR run until each text's first EOS, one ragged
+        NAR pass -> (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0
+        frames).  `seeds`, `generator`, `settle`, `attn_trace`: see ar_generate_tensors.  `info` (best-of-N): receives
+        "stopped", whether each row sampled an EOS, and "text_lens"."""
+        txt_seq, lens, _pool, cond = self.prefill.run(list(text_ids), ref, n_frames=int(max_frames) + 1,
+                                                      style_strength=float(style_strength))
+        toks, n = self.ar_generate_tensors(cond, txt_seq, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                           anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds,
+                                           attn_trace=attn_trace, generator=generator, settle=settle)
+        eos = self.eos_id
+        Ts, stopped = [], []
+        for i in range(len(lens)):
+            row = toks[i, : n[i]]
+            hit = (row == eos).nonzero()[0]
+            Ts.append(int(hit[0]) if hit.size else int(n[i]))
+            stopped.append(bool(hit.size))
+        if info is not None:
+            info["stopped"], info["text_lens"] = stopped, [int(x) for x in lens]
+        Tmax = max(Ts)
+        if Tmax == 0:
+            return Ts, None
+        # NAR refiner over the ragged batch (not causal: `lens` makes the padding act as each utterance's zero padding)
+        rvq1 = torch.from_numpy(toks[:, :Tmax].copy()).to(self.device)
+        codes = self.nar_refine(cond[:, :Tmax], rvq1.clamp_(0, eos - 1), lens=torch.tensor(Ts, dtype=torch.int32))
+        return Ts, codes
 
     @torch.no_grad()
     def generate_tokens(self, text_ids_1d: torch.Tensor, ref: PreparedReference, *, max_frames: int, device=None,
                         top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True, style_strength: float = 1.2,
                         min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
                         generator: Optional[torch.Generator] = None, attn_trace: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """reference model.py:349-401: prefill, AR until the first EOS, cut there, NAR refine -> [T, Q] int64.
-        `attn_trace`: see ar_chunks."""
-        prep = self.prepare_conditioning(text_ids_1d, ref, max_frames=max_frames, style_strength=style_strength)
-        hist: List[int] = []
-        for _t, tok, is_eos in self.ar_stream(prep, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                              anti_loop=anti_loop, min_gen_frames=min_gen_frames, seed=seed, generator=generator,
-                                              attn_trace=attn_trace):
-            hist.append(tok)
-            if is_eos:
-                break
-        T = hist.index(self.eos_id) if self.eos_id in hist else len(hist)
-        if T <= 0:
+        """reference model.py:349-401: prefill, AR until the first EOS, cut there, NAR refine -> [T, Q] int64; the
+        one-text case of generate_codes, the generator settled as the reference leaves it.  `attn_trace`: see
+        ar_generate_tensors."""
+        Ts, codes = self.generate_codes([text_ids_1d], ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                        anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
+                                        seeds=None if seed is None else [seed], generator=generator, settle=True,
+                                        attn_trace=attn_trace)
+        if codes is None:
             return torch.zeros((0, int(self.cfg.num_codebooks)), dtype=torch.long, device=self.device)
-        rvq1 = torch.tensor(hist[:T], device=self.device, dtype=torch.long).unsqueeze(0)
-        return self.nar_refine(prep["cond_ar"][:, :T, :], rvq1).squeeze(0)
+        return codes[0, : Ts[0]]
 
 
 class SoproTTS:
+    # idle Mimi stream states, made by the first stream (sopro_b200/streaming.py), replaced for larger chunks
+    _stream_decoder: Optional[MimiStreamDecoder] = None
+
     def __init__(self, model: SoproModel, cfg: SoproTTSConfig, tokenizer, codec: MimiCodec, device: str):
         self.model = model
         self.cfg = cfg
@@ -498,32 +508,22 @@ class SoproTTS:
         sopro_b200.detect_watermark finds with the same key (sopro_b200/watermark.py)."""
         post = OutputChain(self, sample_rate, speed, loudness, watermark)  # a refused argument raises before any work
         n_best = self._check_best_of(best_of, 1)
-        text_ids = self.encode_text(text)
-        trace = spans = None
-        if word_timestamps:
-            spans = self.tokenizer.encode_with_offsets(text)[1]
-            if n_best == 1:
-                trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, 1, int(text_ids.numel()), self.device)
         if ref is None:
             ref = self.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
-        if n_best == 1:
-            tokens_tq = self.model.generate_tokens(
-                text_ids, ref=ref, max_frames=max_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
-                style_strength=float(style_strength if style_strength is not None else self.cfg.style_strength),
-                min_gen_frames=min_gen_frames, seed=seed, generator=generator, attn_trace=trace)
-        else:
-            tr: Optional[dict] = {} if word_timestamps else None
-            Ts, codes = self._best_codes([text], ref, n_best, seeds=None if seed is None else [int(seed)], trace_out=tr,
-                                         generator=generator, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                         anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
-            tokens_tq = (codes[0, : Ts[0]] if codes is not None
-                         else torch.zeros((0, int(self.cfg.num_codebooks)), dtype=torch.long, device=self.device))
-            if word_timestamps:
-                trace = tr["probs"]
+        tr: Optional[dict] = {} if word_timestamps else None
+        # one take settles the generator as the reference's generate_tokens does; best_of takes draw as synthesize_batch
+        Ts, codes = self._best_codes([text], ref, n_best, seeds=None if seed is None else [int(seed)], trace_out=tr,
+                                     generator=generator, settle=n_best == 1, max_frames=max_frames, top_p=top_p,
+                                     temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
+                                     min_gen_frames=min_gen_frames)
         words = None
         if word_timestamps:
-            words = self._timings([text], [spans], trace, [int(text_ids.numel())], [int(tokens_tq.shape[0])], post.S)[0]
-        wav, _ = post(self.codec.decode_full(tokens_tq))
+            spans = self.tokenizer.encode_with_offsets(text)[1]
+            words = self._timings([text], [spans], tr["probs"], tr["lens"], Ts, post.S)[0]
+        wav = torch.zeros(1, 1, 0, device=self.device)
+        for _chunk, w, lens in self._decode_chunks(codes, Ts):
+            w, lens = post(w, lens)
+            wav = w[:, :, : lens[0]]
         return (wav, words) if word_timestamps else wav
 
     @torch.inference_mode()
@@ -640,7 +640,8 @@ class SoproTTS:
         """_batch_codes with `best_of` candidates per text (sopro_b200/rerank.py): text i's candidate k is row i*N + k
         of ONE _batch_codes pass, with seed seeds[i] + k and text i's voice; every take is scored with one Token2SV
         launch against its text's voice's sv_ref, rerank.choose picks one per text, and only the picked rows are returned
-        (the trace too), so the caller decodes those alone.  best_of = 1 is _batch_codes itself."""
+        (the trace too), so the caller decodes those alone.  best_of = 1 is _batch_codes itself.  `kw`: those of
+        _batch_codes (`settle` only with best_of = 1)."""
         N = int(best_of)
         if N == 1:
             return self._batch_codes(texts, ref, seeds=seeds, trace_out=trace_out, generator=generator, **kw)
@@ -684,42 +685,19 @@ class SoproTTS:
             rerank.check_rows(rows * n, self._batch_limit())
         return n
 
-    def _batch_codes(self, texts: Sequence[str], ref, *, max_frames: int, top_p: float,
-                     temperature: float, anti_loop: bool, style_strength: Optional[float], min_gen_frames: Optional[int],
-                     seeds: Optional[Sequence[int]], trace_out: Optional[dict] = None, generator: Optional[torch.Generator] = None,
-                     info: Optional[dict] = None) -> Tuple[List[int], Optional[torch.Tensor]]:
-        """B texts with one prepared reference, or one each (`ref` as in synthesize_batch): one batched prefill, one
-        persistent AR launch, one ragged NAR pass ->
-        (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0 frames).
-        `trace_out` (word timestamps): receives "probs", the AR launch's attention weights, and "lens", the text lengths.
-        `info` (best-of-N): receives "stopped", whether each row sampled an EOS, and "text_lens"."""
-        st = float(style_strength if style_strength is not None else self.cfg.style_strength)
-        model = self.model
+    def _batch_codes(self, texts: Sequence[str], ref, *, max_frames: int, style_strength: Optional[float],
+                     trace_out: Optional[dict] = None, **kw) -> Tuple[List[int], Optional[torch.Tensor]]:
+        """SoproModel.generate_codes of the texts (`ref` as in synthesize_batch) -> (frames before the first EOS per
+        text, codes [B, Tmax, Q]; None when every text has 0 frames).  `trace_out` (word timestamps): receives "probs",
+        the AR launch's attention weights, and "lens", the text lengths."""
         ids = [self.encode_text(t) for t in texts]
-        txt_seq, lens, _pool, cond = model.prefill.run(ids, ref, n_frames=int(max_frames) + 1, style_strength=st)
         trace = None
         if trace_out is not None:
-            trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, len(texts), max(int(x) for x in lens), self.device)
-            trace_out["probs"], trace_out["lens"] = trace, [int(x) for x in lens]
-        toks, n = model.ar_generate_tensors(cond, txt_seq, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                            anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds,
-                                            attn_trace=trace, generator=generator)
-        eos, B = model.eos_id, len(texts)
-        Ts, stopped = [], []
-        for i in range(B):
-            row = toks[i, : n[i]]
-            hit = (row == eos).nonzero()[0]
-            Ts.append(int(hit[0]) if hit.size else int(n[i]))
-            stopped.append(bool(hit.size))
-        if info is not None:
-            info["stopped"], info["text_lens"] = stopped, [int(x) for x in lens]
-        Tmax = max(Ts)
-        if Tmax == 0:
-            return Ts, None
-        # NAR refiner over the ragged batch (not causal: `lens` makes the padding act as each utterance's zero padding)
-        rvq1 = torch.from_numpy(toks[:, :Tmax].copy()).to(self.device)
-        codes = model.nar_refine(cond[:, :Tmax], rvq1.clamp_(0, eos - 1), lens=torch.tensor(Ts, dtype=torch.int32))  # [B, Tmax, Q]
-        return Ts, codes
+            lens = [int(x.numel()) for x in ids]
+            trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, len(ids), max(lens), self.device)
+            trace_out["probs"], trace_out["lens"] = trace, lens
+        st = float(style_strength if style_strength is not None else self.cfg.style_strength)
+        return self.model.generate_codes(ids, ref, max_frames=max_frames, style_strength=st, attn_trace=trace, **kw)
 
     def _decode_chunks(self, codes: Optional[torch.Tensor], Ts: Sequence[int]) -> Iterator[Tuple[List[int], torch.Tensor, List[int]]]:
         """Padded Mimi decodes of the utterances with frames -> yields (indices, wav [rows, 1, L], valid samples per

@@ -75,6 +75,10 @@ class NarEngine:
     def refine(self, cond_btd: torch.Tensor, rvq1_bt: torch.Tensor, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """cond [B, T, D] f32 (any strides along batch; rows contiguous), rvq1 [B, T] ints, lens [B] or None."""
         B, T, D = cond_btd.shape
+        if lens is not None and lens.device.type == "cpu" and bool((lens == T).all()):
+            # the kernels mask only the positions at or past a row's length, so lengths of T change nothing; without
+            # them a one-row window replays its CUDA graph
+            lens = None
         out = torch.empty((B, T, self.Q), dtype=torch.int32, device=self.device)
         if B == 0 or T == 0:
             return out.long()

@@ -1,70 +1,49 @@
 """Chunked streaming synthesis (reference streaming.py:12-152): every ``chunk_frames`` AR tokens the NAR refiner
 runs over the new frames plus ``rf_nar`` frames of left context and the Mimi stream decoder emits their audio.
 The AR kernel is launched ``chunk_frames`` frames at a time, so time-to-first-audio is prefill + one short
-persistent launch + one NAR window + one Mimi decode."""
+persistent launch + one NAR window + one Mimi decode.
+
+``stream`` and ``stream_batch`` run one chunk loop (``_chunk_loop``), pipelined.  Per chunk k, in device order:
+AR(k) -> [NAR window + Mimi step](k) -> AR(k+1) -> ...  The host enqueues NAR + Mimi of chunk k on a side stream, then
+immediately enqueues AR(k+1) behind them (an event keeps the persistent kernel, which takes every SM, from cutting in
+front of chunk k's audio), and only then waits for chunk k's samples and yields them: the next AR launch runs while the
+consumer handles the audio, and the device never waits for the host between launches.  The reference runs the three
+stages strictly in turn on one thread (streaming.py:81-130)."""
 from __future__ import annotations
 
-from dataclasses import dataclass
 from typing import Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
-from .codec import MimiDecodeState, MimiStreamDecoder
+from .codec import MimiStreamDecoder
 from .output import OutputChain
 from .prefill import PreparedReference
 
 
-@dataclass
-class StreamConfig:
-    chunk_frames: int = 16
-    nar_context_frames: Optional[int] = None
-
-
-class SoproTTSStreamer:
-    """Pipelined chunk loop.  Per chunk k, in device order:  AR(k) -> [NAR window + Mimi step](k) -> AR(k+1) -> ...
-    The host enqueues NAR + Mimi of chunk k on a side stream, then immediately enqueues AR(k+1) behind them (an event
-    keeps the persistent kernel, which takes every SM, from cutting in front of chunk k's audio), and only then waits
-    for chunk k's samples and yields them: the next AR launch runs while the consumer handles the audio, and the device
-    never waits for the host between launches.  The reference runs the three stages strictly in turn on one thread
-    (streaming.py:81-130)."""
-
-    def __init__(self, tts, cfg: Optional[StreamConfig] = None):
-        self.tts = tts
-        self.cfg = cfg or StreamConfig()
-        # one decoder (= one pool of device stream states) per SoproTTS: a finished utterance's state is reset and reused by
-        # the next stream() instead of a 0.8 ms allocation + memset on the time-to-first-audio path
-        need = max(16, int(self.cfg.chunk_frames))
-        dec = getattr(tts, "_stream_decoder", None)
-        if dec is None or dec.max_chunk_frames < need or dec.codec is not tts.codec:
-            dec = MimiStreamDecoder(tts.codec, max_chunk_frames=need)
-            try:
-                tts._stream_decoder = dec
-            except Exception:
-                pass
-        self.mimi_stream = dec
+def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
+           ref: Optional[PreparedReference] = None, max_frames: int = 400, top_p: float = 0.9, temperature: float = 1.05,
+           anti_loop: bool = True, style_strength: Optional[float] = None, ref_seconds: Optional[float] = None,
+           chunk_frames: int = 6, nar_context_frames: Optional[int] = None, min_gen_frames: Optional[int] = None,
+           seed: Optional[int] = None, generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
+           speed: Optional[float] = None, watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
+    """SoproTTS.stream: the chunk loop over one text.  `sample_rate` (extension): chunks at this rate (None = 24 kHz).
+    `speed` (extension): the speaking rate in [0.25, 4.0] (None = the model's own).  `watermark` (extension): a key in
+    [0, 2^32) to mark the audio with (None = no mark).  Each chunk's audio goes through a time-stretch stream, a
+    watermark stream, then a resampler stream, right after its Mimi step, so the chunks concatenate to the one-shot
+    stretch, mark and resample of the 24 kHz stream bit for bit; the last chunk also carries their tails.  A refused
+    sample_rate / speed / watermark raises here, at the call, not at the first chunk."""
+    post = OutputChain(tts, sample_rate, speed, watermark=watermark)
+    dec = _decoder(tts, chunk_frames)
 
     @torch.inference_mode()
-    def stream(self, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
-               ref: Optional[PreparedReference] = None, max_frames: int = 400, top_p: float = 0.9, temperature: float = 1.05,
-               anti_loop: bool = True, style_strength: Optional[float] = None, ref_seconds: Optional[float] = None,
-               chunk_frames: Optional[int] = None, nar_context_frames: Optional[int] = None,
-               min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
-               generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
-               speed: Optional[float] = None, watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
-        """`sample_rate` (extension): chunks at this rate (None = 24 kHz).  `speed` (extension): the speaking rate in
-        [0.25, 4.0] (None = the model's own).  `watermark` (extension): a key in [0, 2^32) to mark the audio with (None =
-        no mark).  Each chunk's audio goes through a time-stretch stream, a watermark stream, then a resampler stream,
-        right after its Mimi step, so the chunks concatenate to the one-shot stretch, mark and resample of the 24 kHz
-        stream bit for bit; the last chunk also carries their tails."""
-        tts = self.tts
-        post = OutputChain(tts, sample_rate, speed, watermark=watermark)  # a refused argument raises before the prefill
-        text_ids = tts.encode_text(text)
-        if ref is None:
-            ref = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
-        rows = self.stream_rows([text_ids], ref, post, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                anti_loop=anti_loop, style_strength=style_strength, chunk_frames=chunk_frames,
-                                nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames,
-                                seeds=None if seed is None else [seed], generator=generator)
+    def chunks():
+        voice = ref
+        if voice is None:
+            voice = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
+        rows = _chunk_loop(tts, dec, [tts.encode_text(text)], voice, post, max_frames=max_frames, top_p=top_p,
+                           temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
+                           chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
+                           min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator)
         try:
             for _i, wav, _last in rows:
                 if wav is not None:
@@ -72,130 +51,7 @@ class SoproTTSStreamer:
         finally:
             rows.close()
 
-    @torch.inference_mode()
-    def stream_rows(self, text_ids: Sequence[torch.Tensor], ref, post: OutputChain, *, max_frames: int = 400,
-                    top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
-                    style_strength: Optional[float] = None, chunk_frames: Optional[int] = None,
-                    nar_context_frames: Optional[int] = None, min_gen_frames: Optional[int] = None,
-                    seeds: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None
-                    ) -> Iterator[Tuple[int, Optional[torch.Tensor], bool]]:
-        """The chunk loop of B utterances (`ref`: one prepared voice, or one per text) -> ``(i, wav or None, last)``:
-        per launch, in row order, each live row's chunk (None when it has no samples), the row's last item once with
-        last=True.  All rows advance in lockstep, `chunk_frames` AR frames per launch, so the NAR window [lo, end) is
-        shared by the live rows (only a row that ends in this launch has a shorter one) and runs as one ragged NAR pass;
-        one Mimi step decodes every row (a row that has ended is fed code 0 and its samples are dropped), then each row's
-        samples go through its own output-chain stream.  Row i's chunks are those of this loop over text i alone."""
-        tts, model = self.tts, self.tts.model
-        B = len(text_ids)
-        st_ = float(style_strength if style_strength is not None else tts.cfg.style_strength)
-        txt, lens, _pool, cond = model.prefill.run(list(text_ids), ref, n_frames=int(max_frames) + 1, style_strength=st_)
-        if B == 1:
-            txt = txt[:, : int(lens[0])]
-        cf = int(chunk_frames if chunk_frames is not None else self.cfg.chunk_frames)
-        ctx = nar_context_frames if nar_context_frames is not None else self.cfg.nar_context_frames
-        ctx = int(model.rf_nar() if ctx is None else ctx)
-        hop = tts.codec.engine.hop
-        hist: List[List[int]] = [[] for _ in range(B)]
-        ended = [False] * B
-        emitted = 0
-        state = self.mimi_stream.new_state(B)
-        # the stretch / resampler states' pushes are bounded by one chunk's samples
-        posts = []
-        on_gpu = tts.device.type == "cuda"
-        main = torch.cuda.current_stream(tts.device) if on_gpu else None
-        side = torch.cuda.Stream(tts.device) if on_gpu else None
-
-        def refine_and_emit(ends: List[int], last: List[bool], live: List[int]) -> List[Optional[torch.Tensor]]:
-            """NAR over the new frames + `ctx` frames of left context, Mimi stream step on the new frames' codes
-            (reference streaming.py:81-104), then each live row's stretch and resampler pushes (and, on its last chunk,
-            their finishes); enqueued on the side stream."""
-            nonlocal emitted, state
-            out: List[Optional[torch.Tensor]] = [None] * B
-            end = max(ends[b] for b in live)
-            rows_wav = None
-            if end > emitted:
-                lo = max(0, emitted - ctx)
-                if B == 1:
-                    toks = torch.as_tensor(hist[0][lo:end], device=tts.device, dtype=torch.long).unsqueeze(0)
-                    win = model.nar_refine(cond[:, lo:end, :], toks).squeeze(0)
-                    rows_wav, state = self.mimi_stream.decode_step(win[emitted - lo:, :], state, _trusted=True)  # our own NAR's codes
-                else:
-                    run = [b for b in live if ends[b] > emitted]
-                    W = end - lo
-                    toks = torch.zeros((len(run), W), dtype=torch.long)
-                    for j, b in enumerate(run):
-                        toks[j, : ends[b] - lo] = torch.as_tensor(hist[b][lo:ends[b]], dtype=torch.long)
-                    idx = torch.tensor(run, device=tts.device)
-                    win = model.nar_refine(cond[idx, lo:end, :], toks.to(tts.device),
-                                           lens=torch.tensor([ends[b] - lo for b in run], dtype=torch.int32))
-                    n = end - emitted
-                    keep = (torch.arange(n)[None, :] < torch.tensor([ends[b] - emitted for b in run])[:, None]).to(tts.device)
-                    codes = torch.zeros((B, n, win.shape[2]), dtype=torch.long, device=tts.device)
-                    codes[idx] = win[:, emitted - lo:, :] * keep[:, :, None]  # a finished row's frames decode code 0
-                    rows_wav, state = self.mimi_stream.decode_step(codes, state, _trusted=True)
-            for b in live:
-                wav = rows_wav[b: b + 1, : (ends[b] - emitted) * hop] if rows_wav is not None and ends[b] > emitted else None
-                wav = posts[b].finish(wav) if last[b] else posts[b].push(wav)
-                out[b] = wav if wav is not None and wav.numel() > 0 else None
-            emitted = end
-            return out
-
-        progress = {"consumed": 0}
-        chunks = model.ar_chunk_rows(cond, txt, lens, max_frames=max_frames, chunk_frames=cf, top_p=top_p,
-                                     temperature=temperature, anti_loop=anti_loop, min_gen_frames=min_gen_frames,
-                                     seeds=seeds, generator=generator, progress=progress)
-        try:
-            for _ in range(B):
-                posts.append(post.stream(self.mimi_stream.max_chunk_frames * hop))
-            for toks_rows, finished, prefetch in chunks:
-                live = [b for b in range(B) if not ended[b]]
-                ends, last = [0] * B, [False] * B
-                for b in live:
-                    toks = toks_rows[b]
-                    # the stream ends at the first EOS regardless of min_gen_frames (reference streaming.py:114-115)
-                    stop = model.eos_id in toks
-                    if stop:
-                        toks = toks[: toks.index(model.eos_id)]
-                    if B == 1:
-                        progress["consumed"] += len(toks) + (1 if stop else 0)  # the reference also draws for the EOS step
-                    hist[b].extend(toks)
-                    last[b] = stop or finished[b]
-                    ends[b] = len(hist[b]) if last[b] else (len(hist[b]) // cf) * cf
-                done = all(last[b] for b in live)
-                if on_gpu:
-                    side.wait_stream(main)
-                    with torch.cuda.stream(side):
-                        wavs = refine_and_emit(ends, last, live)
-                    if not done:
-                        main.wait_stream(side)  # AR(k+1) behind chunk k's NAR + Mimi, never in front of them
-                        prefetch()
-                    side.synchronize()
-                    for w in wavs:
-                        if w is not None:
-                            w.record_stream(main)
-                else:
-                    wavs = refine_and_emit(ends, last, live)
-                for b in live:
-                    if wavs[b] is not None or last[b]:
-                        yield b, wavs[b], last[b]
-                    ended[b] = last[b]
-                if done:
-                    break
-        finally:
-            chunks.close()
-            self.mimi_stream.release(state)
-            for p in posts:
-                p.release()
-
-
-@torch.inference_mode()
-def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
-           ref: Optional[PreparedReference] = None, chunk_frames: int = 6, sample_rate: Optional[int] = None,
-           speed: Optional[float] = None, watermark: Optional[int] = None, **kwargs) -> Iterator[torch.Tensor]:
-    OutputChain(tts, sample_rate, speed, watermark=watermark)  # a refused argument raises at the call, not at the first chunk
-    streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
-    return streamer.stream(text, ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref=ref,
-                           chunk_frames=chunk_frames, sample_rate=sample_rate, speed=speed, watermark=watermark, **kwargs)
+    return chunks()
 
 
 MAX_STREAM_ROWS = 256  # a Mimi stream state holds tens of MB per row (DESIGN.md §5o)
@@ -207,7 +63,7 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
                  nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
                  watermark: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor, bool]]:
     """SoproTTS.stream_batch: every argument is checked here, before any device work or random draw; the returned
-    generator runs SoproTTSStreamer.stream_rows over the texts."""
+    generator runs the chunk loop over the texts."""
     from . import voices
 
     if isinstance(texts, str) or not isinstance(texts, Sequence):
@@ -229,13 +85,13 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
     if not 1 <= chunk_frames <= 256:
         raise ValueError(f"chunk_frames must be in [1, 256], got {chunk_frames}")
     post = OutputChain(tts, sample_rate, speed, watermark=watermark)
-    streamer = SoproTTSStreamer(tts, StreamConfig(chunk_frames=chunk_frames))
+    dec = _decoder(tts, chunk_frames)
 
     def rows_of():
         ids = [tts.encode_text(t) for t in texts]
-        rows = streamer.stream_rows(ids, ref, post, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                    anti_loop=anti_loop, style_strength=style_strength, chunk_frames=chunk_frames,
-                                    nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames, seeds=seeds)
+        rows = _chunk_loop(tts, dec, ids, ref, post, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                           anti_loop=anti_loop, style_strength=style_strength, chunk_frames=chunk_frames,
+                           nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames, seeds=seeds)
         try:
             for i, wav, last in rows:
                 yield i, (wav if wav is not None else torch.zeros(1, 0, device=tts.device)), last
@@ -243,3 +99,119 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
             rows.close()
 
     return rows_of()
+
+
+def _decoder(tts, chunk_frames) -> MimiStreamDecoder:
+    """The SoproTTS's one stream decoder (one pool of device stream states: a finished utterance's state is reset and
+    reused by the next stream instead of a 0.8 ms allocation + memset on the time-to-first-audio path), made on first
+    use and replaced by a larger one when `chunk_frames` exceeds its chunk size."""
+    need = max(16, int(chunk_frames))
+    if tts._stream_decoder is None or tts._stream_decoder.max_chunk_frames < need:
+        tts._stream_decoder = MimiStreamDecoder(tts.codec, max_chunk_frames=need)
+    return tts._stream_decoder
+
+
+@torch.inference_mode()
+def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], ref, post: OutputChain, *,
+                max_frames: int, top_p: float, temperature: float, anti_loop: bool, style_strength: Optional[float],
+                chunk_frames: int, nar_context_frames: Optional[int], min_gen_frames: Optional[int],
+                seeds: Optional[Sequence[int]], generator: Optional[torch.Generator] = None
+                ) -> Iterator[Tuple[int, Optional[torch.Tensor], bool]]:
+    """The chunk loop of B utterances (`ref`: one prepared voice, or one per text) -> ``(i, wav or None, last)``:
+    per launch, in row order, each live row's chunk (None when it has no samples), the row's last item once with
+    last=True.  All rows advance in lockstep, `chunk_frames` AR frames per launch, so the NAR window [lo, end) is
+    shared by the live rows (only a row that ends in this launch has a shorter one) and runs as one ragged NAR pass;
+    one Mimi step decodes every row (a row that has ended is fed code 0 and its samples are dropped), then each row's
+    samples go through its own output-chain stream.  Row i's chunks are those of this loop over text i alone."""
+    model = tts.model
+    B = len(text_ids)
+    st_ = float(style_strength if style_strength is not None else tts.cfg.style_strength)
+    txt, lens, _pool, cond = model.prefill.run(list(text_ids), ref, n_frames=int(max_frames) + 1, style_strength=st_)
+    cf = int(chunk_frames)
+    ctx = int(model.rf_nar() if nar_context_frames is None else nar_context_frames)
+    hop = tts.codec.engine.hop
+    hist: List[List[int]] = [[] for _ in range(B)]
+    ended = [False] * B
+    emitted = 0
+    state = dec.new_state(B)
+    # the stretch / resampler states' pushes are bounded by one chunk's samples
+    posts = []
+    on_gpu = tts.device.type == "cuda"
+    main = torch.cuda.current_stream(tts.device) if on_gpu else None
+    side = torch.cuda.Stream(tts.device) if on_gpu else None
+
+    def refine_and_emit(ends: List[int], last: List[bool], live: List[int]) -> List[Optional[torch.Tensor]]:
+        """NAR over the new frames + `ctx` frames of left context, Mimi stream step on the new frames' codes
+        (reference streaming.py:81-104), then each live row's stretch and resampler pushes (and, on its last chunk,
+        their finishes); enqueued on the side stream."""
+        nonlocal emitted, state
+        out: List[Optional[torch.Tensor]] = [None] * B
+        end = max(ends[b] for b in live)
+        rows_wav = None
+        if end > emitted:
+            lo = max(0, emitted - ctx)
+            run = [b for b in live if ends[b] > emitted]
+            sel = slice(None) if len(run) == B else torch.tensor(run, device=tts.device)
+            toks = torch.tensor([hist[b][lo:ends[b]] + [0] * (end - ends[b]) for b in run], dtype=torch.long,
+                                device=tts.device)
+            win = model.nar_refine(cond[sel, lo:end, :], toks,
+                                   lens=torch.tensor([ends[b] - lo for b in run], dtype=torch.int32))
+            codes = win[:, emitted - lo:, :]
+            n = end - emitted
+            if any(e < end for e in ends):  # a row ended before this window's end: its frames decode code 0
+                keep = (torch.arange(n)[None, :] < torch.tensor([ends[b] - emitted for b in run])[:, None]).to(tts.device)
+                codes, part = torch.zeros((B, n, win.shape[2]), dtype=torch.long, device=tts.device), codes
+                codes[sel] = part * keep[:, :, None]
+            rows_wav, state = dec.decode_step(codes, state, _trusted=True)  # our own NAR's codes
+        for b in live:
+            wav = rows_wav[b: b + 1, : (ends[b] - emitted) * hop] if rows_wav is not None and ends[b] > emitted else None
+            wav = posts[b].finish(wav) if last[b] else posts[b].push(wav)
+            out[b] = wav if wav is not None and wav.numel() > 0 else None
+        emitted = end
+        return out
+
+    progress = {"consumed": 0}
+    chunks = model.ar_chunk_rows(cond, txt, lens, max_frames=max_frames, chunk_frames=cf, top_p=top_p,
+                                 temperature=temperature, anti_loop=anti_loop, min_gen_frames=min_gen_frames,
+                                 seeds=seeds, generator=generator, progress=progress)
+    try:
+        for _ in range(B):
+            posts.append(post.stream(dec.max_chunk_frames * hop))
+        for toks_rows, finished, prefetch in chunks:
+            live = [b for b in range(B) if not ended[b]]
+            ends, last = [0] * B, [False] * B
+            for b in live:
+                toks = toks_rows[b]
+                # the stream ends at the first EOS regardless of min_gen_frames (reference streaming.py:114-115)
+                stop = model.eos_id in toks
+                if stop:
+                    toks = toks[: toks.index(model.eos_id)]
+                progress["consumed"] += len(toks) + (1 if stop else 0)  # the reference also draws for the EOS step
+                hist[b].extend(toks)
+                last[b] = stop or finished[b]
+                ends[b] = len(hist[b]) if last[b] else (len(hist[b]) // cf) * cf
+            done = all(last[b] for b in live)
+            if on_gpu:
+                side.wait_stream(main)
+                with torch.cuda.stream(side):
+                    wavs = refine_and_emit(ends, last, live)
+                if not done:
+                    main.wait_stream(side)  # AR(k+1) behind chunk k's NAR + Mimi, never in front of them
+                    prefetch()
+                side.synchronize()
+                for w in wavs:
+                    if w is not None:
+                        w.record_stream(main)
+            else:
+                wavs = refine_and_emit(ends, last, live)
+            for b in live:
+                if wavs[b] is not None or last[b]:
+                    yield b, wavs[b], last[b]
+                ended[b] = last[b]
+            if done:
+                break
+    finally:
+        chunks.close()
+        dec.release(state)
+        for p in posts:
+            p.release()

@@ -75,6 +75,25 @@ def test_batch_without_seeds_consumes_the_global_generator_utterance_after_utter
         assert n > 0 and got["toks"][i, :n].tolist() == single[:n], i
 
 
+def test_synthesize_settles_the_generator_and_a_batch_of_one_does_not(tts):  # noqa: F811
+    """synthesize(t) leaves the global generator after the draws of its frames and the EOS step, as the reference
+    does; synthesize_batch([t]) draws every tape in full, as it does for any number of texts."""
+    text, V, steps = TEXTS[1], tts.cfg.ar_vocab(), KW["max_frames"] + 1
+    torch.manual_seed(17)
+    one = tts.synthesize(text, ref=tts.ref, **KW)
+    after_one = torch.get_rng_state()
+    torch.manual_seed(17)
+    (batch,) = tts.synthesize_batch([text], ref=tts.ref, **KW)
+    after_batch = torch.get_rng_state()
+    assert torch.equal(one, batch)
+    T = one.shape[-1] // 1920
+    assert T + 1 < steps, f"the case must stop at an EOS before max_frames, got {T} frames"
+    for drawn, state in ((T + 1, after_one), (steps, after_batch)):
+        torch.manual_seed(17)
+        torch.empty(drawn, V).exponential_(1.0)
+        assert torch.equal(torch.get_rng_state(), state), drawn
+
+
 def test_ar_stream_settles_the_passed_generator_to_the_consumed_frames(tts):  # noqa: F811
     prep = tts.model.prepare_conditioning(tts.encode_text(TEXTS[1]), tts.ref, max_frames=20,
                                           style_strength=tts.cfg.style_strength)
@@ -127,9 +146,9 @@ def launches(tts, monkeypatch):  # noqa: F811
 
 
 @pytest.mark.parametrize("chunk_frames, want", [(6, [6, 6, 6, 3]), (0, [21]), (25, [21])])
-def test_ar_chunks_launch_schedule(tts, launches, chunk_frames, want):  # noqa: F811
+def test_ar_stream_launch_schedule(tts, launches, chunk_frames, want):  # noqa: F811
     prep = {"cond_ar": torch.zeros(1, 21, 8), "txt_seq": torch.zeros(1, 4, 8)}
-    list(tts.model.ar_chunks(prep, max_frames=20, chunk_frames=chunk_frames, seed=1))
+    list(tts.model.ar_stream(prep, max_frames=20, launch_frames=chunk_frames, seed=1))
     assert launches == ["begin"] + want
 
 

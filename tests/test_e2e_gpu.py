@@ -119,8 +119,8 @@ def test_batch_synthesis_equals_single():
 
 
 def test_batch_synthesis_equals_single_across_noise_blocks():
-    """At 101 steps a seeded batch draws its tapes and launches in blocks of 24, 36 and 41 frames (synthesize runs one
-    launch); each utterance still equals synthesize(text, seed=s) bit for bit."""
+    """At 101 steps a seeded batch draws its tapes and launches in blocks of 24, 36 and 41 frames; each utterance still
+    equals synthesize(text, seed=s), a batch of one, bit for bit."""
     tts, _ = _tts()
     cfg, sd, inp = e2e_inputs()
     ref = tts.prepare_reference(ref_tokens_tq=inp["ref_tokens_tq"])

@@ -43,7 +43,7 @@ def test_prefill_and_nar_match_reference_fixtures():
 def test_api_surface_mirrors_the_reference():
     """Signatures of SURVEY.md §8b (reference model.py:419-428, 516-523, 531-546, 577-580; streaming.py:134-143)."""
     from sopro_b200 import SoproTTS
-    from sopro_b200.streaming import SoproTTSStreamer, stream
+    from sopro_b200.streaming import stream
 
     def params(f):
         return list(inspect.signature(f).parameters)
@@ -59,7 +59,7 @@ def test_api_surface_mirrors_the_reference():
     assert inspect.signature(stream).parameters["chunk_frames"].default == 6
     for name in ("encode_text", "encode_reference", "encode_speaker", "save_wav", "stream"):
         assert callable(getattr(SoproTTS, name))
-    assert "nar_context_frames" in params(SoproTTSStreamer.stream)
+    assert "nar_context_frames" in params(stream)
 
 
 def test_shared_library_exports_every_declared_symbol():

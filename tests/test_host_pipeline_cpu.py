@@ -228,6 +228,30 @@ def test_tokens_stop_at_first_eos_and_global_rng_is_settled(tts):
     assert torch.equal(a, b)
 
 
+def test_an_utterance_without_frames_is_empty_whatever_the_output_chain(tts):
+    """EOS at the first step: synthesize returns [1, 1, 0] for every combination of sample_rate, speed, loudness and
+    watermark, as synthesize_batch does for such a row."""
+    import copy
+    import itertools
+    import threading
+    import types
+
+    sd = dict(tts.model.engine.sd)
+    sd["ar.head.bias"] = sd["ar.head.bias"].clone()
+    sd["ar.head.bias"][int(tts.cfg.codebook_size)] += 100.0
+    t = copy.copy(tts)
+    t.model = copy.copy(tts.model)
+    t.model.engine = _FakeArEngine(tts.cfg, sd)
+    t.model._sessions, t.model._sessions_busy, t.model._sessions_lock = {}, set(), threading.Lock()
+    t._resampler = lambda sr: None if sr is None else types.SimpleNamespace(sr_out=int(sr))  # no CUDA tap table
+    for sr, speed, loudness, key in itertools.product((None, 16000), (None, 1.3), (None, -20.0), (None, 7)):
+        opts = dict(sample_rate=sr, speed=speed, loudness=loudness, watermark=key)
+        for seed in (None, 3):
+            wav = t.synthesize(TEXTS[0], ref=t.ref, seed=seed, **opts, **KW)
+            assert wav.shape == (1, 1, 0) and wav.dtype == torch.float32, (opts, seed)
+        assert [w.shape for w in t.synthesize_batch(TEXTS[:2], ref=t.ref, seeds=[1, 2], **opts, **KW)] == [(1, 1, 0)] * 2
+
+
 def test_stream_chunks_cover_the_utterance(tts):
     full = tts.synthesize(TEXTS[1], ref=tts.ref, seed=2, **KW)
     T = full.shape[-1] // 1920

@@ -91,12 +91,12 @@ def test_workspace_is_host_arithmetic():
 
 def test_loudness_keyword_defaults_to_none_and_stream_has_none():
     from sopro_b200 import SoproTTS
-    from sopro_b200.streaming import SoproTTSStreamer, stream
+    from sopro_b200.streaming import stream
 
     for f in (SoproTTS.synthesize, SoproTTS.synthesize_batch):
         p = inspect.signature(f).parameters["loudness"]
         assert p.default is None and p.kind == inspect.Parameter.KEYWORD_ONLY, f
-    for f in (SoproTTS.stream, SoproTTSStreamer.stream, stream):
+    for f in (SoproTTS.stream, stream):
         assert "loudness" not in inspect.signature(f).parameters, f
 
 

@@ -85,8 +85,8 @@ def test_public_prepare_conditioning_feeds_the_ar_kernel():
     prep = tts.model.prepare_conditioning(inp["text_ids"], ref, max_frames=40, style_strength=1.0)
     assert set(prep) == {"txt_seq", "text_mask", "txt_pool", "sv_ref", "cond_ar"}
     assert prep["txt_seq"].shape == (1, 52, 384) and prep["cond_ar"].shape == (1, 41, 384) and prep["text_mask"].all()
-    many = tts.model.prepare_conditioning_batch([inp["text_ids"], inp["text_ids"][:9]], ref, max_frames=40, style_strength=1.0)
-    assert torch.equal(many[0]["cond_ar"], prep["cond_ar"]) and many[1]["txt_seq"].shape == (1, 9, 384)
+    txt, lens, _pool, cond = tts.model.prefill.run([inp["text_ids"], inp["text_ids"][:9]], ref, n_frames=41, style_strength=1.0)
+    assert torch.equal(cond[0:1], prep["cond_ar"]) and torch.equal(txt[0:1], prep["txt_seq"]) and lens == [52, 9]
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -71,9 +71,9 @@ def test_identical_rates_and_bad_lengths_are_refused():
 
 def test_sample_rate_keyword_defaults_to_none():
     from sopro_b200 import SoproTTS
-    from sopro_b200.streaming import SoproTTSStreamer, stream
+    from sopro_b200.streaming import stream
 
-    for f in (SoproTTS.synthesize, SoproTTS.synthesize_batch, SoproTTS.stream, SoproTTSStreamer.stream, stream):
+    for f in (SoproTTS.synthesize, SoproTTS.synthesize_batch, SoproTTS.stream, stream):
         p = inspect.signature(f).parameters["sample_rate"]
         assert p.default is None and p.kind == inspect.Parameter.KEYWORD_ONLY, f
     assert inspect.signature(SoproTTS.save_wav).parameters["sample_rate"].default == 24000

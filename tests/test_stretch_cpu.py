@@ -100,9 +100,9 @@ def test_largest_api_size():
 
 def test_speed_keyword_defaults_to_none():
     from sopro_b200 import SoproTTS
-    from sopro_b200.streaming import SoproTTSStreamer, stream
+    from sopro_b200.streaming import stream
 
-    for f in (SoproTTS.synthesize, SoproTTS.synthesize_batch, SoproTTS.stream, SoproTTSStreamer.stream, stream):
+    for f in (SoproTTS.synthesize, SoproTTS.synthesize_batch, SoproTTS.stream, stream):
         p = inspect.signature(f).parameters["speed"]
         assert p.default is None and p.kind == inspect.Parameter.KEYWORD_ONLY, f
 

@@ -242,18 +242,18 @@ def test_synthesize_word_timestamps():
     for extra in ({}, dict(speed=1.3), dict(sample_rate=16000, loudness=-20.0)):
         plain = tts.synthesize(TEXT, ref=ref, seed=5, **KW, **extra)
         captured = {}
-        real = tts.model.generate_tokens
+        real = tts._batch_codes
 
         def spy(*a, **k):
             out = real(*a, **k)
-            captured["trace"], captured["T"] = k["attn_trace"].clone(), int(out.shape[0])
+            captured["trace"], captured["T"] = k["trace_out"]["probs"].clone(), int(out[0][0])
             return out
 
-        tts.model.generate_tokens = spy
+        tts._batch_codes = spy
         try:
             wav, words = tts.synthesize(TEXT, ref=ref, seed=5, word_timestamps=True, **KW, **extra)
         finally:
-            tts.model.generate_tokens = real
+            tts._batch_codes = real
         assert torch.equal(wav, plain)
         _ids, spans = tts.tokenizer.encode_with_offsets(TEXT)
         p = captured["trace"].cpu().numpy()
@@ -309,18 +309,17 @@ def test_synthesize_batch_word_timestamps():
             assert len(words[i]) == len(t.split())
     # the batch trace against a single call's trace (team geometry may reorder fp32 sums)
     one = {}
-    real_g = tts.model.generate_tokens
 
     def spy1(*a, **k):
-        out = real_g(*a, **k)
-        one["trace"] = k["attn_trace"].clone()
+        out = real(*a, **k)
+        one["trace"] = k["trace_out"]["probs"].clone()
         return out
 
-    tts.model.generate_tokens = spy1
+    tts._batch_codes = spy1
     try:
         tts.synthesize(texts[0], ref=ref, seed=seeds[0], word_timestamps=True, **KW)
     finally:
-        tts.model.generate_tokens = real_g
+        tts._batch_codes = real
     a = one["trace"][:, :, 0].cpu()
     L0 = captured["lens"][0]
     b = captured["probs"][:, :, 0, :, :L0].cpu()

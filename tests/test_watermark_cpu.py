@@ -147,10 +147,10 @@ def test_the_library_refuses_keys_and_geometry():
 def test_the_public_api_takes_a_watermark_key():
     from sopro_b200 import detect_watermark
     from sopro_b200.model import SoproTTS
-    from sopro_b200.streaming import SoproTTSStreamer
+    from sopro_b200.streaming import stream
 
     for fn in (SoproTTS.synthesize, SoproTTS.synthesize_batch, SoproTTS.synthesize_long, SoproTTS.stream,
-               SoproTTSStreamer.stream):
+               stream):
         p = inspect.signature(fn).parameters["watermark"]
         assert p.default is None and p.kind is inspect.Parameter.KEYWORD_ONLY
     assert list(inspect.signature(detect_watermark).parameters) == ["wav", "sample_rate", "key", "lens"]

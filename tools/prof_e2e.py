@@ -81,7 +81,7 @@ with torch.inference_mode():
     # synthesize_batch(64) phases
     texts = [" ".join(str((17 * i + 5 + 31 * j) % 1000) for i in range(50)) for j in range(64)]
     ids64 = [tts.encode_text(x) for x in texts]
-    t, preps = timed(lambda: tts.model.prepare_conditioning_batch(ids64, ref, max_frames=400, style_strength=cfg.style_strength), n=3, warm=1)
+    t, _ = timed(lambda: tts.model.prefill.run(ids64, ref, n_frames=401, style_strength=cfg.style_strength), n=3, warm=1)
     print(f"prefill batch 64       {t:8.3f} ms")
     from sopro_b200.sampling import TapeFeed
 

@@ -802,6 +802,44 @@ int sopro_longform_extents(const float* x, int32_t B, int64_t x_stride, const in
  * geometry is SOPRO_ERR_INVALID before any launch.  No call synchronises or allocates. */
 int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host, int64_t pause,
                         float* y, int64_t y_len, void* stream);
+/* Streaming trim: the extent of a row decided while its samples arrive, and the join emitted piece by piece.
+ *   Causal rule: frame k (complete once 240 k + 600 samples have arrived) is classified once, when it completes, against
+ *   thr_k = max(M_k - 40, -40), M_k the largest dB among frames 0 .. k; an earlier decision is never revisited.  When
+ *   no frame of the row is above 0 dB (M <= 0) every thr_k is -40, the one-shot threshold, so the final extent is the
+ *   one-shot extent above and the emitted pieces concatenate to the join bit for bit.  Louder rows get the causal
+ *   rule's extent, which can start earlier than the one-shot one.
+ *   Certain prefix: with f and l the first and last voiced frame so far and n the samples so far, start =
+ *   max(0, 240 f - 720) and end_p = min(n, 240 l + 1320).  end_p only grows and start is fixed once f is, so once
+ *   end_p - start >= 12000 the row is certain to be trimmed to a span of at least 12000 samples, F = 240, and
+ *   [start, end_p - 240) is beyond the reach of its fade-out: that is the available bound.  Before that nothing is
+ *   available.  When the row is final its extent is the one-shot rule's over its n samples (the whole row when
+ *   n < 2400, nothing is voiced or the span is under 12000), and all of it is available.
+ *   Status, per row i64 [5]: n, decided (start is known), start, the available bound (0 when undecided; the extent's
+ *   end once final), final.
+ * A state holds `rows` rows of at most max_len samples each on the device (rows <= 256, max_len <= 2^31); create
+ * allocates and synchronises, and no other call does either.  Calls on one state are ordered on one CUDA stream, or
+ * ordered by the caller. */
+typedef struct sopro_longform_stream sopro_longform_stream_t;
+int sopro_longform_stream_create(int32_t rows, int64_t max_len, int device, sopro_longform_stream_t** out);
+int sopro_longform_stream_destroy(sopro_longform_stream_t* s);
+/* rows [row0, row0 + n_rows) back to no samples (one launch) */
+int sopro_longform_stream_reset(sopro_longform_stream_t* s, int32_t row0, int32_t n_rows, void* stream);
+/* one launch for rows [row0, row0 + n_rows): row row0 + i appends counts_host[i] (HOST i64; 0 = the row did not run)
+ * samples from x + i * x_stride (device f32), classifies its newly complete frames, and becomes final when
+ * final_host[i] (HOST i32) is non-zero; then its status is written on the device.  A count past the capacity, a push
+ * to a final row, or x_stride below the largest count (when n_rows > 1) is SOPRO_ERR_INVALID before any launch. */
+int sopro_longform_stream_push(sopro_longform_stream_t* s, const float* x, int64_t x_stride, int32_t row0, int32_t n_rows,
+                               const int64_t* counts_host, const int32_t* final_host, void* stream);
+/* the status rows [row0, row0 + n_rows) -> status_host (HOST i64 [n_rows][5], pinned for an asynchronous copy) */
+int sopro_longform_stream_status(const sopro_longform_stream_t* s, int32_t row0, int32_t n_rows, int64_t* status_host,
+                                 void* stream);
+/* pieces_host: HOST i64 [n_pieces][5] = (row, a, b, start, end); y (device f32, y_len = the pieces' total) receives,
+ * back to back, samples [a, b) of the row's span [start, end) as the join writes them (fade-in over the span's first F
+ * samples, fade-out over its last F, F = min(240, (end - start) / 2)), or, for end = -1, of a span whose end is not
+ * known yet (F = 240, no fade-out: b must lie within the available bound); row = -1 is b - a pause zeros (a = 0).
+ * Pieces outside the samples pushed are SOPRO_ERR_INVALID before any launch.  One launch per 48 pieces. */
+int sopro_longform_stream_emit(const sopro_longform_stream_t* s, const int64_t* pieces_host, int32_t n_pieces, float* y,
+                               int64_t y_len, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Lossless FLAC output (RFC 9639; no reference counterpart: the reference's demo sends PCM16): mono, 16 bits per sample,

@@ -144,6 +144,156 @@ void fade(int F, float* f) {
 
 int fade_len(long long span) { return (int)std::min<long long>(kFadeMax, span / 2); }
 
+// ---- the streaming trim (include/sopro_b200.h): each row's samples as they are decoded, its frames classified once
+// under the causal threshold, and the certain prefix of its extent published after every push.
+// push_kernel: one CTA per row.  The CTA appends the row's new samples to its buffer, then, after a barrier, computes
+// the newly complete frames in rounds of kPushRound, one warp per frame through frame_db (so every dB equals the
+// one-shot kernel's), and one thread walks the round in frame order updating M, first and last.  Each frame reads only
+// samples of its own row that are stored before the barrier by this CTA or by an earlier launch; no load of the row's
+// buffer precedes the barrier, so the read-only path never holds a line older than the stores.
+// emit_kernel: grid (pieces, items); a piece is a run of a span (faded as join_kernel fades it) or of pause zeros.
+constexpr int kMaxStreamRows = 256;     // rows of one state (their counts travel as a kernel parameter)
+constexpr int kPushRound = 256;         // frames per classification round
+constexpr int kEmitPieces = 48;         // pieces of one emit launch
+constexpr long long kMaxStreamLen = 1LL << 31;
+constexpr long long kNoTail = 1LL << 62;
+
+struct TrimRow {
+  long long n;      // samples appended
+  long long K;      // complete frames classified
+  long long first, last;  // voiced frames (-1: none)
+  double M;         // the largest dB among frames 0 .. K-1
+  int final_;
+};
+
+// status row: n, decided, start, available bound, final (see the header)
+constexpr int kStatus = 5;
+
+struct PushArgs {
+  long long count[kMaxStreamRows];
+  unsigned char fin[kMaxStreamRows];
+};
+static_assert(sizeof(PushArgs) <= 4000, "the push's arguments fit the kernel parameter space");
+
+__global__ void trim_reset_kernel(TrimRow* __restrict__ rows, long long* __restrict__ status, int n_rows) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= n_rows) return;
+  rows[b] = TrimRow{0, 0, -1, -1, -INFINITY, 0};
+  for (int i = 0; i < kStatus; ++i) status[kStatus * b + i] = 0;
+}
+
+__global__ void __launch_bounds__(kExtThreads) push_kernel(const float* __restrict__ x, long long x_stride, const PushArgs a,
+                                                           float* __restrict__ buf, long long cap, TrimRow* __restrict__ rows,
+                                                           long long* __restrict__ status) {
+  __shared__ double db[kPushRound];
+  __shared__ TrimRow s;
+  const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* xb = buf + (long long)b * cap;
+  if (threadIdx.x == 0) s = rows[b];
+  __syncthreads();
+  const long long n0 = s.n, cnt = a.count[b], n = n0 + cnt;
+  const float* src = x + (long long)b * x_stride;
+  for (long long i = threadIdx.x; i < cnt; i += kExtThreads) xb[n0 + i] = src[i];
+  __syncthreads();
+  const long long K = n >= kFrame ? (n - kFrame) / kHop + 1 : 0;
+  for (long long k0 = s.K; k0 < K; k0 += kPushRound) {
+    const int m = (int)std::min<long long>(kPushRound, K - k0);
+    for (int j = warp; j < m; j += kExtWarps) {
+      const double v = frame_db(xb, k0 + j, lane);
+      if (lane == 0) db[j] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int j = 0; j < m; ++j) {  // frame k against thr_k = max(M_k - 40, -40), M_k over frames 0 .. k
+        s.M = fmax(s.M, db[j]);
+        if (db[j] > fmax(s.M - 40.0, -40.0)) {
+          if (s.first < 0) s.first = k0 + j;
+          s.last = k0 + j;
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    s.n = n;
+    s.K = K;
+    s.final_ = s.final_ | a.fin[b];
+    long long decided = 0, start = 0, avail = 0;
+    const long long st = std::max(0LL, s.first * kHop - kPad);
+    const long long end = s.last >= 0 ? std::min(n, s.last * kHop + kFrame + kPad) : 0;
+    if (s.final_) {
+      decided = 1;
+      start = st;
+      avail = end;
+      if (n < kMinRow || s.last < 0 || end - st < kMinKeep) start = 0, avail = n;
+    } else if (s.last >= 0 && end - st >= kMinKeep) {
+      decided = 1;
+      start = st;
+      avail = end - kFadeMax;  // the fade-out may only touch the last 240 samples of the final extent
+    }
+    rows[b] = s;
+    long long* o = status + kStatus * b;
+    o[0] = n;
+    o[1] = decided;
+    o[2] = start;
+    o[3] = avail;
+    o[4] = s.final_;
+  }
+}
+
+struct EmitPiece {
+  const float* src;  // the row's buffer + the span's start; null for pause zeros
+  long long j0, len, off;
+  long long tail;    // span - F: the fade-out's first position (kNoTail while the span's end is unknown)
+  int F;
+};
+
+struct EmitArgs {
+  int n;
+  EmitPiece p[kEmitPieces];
+};
+static_assert(sizeof(EmitArgs) <= 4000, "the emit's arguments fit the kernel parameter space");
+
+__global__ void __launch_bounds__(kJoinThreads) emit_kernel(const EmitArgs a, const float* __restrict__ fades, float* __restrict__ y) {
+  const EmitPiece p = a.p[blockIdx.y];
+  const float* f = fades + (long long)p.F * (p.F - 1) / 2;  // the table of fade length F
+  float* yo = y + p.off;
+  for (long long i = (long long)blockIdx.x * kJoinThreads + threadIdx.x; i < p.len; i += (long long)gridDim.x * kJoinThreads) {
+    float v = 0.0f;
+    if (p.src) {
+      const long long j = p.j0 + i;
+      v = p.src[j];
+      if (j < p.F)
+        v = __fmul_rn(v, __ldg(f + j));
+      else if (j >= p.tail)
+        v = __fmul_rn(v, __ldg(f + (p.tail + p.F - 1 - j)));
+    }
+    yo[i] = v;
+  }
+}
+
+}  // namespace
+
+struct sopro_longform_stream {
+  int rows = 0, device = 0;
+  long long cap = 0;
+  float* buf = nullptr;       // [rows][cap]
+  float* fades = nullptr;     // the fade tables of F = 1 .. 240, back to back
+  TrimRow* state = nullptr;   // [rows]
+  long long* status = nullptr;  // [rows][5]
+  std::vector<long long> n;   // host mirror of the samples pushed per row
+  std::vector<char> fin;      // host mirror of the final flags
+};
+
+namespace {
+
+int check_rows_range(const sopro_longform_stream* s, int row0, int n_rows) {
+  if (!s) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (row0 < 0 || n_rows < 1 || row0 + n_rows > s->rows)
+    return fail(SOPRO_ERR_INVALID, "rows [%d, %d) not inside the state's %d rows", row0, row0 + n_rows, s->rows);
+  return SOPRO_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -237,6 +387,169 @@ int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* l
       const int r = launch();
       if (r != SOPRO_OK) return r;
     }
+  }
+  return SOPRO_OK;
+}
+
+int sopro_longform_stream_destroy(sopro_longform_stream_t* s) {
+  if (!s) return SOPRO_OK;
+  cudaFree(s->buf);
+  cudaFree(s->fades);
+  cudaFree(s->state);
+  cudaFree(s->status);
+  delete s;
+  return SOPRO_OK;
+}
+
+int sopro_longform_stream_create(int32_t rows, int64_t max_len, int device, sopro_longform_stream_t** out) {
+  if (!out) return fail(SOPRO_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (rows < 1 || rows > kMaxStreamRows) return fail(SOPRO_ERR_INVALID, "rows = %d not in [1, %d]", rows, kMaxStreamRows);
+  if (max_len < 1 || max_len > kMaxStreamLen)
+    return fail(SOPRO_ERR_INVALID, "max_len = %lld not in [1, 2^31]", (long long)max_len);
+  const int rc = open_device(device, "the streaming trim");
+  if (rc != SOPRO_OK) return rc;
+  auto* s = new sopro_longform_stream;
+  s->rows = rows;
+  s->device = device;
+  s->cap = (max_len + 31) / 32 * 32;  // every row starts on a 128-byte line
+  s->n.assign(rows, 0);
+  s->fin.assign(rows, 0);
+  std::vector<float> fades((size_t)kFadeMax * (kFadeMax + 1) / 2);
+  for (int F = 1; F <= kFadeMax; ++F) fade(F, fades.data() + (size_t)F * (F - 1) / 2);
+  const cudaError_t e[] = {cudaMalloc(&s->buf, sizeof(float) * (size_t)rows * s->cap),
+                           cudaMalloc(&s->fades, sizeof(float) * fades.size()),
+                           cudaMalloc(&s->state, sizeof(TrimRow) * rows),
+                           cudaMalloc(&s->status, sizeof(long long) * kStatus * rows)};
+  for (cudaError_t ei : e)
+    if (ei != cudaSuccess) {
+      sopro_longform_stream_destroy(s);
+      return fail(SOPRO_ERR_CUDA, "cudaMalloc failed: %s (streaming trim of %d rows x %lld samples)", cudaGetErrorString(ei),
+                  rows, (long long)max_len);
+    }
+  cudaError_t ec = cudaMemcpy(s->fades, fades.data(), sizeof(float) * fades.size(), cudaMemcpyHostToDevice);
+  if (ec == cudaSuccess) {
+    trim_reset_kernel<<<(rows + 127) / 128, 128>>>(s->state, s->status, rows);
+    ec = cudaGetLastError();
+  }
+  if (ec == cudaSuccess) ec = cudaDeviceSynchronize();
+  if (ec != cudaSuccess) {
+    sopro_longform_stream_destroy(s);
+    return fail(SOPRO_ERR_CUDA, "streaming trim set-up failed: %s", cudaGetErrorString(ec));
+  }
+  *out = s;
+  return SOPRO_OK;
+}
+
+int sopro_longform_stream_reset(sopro_longform_stream_t* s, int32_t row0, int32_t n_rows, void* stream) {
+  const int rc = check_rows_range(s, row0, n_rows);
+  if (rc != SOPRO_OK) return rc;
+  trim_reset_kernel<<<(n_rows + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(s->state + row0,
+                                                                                            s->status + kStatus * row0, n_rows);
+  CK(cudaGetLastError());
+  for (int b = row0; b < row0 + n_rows; ++b) s->n[b] = 0, s->fin[b] = 0;
+  return SOPRO_OK;
+}
+
+int sopro_longform_stream_push(sopro_longform_stream_t* s, const float* x, int64_t x_stride, int32_t row0, int32_t n_rows,
+                               const int64_t* counts_host, const int32_t* final_host, void* stream) {
+  int rc = check_rows_range(s, row0, n_rows);
+  if (rc != SOPRO_OK) return rc;
+  if (!counts_host || !final_host) return fail(SOPRO_ERR_INVALID, "null argument");
+  PushArgs a{};
+  long long most = 0;
+  for (int i = 0; i < n_rows; ++i) {
+    const int b = row0 + i;
+    const long long c = counts_host[i];
+    if (c < 0 || c > s->cap - s->n[b])
+      return fail(SOPRO_ERR_INVALID, "row %d: %lld samples after %lld exceed the capacity %lld", b, c, s->n[b], s->cap);
+    if (s->fin[b] && (c > 0 || final_host[i]))
+      return fail(SOPRO_ERR_INVALID, "row %d is final: it takes no more samples until a reset", b);
+    a.count[i] = c;
+    a.fin[i] = final_host[i] ? 1 : 0;
+    most = std::max(most, c);
+  }
+  if (most > 0 && !x) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (n_rows > 1 && x_stride < most)
+    return fail(SOPRO_ERR_INVALID, "x_stride %lld < the largest count %lld", (long long)x_stride, most);
+  push_kernel<<<n_rows, kExtThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, x_stride, a, s->buf + (long long)row0 * s->cap, s->cap, s->state + row0, s->status + kStatus * row0);
+  CK(cudaGetLastError());
+  for (int i = 0; i < n_rows; ++i) {
+    s->n[row0 + i] += a.count[i];
+    s->fin[row0 + i] |= (char)a.fin[i];
+  }
+  return SOPRO_OK;
+}
+
+int sopro_longform_stream_status(const sopro_longform_stream_t* s, int32_t row0, int32_t n_rows, int64_t* status_host,
+                                 void* stream) {
+  const int rc = check_rows_range(s, row0, n_rows);
+  if (rc != SOPRO_OK) return rc;
+  if (!status_host) return fail(SOPRO_ERR_INVALID, "null argument");
+  CK(cudaMemcpyAsync(status_host, s->status + kStatus * row0, sizeof(long long) * kStatus * n_rows, cudaMemcpyDeviceToHost,
+                     reinterpret_cast<cudaStream_t>(stream)));
+  return SOPRO_OK;
+}
+
+int sopro_longform_stream_emit(const sopro_longform_stream_t* s, const int64_t* pieces_host, int32_t n_pieces, float* y,
+                               int64_t y_len, void* stream) {
+  if (!s || !pieces_host) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (n_pieces < 0) return fail(SOPRO_ERR_INVALID, "n_pieces = %d < 0", n_pieces);
+  long long total = 0;
+  for (int i = 0; i < n_pieces; ++i) {
+    const int64_t* q = pieces_host + 5 * i;
+    const long long row = q[0], a = q[1], b = q[2], st = q[3], e = q[4];
+    if (row < -1 || row >= s->rows) return fail(SOPRO_ERR_INVALID, "piece %d: row %lld not in [-1, %d)", i, row, s->rows);
+    if (row == -1) {
+      if (a != 0 || b < 0 || b > kMaxPause) return fail(SOPRO_ERR_INVALID, "piece %d: a pause of [%lld, %lld)", i, a, b);
+    } else {
+      const long long n = s->n[row];
+      if (st < 0 || st > a || a > b || b > n || (e >= 0 && (e < b || e > n)) || e < -1)
+        return fail(SOPRO_ERR_INVALID, "piece %d: samples [%lld, %lld) of the span [%lld, %lld) of row %lld (%lld pushed)", i, a,
+                    b, st, e, row, n);
+    }
+    total += b - a;
+  }
+  if (y_len != total) return fail(SOPRO_ERR_INVALID, "y_len = %lld, the pieces hold %lld", (long long)y_len, total);
+  if (total == 0) return SOPRO_OK;
+  if (!y) return fail(SOPRO_ERR_INVALID, "null argument");
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  EmitArgs args{};
+  long long most = 0, off = 0;
+  for (int i = 0; i < n_pieces; ++i) {
+    const int64_t* q = pieces_host + 5 * i;
+    const long long row = q[0], len = q[2] - q[1];
+    if (len == 0) continue;
+    EmitPiece& p = args.p[args.n++];
+    p.len = len;
+    p.off = off;
+    off += len;
+    if (row < 0) {
+      p.src = nullptr;
+      p.j0 = 0;
+      p.tail = kNoTail;
+      p.F = 0;
+    } else {
+      const long long start = q[3], end = q[4];
+      p.src = s->buf + row * s->cap + start;
+      p.j0 = q[1] - start;
+      p.F = end < 0 ? kFadeMax : fade_len(end - start);  // an undecided end belongs to a span of >= 12000 samples
+      p.tail = end < 0 ? kNoTail : end - start - p.F;
+    }
+    most = std::max(most, len);
+    if (args.n == kEmitPieces) {
+      const unsigned gx = (unsigned)std::min<long long>((most + kJoinThreads - 1) / kJoinThreads, 1024);
+      emit_kernel<<<dim3(gx, args.n), kJoinThreads, 0, st>>>(args, s->fades, y);
+      CK(cudaGetLastError());
+      args.n = 0;
+      most = 0;
+    }
+  }
+  if (args.n > 0) {
+    const unsigned gx = (unsigned)std::min<long long>((most + kJoinThreads - 1) / kJoinThreads, 1024);
+    emit_kernel<<<dim3(gx, args.n), kJoinThreads, 0, st>>>(args, s->fades, y);
+    CK(cudaGetLastError());
   }
   return SOPRO_OK;
 }

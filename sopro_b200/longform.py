@@ -12,7 +12,7 @@ import ctypes as C
 import math
 import numbers
 import re
-from typing import List, Optional, Sequence, Union
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -210,3 +210,165 @@ def join_segments(rows_or_chunks: Union[torch.Tensor, Sequence[torch.Tensor]], e
         _lib.check_arg(_lib.load().sopro_longform_join(src, n, lens, ext.ctypes.data, P, y.data_ptr() if N else None, N,
                                                        _lib.stream_ptr(dev)))
     return y
+
+
+# ---- the streaming trim and join (SoproTTS.stream_long)
+
+class StreamJoin:
+    """The streaming form of speech_extents + join_segments over one passage's segments, as their rows are decoded
+    (the causal rule and the certain prefix: include/sopro_b200.h).  The device state holds the rows of at most two
+    groups of `group` segments, segment i in slot (i // group) % 2, so one group can be emitted while the next one is
+    generated; its buffers take rows x max_len x 4 bytes.
+
+    ``begin`` starts a passage, ``start_group`` a group's rows (on the current stream), ``push`` appends one chunk-loop
+    launch's decoded block and copies the status into pinned host memory (both on the current stream, with no host
+    synchronisation: the reader synchronises that stream before ``take``), and ``take`` emits the next piece of the
+    joined passage that is certain, at most `limit` samples, pause zeros included.  The pause before a span goes out
+    only once that span has samples to follow it.  Allocation happens at construction only, so a pooled state serves the
+    next passage without allocating on its first-item path."""
+
+    def __init__(self, rows: int, max_len: int, device):
+        self.device = torch.device(device)
+        self.rows, self.max_len = int(rows), int(max_len)
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _lib.check_arg(_lib.load().sopro_longform_stream_create(self.rows, self.max_len, self.device.index, C.byref(h)))
+        self._h = h.value
+        self._status = torch.zeros((self.rows, 5), dtype=torch.int64, pin_memory=True)
+        self._st = self._status.numpy()
+        self.begin(1, 0, 1)
+
+    @staticmethod
+    def rows_for(segments: int, group: int) -> int:
+        """Device rows a passage of `segments` needs: one group's worth, or two slots of `group`."""
+        return int(segments) if segments <= group else 2 * int(group)
+
+    def begin(self, segments: int, pause: int, group: int) -> None:
+        if self.rows_for(segments, group) > self.rows:
+            raise ValueError(f"{segments} segments in groups of {group} need {self.rows_for(segments, group)} rows, "
+                             f"the state has {self.rows}")
+        self.B, self.P, self.G = int(segments), int(pause), int(group)
+        self.cur, self.pos, self.pause_left, self.spans = 0, -1, 0, 0  # the segment being emitted, its next sample
+        self.started = 0           # segments [0, started) have begun
+        self.row0 = self.n_rows = 0  # the rows the pushes go to
+        self.pushes = 0
+
+    def _row(self, seg: int) -> int:
+        return seg if self.B <= self.G else ((seg // self.G) % 2) * self.G + seg % self.G
+
+    def can_start(self, g0: int) -> bool:
+        """Whether the slot of the group starting at segment g0 is free: the group it held has been emitted."""
+        return g0 < self.B and g0 == self.started and self.cur >= g0 - self.G
+
+    def start_group(self, g0: int, n: int) -> None:
+        """Segments [g0, g0 + n) take their slot's rows, reset on the current stream."""
+        if not self.can_start(g0):
+            raise _lib.SoproError(f"the group at segment {g0} cannot start yet")
+        self.row0, self.n_rows = self._row(g0), int(n)
+        self._st[self.row0: self.row0 + self.n_rows] = 0  # (no copy into them is in flight: their last one was read)
+        _lib.check_arg(_lib.load().sopro_longform_stream_reset(self._h, self.row0, self.n_rows, _lib.stream_ptr(self.device)))
+        self.started = g0 + int(n)
+
+    def push(self, wav: Optional[torch.Tensor], counts: Sequence[int], final: Sequence[bool]) -> None:
+        """One launch's block: wav [n_rows, L] f32 on the device (None when no row has samples), counts[i] new samples
+        of the group's row i (0 = it did not run), final[i] when the row ends with this push."""
+        n = self.n_rows
+        if len(counts) != n or len(final) != n:
+            raise ValueError(f"{len(counts)} counts and {len(final)} flags for {n} rows")
+        if wav is not None:
+            wav = wav.detach().reshape(n, -1)
+            if wav.dtype != torch.float32 or (wav.numel() and wav.stride(-1) != 1):
+                wav = wav.to(torch.float32).contiguous()
+        cnt = (C.c_int64 * n)(*[int(c) for c in counts])
+        fin = (C.c_int32 * n)(*[1 if f else 0 for f in final])
+        lib, st = _lib.load(), _lib.stream_ptr(self.device)
+        _lib.check_arg(lib.sopro_longform_stream_push(self._h, wav.data_ptr() if wav is not None and wav.numel() else None,
+                                                      int(wav.stride(0)) if wav is not None else 0, self.row0, n, cnt, fin, st))
+        _lib.check_arg(lib.sopro_longform_stream_status(self._h, self.row0, n, self._status[self.row0].data_ptr(), st))
+        self.pushes += 1
+
+    def status(self, seg: int) -> Tuple[int, int, int, int, int]:
+        """(n, decided, start, available bound, final) of segment seg as of the last push read (zeros before its group
+        starts)."""
+        if seg >= self.started:
+            return (0, 0, 0, 0, 0)
+        n, d, s, a, f = (int(v) for v in self._st[self._row(seg)])
+        return n, d, s, a, f
+
+    def group_final(self) -> bool:
+        """Every row of the group being pushed is final."""
+        return all(self.status(self.started - self.n_rows + i)[4] for i in range(self.n_rows))
+
+    def done(self) -> bool:
+        return self.cur >= self.B
+
+    def take(self, limit: int) -> Optional[torch.Tensor]:
+        """The next certain piece of the passage, [1, m] f32 with 0 < m <= limit, written on the current stream; None
+        when nothing is certain yet."""
+        pieces, m = [], 0
+        while m < limit and self.cur < self.B:
+            n, decided, start, avail, final = self.status(self.cur)
+            if not decided:
+                break
+            if final and avail == start:  # a segment with no samples: no span, no pause
+                self.cur += 1
+                continue
+            if self.pos < 0:
+                self.pos, self.pause_left = start, (self.P if self.spans else 0)
+                self.spans += 1
+            if self.pause_left:
+                z = min(self.pause_left, limit - m)
+                pieces.append((-1, 0, z, 0, -1))
+                m, self.pause_left = m + z, self.pause_left - z
+                continue
+            k = min(avail - self.pos, limit - m)
+            if k > 0:
+                pieces.append((self._row(self.cur), self.pos, self.pos + k, start, avail if final else -1))
+                m, self.pos = m + k, self.pos + k
+            if final and self.pos == avail:
+                self.cur, self.pos = self.cur + 1, -1
+                continue
+            break
+        if m == 0:
+            return None
+        q = np.ascontiguousarray(np.asarray(pieces, dtype=np.int64).reshape(-1, 5))
+        y = torch.empty((1, m), dtype=torch.float32, device=self.device)
+        _lib.check_arg(_lib.load().sopro_longform_stream_emit(self._h, q.ctypes.data, len(pieces), y.data_ptr(), m,
+                                                              _lib.stream_ptr(self.device)))
+        return y
+
+    def close(self) -> None:
+        if getattr(self, "_h", None):
+            _lib.load().sopro_longform_stream_destroy(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class StreamJoinPool:
+    """Idle StreamJoin states, reused by the next passage (like MimiStreamDecoder's stream states): ``checkout`` takes
+    one with enough rows and capacity, ``release`` keeps at most MAX_IDLE, the oldest going first."""
+
+    MAX_IDLE = 2
+
+    def __init__(self, device):
+        self.device = device
+        self._idle: List[StreamJoin] = []
+
+    def checkout(self, rows: int, max_len: int) -> StreamJoin:
+        for i in range(len(self._idle) - 1, -1, -1):
+            s = self._idle[i]
+            if s.rows >= rows and s.max_len >= max_len:
+                return self._idle.pop(i)
+        return StreamJoin(rows, max_len, self.device)
+
+    def release(self, s: Optional[StreamJoin]) -> None:
+        if s is None:
+            return
+        self._idle.append(s)
+        while len(self._idle) > self.MAX_IDLE:
+            self._idle.pop(0).close()

@@ -391,6 +391,7 @@ class SoproTTS:
         dev = self.device
         self._stretch_pool = StatePool(lambda n, speed: StretchStream(n, dev, speed))  # idle time-stretch states, any speed
         self._watermark_pool = StatePool(lambda n, key: WatermarkStream(n, dev, key))  # idle watermark states, any key
+        self._join_pool = LF.StreamJoinPool(dev)  # idle streaming-trim states of stream_long
 
     # ---- construction
     @classmethod
@@ -756,6 +757,33 @@ class SoproTTS:
                              min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
                              nar_context_frames=nar_context_frames, sample_rate=sample_rate, speed=speed,
                              watermark=watermark)
+
+    def stream_long(self, text: str, *, ref: PreparedReference, seed: Optional[int] = None, max_frames: int = 400,
+                    max_tokens: int = 64, pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05,
+                    anti_loop: bool = True, style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
+                    chunk_frames: int = 6, nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None,
+                    speed: Optional[float] = None, watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
+        """NEW: a text of any length, streamed -> chunks [1, n] f32 on the device at the output rate.  The segments are
+        synthesize_long's (split_text, `max_tokens`), streamed side by side SEGMENT_GROUP at a time through
+        stream_batch's chunk loop (segment i with seed seed + i; without a seed each group draws from the global
+        generator as stream_batch of the group does).  Each segment's decoded audio is trimmed as it arrives and the
+        spans are joined with `pause_ms` of silence and 10 ms raised-cosine edges, on the GPU
+        (sopro_b200/longform.py::StreamJoin); the joined 24 kHz passage goes through one stretch -> watermark ->
+        resample stream (`speed`, `watermark`, `sample_rate`).  The chunks concatenate to synthesize_long's join of the
+        segments' streamed audio bit for bit whenever no 25 ms frame of a segment is above full scale; a louder segment
+        is trimmed by the causal rule of include/sopro_b200.h.  A segment's audio comes out once its trim is certain:
+        about 0.5 s past its first voiced frame.  Each resumption runs at most one AR chunk; an item holds at most
+        chunk_frames x 1920 samples of the 24 kHz passage.  There is no loudness (it needs the whole passage), best_of
+        or word_timestamps.  Refused before any device work or random draw: a text with nothing to speak, `pause_ms`
+        or `max_tokens` out of range, `chunk_frames` outside [1, 256], a refused sample_rate / speed / watermark.
+        Closing the generator early releases its AR session, noise tapes, Mimi state, trim state and chain states."""
+        from .streaming import stream_long as _stream_long
+
+        return _stream_long(self, text, ref=ref, seed=seed, max_frames=max_frames, max_tokens=max_tokens,
+                            pause_ms=pause_ms, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
+                            style_strength=style_strength, min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
+                            nar_context_frames=nar_context_frames, sample_rate=sample_rate, speed=speed,
+                            watermark=watermark)
 
     def save_wav(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
         """`sample_rate`: the rate the waveform is at (the one passed to synthesize / stream)."""

@@ -11,7 +11,7 @@ consumer handles the audio, and the device never waits for the host between laun
 stages strictly in turn on one thread (streaming.py:81-130)."""
 from __future__ import annotations
 
-from typing import Iterator, List, Optional, Sequence, Tuple
+from typing import Callable, Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -80,10 +80,7 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
         if len(seeds) != len(texts):
             raise ValueError(f"{len(seeds)} seeds for {len(texts)} texts")
     voices.check_voices(ref, len(texts), **voices.geometry(tts.cfg))
-    if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int):
-        raise TypeError(f"chunk_frames must be an int, got {type(chunk_frames).__name__}")
-    if not 1 <= chunk_frames <= 256:
-        raise ValueError(f"chunk_frames must be in [1, 256], got {chunk_frames}")
+    _check_chunk_frames(chunk_frames)
     post = OutputChain(tts, sample_rate, speed, watermark=watermark)
     dec = _decoder(tts, chunk_frames)
 
@@ -101,6 +98,120 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
     return rows_of()
 
 
+def stream_long(tts, text: str, *, ref, seed: Optional[int] = None, max_frames: int = 400, max_tokens: int = 64,
+                pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None, chunk_frames: int = 6,
+                nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
+                watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
+    """SoproTTS.stream_long: every argument is checked here, before any device work or random draw; the returned
+    generator streams the passage.
+
+    The segments of synthesize_long run SEGMENT_GROUP at a time, each group through one chunk loop whose decoded
+    blocks go to the streaming trim (longform.StreamJoin) instead of an output chain; the joined 24 kHz passage goes
+    through one output-chain stream.  Each resumption runs at most one AR chunk, then yields the next piece of the
+    passage (at most chunk_frames x 1920 samples of it before the chain); it runs more chunks only while nothing is
+    certain yet.  A group starts at the first resumption after the group before it has ended and the group before
+    that has been emitted (the trim state holds two groups)."""
+    from . import longform as LF
+
+    post = OutputChain(tts, sample_rate, speed, watermark=watermark)
+    P = LF.pause_samples(pause_ms)
+    budget = LF.check_max_tokens(max_tokens, tts.model.prefill.max_text_len)
+    _check_chunk_frames(chunk_frames)
+    segments = LF.split_text(text, tts.tokenizer, budget)
+    if not segments:
+        raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
+    B, G = len(segments), int(LF.SEGMENT_GROUP)
+    hop = tts.codec.engine.hop
+    limit = int(chunk_frames) * hop
+    dec = _decoder(tts, chunk_frames)
+    bypass = OutputChain(tts)
+
+    @torch.inference_mode()
+    def passage():
+        join = tts._join_pool.checkout(LF.StreamJoin.rows_for(B, G), (int(max_frames) + 1) * hop)
+        join.begin(B, P, G)
+        out = post.stream(limit)
+        main = torch.cuda.current_stream(tts.device)
+        emit = torch.cuda.Stream(tts.device)  # the pieces and the chain: never queued behind the next AR launch
+        loop = None
+
+        def start(g0):
+            part = segments[g0: g0 + G]
+            join.start_group(g0, len(part))
+            return _chunk_loop(tts, dec, [tts.encode_text(t) for t in part], ref, bypass, max_frames=max_frames,
+                               top_p=top_p, temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
+                               chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
+                               min_gen_frames=min_gen_frames,
+                               seeds=None if seed is None else [int(seed) + g0 + i for i in range(len(part))],
+                               on_block=join.push)
+
+        def chunk() -> bool:
+            """One AR chunk of the group being generated (starting the next group when it may); False when there is
+            nothing to run."""
+            nonlocal loop
+            if loop is None:
+                if not join.can_start(join.started):
+                    return False
+                loop = start(join.started)
+            k = join.pushes
+            for _ in loop:  # the launch's items: the trim stage has its block (and the status is on the host)
+                if join.pushes > k:
+                    break
+            if join.group_final():
+                for _ in loop:  # the rest of the last launch's items; the loop then releases its session and state
+                    pass
+                loop.close()
+                loop = None
+            return join.pushes > k
+
+        def piece() -> Optional[torch.Tensor]:
+            """The next non-empty item through the chain, from what is certain now (None: nothing is)."""
+            with torch.cuda.stream(emit):  # (what it reads was pushed on a stream the loop has synchronised)
+                while True:
+                    y = join.take(limit)
+                    if y is None:
+                        return None
+                    y = out.push(y)
+                    if y.numel():
+                        break
+            y.record_stream(main)
+            main.wait_stream(emit)
+            return y
+
+        try:
+            while True:
+                chunk()
+                y = piece()
+                while y is None and not join.done():
+                    if not chunk():
+                        raise RuntimeError("stream_long has nothing to run and nothing certain to emit")
+                    y = piece()
+                if y is None:
+                    break
+                yield y
+            with torch.cuda.stream(emit):
+                tail = out.finish()
+            if tail is not None and tail.numel():
+                tail.record_stream(main)
+                main.wait_stream(emit)
+                yield tail
+        finally:
+            if loop is not None:
+                loop.close()
+            out.release()
+            tts._join_pool.release(join)
+
+    return passage()
+
+
+def _check_chunk_frames(chunk_frames) -> None:
+    if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int):
+        raise TypeError(f"chunk_frames must be an int, got {type(chunk_frames).__name__}")
+    if not 1 <= chunk_frames <= 256:
+        raise ValueError(f"chunk_frames must be in [1, 256], got {chunk_frames}")
+
+
 def _decoder(tts, chunk_frames) -> MimiStreamDecoder:
     """The SoproTTS's one stream decoder (one pool of device stream states: a finished utterance's state is reset and
     reused by the next stream instead of a 0.8 ms allocation + memset on the time-to-first-audio path), made on first
@@ -115,14 +226,19 @@ def _decoder(tts, chunk_frames) -> MimiStreamDecoder:
 def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], ref, post: OutputChain, *,
                 max_frames: int, top_p: float, temperature: float, anti_loop: bool, style_strength: Optional[float],
                 chunk_frames: int, nar_context_frames: Optional[int], min_gen_frames: Optional[int],
-                seeds: Optional[Sequence[int]], generator: Optional[torch.Generator] = None
+                seeds: Optional[Sequence[int]], generator: Optional[torch.Generator] = None,
+                on_block: Optional[Callable[[Optional[torch.Tensor], List[int], List[bool]], None]] = None
                 ) -> Iterator[Tuple[int, Optional[torch.Tensor], bool]]:
     """The chunk loop of B utterances (`ref`: one prepared voice, or one per text) -> ``(i, wav or None, last)``:
     per launch, in row order, each live row's chunk (None when it has no samples), the row's last item once with
     last=True.  All rows advance in lockstep, `chunk_frames` AR frames per launch, so the NAR window [lo, end) is
     shared by the live rows (only a row that ends in this launch has a shorter one) and runs as one ragged NAR pass;
     one Mimi step decodes every row (a row that has ended is fed code 0 and its samples are dropped), then each row's
-    samples go through its own output-chain stream.  Row i's chunks are those of this loop over text i alone."""
+    samples go through its own output-chain stream.  Row i's chunks are those of this loop over text i alone.
+    `on_block` (stream_long's trim stage): called once per launch, on the stream the launch's Mimi step ran on, with
+    the step's decoded block [B, L] (None when nothing was decoded), each row's new samples in it (0 for a row that
+    did not run) and whether each row ends with this launch; the loop synchronises that stream before it yields the
+    launch's items."""
     model = tts.model
     B = len(text_ids)
     st_ = float(style_strength if style_strength is not None else tts.cfg.style_strength)
@@ -163,6 +279,9 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
                 codes, part = torch.zeros((B, n, win.shape[2]), dtype=torch.long, device=tts.device), codes
                 codes[sel] = part * keep[:, :, None]
             rows_wav, state = dec.decode_step(codes, state, _trusted=True)  # our own NAR's codes
+        if on_block is not None:
+            on_block(rows_wav, [(ends[b] - emitted) * hop if rows_wav is not None and ends[b] > emitted else 0
+                                for b in range(B)], last)
         for b in live:
             wav = rows_wav[b: b + 1, : (ends[b] - emitted) * hop] if rows_wav is not None and ends[b] > emitted else None
             wav = posts[b].finish(wav) if last[b] else posts[b].push(wav)

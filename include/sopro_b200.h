@@ -649,6 +649,49 @@ int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const
 int sopro_debug_rope_pack(const float* qkv, const float* table, int tab_T2, void* qh, void* kh, void* vt, int B, int T2, int C, int H,
                           void* stream);
 
+/* test hooks: single fp32 kernels of the Mimi decoder and encoder (no reference counterpart), each launched with the
+ * launch geometry the codec uses.  Device pointers, no allocation; a shape the kernel does not take returns
+ * SOPRO_ERR_INVALID and launches nothing.
+ *
+ * implicit GEMM: out[b][m][n] (at out + b*c_bs + m*ldc + n) = epi(sum_{j, ci} act(A'[m + j*dil - pad][ci]) * W[n][j*Cin + ci]
+ * + bias[n % bias_mod]), A' = A + b*a_bs read as [Min][Cin] (rows outside [0, Min) are zero), act = ELU when a_elu;
+ * epi 0 none, 1 GELU(erf), 2 R' + scale[n]*acc, 3 R' + acc with R'[m][n] = R[b*r_bs + m*N + n].  Each output is one fma
+ * chain over ascending k = j*Cin + ci.  K = taps*Cin, K % 16 == 0, Cin % 4 == 0, Min >= M, ldc >= N, a_bs % 4 == 0;
+ * N % 64 != 0 and N <= 32 takes the 32-column tile. */
+int sopro_debug_mimi_gemm(const float* A, const float* W, const float* bias, const float* R, const float* scale, float* out, int B, int M,
+                          int N, int K, int Min, int Cin, int taps, int dil, int pad, int ldc, int bias_mod, int epi, int a_elu,
+                          int64_t a_bs, int64_t c_bs, int64_t r_bs, void* stream);
+/* RVQ lookup-sum: codes i32 [B][Q][code_T] (frames [0, T) read, code_T >= T), embed [Q][vocab][Dc] -> S [B][T][2*Dc] =
+ * [sum of codebooks q < n_sem | sum of the others], each summed in q order.  A code outside [0, vocab) is clamped and
+ * sets *bad (device i32, sticky). */
+int sopro_debug_mimi_rvq_gather(const int32_t* codes, const float* embed, float* S, int B, int Q, int T, int code_T, int Dc, int vocab,
+                                int n_sem, int32_t* bad, void* stream);
+/* depthwise causal ConvTranspose k=4 s=2: x [B][T][C], w [C][4] -> y [B][2T][C]; y[2t+r] = x[t]*w[r] + x[t-1]*w[r+2],
+ * x[-1] = prev[b] (device [B][C]) or zero when prev is NULL. */
+int sopro_debug_mimi_upsample(const float* x, const float* w, float* y, const float* prev, int B, int T, int C, void* stream);
+/* LayerNorm over C of rows x [rows][C] -> y [rows][C], fp32 (out_bf16 = 0) or bf16. */
+int sopro_debug_mimi_layernorm(const float* x, const float* w, const float* b, void* y, int64_t rows, int C, float eps, int out_bf16,
+                               void* stream);
+/* RoPE then causal sliding-window attention in fp32 over qkv [B][T2][3C] (q and k rotated in place), row t at position
+ * pos0 + t; table [cos rows | sin rows] of tab_T2 >= pos0 + T2 positions, Dh/2 floats each; out [B][T2][C] fp32 or bf16.
+ * Query at position p attends to positions (p - window, p].  With kring / vring (device [B][R][C], both or neither,
+ * R >= T2 + window - 1), each rotated key and value is first written to slot position % R and the keys and values are
+ * read from the rings; without them pos0 = 0.  C % H == 0, (C/H) % 4 == 0. */
+int sopro_debug_mimi_attn(float* qkv, const float* table, int tab_T2, void* out, int B, int T2, int C, int H, int window, int pos0,
+                          float* kring, float* vring, int R, int out_bf16, void* stream);
+/* final conv Cin -> 1, taps in [1, 8]: y[b][t] = bias + sum_j sum_c act(x[b][t + j - (taps-1)][c]) * w[j*Cin + c] over rows
+ * >= lo (lo in [-(taps-1), 0]: rows lo..-1 are context in front of x), item b at x + b*x_bs, y + b*y_bs.  x_bf16 = 0: x
+ * fp32 and act = ELU (final_conv_kernel, Cin % 4 == 0); x_bf16 = 1: x bf16 already ELU'd (final_conv_h_kernel,
+ * Cin % 8 == 0). */
+int sopro_debug_mimi_final_conv(const void* x, int x_bf16, const float* w, const float* bias, float* y, int B, int64_t Tn, int Cin,
+                                int taps, int lo, int64_t x_bs, int64_t y_bs, void* stream);
+/* residual codeword search of the encoder (Dc = 256): proj [B][T][512] = [semantic | acoustic] projections, embed
+ * [n_q][V][256] -> codes i32 [B][n_q][T]; codebooks q < n_sem search from the semantic half, the rest from the acoustic
+ * half, each code torch.argmin of the squared distances to the running residual (the first NaN, else the lowest index of
+ * the minimum: always in [0, V)).  frames: device i32 [B] or NULL; frames of clip b at or past frames[b] are not written. */
+int sopro_debug_mimi_rvq_encode(const float* proj, const float* embed, int32_t* codes, int T, int n_q, int n_sem, int V,
+                                const int32_t* frames, int B, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Output resampling (no reference counterpart: the reference always returns 24 kHz): band-limited resampling of a
  * waveform from sr_in to sr_out with torchaudio.functional.resample's default filter (sinc_interp_hann,

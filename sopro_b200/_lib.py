@@ -226,6 +226,13 @@ SYMBOLS = {
     "sopro_debug_tc_attn": (_I, [_VP, _VP, _VP, _VP, _I, _I, C.c_int64, _I, _I, _I, _VP]),
     "sopro_debug_tc_resblock": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
     "sopro_debug_rope_pack": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
+    "sopro_debug_mimi_gemm": (_I, [_VP, _VP, _VP, _VP, _VP, _VP] + [_I] * 13 + [C.c_int64] * 3 + [_VP]),
+    "sopro_debug_mimi_rvq_gather": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP]),
+    "sopro_debug_mimi_upsample": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _VP]),
+    "sopro_debug_mimi_layernorm": (_I, [_VP, _VP, _VP, _VP, C.c_int64, _I, C.c_float, _I, _VP]),
+    "sopro_debug_mimi_attn": (_I, [_VP, _VP, _I, _VP, _I, _I, _I, _I, _I, _I, _VP, _VP, _I, _I, _VP]),
+    "sopro_debug_mimi_final_conv": (_I, [_VP, _I, _VP, _VP, _VP, _I, C.c_int64, _I, _I, _I, C.c_int64, C.c_int64, _VP]),
+    "sopro_debug_mimi_rvq_encode": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP, _I, _VP]),
     "sopro_resampler_filter": (_I, [C.c_int32, C.c_int32, _I32P, _I32P, _I32P, _VP]),
     "sopro_resampled_length": (C.c_int64, [C.c_int32, C.c_int32, C.c_int64]),
     "sopro_resampler_create": (_I, [C.c_int32, C.c_int32, _I, C.POINTER(_VP)]),

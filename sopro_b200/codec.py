@@ -166,8 +166,8 @@ class MimiEncoderEngine:
         wav = np.ascontiguousarray(wav, dtype=np.float32).reshape(-1)
         T = self.frames(wav.size)
         codes = np.empty((self.num_quantizers, T), dtype=np.int32)
-        _lib.check(self.lib.sopro_mimi_encode_host(self._h, wav.ctypes.data, int(wav.size), codes.ctypes.data, None,
-                                                   int(torch.cuda.current_stream(self.device).cuda_stream)))
+        _lib.check_arg(self.lib.sopro_mimi_encode_host(self._h, wav.ctypes.data, int(wav.size), codes.ctypes.data, None,
+                                                       int(torch.cuda.current_stream(self.device).cuda_stream)))
         return codes
 
     def close(self):
@@ -400,7 +400,10 @@ class MimiCodec:
         """reference codec/mimi.py:41-63 (VAD trim -> resample -> centre crop -> MimiModel.encode)."""
         from .audio import center_crop_audio, load_audio_file, resample, trim_silence_energy
 
+        from .ingest import check_finite
+
         wav, sr = load_audio_file(wav_path)
+        check_finite(wav, wav_path)
         wav = trim_silence_energy(wav, sr)
         wav = resample(wav, sr, TARGET_SR)
         if crop_seconds is not None and crop_seconds > 0:
@@ -420,7 +423,11 @@ class MimiCodec:
     @torch.no_grad()
     def encode_wav(self, wav: torch.Tensor) -> torch.Tensor:
         """mono waveform @24 kHz ([n], [1, n] or [1, 1, n]) -> codes [T, Q] int64 on the device: the model call of
-        ``encode_file`` (reference codec/mimi.py:59-62), on the CUDA encoder."""
+        ``encode_file`` (reference codec/mimi.py:59-62), on the CUDA encoder.  A non-finite sample is a ValueError,
+        raised before the encoder is built or launched."""
+        from .ingest import check_finite
+
+        check_finite(wav, "the waveform")
         return self.encoder.encode(wav).permute(1, 0).contiguous()
 
     @torch.no_grad()

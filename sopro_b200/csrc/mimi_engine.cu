@@ -1486,6 +1486,96 @@ int sopro_debug_rope_pack(const float* qkv, const float* table, int tab_T2, void
   return SOPRO_OK;
 }
 
+int sopro_debug_mimi_gemm(const float* A, const float* W, const float* bias, const float* R, const float* scale, float* out, int B, int M,
+                          int N, int K, int Min, int Cin, int taps, int dil, int pad, int ldc, int bias_mod, int epi, int a_elu,
+                          int64_t a_bs, int64_t c_bs, int64_t r_bs, void* stream) {
+  if (!A || !W || !out) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535 || M < 1 || N < 1 || Cin < 4 || Cin % 4 || taps < 1 || dil < 1 || pad < 0 || K != taps * Cin || K % 16 ||
+      Min < M || ldc < N || a_bs % 4 || a_bs < 0 || c_bs < 0 || r_bs < 0 || epi < EPI_NONE || epi > EPI_RES ||
+      (bias && bias_mod < 1) || (epi >= EPI_RES_SCALE && !R) || (epi == EPI_RES_SCALE && !scale))
+    return fail(SOPRO_ERR_INVALID, "igemm: unsupported shape (B=%d M=%d N=%d K=%d Min=%d Cin=%d taps=%d ldc=%d epi=%d)", B, M, N, K, Min,
+                Cin, taps, ldc, epi);
+  GemmOp g{};
+  g.A = A; g.W = W; g.bias = bias; g.R = R; g.scale = scale; g.C = out;
+  g.a_bs = a_bs; g.c_bs = c_bs; g.r_bs = r_bs;
+  g.M = M; g.N = N; g.K = K; g.Min = Min; g.Cin = Cin; g.taps = taps; g.dil = dil; g.pad = pad; g.ldc = ldc;
+  g.bias_mod = bias ? bias_mod : 1; g.epi = epi; g.a_elu = a_elu ? 1 : 0;
+  return launch_gemm(g, B, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sopro_debug_mimi_rvq_gather(const int32_t* codes, const float* embed, float* S, int B, int Q, int T, int code_T, int Dc, int vocab,
+                                int n_sem, int32_t* bad, void* stream) {
+  if (!codes || !embed || !S || !bad) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535 || Q < 1 || T < 1 || code_T < T || Dc < 1 || vocab < 1 || n_sem < 0 || n_sem > Q)
+    return fail(SOPRO_ERR_INVALID, "rvq gather: unsupported shape (B=%d Q=%d T=%d code_T=%d Dc=%d vocab=%d)", B, Q, T, code_T, Dc, vocab);
+  rvq_gather_kernel<<<dim3(T, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(codes, embed, S, Q, T, code_T, Dc, vocab, n_sem, bad);
+  CK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+int sopro_debug_mimi_upsample(const float* x, const float* w, float* y, const float* prev, int B, int T, int C, void* stream) {
+  if (!x || !w || !y) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535 || T < 1 || T > 0x3fffffff || C < 1)
+    return fail(SOPRO_ERR_INVALID, "upsample: unsupported shape (B=%d T=%d C=%d)", B, T, C);
+  upsample_kernel<<<dim3(2 * T, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, w, y, T, C, prev);
+  CK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+int sopro_debug_mimi_layernorm(const float* x, const float* w, const float* b, void* y, int64_t rows, int C, float eps, int out_bf16,
+                               void* stream) {
+  if (!x || !w || !b || !y) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (rows < 1 || (rows + 7) / 8 > 0x7fffffffLL || C < 1) return fail(SOPRO_ERR_INVALID, "layernorm: unsupported shape (rows=%lld C=%d)", (long long)rows, C);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const unsigned grid = (unsigned)((rows + 7) / 8);  // as run_layers launches it
+  if (out_bf16) layernorm_kernel<<<grid, 256, 0, st>>>(x, w, b, static_cast<__nv_bfloat16*>(y), rows, C, eps);
+  else layernorm_kernel<<<grid, 256, 0, st>>>(x, w, b, static_cast<float*>(y), rows, C, eps);
+  CK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+int sopro_debug_mimi_attn(float* qkv, const float* table, int tab_T2, void* out, int B, int T2, int C, int H, int window, int pos0,
+                          float* kring, float* vring, int R, int out_bf16, void* stream) {
+  if (!qkv || !table || !out || !kring != !vring) return fail(SOPRO_ERR_INVALID, "null argument");
+  const int Dh = H > 0 ? C / H : 0;
+  const size_t asm_bytes = (size_t)8 * (Dh + (size_t)std::max(window, 0)) * 4;
+  if (B < 1 || B > 65535 || T2 < 1 || H < 1 || C < 1 || C % H || Dh % 4 || window < 1 || pos0 < 0 || asm_bytes > 48 * 1024 ||
+      (long long)pos0 + T2 > tab_T2 || (kring ? (long long)R < (long long)T2 + window - 1 : pos0 != 0))
+    return fail(SOPRO_ERR_INVALID, "attention: unsupported shape (B=%d T2=%d C=%d H=%d window=%d pos0=%d R=%d tab_T2=%d)", B, T2, C, H,
+                window, pos0, R, tab_T2);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int Rk = kring ? R : 1;
+  // as run_layers issues them: RoPE in place (and the ring append), then the attention
+  rope_kernel<<<dim3(T2, B), 256, 0, st>>>(qkv, table, T2, tab_T2, C, H, pos0, kring, vring, Rk);
+  if (out_bf16)
+    attn_kernel<<<dim3((T2 + 7) / 8, H, B), 256, asm_bytes, st>>>(qkv, static_cast<__nv_bfloat16*>(out), T2, C, H, window, pos0, kring, vring, Rk);
+  else
+    attn_kernel<<<dim3((T2 + 7) / 8, H, B), 256, asm_bytes, st>>>(qkv, static_cast<float*>(out), T2, C, H, window, pos0, kring, vring, Rk);
+  CK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
+int sopro_debug_mimi_final_conv(const void* x, int x_bf16, const float* w, const float* bias, float* y, int B, int64_t Tn, int Cin,
+                                int taps, int lo, int64_t x_bs, int64_t y_bs, void* stream) {
+  if (!x || !w || !bias || !y) return fail(SOPRO_ERR_INVALID, "null argument");
+  const int vec = x_bf16 ? 8 : 4;  // elements per vector load
+  const size_t smem = (size_t)(taps * 256 + (size_t)taps * Cin) * 4;
+  if (B < 1 || B > 65535 || Tn < 1 || Tn > 0x7fffffffLL || Cin < vec || Cin % vec || taps < 1 || taps > 8 || lo > 0 || lo < -(taps - 1) ||
+      x_bs % vec || (B > 1 && (x_bs < (Tn - lo) * Cin || y_bs < Tn)) || (x_bf16 && smem > 48 * 1024))
+    return fail(SOPRO_ERR_INVALID, "final conv: unsupported shape (B=%d Tn=%lld Cin=%d taps=%d lo=%d)", B, (long long)Tn, Cin, taps, lo);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (x_bf16) {  // as seanet_tc launches it
+    const int per = 256 - (taps - 1);
+    final_conv_h_kernel<<<dim3((unsigned)((Tn + per - 1) / per), B), 256, smem, st>>>(static_cast<const __nv_bfloat16*>(x), w, bias, y, Tn,
+                                                                                      Cin, taps, lo, x_bs, y_bs);
+  } else {
+    final_conv_kernel<<<dim3((unsigned)((Tn + 255) / 256), B), 256, 0, st>>>(static_cast<const float*>(x), w, bias, y, Tn, Cin, taps, lo,
+                                                                              x_bs, y_bs);
+  }
+  CK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
 int sopro_mimi_decode_host(sopro_mimi_t* m, const int32_t* codes_host, int B, int T, float* wav_host, void* stream) {
   if (!m || !codes_host || !wav_host) return fail(SOPRO_ERR_INVALID, "null argument");
   CK(cudaSetDevice(m->device));
@@ -1576,7 +1666,9 @@ __global__ void replicate_pad_kernel(const float* __restrict__ x, float* __restr
 // Residual nearest-neighbour search (MimiResidualVectorQuantizer.encode :1262-1280 with MimiEuclideanCodebook.quantize
 // :1197-1203): one CTA per frame, the residual (Dc = 32*DPL floats) in registers, lane-sliced; a warp scans every 8th
 // code vector, squared distance summed directly (the reference's cdist goes through |x|^2+|e|^2-2xe, same minimiser),
-// lowest index wins ties (torch.argmin).  proj [T][2*Dc] = [semantic input_proj | acoustic input_proj] of the latent.
+// with torch.argmin's rule: the first NaN distance wins, else the lowest index of the smallest distance, so a frame whose
+// every distance is +Inf takes code 0 and every code is in [0, V) whatever the residual holds.  proj [T][2*Dc] =
+// [semantic input_proj | acoustic input_proj] of the latent.
 // Batch (grid.y = B): clip b's proj rows are proj + b * T * 2Dc and its codes codes + b * n_q * T; frames at or past
 // its own info[b][NS - 1] are skipped.
 template <int DPL>
@@ -1600,7 +1692,8 @@ __global__ void __launch_bounds__(256) rvq_encode_kernel(const float* __restrict
     }
     const float* E = embed + (size_t)q * V * Dc;
     float bd = INFINITY;
-    int bi = 0x7fffffff;
+    int bi = warp;  // a warp none of whose distances is below +Inf keeps its first index (>= V only when V < 8)
+#pragma unroll 4  // four code vectors' loads in flight, as the compiler unrolls the loop without the NaN select
     for (int k = warp; k < V; k += 8) {
       const float* e = E + (size_t)k * Dc + lane * DPL;
       float acc = 0.f;
@@ -1618,7 +1711,8 @@ __global__ void __launch_bounds__(256) rvq_encode_kernel(const float* __restrict
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-      if (acc < bd) {  // k ascends within a warp: strict < keeps the lowest index
+      acc = acc != acc ? -1.f : acc;  // a NaN distance ranks below every real one (>= 0)
+      if (acc < bd) {  // k ascends within a warp: strict < keeps the lowest index (the first NaN)
         bd = acc;
         bi = k;
       }
@@ -1930,11 +2024,24 @@ int sopro_mimi_encode_batch(sopro_mimi_encoder_t* e, const float* wav, int32_t B
   return encode_run(e, P, B, wav, stride, e->info_dev, codes, latent, st);
 }
 
+int sopro_debug_mimi_rvq_encode(const float* proj, const float* embed, int32_t* codes, int T, int n_q, int n_sem, int V,
+                                const int32_t* frames, int B, void* stream) {
+  if (!proj || !embed || !codes) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (B < 1 || B > 65535 || T < 1 || n_q < 1 || n_sem < 1 || n_sem > n_q || V < 1)
+    return fail(SOPRO_ERR_INVALID, "rvq encode: unsupported shape (B=%d T=%d n_q=%d n_sem=%d V=%d)", B, T, n_q, n_sem, V);
+  // as encode_run launches it; frames (one column per clip) stands in for the last column of a batch's info
+  rvq_encode_kernel<8><<<dim3(T, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(proj, embed, codes, T, n_q, n_sem, V, frames, 1);
+  CK(cudaGetLastError());
+  return SOPRO_OK;
+}
+
 int sopro_mimi_encode_host(sopro_mimi_encoder_t* e, const float* wav_host, int64_t n_samples, int32_t* codes_host,
                            float* latent_host, void* stream) {
   if (!e || !wav_host || !codes_host) return fail(SOPRO_ERR_INVALID, "null argument");
   if (n_samples < 1 || n_samples > kEncMaxSamples)
     return fail(SOPRO_ERR_INVALID, "n_samples=%lld outside [1, %lld]", (long long)n_samples, kEncMaxSamples);
+  for (int64_t i = 0; i < n_samples; ++i)
+    if (!std::isfinite(wav_host[i])) return fail(SOPRO_ERR_INVALID, "sample %lld is not finite (%g)", (long long)i, (double)wav_host[i]);
   CK(cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
   const long long T = enc_plan(e->cfg, n_samples).T;

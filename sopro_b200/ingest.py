@@ -69,10 +69,19 @@ def _check_wav(wav: torch.Tensor, sr, i: int) -> int:
     return sr
 
 
+def check_finite(wav: torch.Tensor, what: str) -> None:
+    """ValueError unless every sample of wav is finite.  A NaN or infinite sample (a float file can hold one; peak
+    normalising a silent clip makes every sample NaN) has no meaning as audio, and the encoder's codes of it would be
+    the codebooks' first entries, not a voice."""
+    if not bool(torch.isfinite(wav).all()):
+        raise ValueError(f"{what} holds non-finite samples (NaN or infinity)")
+
+
 def load_clips(clips: Sequence[Clip], sample_rates=None) -> Tuple[List[torch.Tensor], List[int]]:
     """The clips checked, then the paths read on the host (audio.load_audio_file) -> (tensors, rates).  `sample_rates`:
-    one rate per clip (None for a path, which supplies its own), or one int for every tensor clip.  Every tensor clip is
-    checked before any file is read; nothing touches the device."""
+    one rate per clip (None for a path, which supplies its own), or one int for every tensor clip.  Every tensor clip's
+    shape, type and rate are checked before any file is read; then every clip's samples must be finite.  Nothing here
+    launches the library's kernels (a clip on the device is read by one torch reduction)."""
     if _is_path(clips) or isinstance(clips, torch.Tensor) or not isinstance(clips, Sequence):
         raise TypeError("clips must be a list of paths and / or tensors")
     clips = list(clips)
@@ -99,6 +108,8 @@ def load_clips(clips: Sequence[Clip], sample_rates=None) -> Tuple[List[torch.Ten
             rates[i] = _check_wav(w, sr, i)
             c = w
         wavs.append(c)
+    for i, w in enumerate(wavs):
+        check_finite(w, f"clip {i}")
     return wavs, rates
 
 

@@ -189,6 +189,11 @@ int sopro_ar_set_timing(sopro_ar_session_t* s, int64_t* buf, int step);
  * ld < 1 with a buffer is SOPRO_ERR_INVALID; sopro_ar_begin and sopro_ar_run refuse ld < the batch's longest text
  * (SOPRO_ERR_INVALID, before any launch). */
 int sopro_ar_set_attn_trace(sopro_ar_session_t* s, float* probs, int64_t ld);
+/* the same into a ring of `ring` step rows: step t goes to row t % ring of probs [ring][n_attn][batch][H][ld] (a stream
+ * consumes each launch's rows before the next launch overwrites them).  sopro_ar_set_attn_trace is the case ring =
+ * the session's steps.  ring < 1 with a buffer is SOPRO_ERR_INVALID; sopro_ar_run refuses a launch of more than `ring`
+ * steps (SOPRO_ERR_INVALID, before any launch). */
+int sopro_ar_set_attn_trace_ring(sopro_ar_session_t* s, float* probs, int64_t ld, int32_t ring);
 /* warp task shape of the GEMV stages of later launches: 0 = picked per stage from the launch geometry (the default),
  * 1 = always R rows x TU utterances (wide), 2 = R x TU/2 (narrow) in every GEMV stage but GLU (teams of one utterance
  * stay wide).  The outputs are bit-identical in every mode. */
@@ -951,6 +956,41 @@ int sopro_align_sizes(int32_t B, int32_t steps, int64_t ld, int64_t* ws_bytes);
  * Bad geometry is SOPRO_ERR_INVALID before any launch.  No call synchronises or allocates. */
 int sopro_align(const float* probs, int32_t steps, int32_t n_attn, int32_t B, int32_t H, int64_t ld, const int32_t* text_len_host,
                 const int32_t* frames_host, void* ws, int32_t* first, void* stream);
+
+/* ---- streaming word alignment: a causal restatement of the one above, for streams.  Fixed-lag Viterbi with binding
+ * commits, per row of L tokens and a lag of D >= 1 frames (oracle/align_stream_oracle.py::StreamAlign in float64):
+ *   A[t][l] and S[t][l] are the one-shot's (same summation order, the stay predecessor winning ties).
+ *   Commit: after S[t] for t >= D, frame c = t - D is committed.  l* = the lowest l with the largest finite S[t][l];
+ *     the backtrack from (t, l*) to frame c gives token k_c; a token whose first frame is <= c on that path has that
+ *     first frame, final (so first[k_c] = c when k_c moved past k_{c-1}; first[0] = 0 at c = 0).
+ *   Prune: S[t][l] = -inf for every l whose backtrack to frame c is not k_c.  Every later path then extends the
+ *     committed prefix: no commit is ever revised.
+ *   End, with T = the row's frames: backtrack from (T-1, L-1) if that state is finite, else from the highest l whose
+ *     S[T-1][l] is finite; tokens past the end state start at T (zero length).  T == 0 gives no path (first all -1).
+ *   With no commit (T <= D) and T >= L the path is the one-shot path.  Unlike the one-shot, T < L still gives a path:
+ *     the committed tokens, then zero-length ones.
+ * The state lives in a caller-allocated device buffer of sopro_align_stream_sizes' bytes; its first
+ * rows x (2 + ld) i32 are, per row, {F = frames committed, K = tokens whose first frame is final, first[ld]}: first[l]
+ * is -1 until committed, and past the row's end F = T, K = L and first is the whole path (-1 from L on, or the whole row
+ * when there is no path).  A stream of several rows: rows <= 256; a row's frames t come from the ring trace of
+ * sopro_ar_set_attn_trace_ring, slot t % ring.  No call synchronises; only create and destroy touch the heap, on the host. */
+typedef struct sopro_align_stream sopro_align_stream_t;
+/* host-only: the device state bytes; SOPRO_ERR_INVALID for bad geometry (rows not in [1, 256], ld, lag or max_frames < 1) */
+int sopro_align_stream_sizes(int32_t rows, int64_t ld, int32_t lag, int32_t max_frames, int64_t* state_bytes);
+/* state: device, sopro_align_stream_sizes' bytes, owned by the caller for the stream's life; max_frames: the most frames
+ * a row takes between two begins */
+int sopro_align_stream_create(int32_t rows, int64_t ld, int32_t lag, int32_t max_frames, void* state,
+                              sopro_align_stream_t** out);
+int sopro_align_stream_destroy(sopro_align_stream_t* s);
+/* every row starts over with text_len_host[b] (HOST i32 [rows], in [1, min(ld, 2048)]) tokens: one reset launch */
+int sopro_align_stream_begin(sopro_align_stream_t* s, const int32_t* text_len_host, void* stream);
+/* probs: the ring trace, device f32 [ring][n_attn][B][H][ld] with B = rows and ld = the state's; frames_host[b] (HOST,
+ * in [0, ring]): row b's new frames, which sit in the ring now; end_host[b] (HOST): nonzero when the row ends after them.
+ * One launch for every row (one CTA per row; none when no row has work).  A row that has ended takes no frames and no
+ * second end until the next begin; a row's frames past max_frames, bad geometry and a null probs with frames are
+ * SOPRO_ERR_INVALID, before any launch. */
+int sopro_align_stream_push(sopro_align_stream_t* s, const float* probs, int32_t ring, int32_t n_attn, int32_t B, int32_t H,
+                            int64_t ld, const int32_t* frames_host, const int32_t* end_host, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Watermark (no reference counterpart): a keyed spread-spectrum mark on 24 kHz audio, and its detector.  A key is an

@@ -166,6 +166,7 @@ SYMBOLS = {
     "sopro_ar_set_trace": (_I, [_VP, _VP, _VP]),
     "sopro_ar_set_timing": (_I, [_VP, _VP, _I]),
     "sopro_ar_set_attn_trace": (_I, [_VP, _VP, C.c_int64]),
+    "sopro_ar_set_attn_trace_ring": (_I, [_VP, _VP, C.c_int64, C.c_int32]),
     "sopro_ar_session_set_task_shape": (_I, [_VP, _I]),
     "sopro_ar_session_stage_shapes": (_I, [_VP, _I32P, _I32P, _I, _I32P]),
     "sopro_ar_debug_sampled": (_I, [_VP, _VP, _VP]),
@@ -280,6 +281,11 @@ SYMBOLS = {
     "sopro_flac_stream_finish": (_I, [_VP, _VP, _VP, _VP, _VP]),
     "sopro_align_sizes": (_I, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_int64)]),
     "sopro_align": (_I, [_VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _I32P, _I32P, _VP, _VP, _VP]),
+    "sopro_align_stream_sizes": (_I, [C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
+    "sopro_align_stream_create": (_I, [C.c_int32, C.c_int64, C.c_int32, C.c_int32, _VP, C.POINTER(_VP)]),
+    "sopro_align_stream_destroy": (_I, [_VP]),
+    "sopro_align_stream_begin": (_I, [_VP, _I32P, _VP]),
+    "sopro_align_stream_push": (_I, [_VP, _VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _I32P, _I32P, _VP]),
     "sopro_watermark_pattern": (_I, [C.c_int64, _VP]),
     "sopro_watermark_sizes": (_I, [C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "sopro_watermark_embed": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP, C.c_int64, _VP, _VP]),

@@ -114,6 +114,7 @@ struct sopro_ar_session {
   int timing_step = -1;
   float* attn_trace = nullptr;  // word timestamps: [steps][n_attn][B][H][attn_ld] (null = off)
   int64_t attn_ld = 0;
+  int attn_ring = 0;  // the trace's step rows: step t goes to row t % attn_ring (0 = the batch's steps, no ring)
   int max_len = 0;  // longest text of the current batch
   bool begun = false;
   std::vector<UttState> host_st;
@@ -748,6 +749,7 @@ static int launch_ar(sopro_ar_session* s, int t_begin, int t_end, cudaStream_t s
   p.attn_trace = s->attn_trace;
   p.attn_ld = s->attn_ld;
   p.attn_step = (long long)e->n_attn * s->B * e->H * s->attn_ld;
+  p.attn_ring = s->attn_ring > 0 ? s->attn_ring : s->steps;
   // ---- team geometry: g teams x P CTAs, Bt utterances per team
   int Bt = s->utts_per_team;
   if (Bt <= 0) {
@@ -891,6 +893,8 @@ int sopro_ar_run(sopro_ar_session_t* s, int n_steps, void* stream) {
   if (t0 >= t1) return SOPRO_OK;
   if (s->attn_trace && s->attn_ld < s->max_len)  // a trace set after sopro_ar_begin
     return fail(SOPRO_ERR_INVALID, "attention trace row stride %lld < longest text %d", (long long)s->attn_ld, s->max_len);
+  if (s->attn_trace && s->attn_ring > 0 && t1 - t0 > s->attn_ring)  // the launch would overwrite its own first steps
+    return fail(SOPRO_ERR_INVALID, "a launch of %d steps into an attention trace ring of %d", t1 - t0, s->attn_ring);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int rc = e->cfg.weight_dtype == SOPRO_W_F32 ? launch_ar<float>(s, t0, t1, st)
                                                : launch_ar<__nv_bfloat16>(s, t0, t1, st);
@@ -985,6 +989,15 @@ int sopro_ar_set_attn_trace(sopro_ar_session_t* s, float* probs, int64_t ld) {
   if (probs && ld < 1) return fail(SOPRO_ERR_INVALID, "attention trace row stride must be >= 1 (got %lld)", (long long)ld);
   s->attn_trace = probs;
   s->attn_ld = probs ? ld : 0;
+  s->attn_ring = 0;
+  return SOPRO_OK;
+}
+
+int sopro_ar_set_attn_trace_ring(sopro_ar_session_t* s, float* probs, int64_t ld, int32_t ring) {
+  if (probs && ring < 1) return fail(SOPRO_ERR_INVALID, "attention trace ring must be >= 1 step (got %d)", ring);
+  const int rc = sopro_ar_set_attn_trace(s, probs, ld);
+  if (rc != SOPRO_OK) return rc;
+  s->attn_ring = probs ? ring : 0;
   return SOPRO_OK;
 }
 

@@ -156,10 +156,11 @@ struct ArParams {
   int g, P, Bt;
   int PH;  // fused Q+attention stage: CTAs per head (P / H); rank r serves head r % H, utterances r / H + j*PH
   int t_begin, t_end;
-  // word timestamps (null = off): every cross-attention weight of step t, [steps][n_attn][B][H][attn_ld] fp32,
-  // attn_step = n_attn * B * H * attn_ld floats per step
+  // word timestamps (null = off): every cross-attention weight of step t, [attn_ring][n_attn][B][H][attn_ld] fp32 in
+  // step row t % attn_ring, attn_step = n_attn * B * H * attn_ld floats per step row
   float* attn_trace;
   long long attn_ld, attn_step;
+  int attn_ring;
 };
 
 // ---------------------------------------------------------------------------
@@ -616,7 +617,7 @@ constexpr int kAttGroup = 256;
 constexpr int kAttG = 32;  // upper bound of the key groups (Dh >= 32)
 constexpr int kAttVU = 8;  // value rows per thread requested together
 
-// word timestamps: the step the CTA is computing (written only by the TRACE instantiations)
+// word timestamps: the trace row of the step the CTA is computing (written only by the TRACE instantiations)
 __shared__ int g_attn_step;
 
 __device__ __forceinline__ void group_sync(int grp) {
@@ -1472,7 +1473,7 @@ __global__ void __launch_bounds__(kThreads, 1) ar_persistent_kernel(const __grid
       s_tok[threadIdx.x] = tok;
       s_done[threadIdx.x] = dn;
     }
-    if (TRACE && threadIdx.x == 0) g_attn_step = t;
+    if (TRACE && threadIdx.x == 0) g_attn_step = t % p.attn_ring;
     if (threadIdx.x < p.n_layers) {  // the only integer divisions of the step: one thread per layer
       const int dl = p.layer[threadIdx.x].dil;
       conv_phase[threadIdx.x] = t % dl;

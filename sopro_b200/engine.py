@@ -210,16 +210,22 @@ class ArSession:
         _lib.check(self.lib.sopro_ar_set_trace(self._h, blocks.data_ptr() if blocks is not None else None,
                                                logits.data_ptr() if logits is not None else None))
 
-    def set_attn_trace(self, probs: Optional[torch.Tensor]) -> None:
+    def set_attn_trace(self, probs: Optional[torch.Tensor], ring: Optional[int] = None) -> None:
         """Word timestamps: later launches store their text cross-attention weights into `probs`, a device f32 tensor
-        [steps, n_attn, batch, H, ld] (ld >= the batch's longest text); None turns the export off."""
+        [steps, n_attn, batch, H, ld] (ld >= the batch's longest text); None turns the export off.  `ring` (streams):
+        `probs` holds `ring` step rows [ring, n_attn, batch, H, ld], step t in row t % ring, and a launch of more than
+        `ring` steps is refused."""
         if probs is None:
             self._attn_trace = None
             _lib.check(self.lib.sopro_ar_set_attn_trace(self._h, None, 0))
             return
         assert probs.dtype == torch.float32 and probs.is_contiguous() and probs.device == self.engine.device and probs.dim() == 5
         self._attn_trace = probs
-        _lib.check(self.lib.sopro_ar_set_attn_trace(self._h, probs.data_ptr(), int(probs.shape[-1])))
+        if ring is None:
+            _lib.check(self.lib.sopro_ar_set_attn_trace(self._h, probs.data_ptr(), int(probs.shape[-1])))
+        else:
+            assert int(probs.shape[0]) >= int(ring)
+            _lib.check(self.lib.sopro_ar_set_attn_trace_ring(self._h, probs.data_ptr(), int(probs.shape[-1]), int(ring)))
 
     def set_timing(self, buf: Optional[torch.Tensor], step: int = -1) -> None:
         self._timing = buf

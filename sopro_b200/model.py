@@ -125,9 +125,11 @@ class SoproModel:
         return self
 
     @contextlib.contextmanager
-    def _lease(self, batch: int, steps: int, text_len: int, attn_trace: Optional[torch.Tensor]) -> Iterator[ArSession]:
+    def _lease(self, batch: int, steps: int, text_len: int, attn_trace: Optional[torch.Tensor],
+               attn_ring: Optional[int] = None) -> Iterator[ArSession]:
         """An idle session of this geometry (a fresh one when every cached one is in use), held for the `with` block,
-        with `attn_trace` (word timestamps) set on it for that time: sessions are cached and shared."""
+        with `attn_trace` (word timestamps; a ring of `attn_ring` steps when given) set on it for that time: sessions
+        are cached and shared."""
         key = (int(batch), int(steps), (int(text_len) + 63) // 64 * 64)
         with self._sessions_lock:
             ses = next((x for x in self._sessions.get(key, []) if id(x) not in self._sessions_busy), None)
@@ -145,7 +147,7 @@ class SoproModel:
             self._sessions_busy.add(id(ses))
         try:
             if attn_trace is not None:
-                ses.set_attn_trace(attn_trace)
+                ses.set_attn_trace(attn_trace, attn_ring)
             yield ses
         finally:
             if attn_trace is not None:
@@ -222,7 +224,7 @@ class SoproModel:
                       loop_streak: int = 8, recovery_top_p: float = 0.85, recovery_temp: float = 1.2,
                       min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                       generator: Optional[torch.Generator] = None, progress: Optional[dict] = None,
-                      attn_trace: Optional[torch.Tensor] = None):
+                      attn_trace: Optional[torch.Tensor] = None, attn_ring: Optional[int] = None):
         """The persistent kernel over B utterances in one session (cond [B, >= steps, D], txt [B, Lmax, D], lens),
         driven `chunk_frames` frames per launch (0 = the whole utterance in one launch): every launch advances all of
         them by the same steps.  Yields ``(tokens, finished, prefetch)`` per launch: one list of new frames (ints) and
@@ -235,7 +237,7 @@ class SoproModel:
         abandoned: on exit its generator is settled to ``progress["consumed"]`` frames (default: every frame yielded),
         i.e. exactly the draws the reference would have made; several rows' are never settled.  `attn_trace` (word
         timestamps): a [max_frames + 1, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text
-        cross-attention weights."""
+        cross-attention weights; with `attn_ring` (streams) a ring of that many step rows, at least `chunk_frames`."""
         B, steps = int(cond.size(0)), int(max_frames) + 1
         if cond.size(1) < steps:
             raise ValueError(f"cond_ar has {cond.size(1)} rows, need max_frames+1 = {steps}")
@@ -245,7 +247,7 @@ class SoproModel:
         lens = [int(x) for x in lens]
         with TapeFeed(B, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device,
                       None if seeds is None else [int(x) for x in seeds], generator) as feed, \
-                self._lease(B, steps, max(lens), attn_trace) as ses:
+                self._lease(B, steps, max(lens), attn_trace, attn_ring) as ses:
             launches = self._launch_blocks(ses, feed, [(a, min(steps, a + per)) for a in range(0, steps, per)],
                                            cond[:, :steps], txt, lens, samp)
 
@@ -724,7 +726,10 @@ class SoproTTS:
     def stream(self, text: str, *, sample_rate: Optional[int] = None, speed: Optional[float] = None,
                watermark: Optional[int] = None, **kwargs) -> Iterator[torch.Tensor]:
         """Chunks of one utterance as they are generated (sopro_b200/streaming.py).  There is no `best_of` here: a
-        stream plays its take while it is generated, so it cannot choose among takes before playing one."""
+        stream plays its take while it is generated, so it cannot choose among takes before playing one.
+        `word_timestamps=True` (extension) yields ``(wav, words)``: the words that became final since the previous
+        item, aligned causally on the GPU (sopro_b200/timestamps.py, lag STREAM_ALIGN_LAG frames); times are seconds of
+        this stream's audio, scaled by `speed` as in synthesize.  The chunks are the same as without it."""
         from .streaming import stream as _stream
 
         return _stream(self, text, sample_rate=sample_rate, speed=speed, watermark=watermark, **kwargs)
@@ -734,7 +739,7 @@ class SoproTTS:
                      temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
                      min_gen_frames: Optional[int] = None, chunk_frames: int = 6, nar_context_frames: Optional[int] = None,
                      sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                     watermark: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor, bool]]:
+                     watermark: Optional[int] = None, word_timestamps: bool = False) -> Iterator[tuple]:
         """NEW: many texts streamed side by side through one chunk loop (sopro_b200/streaming.py): one AR launch of
         `chunk_frames` frames for every row, one ragged NAR pass and one batched Mimi stream step per chunk.  Yields
         ``(i, wav [1, n] on the device at the output rate, last)``; within a chunk the rows come in index order.  Row i
@@ -745,10 +750,11 @@ class SoproTTS:
         final chunk (or empty when the stream yielded nothing more).  Without seeds the rows draw their noise as
         synthesize_batch(texts) does, every tape in full, row after row, from the global generator; that draw happens
         before the first AR launch, so time to first audio wants seeds (one text behaves exactly as stream(), generator
-        included).  There is no loudness (it needs the whole utterance), best_of (see stream) or word_timestamps.
+        included).  There is no loudness (it needs the whole utterance) or best_of (see stream).  `word_timestamps=True`
+        yields ``(i, wav, last, words)``: row i's words that became final since its previous item (see stream).
         Refused before any device work or random draw: empty `texts`, `seeds` of another length, a wrong `ref`
         sequence, `chunk_frames` outside [1, 256], a refused sample_rate / speed / watermark, more texts than
-        min(the AR batch limit, 256).  Closing the generator early releases its AR session, noise tapes, Mimi state and
+        min(the AR batch limit, 256), a non-bool `word_timestamps`, and with it a text over 2048 tokens.  Closing the generator early releases its AR session, noise tapes, Mimi state and
         output-chain states."""
         from .streaming import stream_batch as _stream_batch
 
@@ -756,7 +762,7 @@ class SoproTTS:
                              temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
                              min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
                              nar_context_frames=nar_context_frames, sample_rate=sample_rate, speed=speed,
-                             watermark=watermark)
+                             watermark=watermark, word_timestamps=word_timestamps)
 
     def stream_long(self, text: str, *, ref: PreparedReference, seed: Optional[int] = None, max_frames: int = 400,
                     max_tokens: int = 64, pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05,

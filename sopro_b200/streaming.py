@@ -25,13 +25,17 @@ def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_t
            anti_loop: bool = True, style_strength: Optional[float] = None, ref_seconds: Optional[float] = None,
            chunk_frames: int = 6, nar_context_frames: Optional[int] = None, min_gen_frames: Optional[int] = None,
            seed: Optional[int] = None, generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
-           speed: Optional[float] = None, watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
+           speed: Optional[float] = None, watermark: Optional[int] = None, word_timestamps: bool = False):
     """SoproTTS.stream: the chunk loop over one text.  `sample_rate` (extension): chunks at this rate (None = 24 kHz).
     `speed` (extension): the speaking rate in [0.25, 4.0] (None = the model's own).  `watermark` (extension): a key in
     [0, 2^32) to mark the audio with (None = no mark).  Each chunk's audio goes through a time-stretch stream, a
     watermark stream, then a resampler stream, right after its Mimi step, so the chunks concatenate to the one-shot
     stretch, mark and resample of the 24 kHz stream bit for bit; the last chunk also carries their tails.  A refused
-    sample_rate / speed / watermark raises here, at the call, not at the first chunk."""
+    sample_rate / speed / watermark raises here, at the call, not at the first chunk.  `word_timestamps` (extension):
+    yield ``(wav, words)`` instead, `words` the WordTimings that became final since the previous item (see
+    _chunk_loop); if words are still pending when the stream ends without more audio, the last item is
+    ``([1, 0] wav, words)``.  The chunks are the same as without it."""
+    spans = _word_spans(tts, [text], word_timestamps)
     post = OutputChain(tts, sample_rate, speed, watermark=watermark)
     dec = _decoder(tts, chunk_frames)
 
@@ -43,11 +47,17 @@ def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_t
         rows = _chunk_loop(tts, dec, [tts.encode_text(text)], voice, post, max_frames=max_frames, top_p=top_p,
                            temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
                            chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
-                           min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator)
+                           min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator,
+                           word_texts=None if spans is None else [text], word_spans=spans)
         try:
-            for _i, wav, _last in rows:
-                if wav is not None:
-                    yield wav
+            for _i, wav, last, words in rows:
+                if spans is None:
+                    if wav is not None:
+                        yield wav
+                elif wav is not None:
+                    yield wav, words
+                elif last and words:
+                    yield torch.zeros(1, 0, device=tts.device), words
         finally:
             rows.close()
 
@@ -61,7 +71,7 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
                  top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
                  style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None, chunk_frames: int = 6,
                  nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                 watermark: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor, bool]]:
+                 watermark: Optional[int] = None, word_timestamps: bool = False) -> Iterator[tuple]:
     """SoproTTS.stream_batch: every argument is checked here, before any device work or random draw; the returned
     generator runs the chunk loop over the texts."""
     from . import voices
@@ -81,6 +91,7 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
             raise ValueError(f"{len(seeds)} seeds for {len(texts)} texts")
     voices.check_voices(ref, len(texts), **voices.geometry(tts.cfg))
     _check_chunk_frames(chunk_frames)
+    spans = _word_spans(tts, texts, word_timestamps)
     post = OutputChain(tts, sample_rate, speed, watermark=watermark)
     dec = _decoder(tts, chunk_frames)
 
@@ -88,10 +99,12 @@ def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int
         ids = [tts.encode_text(t) for t in texts]
         rows = _chunk_loop(tts, dec, ids, ref, post, max_frames=max_frames, top_p=top_p, temperature=temperature,
                            anti_loop=anti_loop, style_strength=style_strength, chunk_frames=chunk_frames,
-                           nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames, seeds=seeds)
+                           nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames, seeds=seeds,
+                           word_texts=None if spans is None else texts, word_spans=spans)
         try:
-            for i, wav, last in rows:
-                yield i, (wav if wav is not None else torch.zeros(1, 0, device=tts.device)), last
+            for i, wav, last, words in rows:
+                wav = wav if wav is not None else torch.zeros(1, 0, device=tts.device)
+                yield (i, wav, last) if spans is None else (i, wav, last, words)
         finally:
             rows.close()
 
@@ -205,6 +218,21 @@ def stream_long(tts, text: str, *, ref, seed: Optional[int] = None, max_frames: 
     return passage()
 
 
+def _word_spans(tts, texts: Sequence[str], word_timestamps) -> Optional[list]:
+    """`word_timestamps` checked -> the texts' token character spans (None without it).  Host work only."""
+    from .timestamps import MAX_TOKENS
+
+    if not isinstance(word_timestamps, bool):
+        raise TypeError(f"word_timestamps must be a bool, got {type(word_timestamps).__name__}")
+    if not word_timestamps:
+        return None
+    spans = [tts.tokenizer.encode_with_offsets(t)[1] for t in texts]
+    for i, sp in enumerate(spans):
+        if len(sp) > MAX_TOKENS:
+            raise ValueError(f"text {i} has {len(sp)} tokens; word timestamps align at most {MAX_TOKENS}")
+    return spans
+
+
 def _check_chunk_frames(chunk_frames) -> None:
     if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int):
         raise TypeError(f"chunk_frames must be an int, got {type(chunk_frames).__name__}")
@@ -227,9 +255,10 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
                 max_frames: int, top_p: float, temperature: float, anti_loop: bool, style_strength: Optional[float],
                 chunk_frames: int, nar_context_frames: Optional[int], min_gen_frames: Optional[int],
                 seeds: Optional[Sequence[int]], generator: Optional[torch.Generator] = None,
-                on_block: Optional[Callable[[Optional[torch.Tensor], List[int], List[bool]], None]] = None
-                ) -> Iterator[Tuple[int, Optional[torch.Tensor], bool]]:
-    """The chunk loop of B utterances (`ref`: one prepared voice, or one per text) -> ``(i, wav or None, last)``:
+                on_block: Optional[Callable[[Optional[torch.Tensor], List[int], List[bool]], None]] = None,
+                word_texts: Optional[Sequence[str]] = None, word_spans: Optional[Sequence[Sequence]] = None
+                ) -> Iterator[Tuple[int, Optional[torch.Tensor], bool, Optional[list]]]:
+    """The chunk loop of B utterances (`ref`: one prepared voice, or one per text) -> ``(i, wav or None, last, words)``:
     per launch, in row order, each live row's chunk (None when it has no samples), the row's last item once with
     last=True.  All rows advance in lockstep, `chunk_frames` AR frames per launch, so the NAR window [lo, end) is
     shared by the live rows (only a row that ends in this launch has a shorter one) and runs as one ragged NAR pass;
@@ -238,7 +267,11 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
     `on_block` (stream_long's trim stage): called once per launch, on the stream the launch's Mimi step ran on, with
     the step's decoded block [B, L] (None when nothing was decoded), each row's new samples in it (0 for a row that
     did not run) and whether each row ends with this launch; the loop synchronises that stream before it yields the
-    launch's items."""
+    launch's items.  `word_texts` / `word_spans` (word timestamps): the texts and their tokens' character spans; the
+    AR launches then write their attention weights into a ring of `chunk_frames` steps, each launch's new frames are
+    aligned by one push of a timestamps.StreamAligner on the side stream ahead of that launch's NAR and Mimi step (the
+    main stream's wait for the side stream orders it before the next launch overwrites the ring), and each item's
+    fourth element is the list of the row's words that became final since its previous item (None without them)."""
     model = tts.model
     B = len(text_ids)
     st_ = float(style_strength if style_strength is not None else tts.cfg.style_strength)
@@ -289,16 +322,25 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
         emitted = end
         return out
 
+    aligner = None
+    if word_spans is not None:
+        from .timestamps import StreamAligner
+
+        aligner = StreamAligner(tts.cfg, word_texts, word_spans, ring=cf, max_frames=int(max_frames) + 1, hop=hop,
+                                S=post.S, device=tts.device)
+    pending: List[list] = [[] for _ in range(B)]
     progress = {"consumed": 0}
     chunks = model.ar_chunk_rows(cond, txt, lens, max_frames=max_frames, chunk_frames=cf, top_p=top_p,
                                  temperature=temperature, anti_loop=anti_loop, min_gen_frames=min_gen_frames,
-                                 seeds=seeds, generator=generator, progress=progress)
+                                 seeds=seeds, generator=generator, progress=progress,
+                                 attn_trace=None if aligner is None else aligner.ring,
+                                 attn_ring=None if aligner is None else cf)
     try:
         for _ in range(B):
             posts.append(post.stream(dec.max_chunk_frames * hop))
         for toks_rows, finished, prefetch in chunks:
             live = [b for b in range(B) if not ended[b]]
-            ends, last = [0] * B, [False] * B
+            ends, last, new = [0] * B, [False] * B, [0] * B
             for b in live:
                 toks = toks_rows[b]
                 # the stream ends at the first EOS regardless of min_gen_frames (reference streaming.py:114-115)
@@ -307,12 +349,15 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
                     toks = toks[: toks.index(model.eos_id)]
                 progress["consumed"] += len(toks) + (1 if stop else 0)  # the reference also draws for the EOS step
                 hist[b].extend(toks)
+                new[b] = len(toks)
                 last[b] = stop or finished[b]
                 ends[b] = len(hist[b]) if last[b] else (len(hist[b]) // cf) * cf
             done = all(last[b] for b in live)
             if on_gpu:
                 side.wait_stream(main)
                 with torch.cuda.stream(side):
+                    if aligner is not None:
+                        aligner.push(new, last)
                     wavs = refine_and_emit(ends, last, live)
                 if not done:
                     main.wait_stream(side)  # AR(k+1) behind chunk k's NAR + Mimi, never in front of them
@@ -324,13 +369,18 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
             else:
                 wavs = refine_and_emit(ends, last, live)
             for b in live:
+                if aligner is not None:
+                    pending[b] += aligner.take(b)
                 if wavs[b] is not None or last[b]:
-                    yield b, wavs[b], last[b]
+                    words, pending[b] = (pending[b], []) if aligner is not None else (None, pending[b])
+                    yield b, wavs[b], last[b], words
                 ended[b] = last[b]
             if done:
                 break
     finally:
         chunks.close()
+        if aligner is not None:
+            aligner.close()
         dec.release(state)
         for p in posts:
             p.release()

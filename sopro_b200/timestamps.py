@@ -15,6 +15,13 @@ the host maps tokens to words and frames to seconds of the returned audio:
   sum of the earlier non-empty extents plus one pause each), before the speed scaling.  The words of a skipped segment
   sit at O_i with zero length.
 
+A stream (``stream`` / ``stream_batch`` with ``word_timestamps=True``) cannot wait for the whole utterance: the AR kernel
+writes the weights into a ring of one chunk's steps, and ``StreamAligner`` aligns them as they come with the causal
+rule of include/sopro_b200.h (fixed-lag Viterbi with binding commits, lag ``STREAM_ALIGN_LAG`` frames).  A word is
+final, and handed out, once the committed path has passed its last token (or at the row's end); its timing is then the
+mapping above applied to the committed path, and never changes.  Unlike the one-shot alignment, a stream with fewer
+frames than tokens still gets its committed words, then zero-length ones at its end.
+
 The timings are as good as the checkpoint's attention is monotone; the alignment's mechanics are exact."""
 from __future__ import annotations
 
@@ -30,6 +37,10 @@ import torch
 from . import _lib
 
 SAMPLE_RATE = 24000
+MAX_TOKENS = 2048  # the longest text either alignment takes
+# frames between a frame's generation and the commit of its token in a stream: 4 default chunks, 1.92 s of audio.
+# Whether this trades latency for agreement with the one-shot path well on the released checkpoint is not measured.
+STREAM_ALIGN_LAG = 24
 _WORD = re.compile(r"\S+")
 _NONSPACE = re.compile(r"\S")
 Span = Optional[Tuple[int, int]]
@@ -138,9 +149,109 @@ def utterance_timings(text: str, spans: Sequence[Span], first: Optional[np.ndarr
     if first is None or L == 0 or int(first[0]) < 0:
         return []
     ws = words(text)
-    fr = word_frames([int(v) for v in first[:L]], T, token_words(text, spans, ws), len(ws))
+    return _timings(text, ws, token_words(text, spans, ws), first, T, hop, S)
+
+
+def _timings(text: str, ws: Sequence[Tuple[int, int]], owner: Sequence[Optional[int]], first, T: int, hop: int,
+             S: Optional[int]) -> List[WordTiming]:
+    fr = word_frames([int(v) for v in first[:len(owner)]], T, owner, len(ws))
     return [WordTiming(text[a:b], sample_seconds(f0 * hop, S), sample_seconds(f1 * hop, S), a, b)
             for (a, b), (f0, f1) in zip(ws, fr)]
+
+
+class WordEmitter:
+    """One stream row's words, handed out in text order as they become final: word k is final once the first frame
+    of end_tok[k] is committed (one past the last token of words <= k; L: only at the row's end)."""
+
+    def __init__(self, text: str, spans: Sequence[Span], hop: int, S: Optional[int]):
+        self.text, self.hop, self.S = text, int(hop), S
+        self.ws = words(text)
+        self.owner = token_words(text, spans, self.ws)
+        last = [-1] * len(self.ws)
+        for l, k in enumerate(self.owner):
+            if k is not None:
+                last[k] = l
+        run, self.end_tok = -1, []
+        for x in last:
+            run = max(run, x)
+            self.end_tok.append(run + 1)
+        self.taken = 0
+
+    def take(self, first: np.ndarray, K: int, T: int, ended: bool) -> List[WordTiming]:
+        """The words that became final since the last take, from the committed path: `first` (first frames, -1 where
+        not committed), `K` tokens committed, `T` frames so far, `ended` (then `first` is the whole path)."""
+        if ended:
+            n = len(self.ws) if len(self.owner) and int(first[0]) >= 0 else 0
+        else:
+            n = bisect.bisect_left(self.end_tok, int(K))  # end_tok is non-decreasing: the words with end_tok < K
+        if n <= self.taken:
+            return []
+        out = _timings(self.text, self.ws, self.owner, first, int(T), self.hop, self.S)
+        a, self.taken = self.taken, n
+        return out[a:n]
+
+
+class StreamAligner:
+    """Word timestamps of a stream of B rows: the ring trace the AR session writes (``ring``, for
+    ArSession.set_attn_trace(ring, ring=rows)), the streaming alignment's device state, and per row the words handed
+    out so far.  Per launch: ``push`` (on the stream the trace's readers run on, once the launch's steps are in the
+    ring) enqueues the alignment of each row's new frames and the copy of the committed paths to pinned host memory;
+    after the caller has synchronised that stream, ``take(b)`` returns row b's words that became final since the last
+    take, in text order.  `S`: the stretch's fixed-point speed (None without one)."""
+
+    def __init__(self, cfg, texts: Sequence[str], spans: Sequence[Sequence[Span]], *, ring: int, max_frames: int, hop: int,
+                 S: Optional[int], device):
+        if torch.device(device).type != "cuda":
+            raise _lib.SoproError("the streaming alignment needs a CUDA device; there is no CPU path")
+        lens = [len(sp) for sp in spans]
+        B, ld = len(lens), max(lens)
+        self.lib = _lib.load()
+        self.ring = trace_buffer(cfg, ring, B, ld, device)
+        nb = C.c_int64()
+        lag, mf = int(STREAM_ALIGN_LAG), int(max_frames)
+        _lib.check_arg(self.lib.sopro_align_stream_sizes(B, ld, lag, mf, C.byref(nb)))
+        self.state = torch.empty(int(nb.value), dtype=torch.uint8, device=device)
+        h = C.c_void_p()
+        _lib.check_arg(self.lib.sopro_align_stream_create(B, ld, lag, mf, self.state.data_ptr(), C.byref(h)))
+        self._h = h
+        self._out = self.state[: B * (2 + ld) * 4].view(torch.int32).view(B, 2 + ld)  # {F, K, first[ld]} per row
+        self.host = torch.empty((B, 2 + ld), dtype=torch.int32, pin_memory=True)
+        self.device = torch.device(device)
+        self.B, self.ld = B, ld
+        self.rows = [WordEmitter(t, sp, hop, S) for t, sp in zip(texts, spans)]
+        self.frames = [0] * B
+        self.ended = [False] * B
+        lens_c = (C.c_int32 * B)(*lens)
+        _lib.check_arg(self.lib.sopro_align_stream_begin(self._h, lens_c, _lib.stream_ptr(self.device)))
+
+    def push(self, frames: Sequence[int], ends: Sequence[bool]) -> None:
+        """Row b's next frames[b] frames are in the ring; ends[b]: the row ends after them."""
+        B = self.B
+        n = (C.c_int32 * B)(*[int(x) for x in frames])
+        e = (C.c_int32 * B)(*[1 if x else 0 for x in ends])
+        _, n_attn, _, H, ld = (int(x) for x in self.ring.shape)
+        _lib.check_arg(self.lib.sopro_align_stream_push(self._h, self.ring.data_ptr(), int(self.ring.shape[0]), n_attn, B,
+                                                        H, ld, n, e, _lib.stream_ptr(self.device)))
+        for b in range(B):
+            self.frames[b] += int(frames[b])
+            self.ended[b] = self.ended[b] or bool(ends[b])
+        self.host.copy_(self._out, non_blocking=True)
+
+    def take(self, b: int) -> List[WordTiming]:
+        """Row b's words that became final since the last take (the host copy of the last push must have landed)."""
+        row = self.host[b].numpy()
+        return self.rows[b].take(row[2:], int(row[1]), self.frames[b], self.ended[b])
+
+    def close(self) -> None:
+        if getattr(self, "_h", None):
+            self.lib.sopro_align_stream_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def long_timings(text: str, segments: Sequence[str], seg_spans: Sequence[Sequence[Span]],

@@ -803,7 +803,7 @@ struct SamplerSmem {
 };
 
 __device__ __forceinline__ bool cand_before(float av, int ai, float bv, int bi) {
-  // larger value first; ties -> lower index (torch.argmax / topk / sort keep the first)
+  // the device's tie contract: larger value first, ties -> lower index (torch's CPU topk / sort define no tie order)
   return av > bv || (av == bv && ai < bi);
 }
 __device__ __forceinline__ void warp_argmax(float& v, int& i) {
@@ -1087,7 +1087,7 @@ __device__ __noinline__ void sample_utterance(const ArParams& p, int b, int t, f
   //    set {p : bin(p) <= b} -- a superset of the kk largest, a few elements more on typical data.  (b) if the
   //    candidates fit the kCand slots, block-parallel rank ordering both selects and orders them; otherwise (extremely
   //    peaked rows whose kk-th value sits more than 16 octaves below the maximum, or massive ties) the exact radix
-  //    select (cold) runs.  Order everywhere: value desc, index asc (topk/sort keep the first of a tie).
+  //    select (cold) runs.  Order everywhere: value desc, index asc (the contract; torch's topk/sort leave ties open).
   constexpr int kBins = 1024;
   float bm;
   {

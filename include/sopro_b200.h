@@ -850,6 +850,14 @@ int sopro_longform_extents(const float* x, int32_t B, int64_t x_stride, const in
  * geometry is SOPRO_ERR_INVALID before any launch.  No call synchronises or allocates. */
 int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host, int64_t pause,
                         float* y, int64_t y_len, void* stream);
+/* as sopro_longform_join, but pauses_host: HOST i64 [n_nonempty - 1], the zeros before each non-empty span after the
+ * first, each in [0, 48000] (NULL when at most one span is non-empty); gain: DEVICE f32 [n_seg] or NULL (= 1); span i's
+ * samples are gain[i] * (w * x), the faded product rounded first, exactly as sopro_loudness_normalize scales an
+ * already-joined row, so a run of spans with one gain g equals that run joined alone and scaled by g, bit for bit.
+ * sopro_longform_join is this entry point with every pause equal to `pause` and gain = NULL.  The dialogue join uses
+ * it with a sentence pause inside a turn, a turn pause between turns and one loudness gain per turn. */
+int sopro_longform_join_gaps(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host,
+                             const int64_t* pauses_host, const float* gain, float* y, int64_t y_len, void* stream);
 /* Streaming trim: the extent of a row decided while its samples arrive, and the join emitted piece by piece.
  *   Causal rule: frame k (complete once 240 k + 600 samples have arrived) is classified once, when it completes, against
  *   thr_k = max(M_k - 40, -40), M_k the largest dB among frames 0 .. k; an earlier decision is never revisited.  When

@@ -265,6 +265,7 @@ SYMBOLS = {
     "sopro_longform_fade": (_I, [C.c_int32, _VP]),
     "sopro_longform_extents": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP]),
     "sopro_longform_join": (_I, [_VP, C.c_int32, _VP, _VP, C.c_int64, _VP, C.c_int64, _VP]),
+    "sopro_longform_join_gaps": (_I, [_VP, C.c_int32, _VP, _VP, _VP, _VP, _VP, C.c_int64, _VP]),
     "sopro_longform_stream_create": (_I, [C.c_int32, C.c_int64, _I, C.POINTER(_VP)]),
     "sopro_longform_stream_destroy": (_I, [_VP]),
     "sopro_longform_stream_reset": (_I, [_VP, C.c_int32, C.c_int32, _VP]),

@@ -6,7 +6,9 @@
 //     The row is left whole, (0, n), when n < 2400, nothing is voiced, or end - start < 12000.
 //   join: for each non-empty extent in order, x[start, end) with a raised-cosine fade over its first and last
 //     F = min(240, floor(span / 2)) samples, f[i] = 0.5 - 0.5 cos(pi (i + 0.5) / F) (double on the host, fp32 once; one
-//     fp32 multiply per faded sample), and P zero samples between consecutive spans.
+//     fp32 multiply per faded sample), and P zero samples between consecutive spans.  The general join takes a P per gap
+//     and an optional gain per span, y = g * (f * x): the faded product rounded first, then one more fp32 multiply, as
+//     the loudness stage scales an already-joined row.
 //
 // extents_kernel: one CTA per row.  A warp computes a frame: lane l sums x^2 over the frame's samples l, l + 32, ... in
 // order (each product is exact in fp64), then a butterfly; every frame's dB therefore has one fixed value whatever the
@@ -112,6 +114,7 @@ struct JoinSeg {
   const float* src;  // x + start
   long long span, off;
   long long pause;   // zero samples written after the span
+  int seg;           // the segment's index into the gains
 };
 
 struct JoinArgs {
@@ -121,9 +124,10 @@ struct JoinArgs {
 };
 static_assert(sizeof(JoinArgs) <= 4000, "the join's arguments fit the kernel parameter space");
 
-__global__ void __launch_bounds__(kJoinThreads) join_kernel(const JoinArgs a, float* __restrict__ y) {
+__global__ void __launch_bounds__(kJoinThreads) join_kernel(const JoinArgs a, const float* __restrict__ gain, float* __restrict__ y) {
   const JoinSeg s = a.s[blockIdx.y];
   const long long total = s.span + s.pause;
+  const float g = gain ? __ldg(gain + s.seg) : 1.0f;
   float* yo = y + s.off;
   for (long long j = (long long)blockIdx.x * kJoinThreads + threadIdx.x; j < total; j += (long long)gridDim.x * kJoinThreads) {
     float v = 0.0f;
@@ -133,6 +137,7 @@ __global__ void __launch_bounds__(kJoinThreads) join_kernel(const JoinArgs a, fl
         v = __fmul_rn(v, a.f[j]);
       else if (j >= s.span - a.F)
         v = __fmul_rn(v, a.f[s.span - 1 - j]);
+      if (gain) v = __fmul_rn(g, v);
     }
     yo[j] = v;
   }
@@ -321,12 +326,11 @@ int sopro_longform_extents(const float* x, int32_t B, int64_t x_stride, const in
   return SOPRO_OK;
 }
 
-int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host, int64_t pause,
-                        float* y, int64_t y_len, void* stream) {
+int sopro_longform_join_gaps(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host,
+                             const int64_t* pauses_host, const float* gain, float* y, int64_t y_len, void* stream) {
   if (!src || !lens_host || !ext_host) return fail(SOPRO_ERR_INVALID, "null argument");
   if (n_seg < 1) return fail(SOPRO_ERR_INVALID, "n_seg = %d < 1", n_seg);
-  if (pause < 0 || pause > kMaxPause) return fail(SOPRO_ERR_INVALID, "pause of %lld samples not in [0, %lld]", (long long)pause, kMaxPause);
-  long long total = 0, last = -1;
+  long long total = 0, last = -1, spans = 0;
   for (int i = 0; i < n_seg; ++i) {
     const long long len = lens_host[i], s = ext_host[2 * i], e = ext_host[2 * i + 1];
     if (len < 0 || len > kMaxLen) return fail(SOPRO_ERR_INVALID, "lens[%d] = %lld not in [0, 2^40]", i, len);
@@ -334,21 +338,31 @@ int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* l
       return fail(SOPRO_ERR_INVALID, "extent [%lld, %lld) of segment %d is not inside its %lld samples", s, e, i, len);
     if (e > s && !src[i]) return fail(SOPRO_ERR_INVALID, "null source for segment %d", i);
     if (e > s) {
-      total += (last >= 0 ? pause : 0) + (e - s);
+      if (last >= 0) {
+        if (!pauses_host) return fail(SOPRO_ERR_INVALID, "null argument");
+        const long long p = pauses_host[spans - 1];
+        if (p < 0 || p > kMaxPause)
+          return fail(SOPRO_ERR_INVALID, "pause %lld of %lld samples not in [0, %lld]", spans - 1, p, kMaxPause);
+        total += p;
+      }
+      total += e - s;
       last = i;
+      ++spans;
     }
   }
   if (y_len != total) return fail(SOPRO_ERR_INVALID, "y_len = %lld, the joined length is %lld", (long long)y_len, total);
   if (total == 0) return SOPRO_OK;
   if (!y) return fail(SOPRO_ERR_INVALID, "null argument");
-  // each span's place in y, then one launch per (fade length, run of at most kSegsPerLaunch segments)
-  std::vector<long long> off(n_seg, 0);
+  // each span's place in y and the pause after it, then one launch per (fade length, run of at most kSegsPerLaunch
+  // segments)
+  std::vector<long long> off(n_seg, 0), after(n_seg, 0);
   std::vector<char> done(n_seg, 1);
-  for (long long i = 0, o = 0; i < n_seg; ++i) {
+  for (long long i = 0, o = 0, m = 0; i < n_seg; ++i) {
     const long long span = ext_host[2 * i + 1] - ext_host[2 * i];
     if (span == 0) continue;
     off[i] = o;
-    o += span + pause;
+    after[i] = i == last ? 0 : pauses_host[m++];
+    o += span + after[i];
     done[i] = 0;
   }
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -356,7 +370,7 @@ int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* l
   long long most = 0;  // the longest span + pause of the pending launch
   auto launch = [&]() -> int {
     const unsigned gx = (unsigned)std::min<long long>((most + kJoinThreads - 1) / kJoinThreads, 1024);
-    join_kernel<<<dim3(gx, a.nseg), kJoinThreads, 0, st>>>(a, y);
+    join_kernel<<<dim3(gx, a.nseg), kJoinThreads, 0, st>>>(a, gain, y);
     CK(cudaGetLastError());
     a.nseg = 0;
     most = 0;
@@ -375,7 +389,8 @@ int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* l
       s.src = src[j] + ext_host[2 * j];
       s.span = span;
       s.off = off[j];
-      s.pause = j == last ? 0 : pause;
+      s.pause = after[j];
+      s.seg = j;
       most = std::max(most, span + s.pause);
       done[j] = 1;
       if (a.nseg == kSegsPerLaunch) {
@@ -389,6 +404,13 @@ int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* l
     }
   }
   return SOPRO_OK;
+}
+
+int sopro_longform_join(const float* const* src, int32_t n_seg, const int64_t* lens_host, const int64_t* ext_host, int64_t pause,
+                        float* y, int64_t y_len, void* stream) {
+  if (pause < 0 || pause > kMaxPause) return fail(SOPRO_ERR_INVALID, "pause of %lld samples not in [0, %lld]", (long long)pause, kMaxPause);
+  const std::vector<int64_t> pauses(std::max(n_seg, 1), pause);
+  return sopro_longform_join_gaps(src, n_seg, lens_host, ext_host, pauses.data(), nullptr, y, y_len, stream);
 }
 
 int sopro_longform_stream_destroy(sopro_longform_stream_t* s) {

@@ -188,6 +188,23 @@ def _rows(rows_or_chunks) -> List[torch.Tensor]:
     return out
 
 
+def gap_pauses(extents, pause: int, turn_of: Optional[Sequence[int]] = None, turn_pause: int = 0) -> List[int]:
+    """The zeros before each non-empty span after the first, over the non-empty extents (host int64 [n, 2]): `pause`,
+    or `turn_pause` when the previous non-empty span belongs to another turn (`turn_of`: the turn of each segment;
+    None = one turn).  Empty extents take no part: they have neither a span nor a gap."""
+    ext = np.asarray(extents, dtype=np.int64).reshape(-1, 2)
+    out: List[int] = []
+    prev = None
+    for i, (s, e) in enumerate(ext):
+        if int(e) <= int(s):
+            continue
+        t = 0 if turn_of is None else int(turn_of[i])
+        if prev is not None:
+            out.append(int(turn_pause) if t != prev else int(pause))
+        prev = t
+    return out
+
+
 def join_segments(rows_or_chunks: Union[torch.Tensor, Sequence[torch.Tensor]], extents, pause_ms) -> torch.Tensor:
     """Segment rows and their extents -> one waveform [1, 1, N] f32 on the rows' device: each non-empty extent in order,
     its first and last F = min(240, span // 2) samples faded by a raised cosine, round(pause_ms * 24) zeros between
@@ -195,20 +212,39 @@ def join_segments(rows_or_chunks: Union[torch.Tensor, Sequence[torch.Tensor]], e
     sequence of them and of single rows; each row is read in place.  `extents`: int64 [segments, 2]; on the device, it
     is copied to the host here, the one synchronisation."""
     P = pause_samples(pause_ms)
-    rows = _rows(rows_or_chunks)
     ext = (extents.detach().to("cpu") if isinstance(extents, torch.Tensor) else torch.as_tensor(extents)).to(torch.int64)
-    ext = np.ascontiguousarray(ext.numpy().reshape(-1, 2))
+    ext = ext.numpy().reshape(-1, 2)
+    return join_gaps(rows_or_chunks, ext, gap_pauses(ext, P))
+
+
+def join_gaps(rows_or_chunks: Union[torch.Tensor, Sequence[torch.Tensor]], extents, pauses: Sequence[int],
+              gain: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """join_segments with a pause per gap and a gain per span: `extents` on the host (int [segments, 2]), `pauses`
+    the zeros before each non-empty span after the first (gap_pauses), each in [0, 48000]; `gain`: f32 [segments] on
+    the rows' device or None.  Span i's samples are gain[i] times its faded samples, so spans that share a gain equal
+    their own join scaled by it as normalize_loudness scales a row, bit for bit.  Nothing synchronises."""
+    rows = _rows(rows_or_chunks)
+    ext = np.ascontiguousarray(np.asarray(extents, dtype=np.int64).reshape(-1, 2))
     n = len(rows)
     if n == 0 or ext.shape[0] != n:
         raise ValueError(f"{ext.shape[0]} extents for {n} segment rows")
+    spans = [int(e) - int(s) for s, e in ext if int(e) > int(s)]
+    if len(pauses) != max(0, len(spans) - 1):
+        raise ValueError(f"{len(pauses)} pauses for {len(spans)} non-empty spans")
     dev = rows[0].device
-    N = joined_length(ext, P)
+    if gain is not None:
+        if gain.device != dev or gain.dtype != torch.float32 or gain.numel() != n:
+            raise ValueError(f"gain must be f32 [{n}] on {dev}, got {gain.dtype} [{gain.numel()}] on {gain.device}")
+        gain = gain.reshape(-1).contiguous()
+    gaps = np.ascontiguousarray(np.asarray(list(pauses) or [0], dtype=np.int64))
+    N = sum(spans) + int(gaps[: len(pauses)].sum())
     y = torch.empty((1, 1, N), dtype=torch.float32, device=dev)
     src = (C.c_void_p * n)(*[r.data_ptr() if r.numel() else None for r in rows])
     lens = (C.c_int64 * n)(*[int(r.numel()) for r in rows])
     with torch.cuda.device(dev):
-        _lib.check_arg(_lib.load().sopro_longform_join(src, n, lens, ext.ctypes.data, P, y.data_ptr() if N else None, N,
-                                                       _lib.stream_ptr(dev)))
+        _lib.check_arg(_lib.load().sopro_longform_join_gaps(src, n, lens, ext.ctypes.data, gaps.ctypes.data,
+                                                            None if gain is None else gain.data_ptr(),
+                                                            y.data_ptr() if N else None, N, _lib.stream_ptr(dev)))
     return y
 
 
@@ -243,11 +279,18 @@ class StreamJoin:
         """Device rows a passage of `segments` needs: one group's worth, or two slots of `group`."""
         return int(segments) if segments <= group else 2 * int(group)
 
-    def begin(self, segments: int, pause: int, group: int) -> None:
+    def begin(self, segments: int, pause: int, group: int, turn_of: Optional[Sequence[int]] = None,
+              turn_pause: int = 0) -> None:
+        """A passage of `segments` segments in groups of `group`; the gap before a span is `pause`, or `turn_pause`
+        when the previous span belongs to another turn (gap_pauses; `turn_of`: the turn of each segment, None = one)."""
         if self.rows_for(segments, group) > self.rows:
             raise ValueError(f"{segments} segments in groups of {group} need {self.rows_for(segments, group)} rows, "
                              f"the state has {self.rows}")
+        if turn_of is not None and len(turn_of) != int(segments):
+            raise ValueError(f"{len(turn_of)} turns for {int(segments)} segments")
         self.B, self.P, self.G = int(segments), int(pause), int(group)
+        self.TP, self.turn_of = int(turn_pause), None if turn_of is None else [int(t) for t in turn_of]
+        self.prev_turn = None      # the turn of the last span begun
         self.cur, self.pos, self.pause_left, self.spans = 0, -1, 0, 0  # the segment being emitted, its next sample
         self.started = 0           # segments [0, started) have begun
         self.row0 = self.n_rows = 0  # the rows the pushes go to
@@ -314,8 +357,10 @@ class StreamJoin:
                 self.cur += 1
                 continue
             if self.pos < 0:
-                self.pos, self.pause_left = start, (self.P if self.spans else 0)
-                self.spans += 1
+                turn = 0 if self.turn_of is None else self.turn_of[self.cur]
+                gap = self.P if turn == self.prev_turn else self.TP
+                self.pos, self.pause_left = start, (gap if self.spans else 0)
+                self.spans, self.prev_turn = self.spans + 1, turn
             if self.pause_left:
                 z = min(self.pause_left, limit - m)
                 pieces.append((-1, 0, z, 0, -1))

@@ -594,31 +594,10 @@ class SoproTTS:
         segments = LF.split_text(text, self.tokenizer, budget)
         if not segments:
             raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
-        B, group = len(segments), int(LF.SEGMENT_GROUP)
-        if n_best > 1:
-            limit = self._batch_limit()
-            if limit is not None:
-                group = max(1, min(group, limit // n_best))
-        ext = torch.zeros((B, 2), dtype=torch.int64, device=self.device)
-        rows: List[torch.Tensor] = [torch.zeros(0, device=self.device)] * B
-        firsts: List = []
-        all_Ts: List[int] = []
-        for g0 in range(0, B, group):
-            part = segments[g0: g0 + group]
-            seeds = None if seed is None else [int(seed) + g0 + i for i in range(len(part))]
-            tr: Optional[dict] = {} if word_timestamps else None
-            Ts, codes = self._best_codes(part, ref, n_best, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                         anti_loop=anti_loop, style_strength=style_strength,
-                                         min_gen_frames=min_gen_frames, seeds=seeds, trace_out=tr)
-            if word_timestamps:
-                first = TS.align(tr["probs"], tr["lens"], Ts).cpu().numpy()
-                firsts.extend(first[i] for i in range(len(part)))
-                all_Ts.extend(Ts)
-            for chunk, wav, lens in self._decode_chunks(codes, Ts):
-                flat = wav.view(len(chunk), -1)
-                ext[torch.tensor([g0 + i for i in chunk], device=self.device)] = LF.speech_extents(flat, lens=lens)
-                for j, i in enumerate(chunk):
-                    rows[g0 + i] = flat[j, : lens[j]]  # read in place by the join
+        rows, ext, firsts, all_Ts = self._speak_segments(segments, ref, n_best, seed=seed, word_timestamps=word_timestamps,
+                                                          max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                                          anti_loop=anti_loop, style_strength=style_strength,
+                                                          min_gen_frames=min_gen_frames)
         wav = LF.join_segments(rows, ext, pause_ms)  # the one host read: the B extents
         words = None
         if word_timestamps:
@@ -629,6 +608,73 @@ class SoproTTS:
             return (wav, words) if word_timestamps else wav
         wav, _ = post(wav)
         return (wav, words) if word_timestamps else wav
+
+    @torch.inference_mode()
+    def synthesize_dialogue(self, turns: Sequence[Tuple[PreparedReference, str]], *, seed: Optional[int] = None,
+                            pause_ms: float = 250, turn_pause_ms: float = 500, max_frames: int = 400,
+                            max_tokens: int = 64, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                            style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
+                            sample_rate: Optional[int] = None, speed: Optional[float] = None,
+                            loudness: Optional[float] = None, word_timestamps: bool = False, best_of: int = 1,
+                            watermark: Optional[int] = None):
+        """NEW: a script of ``(voice, text)`` turns, in speaking order -> one waveform [1, 1, N] f32 on the device, each
+        turn in its own voice (sopro_b200/dialogue.py).  Each turn's text is cut as synthesize_long cuts a text and the
+        segments of all turns go through the batch path together, SEGMENT_GROUP at a time: segment k of the script
+        equals synthesize(segment, ref=its turn's voice, seed=seed + k) (without a seed the global generator is consumed
+        segment after segment); turns that pass the same PreparedReference object share its prefill slot.  The trimmed
+        segments are joined on the GPU with `pause_ms` between spans of one turn and `turn_pause_ms` between spans of
+        different turns (both in [0, 2000]; consecutive turns by the same voice still get `turn_pause_ms`), then go
+        through the chain of synthesize_long: stretch (`speed`), watermark, resample (`sample_rate`).  `loudness`
+        levels each turn, not the passage: turn j is scaled by normalize_loudness's gain for its own 24 kHz join (what
+        synthesize_long would join for that turn alone), inside the join, before the chain, and there is no
+        passage-level loudness stage.  A turn whose text is empty or whitespace only speaks nothing; segments that
+        produced no frames are skipped; if nothing was produced the result is [1, 1, 0].  `word_timestamps`: also
+        return each turn's words, ``(wav, List[List[WordTiming]])``, their char spans in that turn's text and their
+        times in seconds of the returned audio.  `best_of`: as in synthesize_long, each segment scored against its own
+        voice.  Refused before any device work or random draw: `turns` that is not a non-empty sequence of
+        (PreparedReference, str) pairs (TypeError; ValueError when empty), a script with nothing to speak, a voice of
+        the wrong geometry, `pause_ms` / `turn_pause_ms` / `max_tokens` out of range, a refused sample_rate / speed /
+        loudness / watermark / best_of."""
+        from .dialogue import synthesize_dialogue as _synthesize_dialogue
+
+        return _synthesize_dialogue(self, turns, seed=seed, pause_ms=pause_ms, turn_pause_ms=turn_pause_ms,
+                                    max_frames=max_frames, max_tokens=max_tokens, top_p=top_p, temperature=temperature,
+                                    anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
+                                    sample_rate=sample_rate, speed=speed, loudness=loudness,
+                                    word_timestamps=word_timestamps, best_of=best_of, watermark=watermark)
+
+    def _speak_segments(self, segments: Sequence[str], ref, n_best: int, *, seed: Optional[int], word_timestamps: bool,
+                        max_frames: int, **kw) -> Tuple[List[torch.Tensor], torch.Tensor, list, List[int]]:
+        """The segments of a long-form passage or a dialogue, generated through the batch path SEGMENT_GROUP at a time
+        (segment k with seed seed + k and its own voice when `ref` is a sequence of one voice per segment) and
+        decoded -> (each segment's 24 kHz row, read in place by the join; their extents, int64 [K, 2] on the device;
+        with word_timestamps each segment's first frames and frame count, else empty lists).  Nothing synchronises."""
+        B, group = len(segments), int(LF.SEGMENT_GROUP)
+        if n_best > 1:
+            limit = self._batch_limit()
+            if limit is not None:
+                group = max(1, min(group, limit // n_best))
+        one = isinstance(ref, PreparedReference)
+        ext = torch.zeros((B, 2), dtype=torch.int64, device=self.device)
+        rows: List[torch.Tensor] = [torch.zeros(0, device=self.device)] * B
+        firsts: List = []
+        all_Ts: List[int] = []
+        for g0 in range(0, B, group):
+            part = segments[g0: g0 + group]
+            seeds = None if seed is None else [int(seed) + g0 + i for i in range(len(part))]
+            tr: Optional[dict] = {} if word_timestamps else None
+            Ts, codes = self._best_codes(part, ref if one else list(ref[g0: g0 + group]), n_best, max_frames=max_frames,
+                                         seeds=seeds, trace_out=tr, **kw)
+            if word_timestamps:
+                first = TS.align(tr["probs"], tr["lens"], Ts).cpu().numpy()
+                firsts.extend(first[i] for i in range(len(part)))
+                all_Ts.extend(Ts)
+            for chunk, wav, lens in self._decode_chunks(codes, Ts):
+                flat = wav.view(len(chunk), -1)
+                ext[torch.tensor([g0 + i for i in chunk], device=self.device)] = LF.speech_extents(flat, lens=lens)
+                for j, i in enumerate(chunk):
+                    rows[g0 + i] = flat[j, : lens[j]]  # read in place by the join
+        return rows, ext, firsts, all_Ts
 
     def _timings(self, texts: Sequence[str], spans, probs: torch.Tensor, lens: Sequence[int], Ts: Sequence[int],
                  S: Optional[int]) -> List[List[TS.WordTiming]]:
@@ -790,6 +836,29 @@ class SoproTTS:
                             style_strength=style_strength, min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
                             nar_context_frames=nar_context_frames, sample_rate=sample_rate, speed=speed,
                             watermark=watermark)
+
+    def stream_dialogue(self, turns: Sequence[Tuple[PreparedReference, str]], *, seed: Optional[int] = None,
+                        pause_ms: float = 250, turn_pause_ms: float = 500, max_frames: int = 400, max_tokens: int = 64,
+                        top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                        style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
+                        chunk_frames: int = 6, nar_context_frames: Optional[int] = None,
+                        sample_rate: Optional[int] = None, speed: Optional[float] = None,
+                        watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
+        """NEW: a script of ``(voice, text)`` turns, streamed -> chunks [1, n] f32 on the device at the output rate.
+        stream_long's passage loop over synthesize_dialogue's segments, each streamed in its turn's voice (segment k
+        with seed seed + k), joined as they arrive with synthesize_dialogue's gaps.  The chunks concatenate to the
+        dialogue join of the segments' streamed audio bit for bit under stream_long's condition (no 25 ms frame of a
+        segment above full scale).  There is no loudness (levelling needs a whole turn), best_of or word_timestamps.
+        Refused before any device work or random draw: what synthesize_dialogue refuses, and `chunk_frames` outside
+        [1, 256].  Closing the generator early releases its AR session, noise tapes, Mimi state, trim state and chain
+        states."""
+        from .streaming import stream_dialogue as _stream_dialogue
+
+        return _stream_dialogue(self, turns, seed=seed, pause_ms=pause_ms, turn_pause_ms=turn_pause_ms,
+                                max_frames=max_frames, max_tokens=max_tokens, top_p=top_p, temperature=temperature,
+                                anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
+                                chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
+                                sample_rate=sample_rate, speed=speed, watermark=watermark)
 
     def save_wav(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
         """`sample_rate`: the rate the waveform is at (the one passed to synthesize / stream)."""

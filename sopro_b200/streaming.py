@@ -134,7 +134,41 @@ def stream_long(tts, text: str, *, ref, seed: Optional[int] = None, max_frames: 
     segments = LF.split_text(text, tts.tokenizer, budget)
     if not segments:
         raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
+    return _stream_passage(tts, segments, ref, post, P, seed=seed, max_frames=max_frames, top_p=top_p,
+                           temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
+                           min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
+                           nar_context_frames=nar_context_frames)
+
+
+def stream_dialogue(tts, turns, *, seed: Optional[int] = None, pause_ms: float = 250, turn_pause_ms: float = 500,
+                    max_frames: int = 400, max_tokens: int = 64, top_p: float = 0.9, temperature: float = 1.05,
+                    anti_loop: bool = True, style_strength: Optional[float] = None,
+                    min_gen_frames: Optional[int] = None, chunk_frames: int = 6,
+                    nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None,
+                    speed: Optional[float] = None, watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
+    """SoproTTS.stream_dialogue: every argument is checked here, before any device work or random draw; the returned
+    generator streams the script as stream_long streams a passage, with a voice per segment and the dialogue's gaps."""
+    from . import dialogue as D
+
+    _turns, segments, turn_of, voice_of, P, TP = D.check_script(tts, turns, pause_ms, turn_pause_ms, max_tokens)
+    _check_chunk_frames(chunk_frames)
+    post = OutputChain(tts, sample_rate, speed, watermark=watermark)
+    return _stream_passage(tts, segments, D.segment_voices(voice_of), post, P, turn_of=turn_of, turn_pause=TP, seed=seed,
+                           max_frames=max_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
+                           style_strength=style_strength, min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
+                           nar_context_frames=nar_context_frames)
+
+
+def _stream_passage(tts, segments: Sequence[str], ref, post: OutputChain, P: int, *,
+                    turn_of: Optional[Sequence[int]] = None, turn_pause: int = 0, seed: Optional[int], max_frames: int,
+                    top_p: float, temperature: float, anti_loop: bool, style_strength: Optional[float],
+                    min_gen_frames: Optional[int], chunk_frames: int, nar_context_frames: Optional[int]):
+    """The passage loop of stream_long and stream_dialogue over checked arguments.  `ref`: one voice, or one per
+    segment; `turn_of` / `turn_pause`: the dialogue's gaps (longform.gap_pauses), None for one turn."""
+    from . import longform as LF
+
     B, G = len(segments), int(LF.SEGMENT_GROUP)
+    one = isinstance(ref, PreparedReference)
     hop = tts.codec.engine.hop
     limit = int(chunk_frames) * hop
     dec = _decoder(tts, chunk_frames)
@@ -143,7 +177,7 @@ def stream_long(tts, text: str, *, ref, seed: Optional[int] = None, max_frames: 
     @torch.inference_mode()
     def passage():
         join = tts._join_pool.checkout(LF.StreamJoin.rows_for(B, G), (int(max_frames) + 1) * hop)
-        join.begin(B, P, G)
+        join.begin(B, P, G, turn_of, turn_pause)
         out = post.stream(limit)
         main = torch.cuda.current_stream(tts.device)
         emit = torch.cuda.Stream(tts.device)  # the pieces and the chain: never queued behind the next AR launch
@@ -152,7 +186,8 @@ def stream_long(tts, text: str, *, ref, seed: Optional[int] = None, max_frames: 
         def start(g0):
             part = segments[g0: g0 + G]
             join.start_group(g0, len(part))
-            return _chunk_loop(tts, dec, [tts.encode_text(t) for t in part], ref, bypass, max_frames=max_frames,
+            voice = ref if one else list(ref[g0: g0 + G])
+            return _chunk_loop(tts, dec, [tts.encode_text(t) for t in part], voice, bypass, max_frames=max_frames,
                                top_p=top_p, temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
                                chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
                                min_gen_frames=min_gen_frames,
@@ -198,7 +233,7 @@ def stream_long(tts, text: str, *, ref, seed: Optional[int] = None, max_frames: 
                 y = piece()
                 while y is None and not join.done():
                     if not chunk():
-                        raise RuntimeError("stream_long has nothing to run and nothing certain to emit")
+                        raise RuntimeError("the passage has nothing to run and nothing certain to emit")
                     y = piece()
                 if y is None:
                     break

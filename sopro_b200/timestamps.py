@@ -28,8 +28,9 @@ from __future__ import annotations
 import bisect
 import ctypes as C
 import dataclasses
+import numbers
 import re
-from typing import List, Optional, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -255,14 +256,21 @@ class StreamAligner:
 
 
 def long_timings(text: str, segments: Sequence[str], seg_spans: Sequence[Sequence[Span]],
-                 firsts: Sequence[Optional[np.ndarray]], Ts: Sequence[int], hop: int, extents, pause: int,
-                 S: Optional[int]) -> List[WordTiming]:
+                 firsts: Sequence[Optional[np.ndarray]], Ts: Sequence[int], hop: int, extents,
+                 pause: Union[int, Sequence[int]], S: Optional[int], start: int = 0) -> List[WordTiming]:
     """The words of a synthesize_long passage, their char spans in the original `text`.  extents: int [segments, 2],
-    the join's (e0, e1) per segment; pause: samples between spans."""
+    the join's (e0, e1) per segment; pause: samples between spans, or one per non-empty span, the zeros that follow it
+    (a dialogue's gaps differ: the one after a turn's last span is the turn pause); start: the passage sample at which
+    the first span begins (a dialogue turn's start).  A segment with an empty extent has its words at the sample where
+    the audio continues."""
     ext = np.asarray(extents, dtype=np.int64).reshape(-1, 2)
+    n_spans = int((ext[:, 1] > ext[:, 0]).sum())
+    after = [int(pause)] * n_spans if isinstance(pause, numbers.Integral) else [int(p) for p in pause]
+    if len(after) != n_spans:
+        raise ValueError(f"{len(after)} pauses for {n_spans} non-empty spans")
     text_words = words(text)
     out: List[WordTiming] = []
-    k, O = 0, 0
+    k, O, m = 0, int(start), 0
     for i, seg in enumerate(segments):
         e0, e1 = int(ext[i, 0]), int(ext[i, 1])
         ws = words(seg)
@@ -279,6 +287,7 @@ def long_timings(text: str, segments: Sequence[str], seg_spans: Sequence[Sequenc
             out.append(WordTiming(text[ta:tb], sample_seconds(y0, S), sample_seconds(y1, S), ta, tb))
             k += 1
         if e1 > e0:
-            O += (e1 - e0) + int(pause)
+            O += (e1 - e0) + after[m]
+            m += 1
     assert k == len(text_words), (k, len(text_words))
     return out

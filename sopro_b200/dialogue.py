@@ -7,20 +7,20 @@ same PreparedReference object share one prefill slot, sopro_b200/voices.py).  Th
 spans of one turn and a turn pause between spans of different turns (longform.gap_pauses), and can scale each turn to
 a common loudness: turn j's gain is normalize_loudness's gain for that turn's own join at 24 kHz, applied inside the
 join kernel (longform.join_gaps), so a levelled turn equals normalize_loudness of its solo join bit for bit.  The
-streaming form is streaming.stream_dialogue.  Host planning lives here; the kernels are sopro_b200/csrc/longform.cu."""
+entry points are SoproTTS.synthesize_dialogue and stream_dialogue.  Host planning lives here; the kernels are
+sopro_b200/csrc/longform.cu."""
 from __future__ import annotations
 
-from typing import List, Optional, Sequence, Tuple
+from typing import List, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import longform as LF
-from . import timestamps as TS
 from . import voices
 from .loudness import normalize_loudness
-from .output import OutputChain
 from .prefill import PreparedReference
+
 
 def check_turns(turns) -> List[Tuple[PreparedReference, str]]:
     """The script as a list of (voice, text) pairs; TypeError for anything but a non-empty sequence of
@@ -120,39 +120,3 @@ def turn_placement(ext: np.ndarray, turn_of: Sequence[int], n_turns: int, pauses
                 O += int(ext[k, 1]) - int(ext[k, 0]) + gap
                 m += 1
     return starts, after
-
-
-def synthesize_dialogue(tts, turns, *, seed: Optional[int] = None, pause_ms=250, turn_pause_ms=500,
-                        max_frames: int = 400, max_tokens: int = 64, top_p: float = 0.9, temperature: float = 1.05,
-                        anti_loop: bool = True, style_strength: Optional[float] = None,
-                        min_gen_frames: Optional[int] = None, sample_rate: Optional[int] = None,
-                        speed: Optional[float] = None, loudness: Optional[float] = None, word_timestamps: bool = False,
-                        best_of: int = 1, watermark: Optional[int] = None):
-    """SoproTTS.synthesize_dialogue (see there)."""
-    turns, segments, turn_of, voice_of, P, TP = check_script(tts, turns, pause_ms, turn_pause_ms, max_tokens)
-    post = OutputChain(tts, sample_rate, speed, loudness, watermark)
-    target, post.target = post.target, None  # levelled per turn at 24 kHz, before the chain
-    n_best = tts._check_best_of(best_of, 1)
-    if not isinstance(word_timestamps, bool):
-        raise TypeError(f"word_timestamps must be a bool, got {type(word_timestamps).__name__}")
-    rows, ext_dev, firsts, Ts = tts._speak_segments(segments, segment_voices(voice_of), n_best, seed=seed,
-                                                    word_timestamps=word_timestamps, max_frames=max_frames, top_p=top_p,
-                                                    temperature=temperature, anti_loop=anti_loop,
-                                                    style_strength=style_strength, min_gen_frames=min_gen_frames)
-    ext = ext_dev.cpu().numpy()  # the one host read: the extents
-    pauses = LF.gap_pauses(ext, P, turn_of, TP)
-    gain = None if target is None else turn_gains(rows, ext, turn_of, len(turns), P, target)
-    wav = LF.join_gaps(rows, ext, pauses, gain)
-    words = None
-    if word_timestamps:
-        starts, after = turn_placement(ext, turn_of, len(turns), pauses)
-        hop = tts.codec.engine.hop
-        words = []
-        for j, ((_voice, text), idx) in enumerate(zip(turns, turn_segments(turn_of, len(turns)))):
-            segs = [segments[k] for k in idx]
-            spans = [tts.tokenizer.encode_with_offsets(t)[1] for t in segs]
-            words.append(TS.long_timings(text, segs, spans, [firsts[k] for k in idx], [Ts[k] for k in idx], hop,
-                                         ext[idx].reshape(-1, 2), after[j], post.S, start=starts[j]))
-    if wav.shape[-1]:
-        wav, _ = post(wav)
-    return (wav, words) if word_timestamps else wav

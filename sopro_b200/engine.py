@@ -39,6 +39,30 @@ class Sampling:
             float(self.repetition_penalty), int(self.top_k), int(bool(self.anti_loop)), int(self.loop_streak),
             int(min(int(self.min_gen_frames), 2 ** 31 - 1)), int(bool(self.stop_on_first_eos)))
 
+    def noise_cols(self, vocab: int) -> int:
+        """Exp(1) draws per step the kernel reads: the top_k sorted ranks with top-p (sampling.py:83-84), every
+        vocabulary id on the unsorted multinomial branch taken when top_p >= 1 (sampling.py:88-93)."""
+        return int(self.top_k) if (self.top_p < 1.0 and self.recovery_top_p < 1.0) else int(vocab)
+
+
+@dataclasses.dataclass(frozen=True)
+class Generation:
+    """The generation settings of one call, resolved once from the public keywords and carried to the AR launch:
+    `max_frames` (the AR runs max_frames + 1 steps), the prefill's `style_strength` and the kernel's `sampling`."""
+    max_frames: int
+    style_strength: float
+    sampling: Sampling
+
+    @classmethod
+    def resolve(cls, cfg: SoproTTSConfig, *, max_frames, top_p, temperature, anti_loop, style_strength,
+                min_gen_frames) -> "Generation":
+        """The public keywords -> the settings: style_strength=None and min_gen_frames=None take the config's,
+        top_p=None is no top-p (legal in the reference, sampling.py:69: `top_p is not None and top_p < 1.0`)."""
+        mg = int(cfg.min_gen_frames if min_gen_frames is None else min_gen_frames)
+        samp = Sampling(top_p=1.0 if top_p is None else float(top_p), temperature=float(temperature),
+                        anti_loop=bool(anti_loop), min_gen_frames=min(mg, 2 ** 31 - 1))
+        return cls(int(max_frames), float(cfg.style_strength if style_strength is None else style_strength), samp)
+
 
 def _f32(t: torch.Tensor) -> torch.Tensor:
     return t.detach().to(device="cpu", dtype=torch.float32).contiguous()

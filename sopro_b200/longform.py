@@ -119,6 +119,14 @@ def split_text(text: str, tokenizer, max_tokens: int = 64) -> List[str]:
     return out
 
 
+def passage_segments(text: str, tokenizer, max_tokens: int) -> List[str]:
+    """split_text for synthesize_long and stream_long; ValueError when the text has nothing to speak.  Host only."""
+    segments = split_text(text, tokenizer, max_tokens)
+    if not segments:
+        raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
+    return segments
+
+
 def check_pause(pause_ms) -> float:
     """The pause between segments in ms as a float; ValueError for anything but a real number in [0, 2000].  Host only."""
     if isinstance(pause_ms, (bool, np.bool_)) or not isinstance(pause_ms, numbers.Real) or \

@@ -13,23 +13,26 @@ additionally accepts ``seed=`` / ``generator=`` (an extension) to leave the glob
 from __future__ import annotations
 
 import contextlib
+import dataclasses
 import os
 import threading
 from typing import Dict, Iterator, List, Optional, Sequence, Tuple, Union
 
 import torch
 
+from . import dialogue as D
 from . import ingest
 from . import longform as LF
 from . import prefill as P
 from . import rerank
+from . import streaming as S
 from . import timestamps as TS
 from . import voices
 from ._lib import StatePool
 from .codec import MimiCodec, MimiStreamDecoder
 from .config import TARGET_SR, SoproTTSConfig
 from .denoising import check_denoise
-from .engine import ArEngine, ArSession, Sampling
+from .engine import ArEngine, ArSession, Generation, Sampling
 from .nar import NarEngine
 from .prefill_cuda import PrefillEngine, RefPrepEngine
 from .prefill import PreparedReference
@@ -89,6 +92,21 @@ def _growing_blocks(steps: int) -> List[Tuple[int, int]]:
         edges.append((a, b))
         a, step = b, (step * 3) // 2
     return edges
+
+
+def _check_texts(texts, seeds) -> Tuple[List[str], Optional[List[int]]]:
+    """synthesize_batch's and stream_batch's `texts` and `seeds` -> (the texts, the seeds as ints or None), before any
+    work: TypeError for a str or anything but a sequence, ValueError for no text or a seeds length that differs."""
+    if isinstance(texts, str) or not isinstance(texts, Sequence):
+        raise TypeError(f"texts must be a sequence of strings, got {type(texts).__name__}")
+    texts = list(texts)
+    if not texts:
+        raise ValueError("texts is empty: give at least one text")
+    if seeds is not None:
+        seeds = [int(x) for x in seeds]
+        if len(seeds) != len(texts):
+            raise ValueError(f"{len(seeds)} seeds for {len(texts)} texts")
+    return texts, seeds
 
 
 class SoproModel:
@@ -203,49 +221,32 @@ class SoproModel:
         return self.nar.refine(cond_seq, rvq1_1xT, lens)
 
     # ---- the hot path
-    def _sampling(self, top_p, temperature, anti_loop, loop_streak, recovery_top_p, recovery_temp, min_gen_frames,
-                  stop_on_first_eos) -> Sampling:
-        mg = int(min_gen_frames if min_gen_frames is not None else self.cfg.min_gen_frames)
-        # top_p=None is legal in the reference (sampling.py:69: `top_p is not None and top_p < 1.0`) == no top-p
-        top_p = 1.0 if top_p is None else top_p
-        recovery_top_p = 1.0 if recovery_top_p is None else recovery_top_p
-        return Sampling(top_p=float(top_p), temperature=float(temperature), recovery_top_p=float(recovery_top_p),
-                        recovery_temp=float(recovery_temp), repetition_penalty=1.1, top_k=50, anti_loop=bool(anti_loop),
-                        loop_streak=int(loop_streak), min_gen_frames=min(mg, 2 ** 31 - 1), stop_on_first_eos=stop_on_first_eos)
-
-    def _noise_cols(self, samp: Sampling) -> int:
-        """Exp(1) draws per step the kernel reads: the top_k sorted ranks with top-p (sampling.py:83-84), every
-        vocabulary id on the unsorted multinomial branch taken when top_p >= 1 (sampling.py:88-93)."""
-        return int(samp.top_k) if (samp.top_p < 1.0 and samp.recovery_top_p < 1.0) else int(self.cfg.ar_vocab())
-
     @torch.no_grad()
-    def ar_chunk_rows(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int,
-                      chunk_frames: int = 0, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
-                      loop_streak: int = 8, recovery_top_p: float = 0.85, recovery_temp: float = 1.2,
-                      min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
+    def ar_chunk_rows(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, gen: Generation,
+                      chunk_frames: int = 0, seeds: Optional[Sequence[int]] = None,
                       generator: Optional[torch.Generator] = None, progress: Optional[dict] = None,
                       attn_trace: Optional[torch.Tensor] = None, attn_ring: Optional[int] = None):
         """The persistent kernel over B utterances in one session (cond [B, >= steps, D], txt [B, Lmax, D], lens),
         driven `chunk_frames` frames per launch (0 = the whole utterance in one launch): every launch advances all of
         them by the same steps.  Yields ``(tokens, finished, prefetch)`` per launch: one list of new frames (ints) and
-        one finished flag (EOS past min_gen_frames, or max_frames reached) per row, and a callable that enqueues the NEXT
-        launch right away on the current CUDA stream -- a streaming consumer queues it behind its own NAR + Mimi work so
-        it runs while the audio is handed out; without the call the next launch is enqueued when the generator is
-        resumed.  `seeds` gives row i the private generator of seeds[i]; without them the rows draw from `generator`
+        one finished flag (EOS past the minimum frame count, or max_frames reached) per row, and a callable that
+        enqueues the NEXT launch right away on the current CUDA stream -- a streaming consumer queues it behind its own
+        NAR + Mimi work so it runs while the audio is handed out; without the call the next launch is enqueued when the
+        generator is resumed.  `seeds` gives row i the private generator of seeds[i]; without them the rows draw from `generator`
         (None: the global one) as ar_generate_tensors does: one row's tape block by block, several rows' tapes in full,
         row after row, before the first launch.  One row's frames computed ahead of a consumer that stops early are
         abandoned: on exit its generator is settled to ``progress["consumed"]`` frames (default: every frame yielded),
         i.e. exactly the draws the reference would have made; several rows' are never settled.  `attn_trace` (word
         timestamps): a [max_frames + 1, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text
         cross-attention weights; with `attn_ring` (streams) a ring of that many step rows, at least `chunk_frames`."""
-        B, steps = int(cond.size(0)), int(max_frames) + 1
+        B, steps = int(cond.size(0)), gen.max_frames + 1
         if cond.size(1) < steps:
             raise ValueError(f"cond_ar has {cond.size(1)} rows, need max_frames+1 = {steps}")
-        samp = self._sampling(top_p, temperature, anti_loop, loop_streak, recovery_top_p, recovery_temp, min_gen_frames, False)
+        samp = dataclasses.replace(gen.sampling, stop_on_first_eos=False)
         per = steps if chunk_frames <= 0 else int(chunk_frames)
         st = {"launched": 0, "read": 0, "yielded": 0}
         lens = [int(x) for x in lens]
-        with TapeFeed(B, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device,
+        with TapeFeed(B, steps, self.cfg.ar_vocab(), samp.noise_cols(self.cfg.ar_vocab()), self.device,
                       None if seeds is None else [int(x) for x in seeds], generator) as feed, \
                 self._lease(B, steps, max(lens), attn_trace, attn_ring) as ses:
             launches = self._launch_blocks(ses, feed, [(a, min(steps, a + per)) for a in range(0, steps, per)],
@@ -286,40 +287,42 @@ class SoproModel:
         """Yields (t, token, is_eos) like the reference generator (model.py:218-305).  The persistent kernel runs
         `launch_frames` frames per launch (0 = the whole utterance in one launch); a consumer that stops iterating
         early simply abandons the frames computed ahead, and the RNG is settled to the frames actually consumed."""
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=None, min_gen_frames=min_gen_frames)
+        # top_p=None is no top-p (see Generation.resolve), and so is recovery_top_p=None
+        samp = dataclasses.replace(gen.sampling, loop_streak=int(loop_streak), recovery_temp=float(recovery_temp),
+                                   recovery_top_p=1.0 if recovery_top_p is None else float(recovery_top_p))
         progress = {"consumed": 0}
-        gen = self.ar_chunk_rows(prep["cond_ar"], prep["txt_seq"], [int(prep["txt_seq"].size(1))], max_frames=max_frames,
-                                 chunk_frames=launch_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
-                                 loop_streak=loop_streak, recovery_top_p=recovery_top_p, recovery_temp=recovery_temp,
-                                 min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator,
-                                 progress=progress, attn_trace=attn_trace)
+        chunks = self.ar_chunk_rows(prep["cond_ar"], prep["txt_seq"], [int(prep["txt_seq"].size(1))],
+                                    gen=dataclasses.replace(gen, sampling=samp), chunk_frames=launch_frames,
+                                    seeds=None if seed is None else [seed], generator=generator, progress=progress,
+                                    attn_trace=attn_trace)
         t = 0
         try:
-            for rows, _finished, _prefetch in gen:
+            for rows, _finished, _prefetch in chunks:
                 for tok in rows[0]:
                     progress["consumed"] = t + 1
                     yield t, tok, tok == self.eos_id
                     t += 1
         finally:
-            gen.close()
+            chunks.close()
 
     @torch.no_grad()
-    def ar_generate_tensors(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, max_frames: int, top_p: float = 0.9,
-                            temperature: float = 1.05, anti_loop: bool = True, min_gen_frames: Optional[int] = None,
-                            seeds: Optional[Sequence[int]] = None, stop_on_first_eos: bool = True,
-                            attn_trace: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None,
-                            settle: bool = False):
+    def ar_generate_tensors(self, cond: torch.Tensor, txt: torch.Tensor, lens: Sequence[int], *, gen: Generation,
+                            seeds: Optional[Sequence[int]] = None, attn_trace: Optional[torch.Tensor] = None,
+                            generator: Optional[torch.Generator] = None, settle: bool = False):
         """B utterances in ONE persistent kernel run from batch tensors (cond [B, >=steps, D], txt [B, Lmax, D], lens).
-        -> (tokens [B, steps] int32 numpy, n_tokens [B]).  With `seeds` and at least 64 steps the run is launched in
-        growing blocks (the kernel resumes from its device state), each block's tapes drawn on host threads while the
-        device generates the block before; otherwise in one launch.  `attn_trace` (word timestamps): a
-        [steps, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text cross-attention weights.  Without
-        `seeds` the tapes draw from `generator` (None: the global one), every tape in full, row after row; `settle`
-        (one row, with stop_on_first_eos) then leaves the generator after exactly the draws of the frames generated, up
-        to and including the first EOS, as the reference's generate_tokens does."""
-        B, steps = int(cond.shape[0]), int(max_frames) + 1
-        samp = self._sampling(top_p, temperature, anti_loop, 8, 0.85, 1.2, min_gen_frames, stop_on_first_eos)
+        -> (tokens [B, steps] int32 numpy, n_tokens [B]); each row stops at its first EOS.  With `seeds` and at least 64
+        steps the run is launched in growing blocks (the kernel resumes from its device state), each block's tapes drawn
+        on host threads while the device generates the block before; otherwise in one launch.  `attn_trace` (word
+        timestamps): a [steps, n_attn, B, H, ld] buffer, ld >= max(lens), that receives the text cross-attention
+        weights.  Without `seeds` the tapes draw from `generator` (None: the global one), every tape in full, row after
+        row; `settle` (one row) then leaves the generator after exactly the draws of the frames generated, up to and
+        including the first EOS, as the reference's generate_tokens does."""
+        B, steps = int(cond.shape[0]), gen.max_frames + 1
+        samp = dataclasses.replace(gen.sampling, stop_on_first_eos=True)
         edges = _growing_blocks(steps) if seeds is not None and steps >= 64 else [(0, steps)]
-        with TapeFeed(B, steps, self.cfg.ar_vocab(), self._noise_cols(samp), self.device, seeds, generator) as feed, \
+        with TapeFeed(B, steps, self.cfg.ar_vocab(), samp.noise_cols(self.cfg.ar_vocab()), self.device, seeds, generator) as feed, \
                 self._lease(B, steps, max(int(x) for x in lens), attn_trace) as ses:
             for _ in self._launch_blocks(ses, feed, edges, cond[:, :steps], txt, [int(x) for x in lens], samp):
                 pass
@@ -329,22 +332,19 @@ class SoproModel:
         return toks, n
 
     @torch.no_grad()
-    def generate_codes(self, text_ids: Sequence[torch.Tensor], ref, *, max_frames: int, top_p: float = 0.9,
-                       temperature: float = 1.05, anti_loop: bool = True, style_strength: float = 1.2,
-                       min_gen_frames: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
-                       generator: Optional[torch.Generator] = None, settle: bool = False,
-                       attn_trace: Optional[torch.Tensor] = None,
+    def generate_codes(self, text_ids: Sequence[torch.Tensor], ref, *, gen: Generation,
+                       seeds: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None,
+                       settle: bool = False, attn_trace: Optional[torch.Tensor] = None,
                        info: Optional[dict] = None) -> Tuple[List[int], Optional[torch.Tensor]]:
         """NEW (the reference is batch-1): B texts with one prepared reference, or one each (`ref` as in
         SoproTTS.synthesize_batch): one batched prefill, one persistent AR run until each text's first EOS, one ragged
         NAR pass -> (frames before the first EOS per text, codes [B, Tmax, Q] on the device; None when every text has 0
         frames).  `seeds`, `generator`, `settle`, `attn_trace`: see ar_generate_tensors.  `info` (best-of-N): receives
         "stopped", whether each row sampled an EOS, and "text_lens"."""
-        txt_seq, lens, _pool, cond = self.prefill.run(list(text_ids), ref, n_frames=int(max_frames) + 1,
-                                                      style_strength=float(style_strength))
-        toks, n = self.ar_generate_tensors(cond, txt_seq, lens, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                           anti_loop=anti_loop, min_gen_frames=min_gen_frames, seeds=seeds,
-                                           attn_trace=attn_trace, generator=generator, settle=settle)
+        txt_seq, lens, _pool, cond = self.prefill.run(list(text_ids), ref, n_frames=gen.max_frames + 1,
+                                                      style_strength=gen.style_strength)
+        toks, n = self.ar_generate_tensors(cond, txt_seq, lens, gen=gen, seeds=seeds, attn_trace=attn_trace,
+                                           generator=generator, settle=settle)
         eos = self.eos_id
         Ts, stopped = [], []
         for i in range(len(lens)):
@@ -370,10 +370,10 @@ class SoproModel:
         """reference model.py:349-401: prefill, AR until the first EOS, cut there, NAR refine -> [T, Q] int64; the
         one-text case of generate_codes, the generator settled as the reference leaves it.  `attn_trace`: see
         ar_generate_tensors."""
-        Ts, codes = self.generate_codes([text_ids_1d], ref, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                        anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
-                                        seeds=None if seed is None else [seed], generator=generator, settle=True,
-                                        attn_trace=attn_trace)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+        Ts, codes = self.generate_codes([text_ids_1d], ref, gen=gen, seeds=None if seed is None else [seed],
+                                        generator=generator, settle=True, attn_trace=attn_trace)
         if codes is None:
             return torch.zeros((0, int(self.cfg.num_codebooks)), dtype=torch.long, device=self.device)
         return codes[0, : Ts[0]]
@@ -511,14 +511,14 @@ class SoproTTS:
         sopro_b200.detect_watermark finds with the same key (sopro_b200/watermark.py)."""
         post = OutputChain(self, sample_rate, speed, loudness, watermark)  # a refused argument raises before any work
         n_best = self._check_best_of(best_of, 1)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
         if ref is None:
             ref = self.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
         tr: Optional[dict] = {} if word_timestamps else None
         # one take settles the generator as the reference's generate_tokens does; best_of takes draw as synthesize_batch
         Ts, codes = self._best_codes([text], ref, n_best, seeds=None if seed is None else [int(seed)], trace_out=tr,
-                                     generator=generator, settle=n_best == 1, max_frames=max_frames, top_p=top_p,
-                                     temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
-                                     min_gen_frames=min_gen_frames)
+                                     gen=gen, generator=generator, settle=n_best == 1)
         words = None
         if word_timestamps:
             spans = self.tokenizer.encode_with_offsets(text)[1]
@@ -546,16 +546,18 @@ class SoproTTS:
         `best_of`: each text's takes are generated in the same pass (B x best_of rows, take k of text i with seed
         seeds[i] + k, in text i's voice) and only the picked take of each text is decoded (see synthesize; text i's takes
         are scored against its own voice's sv_ref).  `watermark`: every utterance carries the key's mark (see
-        synthesize).  A `ref` sequence of the wrong length (ValueError), an element that is not a PreparedReference
-        (TypeError), a voice of another geometry or outside [1, 4096] reference frames (ValueError) or with a key
-        padding mask (NotImplementedError) is refused before any device work or random draw."""
+        synthesize).  Refused before any device work or random draw: `texts` that is a str or not a sequence
+        (TypeError), no text or `seeds` of another length (ValueError), a `ref` sequence of the wrong length
+        (ValueError), an element that is not a PreparedReference (TypeError), a voice of another geometry or outside
+        [1, 4096] reference frames (ValueError) or with a key padding mask (NotImplementedError)."""
         post = OutputChain(self, sample_rate, speed, loudness, watermark)
+        texts, seeds = _check_texts(texts, seeds)
         n_best = self._check_best_of(best_of, len(texts))
         voices.check_voices(ref, len(texts), **voices.geometry(self.cfg))
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
         tr: Optional[dict] = {} if word_timestamps else None
-        Ts, codes = self._best_codes(texts, ref, n_best, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                     anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
-                                     seeds=seeds, trace_out=tr)
+        Ts, codes = self._best_codes(texts, ref, n_best, seeds=seeds, trace_out=tr, gen=gen)
         words = None
         if word_timestamps:
             spans = [self.tokenizer.encode_with_offsets(t)[1] for t in texts]
@@ -591,13 +593,11 @@ class SoproTTS:
         n_best = self._check_best_of(best_of, 1)
         LF.check_pause(pause_ms)
         budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
-        segments = LF.split_text(text, self.tokenizer, budget)
-        if not segments:
-            raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
+        segments = LF.passage_segments(text, self.tokenizer, budget)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
         rows, ext, firsts, all_Ts = self._speak_segments(segments, ref, n_best, seed=seed, word_timestamps=word_timestamps,
-                                                          max_frames=max_frames, top_p=top_p, temperature=temperature,
-                                                          anti_loop=anti_loop, style_strength=style_strength,
-                                                          min_gen_frames=min_gen_frames)
+                                                          gen=gen)
         wav = LF.join_segments(rows, ext, pause_ms)  # the one host read: the B extents
         words = None
         if word_timestamps:
@@ -634,21 +634,42 @@ class SoproTTS:
         voice.  Refused before any device work or random draw: `turns` that is not a non-empty sequence of
         (PreparedReference, str) pairs (TypeError; ValueError when empty), a script with nothing to speak, a voice of
         the wrong geometry, `pause_ms` / `turn_pause_ms` / `max_tokens` out of range, a refused sample_rate / speed /
-        loudness / watermark / best_of."""
-        from .dialogue import synthesize_dialogue as _synthesize_dialogue
-
-        return _synthesize_dialogue(self, turns, seed=seed, pause_ms=pause_ms, turn_pause_ms=turn_pause_ms,
-                                    max_frames=max_frames, max_tokens=max_tokens, top_p=top_p, temperature=temperature,
-                                    anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
-                                    sample_rate=sample_rate, speed=speed, loudness=loudness,
-                                    word_timestamps=word_timestamps, best_of=best_of, watermark=watermark)
+        loudness / watermark / best_of, a non-bool `word_timestamps`."""
+        turns, segments, turn_of, voice_of, pause, turn_pause = D.check_script(self, turns, pause_ms, turn_pause_ms,
+                                                                               max_tokens)
+        post = OutputChain(self, sample_rate, speed, loudness, watermark)
+        target, post.target = post.target, None  # levelled per turn at 24 kHz, before the chain
+        n_best = self._check_best_of(best_of, 1)
+        TS.check_word_timestamps(word_timestamps)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+        rows, ext_dev, firsts, Ts = self._speak_segments(segments, D.segment_voices(voice_of), n_best, seed=seed,
+                                                         word_timestamps=word_timestamps, gen=gen)
+        ext = ext_dev.cpu().numpy()  # the one host read: the extents
+        pauses = LF.gap_pauses(ext, pause, turn_of, turn_pause)
+        gain = None if target is None else D.turn_gains(rows, ext, turn_of, len(turns), pause, target)
+        wav = LF.join_gaps(rows, ext, pauses, gain)
+        words = None
+        if word_timestamps:
+            starts, after = D.turn_placement(ext, turn_of, len(turns), pauses)
+            hop = self.codec.engine.hop
+            words = []
+            for j, ((_voice, text), idx) in enumerate(zip(turns, D.turn_segments(turn_of, len(turns)))):
+                segs = [segments[k] for k in idx]
+                spans = [self.tokenizer.encode_with_offsets(t)[1] for t in segs]
+                words.append(TS.long_timings(text, segs, spans, [firsts[k] for k in idx], [Ts[k] for k in idx], hop,
+                                             ext[idx].reshape(-1, 2), after[j], post.S, start=starts[j]))
+        if wav.shape[-1]:
+            wav, _ = post(wav)
+        return (wav, words) if word_timestamps else wav
 
     def _speak_segments(self, segments: Sequence[str], ref, n_best: int, *, seed: Optional[int], word_timestamps: bool,
-                        max_frames: int, **kw) -> Tuple[List[torch.Tensor], torch.Tensor, list, List[int]]:
+                        **kw) -> Tuple[List[torch.Tensor], torch.Tensor, list, List[int]]:
         """The segments of a long-form passage or a dialogue, generated through the batch path SEGMENT_GROUP at a time
         (segment k with seed seed + k and its own voice when `ref` is a sequence of one voice per segment) and
         decoded -> (each segment's 24 kHz row, read in place by the join; their extents, int64 [K, 2] on the device;
-        with word_timestamps each segment's first frames and frame count, else empty lists).  Nothing synchronises."""
+        with word_timestamps each segment's first frames and frame count, else empty lists).  Nothing synchronises.
+        `kw`: _best_codes's `gen`."""
         B, group = len(segments), int(LF.SEGMENT_GROUP)
         if n_best > 1:
             limit = self._batch_limit()
@@ -663,8 +684,8 @@ class SoproTTS:
             part = segments[g0: g0 + group]
             seeds = None if seed is None else [int(seed) + g0 + i for i in range(len(part))]
             tr: Optional[dict] = {} if word_timestamps else None
-            Ts, codes = self._best_codes(part, ref if one else list(ref[g0: g0 + group]), n_best, max_frames=max_frames,
-                                         seeds=seeds, trace_out=tr, **kw)
+            Ts, codes = self._best_codes(part, ref if one else list(ref[g0: g0 + group]), n_best, seeds=seeds,
+                                         trace_out=tr, **kw)
             if word_timestamps:
                 first = TS.align(tr["probs"], tr["lens"], Ts).cpu().numpy()
                 firsts.extend(first[i] for i in range(len(part)))
@@ -683,24 +704,24 @@ class SoproTTS:
         hop = self.codec.engine.hop
         return [TS.utterance_timings(t, sp, first[i], int(Ts[i]), hop, S) for i, (t, sp) in enumerate(zip(texts, spans))]
 
-    def _best_codes(self, texts: Sequence[str], ref, best_of: int, *, seeds: Optional[Sequence[int]],
+    def _best_codes(self, texts: Sequence[str], ref, best_of: int, *, seeds: Optional[Sequence[int]], gen: Generation,
                     trace_out: Optional[dict] = None, generator: Optional[torch.Generator] = None,
-                    **kw) -> Tuple[List[int], Optional[torch.Tensor]]:
+                    settle: bool = False) -> Tuple[List[int], Optional[torch.Tensor]]:
         """_batch_codes with `best_of` candidates per text (sopro_b200/rerank.py): text i's candidate k is row i*N + k
         of ONE _batch_codes pass, with seed seeds[i] + k and text i's voice; every take is scored with one Token2SV
         launch against its text's voice's sv_ref, rerank.choose picks one per text, and only the picked rows are returned
-        (the trace too), so the caller decodes those alone.  best_of = 1 is _batch_codes itself.  `kw`: those of
-        _batch_codes (`settle` only with best_of = 1)."""
+        (the trace too), so the caller decodes those alone.  best_of = 1 is _batch_codes itself (`settle` only then)."""
         N = int(best_of)
         if N == 1:
-            return self._batch_codes(texts, ref, seeds=seeds, trace_out=trace_out, generator=generator, **kw)
+            return self._batch_codes(texts, ref, seeds=seeds, trace_out=trace_out, gen=gen, generator=generator,
+                                     settle=settle)
         slots, of = voices.voice_slots(ref, len(texts))
         rows = [t for t in texts for _ in range(N)]
         row_ref = slots[0] if len(slots) == 1 else [slots[of[r // N]] for r in range(len(rows))]
         tr: Optional[dict] = {} if trace_out is not None else None
         info: dict = {}
-        Ts, codes = self._batch_codes(rows, row_ref, seeds=rerank.candidate_seeds(seeds, N), trace_out=tr, generator=generator,
-                                      info=info, **kw)
+        Ts, codes = self._batch_codes(rows, row_ref, seeds=rerank.candidate_seeds(seeds, N), trace_out=tr, gen=gen,
+                                      generator=generator, info=info)
         cos = [0.0] * len(rows)
         live = [r for r in range(len(rows)) if Ts[r] > 0]
         if live:  # the takes with frames, in one launch
@@ -734,19 +755,19 @@ class SoproTTS:
             rerank.check_rows(rows * n, self._batch_limit())
         return n
 
-    def _batch_codes(self, texts: Sequence[str], ref, *, max_frames: int, style_strength: Optional[float],
+    def _batch_codes(self, texts: Sequence[str], ref, *, seeds: Optional[Sequence[int]], gen: Generation,
                      trace_out: Optional[dict] = None, **kw) -> Tuple[List[int], Optional[torch.Tensor]]:
         """SoproModel.generate_codes of the texts (`ref` as in synthesize_batch) -> (frames before the first EOS per
         text, codes [B, Tmax, Q]; None when every text has 0 frames).  `trace_out` (word timestamps): receives "probs",
-        the AR launch's attention weights, and "lens", the text lengths."""
+        the AR launch's attention weights, and "lens", the text lengths.  `kw`: generate_codes's `generator`, `settle`
+        and `info`."""
         ids = [self.encode_text(t) for t in texts]
         trace = None
         if trace_out is not None:
             lens = [int(x.numel()) for x in ids]
-            trace = TS.trace_buffer(self.cfg, int(max_frames) + 1, len(ids), max(lens), self.device)
+            trace = TS.trace_buffer(self.cfg, gen.max_frames + 1, len(ids), max(lens), self.device)
             trace_out["probs"], trace_out["lens"] = trace, lens
-        st = float(style_strength if style_strength is not None else self.cfg.style_strength)
-        return self.model.generate_codes(ids, ref, max_frames=max_frames, style_strength=st, attn_trace=trace, **kw)
+        return self.model.generate_codes(ids, ref, gen=gen, seeds=seeds, attn_trace=trace, **kw)
 
     def _decode_chunks(self, codes: Optional[torch.Tensor], Ts: Sequence[int]) -> Iterator[Tuple[List[int], torch.Tensor, List[int]]]:
         """Padded Mimi decodes of the utterances with frames -> yields (indices, wav [rows, 1, L], valid samples per
@@ -769,16 +790,8 @@ class SoproTTS:
             batch = (batch * keep[:, None, :]).contiguous()  # padding frames decode code 0; their samples are cut by lens
             yield chunk, self.codec.engine.decode(batch), [Ts[i] * hop for i in chunk]
 
-    def stream(self, text: str, *, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-               watermark: Optional[int] = None, **kwargs) -> Iterator[torch.Tensor]:
-        """Chunks of one utterance as they are generated (sopro_b200/streaming.py).  There is no `best_of` here: a
-        stream plays its take while it is generated, so it cannot choose among takes before playing one.
-        `word_timestamps=True` (extension) yields ``(wav, words)``: the words that became final since the previous
-        item, aligned causally on the GPU (sopro_b200/timestamps.py, lag STREAM_ALIGN_LAG frames); times are seconds of
-        this stream's audio, scaled by `speed` as in synthesize.  The chunks are the same as without it."""
-        from .streaming import stream as _stream
-
-        return _stream(self, text, sample_rate=sample_rate, speed=speed, watermark=watermark, **kwargs)
+    # the reference's module-level streaming.stream (reference streaming.py:134-143), a method here
+    stream = S.stream
 
     def stream_batch(self, texts: Sequence[str], *, ref: Union[PreparedReference, Sequence[PreparedReference]],
                      seeds: Optional[Sequence[int]] = None, max_frames: int = 400, top_p: float = 0.9,
@@ -802,13 +815,32 @@ class SoproTTS:
         sequence, `chunk_frames` outside [1, 256], a refused sample_rate / speed / watermark, more texts than
         min(the AR batch limit, 256), a non-bool `word_timestamps`, and with it a text over 2048 tokens.  Closing the generator early releases its AR session, noise tapes, Mimi state and
         output-chain states."""
-        from .streaming import stream_batch as _stream_batch
+        texts, seeds = _check_texts(texts, seeds)
+        limit = self._batch_limit()
+        limit = S.MAX_STREAM_ROWS if limit is None else min(int(limit), S.MAX_STREAM_ROWS)
+        if len(texts) > limit:
+            raise ValueError(f"{len(texts)} texts; stream_batch streams at most {limit} side by side on this device")
+        voices.check_voices(ref, len(texts), **voices.geometry(self.cfg))
+        S._check_chunk_frames(chunk_frames)
+        spans = S._word_spans(self, texts, word_timestamps)
+        post = OutputChain(self, sample_rate, speed, watermark=watermark)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+        dec = S._decoder(self, chunk_frames)
 
-        return _stream_batch(self, texts, ref=ref, seeds=seeds, max_frames=max_frames, top_p=top_p,
-                             temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
-                             min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
-                             nar_context_frames=nar_context_frames, sample_rate=sample_rate, speed=speed,
-                             watermark=watermark, word_timestamps=word_timestamps)
+        def rows_of():
+            ids = [self.encode_text(t) for t in texts]
+            rows = S._chunk_loop(self, dec, ids, ref, post, gen=gen, chunk_frames=chunk_frames,
+                                 nar_context_frames=nar_context_frames, seeds=seeds,
+                                 word_texts=None if spans is None else texts, word_spans=spans)
+            try:
+                for i, wav, last, words in rows:
+                    wav = wav if wav is not None else torch.zeros(1, 0, device=self.device)
+                    yield (i, wav, last) if spans is None else (i, wav, last, words)
+            finally:
+                rows.close()
+
+        return rows_of()
 
     def stream_long(self, text: str, *, ref: PreparedReference, seed: Optional[int] = None, max_frames: int = 400,
                     max_tokens: int = 64, pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05,
@@ -829,13 +861,15 @@ class SoproTTS:
         or word_timestamps.  Refused before any device work or random draw: a text with nothing to speak, `pause_ms`
         or `max_tokens` out of range, `chunk_frames` outside [1, 256], a refused sample_rate / speed / watermark.
         Closing the generator early releases its AR session, noise tapes, Mimi state, trim state and chain states."""
-        from .streaming import stream_long as _stream_long
-
-        return _stream_long(self, text, ref=ref, seed=seed, max_frames=max_frames, max_tokens=max_tokens,
-                            pause_ms=pause_ms, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
-                            style_strength=style_strength, min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
-                            nar_context_frames=nar_context_frames, sample_rate=sample_rate, speed=speed,
-                            watermark=watermark)
+        post = OutputChain(self, sample_rate, speed, watermark=watermark)
+        pause = LF.pause_samples(pause_ms)
+        budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
+        S._check_chunk_frames(chunk_frames)
+        segments = LF.passage_segments(text, self.tokenizer, budget)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+        return S._stream_passage(self, segments, ref, post, pause, seed=seed, gen=gen, chunk_frames=chunk_frames,
+                                 nar_context_frames=nar_context_frames)
 
     def stream_dialogue(self, turns: Sequence[Tuple[PreparedReference, str]], *, seed: Optional[int] = None,
                         pause_ms: float = 250, turn_pause_ms: float = 500, max_frames: int = 400, max_tokens: int = 64,
@@ -852,13 +886,14 @@ class SoproTTS:
         Refused before any device work or random draw: what synthesize_dialogue refuses, and `chunk_frames` outside
         [1, 256].  Closing the generator early releases its AR session, noise tapes, Mimi state, trim state and chain
         states."""
-        from .streaming import stream_dialogue as _stream_dialogue
-
-        return _stream_dialogue(self, turns, seed=seed, pause_ms=pause_ms, turn_pause_ms=turn_pause_ms,
-                                max_frames=max_frames, max_tokens=max_tokens, top_p=top_p, temperature=temperature,
-                                anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames,
-                                chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
-                                sample_rate=sample_rate, speed=speed, watermark=watermark)
+        _turns, segments, turn_of, voice_of, pause, turn_pause = D.check_script(self, turns, pause_ms, turn_pause_ms,
+                                                                                max_tokens)
+        S._check_chunk_frames(chunk_frames)
+        post = OutputChain(self, sample_rate, speed, watermark=watermark)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+        return S._stream_passage(self, segments, D.segment_voices(voice_of), post, pause, turn_of=turn_of,
+                                 turn_pause=turn_pause, seed=seed, gen=gen, chunk_frames=chunk_frames, nar_context_frames=nar_context_frames)
 
     def save_wav(self, path: str, wav_1xT: torch.Tensor, sample_rate: int = TARGET_SR) -> None:
         """`sample_rate`: the rate the waveform is at (the one passed to synthesize / stream)."""

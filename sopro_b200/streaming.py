@@ -3,12 +3,13 @@ runs over the new frames plus ``rf_nar`` frames of left context and the Mimi str
 The AR kernel is launched ``chunk_frames`` frames at a time, so time-to-first-audio is prefill + one short
 persistent launch + one NAR window + one Mimi decode.
 
-``stream`` and ``stream_batch`` run one chunk loop (``_chunk_loop``), pipelined.  Per chunk k, in device order:
-AR(k) -> [NAR window + Mimi step](k) -> AR(k+1) -> ...  The host enqueues NAR + Mimi of chunk k on a side stream, then
-immediately enqueues AR(k+1) behind them (an event keeps the persistent kernel, which takes every SM, from cutting in
-front of chunk k's audio), and only then waits for chunk k's samples and yields them: the next AR launch runs while the
-consumer handles the audio, and the device never waits for the host between launches.  The reference runs the three
-stages strictly in turn on one thread (streaming.py:81-130)."""
+``stream`` (SoproTTS.stream) and SoproTTS's other streaming entry points (sopro_b200/model.py) check and resolve their
+arguments, then run the loops here.  ``stream`` and ``stream_batch`` run one chunk loop (``_chunk_loop``), pipelined.
+Per chunk k, in device order: AR(k) -> [NAR window + Mimi step](k) -> AR(k+1) -> ...  The host enqueues NAR + Mimi of
+chunk k on a side stream, then immediately enqueues AR(k+1) behind them (an event keeps the persistent kernel, which
+takes every SM, from cutting in front of chunk k's audio), and only then waits for chunk k's samples and yields them:
+the next AR launch runs while the consumer handles the audio, and the device never waits for the host between
+launches.  The reference runs the three stages strictly in turn on one thread (streaming.py:81-130)."""
 from __future__ import annotations
 
 from typing import Callable, Iterator, List, Optional, Sequence, Tuple
@@ -16,39 +17,46 @@ from typing import Callable, Iterator, List, Optional, Sequence, Tuple
 import torch
 
 from .codec import MimiStreamDecoder
+from .engine import Generation
 from .output import OutputChain
 from .prefill import PreparedReference
 
 
 def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_tq: Optional[torch.Tensor] = None,
-           ref: Optional[PreparedReference] = None, max_frames: int = 400, top_p: float = 0.9, temperature: float = 1.05,
-           anti_loop: bool = True, style_strength: Optional[float] = None, ref_seconds: Optional[float] = None,
-           chunk_frames: int = 6, nar_context_frames: Optional[int] = None, min_gen_frames: Optional[int] = None,
-           seed: Optional[int] = None, generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
-           speed: Optional[float] = None, watermark: Optional[int] = None, word_timestamps: bool = False):
-    """SoproTTS.stream: the chunk loop over one text.  `sample_rate` (extension): chunks at this rate (None = 24 kHz).
-    `speed` (extension): the speaking rate in [0.25, 4.0] (None = the model's own).  `watermark` (extension): a key in
-    [0, 2^32) to mark the audio with (None = no mark).  Each chunk's audio goes through a time-stretch stream, a
-    watermark stream, then a resampler stream, right after its Mimi step, so the chunks concatenate to the one-shot
-    stretch, mark and resample of the 24 kHz stream bit for bit; the last chunk also carries their tails.  A refused
-    sample_rate / speed / watermark raises here, at the call, not at the first chunk.  `word_timestamps` (extension):
-    yield ``(wav, words)`` instead, `words` the WordTimings that became final since the previous item (see
-    _chunk_loop); if words are still pending when the stream ends without more audio, the last item is
+           ref: Optional[PreparedReference] = None, max_frames: int = 400, top_p: float = 0.9,
+           temperature: float = 1.05, anti_loop: bool = True, style_strength: Optional[float] = None,
+           ref_seconds: Optional[float] = None, chunk_frames: int = 6, nar_context_frames: Optional[int] = None,
+           min_gen_frames: Optional[int] = None, seed: Optional[int] = None,
+           generator: Optional[torch.Generator] = None, sample_rate: Optional[int] = None,
+           speed: Optional[float] = None, watermark: Optional[int] = None,
+           word_timestamps: bool = False) -> Iterator[torch.Tensor]:
+    """SoproTTS.stream: chunks [1, n] of one utterance as they are generated, through the chunk loop below.
+    `sample_rate` (extension): chunks at this rate (None = 24 kHz).  `speed` (extension): the speaking rate in
+    [0.25, 4.0] (None = the model's own).  `watermark` (extension): a key in [0, 2^32) to mark the audio with (None =
+    no mark).  Each chunk's audio goes through a time-stretch stream, a watermark stream, then a resampler stream,
+    right after its Mimi step, so the chunks concatenate to the one-shot stretch, mark and resample of the 24 kHz
+    stream bit for bit; the last chunk also carries their tails.  A refused sample_rate / speed / watermark raises
+    here, at the call, not at the first chunk.  There is no `best_of` here: a stream plays its take while it is
+    generated, so it cannot choose among takes before playing one.  `word_timestamps=True` (extension) yields
+    ``(wav, words)``: the words that became final since the previous item, aligned causally on the GPU
+    (sopro_b200/timestamps.py, lag STREAM_ALIGN_LAG frames); times are seconds of this stream's audio, scaled by
+    `speed` as in synthesize.  If words are still pending when the stream ends without more audio, the last item is
     ``([1, 0] wav, words)``.  The chunks are the same as without it."""
     spans = _word_spans(tts, [text], word_timestamps)
     post = OutputChain(tts, sample_rate, speed, watermark=watermark)
+    gen = Generation.resolve(tts.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                             anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
     dec = _decoder(tts, chunk_frames)
 
     @torch.inference_mode()
     def chunks():
         voice = ref
         if voice is None:
-            voice = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq, ref_seconds=ref_seconds)
-        rows = _chunk_loop(tts, dec, [tts.encode_text(text)], voice, post, max_frames=max_frames, top_p=top_p,
-                           temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
-                           chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
-                           min_gen_frames=min_gen_frames, seeds=None if seed is None else [seed], generator=generator,
-                           word_texts=None if spans is None else [text], word_spans=spans)
+            voice = tts.prepare_reference(ref_audio_path=ref_audio_path, ref_tokens_tq=ref_tokens_tq,
+                                          ref_seconds=ref_seconds)
+        rows = _chunk_loop(tts, dec, [tts.encode_text(text)], voice, post, gen=gen, chunk_frames=chunk_frames,
+                           nar_context_frames=nar_context_frames, seeds=None if seed is None else [seed],
+                           generator=generator, word_texts=None if spans is None else [text], word_spans=spans)
         try:
             for _i, wav, last, words in rows:
                 if spans is None:
@@ -67,104 +75,19 @@ def stream(tts, text: str, *, ref_audio_path: Optional[str] = None, ref_tokens_t
 MAX_STREAM_ROWS = 256  # a Mimi stream state holds tens of MB per row (DESIGN.md §5o)
 
 
-def stream_batch(tts, texts: Sequence[str], *, ref, seeds: Optional[Sequence[int]] = None, max_frames: int = 400,
-                 top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
-                 style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None, chunk_frames: int = 6,
-                 nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                 watermark: Optional[int] = None, word_timestamps: bool = False) -> Iterator[tuple]:
-    """SoproTTS.stream_batch: every argument is checked here, before any device work or random draw; the returned
-    generator runs the chunk loop over the texts."""
-    from . import voices
-
-    if isinstance(texts, str) or not isinstance(texts, Sequence):
-        raise TypeError(f"texts must be a sequence of strings, got {type(texts).__name__}")
-    texts = list(texts)
-    if not texts:
-        raise ValueError("texts is empty: stream_batch needs at least one text")
-    limit = tts._batch_limit()
-    limit = MAX_STREAM_ROWS if limit is None else min(int(limit), MAX_STREAM_ROWS)
-    if len(texts) > limit:
-        raise ValueError(f"{len(texts)} texts; stream_batch streams at most {limit} side by side on this device")
-    if seeds is not None:
-        seeds = [int(x) for x in seeds]
-        if len(seeds) != len(texts):
-            raise ValueError(f"{len(seeds)} seeds for {len(texts)} texts")
-    voices.check_voices(ref, len(texts), **voices.geometry(tts.cfg))
-    _check_chunk_frames(chunk_frames)
-    spans = _word_spans(tts, texts, word_timestamps)
-    post = OutputChain(tts, sample_rate, speed, watermark=watermark)
-    dec = _decoder(tts, chunk_frames)
-
-    def rows_of():
-        ids = [tts.encode_text(t) for t in texts]
-        rows = _chunk_loop(tts, dec, ids, ref, post, max_frames=max_frames, top_p=top_p, temperature=temperature,
-                           anti_loop=anti_loop, style_strength=style_strength, chunk_frames=chunk_frames,
-                           nar_context_frames=nar_context_frames, min_gen_frames=min_gen_frames, seeds=seeds,
-                           word_texts=None if spans is None else texts, word_spans=spans)
-        try:
-            for i, wav, last, words in rows:
-                wav = wav if wav is not None else torch.zeros(1, 0, device=tts.device)
-                yield (i, wav, last) if spans is None else (i, wav, last, words)
-        finally:
-            rows.close()
-
-    return rows_of()
-
-
-def stream_long(tts, text: str, *, ref, seed: Optional[int] = None, max_frames: int = 400, max_tokens: int = 64,
-                pause_ms: float = 250, top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
-                style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None, chunk_frames: int = 6,
-                nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None, speed: Optional[float] = None,
-                watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
-    """SoproTTS.stream_long: every argument is checked here, before any device work or random draw; the returned
-    generator streams the passage.
-
-    The segments of synthesize_long run SEGMENT_GROUP at a time, each group through one chunk loop whose decoded
-    blocks go to the streaming trim (longform.StreamJoin) instead of an output chain; the joined 24 kHz passage goes
-    through one output-chain stream.  Each resumption runs at most one AR chunk, then yields the next piece of the
-    passage (at most chunk_frames x 1920 samples of it before the chain); it runs more chunks only while nothing is
-    certain yet.  A group starts at the first resumption after the group before it has ended and the group before
-    that has been emitted (the trim state holds two groups)."""
-    from . import longform as LF
-
-    post = OutputChain(tts, sample_rate, speed, watermark=watermark)
-    P = LF.pause_samples(pause_ms)
-    budget = LF.check_max_tokens(max_tokens, tts.model.prefill.max_text_len)
-    _check_chunk_frames(chunk_frames)
-    segments = LF.split_text(text, tts.tokenizer, budget)
-    if not segments:
-        raise ValueError("the text has nothing to speak (it is empty or whitespace only)")
-    return _stream_passage(tts, segments, ref, post, P, seed=seed, max_frames=max_frames, top_p=top_p,
-                           temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
-                           min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
-                           nar_context_frames=nar_context_frames)
-
-
-def stream_dialogue(tts, turns, *, seed: Optional[int] = None, pause_ms: float = 250, turn_pause_ms: float = 500,
-                    max_frames: int = 400, max_tokens: int = 64, top_p: float = 0.9, temperature: float = 1.05,
-                    anti_loop: bool = True, style_strength: Optional[float] = None,
-                    min_gen_frames: Optional[int] = None, chunk_frames: int = 6,
-                    nar_context_frames: Optional[int] = None, sample_rate: Optional[int] = None,
-                    speed: Optional[float] = None, watermark: Optional[int] = None) -> Iterator[torch.Tensor]:
-    """SoproTTS.stream_dialogue: every argument is checked here, before any device work or random draw; the returned
-    generator streams the script as stream_long streams a passage, with a voice per segment and the dialogue's gaps."""
-    from . import dialogue as D
-
-    _turns, segments, turn_of, voice_of, P, TP = D.check_script(tts, turns, pause_ms, turn_pause_ms, max_tokens)
-    _check_chunk_frames(chunk_frames)
-    post = OutputChain(tts, sample_rate, speed, watermark=watermark)
-    return _stream_passage(tts, segments, D.segment_voices(voice_of), post, P, turn_of=turn_of, turn_pause=TP, seed=seed,
-                           max_frames=max_frames, top_p=top_p, temperature=temperature, anti_loop=anti_loop,
-                           style_strength=style_strength, min_gen_frames=min_gen_frames, chunk_frames=chunk_frames,
-                           nar_context_frames=nar_context_frames)
-
-
 def _stream_passage(tts, segments: Sequence[str], ref, post: OutputChain, P: int, *,
-                    turn_of: Optional[Sequence[int]] = None, turn_pause: int = 0, seed: Optional[int], max_frames: int,
-                    top_p: float, temperature: float, anti_loop: bool, style_strength: Optional[float],
-                    min_gen_frames: Optional[int], chunk_frames: int, nar_context_frames: Optional[int]):
-    """The passage loop of stream_long and stream_dialogue over checked arguments.  `ref`: one voice, or one per
-    segment; `turn_of` / `turn_pause`: the dialogue's gaps (longform.gap_pauses), None for one turn."""
+                    turn_of: Optional[Sequence[int]] = None, turn_pause: int = 0, seed: Optional[int], gen: Generation,
+                    chunk_frames: int, nar_context_frames: Optional[int]):
+    """The passage loop of stream_long and stream_dialogue over checked arguments -> the generator of the passage's
+    chunks.  `ref`: one voice, or one per segment; `turn_of` / `turn_pause`: the dialogue's gaps
+    (longform.gap_pauses), None for one turn.
+
+    The segments run SEGMENT_GROUP at a time, each group through one chunk loop whose decoded blocks go to the
+    streaming trim (longform.StreamJoin) instead of an output chain; the joined 24 kHz passage goes through one
+    output-chain stream.  Each resumption runs at most one AR chunk, then yields the next piece of the passage (at most
+    chunk_frames x 1920 samples of it before the chain); it runs more chunks only while nothing is certain yet.  A
+    group starts at the first resumption after the group before it has ended and the group before that has been
+    emitted (the trim state holds two groups)."""
     from . import longform as LF
 
     B, G = len(segments), int(LF.SEGMENT_GROUP)
@@ -176,7 +99,7 @@ def _stream_passage(tts, segments: Sequence[str], ref, post: OutputChain, P: int
 
     @torch.inference_mode()
     def passage():
-        join = tts._join_pool.checkout(LF.StreamJoin.rows_for(B, G), (int(max_frames) + 1) * hop)
+        join = tts._join_pool.checkout(LF.StreamJoin.rows_for(B, G), (gen.max_frames + 1) * hop)
         join.begin(B, P, G, turn_of, turn_pause)
         out = post.stream(limit)
         main = torch.cuda.current_stream(tts.device)
@@ -187,10 +110,8 @@ def _stream_passage(tts, segments: Sequence[str], ref, post: OutputChain, P: int
             part = segments[g0: g0 + G]
             join.start_group(g0, len(part))
             voice = ref if one else list(ref[g0: g0 + G])
-            return _chunk_loop(tts, dec, [tts.encode_text(t) for t in part], voice, bypass, max_frames=max_frames,
-                               top_p=top_p, temperature=temperature, anti_loop=anti_loop, style_strength=style_strength,
+            return _chunk_loop(tts, dec, [tts.encode_text(t) for t in part], voice, bypass, gen=gen,
                                chunk_frames=chunk_frames, nar_context_frames=nar_context_frames,
-                               min_gen_frames=min_gen_frames,
                                seeds=None if seed is None else [int(seed) + g0 + i for i in range(len(part))],
                                on_block=join.push)
 
@@ -255,11 +176,9 @@ def _stream_passage(tts, segments: Sequence[str], ref, post: OutputChain, P: int
 
 def _word_spans(tts, texts: Sequence[str], word_timestamps) -> Optional[list]:
     """`word_timestamps` checked -> the texts' token character spans (None without it).  Host work only."""
-    from .timestamps import MAX_TOKENS
+    from .timestamps import MAX_TOKENS, check_word_timestamps
 
-    if not isinstance(word_timestamps, bool):
-        raise TypeError(f"word_timestamps must be a bool, got {type(word_timestamps).__name__}")
-    if not word_timestamps:
+    if not check_word_timestamps(word_timestamps):
         return None
     spans = [tts.tokenizer.encode_with_offsets(t)[1] for t in texts]
     for i, sp in enumerate(spans):
@@ -287,8 +206,7 @@ def _decoder(tts, chunk_frames) -> MimiStreamDecoder:
 
 @torch.inference_mode()
 def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], ref, post: OutputChain, *,
-                max_frames: int, top_p: float, temperature: float, anti_loop: bool, style_strength: Optional[float],
-                chunk_frames: int, nar_context_frames: Optional[int], min_gen_frames: Optional[int],
+                gen: Generation, chunk_frames: int, nar_context_frames: Optional[int],
                 seeds: Optional[Sequence[int]], generator: Optional[torch.Generator] = None,
                 on_block: Optional[Callable[[Optional[torch.Tensor], List[int], List[bool]], None]] = None,
                 word_texts: Optional[Sequence[str]] = None, word_spans: Optional[Sequence[Sequence]] = None
@@ -309,8 +227,8 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
     fourth element is the list of the row's words that became final since its previous item (None without them)."""
     model = tts.model
     B = len(text_ids)
-    st_ = float(style_strength if style_strength is not None else tts.cfg.style_strength)
-    txt, lens, _pool, cond = model.prefill.run(list(text_ids), ref, n_frames=int(max_frames) + 1, style_strength=st_)
+    txt, lens, _pool, cond = model.prefill.run(list(text_ids), ref, n_frames=gen.max_frames + 1,
+                                               style_strength=gen.style_strength)
     cf = int(chunk_frames)
     ctx = int(model.rf_nar() if nar_context_frames is None else nar_context_frames)
     hop = tts.codec.engine.hop
@@ -361,13 +279,12 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
     if word_spans is not None:
         from .timestamps import StreamAligner
 
-        aligner = StreamAligner(tts.cfg, word_texts, word_spans, ring=cf, max_frames=int(max_frames) + 1, hop=hop,
+        aligner = StreamAligner(tts.cfg, word_texts, word_spans, ring=cf, max_frames=gen.max_frames + 1, hop=hop,
                                 S=post.S, device=tts.device)
     pending: List[list] = [[] for _ in range(B)]
     progress = {"consumed": 0}
-    chunks = model.ar_chunk_rows(cond, txt, lens, max_frames=max_frames, chunk_frames=cf, top_p=top_p,
-                                 temperature=temperature, anti_loop=anti_loop, min_gen_frames=min_gen_frames,
-                                 seeds=seeds, generator=generator, progress=progress,
+    chunks = model.ar_chunk_rows(cond, txt, lens, gen=gen, chunk_frames=cf, seeds=seeds, generator=generator,
+                                 progress=progress,
                                  attn_trace=None if aligner is None else aligner.ring,
                                  attn_ring=None if aligner is None else cf)
     try:
@@ -378,7 +295,7 @@ def _chunk_loop(tts, dec: MimiStreamDecoder, text_ids: Sequence[torch.Tensor], r
             ends, last, new = [0] * B, [False] * B, [0] * B
             for b in live:
                 toks = toks_rows[b]
-                # the stream ends at the first EOS regardless of min_gen_frames (reference streaming.py:114-115)
+                # the stream ends at the first EOS, even before the minimum frame count (reference streaming.py:114-115)
                 stop = model.eos_id in toks
                 if stop:
                     toks = toks[: toks.index(model.eos_id)]

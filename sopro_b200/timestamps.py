@@ -58,6 +58,13 @@ class WordTiming:
     char_end: int
 
 
+def check_word_timestamps(word_timestamps) -> bool:
+    """The `word_timestamps` argument of an entry point that checks it; TypeError for anything but a bool.  Host only."""
+    if not isinstance(word_timestamps, bool):
+        raise TypeError(f"word_timestamps must be a bool, got {type(word_timestamps).__name__}")
+    return word_timestamps
+
+
 # ---- the device part
 
 def trace_buffer(cfg, steps: int, batch: int, ld: int, device) -> torch.Tensor:

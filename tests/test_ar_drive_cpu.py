@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+from sopro_b200.engine import Generation
 from tests.test_host_pipeline_cpu import SEEDS, TEXTS, _FakeArEngine, tts  # noqa: F401
 
 torch.set_grad_enabled(False)
@@ -159,8 +160,9 @@ def test_ar_stream_launch_schedule(tts, launches, chunk_frames, want):  # noqa: 
     (70, [1, 2], [24, 47]),
     (400, None, [401]),  # the global generator: one launch
 ])
-def test_batch_launch_schedule(tts, launches, max_frames, seeds, want):  # noqa: F811
+def test_batch_launch_schedule_from_resolved_settings(tts, launches, max_frames, seeds, want):  # noqa: F811
     steps = max_frames + 1
-    toks, n = tts.model.ar_generate_tensors(torch.zeros(2, steps, 8), torch.zeros(2, 4, 8), [4, 3], max_frames=max_frames,
-                                            seeds=seeds)
+    gen = Generation.resolve(tts.cfg, max_frames=max_frames, top_p=0.9, temperature=1.05, anti_loop=True,
+                             style_strength=None, min_gen_frames=None)
+    toks, n = tts.model.ar_generate_tensors(torch.zeros(2, steps, 8), torch.zeros(2, 4, 8), [4, 3], gen=gen, seeds=seeds)
     assert launches == ["begin"] + want and n.tolist() == [steps, steps]

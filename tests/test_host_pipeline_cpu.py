@@ -318,3 +318,24 @@ def test_baseline_config0_plumbing(tts):
     wav = tts.synthesize(text, ref=ref, max_frames=12, seed=seed)
     assert wav.shape == (1, 1, T * 1920) and wav.dtype == torch.float32 and bool(torch.isfinite(wav).all())
     assert torch.equal(wav, tts.synthesize(text, ref=ref, max_frames=12, seed=seed))
+
+
+@pytest.mark.parametrize("texts, seeds, err", [
+    ([], None, ValueError),  # no text
+    (TEXTS, [1], ValueError),  # fewer seeds than texts
+    (TEXTS[:2], [1, 2, 3], ValueError),  # more seeds than texts
+    ("8 9", None, TypeError),  # a str is one text, not a sequence of them
+])
+def test_batch_refuses_texts_and_seeds_before_any_work(tts, monkeypatch, texts, seeds, err):
+    """synthesize_batch and stream_batch check `texts` and `seeds` alike, before the prefill or any random draw."""
+
+    def no_prefill(*a, **k):
+        raise AssertionError("the prefill ran")
+
+    monkeypatch.setattr(tts.model.prefill, "run", no_prefill)
+    torch.manual_seed(5)
+    before = torch.get_rng_state()
+    for fn in (tts.synthesize_batch, tts.stream_batch):
+        with pytest.raises(err):
+            fn(texts, ref=tts.ref, seeds=seeds, **KW)
+    assert torch.equal(torch.get_rng_state(), before)

@@ -766,6 +766,15 @@ int sopro_stretch_window(float* w);
  * i32 [B][K_max], K_max = the longest row's frame count) receives every d_k: a test hook. */
 int sopro_stretch(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t S, float* y, int64_t y_stride,
                   int32_t* offsets, void* stream);
+/* as sopro_stretch, with a speed per row: S_host (HOST i32 [B]) holds each row's S.  Row b produces
+ * sopro_stretched_length(S_host[b], lens[b]) outputs.  A row with S_b = 65536 is copied through unchanged (M_b = lens[b])
+ * and runs no frames; any other row's outputs (and offsets) equal sopro_stretch of that row alone at S_b, bit for bit.
+ * One launch covers the whole batch (the rows' lengths and speeds reach it through one stream-ordered copy).
+ * y_stride >= the longest row's outputs when B > 1; offsets: K_max = n_frames of the longest row's outputs, and a
+ * copied row writes none.  Refused before any launch: sopro_stretch's refusals, a null S_host, and an S_b outside
+ * [16384, 262144] in any row. */
+int sopro_stretch_rows(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, const int32_t* S_host, float* y,
+                       int64_t y_stride, int32_t* offsets, void* stream);
 /* Streaming: one utterance pushed in chunks of at most max_chunk samples.  Frame k is ready once
  * max(a_k + D + N/2, a_{k-1} + D + Hs + N/2) input samples have arrived (a_0 + D + N/2 for frame 0); with frames
  * [0, k_done) done, the pushes have emitted the outputs below max(0, k_done - 1) * Hs, and finish emits the rest up to

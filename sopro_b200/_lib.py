@@ -250,6 +250,7 @@ SYMBOLS = {
     "sopro_stretch_positions": (C.c_int64, [C.c_int32, C.c_int64, _VP]),
     "sopro_stretch_window": (_I, [_VP]),
     "sopro_stretch": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, _VP, C.c_int64, _VP, _VP]),
+    "sopro_stretch_rows": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
     "sopro_stretch_stream_create": (_I, [C.c_int64, _I, C.POINTER(_VP)]),
     "sopro_stretch_stream_destroy": (_I, [_VP]),
     "sopro_stretch_stream_reset": (_I, [_VP, C.c_int32]),

@@ -222,6 +222,32 @@ __global__ void __launch_bounds__(kThreads, 1) stretch_batch_kernel(Window wp, c
                  offsets ? offsets + (long long)b * k_stride : nullptr, nullptr);
 }
 
+// one row of a batch with a speed per row: its valid samples and its S
+struct RowSpeed {
+  long long len;
+  int S;
+};
+
+// one-shot, ragged batch, a speed per row: one CTA per row.  A row at S = 65536 is copied through; any other row runs
+// the frames stretch_batch_kernel runs for it at its own S, so its outputs equal that kernel's bit for bit.  A separate
+// kernel, so the one-speed kernel keeps S as a parameter and its code is unchanged.
+__global__ void __launch_bounds__(kThreads, 1) stretch_rows_kernel(Window wp, const float* __restrict__ x, long long x_stride,
+                                                                   const RowSpeed* __restrict__ rows, float* __restrict__ y,
+                                                                   long long y_stride, int* __restrict__ offsets, long long k_stride) {
+  const int b = blockIdx.x;
+  const long long L = rows[b].len;
+  const int S = rows[b].S;
+  const float* xb = x + (long long)b * x_stride;
+  float* yb = y + (long long)b * y_stride;
+  if (S == kOne) {  // uniform per CTA: the whole block returns before stretch_frames' barriers
+    for (long long m = threadIdx.x; m < L; m += kThreads) yb[m] = xb[m];
+    return;
+  }
+  const Src s{xb, nullptr, 0, L, L};
+  const long long M = out_len(S, L);
+  stretch_frames(s, S, 0, n_frames(M), 0, 0.0f, wp, yb, 0, M, offsets ? offsets + (long long)b * k_stride : nullptr, nullptr);
+}
+
 // stream: frames [k_begin, k_end) of one utterance from its carried tail and the new chunk; the carried p / pending
 // are read at the start (k_begin >= 1) and the new ones written back at the end
 __global__ void __launch_bounds__(kThreads, 1) stretch_stream_kernel(Window wp, Src s, int S, long long k_begin, long long k_end,
@@ -333,6 +359,39 @@ int sopro_stretch(const float* x, int32_t B, int64_t x_stride, const int64_t* le
                                                     offsets ? offsets + (long long)b0 * k_max : nullptr, k_max);
     CK(cudaGetLastError());
   }
+  return SOPRO_OK;
+}
+
+int sopro_stretch_rows(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, const int32_t* S_host, float* y,
+                       int64_t y_stride, int32_t* offsets, void* stream) {
+  if (!x || !y || !S_host) return fail(SOPRO_ERR_INVALID, "null argument");
+  long long most = 0;
+  int rc = check_rows(x, B, x_stride, lens_host, kMaxLen, &most);
+  if (rc != SOPRO_OK) return rc;
+  std::vector<RowSpeed> rows(B);
+  long long m_max = 0;
+  for (int b = 0; b < B; ++b) {
+    const int S = S_host[b];
+    if (!valid_S(S))
+      return fail(SOPRO_ERR_INVALID, "S_host[%d] = %d not in [%d, %d] (speed 0.25 .. 4 in 1/65536 steps)", b, S, kMinS, kMaxS);
+    rows[b] = RowSpeed{lens_host ? lens_host[b] : x_stride, S};
+    m_max = std::max(m_max, out_len(S, rows[b].len));
+  }
+  if ((rc = check_out_rows(y, B, y_stride, m_max)) != SOPRO_OK) return rc;
+  if (m_max == 0) return SOPRO_OK;
+  // the rows' lengths and speeds go to the device in one stream-ordered copy, so one launch takes any batch size
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  static const Window wp = make_window();
+  RowSpeed* d_rows = nullptr;
+  CK(cudaMallocAsync(&d_rows, sizeof(RowSpeed) * B, st));
+  cudaError_t e = cudaMemcpyAsync(d_rows, rows.data(), sizeof(RowSpeed) * B, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) {
+    stretch_rows_kernel<<<B, kThreads, 0, st>>>(wp, x, x_stride, d_rows, y, y_stride, offsets, n_frames(m_max));
+    e = cudaGetLastError();
+  }
+  const cudaError_t f = cudaFreeAsync(d_rows, st);
+  CK(e);
+  CK(f);
   return SOPRO_OK;
 }
 

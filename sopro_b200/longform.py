@@ -256,6 +256,37 @@ def join_gaps(rows_or_chunks: Union[torch.Tensor, Sequence[torch.Tensor]], exten
     return y
 
 
+def join_padded(rows: Sequence[torch.Tensor], extents, pauses: Sequence[int], gain: Optional[torch.Tensor], lead: int,
+                trail: int, device) -> torch.Tensor:
+    """join_gaps with gaps of any length and `lead` / `trail` zeros around the passage -> [1, 1, N] f32 on `device`.
+    The spans between two gaps longer than the kernel's 2 s are joined by join_gaps and the long gaps are zeros laid
+    between those joins, so the samples equal one join with those gaps.  Nothing synchronises."""
+    ext = np.asarray(extents, dtype=np.int64).reshape(-1, 2)
+    spoken = [k for k in range(ext.shape[0]) if ext[k, 1] > ext[k, 0]]
+    if len(pauses) != max(0, len(spoken) - 1):
+        raise ValueError(f"{len(pauses)} pauses for {len(spoken)} non-empty spans")
+    longest = pause_samples(MAX_PAUSE_MS)
+
+    def zeros(n: int) -> torch.Tensor:
+        return torch.zeros((1, 1, int(n)), dtype=torch.float32, device=device)
+
+    parts = [zeros(lead)] if lead else []
+    a = 0
+    for m, p in enumerate(list(pauses) + [None] if spoken else []):
+        if p is not None and p <= longest:
+            continue
+        idx = spoken[a: m + 1]
+        parts.append(join_gaps([rows[k] for k in idx], ext[idx], pauses[a: m], None if gain is None else gain[idx]))
+        if p is not None:
+            parts.append(zeros(p))
+        a = m + 1
+    if trail:
+        parts.append(zeros(trail))
+    if not parts:
+        return zeros(0)
+    return parts[0] if len(parts) == 1 else torch.cat(parts, dim=-1)
+
+
 # ---- the streaming trim and join (SoproTTS.stream_long)
 
 class StreamJoin:

@@ -16,7 +16,7 @@ import contextlib
 import dataclasses
 import os
 import threading
-from typing import Dict, Iterator, List, Optional, Sequence, Tuple, Union
+from typing import Dict, Iterator, List, Mapping, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -25,6 +25,7 @@ from . import ingest
 from . import longform as LF
 from . import prefill as P
 from . import rerank
+from . import ssml as SSML
 from . import streaming as S
 from . import timestamps as TS
 from . import voices
@@ -39,7 +40,7 @@ from .prefill import PreparedReference
 from .output import OutputChain
 from .resample import Resampler, check_rates
 from .sampling import TapeFeed
-from .stretch import StretchStream
+from .stretch import StretchStream, stretch_rows, stretched_length
 from .watermark import WatermarkStream
 from .weights import load_safetensors, read_safetensors_cfg
 
@@ -92,6 +93,14 @@ def _growing_blocks(steps: int) -> List[Tuple[int, int]]:
         edges.append((a, b))
         a, step = b, (step * 3) // 2
     return edges
+
+
+def _check_voices(cfg: SoproTTSConfig, voice_of: Sequence[PreparedReference]) -> None:
+    """Every distinct voice of a segment list against the engine's geometry (TypeError for one that is not a
+    PreparedReference)."""
+    geom = voices.geometry(cfg)
+    for r in voices.voice_slots(list(voice_of), len(voice_of))[0]:
+        voices.check_voice(r, **geom)
 
 
 def _check_texts(texts, seeds) -> Tuple[List[str], Optional[List[int]]]:
@@ -662,6 +671,62 @@ class SoproTTS:
         if wav.shape[-1]:
             wav, _ = post(wav)
         return (wav, words) if word_timestamps else wav
+
+    @torch.inference_mode()
+    def synthesize_ssml(self, ssml: str, *, ref: PreparedReference, voices: Optional[Mapping[str, PreparedReference]] = None,
+                        seed: Optional[int] = None, pause_ms: float = 250, paragraph_pause_ms: float = 500,
+                        max_frames: int = 400, max_tokens: int = 64, top_p: float = 0.9, temperature: float = 1.05,
+                        anti_loop: bool = True, style_strength: Optional[float] = None,
+                        min_gen_frames: Optional[int] = None, sample_rate: Optional[int] = None,
+                        speed: Optional[float] = None, loudness: Optional[float] = None,
+                        watermark: Optional[int] = None, best_of: int = 1):
+        """NEW: speech markup -> one waveform [1, 1, N] f32 on the device.  The markup is an SSML subset
+        (sopro_b200/ssml.py: ``<speak>``, ``<p>``, ``<s>``, ``<break>``, ``<prosody rate / volume>``, ``<voice>``,
+        ``<sub>``); ssml.parse turns it into segments, each with its text, voice, rate and volume, and the gaps between
+        them.  The segments go through the batch path together, SEGMENT_GROUP at a time: segment k equals
+        synthesize(segment, ref=its voice, seed=seed + k) (without a seed the global generator is consumed segment
+        after segment).  `ref` speaks outside every ``<voice>``, `voices` maps ``<voice name>`` to prepared voices.
+        Each decoded row is trimmed to its speech, the trimmed spans are time-stretched in one launch at each span's
+        rate times `speed` (a span at rate 1 is copied), and the spans are joined on the GPU with the plan's gaps, each
+        span scaled by its volume's gain, between the leading and trailing silence.  The join then goes through the
+        chain of synthesize: watermark, resample (`sample_rate`), loudness (one level for the whole passage, so the
+        spans' relative volumes survive).  Unlike synthesize_long, `speed` does not stretch the pauses: it is folded
+        into the spans' rates, so a ``<break time="1s"/>`` lasts one second at any speed.  Markup that is plain text
+        in a ``<speak>`` equals synthesize_long of that text.  Segments that produce no speech are skipped and the
+        gaps around them merge into the larger one (ssml.Plan.pauses).  `best_of`: as in synthesize_long.  Refused
+        before any device work or random draw: every refusal of ssml.parse, a voice of the wrong geometry,
+        `pause_ms` / `paragraph_pause_ms` / `max_tokens` out of range, a refused sample_rate / speed / loudness /
+        watermark / best_of."""
+        post = OutputChain(self, sample_rate, None, loudness, watermark)
+        n_best = self._check_best_of(best_of, 1)
+        budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
+        plan = SSML.parse(ssml, voices, ref, pause_ms, paragraph_pause_ms, speed, budget, self.tokenizer)
+        voice_of = [s.voice for s in plan.segments]
+        _check_voices(self.cfg, voice_of)
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+        rows, ext_dev, _f, _T = self._speak_segments([s.text for s in plan.segments], D.segment_voices(voice_of),
+                                                     n_best, seed=seed, word_timestamps=False, gen=gen)
+        ext = ext_dev.cpu().numpy()  # the one host read: the extents
+        spans = [max(0, int(e) - int(s)) for s, e in ext]
+        rates = [s.rate for s in plan.segments]
+        n_out = [stretched_length(r, n) for r, n in zip(rates, spans)]
+        stretched: List[torch.Tensor] = [torch.zeros(0, device=self.device)] * len(spans)
+        if max(spans):
+            batch = torch.zeros((len(spans), max(spans)), dtype=torch.float32, device=self.device)
+            for k, (s, n) in enumerate(zip(ext[:, 0], spans)):
+                if n:
+                    batch[k, :n] = rows[k][int(s): int(s) + n]
+            y = stretch_rows(batch, rates, lens=spans)
+            stretched = [y[k] for k in range(len(spans))]
+        gains = [s.gain for s in plan.segments]
+        gain = None if all(g == 1.0 for g in gains) else torch.tensor(gains, dtype=torch.float32, device=self.device)
+        out_ext = [(0, n) for n in n_out]
+        wav = LF.join_padded(stretched, out_ext, plan.pauses([n > 0 for n in n_out]), gain, plan.lead, plan.trail,
+                             self.device)
+        if wav.shape[-1]:
+            wav, _ = post(wav)
+        return wav
 
     def _speak_segments(self, segments: Sequence[str], ref, n_best: int, *, seed: Optional[int], word_timestamps: bool,
                         **kw) -> Tuple[List[torch.Tensor], torch.Tensor, list, List[int]]:

@@ -97,6 +97,34 @@ def stretch(wav: torch.Tensor, speed, lens: Optional[Sequence[int]] = None,
     return (y, offs) if return_offsets else y
 
 
+def stretch_rows(wav: torch.Tensor, speeds: Sequence, lens: Optional[Sequence[int]] = None,
+                 return_offsets: bool = False) -> Union[torch.Tensor, Tuple[torch.Tensor, torch.Tensor]]:
+    """stretch with a speed per row, in one launch: wav [..., L] on a CUDA device (rows = the leading dims flattened),
+    `speeds` one accepted speed per row -> [..., M] f32, M the longest row's stretched_length(speeds[b], lens[b]).  Row
+    b has stretched_length(speeds[b], lens[b]) outputs, zeros after them; a row whose speed quantises to S = 65536 is
+    its input copied through, any other row equals stretch of that row alone at its speed, bit for bit.  Every speed is
+    checked before any work.  `return_offsets` (a test hook) also returns every frame's d_k, int32 [rows, K_max]; a
+    copied row's stay 0."""
+    x, lead, lp = _lib.rows(wav, lens, "the time-stretch")
+    dev = x.device
+    B, L = x.shape
+    speeds = list(speeds)
+    if len(speeds) != B:
+        raise ValueError(f"{len(speeds)} speeds for {B} rows")
+    S = [_S(v) for v in speeds]
+    n = [L] * B if lens is None else [int(v) for v in lens]
+    M = max((stretched_length(v, k) for v, k in zip(speeds, n)), default=0)
+    y = torch.zeros((B, M), dtype=torch.float32, device=dev)
+    offs = torch.zeros((B, n_frames(M)), dtype=torch.int32, device=dev) if return_offsets else None
+    if B and M:
+        with torch.cuda.device(dev):
+            _lib.check_arg(_lib.load().sopro_stretch_rows(x.data_ptr(), B, L, lp, (C.c_int32 * B)(*S), y.data_ptr(), M,
+                                                          offs.data_ptr() if offs is not None else None,
+                                                          _lib.stream_ptr(dev)))
+    y = y.reshape(*lead, M)
+    return (y, offs) if return_offsets else y
+
+
 class StretchStream(_lib.ChunkStream):
     """One utterance time-stretched chunk by chunk: ``push(x)`` returns every output the frames its input completes
     have finished, ``finish()`` the rest.  Their concatenation equals ``stretch`` of the concatenated input bit for bit.

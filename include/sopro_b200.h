@@ -503,6 +503,7 @@ int sopro_debug_argmax_heads(const float* logits, int64_t rows, int heads, int V
  * prepare_reference (once per voice: Token2SV, reference encoder, K/V projections) is sopro_refprep_* below.
  * ------------------------------------------------------------------------------------------------ */
 #define SOPRO_PREFILL_MAX_REF_LAYERS 8
+#define SOPRO_PREFILL_MAX_BLEND_SEGMENTS 16  /* segments of one blended voice (sopro_prefill_run_blends) */
 
 typedef struct sopro_prefill_config {
   int32_t d_model;        /* 384 */
@@ -560,6 +561,21 @@ int sopro_prefill_run_voices(sopro_prefill_t* p, const int32_t* text_ids, const 
                              const int32_t* voice_of, const float* sv, const int32_t* tr, const float* const* ref_k,
                              const float* const* ref_v, float style_strength, int n_frames, float* txt_seq, float* txt_pool,
                              float* cond_ar, void* stream);
+/* The voice-table prefill over blended voices (SoproTTS.blend_voices, sopro_b200/voices.py).  Voice v's K / V are
+ * n_seg[v] segments one after another along the frame axis: its tr[v] frames split into seg_frames[...] frames each, with
+ * weights seg_w[...].  n_seg: HOST int32 [n_voices], each in [1, SOPRO_PREFILL_MAX_BLEND_SEGMENTS]; seg_frames: HOST int32,
+ * voice 0's n_seg[0] entries, then voice 1's, ..., each >= 1 and summing to tr[v] per voice; seg_w: HOST f32 in the same
+ * order, each finite and > 0 (the caller normalises them).  In each reference cross-attention layer a row of voice v
+ * attends to each segment on its own (its own softmax; non-finite outputs zeroed) and mixes the read-outs,
+ * a = sum_s seg_w[s] a_s in segment order, before the RMS match, out_proj and the gate.  The other arguments and the
+ * outputs are sopro_prefill_run_voices's; anything else in the table returns SOPRO_ERR_INVALID with nothing launched.
+ * A voice of one segment with weight 1.0f gives the rows sopro_prefill_run_voices gives it, bit for bit, and a row equals
+ * the row of a launch with its voice alone.  The segment table travels to the device with the voice table (no host
+ * synchronisation); the host arrays may be released when the call returns. */
+int sopro_prefill_run_blends(sopro_prefill_t* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, int n_voices,
+                             const int32_t* voice_of, const float* sv, const int32_t* tr, const float* const* ref_k,
+                             const float* const* ref_v, const int32_t* n_seg, const int32_t* seg_frames, const float* seg_w,
+                             float style_strength, int n_frames, float* txt_seq, float* txt_pool, float* cond_ar, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Reference preparation: SoproTTSModel.prepare_reference (reference model.py:152-170), once per voice, from the

@@ -223,6 +223,8 @@ SYMBOLS = {
     "sopro_prefill_run": (_I, [_VP, _VP, _VP, _I, _I, _VP, _I, _VP, _VP, _I, C.c_float, _I, _VP, _VP, _VP, _VP]),
     "sopro_refprep_speaker_vectors_per_row": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _VP]),
     "sopro_prefill_run_voices": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, C.c_float, _I, _VP, _VP, _VP, _VP]),
+    "sopro_prefill_run_blends": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float, _I, _VP,
+                                      _VP, _VP, _VP]),
     "sopro_debug_tc_gemm": (_I, [_VP, _I, C.c_int64, _I, _I, _I, _I, _VP, _I, _VP, _I, _I, _VP, _VP, _VP, _VP, _I, _VP]),
     "sopro_debug_tc_attn": (_I, [_VP, _VP, _VP, _VP, _I, _I, C.c_int64, _I, _I, _I, _VP]),
     "sopro_debug_tc_resblock": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),

@@ -913,10 +913,18 @@ __global__ void __launch_bounds__(256) film_rows_kernel(const float* __restrict_
 // Row `row` belongs to utterance b = row / T, which speaks voice v = voice_of[b]: K = Kv[v], V = Vv[v], both [H][Tr][dh]
 // with Tr = tr_of[v].  A row's arithmetic depends on its voice alone (the loops run to that voice's Tr), so it equals
 // the row of a launch with that one voice.  Shared memory per warp: q [D] | p [Tr_max] | a [D].
+// kBlend: voice v is a blend whose K / V are its segments seg_first[v] .. seg_first[v + 1] - 1 one after another along
+// the frame axis, segment s seg_len[s] frames with weight seg_w[s].  Each head runs the pass above over each segment
+// alone (its own max, sum and nan_to_num) and accumulates a = sum_s seg_w[s] a_s in segment order; the RMS match runs
+// once on that mix.  A voice of one segment with weight 1 gives the rows of kBlend = false bit for bit (a = 1 * a_0, and
+// ssa sums the same squares in the same order).
+template <bool kBlend>
 __global__ void __launch_bounds__(256) ref_attn_kernel(const float* __restrict__ q, const float* __restrict__ x,
                                                        const int* __restrict__ voice_of, const int* __restrict__ tr_of,
                                                        const float* const* __restrict__ Kv, const float* const* __restrict__ Vv,
-                                                       float* __restrict__ out, long long rows, int T, int D, int H, int Tr_max) {
+                                                       const int* __restrict__ seg_first, const int* __restrict__ seg_len,
+                                                       const float* __restrict__ seg_w, float* __restrict__ out, long long rows,
+                                                       int T, int D, int H, int Tr_max) {
   extern __shared__ float rsm[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long row = (long long)blockIdx.x * 8 + warp;
@@ -931,43 +939,64 @@ __global__ void __launch_bounds__(256) ref_attn_kernel(const float* __restrict__
   for (int k = lane; k < D; k += 32) qs[k] = q[row * D + k];
   __syncwarp();
   const float scale = 1.0f / sqrtf((float)dh);
+  int s0 = 0, s1 = 1;
+  if constexpr (kBlend) {
+    s0 = seg_first[v];
+    s1 = seg_first[v + 1];
+  }
   float ssa = 0.f;
   for (int h = 0; h < H; ++h) {
-    const float* Kh = Kc + (size_t)h * Tr * dh;
-    const float* Vh = Vc + (size_t)h * Tr * dh;
-    float mx = -INFINITY;
-    for (int j = lane; j < Tr; j += 32) {
-      const float* kr = Kh + (size_t)j * dh;
-      float s = 0.f;
-      for (int d = 0; d < dh; d += 4) {
-        const float4 kk = __ldg(reinterpret_cast<const float4*>(kr + d));
-        const float4 qq = *reinterpret_cast<const float4*>(qs + h * dh + d);
-        s += kk.x * qq.x + kk.y * qq.y + kk.z * qq.z + kk.w * qq.w;
+    int off = 0;
+    for (int g = s0; g < s1; ++g) {
+      const int n = kBlend ? seg_len[g] : Tr;
+      const float* Kh = Kc + ((size_t)h * Tr + off) * dh;
+      const float* Vh = Vc + ((size_t)h * Tr + off) * dh;
+      float mx = -INFINITY;
+      for (int j = lane; j < n; j += 32) {
+        const float* kr = Kh + (size_t)j * dh;
+        float s = 0.f;
+        for (int d = 0; d < dh; d += 4) {
+          const float4 kk = __ldg(reinterpret_cast<const float4*>(kr + d));
+          const float4 qq = *reinterpret_cast<const float4*>(qs + h * dh + d);
+          s += kk.x * qq.x + kk.y * qq.y + kk.z * qq.z + kk.w * qq.w;
+        }
+        s *= scale;
+        ps[j] = s;
+        mx = fmaxf(mx, s);
       }
-      s *= scale;
-      ps[j] = s;
-      mx = fmaxf(mx, s);
-    }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    float sum = 0.f;
-    for (int j = lane; j < Tr; j += 32) {
-      const float e = expf(ps[j] - mx);
-      ps[j] = e;
-      sum += e;
-    }
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      float sum = 0.f;
+      for (int j = lane; j < n; j += 32) {
+        const float e = expf(ps[j] - mx);
+        ps[j] = e;
+        sum += e;
+      }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    __syncwarp();
-    const float inv = 1.0f / sum;
-    for (int d = lane; d < dh; d += 32) {
-      float o = 0.f;
-      for (int j = 0; j < Tr; ++j) o += (ps[j] * inv) * __ldg(Vh + (size_t)j * dh + d);
-      if (!isfinite(o)) o = 0.f;
-      as[h * dh + d] = o;
-      ssa += o * o;
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      __syncwarp();
+      const float inv = 1.0f / sum;
+      for (int d = lane; d < dh; d += 32) {
+        float o = 0.f;
+        for (int j = 0; j < n; ++j) o += (ps[j] * inv) * __ldg(Vh + (size_t)j * dh + d);
+        if (!isfinite(o)) o = 0.f;
+        if constexpr (kBlend) {
+          const float w = seg_w[g];
+          as[h * dh + d] = g == s0 ? w * o : as[h * dh + d] + w * o;
+        } else {
+          as[h * dh + d] = o;
+          ssa += o * o;
+        }
+      }
+      __syncwarp();
+      off += n;
     }
-    __syncwarp();
+    if constexpr (kBlend) {
+      for (int d = lane; d < dh; d += 32) {
+        const float o = as[h * dh + d];
+        ssa += o * o;
+      }
+    }
   }
   float ssx = 0.f;
   for (int k = lane; k < D; k += 32) {
@@ -1070,9 +1099,12 @@ namespace pstage {
 // The prefill of B texts over a table of n_voices voices: text b speaks voice voice_of[b] (host), voice v has speaker
 // vector sv[v] (device [n_voices][SV]), tr[v] reference frames (host) and, for reference layer i, cached K / V at
 // ref_k[i * n_voices + v] / ref_v[...] (host arrays of device pointers).  The one-voice call is n_voices = 1.
+// n_seg != nullptr (sopro_prefill_run_blends, checked there): voice v is a blend of n_seg[v] segments, whose frames and
+// weights follow those of voices 0 .. v-1 in seg_frames / seg_w (host); the reference attention runs the blend kernel.
 int prefill_core(sopro_prefill* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, int n_voices,
                  const int32_t* voice_of, const float* sv, const int32_t* tr, const float* const* ref_k, const float* const* ref_v,
-                 float style_strength, int n_frames, float* txt_seq, float* txt_pool, float* cond_ar, cudaStream_t st) {
+                 float style_strength, int n_frames, float* txt_seq, float* txt_pool, float* cond_ar, cudaStream_t st,
+                 const int32_t* n_seg = nullptr, const int32_t* seg_frames = nullptr, const float* seg_w = nullptr) {
   if (!p || !text_ids || !text_len || !sv || !txt_seq || !txt_pool || !cond_ar || !voice_of) return fail(SOPRO_ERR_INVALID, "null argument");
   const sopro_prefill_config_t& c = p->cfg;
   const int D = c.d_model, SV = c.sv_dim, H = c.ref_heads, RL = c.ref_layers;
@@ -1096,8 +1128,13 @@ int prefill_core(sopro_prefill* p, const int32_t* text_ids, const int32_t* text_
   const long long Mt = (long long)B * Lmax, Mc = (long long)B * n_frames;
   auto al = [](size_t x) { return (x + 63) / 64 * 64; };
   const size_t rows = (size_t)std::max(Mt, Mc);
-  // the voice table: K pointers [RL][n_voices] | V pointers [RL][n_voices] | tr [n_voices] | voice_of [B]
-  const size_t n_ptr = (size_t)RL * n_voices, tab_bytes = 2 * n_ptr * sizeof(void*) + ((size_t)n_voices + B) * sizeof(int);
+  // the voice table: K pointers [RL][n_voices] | V pointers [RL][n_voices] | tr [n_voices] | voice_of [B], and for a
+  // blend launch | seg_first [n_voices + 1] | seg_len [S] | seg_w [S] (float)
+  size_t n_segs = 0;
+  for (int v = 0; n_seg && v < n_voices; ++v) n_segs += (size_t)n_seg[v];
+  const size_t seg_bytes = n_seg ? ((size_t)n_voices + 1 + 2 * n_segs) * sizeof(int) : 0;
+  const size_t n_ptr = (size_t)RL * n_voices,
+               tab_bytes = 2 * n_ptr * sizeof(void*) + ((size_t)n_voices + B) * sizeof(int) + seg_bytes;
   const size_t need = (al(rows * D) * 3 + al(rows * 4 * D) + al((size_t)B * D) + al((size_t)B * 2 * D) + al((tab_bytes + 3) / 4)) * 4;
   if (p->ws_bytes < need) {
     CK(cudaStreamSynchronize(st));
@@ -1118,6 +1155,9 @@ int prefill_core(sopro_prefill* p, const int32_t* text_ids, const int32_t* text_
   const float* const* kv_dev = reinterpret_cast<const float* const*>(tab);
   const int* tr_dev = reinterpret_cast<const int*>(tab + 2 * n_ptr * sizeof(void*));
   const int* voice_dev = tr_dev + n_voices;
+  const int* seg_first_dev = voice_dev + B;
+  const int* seg_len_dev = seg_first_dev + n_voices + 1;
+  const float* seg_w_dev = reinterpret_cast<const float*>(seg_len_dev + n_segs);
   {
     // one copy from pageable memory: cudaMemcpyAsync has staged the bytes when it returns, so `host` may go
     std::vector<char> host(tab_bytes);
@@ -1129,6 +1169,13 @@ int prefill_core(sopro_prefill* p, const int32_t* text_ids, const int32_t* text_
     if (RL > 0) std::copy(tr, tr + n_voices, tr_h.begin());
     memcpy(host.data() + 2 * n_ptr * sizeof(void*), tr_h.data(), (size_t)n_voices * sizeof(int));
     memcpy(host.data() + 2 * n_ptr * sizeof(void*) + (size_t)n_voices * sizeof(int), voice_of, (size_t)B * sizeof(int));
+    if (n_seg) {
+      int* first = reinterpret_cast<int*>(host.data() + 2 * n_ptr * sizeof(void*) + ((size_t)n_voices + B) * sizeof(int));
+      first[0] = 0;
+      for (int v = 0; v < n_voices; ++v) first[v + 1] = first[v] + n_seg[v];
+      memcpy(first + n_voices + 1, seg_frames, n_segs * sizeof(int));
+      memcpy(first + n_voices + 1 + n_segs, seg_w, n_segs * sizeof(float));
+    }
     CK(cudaMemcpyAsync(tab, host.data(), tab_bytes, cudaMemcpyHostToDevice, st));
   }
   const float* W = p->dev;
@@ -1156,15 +1203,24 @@ int prefill_core(sopro_prefill* p, const int32_t* text_ids, const int32_t* text_
   // ---- reference cross-attention stack
   const size_t rsmem = (size_t)8 * (2 * D + ((Tr_max + 3) & ~3)) * 4;
   if (RL > 0 && rsmem > 48 * 1024) {
-    static unsigned long long attr_done = 0;  // per device, like every function attribute
-    if (tc::attr_needed(attr_done)) CK(cudaFuncSetAttribute(ref_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    static unsigned long long attr_done = 0, attr_blend_done = 0;  // per device, like every function attribute
+    if (!n_seg && tc::attr_needed(attr_done))
+      CK(cudaFuncSetAttribute(ref_attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    if (n_seg && tc::attr_needed(attr_blend_done))
+      CK(cudaFuncSetAttribute(ref_attn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
   for (int i = 0; i < RL; ++i) {
     g = dense::DenseOp{};
     g.A = x; g.W = W + p->ref[i].q_w; g.norm_w = W + p->ref[i].nq_w; g.C = q; g.M = (int)Mc; g.N = D; g.K = D; g.ldc = D; g.epi = dense::EPI_BIAS;
     if ((rc = launch_dense(g, 1, st))) return rc;
-    ref_attn_kernel<<<(unsigned)((Mc + 7) / 8), 256, rsmem, st>>>(q, x, voice_dev, tr_dev, kv_dev + (size_t)i * n_voices,
-                                                                  kv_dev + n_ptr + (size_t)i * n_voices, h, Mc, n_frames, D, H, Tr_max);
+    const float* const* Ki = kv_dev + (size_t)i * n_voices;
+    const float* const* Vi = kv_dev + n_ptr + (size_t)i * n_voices;
+    if (n_seg)
+      ref_attn_kernel<true><<<(unsigned)((Mc + 7) / 8), 256, rsmem, st>>>(q, x, voice_dev, tr_dev, Ki, Vi, seg_first_dev, seg_len_dev,
+                                                                          seg_w_dev, h, Mc, n_frames, D, H, Tr_max);
+    else
+      ref_attn_kernel<false><<<(unsigned)((Mc + 7) / 8), 256, rsmem, st>>>(q, x, voice_dev, tr_dev, Ki, Vi, nullptr, nullptr, nullptr,
+                                                                           h, Mc, n_frames, D, H, Tr_max);
     CK(cudaGetLastError());
     g = dense::DenseOp{};
     g.A = h; g.W = W + p->ref[i].o_w; g.R = x; g.C = x; g.M = (int)Mc; g.N = D; g.K = D; g.ldc = D; g.epi = dense::EPI_RES_GATE;
@@ -1206,6 +1262,28 @@ int sopro_prefill_run_voices(sopro_prefill_t* p, const int32_t* text_ids, const 
                              float* cond_ar, void* stream) {
   return pstage::prefill_core(p, text_ids, text_len, B, Lmax, n_voices, voice_of, sv, tr, ref_k, ref_v, style_strength, n_frames, txt_seq,
                               txt_pool, cond_ar, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int sopro_prefill_run_blends(sopro_prefill_t* p, const int32_t* text_ids, const int32_t* text_len, int B, int Lmax, int n_voices,
+                             const int32_t* voice_of, const float* sv, const int32_t* tr, const float* const* ref_k,
+                             const float* const* ref_v, const int32_t* n_seg, const int32_t* seg_frames, const float* seg_w,
+                             float style_strength, int n_frames, float* txt_seq, float* txt_pool, float* cond_ar, void* stream) {
+  if (!p || !n_seg || !seg_frames || !seg_w || !tr) return fail(SOPRO_ERR_INVALID, "null argument");
+  if (n_voices < 1 || n_voices > B) return fail(SOPRO_ERR_INVALID, "n_voices=%d outside [1, B=%d]", n_voices, B);
+  size_t s = 0;
+  for (int v = 0; v < n_voices; ++v) {
+    if (n_seg[v] < 1 || n_seg[v] > SOPRO_PREFILL_MAX_BLEND_SEGMENTS)
+      return fail(SOPRO_ERR_INVALID, "n_seg[%d]=%d outside [1, %d]", v, n_seg[v], SOPRO_PREFILL_MAX_BLEND_SEGMENTS);
+    long long frames = 0;
+    for (int k = 0; k < n_seg[v]; ++k, ++s) {
+      if (seg_frames[s] < 1) return fail(SOPRO_ERR_INVALID, "voice %d, segment %d: %d frames", v, k, seg_frames[s]);
+      if (!std::isfinite(seg_w[s]) || !(seg_w[s] > 0.f)) return fail(SOPRO_ERR_INVALID, "voice %d, segment %d: weight %g", v, k, seg_w[s]);
+      frames += seg_frames[s];
+    }
+    if (frames != tr[v]) return fail(SOPRO_ERR_INVALID, "voice %d: segments of %lld frames, tr=%d", v, frames, tr[v]);
+  }
+  return pstage::prefill_core(p, text_ids, text_len, B, Lmax, n_voices, voice_of, sv, tr, ref_k, ref_v, style_strength, n_frames, txt_seq,
+                              txt_pool, cond_ar, reinterpret_cast<cudaStream_t>(stream), n_seg, seg_frames, seg_w);
 }
 
 }  // extern "C"

@@ -493,6 +493,19 @@ class SoproTTS:
         codes = self.codec.encode_wavs(wav_bl, lens)
         return [self.model.prepare_reference(c, device=self.device) for c in codes]
 
+    @torch.inference_mode()
+    def blend_voices(self, voices: Sequence[PreparedReference], weights: Optional[Sequence[float]] = None) -> PreparedReference:
+        """(extension) A new voice mixed from prepared voices -> a voices.VoiceBlend (a PreparedReference) on the device,
+        accepted wherever a voice is.  `weights`: one > 0 per voice, normalised to sum to 1 (None = equal).  The blend's
+        speaker vector is the normalised weighted mean of the voices'; in each reference cross-attention layer every
+        voice is read out on its own and the read-outs are mixed with the weights (DESIGN.md §5t).  The same object
+        passed twice counts once with its weights added, so ``blend_voices([a])`` and ``blend_voices([a, a])`` speak as
+        ``a``; a blend passed in is flattened into its voices.  Refusals (sopro_b200/voices.py::blend) raise before any
+        device work.  Whether a blend sounds between its voices on the released checkpoint has not been measured."""
+        from . import voices as V  # the `voices` argument shadows the module
+
+        return V.blend(voices, weights, device=self.device, **V.geometry(self.cfg))
+
     # ---- synthesis (model.py:531-580)
     @torch.inference_mode()
     def synthesize(self, text: str, *, ref: Optional[PreparedReference] = None, ref_audio_path: Optional[str] = None,

@@ -60,7 +60,9 @@ class PrefillEngine:
     def run(self, text_ids: Sequence[torch.Tensor], ref, *, n_frames: int, style_strength: float):
         """text_ids: B 1-D id tensors; ref: one PreparedReference for every text, or a sequence of B (a voice per text;
         rows that pass the same object share its K / V).  -> txt_seq [B, Lmax, D], lens (list), txt_pool [B, D],
-        cond_ar [B, n_frames, D] on the device.  Text b's rows equal, bit for bit, those of run(text_ids, ref[b])."""
+        cond_ar [B, n_frames, D] on the device.  Text b's rows equal, bit for bit, those of run(text_ids, ref[b]).
+        A launch with a voices.VoiceBlend among the voices runs sopro_prefill_run_blends (each blend's segment table
+        from voices.segment_table), any other sopro_prefill_run_voices."""
         B = len(text_ids)
         slots, voice_of = voices.check_voices(ref, B, **voices.geometry(self.cfg))
         lens = [int(t.numel()) for t in text_ids]
@@ -109,10 +111,17 @@ class PrefillEngine:
         txt_seq = torch.empty((B, Lmax, self.D), dtype=torch.float32, device=self.device)
         txt_pool = torch.empty((B, self.D), dtype=torch.float32, device=self.device)
         cond = torch.empty((B, int(n_frames), self.D), dtype=torch.float32, device=self.device)
-        _lib.check(self.lib.sopro_prefill_run_voices(self._h, ids.data_ptr(), ln.data_ptr(), B, Lmax, nv, vmap, sv.data_ptr(), tr,
-                                                     kp, vp, float(style_strength), int(n_frames), txt_seq.data_ptr(),
-                                                     txt_pool.data_ptr(), cond.data_ptr(),
-                                                     int(torch.cuda.current_stream(self.device).cuda_stream)))
+        outs = (float(style_strength), int(n_frames), txt_seq.data_ptr(), txt_pool.data_ptr(), cond.data_ptr(),
+                int(torch.cuda.current_stream(self.device).cuda_stream))
+        if any(isinstance(r, voices.VoiceBlend) for r in slots):
+            n_seg, frames, ws = voices.segment_table(slots if len(slots) == nv else slots * nv, trs)
+            _lib.check(self.lib.sopro_prefill_run_blends(self._h, ids.data_ptr(), ln.data_ptr(), B, Lmax, nv, vmap, sv.data_ptr(),
+                                                         tr, kp, vp, (C.c_int32 * nv)(*n_seg),
+                                                         (C.c_int32 * len(frames))(*frames), (C.c_float * len(ws))(*ws),
+                                                         *outs))
+        else:
+            _lib.check(self.lib.sopro_prefill_run_voices(self._h, ids.data_ptr(), ln.data_ptr(), B, Lmax, nv, vmap, sv.data_ptr(),
+                                                         tr, kp, vp, *outs))
         self._keep = (ids, ln, sv, ks, vs)  # alive until the stream has consumed them
         return txt_seq, lens, txt_pool, cond
 

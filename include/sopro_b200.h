@@ -642,10 +642,22 @@ int sopro_refprep_speaker_vectors_per_row(sopro_refprep_t* p, const int32_t* tok
  * reference's embedding lookup raises IndexError); clears the flag */
 int sopro_refprep_check(sopro_refprep_t* p, void* stream);
 
-/* test hook: one tensor-core implicit GEMM (no reference counterpart).  X bf16 [B][rows][cin] (device),
- * W bf16 [N][taps*cin] (device); out[b][m][n] = epi(sum_j sum_ci X[b][m + j*dil - pad][ci] * W[n][j*cin+ci] +
- * bias[n % bias_mod]); epi: 0 none, 1 GELU(erf), 2 R + scale*acc, 3 R + acc; out_f32 / out_bf16 may be null;
- * out_elu applies ELU to the bf16 copy only. */
+/* test hook: one tensor-core implicit GEMM (no reference counterpart), launched through the decoder's own launcher in
+ * its operand geometry.  X bf16 (device): item b at X + b*a_pitch*cin, ctx context rows then M rows of cin channels
+ * (a_pitch >= ctx + M; rows [ctx + M, a_pitch) are never read); W bf16 [N][taps*cin] (device).
+ *   y[b][m][n] = epi(sum_j sum_ci X_b[m + ctx + j - (taps-1)][ci] * W[n][j*cin + ci] + bias[n % bias_mod])
+ * with rows before X_b's first context row read as zero (the causal pad); epi: 0 none, 1 GELU(erf),
+ * 2 R' + scale[n]*acc, 3 R' + acc with R'[b][m][n] = R[(b*r_pitch + m)*N + n] (R may equal out_f32: in place).
+ * out_f32[(b*c_pitch + m)*N + n] = y; out_bf16 at the same offsets gets bf16(y), through ELU when out_elu; either
+ * output may be null.  Nothing outside rows [0, M) of an item is written.  bias may be null (else bias_mod in [4, N], a
+ * multiple of 4); 0 <= ctx <= taps-1, c_pitch >= M, r_pitch >= M (epi 2, 3), pointers 16-byte aligned.  A shape the
+ * kernel does not take returns SOPRO_ERR_INVALID and launches nothing. */
+int sopro_debug_tc_gemm_pitched(const void* X, int B, int M, int ctx, int64_t a_pitch, int cin, int taps, const void* W, int N,
+                                const float* bias, int bias_mod, int epi, const float* R, int64_t r_pitch, const float* scale,
+                                float* out_f32, void* out_bf16, int64_t c_pitch, int out_elu, void* stream);
+/* the same launch in the one-shot decode's packed geometry: X bf16 [B][rows][cin], R and the outputs [B][rows][N], no
+ * context rows (ctx = 0, every pitch = rows); bias_mod <= 0 means N.  Only dil = 1 and pad = taps - 1 are taken (the
+ * geometry the decoder issues); anything else returns SOPRO_ERR_INVALID. */
 int sopro_debug_tc_gemm(const void* X, int B, int64_t rows, int cin, int taps, int dil, int pad, const void* W, int N,
                         const float* bias, int bias_mod, int epi, const float* R, const float* scale, float* out_f32,
                         void* out_bf16, int out_elu, void* stream);
@@ -661,9 +673,14 @@ int sopro_debug_tc_attn(const void* q, const void* k, const void* vt, void* out,
  * ctx rows are left context, 0 <= ctx <= taps-1; the causal zero pad supplies the other taps-1-ctx rows), W1 bf16
  * [hid][taps*2*hid], W2 bf16 [2*hid][hid], bias1 [hid], bias2 [2*hid], Z fp32 [B][M][2*hid]; out_f32 / out_bf16
  * [B][M][2*hid], either may be null, out_elu applies ELU to the bf16 copy only.  hid in {32, 64, 128}, 2*hid*taps a
- * multiple of 64. */
+ * multiple of 64.  Items packed back to back. */
 int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2, const float* Z,
                             float* out_f32, void* out_bf16, int B, int M, int ctx, int hid, int taps, int out_elu, void* stream);
+/* the same launch over pitched items (a stream's buffers): item b of X, Z and the outputs starts a_pitch >= ctx + M,
+ * z_pitch >= M and o_pitch >= M rows after item b - 1; nothing outside rows [0, M) of an output item is written. */
+int sopro_debug_tc_resblock_pitched(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2,
+                                    const float* Z, float* out_f32, void* out_bf16, int B, int M, int ctx, int64_t a_pitch, int64_t z_pitch,
+                                    int64_t o_pitch, int hid, int taps, int out_elu, void* stream);
 /* attention operands from fp32 QKV rows [B][T2][3C]: rotated q -> qh, rotated k -> kh (bf16 [B][T2][C]), v -> vt (bf16
  * [B][C][T2p], T2p = T2 rounded up to 8, pad columns zero).  table: RoPE table of tab_T2 >= T2 positions,
  * [cos rows 0..tab_T2) | sin rows 0..tab_T2)] of 32 floats each; C = 64*H. */

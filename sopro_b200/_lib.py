@@ -226,8 +226,12 @@ SYMBOLS = {
     "sopro_prefill_run_blends": (_I, [_VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float, _I, _VP,
                                       _VP, _VP, _VP]),
     "sopro_debug_tc_gemm": (_I, [_VP, _I, C.c_int64, _I, _I, _I, _I, _VP, _I, _VP, _I, _I, _VP, _VP, _VP, _VP, _I, _VP]),
+    "sopro_debug_tc_gemm_pitched": (_I, [_VP, _I, _I, _I, C.c_int64, _I, _I, _VP, _I, _VP, _I, _I, _VP, C.c_int64, _VP, _VP, _VP,
+                                         C.c_int64, _I, _VP]),
     "sopro_debug_tc_attn": (_I, [_VP, _VP, _VP, _VP, _I, _I, C.c_int64, _I, _I, _I, _VP]),
     "sopro_debug_tc_resblock": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _VP]),
+    "sopro_debug_tc_resblock_pitched": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I, _I, _I, C.c_int64, C.c_int64, C.c_int64,
+                                             _I, _I, _I, _VP]),
     "sopro_debug_rope_pack": (_I, [_VP, _VP, _I, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "sopro_debug_mimi_gemm": (_I, [_VP, _VP, _VP, _VP, _VP, _VP] + [_I] * 13 + [C.c_int64] * 3 + [_VP]),
     "sopro_debug_mimi_rvq_gather": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _I, _I, _VP, _VP]),

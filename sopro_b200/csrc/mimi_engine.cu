@@ -1423,19 +1423,37 @@ int sopro_mimi_set_graphs(sopro_mimi_t* m, int enabled) {
   return SOPRO_OK;
 }
 
+int sopro_debug_tc_gemm_pitched(const void* X, int B, int M, int ctx, int64_t a_pitch, int cin, int taps, const void* W, int N,
+                                const float* bias, int bias_mod, int epi, const float* R, int64_t r_pitch, const float* scale,
+                                float* out_f32, void* out_bf16, int64_t c_pitch, int out_elu, void* stream) {
+  const bool res = epi == tc::EPI_RES || epi == tc::EPI_RES_SCALE;
+  if (!X || !W || (!out_f32 && !out_bf16) || (res && !R) || (epi == tc::EPI_RES_SCALE && !scale))
+    return fail(SOPRO_ERR_INVALID, "null argument");
+  auto misaligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) != 0; };
+  if (misaligned(X) || misaligned(W) || misaligned(bias) || misaligned(R) || misaligned(scale) || misaligned(out_f32) ||
+      misaligned(out_bf16))
+    return fail(SOPRO_ERR_INVALID, "tc gemm: every pointer must be 16-byte aligned");
+  if (B < 1 || B > 65535 || M < 1 || taps < 1 || ctx < 0 || ctx > taps - 1 || a_pitch < (int64_t)ctx + M || c_pitch < M ||
+      (res && r_pitch < M) || epi < tc::EPI_NONE || epi > tc::EPI_RES || (bias && (bias_mod < 4 || bias_mod % 4 || bias_mod > N)) ||
+      !tc::supported(N, taps * cin, cin))
+    return fail(SOPRO_ERR_INVALID, "tc gemm: unsupported shape (B=%d M=%d ctx=%d a_pitch=%lld cin=%d taps=%d N=%d c_pitch=%lld)", B, M,
+                ctx, (long long)a_pitch, cin, taps, N, (long long)c_pitch);
+  // the decoder's own launcher: pad = taps - 1 - ctx, dil = 1 and the item strides come from the same code
+  const Operand a{X, M, ctx, B, a_pitch};
+  return gemm_tc(a, cin, taps, static_cast<const __nv_bfloat16*>(W), bias, N, bias ? bias_mod : N, epi, R, scale, out_f32,
+                 static_cast<__nv_bfloat16*>(out_bf16), out_elu, reinterpret_cast<cudaStream_t>(stream), c_pitch, res ? r_pitch : 0);
+}
+
+// the packed one-shot geometry (no context rows, items back to back) of sopro_debug_tc_gemm_pitched; dil and pad stay in
+// the signature for its callers, and only what the decoder issues (dil = 1, pad = taps - 1) is taken
 int sopro_debug_tc_gemm(const void* X, int B, int64_t rows, int cin, int taps, int dil, int pad, const void* W, int N,
                         const float* bias, int bias_mod, int epi, const float* R, const float* scale, float* out_f32,
                         void* out_bf16, int out_elu, void* stream) {
-  if (!X || !W || (!out_f32 && !out_bf16)) return fail(SOPRO_ERR_INVALID, "null argument");
-  if (B < 1 || B > 65535 || rows < 1 || rows > 0x7fffffffLL || !tc::supported(N, taps * cin, cin))
-    return fail(SOPRO_ERR_INVALID, "tc gemm: unsupported shape (rows=%lld cin=%d taps=%d N=%d)", (long long)rows, cin, taps, N);
-  tc::TcOp o{};
-  o.bias = bias; o.R = R; o.scale = scale; o.out_f32 = out_f32; o.out_bf16 = reinterpret_cast<__nv_bfloat16*>(out_bf16);
-  o.c_bs = rows * N; o.M = (int)rows; o.N = N; o.K = taps * cin; o.Cin = cin; o.dil = dil; o.pad = pad;
-  o.bias_mod = bias_mod > 0 ? bias_mod : N; o.epi = epi; o.out_elu = out_elu;
-  cudaError_t e = tc::launch(X, rows, W, o, B, reinterpret_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "tensor-core GEMM launch: %s", cudaGetErrorString(e));
-  return SOPRO_OK;
+  if (rows < 1 || rows > 0x7fffffffLL || dil != 1 || pad != taps - 1)
+    return fail(SOPRO_ERR_INVALID, "tc gemm: rows=%lld dil=%d pad=%d (the decoder issues dil = 1, pad = taps - 1)", (long long)rows, dil,
+                pad);
+  return sopro_debug_tc_gemm_pitched(X, B, (int)rows, 0, rows, cin, taps, W, N, bias, bias_mod > 0 ? bias_mod : N, epi, R, rows, scale,
+                                     out_f32, out_bf16, rows, out_elu, stream);
 }
 
 int sopro_debug_tc_attn(const void* q, const void* k, const void* vt, void* out, int B, int T2, int64_t T2p, int C, int H, int window,
@@ -1450,14 +1468,19 @@ int sopro_debug_tc_attn(const void* q, const void* k, const void* vt, void* out,
   return SOPRO_OK;
 }
 
-int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2, const float* Z,
-                            float* out_f32, void* out_bf16, int B, int M, int ctx, int hid, int taps, int out_elu, void* stream) {
+int sopro_debug_tc_resblock_pitched(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2,
+                                    const float* Z, float* out_f32, void* out_bf16, int B, int M, int ctx, int64_t a_pitch, int64_t z_pitch,
+                                    int64_t o_pitch, int hid, int taps, int out_elu, void* stream) {
   if (!X || !W1 || !W2 || !bias1 || !bias2 || !Z || (!out_f32 && !out_bf16)) return fail(SOPRO_ERR_INVALID, "null argument");
   if (B < 1 || B > 65535 || M < 1 || taps < 1 || ctx < 0 || ctx > taps - 1 || (long long)M + ctx > 0x7fffffffLL ||
-      !tc::resblock_supported(hid, 2 * hid) || (2 * hid * taps) % 64 != 0)
+      a_pitch < (int64_t)M + ctx || z_pitch < M || o_pitch < M || !tc::resblock_supported(hid, 2 * hid) || (2 * hid * taps) % 64 != 0)
     return fail(SOPRO_ERR_INVALID, "fused ResnetBlock: unsupported shape (B=%d M=%d ctx=%d hid=%d taps=%d)", B, M, ctx, hid, taps);
-  // the operand geometry of seanet_tc: ctx context rows in front of the M rows, the causal zero pad covers the rest
+  // the operand geometry of seanet_tc: ctx context rows in front of the M rows, the causal zero pad covers the rest;
+  // item b of X, Z and the outputs a_pitch, z_pitch and o_pitch rows after item b - 1 (the stream's buffers)
   tc::ResOp ro{};
+  ro.a_pitch = a_pitch;
+  ro.z_bs = z_pitch * 2 * hid;
+  ro.o_bs = o_pitch * 2 * hid;
   ro.bias1 = bias1;
   ro.bias2 = bias2;
   ro.Z = Z;
@@ -1471,6 +1494,13 @@ int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const
   cudaError_t e = tc::launch_resblock(X, W1, W2, hid, ro, B, reinterpret_cast<cudaStream_t>(stream));
   if (e != cudaSuccess) return fail(SOPRO_ERR_CUDA, "fused ResnetBlock launch: %s", cudaGetErrorString(e));
   return SOPRO_OK;
+}
+
+// packed items: X [B][ctx + M][2*hid], Z and the outputs [B][M][2*hid]
+int sopro_debug_tc_resblock(const void* X, const void* W1, const void* W2, const float* bias1, const float* bias2, const float* Z,
+                            float* out_f32, void* out_bf16, int B, int M, int ctx, int hid, int taps, int out_elu, void* stream) {
+  return sopro_debug_tc_resblock_pitched(X, W1, W2, bias1, bias2, Z, out_f32, out_bf16, B, M, ctx, (int64_t)M + ctx, M, M, hid, taps,
+                                         out_elu, stream);
 }
 
 int sopro_debug_rope_pack(const float* qkv, const float* table, int tab_T2, void* qh, void* kh, void* vt, int B, int T2, int C, int H,

@@ -113,72 +113,6 @@ def test_full_size_decode_properties():
         assert torch.equal(wb[i: i + 1], eng.decode(batch[i: i + 1]))
 
 
-def _im2col(x, taps, dil, pad):
-    B, R, Cin = x.shape
-    cols = []
-    for j in range(taps):
-        sh = j * dil - pad
-        y = torch.zeros_like(x)
-        lo, hi = max(0, -sh), min(R, R - sh)
-        if hi > lo:
-            y[:, lo:hi] = x[:, lo + sh:hi + sh]
-        cols.append(y)
-    return torch.cat(cols, dim=-1)
-
-
-TC_GEMM_CASES = [
-    # B, rows, cin, taps, dil, pad, N, bias_mod, epi, out_elu
-    (2, 300, 512, 1, 1, 0, 1536, 0, 0, 0),      # QKV
-    (1, 129, 512, 7, 1, 6, 1024, 1024, 0, 1),   # conv0 -> ELU'd bf16
-    (2, 50, 1024, 2, 1, 1, 4096, 512, 0, 1),    # ConvTranspose stride 8 as a 2-tap conv
-    (1, 1000, 256, 1, 1, 0, 512, 512, 3, 1),    # res conv k=1 + skip
-    (3, 77, 64, 3, 1, 2, 32, 32, 0, 0),         # narrowest layer (N=32, K=192)
-    (1, 260, 2048, 1, 1, 0, 512, 0, 2, 0),      # fc2 + LayerScale residual
-    (2, 5, 512, 1, 1, 0, 2048, 0, 1, 0),        # fc1 + GELU, fewer rows than one tile
-    (1, 200, 128, 3, 2, 4, 640, 128, 0, 0),     # dilation 2, N = 10 x 64
-    (1, 500, 32, 1, 1, 0, 64, 64, 3, 1),        # last ResnetBlock's k=1 conv: 32 channels -> 64-byte rows, K = 32
-    (2, 100, 32, 3, 1, 2, 128, 0, 0, 0),        # 32-channel input with taps
-]
-
-
-@pytest.mark.parametrize("case", TC_GEMM_CASES, ids=lambda c: "x".join(map(str, c)))
-def test_tc_gemm_matches_torch(case):
-    """The tensor-core implicit GEMM alone against torch fp32 on the same bf16-rounded operands (differences are
-    accumulation order only): 1e-3 of the output scale for fp32 results, one bf16 ulp (2^-8 relative) for bf16."""
-    import ctypes as C
-
-    from sopro_b200 import _lib
-
-    lib = _lib.load()
-    B, R, cin, taps, dil, pad, N, bias_mod, epi, out_elu = case
-    g = torch.Generator().manual_seed(sum(case))
-    dev = torch.device("cuda:0")
-    x = (torch.randn(B, R, cin, generator=g)).to(torch.bfloat16).to(dev)
-    w = (torch.randn(N, taps * cin, generator=g) / (taps * cin) ** 0.5).to(torch.bfloat16).to(dev)
-    bias = torch.randn(bias_mod, generator=g).to(dev) if bias_mod else None
-    res = torch.randn(B, R, N, generator=g).to(dev) if epi in (2, 3) else None
-    scale = torch.rand(N, generator=g).to(dev) if epi == 2 else None
-    acc = _im2col(x.float(), taps, dil, pad) @ w.float().t()
-    if bias is not None:
-        acc = acc + bias.repeat(N // bias_mod)
-    if epi == 1:
-        acc = torch.nn.functional.gelu(acc)
-    elif epi == 2:
-        acc = res + scale * acc
-    elif epi == 3:
-        acc = res + acc
-    of = torch.full((B, R, N), float("nan"), device=dev)
-    oh = torch.full((B, R, N), float("nan"), device=dev, dtype=torch.bfloat16)
-    p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-    _lib.check(lib.sopro_debug_tc_gemm(p(x), B, R, cin, taps, dil, pad, p(w), N, p(bias), bias_mod, epi, p(res), p(scale),
-                                       p(of), p(oh), out_elu, C.c_void_p(torch.cuda.current_stream().cuda_stream)))
-    torch.cuda.synchronize()
-    s = float(acc.abs().max())
-    assert float((of - acc).abs().max()) <= 1e-3 * s
-    want_h = torch.nn.functional.elu(acc) if out_elu else acc
-    assert float((oh.float() - want_h).abs().max()) <= 2 ** -8 * s + 1e-3 * s
-
-
 @pytest.mark.parametrize("precision", ["fp32", "bf16_tc"])
 def test_host_buffer_path_and_stream_decoder(precision):
     from sopro_b200.codec import MimiCodec, MimiStreamDecoder

@@ -7,12 +7,18 @@ End to end, the tensor-core decode is compared with models whose own bf16 roundi
     and a per-element bound on random operands;
   * resblock_tc_kernel (fused ResnetBlock): bit-equal to the unfused pair of tensor-core GEMMs and to itself with
     context rows (the stream's geometry), near a float64 reference;
-  * rope_pack_kernel (RoPE + bf16 packing of the attention operands): one bf16 ulp of the float64 rotation, v exact.
+  * rope_pack_kernel (RoPE + bf16 packing of the attention operands): one bf16 ulp of the float64 rotation, v exact;
+  * igemm_tc_kernel (every other contraction of the mode, through the decoder's launcher gemm_tc) at every geometry
+    the decoder and its streams launch: bit-exact on dyadic operands, a derived per-element bound on random ones,
+    sentinels around every item, and output rows that do not depend on the launch around them (tests/mimi_tc_refs.py).
 """
 import ctypes as C
+import dataclasses
 
 import pytest
 import torch
+
+from tests import mimi_tc_refs as T
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
@@ -213,6 +219,26 @@ def _resblock(X, W1, W2, b1, b2, Z, ctx, hid, taps, out_elu, want_f32=True, want
     return of, oh
 
 
+def _resblock_pitched(X, W1, W2, b1, b2, Z, ctx, hid, taps):
+    """The stream's layout of the same launch (seanet_tc: X and Z at z's pitch, the bf16 output at o's pitch behind o's
+    context row): X, Z and both outputs each at its own item pitch, X's rows past ctx + M and Z's past M NaN (never
+    read), every output element outside rows [0, M) of an item a sentinel (never written).  Returns the packed
+    [B][M][2 hid] outputs after checking the sentinels."""
+    lib_mod, lib = _lib()
+    B, M, cout = Z.shape
+    a_pitch, z_pitch, o_pitch = ctx + M + 3, M + 2, M + 5
+    Xp = T.pitched_rows(X, a_pitch, float("nan"))
+    Zp = T.pitched_rows(Z, z_pitch, float("nan"))
+    L = T.Launch(T.Layer("resblock", cout, taps, cout, 0, T.EPI_RES, True, True, True), B, M, ctx, a_pitch, o_pitch, 0, cout)
+    of = T.f32_sentinel(B * o_pitch * cout + cout, Z.device)
+    oh = T.bf16_sentinel(cout + B * o_pitch * cout + cout, Z.device)
+    lib_mod.check(lib.sopro_debug_tc_resblock_pitched(_p(Xp), _p(W1), _p(W2), _p(b1), _p(b2), _p(Zp), _p(of), _p(oh[cout:]), B, M, ctx,
+                                                      a_pitch, z_pitch, o_pitch, hid, taps, 1, _st()))
+    torch.cuda.synchronize()
+    T.check_guards(L, of, oh, f"fused ResnetBlock hid={hid} taps={taps} B={B} M={M} pitched")
+    return T.f32_rows(L, of)[:, :M], T.bf16_rows(L, oh)[0][:, :M]
+
+
 def _gemm(X, rows, cin, taps, pad, W, N, bias, epi, R, of, oh, out_elu):
     lib_mod, lib = _lib()
     lib_mod.check(lib.sopro_debug_tc_gemm(_p(X), X.shape[0], rows, cin, taps, 1, pad, _p(W), N, _p(bias), N, epi, _p(R), None,
@@ -280,10 +306,14 @@ def test_fused_resblock(hid, taps, B, M):
     assert torch.equal(of, uf), f"fp32 out: fused vs unfused differ at {int((of != uf).sum())} elements, max {float((of - uf).abs().max()):.2e}"
     assert torch.equal(oh, uh), f"bf16 out: fused vs unfused differ at {int((oh != uh).sum())} elements"
     # the stream's geometry: ctx context rows in front, no zero pad; equals the one-shot launch over all rows
+    cf, ch = of, oh
     if ctx:
         cf, ch = _resblock(d["Xall"], d["W1"], d["W2"], d["b1"], d["b2"], d["Z"], ctx, hid, taps, 1)
         af, ah = _resblock(d["Xall"], d["W1"], d["W2"], d["b1"], d["b2"], d["Zall"], 0, hid, taps, 1)
         assert torch.equal(cf, af[:, ctx:]) and torch.equal(ch, ah[:, ctx:])
+    # the same launch over pitched items (the stream's buffers): bit-equal, nothing outside the items' rows touched
+    pf, ph = _resblock_pitched(d["Xall"] if ctx else d["X"], d["W1"], d["W2"], d["b1"], d["b2"], d["Z"], ctx, hid, taps)
+    assert torch.equal(pf, cf) and torch.equal(ph, ch), "pitched items differ from packed ones"
     ref, allow = _resblock_ref(X, W1, W2, b1, b2, Z, taps)
     s = float(ref.abs().max())
     e32 = (of.cpu().double() - ref).abs() - allow
@@ -344,8 +374,199 @@ def test_rope_pack(B, T2):
 
 
 # ---------------------------------------------------------------------------------------------------------------
+# tensor-core implicit GEMM (igemm_tc_kernel through gemm_tc)
+# ---------------------------------------------------------------------------------------------------------------
+def _tc_gemm(L, ops):
+    """one launch through sopro_debug_tc_gemm_pitched into fresh output buffers filled with the sentinels -> (fp32 buffer,
+    bf16 buffer), flat; an in-place launch's fp32 buffer starts as a copy of the residual buffer and is its R"""
+    lib_mod, lib = _lib()
+    dev = ops.X.device
+    n = L.B * L.c_pitch * L.N
+    of = ops.R.clone().view(-1) if L.inplace else (T.f32_sentinel(n, dev) if L.f32 else None)
+    oh = T.bf16_sentinel(L.h_off + n, dev) if L.bf16 else None
+    R = of if L.inplace else ops.R
+    lib_mod.check(lib.sopro_debug_tc_gemm_pitched(_p(ops.X), L.B, L.M, L.ctx, L.a_pitch, L.cin, L.taps, _p(ops.W), L.N, _p(ops.bias),
+                                                  L.bias_mod, L.epi, _p(R), L.r_pitch, _p(ops.scale), _p(of),
+                                                  _p(oh[L.h_off:] if L.bf16 else None), L.c_pitch, int(L.elu), _st()))
+    torch.cuda.synchronize()
+    return of, oh
+
+
+def _bits(t):
+    return t.view(torch.int32) if t.dtype == torch.float32 else t.view(torch.int16)
+
+
+def _rows(L, of, oh, lo=0, hi=None):
+    """rows [lo, hi) of every item of both outputs (None where the layer writes no such output)"""
+    hi = L.M if hi is None else hi
+    return (T.f32_rows(L, of)[:, lo:hi] if L.f32 else None, T.bf16_rows(L, oh)[0][:, lo:hi] if L.bf16 else None)
+
+
+def _same_rows(got, want, what):
+    for g, w, kind in zip(got, want, ("fp32", "bf16")):
+        if g is not None:
+            bad = _bits(g) != _bits(w)
+            assert not bool(bad.any()), f"{what} {kind}: {int(bad.sum())} elements differ, first {bad.nonzero()[:4].tolist()}"
+
+
+def _check(L, kind, seed):
+    """launch L on `kind` operands and hold it to the float64 reference (T.check_launch); an in-place launch must also
+    equal, bit for bit, the same launch with R in a buffer of its own.  Returns the worst ratios to the bound per output."""
+    dev = torch.device("cuda:0")
+    ops = T.operands(L, kind, seed, dev)
+    of, oh = _tc_gemm(L, ops)
+    y, a, mag = T.reference(L, ops)
+    if kind == "dyadic":  # the sums are exact; only GELU rounds
+        err = T.bound(L, y, a, mag, ops, exact_sum=True) if L.epi == T.EPI_GELU else None
+    else:
+        err = T.bound(L, y, a, mag, ops)
+    what = f"{L.name} B={L.B} M={L.M} ctx={L.ctx} pitches a/c/r {L.a_pitch}/{L.c_pitch}/{L.r_pitch} h_off={L.h_off} {kind}"
+    worst = T.check_launch(L, of, oh, y, err, what)
+    if L.inplace:
+        Ls = dataclasses.replace(L, layer=dataclasses.replace(L.layer, inplace=False), r_pitch=L.M + 2)
+        sops = dataclasses.replace(ops, R=T.pitched_rows(ops.R[:, : L.M], Ls.r_pitch, T.f32_sentinel(1, dev)))
+        sf, sh = _tc_gemm(Ls, sops)
+        _same_rows(_rows(Ls, sf, sh), _rows(L, of, oh), what + ": in place vs R apart")
+    return worst
+
+
+LAYERS = T.PRODUCTION + T.TILES
+
+
+@pytest.mark.parametrize("layer", LAYERS, ids=lambda l: l.name)
+def test_tc_gemm_exact_on_dyadic_operands(layer):
+    """Every contraction gemm_tc issues (T.PRODUCTION: the transformer's four linears, conv0, the four ConvTransposes,
+    stage 0's unfused ResnetBlock) and every tile instantiation and stage-ring edge (T.TILES), over M in {1, 127,
+    128, 129, 383, 2053}, every ctx in [0, taps-1], B in {1, 3, 64}, packed and pitched items (T.launches).  Operands
+    on the grids of T.dyadic_values, so every fp32 sum is exact: the fp32 output equals float64 bit for bit for NONE,
+    RES and RES_SCALE (the fp32 copy next to an ELU'd bf16 copy is not ELU'd), the plain bf16 output is RNE of it,
+    the ELU'd bf16 output is within half a bf16 ulp of ELU plus elu_fast's absolute floor (T.ELU_FLOOR), and GELU is
+    within its own roundings.  A dropped, doubled or misplaced product, tap or K chunk changes an output.  Operand rows
+    past ctx + M are NaN; every output element outside rows [0, M) of an item must keep its sentinel; in-place
+    residual launches equal the same launch with R apart."""
+    for i, L in enumerate(T.launches(layer)):
+        _check(L, "dyadic", 7919 * i + 1)
+
+
+@pytest.mark.parametrize("layer", LAYERS, ids=lambda l: l.name)
+def test_tc_gemm_random_operands(layer):
+    """The same sweep on random operands (unit activations, weights scaled by 1/sqrt(K), a bias, a residual, a
+    LayerScale of mixed sign), per element within T.bound: the accumulation at 2u per addition of the sum of
+    magnitudes, then each epilogue's own roundings and half a bf16 ulp for the bf16 output.  This covers GELU, the
+    LayerScale and the rounding of the bf16 output away from exact values."""
+    worst = {}
+    for i, L in enumerate(T.launches(layer)):
+        for k, v in _check(L, "random", 104729 * i + 3).items():
+            worst[k] = max(worst.get(k, 0.0), v)
+    print(f"tc gemm {layer.name}: random operands, worst |got - ref| / bound: " + ", ".join(f"{k} {v:.3e}" for k, v in worst.items()))
+
+
+@pytest.mark.parametrize("layer", T.PRODUCTION, ids=lambda l: l.name)
+def test_tc_gemm_rows_do_not_depend_on_the_launch(layer):
+    """An output row's bits do not depend on M, its row within a tile, ctx, the pitches or B:
+      * a stream's chunks (each a pitched launch with the previous chunk's last taps-1 operand rows as context; zero
+        rows before the first) equal the one-shot launch (ctx 0, packed) over all 700 rows, row for row;
+      * item b of a 64-item launch equals item b launched alone, for every b."""
+    dev = torch.device("cuda:0")
+    pad = layer.taps - 1
+    one = T.launch(layer, 2, 700, 0, pitched=False)
+    ops = T.operands(one, "random", 31, dev)
+    of, oh = _tc_gemm(one, ops)
+    xz = torch.cat([torch.zeros(2, pad, layer.cin, dtype=BF16, device=dev), ops.X], dim=1)
+    s = 0
+    for cs in (1, 127, 129, 5, 256, 182):
+        L = T.launch(layer, 2, cs, pad, pitched=True)
+        R = T.pitched_rows(ops.R[:, s: s + cs], L.r_pitch, T.f32_sentinel(1, dev)) if ops.R is not None else None
+        cops = T.Operands(T.pitched_rows(xz[:, s: s + pad + cs], L.a_pitch, float("nan")), ops.W, ops.bias, R, ops.scale)
+        cf, ch = _tc_gemm(L, cops)
+        T.check_guards(L, cf if L.f32 else None, ch, f"{layer.name} chunk at {s}")
+        _same_rows(_rows(L, cf, ch), _rows(one, of, oh, s, s + cs), f"{layer.name}: chunk rows [{s}, {s + cs}) vs one-shot")
+        s += cs
+    assert s == one.M
+    L64 = T.launch(layer, 64, 129, pad, pitched=True)
+    ops = T.operands(L64, "random", 37, dev)
+    of, oh = _tc_gemm(L64, ops)
+    L1 = dataclasses.replace(L64, B=1)
+    for b in range(64):
+        R = ops.R[b: b + 1].clone() if ops.R is not None else None
+        f1, h1 = _tc_gemm(L1, T.Operands(ops.X[b: b + 1].clone(), ops.W, ops.bias, R, ops.scale))
+        got = _rows(L64, of, oh)
+        _same_rows(_rows(L1, f1, h1), tuple(t[b: b + 1] if t is not None else None for t in got), f"{layer.name}: item {b} of 64 vs alone")
+
+
+@pytest.mark.parametrize("name,M", [("convT_r4", 4_800_000), ("conv0", 20_000)])
+def test_tc_gemm_full_size_decode_launches(name, M):
+    """The unfused launches of a 10k-frame one-shot decode at full size: the last ConvTranspose over 4.8M input rows
+    (a 4.9 GB fp32 output: byte offsets past 2^32) and conv0 over 20000 rows, dyadic operands generated on the device.
+    Sampled rows equal float64 exactly (fp32; bf16 ELU within its bound): the first and the last tile, the rows around
+    every 2^k * 128 and the last row; one guard row past M keeps its sentinel."""
+    dev = torch.device("cuda:0")
+    layer = next(l for l in T.PRODUCTION if l.name == name)
+    L = dataclasses.replace(T.launch(layer, 1, M, 0, pitched=False), c_pitch=M + 1)
+    gen = torch.Generator(device=dev).manual_seed(M)
+    X = T.signed_ints(gen, (1, M, layer.cin), 16, dev, torch.int8).to(BF16).div_(16)
+    W = (T.signed_ints(gen, (layer.N, layer.K), 16, dev).double() / 256).to(BF16)
+    bias = T.signed_ints(gen, (layer.bias_mod,), 64, dev).float() / 64
+    ops = T.Operands(X, W, bias, None, None)
+    of, oh = _tc_gemm(L, ops)
+    T.check_guards(L, of if L.f32 else None, oh, f"{name} M={M}")
+    last = (M - 1) // 128 * 128
+    windows = [(0, 128), (last, M)] + [(max(0, (128 << k) - 3), (128 << k) + 3) for k in range(20) if (128 << k) + 3 <= M]
+    for lo, hi in windows:
+        c = min(lo, layer.taps - 1)  # the operand rows the window reads, as context rows in front of it
+        Lw = T.launch(layer, 1, hi - lo, c, pitched=False)
+        y, _, _ = T.reference(Lw, T.Operands(X[:, lo - c: hi], W, bias, None, None))
+        f, b = _rows(L, of, oh, lo, hi)
+        T.check_values(Lw, f, b, y, None, f"{name} M={M} rows [{lo}, {hi})")
+    print(f"tc gemm {name} M={M}: {len(windows)} sampled row windows exact")
+    del X, of, oh, ops
+    torch.cuda.empty_cache()
+
+
+# ---------------------------------------------------------------------------------------------------------------
 # refusals: a shape the kernels do not take is an error and launches nothing
 # ---------------------------------------------------------------------------------------------------------------
+def test_tc_gemm_hook_refuses_and_launches_nothing():
+    """sopro_debug_tc_gemm_pitched refuses null pointers, B outside [1, 65535], M < 1, ctx outside [0, taps-1], pitches
+    shorter than an item, an unknown epilogue, a bias period that is no multiple of 4 or wider than N, misaligned
+    pointers and shapes tc::supported rejects, and writes nothing; the same call with valid arguments runs.  Its packed
+    form sopro_debug_tc_gemm refuses a dilation or a pad the decoder never issues."""
+    _, lib = _lib()
+    dev = torch.device("cuda:0")
+    cin, N, M = 64, 64, 8
+    X = torch.zeros(1, M + 2, cin, dtype=BF16, device=dev)
+    W = torch.zeros(N, 3 * cin, dtype=BF16, device=dev)
+    bias = torch.zeros(N, device=dev)
+    R = torch.zeros(1, M, N, device=dev)
+    scale = torch.zeros(N, device=dev)
+    of = torch.full((1, M, N), 7.0, device=dev)
+    oh = torch.full((1, M, N), 7.0, dtype=BF16, device=dev)
+    good = dict(X=_p(X), B=1, M=M, ctx=2, a_pitch=M + 2, cin=cin, taps=3, W=_p(W), N=N, bias=_p(bias), bias_mod=N, epi=T.EPI_RES,
+                R=_p(R), r_pitch=M, scale=None, of=_p(of), oh=_p(oh), c_pitch=M, elu=1)
+
+    def call(**kw):
+        a = {**good, **kw}
+        return lib.sopro_debug_tc_gemm_pitched(a["X"], a["B"], a["M"], a["ctx"], a["a_pitch"], a["cin"], a["taps"], a["W"], a["N"],
+                                               a["bias"], a["bias_mod"], a["epi"], a["R"], a["r_pitch"], a["scale"], a["of"], a["oh"],
+                                               a["c_pitch"], a["elu"], _st())
+
+    refused = [dict(X=None), dict(W=None), dict(of=None, oh=None), dict(R=None), dict(epi=T.EPI_RES_SCALE), dict(B=0),
+               dict(B=65536), dict(M=0), dict(ctx=-1), dict(ctx=3), dict(a_pitch=M + 1), dict(c_pitch=M - 1), dict(r_pitch=M - 1),
+               dict(epi=4), dict(epi=-1), dict(bias_mod=2), dict(bias_mod=2 * N), dict(taps=0, ctx=0), dict(cin=48),
+               dict(N=48, bias_mod=48), dict(of=C.c_void_p(of.data_ptr() + 4)), dict(X=C.c_void_p(X.data_ptr() + 2))]
+    for kw in refused:
+        assert call(**kw) != 0, kw
+    for dil, pad in ((2, 4), (1, 1), (1, 0)):  # packed form: rows M + 2 of X, 3 taps
+        assert lib.sopro_debug_tc_gemm(_p(X), 1, M + 2, cin, 3, dil, pad, _p(W), N, _p(bias), N, T.EPI_NONE, None, None, _p(of), _p(oh), 1,
+                                       _st()) != 0, (dil, pad)
+    torch.cuda.synchronize()
+    assert bool((of == 7.0).all()) and bool((oh.float() == 7.0).all())
+    of2, oh2 = torch.full_like(of, 7.0), torch.full_like(oh, 7.0)
+    assert call(of=_p(of2), oh=_p(oh2)) == 0
+    torch.cuda.synchronize()
+    assert bool((of2 == 0).all()) and bool((oh2.float() == 0).all())  # zero operands: R + 0, ELU(0)
+
+
 def test_hooks_refuse_unsupported_shapes():
     _, lib = _lib()
     dev = torch.device("cuda:0")
@@ -363,6 +584,9 @@ def test_hooks_refuse_unsupported_shapes():
     of = torch.full((1, M, 2 * hid), 7.0, device=dev)
     for hid_, taps, ctx in ((256, 3, 0), (48, 3, 0), (64, 3, 3), (64, 3, -1), (64, 1, 1), (64, 0, 0)):
         assert lib.sopro_debug_tc_resblock(_p(X), _p(W), _p(W), _p(b), _p(b), _p(Z), _p(of), None, 1, M, ctx, hid_, taps, 1, _st()) != 0
+    for ctx, a_pitch, z_pitch, o_pitch in ((2, M + 1, M, M), (0, M, M - 1, M), (0, M, M, M - 1)):  # an item shorter than its rows
+        assert lib.sopro_debug_tc_resblock_pitched(_p(X), _p(W), _p(W), _p(b), _p(b), _p(Z), _p(of), None, 1, M, ctx, a_pitch, z_pitch,
+                                                   o_pitch, 64, 3, 1, _st()) != 0
     qkv = torch.zeros(B, T2, 3 * Cc, device=dev)
     tab = _rope_table(T2).to(dev)
     for tab_T2, C_, H_ in ((T2 - 1, Cc, H), (T2, 500, H), (T2, 32 * H, H)):

@@ -7,7 +7,7 @@ mkdir -p sopro_b200/lib/obj
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 ARCH=(-gencode arch=compute_90a,code=sm_90a)
 FLAGS=("${ARCH[@]}" -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v --expt-relaxed-constexpr)
-UNITS=(ar_engine mimi_engine nar_engine noise_host resample stretch loudness longform flac align watermark ingest denoise)
+UNITS=(ar_engine mimi_engine nar_engine noise_host resample stretch loudness level longform flac align watermark ingest denoise)
 OBJS=()
 PIDS=()
 for u in "${UNITS[@]}"; do

@@ -867,6 +867,57 @@ int sopro_loudness_measure(const float* x, int32_t B, int64_t x_stride, const in
 int sopro_loudness_normalize(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, double T,
                              float* y, int64_t y_stride, void* ws, double* lufs_dev, float* gain_dev, void* stream);
 
+/* Live loudness: a causal leveller for audio that is still arriving.  It levels a passage, not each moment (it is not
+ * an AGC): the gain follows the integrated loudness of everything so far.  One row x at rate sr (as above) and a target
+ * T in [-60, 0] LUFS; the K-weighting (fp64, zero initial state), s, the blocks z_j and both gates are the meter's
+ * above.  Sub-block k is x[k s, (k + 1) s).
+ *   Meter: for k >= 3, M_k is the integrated loudness over blocks 0 .. k - 3, the meter's L of the prefix
+ *   x[0, (k + 1) s); -inf when no block passes the gates.
+ *   Gain: a_k = min(10^((T - M_k) / 20), 10^(B / 20)) for finite M_k, 1 when M_k = -inf.  B = 30 dB, the largest boost:
+ *   a first block that barely passes the -70 LUFS gate (a breath, room tone) is not raised by 50 dB or more before any
+ *   speech has been metered.
+ *   Release: nothing before sub-block 3 is complete (4 s samples); then sub-blocks 0 .. 3 go out at the constant gain
+ *   a_3, and each later sub-block k as soon as it is complete, under the ramp r(i) = a_{k-1} + (a_k - a_{k-1}) (i + 1) / s
+ *   in double, i the index inside the sub-block.
+ *   Ceiling: c_k = 10^(-1/20) / max|x| over sub-block k; y = fp32_rz(min(r(i), c_k)) * x, one fp32 multiply, the gain
+ *   rounded toward zero, so that max|y| <= fp32(10^(-1/20)) everywhere.
+ *   End: the finish releases what is held: a row of fewer than 4 sub-blocks at gain 1 under each sub-block's ceiling,
+ *   then the partial tail (< s samples) at the last a (1 when there is none) under the tail's own ceiling.
+ * Order: the filter's state at the end of sub-block k is s_k = A^s s_{k-1} + agg_k (A the filter's one-sample
+ * transition, agg_k the state sub-block k leaves from zero state); a sub-block's y^2 sum, the absolute gate's running
+ * sum (in increasing j) and M_k's relative-gated sum each have an order set by k alone.  So the output is a function of
+ * the row's samples only: a stream's concatenated output equals sopro_level of the concatenated input bit for bit
+ * under any push schedule, and a row of a ragged batch equals that row alone. */
+/* host-only: the workspace bytes of sopro_level for B rows of at most max_len samples at sr; < 0 for bad arguments */
+int64_t sopro_level_workspace(int32_t B, int64_t max_len, int32_t sr);
+/* one-shot, ragged batch: row b of x [B][x_stride] f32 (device) has lens_host[b] samples (HOST i64; NULL = x_stride
+ * each); samples at or past lens[b] are not read.  y + b * y_stride (device; y_stride >= the longest row when B > 1)
+ * receives the levelled row over [0, lens[b]); the rest of the row is not written.  meter_dev and gain_dev (nullable,
+ * device f64 [B][floor(max lens / s)]) receive M_k and a_k of every complete sub-block (NaN for k < 3): a test hook.
+ * A refused T or rate is SOPRO_ERR_INVALID before any launch.  No call synchronises or allocates. */
+int sopro_level(const float* x, int32_t B, int64_t x_stride, const int64_t* lens_host, int32_t sr, double T, float* y,
+                int64_t y_stride, void* ws, double* meter_dev, double* gain_dev, void* stream);
+/* Streaming: one utterance pushed in chunks of at most max_chunk samples.  After N input samples the pushes have
+ * released floor(N / s) s samples once floor(N / s) >= 4 and none before, and finish releases the rest up to N.  One launch per push that completes a sub-block.  The state on the device: the filter
+ * state, fewer than 4 s + 2 held input samples, the absolute gate's sum and count, a_{k-1}, and every sub-block's y^2
+ * sum (8 bytes per 100 ms) in a store that starts at ten minutes and doubles in stream order.  Create allocates and
+ * synchronises; output counts are host arithmetic and no other call synchronises.  Calls on one state are ordered on
+ * one CUDA stream. */
+typedef struct sopro_level_stream sopro_level_stream_t;
+int sopro_level_stream_create(int64_t max_chunk, int32_t sr, int device, sopro_level_stream_t** out);
+int sopro_level_stream_destroy(sopro_level_stream_t* s);
+/* back to sample 0 with target T (host-only; also clears the finished state).  A new state takes no push until its
+ * first reset; SOPRO_ERR_INVALID for a refused T. */
+int sopro_level_stream_reset(sopro_level_stream_t* s, double T);
+/* outputs the next call writes: a push of n_more samples (final == 0), or a push of n_more samples followed by finish
+ * (final != 0); < 0 on bad arguments, before the first reset or after finish */
+int64_t sopro_level_stream_ready(const sopro_level_stream_t* s, int64_t n_more, int final);
+/* x [n] f32 (device) -> y (device) receives stream_ready(s, n, 0) outputs.  n > max_chunk: SOPRO_ERR_INVALID, nothing
+ * launched, state unchanged.  After finish: SOPRO_ERR_STATE until a reset. */
+int sopro_level_push(sopro_level_stream_t* s, const float* x, int64_t n, float* y, void* stream);
+/* the remaining stream_ready(s, 0, 1) outputs -> y (device); SOPRO_ERR_STATE when called twice without a reset */
+int sopro_level_finish(sopro_level_stream_t* s, float* y, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Long-form synthesis (no reference counterpart: the reference speaks one utterance of at most max_frames): the speech
  * extent of each segment's decoded 24 kHz row, and the join of those extents into one waveform.

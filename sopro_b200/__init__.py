@@ -7,7 +7,7 @@ from .config import SoproTTSConfig  # noqa: F401
 
 __version__ = "0.1.0"
 __all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac", "WordTiming",
-           "detect_watermark", "denoise"]
+           "detect_watermark", "denoise", "level_live", "LiveLeveller", "level_stream", "level_stream_batch"]
 
 
 def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
@@ -15,6 +15,10 @@ def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
         from . import flac
 
         return getattr(flac, name)
+    if name in ("level_live", "LiveLeveller", "level_stream", "level_stream_batch"):
+        from . import loudness
+
+        return getattr(loudness, name)
     if name == "detect_watermark":
         from .watermark import detect_watermark
 

@@ -269,6 +269,14 @@ SYMBOLS = {
     "sopro_loudness_measure": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, _VP, _VP, _VP]),
     "sopro_loudness_normalize": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, C.c_double, _VP, C.c_int64, _VP, _VP,
                                       _VP, _VP]),
+    "sopro_level_workspace": (C.c_int64, [C.c_int32, C.c_int64, C.c_int32]),
+    "sopro_level": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, C.c_double, _VP, C.c_int64, _VP, _VP, _VP, _VP]),
+    "sopro_level_stream_create": (_I, [C.c_int64, C.c_int32, _I, C.POINTER(_VP)]),
+    "sopro_level_stream_destroy": (_I, [_VP]),
+    "sopro_level_stream_reset": (_I, [_VP, C.c_double]),
+    "sopro_level_stream_ready": (C.c_int64, [_VP, C.c_int64, _I]),
+    "sopro_level_push": (_I, [_VP, _VP, C.c_int64, _VP, _VP]),
+    "sopro_level_finish": (_I, [_VP, _VP, _VP]),
     "sopro_longform_fade": (_I, [C.c_int32, _VP]),
     "sopro_longform_extents": (_I, [_VP, C.c_int32, C.c_int64, _VP, _VP, _VP]),
     "sopro_longform_join": (_I, [_VP, C.c_int32, _VP, _VP, C.c_int64, _VP, C.c_int64, _VP]),

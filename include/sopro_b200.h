@@ -989,6 +989,18 @@ int sopro_longform_stream_status(const sopro_longform_stream_t* s, int32_t row0,
  * Pieces outside the samples pushed are SOPRO_ERR_INVALID before any launch.  One launch per 48 pieces. */
 int sopro_longform_stream_emit(const sopro_longform_stream_t* s, const int64_t* pieces_host, int32_t n_pieces, float* y,
                                int64_t y_len, void* stream);
+/* Timeline mix (timed synthesis): n_items rows placed at absolute sample offsets and summed where they overlap.
+ * src: HOST array of n_items device pointers, item i's row of lens_host[i] samples (HOST i64), read in place and placed
+ * at offs_host[i] (HOST i64).  With i1 < i2 < ... the items covering sample t, in item order, y[t] (device f32 [y_len])
+ * is src[i1][t - offs[i1]], then each later covering item's sample added with one round-to-nearest fp32 add, in item
+ * order; 0 where no item covers t.  Every sample of y is written (the caller does not zero it); a sample covered by a
+ * single item equals that item's sample bit for bit; the result depends only on the items, not on the tiling.
+ * One launch for any item count: each 4096-sample tile's covering items reach the device through one stream-ordered
+ * copy.  Refused before any launch: n_items < 0, a null src / lens_host / offs_host with items, a null source for a
+ * non-empty item, a negative length or offset, offs + lens > y_len, y_len outside [0, 2^40], a null y with
+ * y_len > 0. */
+int sopro_timeline_mix(const float* const* src, int32_t n_items, const int64_t* lens_host, const int64_t* offs_host, float* y,
+                       int64_t y_len, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Lossless FLAC output (RFC 9639; no reference counterpart: the reference's demo sends PCM16): mono, 16 bits per sample,

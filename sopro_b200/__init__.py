@@ -7,7 +7,7 @@ from .config import SoproTTSConfig  # noqa: F401
 
 __version__ = "0.1.0"
 __all__ = ["SoproTTS", "SoproTTSConfig", "encode_flac", "FlacStreamEncoder", "encode_stream_flac", "WordTiming",
-           "detect_watermark", "denoise", "level_live", "LiveLeveller", "level_stream", "level_stream_batch"]
+           "detect_watermark", "denoise", "level_live", "LiveLeveller", "level_stream", "level_stream_batch", "Cue", "CueFit", "parse_cues"]
 
 
 def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
@@ -19,6 +19,14 @@ def __getattr__(name):  # lazy: keep `import sopro_b200` cheap and GPU-free
         from . import loudness
 
         return getattr(loudness, name)
+    if name in ("Cue", "CueFit"):
+        from . import cues
+
+        return getattr(cues, name)
+    if name == "parse_cues":
+        from .cues import parse
+
+        return parse
     if name == "detect_watermark":
         from .watermark import detect_watermark
 

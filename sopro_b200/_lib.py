@@ -287,6 +287,7 @@ SYMBOLS = {
     "sopro_longform_stream_push": (_I, [_VP, _VP, C.c_int64, C.c_int32, C.c_int32, _VP, _VP, _VP]),
     "sopro_longform_stream_status": (_I, [_VP, C.c_int32, C.c_int32, _VP, _VP]),
     "sopro_longform_stream_emit": (_I, [_VP, _VP, C.c_int32, _VP, C.c_int64, _VP]),
+    "sopro_timeline_mix": (_I, [_VP, C.c_int32, _VP, _VP, _VP, C.c_int64, _VP]),
     "sopro_flac_sizes": (_I, [C.c_int32, C.c_int64, C.c_int32, _VP, _VP]),
     "sopro_flac_encode": (_I, [_VP, C.c_int32, C.c_int64, _VP, C.c_int32, _VP, _VP, _VP, _VP, _VP]),
     "sopro_flac_stream_create": (_I, [C.c_int32, C.POINTER(_VP)]),

@@ -16,6 +16,7 @@
 // start, and the last from the end, stopping at the first round that finds one.
 // join_kernel: grid (pieces, segments); the segments of one launch share their F, and their fade table travels in the
 // kernel parameters with the source pointers, so nothing is copied to the device first.
+// The timeline mix (timed synthesis) is the last part of the file.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -274,6 +275,52 @@ __global__ void __launch_bounds__(kJoinThreads) emit_kernel(const EmitArgs a, co
         v = __fmul_rn(v, __ldg(f + (p.tail + p.F - 1 - j)));
     }
     yo[i] = v;
+  }
+}
+
+// ---- the timeline mix (include/sopro_b200.h, sopro_timeline_mix): items placed at absolute offsets and summed where
+// they overlap, y[t] = the first covering item's sample, then each later one added in item order.
+// mix_kernel: one CTA per output tile of kMixTile samples, over a grid-stride range of tiles.  The host lists each
+// tile's covering items in item order (a CSR); thread i owns samples i, i + 256, ... of the tile and keeps their sums in
+// registers while it walks the list, so every sample's adds happen in item order whatever the tiling.
+constexpr int kMixThreads = 256;
+constexpr int kMixPer = 16;                         // samples per thread
+constexpr int kMixTile = kMixThreads * kMixPer;     // 4096
+constexpr int kMixMaxCtas = 4096;
+
+struct MixItem {
+  const float* src;
+  long long off, len;
+};
+
+__global__ void __launch_bounds__(kMixThreads) mix_kernel(const MixItem* __restrict__ items, const long long* __restrict__ ptr,
+                                                          const int* __restrict__ idx, long long n_tiles, float* __restrict__ y,
+                                                          long long y_len) {
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const long long base = tile * kMixTile + threadIdx.x;
+    float acc[kMixPer];
+    unsigned have = 0;  // bit k: sample k has its first item
+#pragma unroll
+    for (int k = 0; k < kMixPer; ++k) acc[k] = 0.0f;
+    const long long e = __ldg(ptr + tile + 1);
+    for (long long j = __ldg(ptr + tile); j < e; ++j) {
+      const MixItem it = items[__ldg(idx + j)];
+      const long long lo = it.off, hi = it.off + it.len;
+#pragma unroll
+      for (int k = 0; k < kMixPer; ++k) {
+        const long long t = base + (long long)k * kMixThreads;
+        if (t >= lo && t < hi) {
+          const float v = __ldg(it.src + (t - lo));
+          acc[k] = (have >> k & 1u) ? __fadd_rn(acc[k], v) : v;
+          have |= 1u << k;
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < kMixPer; ++k) {
+      const long long t = base + (long long)k * kMixThreads;
+      if (t < y_len) y[t] = acc[k];
+    }
   }
 }
 
@@ -573,6 +620,57 @@ int sopro_longform_stream_emit(const sopro_longform_stream_t* s, const int64_t* 
     emit_kernel<<<dim3(gx, args.n), kJoinThreads, 0, st>>>(args, s->fades, y);
     CK(cudaGetLastError());
   }
+  return SOPRO_OK;
+}
+
+int sopro_timeline_mix(const float* const* src, int32_t n_items, const int64_t* lens_host, const int64_t* offs_host, float* y,
+                       int64_t y_len, void* stream) {
+  if (n_items < 0) return fail(SOPRO_ERR_INVALID, "n_items = %d < 0", n_items);
+  if (y_len < 0 || y_len > kMaxLen) return fail(SOPRO_ERR_INVALID, "y_len = %lld not in [0, 2^40]", (long long)y_len);
+  if (n_items > 0 && (!src || !lens_host || !offs_host)) return fail(SOPRO_ERR_INVALID, "null argument");
+  const long long n_tiles = (y_len + kMixTile - 1) / kMixTile;
+  std::vector<long long> ptr(n_tiles + 1, 0);
+  for (int i = 0; i < n_items; ++i) {
+    const long long len = lens_host[i], off = offs_host[i];
+    if (len < 0 || off < 0) return fail(SOPRO_ERR_INVALID, "item %d: length %lld, offset %lld (both must be >= 0)", i, len, off);
+    if (off > y_len - len)
+      return fail(SOPRO_ERR_INVALID, "item %d: [%lld, %lld + %lld) is not inside y_len = %lld", i, off, off, len, (long long)y_len);
+    if (len == 0) continue;
+    if (!src[i]) return fail(SOPRO_ERR_INVALID, "null source for item %d", i);
+    for (long long t = off / kMixTile; t <= (off + len - 1) / kMixTile; ++t) ++ptr[t + 1];
+  }
+  if (y_len == 0) return SOPRO_OK;
+  if (!y) return fail(SOPRO_ERR_INVALID, "null argument");
+  for (long long t = 0; t < n_tiles; ++t) ptr[t + 1] += ptr[t];
+  // each tile's items in item order, then one stream-ordered upload of the items, the CSR and its lists
+  std::vector<int> idx(ptr[n_tiles]);
+  std::vector<long long> fill(ptr.begin(), ptr.end() - 1);
+  std::vector<MixItem> items(n_items);
+  for (int i = 0; i < n_items; ++i) {
+    const long long len = lens_host[i], off = offs_host[i];
+    items[i] = MixItem{src[i], off, len};
+    if (len == 0) continue;
+    for (long long t = off / kMixTile; t <= (off + len - 1) / kMixTile; ++t) idx[fill[t]++] = i;
+  }
+  const size_t b_items = sizeof(MixItem) * items.size(), b_ptr = sizeof(long long) * ptr.size();
+  const size_t b_idx = sizeof(int) * idx.size(), total = b_items + b_ptr + b_idx;
+  std::vector<unsigned char> blob(total);
+  std::memcpy(blob.data(), items.data(), b_items);
+  std::memcpy(blob.data() + b_items, ptr.data(), b_ptr);
+  std::memcpy(blob.data() + b_items + b_ptr, idx.data(), b_idx);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  unsigned char* d = nullptr;
+  CK(cudaMallocAsync(reinterpret_cast<void**>(&d), total, st));
+  cudaError_t e = cudaMemcpyAsync(d, blob.data(), total, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) {
+    const unsigned grid = (unsigned)std::min<long long>(n_tiles, kMixMaxCtas);
+    mix_kernel<<<grid, kMixThreads, 0, st>>>(reinterpret_cast<const MixItem*>(d), reinterpret_cast<const long long*>(d + b_items),
+                                             reinterpret_cast<const int*>(d + b_items + b_ptr), n_tiles, y, y_len);
+    e = cudaGetLastError();
+  }
+  const cudaError_t f = cudaFreeAsync(d, st);
+  CK(e);
+  CK(f);
   return SOPRO_OK;
 }
 

@@ -287,6 +287,38 @@ def join_padded(rows: Sequence[torch.Tensor], extents, pauses: Sequence[int], ga
     return parts[0] if len(parts) == 1 else torch.cat(parts, dim=-1)
 
 
+def mix(rows: Sequence[torch.Tensor], offsets: Sequence[int], length: int, device=None) -> torch.Tensor:
+    """Rows placed at absolute sample offsets on one timeline and summed where they overlap -> [1, 1, length] f32 on
+    the rows' device (SoproTTS.synthesize_timed's placement).  Sample t is the first covering row's sample, then each
+    later covering row's added in one fp32 add, in row order; 0 where no row covers t.  `rows`: 1-D tensors (others
+    are flattened) on one CUDA device, read in place; an empty row covers nothing.  Every row must end by `length`
+    (include/sopro_b200.h, sopro_timeline_mix); `device`: the output's device when there is no row (default: the
+    current CUDA device).  Nothing synchronises."""
+    flat = []
+    for r in rows:
+        if r.device.type != "cuda":
+            raise _lib.SoproError("the mix needs CUDA tensors; there is no CPU path")
+        flat.append(r.detach().to(dtype=torch.float32).reshape(-1).contiguous())
+    n = len(flat)
+    offs = [int(o) for o in offsets]
+    if len(offs) != n:
+        raise ValueError(f"{len(offs)} offsets for {n} rows")
+    dev = flat[0].device if flat else torch.device(device if device is not None else "cuda")
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    if any(r.device != dev for r in flat):
+        raise ValueError("the rows are on different devices")
+    L = int(length)
+    y = torch.empty((1, 1, max(L, 0)), dtype=torch.float32, device=dev)
+    src = (C.c_void_p * max(n, 1))(*[r.data_ptr() if r.numel() else None for r in flat])
+    lens = (C.c_int64 * max(n, 1))(*[int(r.numel()) for r in flat])
+    offp = (C.c_int64 * max(n, 1))(*offs)
+    with torch.cuda.device(dev):
+        _lib.check_arg(_lib.load().sopro_timeline_mix(src, n, lens, offp, y.data_ptr() if L > 0 else None, L,
+                                                      _lib.stream_ptr(dev)))
+    return y
+
+
 # ---- the streaming trim and join (SoproTTS.stream_long)
 
 class StreamJoin:

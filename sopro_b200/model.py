@@ -20,6 +20,7 @@ from typing import Dict, Iterator, List, Mapping, Optional, Sequence, Tuple, Uni
 
 import torch
 
+from . import cues as CU
 from . import dialogue as D
 from . import ingest
 from . import longform as LF
@@ -741,6 +742,93 @@ class SoproTTS:
             wav, _ = post(wav)
         return wav
 
+    @torch.inference_mode()
+    def synthesize_timed(self, cues: Union[str, Sequence[CU.Cue]], *, ref: PreparedReference,
+                         voices: Optional[Mapping[str, PreparedReference]] = None, seed: Optional[int] = None,
+                         max_rate: float = 1.5, pause_ms: float = 250, max_frames: int = 400, max_tokens: int = 64,
+                         top_p: float = 0.9, temperature: float = 1.05, anti_loop: bool = True,
+                         style_strength: Optional[float] = None, min_gen_frames: Optional[int] = None,
+                         sample_rate: Optional[int] = None, loudness: Optional[float] = None,
+                         watermark: Optional[int] = None, best_of: int = 1) -> Tuple[torch.Tensor, List[CU.CueFit]]:
+        """NEW: subtitle cues spoken at their times -> (one waveform [1, 1, N] f32 on the device, one CueFit per cue in
+        input order).  `cues`: an SRT or WebVTT file's text (sopro_b200/cues.py::parse) or a sequence of Cue; a cue
+        without a voice speaks in `ref`, a named one in voices[name].  Each cue's text is cut as synthesize_long cuts a
+        text, and segment k of the track (cue order, then segment order) equals synthesize(segment, ref=its cue's
+        voice, seed=seed + k) (without a seed the global generator is consumed segment after segment).  The cues are
+        processed in groups whose segments fill at most one SEGMENT_GROUP pass (a cue with more segments is a group of
+        its own): the group is generated and decoded, each cue's segments are trimmed and joined with `pause_ms` as by
+        synthesize_long, and the cue rows are time-stretched in one launch; only the stretched rows outlive the group.
+        Fit rule, with n the cue's joined 24 kHz length and slot = round(end * 24000) - round(start * 24000): a cue that
+        fits is not stretched; a longer one is sped up by the least fixed-point speed S = ceil(n * 65536 / slot) that
+        fits, at most round(max_rate * 65536) (`max_rate` in [1, 4]); speech is never slowed down, so a capped cue runs
+        past its end.  Each stretched cue is placed at round(start * 24000) and the cues are summed, in ascending
+        (start sample, input index) order, by one CUDA mix (longform.mix: overlaps add, unclipped; silence elsewhere).
+        The timeline lasts to the later of the last cue's end and the end of its speech, then goes through the chain
+        of synthesize_ssml: watermark, resample (`sample_rate`), loudness (whose -1 dBFS ceiling applies as everywhere).
+        So a cue equals stretch_rows of synthesize_long(its text, ref=its voice, seed=seed + its first segment) at its
+        S.  `best_of`: as in synthesize_long.  Refused before any device work or random draw: every refusal of
+        cues.parse, a sequence element that is not a Cue (TypeError), a cue whose start and end round to one sample,
+        an unknown voice name, a voice of the wrong geometry, `max_rate` / `pause_ms` / `max_tokens` out of range, a
+        refused sample_rate / loudness / watermark / best_of, and a track with nothing to speak."""
+        post = OutputChain(self, sample_rate, None, loudness, watermark)
+        n_best = self._check_best_of(best_of, 1)
+        P = LF.pause_samples(pause_ms)
+        budget = LF.check_max_tokens(max_tokens, self.model.prefill.max_text_len)
+        S_max = CU.check_max_rate(max_rate)
+        track = CU.track(cues)
+        voice_of = CU.cue_voices(track, voices, ref)
+        _check_voices(self.cfg, voice_of)
+        segs = [LF.split_text(c.text, self.tokenizer, budget) for c in track]
+        if not any(segs):
+            raise ValueError("the track has nothing to speak (every cue is empty)")
+        gen = Generation.resolve(self.cfg, max_frames=max_frames, top_p=top_p, temperature=temperature,
+                                 anti_loop=anti_loop, style_strength=style_strength, min_gen_frames=min_gen_frames)
+        K = len(track)
+        offs = [CU.to_samples(c.start) for c in track]
+        ends = [CU.to_samples(c.end) for c in track]
+        S, M = [CU.ONE] * K, [0] * K
+        spoken: List[Optional[torch.Tensor]] = [None] * K
+        k0 = 0  # the track's index of the group's first segment
+        for a, b in CU.groups([len(s) for s in segs], self._segment_group(n_best)):
+            part = [s for c in range(a, b) for s in segs[c]]
+            if not part:
+                continue
+            rows, ext_dev, _f, _T = self._speak_segments(
+                part, D.segment_voices([voice_of[c] for c in range(a, b) for _ in segs[c]]), n_best,
+                seed=None if seed is None else int(seed) + k0, word_timestamps=False, gen=gen)
+            ext = ext_dev.cpu().numpy()  # the group's one host read: the extents
+            joined: List[Optional[torch.Tensor]] = []
+            j = 0
+            for c in range(a, b):
+                e = ext[j: j + len(segs[c])]
+                live = bool(len(e)) and bool((e[:, 1] > e[:, 0]).any())
+                joined.append(LF.join_gaps(rows[j: j + len(segs[c])], e, LF.gap_pauses(e, P)).reshape(-1)
+                              if live else None)
+                j += len(segs[c])
+            n = [0 if w is None else int(w.numel()) for w in joined]
+            for i, c in enumerate(range(a, b)):
+                S[c] = CU.fit_speed(n[i], ends[c] - offs[c], S_max)
+                M[c] = stretched_length(S[c] / CU.ONE, n[i])
+            if max(n):
+                batch = torch.zeros((b - a, max(n)), dtype=torch.float32, device=self.device)
+                for i, w in enumerate(joined):
+                    if w is not None:
+                        batch[i, : n[i]] = w
+                y = stretch_rows(batch, [S[c] / CU.ONE for c in range(a, b)], lens=n)
+                for i, c in enumerate(range(a, b)):
+                    if M[c]:
+                        spoken[c] = y[i, : M[c]].clone()
+                del batch, y
+            del rows, ext_dev, joined  # the group's decodes go before the next group's
+            k0 += len(part)
+        order = [c for c in sorted(range(K), key=lambda c: (offs[c], c)) if M[c]]
+        N = max(max(e, o + m) for e, o, m in zip(ends, offs, M))
+        wav = LF.mix([spoken[c] for c in order], [offs[c] for c in order], N, self.device)
+        wav, _ = post(wav)
+        fits = [CU.CueFit(index=c, rate=S[c] / CU.ONE, spoken=M[c] / CU.SAMPLE_RATE,
+                          overrun=max(0, offs[c] + M[c] - ends[c]) / CU.SAMPLE_RATE) for c in range(K)]
+        return wav, fits
+
     def _speak_segments(self, segments: Sequence[str], ref, n_best: int, *, seed: Optional[int], word_timestamps: bool,
                         **kw) -> Tuple[List[torch.Tensor], torch.Tensor, list, List[int]]:
         """The segments of a long-form passage or a dialogue, generated through the batch path SEGMENT_GROUP at a time
@@ -748,11 +836,7 @@ class SoproTTS:
         decoded -> (each segment's 24 kHz row, read in place by the join; their extents, int64 [K, 2] on the device;
         with word_timestamps each segment's first frames and frame count, else empty lists).  Nothing synchronises.
         `kw`: _best_codes's `gen`."""
-        B, group = len(segments), int(LF.SEGMENT_GROUP)
-        if n_best > 1:
-            limit = self._batch_limit()
-            if limit is not None:
-                group = max(1, min(group, limit // n_best))
+        B, group = len(segments), self._segment_group(n_best)
         one = isinstance(ref, PreparedReference)
         ext = torch.zeros((B, 2), dtype=torch.int64, device=self.device)
         rows: List[torch.Tensor] = [torch.zeros(0, device=self.device)] * B
@@ -774,6 +858,16 @@ class SoproTTS:
                 for j, i in enumerate(chunk):
                     rows[g0 + i] = flat[j, : lens[j]]  # read in place by the join
         return rows, ext, firsts, all_Ts
+
+    def _segment_group(self, n_best: int) -> int:
+        """Segments per batch pass of the passage paths: SEGMENT_GROUP, fewer when their best_of takes would exceed
+        the batch limit."""
+        group = int(LF.SEGMENT_GROUP)
+        if n_best > 1:
+            limit = self._batch_limit()
+            if limit is not None:
+                group = max(1, min(group, limit // n_best))
+        return group
 
     def _timings(self, texts: Sequence[str], spans, probs: torch.Tensor, lens: Sequence[int], Ts: Sequence[int],
                  S: Optional[int]) -> List[List[TS.WordTiming]]:
